@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — scans/sec of the scan-to-submap registration hot path (BASELINE.json metric) on N B200s.
+"""bench.py — scans/sec of the scan-to-submap registration hot path (BASELINE.json metric) on N H100s.
 
 A "step" is one pass of the whole per-scan hot path of BASELINE configs[1] (64-beam ~130k pts/scan + 200 Hz IMU, single
-submap, 1 x B200) over one batch of DISTINCT synthetic scans:
+submap, 1 x H100) over one batch of DISTINCT synthetic scans:
     IMU pre-integration of the 20 samples since the previous scan -> state prediction -> first voxel filter ->
     deskew/transform/range gate -> second voxel filters -> adaptive voxel filters -> Levenberg-Marquardt point-to-grid
     match with the pre-integration residual fused into the same solve,
@@ -20,7 +20,10 @@ rank, so the per-GPU work is the same at every N: weak scaling).
   configs2 / mode_F   extra keys: configs[2] (128-beam, 0.05 m grid, correlative + refine) and the full-cloud matcher mode.
 
 `--impl reference` times the CPU chain alone (all host threads) and prints the same line with "impl": "reference".
-Inputs per step exceed L2 (148 scans x 2.1 MB = 309 MB > 126 MB), so no explicit L2 flush.
+Inputs per step exceed L2 (148 scans x 2.1 MB = 309 MB > the H100's 50 MB), so no explicit L2 flush.
+
+`--dump-outputs DIR` writes what the last timed step returned to its caller (per-scan results and states, the last exchange's
+constraint table) as DIR/<name>.npy; the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -49,6 +52,7 @@ METRIC = "scans/sec (64-beam, 10 Hz) per GPU; pose RMSE vs reference CPU"
 UNIT = "scans/s"
 IMU_NOISE = [3.99e-2, 1.56e-2, 6.4e-5, 3.6e-5]     # D/config/kaist.lua:38-43
 IMU_WEIGHT = 1.0
+HBM_PEAK_GBS = 3350.0   # H100 SXM data sheet (HBM3); used when MEASURED_PEAKS.json gives no measured peak
 
 
 def oracle():
@@ -86,10 +90,9 @@ def physical_cores():
 
 
 def usable_cpus():
-    """(threads to use, description): os.cpu_count() capped by the affinity mask and by the container's CFS quota. The pool's GPU
-    boxes show 128 logical CPUs but run under `cpu.max = 1600000 100000` (16 CPUs' worth of time): 128 busy threads are then
-    throttled to ~700 scans/s, 16 threads run at their full 1 100 scans/s (tools/cpu_scaling.py, profiles/r3_cpu_scaling.json) —
-    the reference arm must use what the box really grants to be the best the host can do."""
+    """(threads to use, description): os.cpu_count() capped by the affinity mask and by the container's CFS quota. A container
+    may show many more logical CPUs than its `cpu.max` quota grants; threads beyond the quota are throttled and make the pool
+    slower (tools/cpu_scaling.py measures this) — the reference arm must use what the host really grants to be the best it can do."""
     n = os.cpu_count() or 1
     note = f"os.cpu_count() = {n}"
     try:
@@ -263,7 +266,7 @@ def workload_config(args, batch):
             "imu": True, "scans_per_step_per_gpu": batch, "distinct_scans": batch, "beams": args.beams,
             "map_scans": args.map_scans, "row_bytes": 4 * args.row_floats,
             "row_layout": {3: "x y z (12 B) + per-point times as runs", 4: "x y z t (16 B)", 8: "RangeMeasurement (32 B)"}[args.row_floats],
-            "l2_policy": f"inputs ({batch} x {130605 * 4 * args.row_floats / 1e6:.1f} MB) exceed the 126 MB L2; no explicit flush",
+            "l2_policy": f"inputs ({batch} x {130605 * 4 * args.row_floats / 1e6:.1f} MB) exceed the 50 MB L2 of an H100; no explicit flush",
             "parallelism": f"scans sharded over {args.gpus} gpu(s); loop-closure pairs sharded by submap owner, one ncclAllGather per step",
             "exchange_thread": f"each step's exchange (searches + all-gather + table on the host) is issued from one of "
                                f"{args.exchange_threads} background host threads (own context + NCCL communicator each, step k -> "
@@ -285,7 +288,8 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--batch", type=int, default=148, help="scans per step per GPU (default: one per SM)")
+    ap.add_argument("--batch", type=int, default=148,
+                    help="scans per step per GPU (148 measured on an H100 at least as fast per scan as one per SM, 132)")
     ap.add_argument("--beams", type=int, default=64)
     ap.add_argument("--map-scans", type=int, default=40)
     ap.add_argument("--pairs", type=int, default=8, help="loop-closure (node, submap) searches per rank and step")
@@ -297,6 +301,8 @@ def main():
                     help="3: x y z rows + the per-point times as runs (12 B/point); 4: TimedPointCloud rows x y z t (what AddRangeData "
                          "receives); 8: RangeMeasurement rows")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2] / mode-F / no-IMU extra measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (results, states, constraint table) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -387,6 +393,7 @@ def main():
             self.pending = 0
             self.error = None
             self.stop = False
+            self.last_table = None   # the constraint table of this worker's latest exchange
             self.start()
 
         def run(self):
@@ -398,6 +405,7 @@ def main():
                         return
                 try:
                     table, info = self.plan()
+                    self.last_table = table
                     with exchange_lock:
                         exchange["ms"].append(info.collective_ms)
                         exchange["found"] = info.found_total
@@ -522,6 +530,11 @@ def main():
     launches = sum(c.launches for c in [ctx, ctx2] + xctxs) - launches0
     profile = ctx.read_profile()
     ctx.set_profiling(False)
+    if args.dump_outputs:
+        last_lane = dev_lanes[(args.steps - 1) % 2]     # the lane the last timed step wrote; later loops overwrite it
+        last_table = workers[(submitted[0] - 1) % len(workers)].last_table if workers else None
+        dump_outputs(args.dump_outputs, last_lane[0].fetch_results(C.c_void_p(last_lane[1].data_ptr()), B),
+                     last_lane[2].cpu().numpy(), last_table)
     collective_ms = float(np.median(exchange["ms"])) if exchange["ms"] else None
     note("device-resident loop done")
     # ---- timed: end to end (host buffers in, results out), streaming and blocking
@@ -530,7 +543,7 @@ def main():
     res_stream, states_stream = run_streaming(args.steps)
     barrier()
     e2e_s = time.perf_counter() - t0
-    sync_steps = max(3, min(args.steps, 20))
+    sync_steps = args.steps
     barrier()
     t0 = time.perf_counter()
     for _ in range(sync_steps):
@@ -629,23 +642,18 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_kind = "of measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "of fallback (6.65 TB/s)"
+        peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
+        peak_kind = "of measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "of the H100 SXM data sheet (3.35 TB/s)"
         achieved = (stages[dom]["bytes_per_step"] or 0.0) / (stages[dom]["ms_per_step"] * 1e-3) / 1e9
         achieved_over = (stages[dom]["bytes_per_step"] or 0.0) / (max(stages[dom]["ms_per_step_overlapped"], 1e-9) * 1e-3) / 1e9
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(dom)
-        except Exception:
-            pass
         roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                    "frac": achieved / peak, "traffic": traffic, "peak_kind": peak_kind,
+                    "frac": achieved / peak, "peak_kind": peak_kind,
                     "achieved_overlapped": achieved_over, "frac_overlapped": achieved_over / peak,
-                    "units": "achieved = algorithmic bytes of one STEP (148 scans, SURVEY 8d's per-point figures) / the stage's own "
+                    "units": f"achieved = algorithmic bytes of one STEP ({B} scans, SURVEY 8d's per-point figures) / the stage's own "
                              "device time per step: CUDA events around the stage's launches with nothing else on the GPU (one "
-                             f"context, its two sub-batches of 74 scans back to back on one stream, {serial_steps} steps after the timed loops); achieved_overlapped divides by "
+                             f"context, its two sub-batches of {B // 2} scans back to back on one stream, {serial_steps} steps after the timed loops); achieved_overlapped divides by "
                              "the same events' time inside the timed region, where two contexts, two sub-batch streams and the "
-                             "exchange share the GPU; traffic = ncu dram bytes of the stage's kernels per STEP (profiles/)",
+                             "exchange share the GPU",
                     "stages": {k: {"ms_per_step": round(v["ms_per_step"], 4),
                                    "ms_per_step_overlapped": round(v["ms_per_step_overlapped"], 4),
                                    "gbps": None if not v["bytes_per_step"] else round(v["bytes_per_step"] / (v["ms_per_step"] * 1e-3) / 1e9, 2)}
@@ -723,16 +731,40 @@ def main():
     note("done")
 
 
+def dump_outputs(out_dir, results, states, table):
+    """What the caller of the timed step receives, as float32 / float64 .npy files (ScanResult fields by name, the 16-vector
+    states p q v ba bg, the constraint table of the step's exchange). A few kB per scan: far below 64 MB at any batch."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"states": np.asarray(states, np.float64)}
+    for name in ("pose_estimate_local", "pose_observation_in_submap"):
+        arrays[name] = np.array([list(getattr(r, name)) for r in results], np.float64).reshape(-1, 7)
+    for name in ("initial_cost", "final_cost"):
+        arrays[name] = np.array([getattr(r.summary, name) for r in results], np.float64)
+    arrays["rtcsm_score"] = np.array([r.rtcsm_score for r in results], np.float32)
+    counts = ["num_iterations", "num_successful_steps", "num_unsuccessful_steps", "termination", "num_evaluations"]
+    arrays["summary_counts"] = np.array([[getattr(r.summary, k) for k in counts] for r in results], np.float64).reshape(-1, len(counts))
+    counts = ["ok", "num_first_filter", "num_returns", "num_misses", "num_high_resolution", "num_low_resolution",
+              "num_cropped_high", "num_cropped_low", "num_passes_high", "num_passes_low"]
+    arrays["result_counts"] = np.array([[getattr(r, k) for k in counts] for r in results], np.float64).reshape(-1, len(counts))
+    if table is not None:
+        arrays["constraint_ids"] = np.array([[c.submap_id, c.node_id, c.found, c.rank] for c in table], np.float64).reshape(-1, 4)
+        arrays["constraint_scores"] = np.array([[c.score, c.low_resolution_score] for c in table], np.float32).reshape(-1, 2)
+        arrays["constraint_poses"] = np.array([list(c.pose) for c in table], np.float64).reshape(-1, 7)
+        arrays["constraint_weights"] = np.array([[c.translation_weight, c.rotation_weight] for c in table], np.float64).reshape(-1, 2)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def measure_extras(args, w, dliom, ctx, timed_device_loop, fetch_lane0, B, fo, hi=None, lo=None):
     """Secondary measurements at N = 1: each is its own short device-timed loop over the same resident batch."""
     extras = {}
-    steps = max(10, min(args.steps, 30))
+    steps = args.steps
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     try:
         ms = timed_device_loop(steps, with_exchange=False)
         extras["front_end_only"] = {"value": B / (ms / steps / 1e3), "unit": UNIT, "ms_per_step": ms / steps,
@@ -914,7 +946,7 @@ def measure_configs2(args, w, dliom, ctx, peak, num_scans=16, map_scans=12, step
                          "frac": None if achieved is None else achieved / peak, "traffic": None,
                          "bytes_model": "R (12 N + 2 N L) per scan: the cloud once per rotation + one 2-byte voxel per (point, translation)",
                          "note": "voxel reads are L1/L2 hits by design (a translation window touches <= 8 bricks): the kernel is "
-                                 "issue-bound, not HBM-bound; see profiles/"},
+                                 "issue-bound, not HBM-bound"},
             "all_ok": bool(all(r.ok == 1 for r in res)),
             "parity_scan0": {"rtcsm_score_equal": bool(np.float32(res[0].rtcsm_score) == np.float32(want["score"])),
                              "gpu_score": float(res[0].rtcsm_score), "oracle_score": float(want["score"])}}

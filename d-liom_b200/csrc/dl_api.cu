@@ -1691,8 +1691,8 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
   fa.origins = f.origins; fa.cap = f.cap; fa.tiles = f.tiles; fa.tcap2 = f.tcap2;
   // First-filter table of the fused path: the next power of two above 2 * cap (load ~0.18 on real sweeps). A compact table of
   // 1.25 slots per point (the kernels take any size: slot = hash * tcap >> 32) saves a third of the memset and of the ingest
-  // kernel's table stream but costs the first filter more in collisions than it saves: 117.5 k vs 119.8 k scans/s
-  // (profiles/r3j_ab.log) — kept as DLIOM_TABLE1_COMPACT=1 for experiments.
+  // kernel's table stream but costs the first filter more in collisions than it saves — kept as DLIOM_TABLE1_COMPACT=1 for
+  // experiments.
   fa.tcap1 = f.tcap;
   if (const char* env = std::getenv("DLIOM_TABLE1_COMPACT"))
     if (std::atoi(env)) fa.tcap1 = std::min<int64_t>(f.tcap, ((f.cap + f.cap / 4 + 63) / 64) * 64);
@@ -1825,13 +1825,14 @@ size_t imu_run_device_bytes(int num_scans, const dl_frontend_imu_samples* raw) {
 // CTAs per least-squares problem. The pipeline's adaptive filters hand the matcher a few hundred points: one CTA. With the filters
 // opened up (min_num_points in the thousands: SURVEY 8d's full-cloud mode F, tens of thousands of points per solve) one 256-thread
 // CTA per problem is latency-bound and leaves half the SMs idle, so the problem is spread over a thread-block cluster — as many
-// CTAs as keep the launch within one wave of the SMs (2 for the bench's 74-problem sub-batches), at most the portable 8.
+// CTAs as keep the launch within one wave of the SMs (on an H100's 132 SMs: 2 for sub-batches of up to 66 problems, 1 for the
+// bench's 74), at most the portable 8.
 // DLIOM_NLS_CLUSTER=n forces n (1 = never).
 int solve_cluster_size(dl_context* ctx, const dl_frontend_options& o, int problems) {
   if (const char* env = std::getenv("DLIOM_NLS_CLUSTER")) return std::max(1, std::min(8, std::atoi(env)));
   const float few = 4096.f;
   if (o.high_resolution_adaptive_voxel_filter.min_num_points < few && o.low_resolution_adaptive_voxel_filter.min_num_points < few) return 1;
-  int sms = 148;
+  int sms = kNumSMs;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
   int cs = 1;
   while (cs < 8 && problems * cs * 2 <= sms) cs *= 2;
@@ -1915,7 +1916,7 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
       for (int b = 0; b < num_scans; ++b) max_runs = std::max(max_runs, (int)(o.time_run_offsets[b + 1] - o.time_run_offsets[b]));
       // The run of a row is found by a binary search of the scan's ~2 k run starts (L1-resident) per survivor. Expanding the run
       // index of EVERY row once per batch (4 B per row, one more kernel and 17 MB of writes per step, then one random sector per
-      // survivor) makes the ingest kernel itself 5 % faster but the step 1.6 % slower (profiles/r3k_sweep.log): DLIOM_EXPAND_RUNS=1.
+      // survivor) makes the ingest kernel itself faster but the step slower: kept as DLIOM_EXPAND_RUNS=1 for experiments.
       const char* expand = std::getenv("DLIOM_EXPAND_RUNS");
       if (expand && std::atoi(expand) != 0) {
         int32_t* d_run_of_row = a.take<int32_t>((size_t)num_scans * in_cap);
@@ -1936,8 +1937,8 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
   // every back half (latency-bound, one or two CTAs per scan) on a HIGH-PRIORITY stream behind its front half's event, so
   // the back half of sub-batch k gets SMs the moment CTAs of front half k+1 retire instead of queueing behind that grid.
   // 0 (default): sub-batches alternate between two equal-priority streams.
-  // (Measured on B200, profiles/r1_pipeline_variants.log: 0 wins — the back half is latency-bound, so serialising all back
-  // halves on one stream costs more than the priority gains; 1 is kept for experiments.)
+  // (0 is the default because the back half is latency-bound, so serialising all back halves on one stream costs more than the
+  // priority gains; 1 is kept for experiments.)
   int split = 0;
   if (const char* env = std::getenv("DLIOM_PIPELINE")) split = rtcsm ? 0 : std::atoi(env);
   // DLIOM_SERIAL=1: every sub-batch on the main stream, nothing overlaps (bench.py's per-stage roofline pass: the stage events then

@@ -1,4 +1,4 @@
-// Multi-GPU exchange steps of the path, issued from the C-ABI over NCCL (NVLink 5 / NVSwitch on the B200 box).
+// Multi-GPU exchange steps of the path, issued from the C-ABI over NCCL (NVLink / NVSwitch within a box).
 //
 // One process per GPU; the scan-to-submap problems are independent, so the front end itself needs no collective. The steps
 // that do exchange data are the ones the reference hands to its constraint-builder thread pool and its pose graph

@@ -4,8 +4,8 @@
 // The reference prunes the (x, y, z) translation window with a stack of max-pooled 8-bit "precomputation" grids
 // (PrecomputationGridStack3D, :57-77; PrecomputeGrid, precomputation_grid_3d.cc:62-81) because a CPU cannot afford the
 // ~10^5 leaves x 10^3 points of the full window. The bounds are exact, so branch and bound returns the best-scoring
-// leaf that passes the low-resolution gate — which is also what scoring EVERY leaf returns. On a B200 the brute-force
-// cube is a few hundred microseconds of L1/L2-resident integer gathers, needs no precomputation stack at all (the
+// leaf that passes the low-resolution gate — which is also what scoring EVERY leaf returns. On the GPU the brute-force
+// cube is L1/L2-resident integer gathers, needs no precomputation stack at all (the
 // 8-bit value is derived from the uint16 cell on the fly with the reference's float expression,
 // precomputation_grid_3d.cc:50-53) and has no data-dependent control flow:
 //   cells      c_i = GetCellIndex(pose * p_i)                                 (float, exact)

@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_second_ins
   // probing it once per raw point. Order does not matter here: the second filter keys on the original index.
   if (n == 0) return;
   // (four slots per thread and step through one 16-byte load: same kernel time in the serial launch list, slightly slower in the
-  //  overlapped step — profiles/r3b_ab.log — so the stream stays one slot per thread)
+  //  overlapped step, so the stream stays one slot per thread)
   for (int h = blockIdx.x * kBlock + threadIdx.x; h < (int)a.tcap1; h += gridDim.x * kBlock) {
     const uint32_t owner = __ldcg(tab + h);
     const bool surv = owner != kEmpty32;
@@ -500,8 +500,8 @@ int launch_fe_first_filter(dl_context* ctx, FrontendArgs a, int first_scan, int 
   a.first_scan = first_scan;
   const int tiles = (int)std::min<int64_t>((a.cap + kBlock - 1) / kBlock, 128);
   if (const char* env = std::getenv("DLIOM_FE_FLAGS")) a.flags = std::atoi(env);  // experiments: 1 = always CAS in the first filter
-  // points in flight per thread: 1 is the measured optimum (profiles/r3a_sweep.log: 113.4 k scans/s; 2 -> 108.8 k; 4 -> 94.2 k) —
-  // the kernel runs at the L2's atomic throughput (~130 G CAS/s), more outstanding atomics only lengthen its queues
+  // points in flight per thread: 1 is the default (2 and 4 measured slower) — the kernel runs at the L2's atomic throughput, more
+  // outstanding atomics only lengthen its queues
   const int batch_points = (a.flags & 3) == 2 ? 2 : ((a.flags & 3) == 3 ? 4 : 1);
   if (batch_points == 1) fe_first_filter_insert<1><<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
   else if (batch_points == 2) fe_first_filter_insert<2><<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
@@ -534,7 +534,7 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
     DL_CUDA(ctx, cudaFuncSetAttribute(fe_emit_tracking, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     emit_attr = true;
   }
-  int parts = 4;  // CTAs per scan: 74 scans x 4 = two CTAs of 512 threads per SM
+  int parts = 4;  // CTAs per scan: a 74-scan sub-batch x 4 = 296 CTAs of 512 threads, about two per SM of an H100
   if (const char* env = std::getenv("DLIOM_EMIT_PARTS")) parts = std::max(1, std::atoi(env));
   fe_emit_tracking<<<dim3(parts, batch), kEmitBlock, smem, ctx->stream>>>(a, max_chunks);
   DL_LAUNCH_CHECK(ctx, "fe_emit_tracking");

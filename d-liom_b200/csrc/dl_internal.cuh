@@ -14,7 +14,7 @@
 
 namespace dl {
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ------------------------------------------------------------------------------------------------ device grid
 // Index-array form of HybridGrid's three levels (hybrid_grid.h:411-412): top cell = 64^3 voxels

@@ -881,7 +881,7 @@ __global__ void grid_lookup_kernel(GridView g, int64_t n, const int32_t* __restr
 // Threads per problem (multiple of 32, <= kBlock). DLIOM_NLS_BLOCK overrides for experiments.
 static int nls_block_threads() {
   static const int threads = [] {
-    int t = kBlock;  // measured on B200 (profiles/r1_pipeline_variants.log): 256 > 128 > 64 > 32 for ~400-point problems
+    int t = kBlock;  // fewer threads per ~400-point problem measured slower: the evaluation pass serialises inside a thread
     if (const char* env = std::getenv("DLIOM_NLS_BLOCK")) t = std::atoi(env);
     t = (t / 32) * 32;
     return t < 32 ? 32 : (t > kBlock ? kBlock : t);

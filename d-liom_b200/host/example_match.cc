@@ -1,5 +1,5 @@
 // Reads like SM/ceres_scan_matcher_3d_test.cc:34-116 and SM/real_time_correlative_scan_matcher_3d_test.cc:36-117,
-// but runs the B200 path through the C++ shim. Build: g++ -std=c++17 example_match.cc -L.. -ldliom_b200
+// but runs the GPU path through the C++ shim. Build: g++ -std=c++17 example_match.cc -L.. -ldliom_b200
 #include <cmath>
 #include <cstdio>
 

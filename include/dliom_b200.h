@@ -1,4 +1,4 @@
-/* dliom_b200 — C-ABI of the B200-native scan-registration hot path.
+/* dliom_b200 — C-ABI of the H100-native (sm_90a) scan-registration hot path.
  *
  * Every entry point replaces one CPU interface of the reference (peterWon/D-LIOM, a Cartographer fork).
  * Citations: C/ = src/cartographer/cartographer/, SM/ = C/mapping/internal/3d/scan_matching/,

@@ -11,22 +11,29 @@ Trajectory: 10 m/s along +x with a 0.2 rad/s-amplitude yaw sinusoid; the sensor 
 import ctypes
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _RAYCAST = None
+RAYCAST_LIB = os.path.join(_HERE, "libraycast.so")
+
+
+def build_raycast(path=RAYCAST_LIB):
+    subprocess.check_call(["gcc", "-O2", "-fopenmp", "-shared", "-fPIC", "-o", path, os.path.join(_HERE, "raycast.c"), "-lm"])
 
 
 def _raycast_lib():
-    """tools/libraycast.so (C, OpenMP): ~40x faster than the numpy path; built on first use, optional."""
+    """tools/libraycast.so (C, OpenMP), made by __graft_entry__.build(): ~40x faster than the numpy path. In a tree that was not
+    built it is compiled into a temporary directory, never into the tree (which may be read-only); optional."""
     global _RAYCAST
     if _RAYCAST is None:
-        path = os.path.join(_HERE, "libraycast.so")
+        path = RAYCAST_LIB
         try:
             if not os.path.exists(path):
-                subprocess.check_call(["gcc", "-O2", "-fopenmp", "-shared", "-fPIC", "-o", path,
-                                       os.path.join(_HERE, "raycast.c"), "-lm"])
+                path = os.path.join(tempfile.mkdtemp(prefix="dliom-raycast-"), "libraycast.so")
+                build_raycast(path)
             L = ctypes.CDLL(path)
             dp = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
             L.synth_raycast.argtypes = [ctypes.c_int64, dp, dp, ctypes.c_double, ctypes.c_double, ctypes.c_int, dp, dp,
