@@ -32,7 +32,7 @@ EXPORTS = [
     "dl_frontend_collect_imu",
     "dl_comm_unique_id", "dl_comm_create", "dl_comm_destroy", "dl_comm_rank", "dl_comm_world_size", "dl_comm_last_error",
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
-    "dl_pose_graph_solve", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
+    "dl_pose_graph_solve", "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
 ]
 
@@ -262,6 +262,12 @@ class PoseGraphInfo(C.Structure):
                 ("all_reduce_ms", C.c_float), ("all_reduce_min_ms", C.c_float)]
 
 
+class PoseGraphSparseInfo(C.Structure):   # dl_pose_graph_sparse_info
+    _fields_ = [("num_local_parameters", C.c_int32), ("all_reduce_count", C.c_int32), ("all_reduce_bytes", C.c_int64),
+                ("all_reduce_ms", C.c_float), ("all_reduce_min_ms", C.c_float), ("num_reduced_parameters", C.c_int32),
+                ("num_pairs", C.c_int32), ("setup_exchange_bytes", C.c_int64)]
+
+
 class LtbOptions(C.Structure):   # dl_ltb_options
     _fields_ = [("frontend", FrontendOptions), ("imu_noise", ImuNoise), ("imu_weight", C.c_double), ("gravity", C.c_double),
                 ("high_resolution", C.c_float), ("low_resolution", C.c_float), ("num_range_data", C.c_int32),
@@ -300,6 +306,22 @@ class MatchingResult(C.Structure):   # dl_matching_result
                 ("state", NavState), ("scan", ScanResult), ("origin_in_local", C.c_float * 3), ("num_returns", C.c_int32),
                 ("num_misses", C.c_int32), ("num_high_resolution", C.c_int32), ("num_low_resolution", C.c_int32),
                 ("num_insertion_submaps", C.c_int32), ("insertion_submap_index", C.c_int32 * 2), ("reserved", C.c_int32)]
+
+
+def spa_constraints(constraints):
+    """(submap, node, zbar7, translation_weight, rotation_weight) tuples -> a dl_spa_constraint array (numpy-packed: graphs of
+    tens of thousands of constraints)."""
+    n = len(constraints)
+    arr = np.zeros(max(n, 1), dtype=np.dtype([("submap", np.int32), ("node", np.int32), ("zbar", np.float64, 7),
+                                               ("tw", np.float64), ("rw", np.float64)], align=True))
+    if n:
+        arr["submap"][:n] = [c[0] for c in constraints]
+        arr["node"][:n] = [c[1] for c in constraints]
+        arr["zbar"][:n] = np.asarray([c[2] for c in constraints], np.float64).reshape(n, 7)
+        arr["tw"][:n] = [c[3] for c in constraints]
+        arr["rw"][:n] = [c[4] for c in constraints]
+    assert arr.dtype.itemsize == C.sizeof(SpaConstraint)
+    return (SpaConstraint * len(arr)).from_buffer(arr)
 
 
 def lib():
@@ -390,6 +412,8 @@ def lib():
     L.dl_window_optimize_batch.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, vp, f64p, vp]
     L.dl_pose_graph_solve.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, C.c_int32, ip(SolveSummary),
                                       ip(PoseGraphInfo)]
+    L.dl_pose_graph_solve_sparse.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, vp, C.c_int32,
+                                             ip(SolveSummary), ip(PoseGraphSparseInfo)]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
     L.dl_ltb_create.argtypes = [vp, ip(LtbOptions), ip(vp)]
     L.dl_ltb_destroy.argtypes = [vp]
@@ -675,6 +699,25 @@ class Context:
         s, info = SolveSummary(), PoseGraphInfo()
         self.check(self.L.dl_pose_graph_solve(self.h, comm.h if comm else None, C.byref(opt), S, N, poses, C.cast(cs, C.c_void_p),
                                               len(constraints), C.byref(s), C.byref(info)))
+        return poses[:S].copy(), poses[S:].copy(), s.as_dict(), info
+
+    def pose_graph_solve_sparse(self, submap_poses, node_poses, constraints, fix_z=False, max_iter=50, comm=None, frozen=None):
+        """The block-sparse (Schur) solve of the same problem for whole trajectories, with frozen poses. frozen: None or
+        len(submaps) + len(nodes) flags (submaps first). -> (submaps, nodes, summary, PoseGraphSparseInfo)."""
+        S, N = len(submap_poses), len(node_poses)
+        poses = np.ascontiguousarray(np.concatenate([np.asarray(submap_poses, np.float64).reshape(S, 7),
+                                                     np.asarray(node_poses, np.float64).reshape(N, 7)]))
+        cs = spa_constraints(constraints)
+        fz = None
+        if frozen is not None:
+            fz = np.ascontiguousarray(np.asarray(frozen, bool).astype(np.uint8).reshape(-1))
+            if len(fz) != S + N:
+                raise ValueError(f"frozen has {len(fz)} flags, the graph {S + N} poses")
+        opt = PoseGraphOptions(int(max_iter), int(bool(fix_z)))
+        s, info = SolveSummary(), PoseGraphSparseInfo()
+        self.check(self.L.dl_pose_graph_solve_sparse(self.h, comm.h if comm else None, C.byref(opt), S, N, poses,
+                                                     fz.ctypes.data if fz is not None else None, C.cast(cs, C.c_void_p),
+                                                     len(constraints), C.byref(s), C.byref(info)))
         return poses[:S].copy(), poses[S:].copy(), s.as_dict(), info
 
     @staticmethod

@@ -16,6 +16,7 @@
 #include <cstdint>
 #include <cstring>
 #include <deque>
+#include <map>
 #include <set>
 #include <stdexcept>
 #include <string>
@@ -564,4 +565,100 @@ class LocalTrajectoryBuilder3D {  // local_trajectory_builder_3d.h:81-113
 };
 
 }  // namespace mapping
+
+namespace optimization {
+
+struct SubmapId {  // mapping::SubmapId
+  int trajectory_id, submap_index;
+  bool operator<(const SubmapId& o) const { return trajectory_id != o.trajectory_id ? trajectory_id < o.trajectory_id : submap_index < o.submap_index; }
+};
+struct NodeId {  // mapping::NodeId
+  int trajectory_id, node_index;
+  bool operator<(const NodeId& o) const { return trajectory_id != o.trajectory_id ? trajectory_id < o.trajectory_id : node_index < o.node_index; }
+};
+struct SubmapSpec3D { Rigid3d global_pose; };  // optimization_problem_3d.h: SubmapSpec3D
+struct NodeSpec3D { Rigid3d global_pose; };    // the part of NodeSpec3D that Solve reads (time, local pose and gravity feed the
+                                               // IMU / odometry terms this fork comments out)
+struct Constraint {  // PoseGraphInterface::Constraint: node observed from submap
+  SubmapId submap_id;
+  NodeId node_id;
+  Rigid3d zbar_ij;
+  double translation_weight, rotation_weight;
+};
+struct OptimizationProblemOptions {  // proto::OptimizationProblemOptions, the fields Solve reads (pose_graph.lua)
+  int max_num_iterations = 50;
+  bool fix_z_in_3d = false;
+};
+
+// optimization::OptimizationProblem3D (optimization_problem_3d.h) as this fork's Solve runs it, on the device's block-sparse pose
+// adjustment (dl_pose_graph_solve_sparse). Submaps and nodes are kept per trajectory in id order; the first submap in that order
+// keeps its translation and yaw; every submap and node of a trajectory in frozen_trajectories is constant. With a communicator,
+// `constraints` are this rank's share and every rank ends with the same poses.
+class OptimizationProblem3D {
+ public:
+  explicit OptimizationProblem3D(Context* ctx, const OptimizationProblemOptions& options = {}, dl_comm* comm = nullptr)
+      : ctx_(ctx), options_(options), comm_(comm) {}
+  void AddSubmap(int trajectory_id, const Rigid3d& global_submap_pose) {
+    submap_data_[{trajectory_id, next_submap_[trajectory_id]++}] = {global_submap_pose};
+  }
+  void AddTrajectoryNode(int trajectory_id, const NodeSpec3D& node_data) { node_data_[{trajectory_id, next_node_[trajectory_id]++}] = node_data; }
+  void SetMaxNumIterations(int32_t max_num_iterations) { options_.max_num_iterations = max_num_iterations; }
+
+  void Solve(const std::vector<Constraint>& constraints, const std::set<int>& frozen_trajectories = {}) {
+    if (node_data_.empty() || submap_data_.empty()) return;  // the reference: nothing to optimize
+    std::map<SubmapId, int> submap_index;
+    std::map<NodeId, int> node_index;
+    std::vector<double> poses;
+    std::vector<uint8_t> frozen;
+    for (const auto& kv : submap_data_) {
+      submap_index[kv.first] = (int)submap_index.size();
+      poses.resize(poses.size() + 7);
+      kv.second.global_pose.to7(poses.data() + poses.size() - 7);
+      frozen.push_back(frozen_trajectories.count(kv.first.trajectory_id) ? 1 : 0);
+    }
+    for (const auto& kv : node_data_) {
+      node_index[kv.first] = (int)node_index.size();
+      poses.resize(poses.size() + 7);
+      kv.second.global_pose.to7(poses.data() + poses.size() - 7);
+      frozen.push_back(frozen_trajectories.count(kv.first.trajectory_id) ? 1 : 0);
+    }
+    std::vector<dl_spa_constraint> cs;
+    cs.reserve(constraints.size());
+    for (const Constraint& c : constraints) {
+      const auto si = submap_index.find(c.submap_id);
+      const auto ni = node_index.find(c.node_id);
+      if (si == submap_index.end() || ni == node_index.end()) throw Error(DL_ERR_ARG, "constraint refers to an unknown submap or node");
+      dl_spa_constraint d{};
+      d.submap = si->second;
+      d.node = ni->second;
+      c.zbar_ij.to7(d.zbar);
+      d.translation_weight = c.translation_weight;
+      d.rotation_weight = c.rotation_weight;
+      cs.push_back(d);
+    }
+    const dl_pose_graph_options o{options_.max_num_iterations, options_.fix_z_in_3d ? 1 : 0};
+    ctx_->check(dl_pose_graph_solve_sparse(ctx_->get(), comm_, &o, (int32_t)submap_data_.size(), (int32_t)node_data_.size(), poses.data(),
+                                           frozen.data(), cs.data(), (int32_t)cs.size(), &summary_, &info_));
+    const double* p = poses.data();
+    for (auto& kv : submap_data_) { kv.second.global_pose = Rigid3d::from7(p); p += 7; }
+    for (auto& kv : node_data_) { kv.second.global_pose = Rigid3d::from7(p); p += 7; }
+  }
+
+  const std::map<SubmapId, SubmapSpec3D>& submap_data() const { return submap_data_; }
+  const std::map<NodeId, NodeSpec3D>& node_data() const { return node_data_; }
+  const dl_solve_summary& summary() const { return summary_; }
+  const dl_pose_graph_sparse_info& info() const { return info_; }
+
+ private:
+  Context* ctx_;
+  OptimizationProblemOptions options_;
+  dl_comm* comm_;
+  std::map<SubmapId, SubmapSpec3D> submap_data_;
+  std::map<NodeId, NodeSpec3D> node_data_;
+  std::map<int, int> next_submap_, next_node_;
+  dl_solve_summary summary_{};
+  dl_pose_graph_sparse_info info_{};
+};
+
+}  // namespace optimization
 }  // namespace dliom

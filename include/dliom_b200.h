@@ -331,6 +331,37 @@ int dl_pose_graph_solve(dl_context* ctx, dl_comm* comm, const dl_pose_graph_opti
                         double* poses, const dl_spa_constraint* constraints, int32_t num_constraints, dl_solve_summary* summary,
                         dl_pose_graph_info* info);
 
+/* ---- The same solve for whole trajectories, block-sparse: every SpaCostFunction3D joins one submap and one node, so the node
+ *      blocks are eliminated (Schur complement) and only the submaps' reduced system is factored densely, in one CTA. poses,
+ *      constraints, options and comm mean what they mean for dl_pose_graph_solve.
+ *      frozen: num_submaps + num_nodes flags (NULL = none); a frozen pose is constant (OptimizationProblem3D::Solve's
+ *      frozen_trajectories, optimization_problem_3d.cc:283-329): it has no parameters, and if it is the first submap its rotation
+ *      is constant too. Constraints between two frozen poses only add a fixed cost: initial_cost / final_cost include it (as
+ *      Ceres 1.13 reports them) while the tolerances see the rest. With every pose frozen the poses come back unchanged,
+ *      termination CONVERGENCE, no iterations.
+ *      Deterministic: no floating-point atomics; two calls on the same input return bit-identical poses, and with a communicator
+ *      every rank does identical work after the all-reduce.
+ *      Errors (DL_ERR_ARG, all detected before the first collective except the last, which every rank detects together after the
+ *      set-up all-gather): an index outside the graph; more than DL_POSE_GRAPH_MAX_REDUCED submap parameters; a graph whose
+ *      submap / node counts, frozen poses, reduced size, fix_z or iteration limit differ between the ranks. A device-memory
+ *      reservation made after the first collective is agreed on by all ranks (a one-int all-gather), so every rank returns the
+ *      same failure instead of one leaving its peers waiting. ------------------------------------------------------------- */
+#define DL_POSE_GRAPH_MAX_REDUCED 3072
+typedef struct dl_pose_graph_sparse_info {
+  int32_t num_local_parameters;   /* live parameters of all poses */
+  int32_t all_reduce_count;       /* one per evaluation */
+  int64_t all_reduce_bytes;       /* per all-reduce: 8 * (2 + 42 * (num_submaps + num_nodes) + 36 * num_pairs) */
+  float all_reduce_ms;            /* summed device time of the all-reduces (CUDA events) */
+  float all_reduce_min_ms;        /* fastest single all-reduce */
+  int32_t num_reduced_parameters; /* size of the factored system: the live parameters of the submaps */
+  int32_t num_pairs;              /* distinct (submap, node) pairs with a constraint not between two frozen poses, all ranks */
+  int64_t setup_exchange_bytes;   /* received by this rank in the set-up all-gathers (0 without a communicator):
+                                     world * (32 + 4), plus world * (4 + 8 * largest per-rank pair count) if any rank has pairs */
+} dl_pose_graph_sparse_info;
+int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const dl_pose_graph_options* options, int32_t num_submaps,
+                               int32_t num_nodes, double* poses, const uint8_t* frozen, const dl_spa_constraint* constraints,
+                               int32_t num_constraints, dl_solve_summary* summary, dl_pose_graph_sparse_info* info);
+
 /* ---- IMU: pre-integration (LocalTrajectoryBuilder3D::AddImuData, LTB:164-201, with the in-repo mid-point integrator
  *      C/mapping/internal/3d/initialization/integration_base.h:109-265 instead of the un-vendored GTSAM one) and the
  *      scan match with the pre-integration residual (integration_base.h:267-301) fused into the same solve.
