@@ -4,7 +4,7 @@
 // that do exchange data are the ones the reference hands to its constraint-builder thread pool and its pose graph
 // (SURVEY 8e): every rank searches the (node, submap) pairs whose submap it OWNS (constraint_builder_3d.cc:189-197) and the
 // found constraints (constraint_builder_3d.cc:328-333) are all-gathered so that every rank holds the same table for the
-// replicated pose graph; the pose graph's normal equations are all-reduced in fp64 (dl_posegraph.cu); a finished submap
+// replicated pose graph; the pose graph's normal-equation blocks are all-reduced in fp64 (dl_posegraph_sparse.cu); a finished submap
 // moves between ranks by one broadcast of its brick arrays.
 //
 // NCCL is bound at run time (dlopen of libnccl.so.2, the library the host process already uses when it is a

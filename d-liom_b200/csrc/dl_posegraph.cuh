@@ -1,8 +1,8 @@
-// Pieces shared by the dense (dl_posegraph.cu) and the block-sparse (dl_posegraph_sparse.cu) pose-graph solvers:
+// Building blocks of the block-sparse pose-graph solve (dl_posegraph_sparse.cu):
 //   - forward-mode duals over the 14 ambient parameters of one SpaCostFunction3D and the residual itself,
 //   - the one-CTA dense Cholesky factor and triangular solves,
 //   - the Ceres 1.13 TrustRegionMinimizer state machine (LM, monotonic steps, pose_graph.lua's options) run on the host, with
-//     the solver-specific evaluation and step behind callbacks.
+//     the device evaluation and step behind callbacks (tests/schur_oracle.py mirrors the same state machine on the CPU).
 #pragma once
 #include <cmath>
 #include <functional>

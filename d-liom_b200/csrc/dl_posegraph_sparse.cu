@@ -1,11 +1,12 @@
 // Block-sparse sparse pose adjustment: OptimizationProblem3D::Solve (optimization_problem_3d.cc:259-589) on whole trajectories,
-// with frozen trajectories (:283-329), for graphs the dense solver (dl_posegraph.cu) cannot hold.
+// with frozen trajectories (:283-329).
 //
 // Structure: every residual of this fork is a SpaCostFunction3D between one submap and one node, so the normal equations are
 //   [ blockdiag(H_ss)  H_sn            ]
 //   [ H_ns             blockdiag(H_nn) ]
-// Eliminating the node blocks (Schur complement) leaves a dense system over the submaps only, which one CTA factors with the
-// dense solver's Cholesky; the node steps follow by back-substitution. In exact arithmetic this is the dense solver's LM step.
+// Eliminating the node blocks (Schur complement) leaves a dense system over the submaps only, which one CTA factors with a
+// Cholesky; the node steps follow by back-substitution. In exact arithmetic this is the LM step of the dense normal equations,
+// as the oracle (oracle/orc_posegraph.h) takes it.
 //
 // Every pose owns a 6-slot block; its first dim(p) slots are live: 0 if frozen (Ceres removes constant blocks), 2 for the first
 // submap (constant translation, ConstantYawQuaternionPlus), else 3 + tdof (fix_z: tdof = 2). Dead slots carry zeros in the
@@ -376,7 +377,7 @@ __global__ void sp_reduce_kernel(Payload pl, int S, const int* __restrict__ dim,
   }
 }
 
-// One CTA: the reduced system's dense Cholesky and solves (the dense solver's factor).
+// One CTA: the reduced system's dense Cholesky and solves (cta_cholesky_*, dl_posegraph.cuh).
 __global__ void __launch_bounds__(1024) sp_reduced_solve_kernel(int n_red, StepBufs b) {
   __shared__ int ok_s;
   cta_cholesky_factor(b.A, n_red, &ok_s);

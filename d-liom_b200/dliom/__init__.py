@@ -32,7 +32,7 @@ EXPORTS = [
     "dl_frontend_collect_imu",
     "dl_comm_unique_id", "dl_comm_create", "dl_comm_destroy", "dl_comm_rank", "dl_comm_world_size", "dl_comm_last_error",
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
-    "dl_pose_graph_solve", "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
+    "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
 ]
 
@@ -257,11 +257,6 @@ class PoseGraphOptions(C.Structure):
     _fields_ = [("max_num_iterations", C.c_int32), ("fix_z", C.c_int32)]
 
 
-class PoseGraphInfo(C.Structure):
-    _fields_ = [("num_local_parameters", C.c_int32), ("all_reduce_count", C.c_int32), ("all_reduce_bytes", C.c_int64),
-                ("all_reduce_ms", C.c_float), ("all_reduce_min_ms", C.c_float)]
-
-
 class PoseGraphSparseInfo(C.Structure):   # dl_pose_graph_sparse_info
     _fields_ = [("num_local_parameters", C.c_int32), ("all_reduce_count", C.c_int32), ("all_reduce_bytes", C.c_int64),
                 ("all_reduce_ms", C.c_float), ("all_reduce_min_ms", C.c_float), ("num_reduced_parameters", C.c_int32),
@@ -410,8 +405,6 @@ def lib():
     L.dl_constraint_search_exchange.argtypes = [vp, vp, ip(ConstraintOptions), C.c_int32, C.c_int32, i32p, i32p, f64p, f32p, i64p,
                                                 f32p, i64p, C.c_void_p, C.c_void_p, ip(ConstraintRow), ip(ExchangeInfo)]
     L.dl_window_optimize_batch.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, vp, f64p, vp]
-    L.dl_pose_graph_solve.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, C.c_int32, ip(SolveSummary),
-                                      ip(PoseGraphInfo)]
     L.dl_pose_graph_solve_sparse.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, vp, C.c_int32,
                                              ip(SolveSummary), ip(PoseGraphSparseInfo)]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
@@ -686,24 +679,11 @@ class Context:
                                                    C.cast(out_j, C.c_void_p), info.reshape(-1), C.cast(sums, C.c_void_p)))
         return (np.array([o.to16() for o in out_i]), np.array([o.to16() for o in out_j]), info, [s.as_dict() for s in sums])
 
-    def pose_graph_solve(self, submap_poses, node_poses, constraints, fix_z=False, max_iter=50, comm=None):
-        """OptimizationProblem3D::Solve (SPA only) on the device. constraints: this rank's (submap, node, zbar7, translation_weight,
-        rotation_weight) tuples; with `comm` the normal equations are all-reduced over the ranks. -> (submaps, nodes, summary, info)."""
-        S, N = len(submap_poses), len(node_poses)
-        poses = np.ascontiguousarray(np.concatenate([np.asarray(submap_poses, np.float64).reshape(S, 7),
-                                                     np.asarray(node_poses, np.float64).reshape(N, 7)]))
-        cs = (SpaConstraint * max(len(constraints), 1))()
-        for k, (i, j, z, tw, rw) in enumerate(constraints):
-            cs[k] = SpaConstraint(int(i), int(j), (C.c_double * 7)(*[float(v) for v in z]), float(tw), float(rw))
-        opt = PoseGraphOptions(int(max_iter), int(bool(fix_z)))
-        s, info = SolveSummary(), PoseGraphInfo()
-        self.check(self.L.dl_pose_graph_solve(self.h, comm.h if comm else None, C.byref(opt), S, N, poses, C.cast(cs, C.c_void_p),
-                                              len(constraints), C.byref(s), C.byref(info)))
-        return poses[:S].copy(), poses[S:].copy(), s.as_dict(), info
-
     def pose_graph_solve_sparse(self, submap_poses, node_poses, constraints, fix_z=False, max_iter=50, comm=None, frozen=None):
-        """The block-sparse (Schur) solve of the same problem for whole trajectories, with frozen poses. frozen: None or
-        len(submaps) + len(nodes) flags (submaps first). -> (submaps, nodes, summary, PoseGraphSparseInfo)."""
+        """OptimizationProblem3D::Solve (SPA only) on the device, block-sparse (Schur complement of the node blocks), for whole
+        trajectories. constraints: this rank's (submap, node, zbar7, translation_weight, rotation_weight) tuples; with `comm` the
+        normal-equation blocks are all-reduced over the ranks. frozen: None or len(submaps) + len(nodes) flags (submaps first).
+        -> (submaps, nodes, summary, PoseGraphSparseInfo)."""
         S, N = len(submap_poses), len(node_poses)
         poses = np.ascontiguousarray(np.concatenate([np.asarray(submap_poses, np.float64).reshape(S, 7),
                                                      np.asarray(node_poses, np.float64).reshape(N, 7)]))

@@ -307,33 +307,12 @@ int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_const
 /* ---- optimization::OptimizationProblem3D::Solve as this fork runs it (C/mapping/internal/optimization/optimization_problem_3d.cc:259-589
  *      with the IMU / consecutive-node terms commented out there): sparse pose adjustment over the SpaCostFunction3D constraints
  *      (cost_functions/spa_cost_function_3d.h:35-58), first submap's translation constant and yaw fixed, LM as pose_graph.lua sets
- *      it. poses: num_submaps submap poses then num_nodes node poses, 7 doubles each (t xyz, q wxyz), in-out, identical on every
+ *      it. Block-sparse: every SpaCostFunction3D joins one submap and one node, so the node blocks are eliminated (Schur
+ *      complement) and only the submaps' reduced system is factored densely, in one CTA.
+ *      poses: num_submaps submap poses then num_nodes node poses, 7 doubles each (t xyz, q wxyz), in-out, identical on every
  *      rank. constraints: THIS RANK'S share (e.g. the rows it contributed to dl_constraint_search_exchange); with a communicator
- *      the per-rank normal equations are summed by one ncclAllReduce(fp64) per evaluation and every rank returns the same poses.
- *      comm may be NULL (single process: all constraints local). Dense normal equations: local size <= 3072. ------------------- */
-typedef struct dl_spa_constraint { /* PoseGraphInterface::Constraint: node j observed from submap i */
-  int32_t submap, node;
-  double zbar[7];
-  double translation_weight, rotation_weight;
-} dl_spa_constraint;
-typedef struct dl_pose_graph_options {
-  int32_t max_num_iterations; /* pose_graph.lua optimization_problem.ceres_solver_options.max_num_iterations (50) */
-  int32_t fix_z;              /* optimization_problem.fix_z_in_3d */
-} dl_pose_graph_options;
-typedef struct dl_pose_graph_info {
-  int32_t num_local_parameters;
-  int32_t all_reduce_count;   /* one per evaluation */
-  int64_t all_reduce_bytes;   /* per all-reduce: (n^2 + n + 1) doubles */
-  float all_reduce_ms;        /* summed device time of the all-reduces (CUDA events) */
-  float all_reduce_min_ms;    /* fastest single all-reduce (the first one carries NCCL's lazy connection set-up) */
-} dl_pose_graph_info;
-int dl_pose_graph_solve(dl_context* ctx, dl_comm* comm, const dl_pose_graph_options* options, int32_t num_submaps, int32_t num_nodes,
-                        double* poses, const dl_spa_constraint* constraints, int32_t num_constraints, dl_solve_summary* summary,
-                        dl_pose_graph_info* info);
-
-/* ---- The same solve for whole trajectories, block-sparse: every SpaCostFunction3D joins one submap and one node, so the node
- *      blocks are eliminated (Schur complement) and only the submaps' reduced system is factored densely, in one CTA. poses,
- *      constraints, options and comm mean what they mean for dl_pose_graph_solve.
+ *      the per-rank blocks of the normal equations are summed by one ncclAllReduce(fp64) per evaluation and every rank returns
+ *      the same poses. comm may be NULL (single process: all constraints local).
  *      frozen: num_submaps + num_nodes flags (NULL = none); a frozen pose is constant (OptimizationProblem3D::Solve's
  *      frozen_trajectories, optimization_problem_3d.cc:283-329): it has no parameters, and if it is the first submap its rotation
  *      is constant too. Constraints between two frozen poses only add a fixed cost: initial_cost / final_cost include it (as
@@ -346,6 +325,15 @@ int dl_pose_graph_solve(dl_context* ctx, dl_comm* comm, const dl_pose_graph_opti
  *      submap / node counts, frozen poses, reduced size, fix_z or iteration limit differ between the ranks. A device-memory
  *      reservation made after the first collective is agreed on by all ranks (a one-int all-gather), so every rank returns the
  *      same failure instead of one leaving its peers waiting. ------------------------------------------------------------- */
+typedef struct dl_spa_constraint { /* PoseGraphInterface::Constraint: node j observed from submap i */
+  int32_t submap, node;
+  double zbar[7];
+  double translation_weight, rotation_weight;
+} dl_spa_constraint;
+typedef struct dl_pose_graph_options {
+  int32_t max_num_iterations; /* pose_graph.lua optimization_problem.ceres_solver_options.max_num_iterations (50) */
+  int32_t fix_z;              /* optimization_problem.fix_z_in_3d */
+} dl_pose_graph_options;
 #define DL_POSE_GRAPH_MAX_REDUCED 3072
 typedef struct dl_pose_graph_sparse_info {
   int32_t num_local_parameters;   /* live parameters of all poses */

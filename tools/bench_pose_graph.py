@@ -1,12 +1,11 @@
 #!/usr/bin/env python
-"""Global step of BASELINE configs[4] on N GPUs: the sparse pose adjustment with the constraints sharded by submap owner and the
-normal equations reduced with ncclAllReduce(fp64) issued from the C-ABI (dl_pose_graph_solve). Launch with torchrun like bench.py:
+"""Global step of BASELINE configs[4] on N GPUs: the block-sparse pose adjustment (dl_pose_graph_solve_sparse) with the
+constraints sharded by submap owner and the normal-equation blocks reduced with ncclAllReduce(fp64) issued from the C-ABI. Launch
+with torchrun like bench.py:
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 tools/bench_pose_graph.py
 Prints one JSON line on rank 0: solve time, all-reduce count / bytes / device time, achieved bus bandwidth, and whether every rank
-ended with bit-identical poses.
---solver sparse runs the block-sparse solve (dl_pose_graph_solve_sparse) instead; --solver both runs the two on the same graph in
-one process and adds both times, both iteration counts and the largest pose difference. --shape trajectory builds a drive (each
-node seen by its two active submaps, every --loop-every-th node also by an older submap) instead of random constraints."""
+ended with bit-identical poses. --shape trajectory builds a drive (each node seen by its two active submaps, every --loop-every-th
+node also by an older submap) instead of random constraints."""
 import argparse
 import json
 import os
@@ -37,7 +36,6 @@ def main():
     ap.add_argument("--nodes", type=int, default=400)
     ap.add_argument("--per-node", type=int, default=3, help="constraints per node (to random submaps)")
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--solver", choices=("dense", "sparse", "both"), default="dense")
     ap.add_argument("--shape", choices=("random", "trajectory"), default="random")
     ap.add_argument("--loop-every", type=int, default=1, help="trajectory shape: one loop closure every this many nodes")
     args = ap.parse_args()
@@ -76,65 +74,41 @@ def main():
         start_nodes = [compose(t, np.array([*rng.uniform(-0.5, 0.5, 3), *aa_to_q(rng.uniform(-0.1, 0.1, 3))])) for t in truth]
         start_submaps = [submaps[0]] + [compose(s, np.array([*rng.uniform(-0.3, 0.3, 3), *aa_to_q(rng.uniform(-0.05, 0.05, 3))])) for s in submaps[1:]]
     mine = [c for c in cons if c[0] % world == rank]
-    solvers = {"dense": ["dense"], "sparse": ["sparse"], "both": ["dense", "sparse"]}[args.solver]
-    results = {}
-    for solver in solvers:
-        out = None
-        times = []
-        for _ in range(args.repeats):
-            torch.cuda.synchronize()
-            if dist is not None:
-                dist.barrier()
-            t0 = time.perf_counter()
-            if solver == "dense":
-                out = ctx.pose_graph_solve(start_submaps, start_nodes, mine, comm=comm)
-            else:
-                out = ctx.pose_graph_solve_sparse(start_submaps, start_nodes, mine, comm=comm)
-            times.append(time.perf_counter() - t0)
-        s_out, n_out, summary, info = out
-        digest = torch.tensor([float(np.sum(np.abs(n_out))), float(np.sum(np.abs(s_out)))], dtype=torch.float64, device=f"cuda:{local}")
-        lo, hi = digest.clone(), digest.clone()
-        tmax = torch.tensor([min(times)], dtype=torch.float64, device=f"cuda:{local}")
+    times = []
+    for _ in range(args.repeats):
+        torch.cuda.synchronize()
         if dist is not None:
-            dist.all_reduce(lo, op=dist.ReduceOp.MIN)
-            dist.all_reduce(hi, op=dist.ReduceOp.MAX)
-            dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
-        results[solver] = (s_out, n_out, summary, info, float(tmax[0]), bool(torch.equal(lo, hi)))
+            dist.barrier()
+        t0 = time.perf_counter()
+        s_out, n_out, summary, info = ctx.pose_graph_solve_sparse(start_submaps, start_nodes, mine, comm=comm)
+        times.append(time.perf_counter() - t0)
+    digest = torch.tensor([float(np.sum(np.abs(n_out))), float(np.sum(np.abs(s_out)))], dtype=torch.float64, device=f"cuda:{local}")
+    lo, hi = digest.clone(), digest.clone()
+    tmax = torch.tensor([min(times)], dtype=torch.float64, device=f"cuda:{local}")
+    if dist is not None:
+        dist.all_reduce(lo, op=dist.ReduceOp.MIN)
+        dist.all_reduce(hi, op=dist.ReduceOp.MAX)
+        dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
     if rank == 0:
         props = torch.cuda.get_device_properties(local)
-        gpu = {"name": props.name, "power_limit_w": _power_limit_w(local)}
-        for solver in solvers:
-            s_out, n_out, summary, info, solve_s, identical = results[solver]
-            err = (max(np.linalg.norm(compose(inverse(t), compose(inverse(s_out[0]), p))[:3]) for t, p in zip(truth, n_out))
-                   if truth is not None else None)
-            ar_ms = info.all_reduce_min_ms if info.all_reduce_min_ms > 0 else info.all_reduce_ms / max(info.all_reduce_count, 1)
-            line = {"what": ("dl_pose_graph_solve: SPA with ncclAllReduce(fp64) of the normal equations" if solver == "dense" else
-                             "dl_pose_graph_solve_sparse: SPA, Schur complement of the node blocks, ncclAllReduce(fp64) of the blocks"),
-                    "ranks": world, "shape": args.shape,
-                    "submaps": S, "nodes": N, "constraints": len(cons), "constraints_this_rank": len(mine),
-                    "local_parameters": info.num_local_parameters, "iterations": summary["num_iterations"],
-                    "evaluations": summary["num_evaluations"], "initial_cost": summary["initial_cost"],
-                    "final_cost": summary["final_cost"], "solve_s": solve_s,
-                    "all_reduce": {"count": info.all_reduce_count, "bytes_each": int(info.all_reduce_bytes), "ms_each": ar_ms,
-                                   "ms_mean": info.all_reduce_ms / max(info.all_reduce_count, 1),
-                                   "algbw_gbs": info.all_reduce_bytes / (ar_ms * 1e-3) / 1e9 if ar_ms > 0 else None,
-                                   "busbw_gbs": (info.all_reduce_bytes / (ar_ms * 1e-3) / 1e9 * 2 * (world - 1) / world) if ar_ms > 0 and world > 1 else None},
-                    "replicas_bit_identical": identical, "max_node_error_m": err, "gpu": gpu}
-            if solver == "sparse":
-                line.update(reduced_parameters=info.num_reduced_parameters, pairs=info.num_pairs,
-                            setup_exchange_bytes=int(info.setup_exchange_bytes))
-            if args.solver != "both":
-                print(json.dumps(line))
-        if args.solver == "both":
-            d, sp = results["dense"], results["sparse"]
-            diff = max(max(np.linalg.norm(a[:3] - b[:3]), np.linalg.norm(a[3:] - b[3:])) for a, b in
-                       zip(np.concatenate([d[0], d[1]]), np.concatenate([sp[0], sp[1]])))
-            print(json.dumps({"what": "dense vs block-sparse pose-graph solve, same graph", "ranks": world, "shape": args.shape,
-                              "submaps": S, "nodes": N, "constraints": len(cons), "dense_s": d[4], "sparse_s": sp[4],
-                              "speedup": d[4] / sp[4], "dense_iterations": d[2]["num_iterations"],
-                              "sparse_iterations": sp[2]["num_iterations"], "max_pose_difference": float(diff),
-                              "dense_all_reduce_bytes": int(d[3].all_reduce_bytes), "sparse_all_reduce_bytes": int(sp[3].all_reduce_bytes),
-                              "replicas_bit_identical": {"dense": d[5], "sparse": sp[5]}, "gpu": gpu}))
+        err = (max(np.linalg.norm(compose(inverse(t), compose(inverse(s_out[0]), p))[:3]) for t, p in zip(truth, n_out))
+               if truth is not None else None)
+        ar_ms = info.all_reduce_min_ms if info.all_reduce_min_ms > 0 else info.all_reduce_ms / max(info.all_reduce_count, 1)
+        print(json.dumps({"what": "dl_pose_graph_solve_sparse: SPA, Schur complement of the node blocks, ncclAllReduce(fp64) of the blocks",
+                          "ranks": world, "shape": args.shape,
+                          "submaps": S, "nodes": N, "constraints": len(cons), "constraints_this_rank": len(mine),
+                          "local_parameters": info.num_local_parameters, "iterations": summary["num_iterations"],
+                          "evaluations": summary["num_evaluations"], "initial_cost": summary["initial_cost"],
+                          "final_cost": summary["final_cost"], "solve_s": float(tmax[0]),
+                          "all_reduce": {"count": info.all_reduce_count, "bytes_each": int(info.all_reduce_bytes), "ms_each": ar_ms,
+                                         "ms_mean": info.all_reduce_ms / max(info.all_reduce_count, 1),
+                                         "algbw_gbs": info.all_reduce_bytes / (ar_ms * 1e-3) / 1e9 if ar_ms > 0 else None,
+                                         "busbw_gbs": (info.all_reduce_bytes / (ar_ms * 1e-3) / 1e9 * 2 * (world - 1) / world)
+                                         if ar_ms > 0 and world > 1 else None},
+                          "replicas_bit_identical": bool(torch.equal(lo, hi)), "max_node_error_m": err,
+                          "gpu": {"name": props.name, "power_limit_w": _power_limit_w(local)},
+                          "reduced_parameters": info.num_reduced_parameters, "pairs": info.num_pairs,
+                          "setup_exchange_bytes": int(info.setup_exchange_bytes)}))
     comm.close()
     if dist is not None:
         dist.destroy_process_group()
