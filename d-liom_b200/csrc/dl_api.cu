@@ -986,8 +986,7 @@ struct CoarseSearch {  // device state of one chunk of (node, submap) pairs
   FcsmPair* d_pairs;
   FcsmPick* d_picks;
   unsigned long long* d_best;
-  const float* d_hi;  // chunk-relative clouds
-  const float* d_lo;
+  std::vector<const float*> hi, lo;  // per pair of the chunk: its clouds on the device (uploaded or resident)
 };
 int check_fcsm_options(dl_context* ctx, const dl_fcsm_options& o) {
   if (o.branch_and_bound_depth < 1 || o.full_resolution_depth < 1)
@@ -1049,23 +1048,34 @@ int ensure_search_index(dl_context* ctx, dl_grid* g, bool* have) {
   return DL_OK;
 }
 
-// Uploads pairs [first, first + n) and runs the coarse search for them; leaves the picks on the device.
+// Runs the coarse search for pairs [first, first + n), uploading their clouds first unless they are device-resident; leaves the
+// picks on the device.
 int coarse_search(dl_context* ctx, Arena& a, const dl_fcsm_options& o, float min_score, int first, int n, const double* guesses,
-                  const float* hi_pts, const int64_t* hi_off, const float* lo_pts, const int64_t* lo_off,
-                  const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, float* d_all_scores, CoarseSearch* out) {
+                  const PairClouds& pc, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, float* d_all_scores,
+                  CoarseSearch* out) {
+  const int64_t* hi_off = pc.hi_off;
+  const int64_t* lo_off = pc.lo_off;
   const int64_t hi0 = hi_off[first], lo0 = lo_off[first];
   const int64_t n_hi = hi_off[first + n] - hi0, n_lo = lo_off[first + n] - lo0;
-  float* d_hi = a.take<float>(3 * n_hi);
-  float* d_lo = a.take<float>(3 * n_lo);
+  const bool resident = pc.hi_store != nullptr;
+  float* d_hi = resident ? nullptr : a.take<float>(3 * n_hi);
+  float* d_lo = resident ? nullptr : a.take<float>(3 * n_lo);
   int* d_cells = a.take<int>(3 * n_hi);
   float* d_rot = a.take<float>(3 * n_lo);
   out->d_pairs = a.take<FcsmPair>(n);
   out->d_picks = a.take<FcsmPick>(n);
   out->d_best = a.take<unsigned long long>(n);
-  out->d_hi = d_hi;
-  out->d_lo = d_lo;
-  DL_TRY(h2d(ctx, d_hi, hi_pts + 3 * hi0, 3 * n_hi));
-  DL_TRY(h2d(ctx, d_lo, lo_pts + 3 * lo0, 3 * n_lo));
+  out->hi.resize(n);
+  out->lo.resize(n);
+  for (int k = 0; k < n; ++k) {
+    const int g = first + k;
+    out->hi[k] = resident ? pc.hi_store + 3 * pc.hi_begin[g] : d_hi + 3 * (hi_off[g] - hi0);
+    out->lo[k] = resident ? pc.lo_store + 3 * pc.lo_begin[g] : d_lo + 3 * (lo_off[g] - lo0);
+  }
+  if (!resident) {
+    DL_TRY(h2d(ctx, d_hi, pc.hi_pts + 3 * hi0, 3 * n_hi));
+    DL_TRY(h2d(ctx, d_lo, pc.lo_pts + 3 * lo0, 3 * n_lo));
+  }
   std::vector<FcsmPair> pairs(n);
   int max_points = 1, max_blocks = 1;
   long long max_candidates = 1;
@@ -1082,8 +1092,8 @@ int coarse_search(dl_context* ctx, Arena& a, const dl_fcsm_options& o, float min
     std::memset(&p, 0, sizeof(p));
     p.hi = hi_grids[g]->view();
     p.lo = lo_grids[g]->view();
-    p.hi_pts = d_hi + 3 * (hi_off[g] - hi0);
-    p.lo_pts = d_lo + 3 * (lo_off[g] - lo0);
+    p.hi_pts = out->hi[k];
+    p.lo_pts = out->lo[k];
     p.cells = d_cells + 3 * (hi_off[g] - hi0);
     p.lo_rot = d_rot + 3 * (lo_off[g] - lo0);
     p.n_hi = (int)(hi_off[g + 1] - hi_off[g]);
@@ -1150,7 +1160,12 @@ int dl_fcsm_match_3dof(dl_context* ctx, const dl_fcsm_options* o, const double* 
   DL_TRY(ctx->reserve_device(coarse_bytes(n_hi, n_lo, 1)));
   Arena a(ctx->d_scratch);
   CoarseSearch cs;
-  DL_TRY(coarse_search(ctx, a, *o, min_score, 0, 1, guess, hi_pts, hi_off, lo_pts, lo_off, &hi, &lo, nullptr, &cs));
+  PairClouds pc;
+  pc.hi_pts = hi_pts;
+  pc.lo_pts = lo_pts;
+  pc.hi_off = hi_off;
+  pc.lo_off = lo_off;
+  DL_TRY(coarse_search(ctx, a, *o, min_score, 0, 1, guess, pc, &hi, &lo, nullptr, &cs));
   FcsmPick pick;
   DL_TRY(d2h(ctx, &pick, cs.d_picks, 1));
   DL_TRY(sync(ctx));
@@ -1252,8 +1267,12 @@ int dl_fcsm_match(dl_context* ctx, const dl_fcsm_options* o, const float* submap
     DL_TRY(ctx->reserve_device(coarse_bytes((int64_t)m * n_hi, (int64_t)m * n_lo, m)));
     Arena a(ctx->d_scratch);
     CoarseSearch cs;
-    DL_TRY(coarse_search(ctx, a, *o, min_score, first, m, guesses.data(), hi_all.data(), hi_off.data(), lo_all.data(), lo_off.data(),
-                         his.data(), los.data(), nullptr, &cs));
+    PairClouds pc;
+    pc.hi_pts = hi_all.data();
+    pc.lo_pts = lo_all.data();
+    pc.hi_off = hi_off.data();
+    pc.lo_off = lo_off.data();
+    DL_TRY(coarse_search(ctx, a, *o, min_score, first, m, guesses.data(), pc, his.data(), los.data(), nullptr, &cs));
     std::vector<FcsmPick> picks(m);
     DL_TRY(d2h(ctx, picks.data(), cs.d_picks, m));
     DL_TRY(sync(ctx));
@@ -1283,8 +1302,27 @@ int dl_constraint_search_batch(dl_context* ctx, const dl_constraint_options* opt
   if (count == 0) return DL_OK;
   if (!constraints) return DL_ERR_ARG;
   DL_TRY(check_pairs(ctx, count, guesses, hi_pts, hi_off, lo_pts, lo_off, hi_grids, lo_grids));
-  DL_TRY(check_fcsm_options(ctx, options->fast_correlative_scan_matcher_3d));
-  DL_TRY(check_ceres_options(ctx, &options->ceres_scan_matcher_3d, 2));
+  DL_TRY(check_constraint_options(ctx, *options));
+  PairClouds pc;
+  pc.hi_pts = hi_pts;
+  pc.lo_pts = lo_pts;
+  pc.hi_off = hi_off;
+  pc.lo_off = lo_off;
+  return constraint_search(ctx, *options, count, guesses, pc, hi_grids, lo_grids, constraints);
+}
+
+}  // extern "C"
+
+namespace dl {
+int check_constraint_options(dl_context* ctx, const dl_constraint_options& o) {
+  DL_TRY(check_fcsm_options(ctx, o.fast_correlative_scan_matcher_3d));
+  return check_ceres_options(ctx, &o.ceres_scan_matcher_3d, 2);
+}
+int constraint_search(dl_context* ctx, const dl_constraint_options& o, int count, const double* guesses, const PairClouds& pc,
+                      const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, dl_constraint* constraints) {
+  const dl_constraint_options* options = &o;
+  const int64_t* hi_off = pc.hi_off;
+  const int64_t* lo_off = pc.lo_off;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const NlsOptions nls = to_nls_options(options->ceres_scan_matcher_3d, 2);
   constexpr int kChunk = 1024;  // pairs per launch set: bounds the scratch, keeps every grid dimension legal
@@ -1294,16 +1332,16 @@ int dl_constraint_search_batch(dl_context* ctx, const dl_constraint_options* opt
     DL_TRY(ctx->reserve_device(coarse_bytes(n_hi, n_lo, n) + arena_bytes({(size_t)n * sizeof(NlsProblem), (size_t)n * sizeof(NlsOutput)})));
     Arena a(ctx->d_scratch);
     CoarseSearch cs;
-    DL_TRY(coarse_search(ctx, a, options->fast_correlative_scan_matcher_3d, (float)options->min_score, first, n, guesses, hi_pts,
-                         hi_off, lo_pts, lo_off, hi_grids, lo_grids, nullptr, &cs));
+    DL_TRY(coarse_search(ctx, a, options->fast_correlative_scan_matcher_3d, (float)options->min_score, first, n, guesses, pc,
+                         hi_grids, lo_grids, nullptr, &cs));
     // refinement: initial pose = translation target = the coarse pose, read from the pick record on the device
     std::vector<NlsProblem> problems(n);
     for (int k = 0; k < n; ++k) {
       const int g = first + k;
       NlsProblem& p = problems[k];
       std::memset(&p, 0, sizeof(p));
-      p.cloud[0] = cs.d_hi + 3 * (hi_off[g] - hi_off[first]);
-      p.cloud[1] = cs.d_lo + 3 * (lo_off[g] - lo_off[first]);
+      p.cloud[0] = cs.hi[k];
+      p.cloud[1] = cs.lo[k];
       p.count[0] = (int32_t)(hi_off[g + 1] - hi_off[g]);
       p.count[1] = (int32_t)(lo_off[g + 1] - lo_off[g]);
       p.grid[0] = hi_grids[g]->view();
@@ -1341,8 +1379,7 @@ int dl_constraint_search_batch(dl_context* ctx, const dl_constraint_options* opt
   }
   return DL_OK;
 }
-
-}  // extern "C"
+}  // namespace dl
 
 extern "C" {
 
@@ -1355,8 +1392,7 @@ int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_const
   if (capacity > 1024) return ctx->fail(DL_ERR_ARG, "capacity > 1024 pairs per rank and exchange: split the call");
   if (count > 0 && (!submap_ids || !node_ids)) return DL_ERR_ARG;
   if (count > 0) DL_TRY(check_pairs(ctx, count, guesses, hi_pts, hi_off, lo_pts, lo_off, hi_grids, lo_grids));
-  DL_TRY(check_fcsm_options(ctx, options->fast_correlative_scan_matcher_3d));
-  DL_TRY(check_ceres_options(ctx, &options->ceres_scan_matcher_3d, 2));
+  DL_TRY(check_constraint_options(ctx, *options));
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const int world = dl_comm_world_size(comm), rank = dl_comm_rank(comm);
   const size_t row_bytes = sizeof(dl_constraint_row), block = (size_t)capacity * row_bytes;
@@ -1373,14 +1409,19 @@ int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_const
                                arena_bytes({(size_t)n * sizeof(NlsProblem), (size_t)n * sizeof(NlsOutput), (size_t)n * 8})));
     Arena a(ctx->d_scratch);
     CoarseSearch cs;
-    DL_TRY(coarse_search(ctx, a, options->fast_correlative_scan_matcher_3d, (float)options->min_score, 0, n, guesses, hi_pts,
-                         hi_off, lo_pts, lo_off, hi_grids, lo_grids, nullptr, &cs));
+    PairClouds pc;
+    pc.hi_pts = hi_pts;
+    pc.lo_pts = lo_pts;
+    pc.hi_off = hi_off;
+    pc.lo_off = lo_off;
+    DL_TRY(coarse_search(ctx, a, options->fast_correlative_scan_matcher_3d, (float)options->min_score, 0, n, guesses, pc,
+                         hi_grids, lo_grids, nullptr, &cs));
     std::vector<NlsProblem> problems(n);
     for (int k = 0; k < n; ++k) {
       NlsProblem& p = problems[k];
       std::memset(&p, 0, sizeof(p));
-      p.cloud[0] = cs.d_hi + 3 * (hi_off[k] - hi_off[0]);
-      p.cloud[1] = cs.d_lo + 3 * (lo_off[k] - lo_off[0]);
+      p.cloud[0] = cs.hi[k];
+      p.cloud[1] = cs.lo[k];
       p.count[0] = (int32_t)(hi_off[k + 1] - hi_off[k]);
       p.count[1] = (int32_t)(lo_off[k + 1] - lo_off[k]);
       p.grid[0] = hi_grids[k]->view();

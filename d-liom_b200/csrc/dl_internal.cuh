@@ -341,6 +341,27 @@ int comm_all_gather(dl_comm* c, const void* send_dev, void* recv_dev, size_t byt
 int launch_pack_constraint_rows(dl_context* ctx, int n, const FcsmPick* picks, const NlsOutput* refined, const int32_t* submap_ids,
                                 const int32_t* node_ids, double translation_weight, double rotation_weight, int rank,
                                 dl_constraint_row* rows);
+// The clouds of a batch of (node, submap) loop-closure searches. Pair k has hi_off[k+1] - hi_off[k] high-resolution points
+// (likewise low). Host batch (hi_store == nullptr): they are rows [off[k], off[k+1]) of the host arrays hi_pts / lo_pts and the
+// search uploads them. Device-resident (hi_store / lo_store set, dl_posegraph3d.cu's node store): they already sit on the
+// device at hi_store + 3 * hi_begin[k] (lo likewise); nothing is uploaded and the host arrays are not read.
+struct PairClouds {
+  const float* hi_pts = nullptr;
+  const float* lo_pts = nullptr;
+  const int64_t* hi_off = nullptr;
+  const int64_t* lo_off = nullptr;
+  const float* hi_store = nullptr;
+  const float* lo_store = nullptr;
+  const int64_t* hi_begin = nullptr;
+  const int64_t* lo_begin = nullptr;
+};
+// dl_api.cu: the option checks of dl_constraint_search_batch (fast correlative matcher, and the refine's two-weight Ceres
+// options), shared by every entry point that searches.
+int check_constraint_options(dl_context* ctx, const dl_constraint_options& options);
+// dl_api.cu: dl_constraint_search_batch's body (coarse search, min_score prune, refine) for `count` pairs in chunks of 1024.
+int constraint_search(dl_context* ctx, const dl_constraint_options& options, int count, const double* guesses,
+                      const PairClouds& clouds, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids,
+                      dl_constraint* constraints);
 int launch_interpolate(dl_context* ctx, const GridView& grid, int64_t n, const double* xyz, double* out);
 int launch_grid_lookup(dl_context* ctx, const GridView& grid, int64_t n, const int32_t* xyz, uint16_t* out);
 

@@ -1,0 +1,529 @@
+// mapping::PoseGraph3D on the fork's live loop-closure path (C/mapping/internal/3d/pose_graph_3d.cc,
+// C/mapping/internal/constraints/constraint_builder_3d.cc:162-333): id bookkeeping, InitializeGlobalSubmapPoses, INTRA_SUBMAP
+// constraints, the fan-out of the host's submap matches into (node, submap) searches, the optimization trigger and
+// RunOptimization's update. The graph bookkeeping is host code (a few hundred bytes per node); the node clouds live in a device
+// node store, uploaded once per node, and every search reads them there through dl::constraint_search — the kernels of
+// dl_constraint_search_batch. The optimization calls dl_pose_graph_solve_sparse on the graph's poses: that call is the block-sparse
+// solve's one host entry (it takes host poses, sets up the CSR lists and runs the LM state machine on the host), and the poses
+// it moves are 56 bytes per submap or node, so there is no second copy of its set-up here. See include/dliom_b200.h.
+#include <algorithm>
+#include <chrono>
+#include <cmath>
+#include <cstring>
+#include <map>
+#include <set>
+#include <utility>
+#include <vector>
+
+#include "dl_internal.cuh"
+
+using namespace dl;
+
+namespace {
+
+struct Submap {
+  const dl_grid* hi = nullptr;
+  const dl_grid* lo = nullptr;
+  Rigidd local;
+  bool finished = false;
+  std::vector<int32_t> node_ids;  // InternalSubmapData::node_ids: nodes of this trajectory inserted into it, in id order
+  Rigidd global;                  // optimization_problem_->submap_data()
+  bool optimized = false;         // present in global_submap_poses_ (the result of the last RunOptimization) ...
+  Rigidd optimized_global;        // ... with this pose
+};
+struct Node {
+  double time = 0.0;
+  Rigidd local;
+  Rigidd global;          // trajectory_nodes_' global_pose
+  Rigidd problem_global;  // optimization_problem_->node_data()
+  int64_t hi_begin = 0, n_hi = 0, lo_begin = 0, n_lo = 0;  // points in the node store
+};
+struct Trajectory {
+  std::vector<Submap> submaps;
+  std::vector<Node> nodes;
+};
+using Id = std::pair<int32_t, int32_t>;  // (trajectory_id, index)
+
+double ms_since(std::chrono::steady_clock::time_point t0) {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+Rigidd identity() { return {{0.0, 0.0, 0.0}, {1.0, 0.0, 0.0, 0.0}}; }
+Rigidd rotation_only(const Quatd& q) { return {{0.0, 0.0, 0.0}, q}; }
+// Eigen::AngleAxis(angle, UnitZ) as a quaternion
+Quatd yaw_quaternion(double angle) { return {std::cos(0.5 * angle), 0.0, 0.0, std::sin(0.5 * angle)}; }
+// transform::GetYaw: atan2 of the rotated x axis
+double get_yaw(const Quatd& q) {
+  const Vec3d d = rotate(q, Vec3d{1.0, 0.0, 0.0});
+  return std::atan2(d.y, d.x);
+}
+// The rotation-only gravity alignment of a submap pose with its yaw removed (constraint_builder_3d.cc:241-251):
+// Embed3D(Rigid2d::Rotation(-yaw)) * Rigid3d::Rotation(rotation).
+Rigidd yaw_free_alignment(const Rigidd& submap_pose) {
+  const Rigidd aligned = rotation_only(submap_pose.q);
+  return compose(rotation_only(yaw_quaternion(-get_yaw(aligned.q))), aligned);
+}
+
+}  // namespace
+
+struct dl_pose_graph_3d {
+  dl_context* ctx = nullptr;
+  dl_pose_graph_3d_options options{};
+  std::map<int32_t, Trajectory> trajectories;
+  std::set<int32_t> frozen;
+  std::vector<dl_pg3d_constraint> constraints;           // constraints_
+  std::vector<dl_pg3d_constraint> pending;               // found by the searches, not yet handed to the optimization
+  std::map<Id, std::set<Id>> computed;                   // ConstraintBuilder3D::computed_constraints_: submap -> nodes
+  int32_t num_nodes_since_last_loop_closure = 0;
+  std::vector<dl_pg3d_search> last_searches;             // of the last add_node call
+  float* d_store = nullptr;                             // node store: xyz floats, each node's high- then low-resolution cloud
+  int64_t store_capacity = 0, store_used = 0;            // in floats
+  int64_t bytes_uploaded = 0;
+
+  // ComputeLocalToGlobalTransform (:914-935) over global_submap_poses_ (optimized) or submap_data (the problem's poses)
+  Rigidd local_to_global(int32_t trajectory_id, bool optimized) const {
+    const auto it = trajectories.find(trajectory_id);
+    if (it == trajectories.end()) return identity();
+    const std::vector<Submap>& s = it->second.submaps;
+    for (int i = (int)s.size() - 1; i >= 0; --i)
+      if (!optimized || s[i].optimized) return compose(optimized ? s[i].optimized_global : s[i].global, inverse(s[i].local));
+    return identity();
+  }
+  int reserve_store(int64_t floats) {
+    if (store_used + floats <= store_capacity) return DL_OK;
+    const int64_t cap = std::max<int64_t>({store_used + floats, 2 * store_capacity, (int64_t)1 << 20});
+    float* fresh = nullptr;
+    DL_CUDA(ctx, cudaSetDevice(ctx->device));
+    DL_CUDA(ctx, cudaMalloc(&fresh, (size_t)cap * sizeof(float)));
+    if (store_used > 0) {
+      cudaError_t e = cudaMemcpyAsync(fresh, d_store, (size_t)store_used * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream);
+      if (e == cudaSuccess) e = ctx->wait_stream();
+      if (e != cudaSuccess) {
+        cudaFree(fresh);
+        return ctx->cuda_fail(e, "node store growth");
+      }
+    }
+    if (d_store) cudaFree(d_store);
+    d_store = fresh;
+    store_capacity = cap;
+    return DL_OK;
+  }
+  int optimize(dl_solve_summary* summary);
+};
+
+namespace {
+
+struct Pair {  // one (node, submap) search of the fan-out
+  Id submap, node;
+  double guess[7];
+  int64_t hi_begin, n_hi, lo_begin, n_lo;
+};
+
+int check_options(dl_context* ctx, const dl_pose_graph_3d_options& o) {
+  if (o.optimize_every_n_nodes < 0) return ctx->fail(DL_ERR_ARG, "optimize_every_n_nodes must be >= 0");
+  if (o.every_nodes_to_find_constraint < 1) return ctx->fail(DL_ERR_ARG, "every_nodes_to_find_constraint must be >= 1");
+  if (o.optimization_problem.max_num_iterations < 0) return ctx->fail(DL_ERR_ARG, "max_num_iterations must be >= 0");
+  return check_constraint_options(ctx, o.constraint_builder);  // the checks of dl_constraint_search_batch
+}
+
+}  // namespace
+
+// HandleWorkQueue (:444-470) + RunOptimization (:718-770)
+int dl_pose_graph_3d::optimize(dl_solve_summary* summary) {
+  const size_t table_size = constraints.size();  // a failed solve puts the pending constraints back
+  for (const dl_pg3d_constraint& c : pending) {
+    bool has_added = false;
+    for (const dl_pg3d_constraint& t : constraints)
+      if (t.submap_trajectory_id == c.submap_trajectory_id && t.submap_index == c.submap_index &&
+          t.node_trajectory_id == c.node_trajectory_id && t.node_index == c.node_index) {
+        has_added = true;
+        break;
+      }
+    if (!has_added) constraints.push_back(c);
+  }
+  if (summary) std::memset(summary, 0, sizeof(*summary));
+  // poses: submaps then nodes, each in (trajectory, index) order
+  std::map<int32_t, int32_t> submap_base, node_base;
+  int32_t S = 0, N = 0;
+  for (const auto& [id, t] : trajectories) {
+    submap_base[id] = S;
+    node_base[id] = N;
+    S += (int32_t)t.submaps.size();
+    N += (int32_t)t.nodes.size();
+  }
+  if (S == 0) {  // RunOptimization: nothing to optimize
+    pending.clear();
+    return DL_OK;
+  }
+  std::vector<double> poses(7 * (size_t)(S + N));
+  std::vector<uint8_t> frozen_mask(S + N, 0);
+  for (const auto& [id, t] : trajectories) {
+    const uint8_t f = frozen.count(id) ? 1 : 0;
+    for (size_t i = 0; i < t.submaps.size(); ++i) {
+      pose_to7(t.submaps[i].global, &poses[7 * (submap_base[id] + i)]);
+      frozen_mask[submap_base[id] + i] = f;
+    }
+    for (size_t i = 0; i < t.nodes.size(); ++i) {
+      pose_to7(t.nodes[i].problem_global, &poses[7 * (S + node_base[id] + i)]);
+      frozen_mask[S + node_base[id] + i] = f;
+    }
+  }
+  std::vector<dl_spa_constraint> spa(constraints.size());
+  for (size_t k = 0; k < constraints.size(); ++k) {
+    const dl_pg3d_constraint& c = constraints[k];
+    dl_spa_constraint& s = spa[k];
+    s.submap = submap_base[c.submap_trajectory_id] + c.submap_index;
+    s.node = node_base[c.node_trajectory_id] + c.node_index;
+    std::memcpy(s.zbar, c.zbar, sizeof(s.zbar));
+    s.translation_weight = c.translation_weight;
+    s.rotation_weight = c.rotation_weight;
+  }
+  dl_solve_summary local{};
+  const int st = dl_pose_graph_solve_sparse(ctx, nullptr, &options.optimization_problem, S, N, poses.data(), frozen_mask.data(),
+                                            spa.data(), (int32_t)spa.size(), &local, nullptr);
+  if (st != DL_OK) {
+    constraints.resize(table_size);
+    return st;
+  }
+  pending.clear();
+  if (summary) *summary = local;
+  for (auto& [id, t] : trajectories) {
+    for (size_t i = 0; i < t.submaps.size(); ++i) t.submaps[i].global = pose_from7(&poses[7 * (submap_base[id] + i)]);
+    for (size_t i = 0; i < t.nodes.size(); ++i) {
+      t.nodes[i].problem_global = pose_from7(&poses[7 * (S + node_base[id] + i)]);
+      // every node is in node_data here (the calls are synchronous), so RunOptimization's extrapolation of the nodes added
+      // after the solve started (:748-762) has nothing to move
+      t.nodes[i].global = t.nodes[i].problem_global;
+    }
+  }
+  for (auto& [id, t] : trajectories)  // global_submap_poses_ = submap_data
+    for (Submap& s : t.submaps) {
+      s.optimized = true;
+      s.optimized_global = s.global;
+    }
+  num_nodes_since_last_loop_closure = 0;
+  return DL_OK;
+}
+
+extern "C" {
+
+int dl_pose_graph_3d_create(dl_context* ctx, const dl_pose_graph_3d_options* options, dl_pose_graph_3d** out) {
+  if (!ctx || !options || !out) return DL_ERR_ARG;
+  *out = nullptr;
+  DL_TRY_STATUS(check_options(ctx, *options));
+  dl_pose_graph_3d* g = new dl_pose_graph_3d;
+  g->ctx = ctx;
+  g->options = *options;
+  *out = g;
+  return DL_OK;
+}
+
+void dl_pose_graph_3d_destroy(dl_pose_graph_3d* g) {
+  if (!g) return;
+  if (g->d_store) {
+    cudaSetDevice(g->ctx->device);
+    cudaStreamSynchronize(g->ctx->stream);
+    cudaFree(g->d_store);
+  }
+  delete g;
+}
+
+int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int32_t num_matches,
+                              const dl_pg3d_submap_match* matches, dl_pg3d_add_node_info* info) {
+  if (!g || !node || num_matches < 0 || (num_matches > 0 && !matches)) return DL_ERR_ARG;
+  dl_context* ctx = g->ctx;
+  const auto t0 = std::chrono::steady_clock::now();
+  const int m = node->num_insertion_submaps;
+  if (m != 1 && m != 2) return ctx->fail(DL_ERR_ARG, "a node has one or two insertion submaps");
+  if (node->num_high_resolution < 1 || node->num_low_resolution < 1 || !node->high_resolution_points || !node->low_resolution_points)
+    return ctx->fail(DL_ERR_EMPTY, "a node needs non-empty high- and low-resolution clouds");
+  if (node->num_high_resolution > INT32_MAX || node->num_low_resolution > INT32_MAX) return ctx->fail(DL_ERR_ARG, "cloud too large");
+  const dl_pg3d_insertion_submap* ins = node->insertion_submaps;
+  for (int i = 0; i < m; ++i)
+    if (!ins[i].high_resolution_grid || !ins[i].low_resolution_grid) return ctx->fail(DL_ERR_ARG, "insertion submap without grids");
+  const int32_t tid = node->trajectory_id;
+  if (tid < 0) return ctx->fail(DL_ERR_ARG, "negative trajectory id");
+  const auto tit = g->trajectories.find(tid);
+  const int32_t S = tit == g->trajectories.end() ? 0 : (int32_t)tit->second.submaps.size();
+  // AddNode's "is insertion_submaps.back() new" and InitializeGlobalSubmapPoses' CHECKs, as index rules
+  bool back_is_new;
+  if (m == 1) {
+    if (ins[0].submap_index != 0 || S > 1) return ctx->fail(DL_ERR_ARG, "one insertion submap: it must be the trajectory's submap 0");
+    back_is_new = S == 0;
+  } else {
+    const int32_t a = ins[0].submap_index, b = ins[1].submap_index;
+    if (S >= 1 && a == S - 1 && b == S) back_is_new = true;
+    else if (S >= 2 && a == S - 2 && b == S - 1) back_is_new = false;
+    else return ctx->fail(DL_ERR_ARG, "insertion submaps do not continue the trajectory's submap sequence");
+  }
+  if (tit != g->trajectories.end())
+    for (int i = 0; i < m; ++i)
+      if (ins[i].submap_index < S && tit->second.submaps[ins[i].submap_index].finished)
+        return ctx->fail(DL_ERR_ARG, "insertion submap is already finished");
+  const bool newly_finished = ins[0].finished != 0;
+  if (!newly_finished && num_matches > 0) return ctx->fail(DL_ERR_ARG, "submap matches passed but no insertion submap finished");
+  const Id front_id{tid, ins[0].submap_index};
+  std::vector<dl_pg3d_submap_match> sorted(matches, matches + num_matches);
+  std::sort(sorted.begin(), sorted.end(), [](const dl_pg3d_submap_match& x, const dl_pg3d_submap_match& y) {
+    return Id{x.trajectory_id, x.submap_index} < Id{y.trajectory_id, y.submap_index};
+  });
+  for (size_t k = 0; k < sorted.size(); ++k) {
+    const Id to{sorted[k].trajectory_id, sorted[k].submap_index};
+    if (to == front_id) return ctx->fail(DL_ERR_ARG, "a match names the finished submap itself");
+    if (to.first == tid && std::abs(to.second - front_id.second) <= 2)
+      return ctx->fail(DL_ERR_ARG, "a match names a same-trajectory submap within two indices");
+    const auto it = g->trajectories.find(to.first);
+    if (it == g->trajectories.end() || to.second < 0 || to.second >= (int32_t)it->second.submaps.size())
+      return ctx->fail(DL_ERR_ARG, "a match names an unknown submap");
+    if (!it->second.submaps[to.second].finished) return ctx->fail(DL_ERR_ARG, "a match names an unfinished submap");
+    if (k > 0 && to == Id{sorted[k - 1].trajectory_id, sorted[k - 1].submap_index})
+      return ctx->fail(DL_ERR_ARG, "a submap is matched twice");
+  }
+
+  // ---- 2. the node's clouds into the node store (store_used moves on only at the commit below)
+  const int64_t n_hi = node->num_high_resolution, n_lo = node->num_low_resolution;
+  DL_TRY_STATUS(g->reserve_store(3 * (n_hi + n_lo)));
+  const int64_t hi_begin = g->store_used / 3, lo_begin = hi_begin + n_hi;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  DL_CUDA(ctx, cudaMemcpyAsync(g->d_store + 3 * hi_begin, node->high_resolution_points, (size_t)n_hi * 12, cudaMemcpyHostToDevice,
+                               ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(g->d_store + 3 * lo_begin, node->low_resolution_points, (size_t)n_lo * 12, cudaMemcpyHostToDevice,
+                               ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());  // pageable host memory
+  const int64_t uploaded = 12 * (n_hi + n_lo);
+
+  // ---- 4. fan-out and searches of a newly finished submap, before anything is committed
+  const Rigidd local_pose = pose_from7(node->local_pose);
+  const int32_t node_index = tit == g->trajectories.end() ? 0 : (int32_t)tit->second.nodes.size();
+  std::vector<Pair> pairs;
+  std::vector<dl_constraint> results;
+  double search_ms = 0.0;
+  if (newly_finished && !sorted.empty()) {
+    const Trajectory* tr = tit == g->trajectories.end() ? nullptr : &tit->second;
+    const Rigidd local_from = pose_from7(ins[0].local_pose);  // a finished submap was seen before: the same pose
+    const Rigidd from_local = tr && front_id.second < S ? tr->submaps[front_id.second].local : local_from;
+    std::vector<int32_t> nodes_in_submap = tr && front_id.second < S ? tr->submaps[front_id.second].node_ids : std::vector<int32_t>();
+    nodes_in_submap.push_back(node_index);  // this node was just inserted into it
+    const Rigidd T_S2_G2 = yaw_free_alignment(from_local);
+    const Rigidd from_local_inv = inverse(from_local);
+    for (const dl_pg3d_submap_match& mt : sorted) {
+      const Id to{mt.trajectory_id, mt.submap_index};
+      const Submap& target = g->trajectories.at(to.first).submaps[to.second];
+      const Rigidd T_G1_S1 = inverse(yaw_free_alignment(target.local));
+      const Rigidd submap_to_submap_2d{{mt.x, mt.y, 0.0}, yaw_quaternion(mt.theta)};  // Embed3D(Rigid2d)
+      const Rigidd left = compose(compose(T_G1_S1, submap_to_submap_2d), T_S2_G2);
+      const auto done = g->computed.find(to);
+      int j = 0;
+      for (const int32_t n : nodes_in_submap) {
+        if (j++ % g->options.every_nodes_to_find_constraint != 0) continue;
+        if (done != g->computed.end() && done->second.count(Id{tid, n})) continue;
+        const bool is_new = n == node_index;
+        const Node* nd = is_new ? nullptr : &tr->nodes[n];
+        Pair p;
+        p.submap = to;
+        p.node = Id{tid, n};
+        pose_to7(compose(left, compose(from_local_inv, is_new ? local_pose : nd->local)), p.guess);
+        p.hi_begin = is_new ? hi_begin : nd->hi_begin;
+        p.n_hi = is_new ? n_hi : nd->n_hi;
+        p.lo_begin = is_new ? lo_begin : nd->lo_begin;
+        p.n_lo = is_new ? n_lo : nd->n_lo;
+        pairs.push_back(p);
+      }
+    }
+    if (!pairs.empty()) {
+      const auto ts = std::chrono::steady_clock::now();
+      const int n = (int)pairs.size();
+      std::vector<double> guesses(7 * (size_t)n);
+      std::vector<int64_t> hi_off(n + 1, 0), lo_off(n + 1, 0), hib(n), lob(n);
+      std::vector<const dl_grid*> hg(n), lg(n);
+      for (int k = 0; k < n; ++k) {
+        const Pair& p = pairs[k];
+        std::memcpy(&guesses[7 * (size_t)k], p.guess, sizeof(p.guess));
+        hi_off[k + 1] = hi_off[k] + p.n_hi;
+        lo_off[k + 1] = lo_off[k] + p.n_lo;
+        hib[k] = p.hi_begin;
+        lob[k] = p.lo_begin;
+        const Submap& target = g->trajectories.at(p.submap.first).submaps[p.submap.second];
+        if (target.hi->structure_dirty || target.lo->structure_dirty)
+          return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+        hg[k] = target.hi;
+        lg[k] = target.lo;
+      }
+      PairClouds pc;
+      pc.hi_off = hi_off.data();
+      pc.lo_off = lo_off.data();
+      pc.hi_store = g->d_store;
+      pc.lo_store = g->d_store;
+      pc.hi_begin = hib.data();
+      pc.lo_begin = lob.data();
+      results.resize(n);
+      DL_TRY_STATUS(constraint_search(ctx, g->options.constraint_builder, n, guesses.data(), pc, hg.data(), lg.data(), results.data()));
+      search_ms = ms_since(ts);
+    }
+  }
+
+  // ---- commit: 1. AddNode, 3. ComputeConstraintsForNode, 4. the searches' results
+  Trajectory& t = g->trajectories[tid];
+  g->store_used += 3 * (n_hi + n_lo);
+  g->bytes_uploaded += uploaded;
+  Node nd;
+  nd.time = node->time;
+  nd.local = local_pose;
+  nd.global = compose(g->local_to_global(tid, true), local_pose);  // GetLocalToGlobalTransform * local_pose (:115-116)
+  nd.hi_begin = hi_begin;
+  nd.n_hi = n_hi;
+  nd.lo_begin = lo_begin;
+  nd.n_lo = n_lo;
+  if (back_is_new) {
+    Submap s;
+    s.hi = ins[m - 1].high_resolution_grid;
+    s.lo = ins[m - 1].low_resolution_grid;
+    s.local = pose_from7(ins[m - 1].local_pose);
+    // InitializeGlobalSubmapPoses (:67-110)
+    if (m == 1) s.global = compose(g->local_to_global(tid, true), s.local);
+    else s.global = compose(compose(t.submaps[ins[0].submap_index].global, inverse(t.submaps[ins[0].submap_index].local)), s.local);
+    t.submaps.push_back(s);
+  }
+  const Submap& matching = t.submaps[ins[0].submap_index];
+  nd.problem_global = compose(compose(matching.global, inverse(matching.local)), local_pose);  // :345-347
+  t.nodes.push_back(nd);
+  for (int i = 0; i < m; ++i) {
+    Submap& s = t.submaps[ins[i].submap_index];
+    s.node_ids.push_back(node_index);
+    dl_pg3d_constraint c{};
+    c.submap_trajectory_id = tid;
+    c.submap_index = ins[i].submap_index;
+    c.node_trajectory_id = tid;
+    c.node_index = node_index;
+    pose_to7(compose(inverse(s.local), local_pose), c.zbar);  // :358-359
+    c.translation_weight = g->options.matcher_translation_weight;
+    c.rotation_weight = g->options.matcher_rotation_weight;
+    c.tag = DL_PG3D_INTRA_SUBMAP;
+    g->constraints.push_back(c);
+  }
+  int32_t found = 0;
+  g->last_searches.assign(pairs.size(), dl_pg3d_search{});
+  for (size_t k = 0; k < pairs.size(); ++k) {
+    dl_pg3d_search& s = g->last_searches[k];
+    s.submap_trajectory_id = pairs[k].submap.first;
+    s.submap_index = pairs[k].submap.second;
+    s.node_trajectory_id = pairs[k].node.first;
+    s.node_index = pairs[k].node.second;
+    std::memcpy(s.pose_guess, pairs[k].guess, sizeof(s.pose_guess));
+    s.result = results[k];
+  }
+  if (newly_finished) {
+    t.submaps[ins[0].submap_index].finished = true;
+    for (size_t k = 0; k < pairs.size(); ++k) {
+      if (!results[k].found) continue;
+      ++found;
+      g->computed[pairs[k].submap].insert(pairs[k].node);  // constraint_builder_3d.cc:334
+      dl_pg3d_constraint c{};
+      c.submap_trajectory_id = pairs[k].submap.first;
+      c.submap_index = pairs[k].submap.second;
+      c.node_trajectory_id = pairs[k].node.first;
+      c.node_index = pairs[k].node.second;
+      std::memcpy(c.zbar, results[k].pose, sizeof(c.zbar));
+      c.translation_weight = results[k].translation_weight;
+      c.rotation_weight = results[k].rotation_weight;
+      c.tag = DL_PG3D_INTER_SUBMAP;
+      g->pending.push_back(c);
+    }
+  }
+  const double bookkeeping_ms = ms_since(t0) - search_ms;
+
+  // ---- 5. the optimization trigger (:393-398)
+  ++g->num_nodes_since_last_loop_closure;
+  dl_solve_summary summary{};
+  int32_t optimized = 0;
+  double solve_ms = 0.0;
+  if (g->options.optimize_every_n_nodes > 0 && g->num_nodes_since_last_loop_closure > g->options.optimize_every_n_nodes) {
+    const auto ts = std::chrono::steady_clock::now();
+    DL_TRY_STATUS(g->optimize(&summary));
+    solve_ms = ms_since(ts);
+    optimized = 1;
+  }
+  if (info) {
+    std::memset(info, 0, sizeof(*info));
+    info->node_index = node_index;
+    info->num_searched = (int32_t)pairs.size();
+    info->num_found = found;
+    info->optimized = optimized;
+    info->cloud_bytes_uploaded = uploaded;
+    info->bookkeeping_ms = bookkeeping_ms;
+    info->search_ms = search_ms;
+    info->solve_ms = solve_ms;
+    info->summary = summary;
+  }
+  return DL_OK;
+}
+
+int dl_pose_graph_3d_freeze_trajectory(dl_pose_graph_3d* g, int32_t trajectory_id) {
+  if (!g || trajectory_id < 0) return DL_ERR_ARG;
+  g->frozen.insert(trajectory_id);
+  return DL_OK;
+}
+
+int dl_pose_graph_3d_run_final_optimization(dl_pose_graph_3d* g, dl_solve_summary* summary) {
+  if (!g) return DL_ERR_ARG;
+  // max_num_final_iterations is set and then overwritten with the regular cap (pose_graph_3d.cc:677-682): the same solve
+  return g->optimize(summary);
+}
+
+int dl_pose_graph_3d_poses(const dl_pose_graph_3d* g, int32_t trajectory_id, int32_t which, int32_t capacity, double* poses,
+                           int32_t* count) {
+  if (!g || !count || which < DL_PG3D_NODE_POSES || which > DL_PG3D_OPTIMIZATION_SUBMAPS || capacity < 0) return DL_ERR_ARG;
+  const auto it = g->trajectories.find(trajectory_id);
+  const bool nodes = which == DL_PG3D_NODE_POSES || which == DL_PG3D_OPTIMIZATION_NODES;
+  const int32_t n = it == g->trajectories.end() ? 0 : (int32_t)(nodes ? it->second.nodes.size() : it->second.submaps.size());
+  *count = n;
+  if (!poses) return DL_OK;
+  if (capacity < n) return g->ctx->fail(DL_ERR_ARG, "capacity smaller than the trajectory");
+  const Rigidd extrapolate = g->local_to_global(trajectory_id, true);
+  for (int32_t i = 0; i < n; ++i) {
+    Rigidd p;
+    if (which == DL_PG3D_NODE_POSES) p = it->second.nodes[i].global;
+    else if (which == DL_PG3D_OPTIMIZATION_NODES) p = it->second.nodes[i].problem_global;
+    else if (which == DL_PG3D_OPTIMIZATION_SUBMAPS) p = it->second.submaps[i].global;
+    else {
+      const Submap& s = it->second.submaps[i];
+      p = s.optimized ? s.optimized_global : compose(extrapolate, s.local);
+    }
+    pose_to7(p, poses + 7 * (size_t)i);
+  }
+  return DL_OK;
+}
+
+int dl_pose_graph_3d_local_to_global(const dl_pose_graph_3d* g, int32_t trajectory_id, double* pose) {
+  if (!g || !pose) return DL_ERR_ARG;
+  pose_to7(g->local_to_global(trajectory_id, true), pose);
+  return DL_OK;
+}
+
+int dl_pose_graph_3d_constraints(const dl_pose_graph_3d* g, int32_t capacity, dl_pg3d_constraint* out, int32_t* count) {
+  if (!g || !count || capacity < 0) return DL_ERR_ARG;
+  const int32_t n = (int32_t)g->constraints.size();
+  *count = n;
+  if (!out) return DL_OK;
+  if (capacity < n) return g->ctx->fail(DL_ERR_ARG, "capacity smaller than the constraint table");
+  std::copy(g->constraints.begin(), g->constraints.end(), out);
+  return DL_OK;
+}
+
+int dl_pose_graph_3d_last_searches(const dl_pose_graph_3d* g, int32_t capacity, dl_pg3d_search* out, int32_t* count) {
+  if (!g || !count || capacity < 0) return DL_ERR_ARG;
+  const int32_t n = (int32_t)g->last_searches.size();
+  *count = n;
+  if (!out) return DL_OK;
+  if (capacity < n) return g->ctx->fail(DL_ERR_ARG, "capacity smaller than the search list");
+  std::copy(g->last_searches.begin(), g->last_searches.end(), out);
+  return DL_OK;
+}
+
+int dl_pose_graph_3d_store_bytes(const dl_pose_graph_3d* g, int64_t* uploaded, int64_t* capacity) {
+  if (!g) return DL_ERR_ARG;
+  if (uploaded) *uploaded = g->bytes_uploaded;
+  if (capacity) *capacity = g->store_capacity * (int64_t)sizeof(float);
+  return DL_OK;
+}
+
+}  // extern "C"

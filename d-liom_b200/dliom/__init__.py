@@ -34,6 +34,9 @@ EXPORTS = [
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
     "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
+    "dl_pose_graph_3d_create", "dl_pose_graph_3d_destroy", "dl_pose_graph_3d_add_node", "dl_pose_graph_3d_freeze_trajectory",
+    "dl_pose_graph_3d_run_final_optimization", "dl_pose_graph_3d_poses", "dl_pose_graph_3d_local_to_global",
+    "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
 ]
 
 
@@ -303,6 +306,57 @@ class MatchingResult(C.Structure):   # dl_matching_result
                 ("num_insertion_submaps", C.c_int32), ("insertion_submap_index", C.c_int32 * 2), ("reserved", C.c_int32)]
 
 
+class PoseGraph3DOptions(C.Structure):   # dl_pose_graph_3d_options
+    _fields_ = [("optimize_every_n_nodes", C.c_int32), ("every_nodes_to_find_constraint", C.c_int32),
+                ("matcher_translation_weight", C.c_double), ("matcher_rotation_weight", C.c_double),
+                ("constraint_builder", ConstraintOptions), ("optimization_problem", PoseGraphOptions)]
+
+    @staticmethod
+    def defaults(optimize_every_n_nodes=90, every_nodes_to_find_constraint=5, max_num_iterations=50, fix_z=False, **kw):
+        """pose_graph.lua: matcher weights 5e2 / 1.6e3, optimize_every_n_nodes 90, every_nodes_to_find_constraint 5, 50 iterations; kw go to
+        ConstraintOptions.defaults."""
+        return PoseGraph3DOptions(int(optimize_every_n_nodes), int(every_nodes_to_find_constraint), 5e2, 1.6e3,
+                                  ConstraintOptions.defaults(**kw), PoseGraphOptions(int(max_num_iterations), int(bool(fix_z))))
+
+
+class Pg3dInsertionSubmap(C.Structure):   # dl_pg3d_insertion_submap
+    _fields_ = [("submap_index", C.c_int32), ("finished", C.c_int32), ("high_resolution_grid", C.c_void_p),
+                ("low_resolution_grid", C.c_void_p), ("local_pose", C.c_double * 7)]
+
+
+class Pg3dNode(C.Structure):   # dl_pg3d_node
+    _fields_ = [("trajectory_id", C.c_int32), ("num_insertion_submaps", C.c_int32), ("time", C.c_double),
+                ("local_pose", C.c_double * 7), ("high_resolution_points", C.c_void_p), ("num_high_resolution", C.c_int64),
+                ("low_resolution_points", C.c_void_p), ("num_low_resolution", C.c_int64),
+                ("insertion_submaps", Pg3dInsertionSubmap * 2)]
+
+
+class Pg3dSubmapMatch(C.Structure):   # dl_pg3d_submap_match
+    _fields_ = [("trajectory_id", C.c_int32), ("submap_index", C.c_int32), ("x", C.c_double), ("y", C.c_double),
+                ("theta", C.c_double)]
+
+
+class Pg3dAddNodeInfo(C.Structure):   # dl_pg3d_add_node_info
+    _fields_ = [("node_index", C.c_int32), ("num_searched", C.c_int32), ("num_found", C.c_int32), ("optimized", C.c_int32),
+                ("cloud_bytes_uploaded", C.c_int64), ("bookkeeping_ms", C.c_double), ("search_ms", C.c_double),
+                ("solve_ms", C.c_double), ("summary", SolveSummary)]
+
+
+class Pg3dConstraint(C.Structure):   # dl_pg3d_constraint
+    _fields_ = [("submap_trajectory_id", C.c_int32), ("submap_index", C.c_int32), ("node_trajectory_id", C.c_int32),
+                ("node_index", C.c_int32), ("zbar", C.c_double * 7), ("translation_weight", C.c_double),
+                ("rotation_weight", C.c_double), ("tag", C.c_int32), ("reserved", C.c_int32)]
+
+
+class Pg3dSearch(C.Structure):   # dl_pg3d_search
+    _fields_ = [("submap_trajectory_id", C.c_int32), ("submap_index", C.c_int32), ("node_trajectory_id", C.c_int32),
+                ("node_index", C.c_int32), ("pose_guess", C.c_double * 7), ("result", Constraint)]
+
+
+PG3D_INTRA_SUBMAP, PG3D_INTER_SUBMAP = 0, 1
+PG3D_NODE_POSES, PG3D_SUBMAP_POSES, PG3D_OPTIMIZATION_NODES, PG3D_OPTIMIZATION_SUBMAPS = 0, 1, 2, 3
+
+
 def spa_constraints(constraints):
     """(submap, node, zbar7, translation_weight, rotation_weight) tuples -> a dl_spa_constraint array (numpy-packed: graphs of
     tens of thousands of constraints)."""
@@ -407,6 +461,17 @@ def lib():
     L.dl_window_optimize_batch.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, vp, f64p, vp]
     L.dl_pose_graph_solve_sparse.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, vp, C.c_int32,
                                              ip(SolveSummary), ip(PoseGraphSparseInfo)]
+    L.dl_pose_graph_3d_create.argtypes = [vp, ip(PoseGraph3DOptions), ip(vp)]
+    L.dl_pose_graph_3d_destroy.argtypes = [vp]
+    L.dl_pose_graph_3d_destroy.restype = None
+    L.dl_pose_graph_3d_add_node.argtypes = [vp, ip(Pg3dNode), C.c_int32, vp, vp]
+    L.dl_pose_graph_3d_freeze_trajectory.argtypes = [vp, C.c_int32]
+    L.dl_pose_graph_3d_run_final_optimization.argtypes = [vp, vp]
+    L.dl_pose_graph_3d_poses.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, ip(C.c_int32)]
+    L.dl_pose_graph_3d_local_to_global.argtypes = [vp, C.c_int32, vp]
+    L.dl_pose_graph_3d_constraints.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
+    L.dl_pose_graph_3d_last_searches.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
+    L.dl_pose_graph_3d_store_bytes.argtypes = [vp, ip(C.c_int64), ip(C.c_int64)]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
     L.dl_ltb_create.argtypes = [vp, ip(LtbOptions), ip(vp)]
     L.dl_ltb_destroy.argtypes = [vp]
@@ -1006,6 +1071,116 @@ class LocalTrajectoryBuilder:
         init = C.c_int32(0)
         self.ctx.check(self.ctx.L.dl_ltb_get_state(self.h, C.byref(s), C.byref(init)))
         return s.to16(), bool(init.value)
+
+
+class PoseGraph3D:
+    """mapping::PoseGraph3D on the fork's live loop-closure path (dl_pose_graph_3d_*): nodes from the local trajectory builders,
+    submap matches from the host SURF stage -> INTRA / INTER_SUBMAP constraints and optimized poses. Node clouds are uploaded
+    once into the object's device node store."""
+
+    def __init__(self, ctx, options=None):
+        self.ctx, self.options = ctx, options if options is not None else PoseGraph3DOptions.defaults()
+        self.h = C.c_void_p()
+        self._grids = {}   # the borrowed grids' Python handles stay alive with the graph, one entry per grid
+        ctx.check(ctx.L.dl_pose_graph_3d_create(ctx.h, C.byref(self.options), C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.ctx.L.dl_pose_graph_3d_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):
+            self.close()
+
+    def add_node(self, trajectory_id, time, local_pose, hi_points, lo_points, insertion_submaps, matches=()):
+        """insertion_submaps: 1 or 2 (submap_index, finished, hi Grid, lo Grid, local_pose7); matches: (trajectory_id,
+        submap_index, x, y, theta) of earlier finished submaps, only when insertion_submaps[0] finished -> Pg3dAddNodeInfo."""
+        hi = np.ascontiguousarray(hi_points, np.float32).reshape(-1, 3)
+        lo = np.ascontiguousarray(lo_points, np.float32).reshape(-1, 3)
+        n = Pg3dNode()
+        n.trajectory_id, n.num_insertion_submaps, n.time = int(trajectory_id), len(insertion_submaps), float(time)
+        n.local_pose[:] = [float(v) for v in local_pose]
+        n.high_resolution_points, n.num_high_resolution = hi.ctypes.data, len(hi)
+        n.low_resolution_points, n.num_low_resolution = lo.ctypes.data, len(lo)
+        for i, (index, finished, hg, lg, pose) in enumerate(insertion_submaps[:2]):
+            s = n.insertion_submaps[i]
+            s.submap_index, s.finished = int(index), int(bool(finished))
+            s.high_resolution_grid, s.low_resolution_grid = hg.h, lg.h
+            s.local_pose[:] = [float(v) for v in pose]
+            self._grids[hg.h.value if isinstance(hg.h, C.c_void_p) else hg.h] = hg
+            self._grids[lg.h.value if isinstance(lg.h, C.c_void_p) else lg.h] = lg
+        m = (Pg3dSubmapMatch * max(len(matches), 1))(*[Pg3dSubmapMatch(int(t), int(i), float(x), float(y), float(th))
+                                                        for t, i, x, y, th in matches])
+        info = Pg3dAddNodeInfo()
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_add_node(self.h, C.byref(n), len(matches), C.cast(m, C.c_void_p),
+                                                            C.byref(info)))
+        return info
+
+    def add_node_from_builder(self, trajectory_id, builder, result, matches=()):
+        """GlobalTrajectoryBuilder's AddNode call site: the node of a dl_ltb MatchingResult with insertion submaps, its clouds
+        and the submaps' grids, local poses and finished flags from the builder."""
+        subs = []
+        for i in range(result.num_insertion_submaps):
+            index = result.insertion_submap_index[i]
+            hg, lg, pose, _, finished = builder.submap(index)
+            subs.append((index, finished, hg, lg, pose))
+        return self.add_node(trajectory_id, result.time, np.array(result.local_pose[:]), builder.cloud(2), builder.cloud(3),
+                             subs, matches)
+
+    def freeze_trajectory(self, trajectory_id):
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_freeze_trajectory(self.h, int(trajectory_id)))
+
+    def run_final_optimization(self):
+        s = SolveSummary()
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_run_final_optimization(self.h, C.byref(s)))
+        return s.as_dict()
+
+    def _poses(self, trajectory_id, which):
+        n = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_poses(self.h, int(trajectory_id), which, 0, None, C.byref(n)))
+        out = np.zeros((max(n.value, 1), 7))
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_poses(self.h, int(trajectory_id), which, n.value, out.ctypes.data, C.byref(n)))
+        return out[:n.value]
+
+    def node_poses(self, trajectory_id):
+        return self._poses(trajectory_id, PG3D_NODE_POSES)
+
+    def submap_poses(self, trajectory_id):
+        return self._poses(trajectory_id, PG3D_SUBMAP_POSES)
+
+    def optimization_poses(self, trajectory_id):
+        """(submap_data, node_data) poses of the optimization problem: what the next solve starts from."""
+        return self._poses(trajectory_id, PG3D_OPTIMIZATION_SUBMAPS), self._poses(trajectory_id, PG3D_OPTIMIZATION_NODES)
+
+    def local_to_global(self, trajectory_id):
+        out = np.zeros(7)
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_local_to_global(self.h, int(trajectory_id), out.ctypes.data))
+        return out
+
+    def constraints(self):
+        """[(submap (trajectory, index), node (trajectory, index), zbar7, translation_weight, rotation_weight, tag)]"""
+        n = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_constraints(self.h, 0, None, C.byref(n)))
+        out = (Pg3dConstraint * max(n.value, 1))()
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_constraints(self.h, n.value, C.cast(out, C.c_void_p), C.byref(n)))
+        return [((c.submap_trajectory_id, c.submap_index), (c.node_trajectory_id, c.node_index), np.array(c.zbar[:]),
+                 c.translation_weight, c.rotation_weight, c.tag) for c in list(out)[:n.value]]
+
+    def last_searches(self):
+        """The (node, submap) searches of the last add_node call: [(submap id, node id, guess7, Constraint)]"""
+        n = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_last_searches(self.h, 0, None, C.byref(n)))
+        out = (Pg3dSearch * max(n.value, 1))()
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_last_searches(self.h, n.value, C.cast(out, C.c_void_p), C.byref(n)))
+        return [((s.submap_trajectory_id, s.submap_index), (s.node_trajectory_id, s.node_index), np.array(s.pose_guess[:]), s.result)
+                for s in list(out)[:n.value]]
+
+    def store_bytes(self):
+        """(cloud bytes uploaded since creation, node store capacity in bytes)"""
+        up, cap = C.c_int64(0), C.c_int64(0)
+        self.ctx.check(self.ctx.L.dl_pose_graph_3d_store_bytes(self.h, C.byref(up), C.byref(cap)))
+        return up.value, cap.value
 
 
 def comm_unique_id():

@@ -287,6 +287,24 @@ struct ConstraintBuilderOptions {  // proto::ConstraintBuilderOptions, the field
     ceres_scan_matcher_options_3d.rotation_weight = 1.;
     ceres_scan_matcher_options_3d.max_num_iterations = 10;
   }
+  dl_constraint_options c() const {
+    dl_constraint_options o{};
+    o.min_score = min_score;
+    o.loop_closure_translation_weight = loop_closure_translation_weight;
+    o.loop_closure_rotation_weight = loop_closure_rotation_weight;
+    o.fast_correlative_scan_matcher_3d = fast_correlative_scan_matcher_options_3d.c();
+    const auto& m = ceres_scan_matcher_options_3d;
+    o.ceres_scan_matcher_3d.num_occupied_space_weights = (int32_t)m.occupied_space_weight.size();
+    for (size_t i = 0; i < m.occupied_space_weight.size() && i < DL_MAX_PAIRS; ++i)
+      o.ceres_scan_matcher_3d.occupied_space_weight[i] = m.occupied_space_weight[i];
+    o.ceres_scan_matcher_3d.translation_weight = m.translation_weight;
+    o.ceres_scan_matcher_3d.rotation_weight = m.rotation_weight;
+    o.ceres_scan_matcher_3d.only_optimize_yaw = m.only_optimize_yaw;
+    o.ceres_scan_matcher_3d.use_nonmonotonic_steps = m.use_nonmonotonic_steps;
+    o.ceres_scan_matcher_3d.max_num_iterations = m.max_num_iterations;
+    o.ceres_scan_matcher_3d.num_threads = m.num_threads;
+    return o;
+  }
 };
 
 struct Constraint {  // PoseGraphInterface::Constraint (INTER_SUBMAP)
@@ -318,21 +336,7 @@ class ConstraintBuilder3D {
   }
   int GetNumQueuedSearches() const { return (int)ids_.size(); }
   std::vector<Constraint> Compute() {
-    dl_constraint_options o{};
-    o.min_score = options_.min_score;
-    o.loop_closure_translation_weight = options_.loop_closure_translation_weight;
-    o.loop_closure_rotation_weight = options_.loop_closure_rotation_weight;
-    o.fast_correlative_scan_matcher_3d = options_.fast_correlative_scan_matcher_options_3d.c();
-    const auto& c = options_.ceres_scan_matcher_options_3d;
-    o.ceres_scan_matcher_3d.num_occupied_space_weights = (int32_t)c.occupied_space_weight.size();
-    for (size_t i = 0; i < c.occupied_space_weight.size() && i < DL_MAX_PAIRS; ++i)
-      o.ceres_scan_matcher_3d.occupied_space_weight[i] = c.occupied_space_weight[i];
-    o.ceres_scan_matcher_3d.translation_weight = c.translation_weight;
-    o.ceres_scan_matcher_3d.rotation_weight = c.rotation_weight;
-    o.ceres_scan_matcher_3d.only_optimize_yaw = c.only_optimize_yaw;
-    o.ceres_scan_matcher_3d.use_nonmonotonic_steps = c.use_nonmonotonic_steps;
-    o.ceres_scan_matcher_3d.max_num_iterations = c.max_num_iterations;
-    o.ceres_scan_matcher_3d.num_threads = c.num_threads;
+    const dl_constraint_options o = options_.c();
     std::vector<dl_constraint> raw(ids_.size());
     ctx_->check(dl_constraint_search_batch(ctx_->get(), &o, (int32_t)ids_.size(), guesses_.data(), hi_.data(), hi_off_.data(),
                                            lo_.data(), lo_off_.data(), hi_grids_.data(), lo_grids_.data(), raw.data()));
@@ -661,4 +665,121 @@ class OptimizationProblem3D {
 };
 
 }  // namespace optimization
+
+namespace mapping {
+
+struct PoseGraphOptions {  // proto::PoseGraphOptions, the fields the live loop-closure path reads (pose_graph.lua)
+  int optimize_every_n_nodes = 90;
+  int every_nodes_to_find_constraint = 5;   // constraint_builder.every_nodes_to_find_constraint
+  double matcher_translation_weight = 5e2, matcher_rotation_weight = 1.6e3;
+  constraints::ConstraintBuilderOptions constraint_builder_options;
+  optimization::OptimizationProblemOptions optimization_problem_options;
+};
+struct SubmapMatch {  // one entry of ConstraintBuilder3D's matched_submaps: an earlier finished submap and Embed3D(Rigid2d)
+  optimization::SubmapId submap_id;
+  double x, y, theta;
+};
+struct PoseGraphConstraint {  // PoseGraphInterface::Constraint with its tag
+  enum Tag { INTRA_SUBMAP = DL_PG3D_INTRA_SUBMAP, INTER_SUBMAP = DL_PG3D_INTER_SUBMAP };
+  optimization::SubmapId submap_id;
+  optimization::NodeId node_id;
+  Rigid3d zbar_ij;
+  double translation_weight, rotation_weight;
+  Tag tag;
+};
+
+// mapping::PoseGraph3D (pose_graph_3d.cc) on the live loop-closure path: a thin owner of the C object dl_pose_graph_3d, which
+// holds the graph, the device node store and the constraint table, runs the searches and the solve (include/dliom_b200.h).
+// AddNode is the call GlobalTrajectoryBuilder makes (global_trajectory_builder.cc:80-82) with the builder whose submaps the
+// node was inserted into; `matches` is the host SURF stage's output for a newly finished submap (empty otherwise).
+class PoseGraph3D {
+ public:
+  PoseGraph3D(Context* ctx, const PoseGraphOptions& options) : ctx_(ctx) {
+    dl_pose_graph_3d_options o{};
+    o.optimize_every_n_nodes = options.optimize_every_n_nodes;
+    o.every_nodes_to_find_constraint = options.every_nodes_to_find_constraint;
+    o.matcher_translation_weight = options.matcher_translation_weight;
+    o.matcher_rotation_weight = options.matcher_rotation_weight;
+    o.constraint_builder = options.constraint_builder_options.c();
+    o.optimization_problem = {options.optimization_problem_options.max_num_iterations,
+                              options.optimization_problem_options.fix_z_in_3d ? 1 : 0};
+    ctx->check(dl_pose_graph_3d_create(ctx->get(), &o, &graph_));
+  }
+  ~PoseGraph3D() { dl_pose_graph_3d_destroy(graph_); }
+  PoseGraph3D(const PoseGraph3D&) = delete;
+  PoseGraph3D& operator=(const PoseGraph3D&) = delete;
+
+  // -> the node's id; the submaps' grids, local poses and finished flags come from the builder (dl_ltb_get_submap).
+  optimization::NodeId AddNode(int trajectory_id, const LocalTrajectoryBuilder3D& builder,
+                               const LocalTrajectoryBuilder3D::InsertionResult& insertion_result,
+                               const std::vector<SubmapMatch>& matches = {}, dl_pg3d_add_node_info* info = nullptr) {
+    const TrajectoryNodeData& data = *insertion_result.constant_data;
+    dl_pg3d_node node{};
+    node.trajectory_id = trajectory_id;
+    node.num_insertion_submaps = (int32_t)insertion_result.insertion_submaps.size();
+    if (node.num_insertion_submaps < 1 || node.num_insertion_submaps > 2) throw Error(DL_ERR_ARG, "one or two insertion submaps");
+    node.time = data.time;
+    data.local_pose.to7(node.local_pose);
+    node.high_resolution_points = data.high_resolution_point_cloud.empty() ? nullptr : data.high_resolution_point_cloud[0].data();
+    node.num_high_resolution = (int64_t)data.high_resolution_point_cloud.size();
+    node.low_resolution_points = data.low_resolution_point_cloud.empty() ? nullptr : data.low_resolution_point_cloud[0].data();
+    node.num_low_resolution = (int64_t)data.low_resolution_point_cloud.size();
+    for (int i = 0; i < node.num_insertion_submaps; ++i) {
+      dl_pg3d_insertion_submap& s = node.insertion_submaps[i];
+      dl_grid *hi = nullptr, *lo = nullptr;
+      int32_t num_range_data = 0;
+      s.submap_index = insertion_result.insertion_submaps[i];
+      ctx_->check(dl_ltb_get_submap(builder.get(), s.submap_index, &hi, &lo, s.local_pose, &num_range_data, &s.finished));
+      s.high_resolution_grid = hi;
+      s.low_resolution_grid = lo;
+    }
+    std::vector<dl_pg3d_submap_match> m;
+    for (const SubmapMatch& sm : matches) m.push_back({sm.submap_id.trajectory_id, sm.submap_id.submap_index, sm.x, sm.y, sm.theta});
+    dl_pg3d_add_node_info local{};
+    ctx_->check(dl_pose_graph_3d_add_node(graph_, &node, (int32_t)m.size(), m.data(), &local));
+    if (info) *info = local;
+    return {trajectory_id, local.node_index};
+  }
+  void FreezeTrajectory(int trajectory_id) { ctx_->check(dl_pose_graph_3d_freeze_trajectory(graph_, trajectory_id)); }
+  dl_solve_summary RunFinalOptimization() {
+    dl_solve_summary s{};
+    ctx_->check(dl_pose_graph_3d_run_final_optimization(graph_, &s));
+    return s;
+  }
+  std::vector<Rigid3d> GetTrajectoryNodePoses(int trajectory_id) const { return Poses(trajectory_id, DL_PG3D_NODE_POSES); }
+  // GetAllSubmapPoses for one trajectory: the optimized pose, or extrapolated with the local-to-global transform.
+  std::vector<Rigid3d> GetAllSubmapPoses(int trajectory_id) const { return Poses(trajectory_id, DL_PG3D_SUBMAP_POSES); }
+  Rigid3d GetLocalToGlobalTransform(int trajectory_id) const {
+    double p[7];
+    ctx_->check(dl_pose_graph_3d_local_to_global(graph_, trajectory_id, p));
+    return Rigid3d::from7(p);
+  }
+  std::vector<PoseGraphConstraint> constraints() const {
+    int32_t n = 0;
+    ctx_->check(dl_pose_graph_3d_constraints(graph_, 0, nullptr, &n));
+    std::vector<dl_pg3d_constraint> raw((size_t)n);
+    if (n) ctx_->check(dl_pose_graph_3d_constraints(graph_, n, raw.data(), &n));
+    std::vector<PoseGraphConstraint> out;
+    for (const dl_pg3d_constraint& c : raw)
+      out.push_back({{c.submap_trajectory_id, c.submap_index}, {c.node_trajectory_id, c.node_index}, Rigid3d::from7(c.zbar),
+                     c.translation_weight, c.rotation_weight, (PoseGraphConstraint::Tag)c.tag});
+    return out;
+  }
+  dl_pose_graph_3d* get() const { return graph_; }
+
+ private:
+  std::vector<Rigid3d> Poses(int trajectory_id, int which) const {
+    int32_t n = 0;
+    ctx_->check(dl_pose_graph_3d_poses(graph_, trajectory_id, which, 0, nullptr, &n));
+    std::vector<double> p(7 * (size_t)n);
+    if (n) ctx_->check(dl_pose_graph_3d_poses(graph_, trajectory_id, which, n, p.data(), &n));
+    std::vector<Rigid3d> out;
+    for (int32_t i = 0; i < n; ++i) out.push_back(Rigid3d::from7(&p[7 * (size_t)i]));
+    return out;
+  }
+  Context* ctx_;
+  dl_pose_graph_3d* graph_ = nullptr;
+};
+
+}  // namespace mapping
 }  // namespace dliom

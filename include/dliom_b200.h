@@ -350,6 +350,129 @@ int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const dl_pose_gra
                                int32_t num_nodes, double* poses, const uint8_t* frozen, const dl_spa_constraint* constraints,
                                int32_t num_constraints, dl_solve_summary* summary, dl_pose_graph_sparse_info* info);
 
+/* ---- mapping::PoseGraph3D (C/mapping/internal/3d/pose_graph_3d.cc) on the fork's live loop-closure path: the object between the
+ *      local trajectory builder and the optimizer. dl_pose_graph_3d_add_node restates, synchronously and in this order:
+ *        1. AddNode (:112-144): the node's index; a new submap id when insertion_submaps.back() is new; the node's pose
+ *           GetLocalToGlobalTransform * local_pose.
+ *        2. the node's high- and low-resolution clouds are uploaded ONCE into the object's device node store; every later
+ *           loop-closure search reads them there.
+ *        3. ComputeConstraintsForNode (:335-399): InitializeGlobalSubmapPoses (:67-110, both branches), the node's global pose
+ *           (:345-347), one INTRA_SUBMAP constraint local_submap^-1 * local_pose per insertion submap (matcher weights).
+ *        4. if insertion_submaps.front() is finished (:138, :384-391): it is marked finished and `matches` (the output of the
+ *           host SURF / RANSAC stage, ExtractFeaturesForSubmap, constraint_builder_3d.cc:436-532) are fanned out as
+ *           ComputeConstraintsBetweenSubmaps does (:162-200): per matched submap, in (trajectory, index) order, the counter j
+ *           restarts and runs over the finished submap's nodes in id order; a node with j % every_nodes_to_find_constraint != 0
+ *           or already in computed_constraints_ for the target submap is skipped. The pose guess is (:226-259)
+ *           T_G1_S1 * Embed3D(match) * T_S2_G2 * local_submap_from^-1 * local_pose with the rotation-only, yaw-removed gravity
+ *           alignments of the two submaps' LOCAL poses (ComputeConstraintsForSubmap, :1075-1097, passes the local pose). All
+ *           pairs of the submap run as one dl_constraint_search_batch (same kernels, same results) whose clouds are read from
+ *           the node store. Found constraints enter computed_constraints_ and wait as pending.
+ *        5. ++num_nodes_since_last_loop_closure; if optimize_every_n_nodes > 0 and the count is GREATER than it (:395-398), the
+ *           optimization runs: the pending constraints are appended in search order, skipping a (submap, node) already in the
+ *           table under either tag (HandleWorkQueue, :450-463); dl_pose_graph_solve_sparse over submaps then nodes, each ordered
+ *           by (trajectory, index), with the frozen trajectories' poses frozen; RunOptimization's update (:734-764); the count
+ *           is reset.
+ *      dl_pose_graph_3d_run_final_optimization runs the same step. The fork sets max_num_final_iterations and then overwrites it
+ *      with the regular cap (:677-682), so the final optimization uses optimization_problem.max_num_iterations as well.
+ *      Rejected with DL_ERR_ARG, the graph unchanged: a match naming an unknown or unfinished submap, the finished submap itself,
+ *      a same-trajectory submap with |index difference| <= 2 (ExtractFeaturesForSubmap never yields these, :466-473) or a
+ *      submap twice; matches when no submap finished; insertion submaps that do not continue the trajectory's sequence (a new
+ *      submap whose index is not the trajectory's next one). Graph state is committed only after the device work of steps 2-4
+ *      succeeded. If the solve of step 5 fails, the node stays added, the poses stay those of the previous optimization and
+ *      the found constraints stay pending (the next optimization appends them); the call returns the solve's status.
+ *      Deliberate differences: execution is synchronous and deterministic (the reference's thread pool may or may not finish a
+ *      search before WhenDone); not built: the per-node proximity search (its MaybeAdd*Constraint bodies are commented out in
+ *      this fork, :205-323, :367-381), trimming and trajectory connectivity, landmark / fixed-frame / odometry / IMU terms,
+ *      .pbstream loading, and a communicator (one GPU; the search and the solve it calls have NCCL variants).
+ *      The submap grids are borrowed (owner: the caller, e.g. the dl_local_trajectory_builder) and must outlive the graph. ---- */
+typedef struct dl_pose_graph_3d dl_pose_graph_3d;
+typedef struct dl_pose_graph_3d_options { /* proto::PoseGraphOptions, the fields this path reads */
+  int32_t optimize_every_n_nodes;         /* 0: only on dl_pose_graph_3d_run_final_optimization */
+  int32_t every_nodes_to_find_constraint; /* constraint_builder.every_nodes_to_find_constraint (>= 1) */
+  double matcher_translation_weight;      /* INTRA_SUBMAP weights */
+  double matcher_rotation_weight;
+  dl_constraint_options constraint_builder;
+  dl_pose_graph_options optimization_problem;
+} dl_pose_graph_3d_options;
+typedef struct dl_pg3d_insertion_submap {  /* one of InsertionResult::insertion_submaps */
+  int32_t submap_index;                    /* index in its trajectory (dl_matching_result::insertion_submap_index) */
+  int32_t finished;                        /* Submap3D::finished() after the node's insertion */
+  const dl_grid* high_resolution_grid;     /* borrowed */
+  const dl_grid* low_resolution_grid;
+  double local_pose[7];
+} dl_pg3d_insertion_submap;
+typedef struct dl_pg3d_node {              /* TrajectoryNode::Data + the insertion submaps */
+  int32_t trajectory_id;
+  int32_t num_insertion_submaps;           /* 1 or 2 */
+  double time;
+  double local_pose[7];
+  const float* high_resolution_points;     /* xyz floats, tracking frame */
+  int64_t num_high_resolution;
+  const float* low_resolution_points;
+  int64_t num_low_resolution;
+  dl_pg3d_insertion_submap insertion_submaps[2];
+} dl_pg3d_node;
+typedef struct dl_pg3d_submap_match {      /* one entry of matched_submaps: an earlier finished submap + Rigid2d (x, y, theta) */
+  int32_t trajectory_id;
+  int32_t submap_index;
+  double x, y, theta;
+} dl_pg3d_submap_match;
+typedef struct dl_pg3d_add_node_info {
+  int32_t node_index;                      /* NodeId::node_index in its trajectory */
+  int32_t num_searched;                    /* (node, submap) pairs searched by this call */
+  int32_t num_found;                       /* ... of which the coarse search passed min_score */
+  int32_t optimized;                       /* 1 if this call ran the optimization */
+  int64_t cloud_bytes_uploaded;            /* host-to-device bytes of point clouds: 12 * (n_hi + n_lo) of this node, nothing else */
+  double bookkeeping_ms, search_ms, solve_ms; /* host wall time of the call's parts (each ends in a device synchronise) */
+  dl_solve_summary summary;                /* of the optimization, if optimized */
+} dl_pg3d_add_node_info;
+#define DL_PG3D_INTRA_SUBMAP 0
+#define DL_PG3D_INTER_SUBMAP 1
+typedef struct dl_pg3d_constraint {        /* PoseGraphInterface::Constraint */
+  int32_t submap_trajectory_id, submap_index;
+  int32_t node_trajectory_id, node_index;
+  double zbar[7];
+  double translation_weight, rotation_weight;
+  int32_t tag;                             /* DL_PG3D_INTRA_SUBMAP / DL_PG3D_INTER_SUBMAP */
+  int32_t reserved;
+} dl_pg3d_constraint;
+int dl_pose_graph_3d_create(dl_context* ctx, const dl_pose_graph_3d_options* options, dl_pose_graph_3d** out);
+void dl_pose_graph_3d_destroy(dl_pose_graph_3d* graph);
+/* matches: num_matches entries, only when insertion_submaps[0].finished (else num_matches must be 0). info may be NULL. */
+int dl_pose_graph_3d_add_node(dl_pose_graph_3d* graph, const dl_pg3d_node* node, int32_t num_matches,
+                              const dl_pg3d_submap_match* matches, dl_pg3d_add_node_info* info);
+int dl_pose_graph_3d_freeze_trajectory(dl_pose_graph_3d* graph, int32_t trajectory_id);
+/* summary may be NULL. With no submap in the graph it returns DL_OK and leaves summary zeroed. */
+int dl_pose_graph_3d_run_final_optimization(dl_pose_graph_3d* graph, dl_solve_summary* summary);
+/* Poses of one trajectory, 7 doubles each, in index order. which:
+ *   DL_PG3D_NODE_POSES          trajectory_nodes_' global poses (GetTrajectoryNodePoses);
+ *   DL_PG3D_SUBMAP_POSES        GetSubmapDataUnderLock (:937-952): the optimized pose, or local_to_global * local_pose for a
+ *                               submap not optimized yet;
+ *   DL_PG3D_OPTIMIZATION_NODES  / DL_PG3D_OPTIMIZATION_SUBMAPS  the optimization problem's node_data / submap_data, i.e. the
+ *                               poses the next solve starts from.
+ * Pass poses = NULL to query *count (the trajectory's size; 0 for an unknown trajectory). */
+#define DL_PG3D_NODE_POSES 0
+#define DL_PG3D_SUBMAP_POSES 1
+#define DL_PG3D_OPTIMIZATION_NODES 2
+#define DL_PG3D_OPTIMIZATION_SUBMAPS 3
+int dl_pose_graph_3d_poses(const dl_pose_graph_3d* graph, int32_t trajectory_id, int32_t which, int32_t capacity, double* poses,
+                           int32_t* count);
+/* GetLocalToGlobalTransform (:914-935): last optimized submap's global pose * its local pose^-1 (identity before any). */
+int dl_pose_graph_3d_local_to_global(const dl_pose_graph_3d* graph, int32_t trajectory_id, double* pose);
+/* The constraint table in insertion order. Pass out = NULL to query *count. */
+int dl_pose_graph_3d_constraints(const dl_pose_graph_3d* graph, int32_t capacity, dl_pg3d_constraint* out, int32_t* count);
+/* The (node, submap) searches of the last successful dl_pose_graph_3d_add_node call in search order: ids, the pose guess and the
+ * dl_constraint_search_batch record. Pass out = NULL to query *count. */
+typedef struct dl_pg3d_search {
+  int32_t submap_trajectory_id, submap_index;
+  int32_t node_trajectory_id, node_index;
+  double pose_guess[7];
+  dl_constraint result;
+} dl_pg3d_search;
+int dl_pose_graph_3d_last_searches(const dl_pose_graph_3d* graph, int32_t capacity, dl_pg3d_search* out, int32_t* count);
+/* Bytes of clouds uploaded into the node store since creation, and its capacity in bytes. */
+int dl_pose_graph_3d_store_bytes(const dl_pose_graph_3d* graph, int64_t* uploaded, int64_t* capacity);
+
 /* ---- IMU: pre-integration (LocalTrajectoryBuilder3D::AddImuData, LTB:164-201, with the in-repo mid-point integrator
  *      C/mapping/internal/3d/initialization/integration_base.h:109-265 instead of the un-vendored GTSAM one) and the
  *      scan match with the pre-integration residual (integration_base.h:267-301) fused into the same solve.
