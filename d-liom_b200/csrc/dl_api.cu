@@ -1674,21 +1674,6 @@ struct FrontendBuffers {
 // Device scratch of one front-end run. The stage-wise buffers (one voxel-filter pass per launch: dl_voxel.cu / dl_ingest.cu)
 // exist only for dl_ingest_scan, which cross-checks the fused front half against them; the batched path does not carve them
 // (round 1 did: ~150 B x cap x batch of dead scratch per context).
-size_t frontend_bytes(int batch, int64_t cap, int num_origins, size_t extra, bool stagewise = false) {
-  const size_t B = (size_t)batch, C = (size_t)cap;
-  const size_t tcap = (size_t)next_pow2(2 * cap);
-  const size_t tiles = (C + 255) / 256;
-  size_t bytes = arena_bytes({B * 4, B * 4, B * 4, B * 4, B * 4, B * 4, B * 8, B * 8, B * 8, B * tiles * 8,
-                              B * tcap * 4, B * 2 * tcap * 4, B * 4 * C * 4, B * 2 * C * 4,
-                              B * C * 12, B * C * 12, B * 2 * C * 12, B * 28, (size_t)num_origins * 12,
-                              B * 2 * 32 * 4, B * 4, B * sizeof(ScanConstants), 2 * sizeof(AdaptiveParams), B * 56, B * 24,
-                              B * sizeof(NlsProblem), B * sizeof(NlsOutput),
-                              B * (size_t)next_pow2(cap) * 8, B * 2 * ((C + 31) / 32) * 4, B * 4, B * 4 + 64, B * C * 16,
-                              adaptive_first_pass_bytes(2 * batch, cap) + 16 * 1024});
-  if (stagewise) bytes += arena_bytes({B * tiles * 4, B * C * 4, B * C * 4, B * C * 4, B * C * 4, B * C * 12, B * C * 12, B * C * 12, B * C});
-  return bytes + extra + 8192;
-}
-
 void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f, bool stagewise = false) {
   const size_t B = (size_t)batch, C = (size_t)cap;
   f->batch = batch;
@@ -1725,6 +1710,14 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   }
 }
 
+// Bytes `carve` takes (counted by carving a null arena), plus slack for the few small takes of a run.
+size_t frontend_bytes(int batch, int64_t cap, int num_origins, bool stagewise = false) {
+  Arena count(nullptr);
+  FrontendBuffers f;
+  carve(count, batch, cap, num_origins, &f, stagewise);
+  return count.off + 8192;
+}
+
 FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuffers& f, const float* d_ranges,
                                 int64_t in_cap, int row_floats) {
   FrontendArgs fa{};
@@ -1732,11 +1725,8 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
   fa.origins = f.origins; fa.cap = f.cap; fa.tiles = f.tiles; fa.tcap2 = f.tcap2;
   // First-filter table of the fused path: the next power of two above 2 * cap (load ~0.18 on real sweeps). A compact table of
   // 1.25 slots per point (the kernels take any size: slot = hash * tcap >> 32) saves a third of the memset and of the ingest
-  // kernel's table stream but costs the first filter more in collisions than it saves — kept as DLIOM_TABLE1_COMPACT=1 for
-  // experiments.
+  // kernel's table stream but costs the first filter more in collisions than it saves.
   fa.tcap1 = f.tcap;
-  if (const char* env = std::getenv("DLIOM_TABLE1_COMPACT"))
-    if (std::atoi(env)) fa.tcap1 = std::min<int64_t>(f.tcap, ((f.cap + f.cap / 4 + 63) / 64) * 64);
   fa.first_resolution = 0.5f * o.voxel_filter_size;  // LTB:394
   fa.second_resolution = o.voxel_filter_size;        // LTB:479-484
   fa.min_range = o.min_range; fa.max_range = o.max_range; fa.scan_period = o.scan_period;
@@ -1751,13 +1741,11 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
   return fa;
 }
 
-size_t time_runs_bytes(const dl_frontend_options& o, int num_scans) {  // device copies of the time_run_* arrays
+// Device copies of the time_run_* arrays and the table of per-run deskew poses (32 B per run).
+size_t time_runs_bytes(const dl_frontend_options& o, int num_scans) {
   if (o.range_row_floats != 3 || !o.time_run_offsets || num_scans <= 0) return 0;
-  return arena_bytes({(size_t)(num_scans + 1) * 4, (size_t)o.time_run_offsets[num_scans] * 4, (size_t)o.time_run_offsets[num_scans] * 4});
-}
-size_t time_expand_bytes(const dl_frontend_options& o, int num_scans, int64_t cap) {
-  if (o.range_row_floats != 3 || !o.time_run_offsets || num_scans <= 0) return 0;
-  return (size_t)num_scans * (size_t)cap * 4 + (size_t)o.time_run_offsets[num_scans] * 32 + 768;  // run ids per row + run poses
+  const size_t runs = (size_t)o.time_run_offsets[num_scans];
+  return arena_bytes({(size_t)(num_scans + 1) * 4, runs * 4, runs * 4, runs * 32});
 }
 int row_floats_of(const dl_frontend_options& o) { return o.range_row_floats == 4 ? 4 : (o.range_row_floats == 3 ? 3 : 8); }
 
@@ -1955,15 +1943,6 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
     if (runs > (size_t)8 * num_scans) {  // many runs per scan: one deskew pose per run (fe_run_poses) instead of one per survivor
       int max_runs = 0;
       for (int b = 0; b < num_scans; ++b) max_runs = std::max(max_runs, (int)(o.time_run_offsets[b + 1] - o.time_run_offsets[b]));
-      // The run of a row is found by a binary search of the scan's ~2 k run starts (L1-resident) per survivor. Expanding the run
-      // index of EVERY row once per batch (4 B per row, one more kernel and 17 MB of writes per step, then one random sector per
-      // survivor) makes the ingest kernel itself faster but the step slower: kept as DLIOM_EXPAND_RUNS=1 for experiments.
-      const char* expand = std::getenv("DLIOM_EXPAND_RUNS");
-      if (expand && std::atoi(expand) != 0) {
-        int32_t* d_run_of_row = a.take<int32_t>((size_t)num_scans * in_cap);
-        DL_TRY(launch_fe_expand_runs(ctx, fa, num_scans, max_runs, d_run_of_row));  // needs counts + runs only, both uploaded above
-        fa.run_of_row = d_run_of_row;
-      }
       fa.run_pose = a.take<float>(runs * 8);  // filled per sub-batch by fe_run_poses once the scans' deskew constants exist
       fa.max_runs = max_runs;
     }
@@ -1972,19 +1951,12 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
   const Rigidd submap = pose_from7(submap_local_pose);
   const bool rtcsm = o.use_online_correlative_scan_matching != 0;
   int chunks = rtcsm ? 1 : (host_ranges ? 5 : 2);
-  if (const char* env = std::getenv(host_ranges ? "DLIOM_CHUNKS_HOST" : "DLIOM_CHUNKS_DEV")) chunks = rtcsm ? 1 : std::max(1, std::atoi(env));
   if (f.batch < 8 * chunks) chunks = std::max(1, f.batch / 8);
-  // Pipeline shape. 1: every front half (bandwidth-bound, thousands of CTAs) runs in order on the main stream and
-  // every back half (latency-bound, one or two CTAs per scan) on a HIGH-PRIORITY stream behind its front half's event, so
-  // the back half of sub-batch k gets SMs the moment CTAs of front half k+1 retire instead of queueing behind that grid.
-  // 0 (default): sub-batches alternate between two equal-priority streams.
-  // (0 is the default because the back half is latency-bound, so serialising all back halves on one stream costs more than the
-  // priority gains; 1 is kept for experiments.)
-  int split = 0;
-  if (const char* env = std::getenv("DLIOM_PIPELINE")) split = rtcsm ? 0 : std::atoi(env);
+  // Sub-batches alternate between two equal-priority streams. Every back half (latency-bound, one or two CTAs per scan) on one
+  // high-priority stream behind its front half would serialise the back halves, which costs more than the priority gains.
   // DLIOM_SERIAL=1: every sub-batch on the main stream, nothing overlaps (bench.py's per-stage roofline pass: the stage events then
   // bracket the kernels' own durations at the sub-batch size the step really uses)
-  const bool serial = std::getenv("DLIOM_SERIAL") != nullptr && !split;
+  const bool serial = std::getenv("DLIOM_SERIAL") != nullptr;
   cudaStream_t main_stream = ctx->stream;
   cudaEvent_t prepared = ctx->take_event();
   DL_CUDA(ctx, cudaEventRecord(prepared, main_stream));
@@ -2028,7 +2000,7 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
   std::vector<int> bounds(chunks + 1, 0);
   {
     std::vector<double> share(chunks, 1.0);
-    if (host_ranges && chunks >= 3 && !std::getenv("DLIOM_EQUAL_CHUNKS")) {
+    if (host_ranges && chunks >= 3) {
       share[chunks - 2] = 0.5;
       share[chunks - 1] = 0.25;
     }
@@ -2042,7 +2014,7 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
   for (int k = 0; k < chunks && status == DL_OK; ++k) {
     const int b0 = bounds[k], b1 = bounds[k + 1], nb = b1 - b0;
     if (nb <= 0) continue;
-    ctx->stream = (split || serial) ? main_stream : ((k & 1) ? ctx->aux_stream : main_stream);
+    ctx->stream = (!serial && (k & 1)) ? ctx->aux_stream : main_stream;
     auto run = [&]() -> int {
       {
         StageScope st(ctx, "voxel_filter_first");
@@ -2071,13 +2043,6 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
       {
         StageScope st(ctx, "ingest_second_filter");
         DL_TRY(launch_fe_rest(ctx, fa, b0, nb));
-      }
-      if (split) {
-        cudaEvent_t front_done = ctx->take_event();
-        DL_CUDA(ctx, cudaEventRecord(front_done, main_stream));
-        DL_CUDA(ctx, cudaStreamWaitEvent(ctx->tail_stream, front_done, 0));
-        ctx->event_pool.push_back(front_done);
-        ctx->stream = ctx->tail_stream;
       }
       {
         // adaptive voxel filters (high, low resolution) on the tracking-frame returns: one CTA per (scan, filter)
@@ -2146,9 +2111,9 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
   }
   ctx->stream = main_stream;
   if (imu_ready) ctx->event_pool.push_back(imu_ready);
-  if (chunks > 1 || split) {  // later work on the main stream (result copies, the next call) waits for the other streams
+  if (chunks > 1) {  // later work on the main stream (result copies, the next call) waits for the other stream
     cudaEvent_t joined = ctx->take_event();
-    DL_CUDA(ctx, cudaEventRecord(joined, split ? ctx->tail_stream : ctx->aux_stream));
+    DL_CUDA(ctx, cudaEventRecord(joined, ctx->aux_stream));
     DL_CUDA(ctx, cudaStreamWaitEvent(main_stream, joined, 0));
     ctx->event_pool.push_back(joined);
   }
@@ -2183,6 +2148,61 @@ int check_frontend(dl_context* ctx, const dl_frontend_options* o, int num_scans,
   return DL_OK;
 }
 
+// Where the scans of a batch are: host rows, one pointer per scan, which the batch uploads into its scratch; or device rows
+// (scan b at row b * cap_rows) with a caller-provided device buffer for the results (and, with raw IMU samples, one for the
+// estimated states in ImuRun::d_states_out).
+struct FrontendScans {
+  const void* const* host = nullptr;
+  bool on_device = false;
+  const void* dev = nullptr;
+  int64_t cap_rows = 0;
+  dl_scan_result* results_dev = nullptr;
+};
+
+// Validates, reserves, carves and enqueues one front-end batch: the one place that sizes a batch's scratch. On return
+// *d_results_out holds the device results (not yet synchronised).
+int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int num_scans, const FrontendScans& in,
+                     const int64_t* sizes, const float* origins, int num_origins, const double* prev_poses,
+                     const double* predicted_poses, const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo,
+                     size_t pinned_extra, dl_scan_result** d_results_out, ImuRun* imu = nullptr,
+                     FrontendBuffers* buffers_out = nullptr) {
+  int64_t max_size = 0;
+  DL_TRY(check_frontend(ctx, options, num_scans, sizes, hi, lo, &max_size));
+  if (num_scans == 0) return DL_OK;
+  const bool raw = imu && imu->samples;
+  if (!origins || num_origins < 1 || (!raw && (!prev_poses || !predicted_poses)) || !submap_local_pose) return DL_ERR_ARG;
+  if (in.on_device) {
+    if (!in.dev || !in.results_dev || (imu && !imu->d_states_out) || in.cap_rows < max_size || in.cap_rows < 1) return DL_ERR_ARG;
+  } else {
+    if (!in.host) return DL_ERR_ARG;
+    for (int b = 0; b < num_scans; ++b)
+      if (sizes[b] > 0 && !in.host[b]) return DL_ERR_ARG;
+    if (options->host_scan_stride_rows != 0) {
+      const int64_t stride = options->host_scan_stride_rows;
+      const size_t row_bytes = (size_t)row_floats_of(*options) * 4;
+      if (stride < max_size) return ctx->fail(DL_ERR_ARG, "host_scan_stride_rows is smaller than a scan");
+      for (int b = 0; b < num_scans; ++b)
+        if ((const char*)in.host[b] != (const char*)in.host[0] + (size_t)b * stride * row_bytes)
+          return ctx->fail(DL_ERR_ARG, "host_scan_stride_rows does not describe the ranges pointers");
+    }
+  }
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int64_t cap = in.on_device ? in.cap_rows : std::max<int64_t>(max_size, 1);
+  size_t bytes = frontend_bytes(num_scans, cap, num_origins) + time_runs_bytes(*options, num_scans);
+  if (options->use_online_correlative_scan_matching)
+    bytes += (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, hi->resolution, false);
+  if (imu) bytes += imu_run_device_bytes(num_scans, imu->samples);
+  if (!in.on_device) bytes += arena_bytes({(size_t)num_scans * cap * 32, (size_t)num_scans * sizeof(dl_scan_result)});
+  DL_TRY(ctx->reserve_device(bytes));
+  if (pinned_extra) DL_TRY(ctx->reserve_pinned(frontend_small_bytes(num_scans, num_origins) + pinned_extra + 256));
+  Arena a(ctx->d_scratch);
+  float* d_ranges = in.on_device ? (float*)in.dev : a.take<float>((size_t)num_scans * cap * 8);
+  dl_scan_result* d_results = in.on_device ? in.results_dev : a.take<dl_scan_result>(num_scans);
+  if (d_results_out) *d_results_out = d_results;
+  return frontend_run(ctx, *options, num_scans, d_ranges, cap, in.host, sizes, origins, num_origins, prev_poses,
+                      predicted_poses, submap_local_pose, hi, lo, a, d_results, imu, buffers_out);
+}
+
 }  // namespace
 
 extern "C" {
@@ -2193,19 +2213,13 @@ int dl_frontend_match_batch_dev(dl_context* ctx, const dl_frontend_options* opti
                                 const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo,
                                 dl_scan_result* results_dev) {
   if (!ctx) return DL_ERR_ARG;
-  int64_t max_size = 0;
-  DL_TRY(check_frontend(ctx, options, num_scans, sizes, hi, lo, &max_size));
-  if (num_scans == 0) return DL_OK;
-  if (!ranges_dev || !origins || num_origins < 1 || !prev_poses || !predicted_poses || !submap_local_pose || !results_dev ||
-      cap_rows < max_size || cap_rows < 1)
-    return DL_ERR_ARG;
-  DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t extra = options->use_online_correlative_scan_matching
-                           ? (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, hi->resolution, false) : 0;
-  DL_TRY(ctx->reserve_device(frontend_bytes(num_scans, cap_rows, num_origins, extra) + time_runs_bytes(*options, num_scans) + time_expand_bytes(*options, num_scans, cap_rows)));
-  Arena a(ctx->d_scratch);
-  return frontend_run(ctx, *options, num_scans, (float*)ranges_dev, cap_rows, nullptr, sizes, origins, num_origins,
-                      prev_poses, predicted_poses, submap_local_pose, hi, lo, a, results_dev);
+  FrontendScans in;
+  in.on_device = true;
+  in.dev = ranges_dev;
+  in.cap_rows = cap_rows;
+  in.results_dev = results_dev;
+  return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, prev_poses, predicted_poses,
+                          submap_local_pose, hi, lo, 0, nullptr);
 }
 
 int dl_frontend_fetch_results(dl_context* ctx, const dl_scan_result* results_dev, int32_t num_scans,
@@ -2213,41 +2227,6 @@ int dl_frontend_fetch_results(dl_context* ctx, const dl_scan_result* results_dev
   if (!ctx || num_scans < 0 || (num_scans > 0 && (!results_dev || !results))) return DL_ERR_ARG;
   DL_TRY(d2h(ctx, results, results_dev, num_scans));
   return sync(ctx);
-}
-
-// Validates, reserves and enqueues one host-buffer batch; on return *d_results_out holds the device results (not yet synchronised).
-static int frontend_enqueue_host(dl_context* ctx, const dl_frontend_options* options, int32_t num_scans, const void* const* ranges,
-                                 const int64_t* sizes, const float* origins, int32_t num_origins, const double* prev_poses,
-                                 const double* predicted_poses, const double* submap_local_pose, const dl_grid* hi,
-                                 const dl_grid* lo, size_t pinned_extra, dl_scan_result** d_results_out, ImuRun* imu = nullptr,
-                                 FrontendBuffers* buffers_out = nullptr) {
-  int64_t max_size = 0;
-  DL_TRY(check_frontend(ctx, options, num_scans, sizes, hi, lo, &max_size));
-  const bool raw = imu && imu->samples;
-  if (!ranges || !origins || num_origins < 1 || (!raw && (!prev_poses || !predicted_poses)) || !submap_local_pose) return DL_ERR_ARG;
-  for (int b = 0; b < num_scans; ++b)
-    if (sizes[b] > 0 && !ranges[b]) return DL_ERR_ARG;
-  if (options->host_scan_stride_rows != 0) {
-    const int64_t stride = options->host_scan_stride_rows;
-    const size_t row_bytes = (size_t)row_floats_of(*options) * 4;
-    if (stride < max_size) return ctx->fail(DL_ERR_ARG, "host_scan_stride_rows is smaller than a scan");
-    for (int b = 0; b < num_scans; ++b)
-      if ((const char*)ranges[b] != (const char*)ranges[0] + (size_t)b * stride * row_bytes)
-        return ctx->fail(DL_ERR_ARG, "host_scan_stride_rows does not describe the ranges pointers");
-  }
-  DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int64_t cap = std::max<int64_t>(max_size, 1);
-  const size_t extra = options->use_online_correlative_scan_matching
-                           ? (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, hi->resolution, false) : 0;
-  const size_t device_extra = imu ? imu_run_device_bytes(num_scans, imu->samples) : 0;
-  DL_TRY(ctx->reserve_device(frontend_bytes(num_scans, cap, num_origins, extra) + (size_t)num_scans * cap * 32 + 256 +
-                             (size_t)num_scans * sizeof(dl_scan_result) + 256 + device_extra + time_runs_bytes(*options, num_scans) + time_expand_bytes(*options, num_scans, cap)));
-  if (pinned_extra) DL_TRY(ctx->reserve_pinned(frontend_small_bytes(num_scans, num_origins) + pinned_extra + 256));
-  Arena a(ctx->d_scratch);
-  float* d_ranges = a.take<float>((size_t)num_scans * cap * 8);
-  *d_results_out = a.take<dl_scan_result>(num_scans);
-  return frontend_run(ctx, *options, num_scans, d_ranges, cap, ranges, sizes, origins, num_origins, prev_poses,
-                      predicted_poses, submap_local_pose, hi, lo, a, *d_results_out, imu, buffers_out);
 }
 
 int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options, int32_t num_scans,
@@ -2261,8 +2240,8 @@ int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options,
   }
   if (!results) return DL_ERR_ARG;
   dl_scan_result* d_results = nullptr;
-  DL_TRY(frontend_enqueue_host(ctx, options, num_scans, ranges, sizes, origins, num_origins, prev_poses, predicted_poses,
-                               submap_local_pose, hi, lo, 0, &d_results));
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev_poses, predicted_poses,
+                          submap_local_pose, hi, lo, 0, &d_results));
   DL_TRY(d2h(ctx, results, d_results, num_scans));
   return sync(ctx);
 }
@@ -2295,8 +2274,8 @@ int dl_frontend_match_batch_imu(dl_context* ctx, const dl_frontend_options* opti
   dl_scan_result* d_results = nullptr;
   ImuRun run;
   run.host = imu;
-  DL_TRY(frontend_enqueue_host(ctx, options, num_scans, ranges, sizes, origins, num_origins, prev.data(), pred.data(),
-                               submap_local_pose, hi, lo, 0, &d_results, &run));
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev.data(), pred.data(),
+                          submap_local_pose, hi, lo, 0, &d_results, &run));
   DL_TRY(d2h(ctx, results, d_results, num_scans));
   DL_TRY(d2h(ctx, imu->states_out, run.d_states, num_scans));
   return sync(ctx);
@@ -2325,8 +2304,8 @@ int dl_frontend_match_batch_imu_samples(dl_context* ctx, const dl_frontend_optio
   dl_scan_result* d_results = nullptr;
   ImuRun run;
   run.samples = imu;
-  DL_TRY(frontend_enqueue_host(ctx, options, num_scans, ranges, sizes, origins, num_origins, nullptr, nullptr,
-                               submap_local_pose, hi, lo, 0, &d_results, &run));
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, nullptr, nullptr,
+                          submap_local_pose, hi, lo, 0, &d_results, &run));
   DL_TRY(d2h(ctx, results, d_results, num_scans));
   DL_TRY(d2h(ctx, states_out, run.d_states, num_scans));
   if (predicted_states_out) DL_TRY(d2h(ctx, predicted_states_out, run.d_predicted, num_scans));
@@ -2340,21 +2319,16 @@ int dl_frontend_match_batch_imu_samples_dev(dl_context* ctx, const dl_frontend_o
                                             dl_scan_result* results_dev, dl_nav_state* states_out_dev) {
   if (!ctx) return DL_ERR_ARG;
   DL_TRY(check_imu_samples(ctx, options, imu, num_scans));
-  int64_t max_size = 0;
-  DL_TRY(check_frontend(ctx, options, num_scans, sizes, hi, lo, &max_size));
-  if (num_scans == 0) return DL_OK;
-  if (!ranges_dev || !origins || num_origins < 1 || !submap_local_pose || !results_dev || !states_out_dev || cap_rows < max_size ||
-      cap_rows < 1)
-    return DL_ERR_ARG;
-  DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(frontend_bytes(num_scans, cap_rows, num_origins, 0) + imu_run_device_bytes(num_scans, imu) +
-                             time_runs_bytes(*options, num_scans) + time_expand_bytes(*options, num_scans, cap_rows)));
-  Arena a(ctx->d_scratch);
+  FrontendScans in;
+  in.on_device = true;
+  in.dev = ranges_dev;
+  in.cap_rows = cap_rows;
+  in.results_dev = results_dev;
   ImuRun run;
   run.samples = imu;
   run.d_states_out = states_out_dev;
-  return frontend_run(ctx, *options, num_scans, (float*)ranges_dev, cap_rows, nullptr, sizes, origins, num_origins, nullptr,
-                      nullptr, submap_local_pose, hi, lo, a, results_dev, &run);
+  return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, nullptr, nullptr, submap_local_pose, hi, lo, 0,
+                          nullptr, &run);
 }
 
 // Tail of a submit: the results (and, with the IMU, the estimated states) go to pinned staging behind the batch.
@@ -2382,8 +2356,8 @@ int dl_frontend_submit(dl_context* ctx, const dl_frontend_options* options, int3
   if (!ctx || num_scans < 1) return DL_ERR_ARG;
   if (ctx->in_flight) return ctx->fail(DL_ERR_ARG, "a submitted batch is already in flight on this context");
   dl_scan_result* d_results = nullptr;
-  DL_TRY(frontend_enqueue_host(ctx, options, num_scans, ranges, sizes, origins, num_origins, prev_poses, predicted_poses,
-                               submap_local_pose, hi, lo, submit_pinned_bytes(num_scans), &d_results));
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev_poses, predicted_poses,
+                          submap_local_pose, hi, lo, submit_pinned_bytes(num_scans), &d_results));
   return submit_finish(ctx, num_scans, num_origins, d_results, nullptr);
 }
 
@@ -2396,8 +2370,8 @@ int dl_frontend_submit_imu_samples(dl_context* ctx, const dl_frontend_options* o
   dl_scan_result* d_results = nullptr;
   ImuRun run;
   run.samples = imu;
-  DL_TRY(frontend_enqueue_host(ctx, options, num_scans, ranges, sizes, origins, num_origins, nullptr, nullptr, submap_local_pose,
-                               hi, lo, submit_pinned_bytes(num_scans), &d_results, &run));
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, nullptr, nullptr, submap_local_pose,
+                          hi, lo, submit_pinned_bytes(num_scans), &d_results, &run));
   return submit_finish(ctx, num_scans, num_origins, d_results, run.d_states);
 }
 
@@ -2498,7 +2472,7 @@ int dl_ingest_scan(dl_context* ctx, const dl_frontend_options* options, const vo
       !counts_out)
     return DL_ERR_ARG;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(frontend_bytes(1, n, num_origins, 0, true) + (size_t)n * 32 + 256));
+  DL_TRY(ctx->reserve_device(frontend_bytes(1, n, num_origins, true) + (size_t)n * 32 + 256));
   Arena a(ctx->d_scratch);
   float* d_ranges = a.take<float>((size_t)n * 8);
   DL_TRY(h2d(ctx, d_ranges, (const float*)ranges, (size_t)n * 8));
@@ -2765,8 +2739,8 @@ int dl_ltb_add_synchronized_range_data(dl_local_trajectory_builder* b, double ti
   if (!b->opt.two_stage) {
     ImuRun run;
     run.samples = &imu;
-    DL_TRY(frontend_enqueue_host(ctx, &fo, 1, ranges, sizes, origin, num_origins, nullptr, nullptr, submap_pose, matching.hi, matching.lo,
-                                 0, &d_results, &run, &f));
+    DL_TRY(frontend_enqueue(ctx, &fo, 1, FrontendScans{ranges}, sizes, origin, num_origins, nullptr, nullptr, submap_pose, matching.hi, matching.lo,
+                            0, &d_results, &run, &f));
     DL_TRY(d2h(ctx, &r, d_results, 1));
     DL_TRY(d2h(ctx, &state, run.d_states, 1));
     DL_TRY(d2h(ctx, cur7, f.current_pose, 7));
@@ -2782,8 +2756,8 @@ int dl_ltb_add_synchronized_range_data(dl_local_trajectory_builder* b, double ti
     double prev7[7], pred7[7];
     for (int k = 0; k < 3; ++k) { prev7[k] = b->prev_state.p[k]; pred7[k] = pred.p[k]; }
     for (int k = 0; k < 4; ++k) { prev7[3 + k] = b->prev_state.q[k]; pred7[3 + k] = pred.q[k]; }
-    DL_TRY(frontend_enqueue_host(ctx, &fo, 1, ranges, sizes, origin, num_origins, prev7, pred7, submap_pose, matching.hi, matching.lo, 0,
-                                 &d_results, nullptr, &f));
+    DL_TRY(frontend_enqueue(ctx, &fo, 1, FrontendScans{ranges}, sizes, origin, num_origins, prev7, pred7, submap_pose, matching.hi, matching.lo, 0,
+                            &d_results, nullptr, &f));
     DL_TRY(d2h(ctx, &r, d_results, 1));
     DL_TRY(d2h(ctx, cur7, f.current_pose, 7));
     DL_TRY(sync(ctx));

@@ -27,8 +27,6 @@
 //
 // Algorithmic traffic per raw point: A reads 12/16 B; B reads 4 B slot (+12/16 B row + 4 B time, writes 16 B record + 8 B slot
 // for survivors); C1 reads 8 B per slot; C2 reads 16 B and writes 12 B per output point.
-#include <cstdlib>
-
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
 
@@ -59,9 +57,10 @@ __device__ __forceinline__ Vec3f load_xyz(const float* __restrict__ rows, int ro
   return {v.x, v.y, v.z};
 }
 
-// 12-byte rows: index (into the batch's run arrays) of the time run that contains row i of scan b.
+// 12-byte rows: index (into the batch's run arrays) of the time run that contains row i of scan b. A binary search of the scan's
+// ~2 k run starts (L1-resident) per survivor: expanding the run index of every row once per batch (4 B per row, one more kernel
+// and 17 MB of writes per step) made the ingest kernel faster but the step slower.
 __device__ __forceinline__ int run_index(const FrontendArgs& a, int b, int i) {
-  if (a.run_of_row) return a.run_of_row[(size_t)b * a.in_cap + i];
   int lo = a.run_offsets[b], hi = a.run_offsets[b + 1] - 1;  // last run whose first row is <= i
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -76,23 +75,10 @@ __device__ __forceinline__ float point_time(const FrontendArgs& a, int b, const 
   return a.run_value[run_index(a, b, i)];
 }
 
-// 12-byte rows, optional (DLIOM_EXPAND_RUNS=1; the default is the binary search in run_index): the run index of every row, written
-// once per batch (one warp per run, contiguous stores), one 4-byte load per survivor instead of an 11-step search of the run table.
-__global__ void __launch_bounds__(kBlock) fe_expand_runs(FrontendArgs a, int32_t* __restrict__ run_of_row) {
-  const int b = blockIdx.y;
-  const int r0 = a.run_offsets[b], r1 = a.run_offsets[b + 1];
-  const int r = r0 + blockIdx.x * (kBlock / 32) + (threadIdx.x >> 5);
-  if (r >= r1) return;
-  const int n = a.counts[b];
-  const int begin = max(0, a.run_first_row[r]), end = min(n, r + 1 < r1 ? a.run_first_row[r + 1] : n);  // clamped to the scan
-  int32_t* out = run_of_row + (size_t)b * a.in_cap;
-  for (int i = begin + (threadIdx.x & 31); i < end; i += 32) out[i] = r;
-}
-
 // ---------------------------------------------------------------------------------------------------- A
-// kFirstBatch points in flight per thread (all row loads, then all claims, then the collisions): an experiment knob, see the launcher.
-template <int kFirstBatch>
-__global__ void __launch_bounds__(kBlock, kFirstBatch == 1 ? 8 : (kFirstBatch == 2 ? 6 : 5)) fe_first_filter_insert(FrontendArgs a) {
+// One point in flight per thread: the kernel runs at the L2's atomic throughput, and 2 or 4 points per thread (more outstanding
+// atomics) measured slower because they only lengthen the L2 queues.
+__global__ void __launch_bounds__(kBlock, 8) fe_first_filter_insert(FrontendArgs a) {
   const int b = a.first_scan + blockIdx.y;
   const int n = a.counts[b];
   const float* rows = a.ranges + (size_t)b * a.in_cap * a.row_floats;
@@ -100,33 +86,18 @@ __global__ void __launch_bounds__(kBlock, kFirstBatch == 1 ? 8 : (kFirstBatch ==
   const uint32_t tcap = (uint32_t)a.tcap1;  // any size (not a power of two): slot = hash * tcap >> 32
   const CellDivider res = make_divider(a.first_resolution);
   const int stride = gridDim.x * kBlock;
-  for (int i0 = blockIdx.x * kBlock + threadIdx.x; i0 < n; i0 += kFirstBatch * stride) {
-    Int3 c[kFirstBatch];
-    uint32_t h[kFirstBatch], prev[kFirstBatch];
-#pragma unroll
-    for (int u = 0; u < kFirstBatch; ++u) {
-      const int i = i0 + u * stride;
-      c[u] = cell_index(i < n ? load_xyz(rows, a.row_floats, i) : Vec3f{0.f, 0.f, 0.f}, res);
-      h[u] = table_slot(hash_cell(c[u]), tcap);
-    }
-#pragma unroll
-    for (int u = 0; u < kFirstBatch; ++u) {
-      const int i = i0 + u * stride;
-      prev[u] = i < n ? atomicCAS(tab + h[u], kEmpty32, (uint32_t)i) : kEmpty32;
-    }
-#pragma unroll
-    for (int u = 0; u < kFirstBatch; ++u) {
-      const int i = i0 + u * stride;
-      uint32_t p = prev[u], hh = h[u];
-      while (p != kEmpty32) {  // the slot has an owner: same voxel -> the lower index stays; else probe on
-        const Int3 o = cell_index(load_xyz(rows, a.row_floats, p), res);
-        if (o.x == c[u].x && o.y == c[u].y && o.z == c[u].z) {
-          if ((uint32_t)i < p) atomicMin(tab + hh, (uint32_t)i);  // the owner only ever decreases
-          break;
-        }
-        hh = hh + 1 == tcap ? 0u : hh + 1;
-        p = atomicCAS(tab + hh, kEmpty32, (uint32_t)i);
+  for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += stride) {
+    const Int3 c = cell_index(load_xyz(rows, a.row_floats, i), res);
+    uint32_t hh = table_slot(hash_cell(c), tcap);
+    uint32_t p = atomicCAS(tab + hh, kEmpty32, (uint32_t)i);
+    while (p != kEmpty32) {  // the slot has an owner: same voxel -> the lower index stays; else probe on
+      const Int3 o = cell_index(load_xyz(rows, a.row_floats, p), res);
+      if (o.x == c.x && o.y == c.y && o.z == c.z) {
+        if ((uint32_t)i < p) atomicMin(tab + hh, (uint32_t)i);  // the owner only ever decreases
+        break;
       }
+      hh = hh + 1 == tcap ? 0u : hh + 1;
+      p = atomicCAS(tab + hh, kEmpty32, (uint32_t)i);
     }
   }
 }
@@ -487,25 +458,12 @@ int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch) {
   return DL_OK;
 }
 
-int launch_fe_expand_runs(dl_context* ctx, const FrontendArgs& a, int batch, int max_runs_per_scan, int32_t* run_of_row_out) {
-  if (batch <= 0 || max_runs_per_scan <= 0) return DL_OK;
-  fe_expand_runs<<<dim3((max_runs_per_scan + kBlock / 32 - 1) / (kBlock / 32), batch), kBlock, 0, ctx->stream>>>(a, run_of_row_out);
-  DL_LAUNCH_CHECK(ctx, "fe_expand_runs");
-  return DL_OK;
-}
-
 // Kernel A for scans [first_scan, first_scan + num_scans): lets the host overlap the upload of later scans.
 int launch_fe_first_filter(dl_context* ctx, FrontendArgs a, int first_scan, int num_scans) {
   if (num_scans <= 0) return DL_OK;
   a.first_scan = first_scan;
   const int tiles = (int)std::min<int64_t>((a.cap + kBlock - 1) / kBlock, 128);
-  if (const char* env = std::getenv("DLIOM_FE_FLAGS")) a.flags = std::atoi(env);  // experiments: 1 = always CAS in the first filter
-  // points in flight per thread: 1 is the default (2 and 4 measured slower) — the kernel runs at the L2's atomic throughput, more
-  // outstanding atomics only lengthen its queues
-  const int batch_points = (a.flags & 3) == 2 ? 2 : ((a.flags & 3) == 3 ? 4 : 1);
-  if (batch_points == 1) fe_first_filter_insert<1><<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
-  else if (batch_points == 2) fe_first_filter_insert<2><<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
-  else fe_first_filter_insert<4><<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
+  fe_first_filter_insert<<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
   DL_LAUNCH_CHECK(ctx, "fe_first_filter_insert");
   return DL_OK;
 }
@@ -514,8 +472,7 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
   if (batch <= 0) return DL_OK;
   a.first_scan = first_scan;
   const int tiles = (int)std::min<int64_t>((a.cap + kBlock - 1) / kBlock, 128);
-  int per_scan = 48;  // measured best of {8, 20, 32, 48, 64}: enough CTAs in flight to hide the random-access latency
-  if (const char* env = std::getenv("DLIOM_INGEST_GRID")) per_scan = std::max(1, std::atoi(env));
+  const int per_scan = 48;  // measured best of {8, 20, 32, 48, 64}: enough CTAs in flight to hide the random-access latency
   if (a.run_pose && a.max_runs > 0) {
     fe_run_poses<<<dim3((a.max_runs + 127) / 128, batch), 128, 0, ctx->stream>>>(a);
     DL_LAUNCH_CHECK(ctx, "fe_run_poses");
@@ -534,8 +491,7 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
     DL_CUDA(ctx, cudaFuncSetAttribute(fe_emit_tracking, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     emit_attr = true;
   }
-  int parts = 4;  // CTAs per scan: a 74-scan sub-batch x 4 = 296 CTAs of 512 threads, about two per SM of an H100
-  if (const char* env = std::getenv("DLIOM_EMIT_PARTS")) parts = std::max(1, std::atoi(env));
+  const int parts = 4;  // CTAs per scan: a 74-scan sub-batch x 4 = 296 CTAs of 512 threads, about two per SM of an H100
   fe_emit_tracking<<<dim3(parts, batch), kEmitBlock, smem, ctx->stream>>>(a, max_chunks);
   DL_LAUNCH_CHECK(ctx, "fe_emit_tracking");
   return DL_OK;

@@ -49,7 +49,7 @@ struct dl_context {
   cudaStream_t stream = nullptr;
   cudaStream_t copy_stream = nullptr;   // uploads of host scans, overlapped with the kernels of the previous sub-batch
   cudaStream_t aux_stream = nullptr;    // odd sub-batches of the front end (see frontend_run)
-  cudaStream_t tail_stream = nullptr;   // high priority: the latency-bound back half (adaptive filter, LM solve) of every sub-batch
+  cudaStream_t tail_stream = nullptr;   // high priority: the front end's raw-IMU chain (pre-integration, prediction), next to the first filter
   cudaEvent_t staging_done = nullptr;   // the pinned staging block of the previous call has been consumed
   cudaEvent_t batch_done = nullptr;     // dl_frontend_submit: everything of the batch in flight, incl. the result download
   // adaptive voxel filter: how many (cloud, filter) pairs of the last probed launch needed the single-CTA search
@@ -171,14 +171,14 @@ struct StageScope {
   }
 };
 
-struct Arena {  // bump allocator over the context's device scratch
+struct Arena {  // bump allocator over the context's device scratch; with a null base it only counts (`off` = bytes taken)
   char* base;
   size_t off = 0;
   explicit Arena(void* p) : base((char*)p) {}
   template <typename T>
   T* take(size_t count) {
     off = (off + 255) & ~size_t(255);
-    T* p = (T*)(base + off);
+    T* p = base ? (T*)(base + off) : nullptr;
     off += count * sizeof(T);
     return p;
   }

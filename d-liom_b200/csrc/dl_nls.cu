@@ -21,7 +21,6 @@
 // mix exactly, so the piecewise-polynomial pieces are the same ones the CPU path picks.
 //
 // Algorithmic bytes: 12 B point + 8 corners * 2 B = 28 B per point per evaluation (SURVEY 8d).
-#include <cstdlib>
 #include <type_traits>
 
 #include <cooperative_groups.h>
@@ -878,25 +877,15 @@ __global__ void grid_lookup_kernel(GridView g, int64_t n, const int32_t* __restr
 
 }  // namespace
 
-// Threads per problem (multiple of 32, <= kBlock). DLIOM_NLS_BLOCK overrides for experiments.
-static int nls_block_threads() {
-  static const int threads = [] {
-    int t = kBlock;  // fewer threads per ~400-point problem measured slower: the evaluation pass serialises inside a thread
-    if (const char* env = std::getenv("DLIOM_NLS_BLOCK")) t = std::atoi(env);
-    t = (t / 32) * 32;
-    return t < 32 ? 32 : (t > kBlock ? kBlock : t);
-  }();
-  return threads;
-}
-
-// One CTA per problem, or opt.cluster CTAs (a thread-block cluster) per problem. The kernels find their problem as
-// blockIdx.x / cluster size.
+// One CTA of kBlock threads per problem, or opt.cluster CTAs (a thread-block cluster) per problem. The kernels find their
+// problem as blockIdx.x / cluster size. (Fewer threads per ~400-point problem measured slower: the evaluation pass serialises
+// inside a thread.)
 template <typename Kernel, typename... Args>
 static cudaError_t launch_solve(Kernel kernel, const NlsOptions& opt, int count, cudaStream_t stream, Args... args) {
   const int cs = opt.cluster > 1 ? opt.cluster : 1;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(count * cs));
-  cfg.blockDim = dim3((unsigned)(cs > 1 ? kBlock : nls_block_threads()));
+  cfg.blockDim = dim3((unsigned)kBlock);
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;

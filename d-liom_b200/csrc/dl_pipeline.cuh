@@ -74,12 +74,10 @@ struct FrontendArgs {
   const int32_t* run_offsets;    // row_floats == 3: per-point times as runs (dl_frontend_options::time_run_*), device copies
   const int32_t* run_first_row;
   const float* run_value;
-  const int32_t* run_of_row;     // optional: the run index of every row (scan b at b * in_cap); null = search the runs
-  float* run_pose;               // optional (with run_of_row): deskew pose of every run, 8 floats (t xyz, q wxyz, pad), fe_run_poses
+  float* run_pose;               // optional: deskew pose of every run, 8 floats (t xyz, q wxyz, pad), fe_run_poses
   int max_runs;                  // most runs any scan of the batch has
   int64_t in_cap;
   int row_floats;
-  int flags;             // experiment switches (DLIOM_FE_FLAGS), 0 = defaults
   int first_scan;        // kernels handle scans [first_scan, first_scan + gridDim.y): lets sub-batches pipeline
   const int32_t* counts;
   const ScanConstants* scans;
@@ -102,7 +100,6 @@ struct FrontendArgs {
   int32_t* error_flag;            // one per scan
 };
 int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch);
-int launch_fe_expand_runs(dl_context* ctx, const FrontendArgs& a, int batch, int max_runs_per_scan, int32_t* run_of_row_out);
 int launch_fe_first_filter(dl_context* ctx, FrontendArgs a, int first_scan, int num_scans);
 int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch);
 

@@ -817,7 +817,7 @@ int launch_adaptive_voxel_filter(dl_context* ctx, const float* points, int strid
   // The grid-wide first pass keeps its keys + min indices in the head of each pair's table region (the single-CTA search only
   // touches that region afterwards, for its own pair) and its winner bytes, tile counts and bookkeeping in first_pass_scratch
   // (adaptive_first_pass_bytes). Tables too small for it (tiny clouds) go straight to the single-CTA search.
-  bool first_pass = first_pass_scratch && (size_t)table_cap * 4 >= (size_t)kEdgeSlots * 12 && !std::getenv("DLIOM_ADAPTIVE_SINGLE_CTA");
+  bool first_pass = first_pass_scratch && (size_t)table_cap * 4 >= (size_t)kEdgeSlots * 12;
   // Self-tuning: the grid-wide pass only pays when the first edge usually suffices. The share of pairs that fell through to the
   // single-CTA search in the last probed launch is read from a pinned counter (no synchronisation: a stale or half-updated
   // value only changes which of two exact paths runs); when most pairs fall through, skip the pass and re-probe every 16th call.
