@@ -82,18 +82,6 @@ int h2d(dl_context* ctx, T* dst, const T* src, size_t count) {
   DL_CUDA(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
   return DL_OK;
 }
-template <typename T>
-int ensure_capacity(dl_context* ctx, T** ptr, size_t* cap, size_t need) {
-  if (need <= *cap) return DL_OK;
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (*ptr) DL_CUDA(ctx, cudaFree(*ptr));
-  *ptr = nullptr;
-  const size_t want = need + need / 2 + 512;
-  DL_CUDA(ctx, cudaMalloc((void**)ptr, want * sizeof(T)));
-  *cap = want;
-  return DL_OK;
-}
-
 // (Re)allocates a pool to at least `need` elements, preserving the first `used` elements and initialising the rest
 // with `fill` bytes: free node slots must read -1 and free brick slots 0 for the lock-free device-side growth.
 template <typename T>
@@ -401,10 +389,12 @@ int dl_grid_lookup(dl_context* ctx, const dl_grid* g, int64_t n, const int32_t* 
   if (!ctx || !g || n < 0 || (n > 0 && (!xyz || !value_out))) return DL_ERR_ARG;
   if (g->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * 12, (size_t)n * 2})));
-  Arena a(ctx->d_scratch);
-  int32_t* d_xyz = a.take<int32_t>(3 * n);
-  uint16_t* d_out = a.take<uint16_t>(n);
+  int32_t* d_xyz;
+  uint16_t* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_xyz = a.take<int32_t>(3 * n);
+    d_out = a.take<uint16_t>(n);
+  }));
   DL_TRY(h2d(ctx, d_xyz, xyz, 3 * n));
   DL_TRY(launch_grid_lookup(ctx, g->view(), n, d_xyz, d_out));
   DL_TRY(d2h(ctx, value_out, d_out, n));
@@ -415,10 +405,11 @@ int dl_grid_interpolate(dl_context* ctx, const dl_grid* g, int64_t n, const doub
   if (!ctx || !g || n < 0 || (n > 0 && (!xyz || !out))) return DL_ERR_ARG;
   if (g->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * 24, (size_t)n * 32})));
-  Arena a(ctx->d_scratch);
-  double* d_xyz = a.take<double>(3 * n);
-  double* d_out = a.take<double>(4 * n);
+  double *d_xyz, *d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_xyz = a.take<double>(3 * n);
+    d_out = a.take<double>(4 * n);
+  }));
   DL_TRY(h2d(ctx, d_xyz, xyz, 3 * n));
   DL_TRY(launch_interpolate(ctx, g->view(), n, d_xyz, d_out));
   DL_TRY(d2h(ctx, out, d_out, 4 * n));
@@ -455,7 +446,13 @@ struct InsertScratch {
   int32_t* bbox;
   uint32_t* update_list;
 };
-int prepare_insert(dl_context* ctx, Arena& a, const dl_range_data_inserter_options& o, int64_t n, InsertScratch* s) {
+void carve_insert(Arena& a, const dl_range_data_inserter_options& o, int64_t n, InsertScratch* s) {
+  s->hit_table = a.take<uint16_t>(32768);
+  s->miss_table = a.take<uint16_t>(32768);
+  s->bbox = a.take<int32_t>(8);
+  s->update_list = a.take<uint32_t>((size_t)n * (size_t)(1 + std::max(o.num_free_space_voxels, 0)));
+}
+int upload_odds_tables(dl_context* ctx, const dl_range_data_inserter_options& o, const InsertScratch& s) {
   static thread_local std::vector<uint16_t> tables(65536);
   static thread_local double cached_hit = -1, cached_miss = -1;
   if (cached_hit != o.hit_probability || cached_miss != o.miss_probability) {
@@ -464,16 +461,9 @@ int prepare_insert(dl_context* ctx, Arena& a, const dl_range_data_inserter_optio
     cached_hit = o.hit_probability;
     cached_miss = o.miss_probability;
   }
-  s->hit_table = a.take<uint16_t>(32768);
-  s->miss_table = a.take<uint16_t>(32768);
-  s->bbox = a.take<int32_t>(8);
-  s->update_list = a.take<uint32_t>((size_t)n * (size_t)(1 + std::max(o.num_free_space_voxels, 0)));
-  DL_TRY(h2d(ctx, s->hit_table, tables.data(), 32768));
-  DL_TRY(h2d(ctx, s->miss_table, tables.data() + 32768, 32768));
+  DL_TRY(h2d(ctx, s.hit_table, tables.data(), 32768));
+  DL_TRY(h2d(ctx, s.miss_table, tables.data() + 32768, 32768));
   return DL_OK;
-}
-size_t insert_scratch_bytes(const dl_range_data_inserter_options& o, int64_t n) {
-  return arena_bytes({65536, 65536, 64, (size_t)n * (size_t)(1 + std::max(o.num_free_space_voxels, 0)) * 4});
 }
 int check_inserter(dl_context* ctx, const dl_range_data_inserter_options* o) {
   if (!o) return DL_ERR_ARG;
@@ -491,12 +481,14 @@ int dl_grid_insert_range_data(dl_context* ctx, dl_grid* grid, const dl_range_dat
   DL_TRY(check_inserter(ctx, options));
   if (n == 0) return DL_OK;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * 12}) + insert_scratch_bytes(*options, n)));
-  Arena a(ctx->d_scratch);
-  float* d_returns = a.take<float>(3 * n);
-  DL_TRY(h2d(ctx, d_returns, returns, 3 * n));
+  float* d_returns;
   InsertScratch s;
-  DL_TRY(prepare_insert(ctx, a, *options, n, &s));
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_returns = a.take<float>(3 * n);
+    carve_insert(a, *options, n, &s);
+  }));
+  DL_TRY(h2d(ctx, d_returns, returns, 3 * n));
+  DL_TRY(upload_odds_tables(ctx, *options, s));
   DL_TRY(grid_insert_device(ctx, grid, Vec3f{origin[0], origin[1], origin[2]}, d_returns, (int)n,
                             options->num_free_space_voxels, s.hit_table, s.miss_table, s.bbox, s.update_list));
   return sync(ctx);
@@ -510,14 +502,17 @@ int dl_submap_insert_range_data(dl_context* ctx, dl_grid* hi, dl_grid* lo, const
   if (n == 0) return DL_OK;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t tiles = (size_t)(n + 255) / 256;
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * 12, (size_t)n * 12, (size_t)n * 12, 64, tiles * 4}) +
-                             insert_scratch_bytes(*options, n)));
-  Arena a(ctx->d_scratch);
-  float* d_in = a.take<float>(3 * n);
-  float* d_all = a.take<float>(3 * n);
-  float* d_near = a.take<float>(3 * n);
-  int32_t* d_near_count = a.take<int32_t>(1);
-  int32_t* d_tiles = a.take<int32_t>(tiles);
+  float *d_in, *d_all, *d_near;
+  int32_t *d_near_count, *d_tiles;
+  InsertScratch s;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_in = a.take<float>(3 * n);
+    d_all = a.take<float>(3 * n);
+    d_near = a.take<float>(3 * n);
+    d_near_count = a.take<int32_t>(1);
+    d_tiles = a.take<int32_t>(tiles);
+    carve_insert(a, *options, n, &s);
+  }));
   DL_TRY(h2d(ctx, d_in, returns, 3 * n));
   // TransformRangeData(range_data, local_pose().inverse().cast<float>())
   const Rigidf to_submap = to_float(inverse(pose_from7(submap_local_pose)));
@@ -527,8 +522,7 @@ int dl_submap_insert_range_data(dl_context* ctx, dl_grid* hi, dl_grid* lo, const
   int32_t near_count = 0;
   DL_TRY(d2h(ctx, &near_count, d_near_count, 1));
   DL_TRY(sync(ctx));
-  InsertScratch s;
-  DL_TRY(prepare_insert(ctx, a, *options, n, &s));
+  DL_TRY(upload_odds_tables(ctx, *options, s));
   DL_TRY(grid_insert_device(ctx, hi, origin_submap, d_near, near_count, options->num_free_space_voxels, s.hit_table,
                             s.miss_table, s.bbox, s.update_list));
   DL_TRY(grid_insert_device(ctx, lo, origin_submap, d_all, (int)n, options->num_free_space_voxels, s.hit_table, s.miss_table,
@@ -569,10 +563,12 @@ int dl_grid_export_cells(dl_grid* g, int64_t capacity, int32_t* xs, int32_t* ys,
 int dl_voxel_indices(dl_context* ctx, const float* points, int64_t n, int stride, float resolution, int32_t* out) {
   if (!ctx || n < 0 || stride < 3 || !(resolution > 0.f) || (n > 0 && (!points || !out))) return DL_ERR_ARG;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * stride * 4, (size_t)n * 12})));
-  Arena a(ctx->d_scratch);
-  float* d_pts = a.take<float>(n * stride);
-  int32_t* d_out = a.take<int32_t>(3 * n);
+  float* d_pts;
+  int32_t* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(n * stride);
+    d_out = a.take<int32_t>(3 * n);
+  }));
   DL_TRY(h2d(ctx, d_pts, points, n * stride));
   DL_TRY(launch_voxel_indices(ctx, d_pts, stride, n, resolution, d_out));
   DL_TRY(d2h(ctx, out, d_out, 3 * n));
@@ -589,15 +585,17 @@ int dl_voxel_filter(dl_context* ctx, const float* points, int64_t n, int stride,
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const int64_t tcap = next_pow2(2 * n);
   const int tiles = (int)((n + 255) / 256);
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * stride * 4, (size_t)tcap * 4, (size_t)n * 4, (size_t)n * 4,
-                                          (size_t)tiles * 4, 64})));
-  Arena a(ctx->d_scratch);
-  float* d_pts = a.take<float>(n * stride);
-  uint32_t* d_table = a.take<uint32_t>(tcap);
-  uint32_t* d_slot = a.take<uint32_t>(n);
-  int32_t* d_keep = a.take<int32_t>(n);
-  int32_t* d_blocks = a.take<int32_t>(tiles);
-  int32_t* d_counts = a.take<int32_t>(2);  // [0] = n, [1] = survivors
+  float* d_pts;
+  uint32_t *d_table, *d_slot;
+  int32_t *d_keep, *d_blocks, *d_counts;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(n * stride);
+    d_table = a.take<uint32_t>(tcap);
+    d_slot = a.take<uint32_t>(n);
+    d_keep = a.take<int32_t>(n);
+    d_blocks = a.take<int32_t>(tiles);
+    d_counts = a.take<int32_t>(2);  // [0] = n, [1] = survivors
+  }));
   const int32_t n32 = (int32_t)n;
   DL_TRY(h2d(ctx, d_pts, points, n * stride));
   DL_TRY(h2d(ctx, d_counts, &n32, 1));
@@ -624,17 +622,21 @@ int dl_adaptive_voxel_filter(dl_context* ctx, const dl_adaptive_voxel_filter_opt
   if (n > 0x7fffffff) return ctx->fail(DL_ERR_ARG, "more than 2^31-1 points");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const int64_t tcap = next_pow2(2 * n);
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * stride * 4, (size_t)tcap * 4, (size_t)n * 8, (size_t)n * 4,
-                                          adaptive_first_pass_bytes(1, n), 64, sizeof(AdaptiveParams), 32 * 4, 64})));
-  Arena a(ctx->d_scratch);
-  float* d_pts = a.take<float>(n * stride);
-  uint32_t* d_table = a.take<uint32_t>(tcap);
-  uint32_t* d_scratch = a.take<uint32_t>(2 * n);
-  int32_t* d_keep = a.take<int32_t>(n);
-  uint8_t* d_first = a.take<uint8_t>(adaptive_first_pass_bytes(1, n));
-  int32_t* d_counts = a.take<int32_t>(3);  // n, survivors, passes
-  AdaptiveParams* d_params = a.take<AdaptiveParams>(1);
-  float* d_passes = a.take<float>(32);
+  float *d_pts, *d_passes;
+  uint32_t *d_table, *d_scratch;
+  int32_t *d_keep, *d_counts;
+  uint8_t* d_first;
+  AdaptiveParams* d_params;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(n * stride);
+    d_table = a.take<uint32_t>(tcap);
+    d_scratch = a.take<uint32_t>(2 * n);
+    d_keep = a.take<int32_t>(n);
+    d_first = a.take<uint8_t>(adaptive_first_pass_bytes(1, n));
+    d_counts = a.take<int32_t>(3);  // n, survivors, passes
+    d_params = a.take<AdaptiveParams>(1);
+    d_passes = a.take<float>(32);
+  }));
   const int32_t n32 = (int32_t)n;
   const AdaptiveParams params{options->max_length, options->min_num_points, options->max_range};
   DL_TRY(h2d(ctx, d_pts, points, n * stride));
@@ -824,8 +826,10 @@ int rtcsm_device(dl_context* ctx, const dl_rtcsm_options& opt, const Rigidd& ini
   return DL_OK;
 }
 
-// Upper bound of the scratch rtcsm_device needs, from the options alone (max range <= farthest possible point is
-// unknown before the reduction, so bound the angular window by the window / smallest possible step).
+// Upper bound of the scratch rtcsm_device takes for one cloud, from the options alone. This is the one reservation that cannot
+// be counted from a carve: the candidate tables' size follows from the cloud's farthest point, which a device reduction finds
+// in the middle of the call, when the scratch already holds the call's inputs and cannot grow. So the angular window is
+// bounded by the window / smallest possible step. rtcsm_batch_device checks the bound before it uploads the tables.
 size_t rtcsm_scratch_bound(const dl_rtcsm_options& opt, float resolution, bool scores) {
   const int L1 = 2 * (int)std::lround(opt.linear_search_window / resolution) + 1;
   // step >= 0.999 * acos(1 - res^2 / (2 r^2)) with r <= 200 m (beyond any LiDAR the front end accepts)
@@ -833,7 +837,13 @@ size_t rtcsm_scratch_bound(const dl_rtcsm_options& opt, float resolution, bool s
   const float step = 0.999f * std::acos(1.f - (resolution * resolution) / (2.f * r * r));
   const int A1 = 2 * (int)std::lround(opt.angular_search_window / step) + 1;
   const size_t R = (size_t)A1 * A1 * A1, L = (size_t)L1 * L1 * L1;
-  return arena_bytes({64, 64, R * 16 + L * 12 + R * 8 + L * 8 + 256 + sizeof(RtcsmScan) + 64, 64, scores ? R * L * 4 : 0}) + 4096;
+  Arena bound(nullptr);  // rtcsm_device's takes at the largest tables, with room for the blob's 16-byte alignment
+  bound.take<float>(1);
+  bound.take<int32_t>(1);
+  bound.take<float>(scores ? R * L : 0);
+  bound.take<unsigned char>(R * 16 + L * 12 + R * 8 + L * 8 + 256 + sizeof(RtcsmScan) + 64);
+  bound.take<unsigned long long>(1);
+  return bound.off + 4096;
 }
 
 }  // namespace
@@ -847,9 +857,10 @@ int dl_rtcsm_match(dl_context* ctx, const dl_rtcsm_options* options, const doubl
   if (n == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
   if (grid->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * 12}) + rtcsm_scratch_bound(*options, grid->resolution, all_scores != nullptr)));
-  Arena a(ctx->d_scratch);
-  float* d_pts = a.take<float>(3 * n);
+  float* d_pts;
+  Arena a(nullptr);
+  DL_TRY(carve_scratch(ctx, [&](Arena& c) { d_pts = c.take<float>(3 * n); },
+                       rtcsm_scratch_bound(*options, grid->resolution, all_scores != nullptr), &a));
   DL_TRY(h2d(ctx, d_pts, points, 3 * n));
   Rigidd best;
   DL_TRY(rtcsm_device(ctx, *options, pose_from7(initial_pose), d_pts, n, grid, a, &best, score_out, info, all_scores));
@@ -890,33 +901,33 @@ int dl_ceres_match_batch(dl_context* ctx, const dl_ceres_options* options, int32
     return DL_ERR_ARG;
   if (count == 0) return DL_OK;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  size_t total_points = 0;
   for (int i = 0; i < count * num_pairs; ++i) {
     if (sizes[i] < 0 || !grids[i] || (sizes[i] > 0 && !clouds[i])) return DL_ERR_ARG;
     if (sizes[i] == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
     if (grids[i]->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
-    total_points += (size_t)sizes[i];
   }
-  DL_TRY(ctx->reserve_device(arena_bytes({total_points * 12 + (size_t)count * num_pairs * 256,
-                                          (size_t)count * sizeof(NlsProblem), (size_t)count * sizeof(NlsOutput)})));
-  Arena a(ctx->d_scratch);
+  std::vector<float*> d_clouds(count * num_pairs);
+  NlsProblem* d_problems;
+  NlsOutput* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    for (int i = 0; i < count * num_pairs; ++i) d_clouds[i] = a.take<float>(3 * sizes[i]);
+    d_problems = a.take<NlsProblem>(count);
+    d_out = a.take<NlsOutput>(count);
+  }));
   std::vector<NlsProblem> problems(count);
   for (int c = 0; c < count; ++c) {
     NlsProblem& p = problems[c];
     std::memset(&p, 0, sizeof(p));
     for (int k = 0; k < num_pairs; ++k) {
       const int i = c * num_pairs + k;
-      float* d = a.take<float>(3 * sizes[i]);
-      DL_TRY(h2d(ctx, d, clouds[i], 3 * sizes[i]));
-      p.cloud[k] = d;
+      DL_TRY(h2d(ctx, d_clouds[i], clouds[i], 3 * sizes[i]));
+      p.cloud[k] = d_clouds[i];
       p.count[k] = (int32_t)sizes[i];
       p.grid[k] = grids[i]->view();
     }
     for (int j = 0; j < 3; ++j) p.target_t[j] = target_translations[3 * c + j];
     for (int j = 0; j < 7; ++j) p.initial[j] = initial_poses[7 * c + j];
   }
-  NlsProblem* d_problems = a.take<NlsProblem>(count);
-  NlsOutput* d_out = a.take<NlsOutput>(count);
   DL_TRY(h2d(ctx, d_problems, problems.data(), count));
   DL_TRY(launch_nls(ctx, to_nls_options(*options, num_pairs), d_problems, count, d_out));
   std::vector<NlsOutput> out(count);
@@ -945,24 +956,25 @@ int dl_ceres_normal_equations(dl_context* ctx, const dl_ceres_options* options, 
   if (!target_translation || !reference_pose || !at_pose || !clouds || !sizes || !grids || !cost || !gradient6 || !hessian36)
     return DL_ERR_ARG;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  size_t total_points = 0;
-  for (int i = 0; i < num_pairs; ++i) total_points += (size_t)sizes[i];
-  DL_TRY(ctx->reserve_device(arena_bytes({total_points * 12 + (size_t)num_pairs * 256, sizeof(NlsProblem), 64, 28 * 8})));
-  Arena a(ctx->d_scratch);
+  float* d_clouds[DL_MAX_PAIRS];
+  NlsProblem* d_p;
+  double *d_at, *d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    for (int k = 0; k < num_pairs; ++k) d_clouds[k] = a.take<float>(3 * sizes[k]);
+    d_p = a.take<NlsProblem>(1);
+    d_at = a.take<double>(7);
+    d_out = a.take<double>(28);
+  }));
   NlsProblem p;
   std::memset(&p, 0, sizeof(p));
   for (int k = 0; k < num_pairs; ++k) {
-    float* d = a.take<float>(3 * sizes[k]);
-    DL_TRY(h2d(ctx, d, clouds[k], 3 * sizes[k]));
-    p.cloud[k] = d;
+    DL_TRY(h2d(ctx, d_clouds[k], clouds[k], 3 * sizes[k]));
+    p.cloud[k] = d_clouds[k];
     p.count[k] = (int32_t)sizes[k];
     p.grid[k] = grids[k]->view();
   }
   for (int j = 0; j < 3; ++j) p.target_t[j] = target_translation[j];
   for (int j = 0; j < 7; ++j) p.initial[j] = reference_pose[j];
-  NlsProblem* d_p = a.take<NlsProblem>(1);
-  double* d_at = a.take<double>(7);
-  double* d_out = a.take<double>(28);
   DL_TRY(h2d(ctx, d_p, &p, 1));
   DL_TRY(h2d(ctx, d_at, at_pose, 7));
   DL_TRY(launch_nls_normal_equations(ctx, to_nls_options(*options, num_pairs), d_p, d_at, d_out));
@@ -983,9 +995,15 @@ int dl_ceres_normal_equations(dl_context* ctx, const dl_ceres_options* options, 
 // ------------------------------------------------------------------------------------------------ loop closure
 namespace {
 struct CoarseSearch {  // device state of one chunk of (node, submap) pairs
+  bool pruned;     // pruned search (plan_coarse); otherwise exhaustive
+  int max_blocks;  // most pruning blocks of any pair of the chunk (pruned search)
+  float *d_hi, *d_lo;  // uploaded clouds (null when device-resident)
+  int* d_cells;
+  float* d_rot;
   FcsmPair* d_pairs;
   FcsmPick* d_picks;
   unsigned long long* d_best;
+  int *d_bounds, *d_max_bound;  // pruned search only
   std::vector<const float*> hi, lo;  // per pair of the chunk: its clouds on the device (uploaded or resident)
 };
 int check_fcsm_options(dl_context* ctx, const dl_fcsm_options& o) {
@@ -1048,44 +1066,73 @@ int ensure_search_index(dl_context* ctx, dl_grid* g, bool* have) {
   return DL_OK;
 }
 
-// Runs the coarse search for pairs [first, first + n), uploading their clouds first unless they are device-resident; leaves the
-// picks on the device.
-int coarse_search(dl_context* ctx, Arena& a, const dl_fcsm_options& o, float min_score, int first, int n, const double* guesses,
-                  const PairClouds& pc, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, float* d_all_scores,
-                  CoarseSearch* out) {
+// Window half-widths in cells of a search in `hi` (double / float -> double, common::RoundToInt, cc:174-176).
+void search_window(const dl_fcsm_options& o, const dl_grid* hi, int* wxy, int* wz) {
+  *wxy = (int)std::lround(o.linear_xy_search_window / hi->resolution);
+  *wz = (int)std::lround(o.linear_z_search_window / hi->resolution);
+}
+// Decides, before the scratch is carved, whether pairs [first, first + n) get the pruned search and how many pruning blocks
+// its bounds table needs per pair. The pruned search needs the index of every high-resolution grid of the chunk
+// (DLIOM_FCSM_EXHAUSTIVE=1 forces the fallback) and at most 60 000 blocks per pair (one CTA per block and pair in grid.x).
+int plan_coarse(dl_context* ctx, const dl_fcsm_options& o, int first, int n, const dl_grid* const* hi_grids, CoarseSearch* cs) {
+  cs->pruned = std::getenv("DLIOM_FCSM_EXHAUSTIVE") == nullptr;
+  cs->max_blocks = 1;
+  for (int k = 0; k < n && cs->pruned; ++k) {
+    bool have = false;
+    DL_TRY(ensure_search_index(ctx, const_cast<dl_grid*>(hi_grids[first + k]), &have));
+    cs->pruned = have;
+  }
+  for (int k = 0; k < n; ++k) {
+    int wxy, wz;
+    search_window(o, hi_grids[first + k], &wxy, &wz);
+    const long long side = 2ll * wxy + 1, K = side * side * (2ll * wz + 1);
+    if (K >= 0xFFFFFFFFll) return ctx->fail(DL_ERR_ARG, "more than 2^32-1 translation candidates");
+    if (cs->pruned) {
+      const long long bxy = (side + 7) / 8, bz = (2ll * wz + 1 + 7) / 8;
+      if (bxy * bxy * bz > 60000) cs->pruned = false;
+      cs->max_blocks = (int)std::max<long long>(cs->max_blocks, bxy * bxy * bz);
+    }
+  }
+  return DL_OK;
+}
+// The device buffers of the coarse search of pairs [first, first + n), as plan_coarse decided it.
+void carve_coarse(Arena& a, const PairClouds& pc, int first, int n, CoarseSearch* cs) {
+  const int64_t n_hi = pc.hi_off[first + n] - pc.hi_off[first], n_lo = pc.lo_off[first + n] - pc.lo_off[first];
+  const bool resident = pc.hi_store != nullptr;
+  cs->d_hi = resident ? nullptr : a.take<float>(3 * n_hi);
+  cs->d_lo = resident ? nullptr : a.take<float>(3 * n_lo);
+  cs->d_cells = a.take<int>(3 * n_hi);
+  cs->d_rot = a.take<float>(3 * n_lo);
+  cs->d_pairs = a.take<FcsmPair>(n);
+  cs->d_picks = a.take<FcsmPick>(n);
+  cs->d_best = a.take<unsigned long long>(n);
+  cs->d_bounds = cs->pruned ? a.take<int>((size_t)n * cs->max_blocks) : nullptr;
+  cs->d_max_bound = cs->pruned ? a.take<int>(n) : nullptr;
+}
+
+// Runs the coarse search for pairs [first, first + n) in the buffers carve_coarse took, uploading their clouds first unless they
+// are device-resident; leaves the picks on the device.
+int coarse_search(dl_context* ctx, const dl_fcsm_options& o, float min_score, int first, int n, const double* guesses,
+                  const PairClouds& pc, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, CoarseSearch* out) {
   const int64_t* hi_off = pc.hi_off;
   const int64_t* lo_off = pc.lo_off;
   const int64_t hi0 = hi_off[first], lo0 = lo_off[first];
   const int64_t n_hi = hi_off[first + n] - hi0, n_lo = lo_off[first + n] - lo0;
   const bool resident = pc.hi_store != nullptr;
-  float* d_hi = resident ? nullptr : a.take<float>(3 * n_hi);
-  float* d_lo = resident ? nullptr : a.take<float>(3 * n_lo);
-  int* d_cells = a.take<int>(3 * n_hi);
-  float* d_rot = a.take<float>(3 * n_lo);
-  out->d_pairs = a.take<FcsmPair>(n);
-  out->d_picks = a.take<FcsmPick>(n);
-  out->d_best = a.take<unsigned long long>(n);
   out->hi.resize(n);
   out->lo.resize(n);
   for (int k = 0; k < n; ++k) {
     const int g = first + k;
-    out->hi[k] = resident ? pc.hi_store + 3 * pc.hi_begin[g] : d_hi + 3 * (hi_off[g] - hi0);
-    out->lo[k] = resident ? pc.lo_store + 3 * pc.lo_begin[g] : d_lo + 3 * (lo_off[g] - lo0);
+    out->hi[k] = resident ? pc.hi_store + 3 * pc.hi_begin[g] : out->d_hi + 3 * (hi_off[g] - hi0);
+    out->lo[k] = resident ? pc.lo_store + 3 * pc.lo_begin[g] : out->d_lo + 3 * (lo_off[g] - lo0);
   }
   if (!resident) {
-    DL_TRY(h2d(ctx, d_hi, pc.hi_pts + 3 * hi0, 3 * n_hi));
-    DL_TRY(h2d(ctx, d_lo, pc.lo_pts + 3 * lo0, 3 * n_lo));
+    DL_TRY(h2d(ctx, out->d_hi, pc.hi_pts + 3 * hi0, 3 * n_hi));
+    DL_TRY(h2d(ctx, out->d_lo, pc.lo_pts + 3 * lo0, 3 * n_lo));
   }
   std::vector<FcsmPair> pairs(n);
-  int max_points = 1, max_blocks = 1;
+  int max_points = 1;
   long long max_candidates = 1;
-  // pruned search needs the index of every high-resolution grid of the chunk (DLIOM_FCSM_EXHAUSTIVE=1 forces the fallback)
-  bool pruned = std::getenv("DLIOM_FCSM_EXHAUSTIVE") == nullptr && d_all_scores == nullptr;
-  for (int k = 0; k < n && pruned; ++k) {
-    bool have = false;
-    DL_TRY(ensure_search_index(ctx, const_cast<dl_grid*>(hi_grids[first + k]), &have));
-    pruned = have;
-  }
   for (int k = 0; k < n; ++k) {
     const int g = first + k;
     FcsmPair& p = pairs[k];
@@ -1094,39 +1141,29 @@ int coarse_search(dl_context* ctx, Arena& a, const dl_fcsm_options& o, float min
     p.lo = lo_grids[g]->view();
     p.hi_pts = out->hi[k];
     p.lo_pts = out->lo[k];
-    p.cells = d_cells + 3 * (hi_off[g] - hi0);
-    p.lo_rot = d_rot + 3 * (lo_off[g] - lo0);
+    p.cells = out->d_cells + 3 * (hi_off[g] - hi0);
+    p.lo_rot = out->d_rot + 3 * (lo_off[g] - lo0);
     p.n_hi = (int)(hi_off[g + 1] - hi_off[g]);
     p.n_lo = (int)(lo_off[g + 1] - lo_off[g]);
     p.pose = to_float(pose_from7(guesses + 7 * g));
-    const float res = hi_grids[g]->resolution;
-    p.wxy = (int)std::lround(o.linear_xy_search_window / res);  // double / float -> double, common::RoundToInt (cc:174-176)
-    p.wz = (int)std::lround(o.linear_z_search_window / res);
+    search_window(o, hi_grids[g], &p.wxy, &p.wz);
     p.min_score = min_score;
     p.min_low = o.min_low_resolution_score;
-    const long long side = 2ll * p.wxy + 1, K = side * side * (2ll * p.wz + 1);
-    if (K >= 0xFFFFFFFFll) return ctx->fail(DL_ERR_ARG, "more than 2^32-1 translation candidates");
-    if (pruned) {
+    if (out->pruned) {
       p.m8 = hi_grids[g]->d_m8;
       for (int a3 = 0; a3 < 3; ++a3) { p.m8_org[a3] = hi_grids[g]->m8_org[a3]; p.m8_dim[a3] = hi_grids[g]->m8_dim[a3]; }
-      const long long bxy = (side + 7) / 8, bz = (2ll * p.wz + 1 + 7) / 8;
-      if (bxy * bxy * bz > 60000) pruned = false;  // one CTA per block and pair in grid.x
-      max_blocks = (int)std::max<long long>(max_blocks, bxy * bxy * bz);
     }
+    const long long side = 2ll * p.wxy + 1;
     max_candidates = std::max(max_candidates, side * (2ll * p.wz + 1) * ((side + kFcsmRun - 1) / kFcsmRun));  // search threads
     max_points = std::max(max_points, std::max(p.n_hi, p.n_lo));
   }
-  if (!pruned)
-    for (FcsmPair& p : pairs) p.m8 = nullptr;
   DL_TRY(h2d(ctx, out->d_pairs, pairs.data(), n));
   DL_TRY(sync(ctx));  // `pairs` is pageable host memory
   StageScope st(ctx, "loop_closure_search");
-  if (pruned) {
-    int* d_bounds = a.take<int>((size_t)n * max_blocks);
-    int* d_max_bound = a.take<int>(n);
-    return launch_fcsm_pruned(ctx, out->d_pairs, n, max_points, max_blocks, d_bounds, d_max_bound, out->d_best, out->d_picks);
-  }
-  return launch_fcsm(ctx, out->d_pairs, n, max_points, max_candidates, out->d_best, out->d_picks, d_all_scores);
+  if (out->pruned)
+    return launch_fcsm_pruned(ctx, out->d_pairs, n, max_points, out->max_blocks, out->d_bounds, out->d_max_bound, out->d_best,
+                              out->d_picks);
+  return launch_fcsm(ctx, out->d_pairs, n, max_points, max_candidates, out->d_best, out->d_picks, nullptr);
 }
 int check_pairs(dl_context* ctx, int count, const double* guesses, const float* hi_pts, const int64_t* hi_off, const float* lo_pts,
                 const int64_t* lo_off, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids) {
@@ -1139,10 +1176,6 @@ int check_pairs(dl_context* ctx, int count, const double* guesses, const float* 
       return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
   }
   return DL_OK;
-}
-size_t coarse_bytes(int64_t n_hi, int64_t n_lo, int n) {
-  return arena_bytes({(size_t)n_hi * 12, (size_t)n_lo * 12, (size_t)n_hi * 12, (size_t)n_lo * 12, (size_t)n * sizeof(FcsmPair),
-                      (size_t)n * sizeof(FcsmPick), (size_t)n * 8, (size_t)n * 60000 * 4, (size_t)n * 4});
 }
 }  // namespace
 
@@ -1157,15 +1190,15 @@ int dl_fcsm_match_3dof(dl_context* ctx, const dl_fcsm_options* o, const double* 
   DL_TRY(check_pairs(ctx, 1, guess, hi_pts, hi_off, lo_pts, lo_off, &hi, &lo));
   DL_TRY(check_fcsm_options(ctx, *o));
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(coarse_bytes(n_hi, n_lo, 1)));
-  Arena a(ctx->d_scratch);
   CoarseSearch cs;
   PairClouds pc;
   pc.hi_pts = hi_pts;
   pc.lo_pts = lo_pts;
   pc.hi_off = hi_off;
   pc.lo_off = lo_off;
-  DL_TRY(coarse_search(ctx, a, *o, min_score, 0, 1, guess, pc, &hi, &lo, nullptr, &cs));
+  DL_TRY(plan_coarse(ctx, *o, 0, 1, &hi, &cs));
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) { carve_coarse(a, pc, 0, 1, &cs); }));
+  DL_TRY(coarse_search(ctx, *o, min_score, 0, 1, guess, pc, &hi, &lo, &cs));
   FcsmPick pick;
   DL_TRY(d2h(ctx, &pick, cs.d_picks, 1));
   DL_TRY(sync(ctx));
@@ -1264,15 +1297,15 @@ int dl_fcsm_match(dl_context* ctx, const dl_fcsm_options* o, const float* submap
   constexpr int kChunk = 1024;
   for (int first = 0; first < n; first += kChunk) {
     const int m = std::min(kChunk, n - first);
-    DL_TRY(ctx->reserve_device(coarse_bytes((int64_t)m * n_hi, (int64_t)m * n_lo, m)));
-    Arena a(ctx->d_scratch);
     CoarseSearch cs;
     PairClouds pc;
     pc.hi_pts = hi_all.data();
     pc.lo_pts = lo_all.data();
     pc.hi_off = hi_off.data();
     pc.lo_off = lo_off.data();
-    DL_TRY(coarse_search(ctx, a, *o, min_score, first, m, guesses.data(), pc, his.data(), los.data(), nullptr, &cs));
+    DL_TRY(plan_coarse(ctx, *o, first, m, his.data(), &cs));
+    DL_TRY(carve_scratch(ctx, [&](Arena& a) { carve_coarse(a, pc, first, m, &cs); }));
+    DL_TRY(coarse_search(ctx, *o, min_score, first, m, guesses.data(), pc, his.data(), los.data(), &cs));
     std::vector<FcsmPick> picks(m);
     DL_TRY(d2h(ctx, picks.data(), cs.d_picks, m));
     DL_TRY(sync(ctx));
@@ -1328,12 +1361,17 @@ int constraint_search(dl_context* ctx, const dl_constraint_options& o, int count
   constexpr int kChunk = 1024;  // pairs per launch set: bounds the scratch, keeps every grid dimension legal
   for (int first = 0; first < count; first += kChunk) {
     const int n = std::min(kChunk, count - first);
-    const int64_t n_hi = hi_off[first + n] - hi_off[first], n_lo = lo_off[first + n] - lo_off[first];
-    DL_TRY(ctx->reserve_device(coarse_bytes(n_hi, n_lo, n) + arena_bytes({(size_t)n * sizeof(NlsProblem), (size_t)n * sizeof(NlsOutput)})));
-    Arena a(ctx->d_scratch);
     CoarseSearch cs;
-    DL_TRY(coarse_search(ctx, a, options->fast_correlative_scan_matcher_3d, (float)options->min_score, first, n, guesses, pc,
-                         hi_grids, lo_grids, nullptr, &cs));
+    NlsProblem* d_problems;
+    NlsOutput* d_out;
+    DL_TRY(plan_coarse(ctx, options->fast_correlative_scan_matcher_3d, first, n, hi_grids, &cs));
+    DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+      carve_coarse(a, pc, first, n, &cs);
+      d_problems = a.take<NlsProblem>(n);
+      d_out = a.take<NlsOutput>(n);
+    }));
+    DL_TRY(coarse_search(ctx, options->fast_correlative_scan_matcher_3d, (float)options->min_score, first, n, guesses, pc,
+                         hi_grids, lo_grids, &cs));
     // refinement: initial pose = translation target = the coarse pose, read from the pick record on the device
     std::vector<NlsProblem> problems(n);
     for (int k = 0; k < n; ++k) {
@@ -1349,8 +1387,6 @@ int constraint_search(dl_context* ctx, const dl_constraint_options& o, int count
       p.initial_dev = cs.d_picks[k].pose;  // address arithmetic only
       p.enabled_dev = &cs.d_picks[k].found;
     }
-    NlsProblem* d_problems = a.take<NlsProblem>(n);
-    NlsOutput* d_out = a.take<NlsOutput>(n);
     DL_TRY(h2d(ctx, d_problems, problems.data(), n));
     DL_CUDA(ctx, cudaMemsetAsync(d_out, 0, sizeof(NlsOutput) * n, ctx->stream));
     {
@@ -1404,18 +1440,24 @@ int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_const
   if (count > 0) {
     const NlsOptions nls = to_nls_options(options->ceres_scan_matcher_3d, 2);
     const int n = count;
-    const int64_t n_hi = hi_off[n] - hi_off[0], n_lo = lo_off[n] - lo_off[0];
-    DL_TRY(ctx->reserve_device(coarse_bytes(n_hi, n_lo, n) +
-                               arena_bytes({(size_t)n * sizeof(NlsProblem), (size_t)n * sizeof(NlsOutput), (size_t)n * 8})));
-    Arena a(ctx->d_scratch);
     CoarseSearch cs;
     PairClouds pc;
     pc.hi_pts = hi_pts;
     pc.lo_pts = lo_pts;
     pc.hi_off = hi_off;
     pc.lo_off = lo_off;
-    DL_TRY(coarse_search(ctx, a, options->fast_correlative_scan_matcher_3d, (float)options->min_score, 0, n, guesses, pc,
-                         hi_grids, lo_grids, nullptr, &cs));
+    NlsProblem* d_problems;
+    NlsOutput* d_out;
+    int32_t* d_ids;
+    DL_TRY(plan_coarse(ctx, options->fast_correlative_scan_matcher_3d, 0, n, hi_grids, &cs));
+    DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+      carve_coarse(a, pc, 0, n, &cs);
+      d_problems = a.take<NlsProblem>(n);
+      d_out = a.take<NlsOutput>(n);
+      d_ids = a.take<int32_t>(2 * (size_t)n);
+    }));
+    DL_TRY(coarse_search(ctx, options->fast_correlative_scan_matcher_3d, (float)options->min_score, 0, n, guesses, pc,
+                         hi_grids, lo_grids, &cs));
     std::vector<NlsProblem> problems(n);
     for (int k = 0; k < n; ++k) {
       NlsProblem& p = problems[k];
@@ -1429,9 +1471,6 @@ int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_const
       p.initial_dev = cs.d_picks[k].pose;  // address arithmetic only
       p.enabled_dev = &cs.d_picks[k].found;
     }
-    NlsProblem* d_problems = a.take<NlsProblem>(n);
-    NlsOutput* d_out = a.take<NlsOutput>(n);
-    int32_t* d_ids = a.take<int32_t>(2 * (size_t)n);
     DL_TRY(h2d(ctx, d_problems, problems.data(), n));
     DL_TRY(h2d(ctx, d_ids, submap_ids, n));
     DL_TRY(h2d(ctx, d_ids + n, node_ids, n));
@@ -1544,15 +1583,17 @@ int dl_imu_preintegrate(dl_context* ctx, const dl_imu_noise* noise, int32_t coun
   const size_t n = (size_t)offsets[count];
   for (int k = 0; k < count; ++k)
     if (offsets[k + 1] < offsets[k]) return ctx->fail(DL_ERR_ARG, "offsets must be non-decreasing");
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)(count + 1) * 4, n * 8, n * 24, n * 24, (size_t)count * 48,
-                                          (size_t)count * sizeof(dl_preintegration)})));
-  Arena a(ctx->d_scratch);
-  int32_t* d_off = a.take<int32_t>(count + 1);
-  double* d_dt = a.take<double>(n);
-  double* d_acc = a.take<double>(3 * n);
-  double* d_gyr = a.take<double>(3 * n);
-  double* d_bias = a.take<double>(6 * (size_t)count);
-  dl_preintegration* d_out = a.take<dl_preintegration>(count);
+  int32_t* d_off;
+  double *d_dt, *d_acc, *d_gyr, *d_bias;
+  dl_preintegration* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_off = a.take<int32_t>(count + 1);
+    d_dt = a.take<double>(n);
+    d_acc = a.take<double>(3 * n);
+    d_gyr = a.take<double>(3 * n);
+    d_bias = a.take<double>(6 * (size_t)count);
+    d_out = a.take<dl_preintegration>(count);
+  }));
   DL_TRY(h2d(ctx, d_off, offsets, count + 1));
   DL_TRY(h2d(ctx, d_dt, dt, n));
   DL_TRY(h2d(ctx, d_acc, acc, 3 * n));
@@ -1592,17 +1633,23 @@ int dl_fused_match_batch(dl_context* ctx, const dl_ceres_options* options, doubl
     return DL_ERR_ARG;
   if (count == 0) return DL_OK;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  size_t total_points = 0;
   for (int i = 0; i < count * num_pairs; ++i) {
     if (sizes[i] < 0 || !grids[i] || (sizes[i] > 0 && !clouds[i])) return DL_ERR_ARG;
     if (sizes[i] == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
     if (grids[i]->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
-    total_points += (size_t)sizes[i];
   }
-  DL_TRY(ctx->reserve_device(arena_bytes({total_points * 12 + (size_t)count * num_pairs * 256, (size_t)count * sizeof(NlsProblem),
-                                          (size_t)count * sizeof(HostImuTerm), (size_t)count * 128,
-                                          (size_t)count * sizeof(FusedOutput)})));
-  Arena a(ctx->d_scratch);
+  std::vector<float*> d_clouds(count * num_pairs);
+  NlsProblem* d_problems;
+  HostImuTerm* d_terms;
+  double* d_init;
+  FusedOutput* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    for (int i = 0; i < count * num_pairs; ++i) d_clouds[i] = a.take<float>(3 * sizes[i]);
+    d_problems = a.take<NlsProblem>(count);
+    d_terms = a.take<HostImuTerm>(count);
+    d_init = a.take<double>((size_t)count * 16);
+    d_out = a.take<FusedOutput>(count);
+  }));
   std::vector<NlsProblem> problems(count);
   std::vector<HostImuTerm> terms(count);
   std::vector<double> init16((size_t)count * 16);
@@ -1615,19 +1662,14 @@ int dl_fused_match_batch(dl_context* ctx, const dl_ceres_options* options, doubl
     std::memset(&p, 0, sizeof(p));
     for (int k = 0; k < num_pairs; ++k) {
       const int i = c * num_pairs + k;
-      float* d = a.take<float>(3 * sizes[i]);
-      DL_TRY(h2d(ctx, d, clouds[i], 3 * sizes[i]));
-      p.cloud[k] = d;
+      DL_TRY(h2d(ctx, d_clouds[i], clouds[i], 3 * sizes[i]));
+      p.cloud[k] = d_clouds[i];
       p.count[k] = (int32_t)sizes[i];
       p.grid[k] = grids[i]->view();
     }
     for (int k = 0; k < 7; ++k) p.initial[k] = x[k];
     for (int k = 0; k < 3; ++k) p.target_t[k] = x[k];  // the translation prior (if weighted) pulls to the IMU prediction
   }
-  NlsProblem* d_problems = a.take<NlsProblem>(count);
-  HostImuTerm* d_terms = a.take<HostImuTerm>(count);
-  double* d_init = a.take<double>((size_t)count * 16);
-  FusedOutput* d_out = a.take<FusedOutput>(count);
   DL_TRY(h2d(ctx, d_problems, problems.data(), count));
   DL_TRY(h2d(ctx, d_terms, terms.data(), count));
   DL_TRY(h2d(ctx, d_init, init16.data(), (size_t)count * 16));
@@ -1669,6 +1711,9 @@ struct FrontendBuffers {
   double *initial_pose, *target;
   NlsProblem* problems;
   NlsOutput* nls_out;
+  // 12-byte rows only (carve_time_runs)
+  int32_t *run_offsets = nullptr, *run_first_row = nullptr;
+  float *run_value = nullptr, *run_pose = nullptr;
 };
 
 // Device scratch of one front-end run. The stage-wise buffers (one voxel-filter pass per launch: dl_voxel.cu / dl_ingest.cu)
@@ -1710,12 +1755,15 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   }
 }
 
-// Bytes `carve` takes (counted by carving a null arena), plus slack for the few small takes of a run.
-size_t frontend_bytes(int batch, int64_t cap, int num_origins, bool stagewise = false) {
-  Arena count(nullptr);
-  FrontendBuffers f;
-  carve(count, batch, cap, num_origins, &f, stagewise);
-  return count.off + 8192;
+// Device copies of the time_run_* arrays of 12-byte rows (validated by check_frontend) and, with many runs per scan, the table
+// of per-run deskew poses: one pose per run (fe_run_poses) instead of one per survivor.
+void carve_time_runs(Arena& a, const dl_frontend_options& o, int num_scans, FrontendBuffers* f) {
+  if (o.range_row_floats != 3) return;
+  const size_t runs = (size_t)o.time_run_offsets[num_scans];
+  f->run_offsets = a.take<int32_t>((size_t)num_scans + 1);
+  f->run_first_row = a.take<int32_t>(runs);
+  f->run_value = a.take<float>(runs);
+  if (runs > (size_t)8 * num_scans) f->run_pose = a.take<float>(runs * 8);
 }
 
 FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuffers& f, const float* d_ranges,
@@ -1741,12 +1789,6 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
   return fa;
 }
 
-// Device copies of the time_run_* arrays and the table of per-run deskew poses (32 B per run).
-size_t time_runs_bytes(const dl_frontend_options& o, int num_scans) {
-  if (o.range_row_floats != 3 || !o.time_run_offsets || num_scans <= 0) return 0;
-  const size_t runs = (size_t)o.time_run_offsets[num_scans];
-  return arena_bytes({(size_t)(num_scans + 1) * 4, runs * 4, runs * 4, runs * 32});
-}
 int row_floats_of(const dl_frontend_options& o) { return o.range_row_floats == 4 ? 4 : (o.range_row_floats == 3 ? 3 : 8); }
 
 ScanConstants make_scan_constants(const double* prev7, const double* cur7) {  // dl_pipeline.cuh has the arithmetic
@@ -1781,29 +1823,45 @@ int frontend_ingest(dl_context* ctx, const dl_frontend_options& o, const Fronten
   return DL_OK;
 }
 
-// Uploads the small per-call tables (counts, deskew constants, origins, filter options, NLS problem records)
-// through one pinned staging block. No host synchronisation: the block is reused only after `staging_done`.
-size_t frontend_small_bytes(int batch, int num_origins) {
+// The pinned staging block of a front-end batch: the small per-call tables, then the results and estimated IMU states that a
+// submitted batch downloads (dl_frontend_submit*, collected by dl_frontend_collect*).
+struct Staging {
+  int32_t* counts;
+  ScanConstants* scans;
+  float* origins;
+  AdaptiveParams* filters;
+  NlsProblem* problems;
+  dl_scan_result* results;
+  dl_nav_state* states;
+};
+void carve_staging(Arena& h, int batch, int num_origins, Staging* s) {
   const size_t B = (size_t)batch;
-  return arena_bytes({B * 4, B * sizeof(ScanConstants), (size_t)num_origins * 12, 2 * sizeof(AdaptiveParams), B * sizeof(NlsProblem)});
+  s->counts = h.take<int32_t>(B);
+  s->scans = h.take<ScanConstants>(B);
+  s->origins = h.take<float>((size_t)num_origins * 3);
+  s->filters = h.take<AdaptiveParams>(2);
+  s->problems = h.take<NlsProblem>(B);
+  s->results = h.take<dl_scan_result>(B);
+  s->states = h.take<dl_nav_state>(B);
 }
+
+// Uploads the small per-call tables (counts, deskew constants, origins, filter options, NLS problem records)
+// through the pinned staging block. No host synchronisation: the block is reused only after `staging_done`.
 int frontend_upload_small(dl_context* ctx, const dl_frontend_options& o, const FrontendBuffers& f, const int64_t* sizes,
                           const float* origins, int num_origins, const double* prev_poses, const double* cur_poses,
                           const dl_grid* hi, const dl_grid* lo, const int32_t* enabled_dev = nullptr) {
   const size_t B = (size_t)f.batch;
-  const size_t bytes = frontend_small_bytes(f.batch, num_origins);
-  DL_TRY(ctx->reserve_pinned(bytes));
+  Staging s;
+  Arena count(nullptr);
+  carve_staging(count, f.batch, num_origins, &s);
+  DL_TRY(ctx->reserve_pinned(count.off));
   DL_CUDA(ctx, cudaEventSynchronize(ctx->staging_done));
   Arena h(ctx->h_pinned);
-  int32_t* counts = h.take<int32_t>(B);
-  ScanConstants* sc = h.take<ScanConstants>(B);
-  float* org = h.take<float>((size_t)num_origins * 3);
-  AdaptiveParams* filt = h.take<AdaptiveParams>(2);
-  NlsProblem* problems = h.take<NlsProblem>(B);
+  carve_staging(h, f.batch, num_origins, &s);
   for (int b = 0; b < f.batch; ++b) {
-    counts[b] = (int32_t)sizes[b];
-    if (prev_poses) sc[b] = make_scan_constants(prev_poses + 7 * b, cur_poses + 7 * b);
-    NlsProblem& p = problems[b];
+    s.counts[b] = (int32_t)sizes[b];
+    if (prev_poses) s.scans[b] = make_scan_constants(prev_poses + 7 * b, cur_poses + 7 * b);
+    NlsProblem& p = s.problems[b];
     std::memset(&p, 0, sizeof(p));
     if (hi && lo) {
       for (int k = 0; k < 2; ++k) {
@@ -1816,39 +1874,53 @@ int frontend_upload_small(dl_context* ctx, const dl_frontend_options& o, const F
       if (enabled_dev) p.enabled_dev = enabled_dev + b;  // scans whose IMU factor could not be formed are not solved
     }
   }
-  std::memcpy(org, origins, (size_t)num_origins * 12);
-  filt[0] = {o.high_resolution_adaptive_voxel_filter.max_length, o.high_resolution_adaptive_voxel_filter.min_num_points,
-             o.high_resolution_adaptive_voxel_filter.max_range};
-  filt[1] = {o.low_resolution_adaptive_voxel_filter.max_length, o.low_resolution_adaptive_voxel_filter.min_num_points,
-             o.low_resolution_adaptive_voxel_filter.max_range};
-  DL_TRY(h2d(ctx, f.counts0, counts, B));
-  if (prev_poses) DL_TRY(h2d(ctx, f.scans, sc, B));  // otherwise imu_prepare_kernel writes them on the device
-  DL_TRY(h2d(ctx, f.origins, org, (size_t)num_origins * 3));
-  DL_TRY(h2d(ctx, f.filters, filt, 2));
-  DL_TRY(h2d(ctx, f.problems, problems, B));
+  std::memcpy(s.origins, origins, (size_t)num_origins * 12);
+  s.filters[0] = {o.high_resolution_adaptive_voxel_filter.max_length, o.high_resolution_adaptive_voxel_filter.min_num_points,
+                  o.high_resolution_adaptive_voxel_filter.max_range};
+  s.filters[1] = {o.low_resolution_adaptive_voxel_filter.max_length, o.low_resolution_adaptive_voxel_filter.min_num_points,
+                  o.low_resolution_adaptive_voxel_filter.max_range};
+  DL_TRY(h2d(ctx, f.counts0, s.counts, B));
+  if (prev_poses) DL_TRY(h2d(ctx, f.scans, s.scans, B));  // otherwise imu_prepare_kernel writes them on the device
+  DL_TRY(h2d(ctx, f.origins, s.origins, (size_t)num_origins * 3));
+  DL_TRY(h2d(ctx, f.filters, s.filters, 2));
+  DL_TRY(h2d(ctx, f.problems, s.problems, B));
   DL_CUDA(ctx, cudaEventRecord(ctx->staging_done, ctx->stream));
   return DL_OK;
 }
 
 // IMU coupling of one front-end run: either finished pre-integrations (`host`, factors built on the host) or raw samples
-// (`samples`, everything on the device). frontend_run fills in where the device outputs are.
+// (`samples`, everything on the device), and its device buffers (carve_imu).
 struct ImuRun {
   const dl_frontend_imu* host = nullptr;
   const dl_frontend_imu_samples* samples = nullptr;
   dl_nav_state* d_states_out = nullptr;  // in: optional caller-provided device buffer for the estimated states
-  FusedOutput* d_fused = nullptr;        // out
-  dl_nav_state* d_states = nullptr;      // out: estimated states, local frame
-  dl_nav_state* d_predicted = nullptr;   // out (samples only): predicted states, local frame
+  HostImuTerm* d_terms = nullptr;
+  double* d_init16 = nullptr;
+  FusedOutput* d_fused = nullptr;
+  dl_nav_state* d_states = nullptr;      // estimated states, local frame
+  // raw samples only
+  int32_t* d_off = nullptr;
+  double *d_dt = nullptr, *d_acc = nullptr, *d_gyr = nullptr;
+  dl_nav_state* d_si = nullptr;
+  dl_preintegration* d_pre = nullptr;
+  dl_nav_state* d_predicted = nullptr;   // predicted states, local frame
+  int32_t* d_ok = nullptr;               // per scan: its IMU factor could be formed
 };
-size_t imu_run_device_bytes(int num_scans, const dl_frontend_imu_samples* raw) {
-  const size_t B = (size_t)num_scans;
-  size_t bytes = arena_bytes({B * sizeof(HostImuTerm), B * 128, B * sizeof(FusedOutput), B * sizeof(dl_nav_state)});
-  if (raw) {
-    const size_t ns = (size_t)raw->offsets[num_scans];
-    bytes += arena_bytes({(B + 1) * 4, ns * 8, ns * 24, ns * 24, B * sizeof(dl_nav_state), B * sizeof(dl_preintegration),
-                          B * sizeof(dl_nav_state), B * 4});
-  }
-  return bytes + 1024;
+void carve_imu(Arena& a, int num_scans, ImuRun* r) {
+  r->d_terms = a.take<HostImuTerm>(num_scans);
+  r->d_init16 = a.take<double>((size_t)num_scans * 16);
+  r->d_fused = a.take<FusedOutput>(num_scans);
+  r->d_states = r->d_states_out ? r->d_states_out : a.take<dl_nav_state>(num_scans);
+  if (!r->samples) return;
+  const size_t ns = (size_t)r->samples->offsets[num_scans];
+  r->d_off = a.take<int32_t>(num_scans + 1);
+  r->d_dt = a.take<double>(ns);
+  r->d_acc = a.take<double>(3 * ns);
+  r->d_gyr = a.take<double>(3 * ns);
+  r->d_si = a.take<dl_nav_state>(num_scans);
+  r->d_pre = a.take<dl_preintegration>(num_scans);
+  r->d_predicted = a.take<dl_nav_state>(num_scans);
+  r->d_ok = a.take<int32_t>(num_scans);
 }
 
 // CTAs per least-squares problem. The pipeline's adaptive filters hand the matcher a few hundred points: one CTA. With the filters
@@ -1876,44 +1948,12 @@ int solve_cluster_size(dl_context* ctx, const dl_frontend_options& o, int proble
 int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, float* d_ranges, int64_t in_cap,
                  const void* const* host_ranges, const int64_t* sizes, const float* origins, int num_origins,
                  const double* prev_poses, const double* cur_poses, const double* submap_local_pose, const dl_grid* hi,
-                 const dl_grid* lo, Arena& a, dl_scan_result* d_results, ImuRun* imu_run = nullptr,
-                 FrontendBuffers* buffers_out = nullptr) {
-  FrontendBuffers f;
-  carve(a, num_scans, in_cap, num_origins, &f);
-  if (buffers_out) *buffers_out = f;
+                 const dl_grid* lo, const FrontendBuffers& f, Arena& a, dl_scan_result* d_results, ImuRun* imu_run = nullptr) {
   // optional IMU coupling: one pre-integration factor per scan, the 15-parameter solve instead of the 6-parameter one
-  const dl_frontend_imu* imu = imu_run ? imu_run->host : nullptr;
-  const dl_frontend_imu_samples* raw = imu_run ? imu_run->samples : nullptr;
-  HostImuTerm* d_terms = nullptr;
-  double* d_init16 = nullptr;
-  FusedOutput* d_fused = nullptr;
-  int32_t* d_imu_ok = nullptr;
-  dl_nav_state* d_states_out = nullptr;
-  if (imu || raw) {
-    d_terms = a.take<HostImuTerm>(num_scans);
-    d_init16 = a.take<double>((size_t)num_scans * 16);
-    d_fused = a.take<FusedOutput>(num_scans);
-    d_states_out = imu_run->d_states_out ? imu_run->d_states_out : a.take<dl_nav_state>(num_scans);
-    imu_run->d_fused = d_fused;
-    imu_run->d_states = d_states_out;
-  }
-  int32_t* d_off = nullptr;
-  double *d_dt = nullptr, *d_acc = nullptr, *d_gyr = nullptr;
-  dl_nav_state *d_si = nullptr, *d_pred = nullptr;
-  dl_preintegration* d_pre = nullptr;
-  size_t ns = 0;
-  if (raw) {
-    ns = (size_t)raw->offsets[num_scans];
-    d_off = a.take<int32_t>(num_scans + 1);
-    d_dt = a.take<double>(ns);
-    d_acc = a.take<double>(3 * ns);
-    d_gyr = a.take<double>(3 * ns);
-    d_si = a.take<dl_nav_state>(num_scans);
-    d_pre = a.take<dl_preintegration>(num_scans);
-    d_pred = a.take<dl_nav_state>(num_scans);
-    d_imu_ok = a.take<int32_t>(num_scans);
-    imu_run->d_predicted = d_pred;
-  }
+  const ImuRun no_imu;
+  const ImuRun& m = imu_run ? *imu_run : no_imu;
+  const dl_frontend_imu* imu = m.host;
+  const dl_frontend_imu_samples* raw = m.samples;
   if (imu) {
     std::vector<HostImuTerm> terms(num_scans);
     std::vector<double> init16((size_t)num_scans * 16);
@@ -1922,28 +1962,24 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
       if (!build_imu_term(to_submap, imu->states_i[b], imu->predicted_states[b], imu->preintegrations[b], imu->gravity,
                           imu->imu_weight, &terms[b], init16.data() + 16 * b))
         return ctx->fail(DL_ERR_ARG, "pre-integration covariance is not positive definite");
-    DL_TRY(h2d(ctx, d_terms, terms.data(), num_scans));
-    DL_TRY(h2d(ctx, d_init16, init16.data(), (size_t)num_scans * 16));
+    DL_TRY(h2d(ctx, m.d_terms, terms.data(), num_scans));
+    DL_TRY(h2d(ctx, m.d_init16, init16.data(), (size_t)num_scans * 16));
     DL_TRY(sync(ctx));  // the staging vectors are pageable and local
   }
-  if (imu || raw) DL_CUDA(ctx, cudaMemsetAsync(d_fused, 0, sizeof(FusedOutput) * num_scans, ctx->stream));
+  if (imu || raw) DL_CUDA(ctx, cudaMemsetAsync(m.d_fused, 0, sizeof(FusedOutput) * num_scans, ctx->stream));
   const int rf = row_floats_of(o);
-  DL_TRY(frontend_upload_small(ctx, o, f, sizes, origins, num_origins, raw ? nullptr : prev_poses, cur_poses, hi, lo,
-                               d_imu_ok));
+  DL_TRY(frontend_upload_small(ctx, o, f, sizes, origins, num_origins, raw ? nullptr : prev_poses, cur_poses, hi, lo, m.d_ok));
   FrontendArgs fa = make_frontend_args(o, f, d_ranges, in_cap, rf);
   if (rf == 3) {  // per-point times as runs: validated by check_frontend, uploaded next to the scans
     const size_t runs = (size_t)o.time_run_offsets[num_scans];
-    int32_t* d_ro = a.take<int32_t>((size_t)num_scans + 1);
-    int32_t* d_rf = a.take<int32_t>(runs);
-    float* d_rv = a.take<float>(runs);
-    DL_TRY(h2d(ctx, d_ro, o.time_run_offsets, (size_t)num_scans + 1));
-    DL_TRY(h2d(ctx, d_rf, o.time_run_first_row, runs));
-    DL_TRY(h2d(ctx, d_rv, o.time_run_value, runs));
-    fa.run_offsets = d_ro; fa.run_first_row = d_rf; fa.run_value = d_rv;
-    if (runs > (size_t)8 * num_scans) {  // many runs per scan: one deskew pose per run (fe_run_poses) instead of one per survivor
+    DL_TRY(h2d(ctx, f.run_offsets, o.time_run_offsets, (size_t)num_scans + 1));
+    DL_TRY(h2d(ctx, f.run_first_row, o.time_run_first_row, runs));
+    DL_TRY(h2d(ctx, f.run_value, o.time_run_value, runs));
+    fa.run_offsets = f.run_offsets; fa.run_first_row = f.run_first_row; fa.run_value = f.run_value;
+    if (f.run_pose) {
       int max_runs = 0;
       for (int b = 0; b < num_scans; ++b) max_runs = std::max(max_runs, (int)(o.time_run_offsets[b + 1] - o.time_run_offsets[b]));
-      fa.run_pose = a.take<float>(runs * 8);  // filled per sub-batch by fe_run_poses once the scans' deskew constants exist
+      fa.run_pose = f.run_pose;  // filled per sub-batch by fe_run_poses once the scans' deskew constants exist
       fa.max_runs = max_runs;
     }
   }
@@ -1972,17 +2008,19 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
     ctx->stream = ctx->tail_stream;
     auto chain = [&]() -> int {
       StageScope st(ctx, "imu_preintegrate_predict");
-      DL_TRY(h2d(ctx, d_off, raw->offsets, (size_t)num_scans + 1));
-      DL_TRY(h2d(ctx, d_dt, raw->dt, ns));
-      DL_TRY(h2d(ctx, d_acc, raw->acc, 3 * ns));
-      DL_TRY(h2d(ctx, d_gyr, raw->gyr, 3 * ns));
-      DL_TRY(h2d(ctx, d_si, raw->states_i, (size_t)num_scans));
-      DL_TRY(launch_imu_preintegrate(ctx, num_scans, d_off, d_dt, d_acc, d_gyr, (const double*)d_si + 10, 16, raw->noise, d_pre));
+      const size_t ns = (size_t)raw->offsets[num_scans];
+      DL_TRY(h2d(ctx, m.d_off, raw->offsets, (size_t)num_scans + 1));
+      DL_TRY(h2d(ctx, m.d_dt, raw->dt, ns));
+      DL_TRY(h2d(ctx, m.d_acc, raw->acc, 3 * ns));
+      DL_TRY(h2d(ctx, m.d_gyr, raw->gyr, 3 * ns));
+      DL_TRY(h2d(ctx, m.d_si, raw->states_i, (size_t)num_scans));
+      DL_TRY(launch_imu_preintegrate(ctx, num_scans, m.d_off, m.d_dt, m.d_acc, m.d_gyr, (const double*)m.d_si + 10, 16, raw->noise,
+                                     m.d_pre));
       ImuPrepareArgs pa{};
-      pa.count = num_scans; pa.preint = d_pre; pa.states_i = d_si; pa.to_submap = inverse(pose_from7(submap_local_pose));
+      pa.count = num_scans; pa.preint = m.d_pre; pa.states_i = m.d_si; pa.to_submap = inverse(pose_from7(submap_local_pose));
       for (int k = 0; k < 3; ++k) pa.gravity[k] = raw->gravity[k];
-      pa.imu_weight = raw->imu_weight; pa.scans = f.scans; pa.terms = d_terms; pa.init16 = d_init16; pa.predicted = d_pred;
-      pa.ok = d_imu_ok;
+      pa.imu_weight = raw->imu_weight; pa.scans = f.scans; pa.terms = m.d_terms; pa.init16 = m.d_init16; pa.predicted = m.d_predicted;
+      pa.ok = m.d_ok;
       return launch_imu_prepare(ctx, pa);
     };
     const int st_imu = chain();
@@ -2094,16 +2132,16 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
         NlsOptions no = to_nls_options(o.ceres_scan_matcher, 2);
         no.cluster = solve_cluster_size(ctx, o, nb);
         if (imu || raw)  // pose part of the initial state comes from problems[].initial_dev like the plain solve's
-          DL_TRY(launch_nls_fused(ctx, no, f.problems + b0, d_terms + b0, d_init16 + 16 * b0, nb, d_fused + b0));
+          DL_TRY(launch_nls_fused(ctx, no, f.problems + b0, m.d_terms + b0, m.d_init16 + 16 * b0, nb, m.d_fused + b0));
         else
           DL_TRY(launch_nls(ctx, no, f.problems + b0, nb, f.nls_out + b0));
       }
       ResultArgs ra{};
       ra.batch = nb; ra.first_counts = f.n1 + b0; ra.return_counts = f.n2 + b0; ra.miss_counts = f.n3 + b0;
       ra.adaptive_counts = f.countsA + 2 * b0; ra.adaptive_cropped = f.croppedA + 2 * b0; ra.adaptive_passes = f.npassesA + 2 * b0;
-      ra.rtcsm_scores = have_scores ? f.rtcsm_scores + b0 : nullptr; ra.nls = f.nls_out + b0; ra.fused = (imu || raw) ? d_fused + b0 : nullptr; ra.submap = submap;
+      ra.rtcsm_scores = have_scores ? f.rtcsm_scores + b0 : nullptr; ra.nls = f.nls_out + b0; ra.fused = (imu || raw) ? m.d_fused + b0 : nullptr; ra.submap = submap;
       ra.results = d_results + b0; ra.error_flag = f.error_flag + b0;
-      ra.imu_ok = d_imu_ok ? d_imu_ok + b0 : nullptr; ra.states_out = d_states_out ? d_states_out + b0 : nullptr;
+      ra.imu_ok = m.d_ok ? m.d_ok + b0 : nullptr; ra.states_out = m.d_states ? m.d_states + b0 : nullptr;
       DL_TRY(launch_finalize_results(ctx, ra));
       return DL_OK;
     };
@@ -2164,8 +2202,7 @@ struct FrontendScans {
 int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int num_scans, const FrontendScans& in,
                      const int64_t* sizes, const float* origins, int num_origins, const double* prev_poses,
                      const double* predicted_poses, const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo,
-                     size_t pinned_extra, dl_scan_result** d_results_out, ImuRun* imu = nullptr,
-                     FrontendBuffers* buffers_out = nullptr) {
+                     dl_scan_result** d_results_out, ImuRun* imu = nullptr, FrontendBuffers* buffers_out = nullptr) {
   int64_t max_size = 0;
   DL_TRY(check_frontend(ctx, options, num_scans, sizes, hi, lo, &max_size));
   if (num_scans == 0) return DL_OK;
@@ -2188,19 +2225,25 @@ int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int nu
   }
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const int64_t cap = in.on_device ? in.cap_rows : std::max<int64_t>(max_size, 1);
-  size_t bytes = frontend_bytes(num_scans, cap, num_origins) + time_runs_bytes(*options, num_scans);
-  if (options->use_online_correlative_scan_matching)
-    bytes += (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, hi->resolution, false);
-  if (imu) bytes += imu_run_device_bytes(num_scans, imu->samples);
-  if (!in.on_device) bytes += arena_bytes({(size_t)num_scans * cap * 32, (size_t)num_scans * sizeof(dl_scan_result)});
-  DL_TRY(ctx->reserve_device(bytes));
-  if (pinned_extra) DL_TRY(ctx->reserve_pinned(frontend_small_bytes(num_scans, num_origins) + pinned_extra + 256));
-  Arena a(ctx->d_scratch);
-  float* d_ranges = in.on_device ? (float*)in.dev : a.take<float>((size_t)num_scans * cap * 8);
-  dl_scan_result* d_results = in.on_device ? in.results_dev : a.take<dl_scan_result>(num_scans);
+  // The correlative pre-match takes its candidate tables after the carve (see rtcsm_scratch_bound).
+  const size_t rtcsm_extra = options->use_online_correlative_scan_matching
+      ? (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, hi->resolution, false)
+      : 0;
+  float* d_ranges;
+  dl_scan_result* d_results;
+  FrontendBuffers f;
+  Arena rest(nullptr);
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_ranges = in.on_device ? (float*)in.dev : a.take<float>((size_t)num_scans * cap * 8);
+    d_results = in.on_device ? in.results_dev : a.take<dl_scan_result>(num_scans);
+    carve(a, num_scans, cap, num_origins, &f);
+    if (imu) carve_imu(a, num_scans, imu);
+    carve_time_runs(a, *options, num_scans, &f);
+  }, rtcsm_extra, &rest));
   if (d_results_out) *d_results_out = d_results;
+  if (buffers_out) *buffers_out = f;
   return frontend_run(ctx, *options, num_scans, d_ranges, cap, in.host, sizes, origins, num_origins, prev_poses,
-                      predicted_poses, submap_local_pose, hi, lo, a, d_results, imu, buffers_out);
+                      predicted_poses, submap_local_pose, hi, lo, f, rest, d_results, imu);
 }
 
 }  // namespace
@@ -2219,7 +2262,7 @@ int dl_frontend_match_batch_dev(dl_context* ctx, const dl_frontend_options* opti
   in.cap_rows = cap_rows;
   in.results_dev = results_dev;
   return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, prev_poses, predicted_poses,
-                          submap_local_pose, hi, lo, 0, nullptr);
+                          submap_local_pose, hi, lo, nullptr);
 }
 
 int dl_frontend_fetch_results(dl_context* ctx, const dl_scan_result* results_dev, int32_t num_scans,
@@ -2241,7 +2284,7 @@ int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options,
   if (!results) return DL_ERR_ARG;
   dl_scan_result* d_results = nullptr;
   DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev_poses, predicted_poses,
-                          submap_local_pose, hi, lo, 0, &d_results));
+                          submap_local_pose, hi, lo, &d_results));
   DL_TRY(d2h(ctx, results, d_results, num_scans));
   return sync(ctx);
 }
@@ -2275,7 +2318,7 @@ int dl_frontend_match_batch_imu(dl_context* ctx, const dl_frontend_options* opti
   ImuRun run;
   run.host = imu;
   DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev.data(), pred.data(),
-                          submap_local_pose, hi, lo, 0, &d_results, &run));
+                          submap_local_pose, hi, lo, &d_results, &run));
   DL_TRY(d2h(ctx, results, d_results, num_scans));
   DL_TRY(d2h(ctx, imu->states_out, run.d_states, num_scans));
   return sync(ctx);
@@ -2305,7 +2348,7 @@ int dl_frontend_match_batch_imu_samples(dl_context* ctx, const dl_frontend_optio
   ImuRun run;
   run.samples = imu;
   DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, nullptr, nullptr,
-                          submap_local_pose, hi, lo, 0, &d_results, &run));
+                          submap_local_pose, hi, lo, &d_results, &run));
   DL_TRY(d2h(ctx, results, d_results, num_scans));
   DL_TRY(d2h(ctx, states_out, run.d_states, num_scans));
   if (predicted_states_out) DL_TRY(d2h(ctx, predicted_states_out, run.d_predicted, num_scans));
@@ -2327,27 +2370,26 @@ int dl_frontend_match_batch_imu_samples_dev(dl_context* ctx, const dl_frontend_o
   ImuRun run;
   run.samples = imu;
   run.d_states_out = states_out_dev;
-  return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, nullptr, nullptr, submap_local_pose, hi, lo, 0,
+  return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, nullptr, nullptr, submap_local_pose, hi, lo,
                           nullptr, &run);
 }
 
 // Tail of a submit: the results (and, with the IMU, the estimated states) go to pinned staging behind the batch.
 static int submit_finish(dl_context* ctx, int num_scans, int num_origins, const dl_scan_result* d_results,
                          const dl_nav_state* d_states) {
-  const size_t result_bytes = (size_t)num_scans * sizeof(dl_scan_result);
-  ctx->results_staging_offset = (frontend_small_bytes(num_scans, num_origins) + 255) & ~size_t(255);
-  char* dst = (char*)ctx->h_pinned + ctx->results_staging_offset;
-  DL_CUDA(ctx, cudaMemcpyAsync(dst, d_results, result_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  Staging s;
+  Arena h(ctx->h_pinned);  // the block frontend_upload_small reserved for this batch
+  carve_staging(h, num_scans, num_origins, &s);
+  DL_CUDA(ctx, cudaMemcpyAsync(s.results, d_results, (size_t)num_scans * sizeof(dl_scan_result), cudaMemcpyDeviceToHost,
+                               ctx->stream));
   if (d_states)
-    DL_CUDA(ctx, cudaMemcpyAsync(dst + ((result_bytes + 255) & ~size_t(255)), d_states, (size_t)num_scans * sizeof(dl_nav_state),
-                                 cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(s.states, d_states, (size_t)num_scans * sizeof(dl_nav_state), cudaMemcpyDeviceToHost, ctx->stream));
   DL_CUDA(ctx, cudaEventRecord(ctx->batch_done, ctx->stream));
   ctx->in_flight = num_scans;
   ctx->in_flight_states = d_states != nullptr;
+  ctx->staged_results = s.results;
+  ctx->staged_states = s.states;
   return DL_OK;
-}
-static size_t submit_pinned_bytes(int num_scans) {
-  return (((size_t)num_scans * sizeof(dl_scan_result) + 255) & ~size_t(255)) + (size_t)num_scans * sizeof(dl_nav_state) + 256;
 }
 
 int dl_frontend_submit(dl_context* ctx, const dl_frontend_options* options, int32_t num_scans, const void* const* ranges,
@@ -2357,7 +2399,7 @@ int dl_frontend_submit(dl_context* ctx, const dl_frontend_options* options, int3
   if (ctx->in_flight) return ctx->fail(DL_ERR_ARG, "a submitted batch is already in flight on this context");
   dl_scan_result* d_results = nullptr;
   DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev_poses, predicted_poses,
-                          submap_local_pose, hi, lo, submit_pinned_bytes(num_scans), &d_results));
+                          submap_local_pose, hi, lo, &d_results));
   return submit_finish(ctx, num_scans, num_origins, d_results, nullptr);
 }
 
@@ -2371,7 +2413,7 @@ int dl_frontend_submit_imu_samples(dl_context* ctx, const dl_frontend_options* o
   ImuRun run;
   run.samples = imu;
   DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, nullptr, nullptr, submap_local_pose,
-                          hi, lo, submit_pinned_bytes(num_scans), &d_results, &run));
+                          hi, lo, &d_results, &run));
   return submit_finish(ctx, num_scans, num_origins, d_results, run.d_states);
 }
 
@@ -2384,10 +2426,8 @@ static int collect_common(dl_context* ctx, int32_t num_scans, dl_scan_result* re
   const cudaError_t e = cudaEventSynchronize(ctx->batch_done);
   ctx->in_flight = 0;
   if (e != cudaSuccess) return ctx->cuda_fail(e, "dl_frontend_collect");
-  const size_t result_bytes = (size_t)num_scans * sizeof(dl_scan_result);
-  const char* src = (const char*)ctx->h_pinned + ctx->results_staging_offset;
-  std::memcpy(results, src, result_bytes);
-  if (states_out) std::memcpy(states_out, src + ((result_bytes + 255) & ~size_t(255)), (size_t)num_scans * sizeof(dl_nav_state));
+  std::memcpy(results, ctx->staged_results, (size_t)num_scans * sizeof(dl_scan_result));
+  if (states_out) std::memcpy(states_out, ctx->staged_states, (size_t)num_scans * sizeof(dl_nav_state));
   return DL_OK;
 }
 int dl_frontend_collect(dl_context* ctx, int32_t num_scans, dl_scan_result* results) {
@@ -2416,21 +2456,22 @@ int decode_common(dl_context* ctx, const dl_point_cloud2_layout* l, const void* 
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t bytes = (size_t)n * l->point_step;
   const size_t tiles = (size_t)((n + 255) / 256);
-  DL_TRY(ctx->reserve_device(arena_bytes({data_host ? bytes : 0, rows_host ? (size_t)n * 16 : 0, tiles * 4, 64, 64})));
-  Arena a(ctx->d_scratch);
   DecodeArgs d{};
+  uint8_t* up = nullptr;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    if (data_host) up = a.take<uint8_t>(bytes);
+    d.rows_out = rows_host ? a.take<float>((size_t)n * 4) : rows_dev;
+    d.tile_counts = a.take<int32_t>(tiles);
+    d.num_out = a.take<int32_t>(1);
+    d.stamp_offset = a.take<double>(1);
+  }));
   if (data_host) {
-    uint8_t* up = a.take<uint8_t>(bytes);
     DL_TRY(h2d(ctx, up, (const uint8_t*)data_host, bytes));
     d.data = up;
   } else {
     d.data = (const uint8_t*)data_dev;
   }
-  d.rows_out = rows_host ? a.take<float>((size_t)n * 4) : rows_dev;
   if (((uintptr_t)d.rows_out & 15) != 0) return ctx->fail(DL_ERR_ARG, "rows_out must be 16-byte aligned");
-  d.tile_counts = a.take<int32_t>(tiles);
-  d.num_out = a.take<int32_t>(1);
-  d.stamp_offset = a.take<double>(1);
   d.n = n;
   d.point_step = l->point_step; d.offset_x = l->offset_x; d.offset_y = l->offset_y; d.offset_z = l->offset_z;
   d.offset_time = l->offset_time; d.time_type = l->time_type;
@@ -2472,12 +2513,13 @@ int dl_ingest_scan(dl_context* ctx, const dl_frontend_options* options, const vo
       !counts_out)
     return DL_ERR_ARG;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(frontend_bytes(1, n, num_origins, true) + (size_t)n * 32 + 256));
-  Arena a(ctx->d_scratch);
-  float* d_ranges = a.take<float>((size_t)n * 8);
-  DL_TRY(h2d(ctx, d_ranges, (const float*)ranges, (size_t)n * 8));
+  float* d_ranges;
   FrontendBuffers f;
-  carve(a, 1, n, num_origins, &f, true);
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_ranges = a.take<float>((size_t)n * 8);
+    carve(a, 1, n, num_origins, &f, true);
+  }));
+  DL_TRY(h2d(ctx, d_ranges, (const float*)ranges, (size_t)n * 8));
   if (row_floats_of(*options) != 8) return ctx->fail(DL_ERR_ARG, "dl_ingest_scan takes RangeMeasurement rows (range_row_floats = 8)");
   DL_TRY(frontend_upload_small(ctx, *options, f, &n, origins, num_origins, prev_pose, predicted_pose, nullptr, nullptr));
   // stage-wise kernels (first_keep, returns_local) ...
@@ -2522,13 +2564,16 @@ int dl_ingest_scan(dl_context* ctx, const dl_frontend_options* options, const vo
 extern "C" int dl_rotational_histogram(dl_context* ctx, const float* points, int64_t n, int32_t size, float* histogram_out) {
   if (!ctx || n < 0 || (n > 0 && !points) || !histogram_out) return DL_ERR_ARG;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY(ctx->reserve_device(arena_bytes({(size_t)n * 12, (size_t)size * 4}) + rotational_histogram_scratch_bytes(n)));
-  Arena a(ctx->d_scratch);
-  float* d_pts = a.take<float>(3 * (size_t)std::max<int64_t>(n, 1));
-  float* d_hist = a.take<float>(std::max(size, 1));
+  float *d_pts, *d_hist;
+  HistogramScratch hs;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(3 * (size_t)std::max<int64_t>(n, 1));
+    d_hist = a.take<float>(std::max(size, 1));
+    carve_rotational_histogram(a, n, &hs);
+  }));
   DL_TRY(h2d(ctx, d_pts, points, 3 * (size_t)n));
   int32_t* d_err = nullptr;
-  DL_TRY(launch_rotational_histogram(ctx, a, d_pts, n, size, d_hist, &d_err));
+  DL_TRY(launch_rotational_histogram(ctx, hs, d_pts, n, size, d_hist, &d_err));
   int32_t err = 0;
   DL_TRY(d2h(ctx, histogram_out, d_hist, (size_t)size));
   DL_TRY(d2h(ctx, &err, d_err, 1));
@@ -2740,7 +2785,7 @@ int dl_ltb_add_synchronized_range_data(dl_local_trajectory_builder* b, double ti
     ImuRun run;
     run.samples = &imu;
     DL_TRY(frontend_enqueue(ctx, &fo, 1, FrontendScans{ranges}, sizes, origin, num_origins, nullptr, nullptr, submap_pose, matching.hi, matching.lo,
-                            0, &d_results, &run, &f));
+                            &d_results, &run, &f));
     DL_TRY(d2h(ctx, &r, d_results, 1));
     DL_TRY(d2h(ctx, &state, run.d_states, 1));
     DL_TRY(d2h(ctx, cur7, f.current_pose, 7));
@@ -2756,7 +2801,7 @@ int dl_ltb_add_synchronized_range_data(dl_local_trajectory_builder* b, double ti
     double prev7[7], pred7[7];
     for (int k = 0; k < 3; ++k) { prev7[k] = b->prev_state.p[k]; pred7[k] = pred.p[k]; }
     for (int k = 0; k < 4; ++k) { prev7[3 + k] = b->prev_state.q[k]; pred7[3 + k] = pred.q[k]; }
-    DL_TRY(frontend_enqueue(ctx, &fo, 1, FrontendScans{ranges}, sizes, origin, num_origins, prev7, pred7, submap_pose, matching.hi, matching.lo, 0,
+    DL_TRY(frontend_enqueue(ctx, &fo, 1, FrontendScans{ranges}, sizes, origin, num_origins, prev7, pred7, submap_pose, matching.hi, matching.lo,
                             &d_results, nullptr, &f));
     DL_TRY(d2h(ctx, &r, d_results, 1));
     DL_TRY(d2h(ctx, cur7, f.current_pose, 7));
@@ -2918,19 +2963,21 @@ extern "C" int dl_window_optimize_batch(dl_context* ctx, const dl_window_options
     return ctx->fail(DL_ERR_ARG, "dl_window_options: sigmas and the IMU weight must be positive");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t n = (size_t)count;
-  DL_TRY(ctx->reserve_device(arena_bytes({n * sizeof(dl_nav_state), n * 225 * 8, n * sizeof(dl_preintegration), n * 56,
-                                          n * sizeof(dl_nav_state), n * sizeof(dl_nav_state), n * sizeof(dl_nav_state), n * 225 * 8,
-                                          n * sizeof(dl_solve_summary)})));
-  Arena a(ctx->d_scratch);
-  dl_nav_state* d_si = a.take<dl_nav_state>(n);
-  double* d_prior = a.take<double>(n * 225);
-  dl_preintegration* d_pre = a.take<dl_preintegration>(n);
-  double* d_z = a.take<double>(n * 7);
-  dl_nav_state* d_init = a.take<dl_nav_state>(n);
-  dl_nav_state* d_si_out = a.take<dl_nav_state>(n);
-  dl_nav_state* d_sj_out = a.take<dl_nav_state>(n);
-  double* d_info = a.take<double>(n * 225);
-  dl_solve_summary* d_sum = a.take<dl_solve_summary>(n);
+  dl_nav_state *d_si, *d_init, *d_si_out, *d_sj_out;
+  double *d_prior, *d_z, *d_info;
+  dl_preintegration* d_pre;
+  dl_solve_summary* d_sum;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_si = a.take<dl_nav_state>(n);
+    d_prior = a.take<double>(n * 225);
+    d_pre = a.take<dl_preintegration>(n);
+    d_z = a.take<double>(n * 7);
+    d_init = a.take<dl_nav_state>(n);
+    d_si_out = a.take<dl_nav_state>(n);
+    d_sj_out = a.take<dl_nav_state>(n);
+    d_info = a.take<double>(n * 225);
+    d_sum = a.take<dl_solve_summary>(n);
+  }));
   DL_TRY(h2d(ctx, d_si, states_i, n));
   DL_TRY(h2d(ctx, d_prior, prior_information, n * 225));
   DL_TRY(h2d(ctx, d_pre, preintegrations, n));

@@ -242,30 +242,37 @@ __global__ void __launch_bounds__(kThreads) rotational_histogram_kernel(Histogra
 
 }  // namespace
 
-size_t rotational_histogram_scratch_bytes(int64_t n) {
+static int64_t histogram_np2(int64_t n) {
   int64_t np2 = 64;
   while (np2 < n) np2 <<= 1;
-  return arena_bytes({(size_t)np2 * 8, (size_t)(n + 1) * 4, (size_t)n * 16, (size_t)n * 4, (size_t)n * 4, 64, 1024 * 4});
+  return np2;
 }
 
-// d_points: n x 3 floats on the device. d_histogram: `size` floats (size <= 1024). Scratch is carved from `a`.
-int launch_rotational_histogram(dl_context* ctx, Arena& a, const float* d_points, int64_t n, int size, float* d_histogram,
-                                int32_t** d_error_out) {
+void carve_rotational_histogram(Arena& a, int64_t n, HistogramScratch* s) {
+  s->keys = a.take<unsigned long long>(histogram_np2(n));
+  s->slice_first = a.take<int>(n + 1);
+  s->centroid = a.take<float>(4 * (size_t)n + 4);  // 2 n centroid floats (upper bound) + n bucket ints
+  s->ev_bucket = a.take<int>(n + 1);
+  s->ev_value = a.take<float>(n + 1);
+  s->counters = a.take<int>(2);
+}
+
+// d_points: n x 3 floats on the device. d_histogram: `size` floats (size <= 1024). `s` is carved for n points.
+int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, const float* d_points, int64_t n, int size,
+                                float* d_histogram, int32_t** d_error_out) {
   if (size < 1 || size > kThreads) return ctx->fail(DL_ERR_ARG, "histogram size must be in [1, 1024]");
   if (n > (1 << 20)) return ctx->fail(DL_ERR_ARG, "more than 2^20 points in a rotational histogram");
   HistogramArgs h{};
   h.points = d_points;
   h.n = (int)n;
-  int np2 = 64;
-  while (np2 < n) np2 <<= 1;
-  h.np2 = np2;
+  h.np2 = (int)histogram_np2(n);
   h.size = size;
-  h.keys = a.take<unsigned long long>(np2);
-  h.slice_first = a.take<int>(n + 1);
-  h.centroid = a.take<float>(4 * (size_t)n + 4);  // 2 n centroid floats (upper bound) + n bucket ints
-  h.ev_bucket = a.take<int>(n + 1);
-  h.ev_value = a.take<float>(n + 1);
-  h.counters = a.take<int>(2);
+  h.keys = s.keys;
+  h.slice_first = s.slice_first;
+  h.centroid = s.centroid;
+  h.ev_bucket = s.ev_bucket;
+  h.ev_value = s.ev_value;
+  h.counters = s.counters;
   h.histogram = d_histogram;
   DL_CUDA(ctx, cudaMemsetAsync(h.counters, 0, 2 * sizeof(int), ctx->stream));
   if (n == 0) {

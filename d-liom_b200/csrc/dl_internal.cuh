@@ -60,7 +60,8 @@ struct dl_context {
   uint8_t* d_fcsm_lut = nullptr;        // loop-closure search: cell value -> 8-bit precomputation value (dl_fcsm.cu), built on first use
   int in_flight = 0;                    // scans of the submitted, not yet collected batch
   bool in_flight_states = false;        // ... and whether it also stages the estimated IMU states
-  size_t results_staging_offset = 0;    // where in h_pinned the in-flight batch's results land
+  dl_scan_result* staged_results = nullptr;  // where in h_pinned the in-flight batch's results land
+  dl_nav_state* staged_states = nullptr;     // ... and its estimated IMU states
   std::string error;
   int64_t launches = 0;
   // growable scratch arenas (device + pinned host), reused across calls
@@ -183,10 +184,19 @@ struct Arena {  // bump allocator over the context's device scratch; with a null
     return p;
   }
 };
-inline size_t arena_bytes(std::initializer_list<size_t> sizes) {
-  size_t t = 0;
-  for (size_t s : sizes) t = ((t + 255) & ~size_t(255)) + s;
-  return t + 256;
+// Reserves the device scratch of one call and carves it. `carve(Arena&)` makes only takes (no copies, launches or other side
+// effects): it runs once on a counting arena, the reservation is what that took plus `extra` bytes for takes whose sizes are
+// not known before the call's device work, and it runs again on the scratch. `rest`, if given, continues after the carve.
+template <typename Carve>
+int carve_scratch(dl_context* ctx, Carve&& carve, size_t extra = 0, Arena* rest = nullptr) {
+  Arena count(nullptr);
+  carve(count);
+  const int st = ctx->reserve_device(count.off + extra);
+  if (st != DL_OK) return st;
+  Arena a(ctx->d_scratch);
+  carve(a);
+  if (rest) *rest = a;
+  return DL_OK;
 }
 
 // ---- kernel launchers (each defined in its own .cu), all asynchronous on `stream`, device pointers only.
@@ -329,9 +339,17 @@ int launch_window_optimize(dl_context* ctx, int count, const dl_nav_state* state
                            const dl_window_options& opt, dl_nav_state* states_i_out, dl_nav_state* states_j_out,
                            double* information_out, dl_solve_summary* summaries);
 // dl_histogram.cu
-size_t rotational_histogram_scratch_bytes(int64_t n);
-int launch_rotational_histogram(dl_context* ctx, Arena& a, const float* d_points, int64_t n, int size, float* d_histogram,
-                                int32_t** d_error_out);
+struct HistogramScratch {  // device scratch of one rotational histogram of n points
+  unsigned long long* keys;
+  int* slice_first;
+  float* centroid;
+  int* ev_bucket;
+  float* ev_value;
+  int* counters;
+};
+void carve_rotational_histogram(Arena& a, int64_t n, HistogramScratch* s);
+int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, const float* d_points, int64_t n, int size,
+                                float* d_histogram, int32_t** d_error_out);
 // dl_comm.cu: staging buffers of the constraint exchange and the timed all-gather
 int comm_reserve(dl_comm* c, size_t bytes_per_rank);
 void* comm_send_buffer(dl_comm* c);

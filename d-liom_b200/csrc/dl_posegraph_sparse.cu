@@ -570,10 +570,11 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     }
     if (most > 0) {
       const size_t per = (size_t)most * sizeof(int2);
-      DL_TRY_STATUS(agree(ctx->reserve_device(per * (world + 1) + 1024)));
-      Arena a1(ctx->d_scratch);
-      int2* d_send = a1.take<int2>(most);
-      int2* d_recv = a1.take<int2>((size_t)most * world);
+      int2 *d_send, *d_recv;
+      DL_TRY_STATUS(agree(carve_scratch(ctx, [&](Arena& a) {
+        d_send = a.take<int2>(most);
+        d_recv = a.take<int2>((size_t)most * world);
+      })));
       std::vector<int2> send(most, make_int2(-1, -1));
       for (size_t i = 0; i < local_pairs.size(); ++i) send[i] = make_int2(local_pairs[i].first, local_pairs[i].second);
       PG_CUDA(cudaMemcpyAsync(d_send, send.data(), per, cudaMemcpyHostToDevice, ctx->stream));
@@ -642,61 +643,64 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   const Payload pl{P, K};
   const size_t sys = pl.size(), nr = (size_t)std::max(n_red, 1);
   auto I = [](size_t v) { return std::max<size_t>(v, 1); };
-  const size_t doubles = 2 * sys + (size_t)P * (4 * 7 + 4 * 6 + 36 + 1) + I((size_t)M * 72) + I((size_t)M * 6) + I(cons.size()) +
-                         I(K) * 72 + nr * nr + nr + 16;
-  const size_t ints = (size_t)P + S + pose_con.ptr.size() + pose_con.idx.size() + pair_con.ptr.size() + pair_con.idx.size() +
-                      2 * I(K) + sub_pairs.ptr.size() + node_pairs.ptr.size() + node_pairs.idx.size() + 2 * I(R) + blk.ptr.size() +
-                      2 * I(terms.size()) + 16;
-  const size_t bytes = doubles * 8 + ints * 4 + I(cons.size()) * sizeof(dl_spa_constraint) + 48 * 256;  // 256: per-take alignment
-  DL_TRY_STATUS(agree(ctx->reserve_device(bytes)));
-  Arena a(ctx->d_scratch);
-  double* d_sys[2] = {a.take<double>(sys), a.take<double>(sys)};
-  double* d_x = a.take<double>((size_t)7 * P);
-  double* d_cand = a.take<double>((size_t)7 * P);
-  double* d_tmp = a.take<double>((size_t)7 * P);
-  double* d_best = a.take<double>((size_t)7 * P);
-  double* d_J = a.take<double>(I((size_t)M * 72));
-  double* d_e = a.take<double>(I((size_t)M * 6));
-  double* d_c2 = a.take<double>(I(cons.size()));
-  double* d_misc = a.take<double>(8);  // [0] fixed cost2, [1..3] norms, [4..7] step scalars out
+  double *d_sys[2], *d_x, *d_cand, *d_tmp, *d_best, *d_J, *d_e, *d_c2, *d_misc;
   StepBufs sb;
   sb.sys = nullptr;
-  sb.scale = a.take<double>((size_t)6 * P);
-  sb.diag = a.take<double>((size_t)6 * P);
-  sb.znode = a.take<double>((size_t)6 * P);
-  sb.delta = a.take<double>((size_t)6 * P);
-  sb.Lnode = a.take<double>((size_t)36 * P);
-  sb.part = a.take<double>((size_t)P);
-  sb.W = a.take<double>(I(K) * 36);
-  sb.Y = a.take<double>(I(K) * 36);
-  sb.A = a.take<double>(nr * nr);
-  sb.rhs = a.take<double>(nr);
-  sb.scalars = a.take<double>(8);
-  sb.ok = a.take<int>(4);
-  dl_spa_constraint* d_c = a.take<dl_spa_constraint>(I(cons.size()));
-  int* d_dim = a.take<int>(P);
-  int* d_roff = a.take<int>(S);
-  auto up_i = [&](const std::vector<int>& v) -> int* {
-    int* d = a.take<int>(I(v.size()));
-    if (!v.empty()) cudaMemcpyAsync(d, v.data(), v.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
-    return d;
+  dl_spa_constraint* d_c;
+  int *d_dim, *d_roff, *d_pose_ptr, *d_pose_con, *d_pair_ptr, *d_pair_con, *d_sub_ptr, *d_node_ptr, *d_node_pairs, *d_blk_ptr;
+  int2 *d_pairs, *d_blocks, *d_terms;
+  DL_TRY_STATUS(agree(carve_scratch(ctx, [&](Arena& a) {
+    d_sys[0] = a.take<double>(sys);
+    d_sys[1] = a.take<double>(sys);
+    d_x = a.take<double>((size_t)7 * P);
+    d_cand = a.take<double>((size_t)7 * P);
+    d_tmp = a.take<double>((size_t)7 * P);
+    d_best = a.take<double>((size_t)7 * P);
+    d_J = a.take<double>(I((size_t)M * 72));
+    d_e = a.take<double>(I((size_t)M * 6));
+    d_c2 = a.take<double>(I(cons.size()));
+    d_misc = a.take<double>(8);  // [0] fixed cost2, [1..3] norms, [4..7] step scalars out
+    sb.scale = a.take<double>((size_t)6 * P);
+    sb.diag = a.take<double>((size_t)6 * P);
+    sb.znode = a.take<double>((size_t)6 * P);
+    sb.delta = a.take<double>((size_t)6 * P);
+    sb.Lnode = a.take<double>((size_t)36 * P);
+    sb.part = a.take<double>((size_t)P);
+    sb.W = a.take<double>(I(K) * 36);
+    sb.Y = a.take<double>(I(K) * 36);
+    sb.A = a.take<double>(nr * nr);
+    sb.rhs = a.take<double>(nr);
+    sb.scalars = a.take<double>(8);
+    sb.ok = a.take<int>(4);
+    d_c = a.take<dl_spa_constraint>(I(cons.size()));
+    d_dim = a.take<int>(P);
+    d_roff = a.take<int>(S);
+    d_pose_ptr = a.take<int>(I(pose_con.ptr.size()));
+    d_pose_con = a.take<int>(I(pose_con.idx.size()));
+    d_pair_ptr = a.take<int>(I(pair_con.ptr.size()));
+    d_pair_con = a.take<int>(I(pair_con.idx.size()));
+    d_pairs = a.take<int2>(I(pairs2.size()));
+    d_sub_ptr = a.take<int>(I(sub_pairs.ptr.size()));
+    d_node_ptr = a.take<int>(I(node_pairs.ptr.size()));
+    d_node_pairs = a.take<int>(I(node_pairs.idx.size()));
+    d_blocks = a.take<int2>(I(blocks.size()));
+    d_blk_ptr = a.take<int>(I(blk.ptr.size()));
+    d_terms = a.take<int2>(I(terms.size()));
+  })));
+  auto up = [&](void* d, const auto& v) {
+    if (!v.empty()) cudaMemcpyAsync(d, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice, ctx->stream);
   };
-  auto up_2 = [&](const std::vector<int2>& v) -> int2* {
-    int2* d = a.take<int2>(I(v.size()));
-    if (!v.empty()) cudaMemcpyAsync(d, v.data(), v.size() * 8, cudaMemcpyHostToDevice, ctx->stream);
-    return d;
-  };
-  int* d_pose_ptr = up_i(pose_con.ptr);
-  int* d_pose_con = up_i(pose_con.idx);
-  int* d_pair_ptr = up_i(pair_con.ptr);
-  int* d_pair_con = up_i(pair_con.idx);
-  int2* d_pairs = up_2(pairs2);
-  int* d_sub_ptr = up_i(sub_pairs.ptr);
-  int* d_node_ptr = up_i(node_pairs.ptr);
-  int* d_node_pairs = up_i(node_pairs.idx);
-  int2* d_blocks = up_2(blocks);
-  int* d_blk_ptr = up_i(blk.ptr);
-  int2* d_terms = up_2(terms);
+  up(d_pose_ptr, pose_con.ptr);
+  up(d_pose_con, pose_con.idx);
+  up(d_pair_ptr, pair_con.ptr);
+  up(d_pair_con, pair_con.idx);
+  up(d_pairs, pairs2);
+  up(d_sub_ptr, sub_pairs.ptr);
+  up(d_node_ptr, node_pairs.ptr);
+  up(d_node_pairs, node_pairs.idx);
+  up(d_blocks, blocks);
+  up(d_blk_ptr, blk.ptr);
+  up(d_terms, terms);
   PG_CUDA(cudaMemcpyAsync(d_dim, dim.data(), (size_t)P * 4, cudaMemcpyHostToDevice, ctx->stream));
   PG_CUDA(cudaMemcpyAsync(d_roff, roff.data(), (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
   PG_CUDA(cudaMemcpyAsync(d_x, poses, (size_t)P * 56, cudaMemcpyHostToDevice, ctx->stream));
