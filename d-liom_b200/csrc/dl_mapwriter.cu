@@ -1,0 +1,838 @@
+// The assets writer's point pipeline on the device (cartographer_ros/assets_writer.cc:120-160 HandleMessage with the processors
+// of the fork's dlio/config/assets_writer_tongji.lua plus the moving-object removal): trajectory lookup, transform to the map,
+// min_max_range_filter and voxel_filter_and_remove_moving_objects with the reference's restart protocol. See include/dliom_b200.h.
+//
+// One call takes many messages; its rows are numbered in message order ("virtual rows"). Per call:
+//   mw_heads_count / tile prefix   a run is a maximal stretch of a message's rows with the same time bits; count run heads
+//   mw_run_poses                   one pose per run (fp64 lookup + slerp + composition, cast to float), the run of every row,
+//                                  and per message the last run with a pose (integer atomicMax: the batch origin)
+//   mw_select (count / scatter)    transform, Has, range gate, ordered compaction by tile counts (the decode's scheme)
+//   pass 1  mw_insert_hits          cell -> hits in an open-addressing table (64-bit key CAS, 32-bit atomicAdd)
+//   pass 2  mw_rays                 one thread per point walks its ray; consecutive samples in one cell share a lookup and an atomic
+//   pass 3  mw_gate (count/scatter) remove iff !(rays < 3 * hits), ordered compaction into the output
+// The acos / sin of a node interval's slerp are computed on the host (glibc), once per interval; the per-run sin of the
+// interpolation factor is the device's (DESIGN §4).
+#include <algorithm>
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+#include <map>
+#include <vector>
+
+#include "dl_internal.cuh"
+
+using namespace dl;
+
+namespace {
+
+constexpr int kBlock = 256;
+constexpr int kGridHalf = 8192;  // 64 << 8 cells per axis at the largest extent the reference's grid grows to (bits = 8)
+constexpr unsigned long long kEmpty = ~0ull;
+
+struct NodeRec {          // node i of a trajectory, and the slerp constants of the interval (i - 1, i), computed on the host
+  Rigidd pose;
+  double theta, sin_theta;
+  int32_t linear, negative;
+};
+struct TrajRec {
+  int64_t first, count;   // nodes [first, first + count) of the writer's node arrays
+};
+struct MsgRec {
+  int64_t stamp, first_row, voff;  // voff: first virtual row of the message
+  int32_t slot, pad;
+  Rigidd sensor_to_tracking;
+};
+struct RunPose {
+  Rigidf sensor_to_map;
+  int32_t valid;
+};
+enum Counter { kNoPose = 0, kRange = 1, kSamples = 2, kOutside = 3, kNumCounters = 4 };
+
+struct SelectArgs {
+  const float4* rows;
+  int64_t num_rows;          // bound of the call's row buffer
+  const MsgRec* msgs;
+  int num_msgs;
+  int64_t n;                 // virtual rows
+  const int64_t* times;      // the writer's node tables
+  const NodeRec* nodes;
+  const TrajRec* trajs;
+  int32_t* head_tiles;       // per tile: run heads, then their exclusive prefix
+  int32_t* num_runs;
+  int32_t* run_of_row;
+  RunPose* runs;
+  int32_t* msg_last_run;     // -1: no kept point
+  float* origins;            // 3 per message
+  int range_filter;
+  double min_range, max_range;
+  int32_t* keep_tiles;
+  int32_t* num_keep;
+  float4* compact;           // x y z + message index (bits) of every kept point, in order
+  float* out_xyz;            // or x y z only, straight into the output
+  int check_extent;
+  float resolution;
+  unsigned long long* counters;
+};
+
+struct Table {
+  unsigned long long* keys;
+  int32_t* hits;
+  int32_t* rays;
+  int64_t mask;
+  int shift;
+  int32_t* num_cells;
+};
+
+__device__ __forceinline__ int message_of(const MsgRec* msgs, int num_msgs, int64_t v) {
+  int lo = 0, hi = num_msgs;  // last message with voff <= v (empty messages share the next one's voff)
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (msgs[mid].voff <= v) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ int block_inclusive_scan(int value, int* total) {
+  __shared__ int warp_sums[kBlock / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int inc = value;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int o = __shfl_up_sync(0xffffffffu, inc, d);
+    if (lane >= d) inc += o;
+  }
+  __syncthreads();
+  if (lane == 31) warp_sums[warp] = inc;
+  __syncthreads();
+  int base = 0, sum = 0;
+#pragma unroll
+  for (int w = 0; w < kBlock / 32; ++w) {
+    if (w < warp) base += warp_sums[w];
+    sum += warp_sums[w];
+  }
+  *total = sum;
+  return base + inc;
+}
+
+// exclusive prefix of per-tile counts in place (one CTA), total -> *total
+__global__ void __launch_bounds__(kBlock) mw_tile_prefix(int32_t* counts, int tiles, int32_t* total) {
+  __shared__ int carry;
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (int base = 0; base < tiles; base += kBlock) {
+    const int t = base + threadIdx.x;
+    const int v = t < tiles ? counts[t] : 0;
+    int sum;
+    const int inc = block_inclusive_scan(v, &sum);
+    if (t < tiles) counts[t] = carry + inc - v;
+    __syncthreads();
+    if (threadIdx.x == 0) carry += sum;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *total = carry;
+}
+
+struct RowRef {
+  int m;
+  float4 p;
+  bool head;
+};
+__device__ __forceinline__ RowRef row_ref(const SelectArgs& a, int64_t v) {
+  RowRef r;
+  r.m = message_of(a.msgs, a.num_msgs, v);
+  const MsgRec& msg = a.msgs[r.m];
+  const int64_t row = msg.first_row + (v - msg.voff);
+  r.p = a.rows[row];
+  r.head = v == msg.voff || __float_as_uint(a.rows[row - 1].w) != __float_as_uint(r.p.w);
+  return r;
+}
+
+__global__ void __launch_bounds__(kBlock) mw_heads_count(SelectArgs a) {
+  const int64_t v = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  const bool head = v < a.n && row_ref(a, v).head;
+  const int c = __syncthreads_count(head);
+  if (threadIdx.x == 0) a.head_tiles[blockIdx.x] = c;
+}
+
+// TransformInterpolationBuffer::Has + Lookup (transform_interpolation_buffer.cc:45-66) and Interpolate
+// (timestamped_transform.cc:22-37): lower_bound over the node times, an exact tick returns the node's pose unchanged.
+__device__ bool lookup(const int64_t* times, const NodeRec* nodes, int64_t count, int64_t tick, Rigidd* out) {
+  if (count == 0 || tick < times[0] || tick > times[count - 1]) return false;
+  int64_t lo = 0, hi = count;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (times[mid] < tick) lo = mid + 1; else hi = mid;
+  }
+  const NodeRec& e = nodes[lo];
+  if (times[lo] == tick) {
+    *out = e.pose;
+    return true;
+  }
+  const NodeRec& s = nodes[lo - 1];
+  const double duration = (double)(times[lo] - times[lo - 1]) / 1e7;  // common::ToSeconds
+  const double factor = ((double)(tick - times[lo - 1]) / 1e7) / duration;
+  out->t = {s.pose.t.x + (e.pose.t.x - s.pose.t.x) * factor, s.pose.t.y + (e.pose.t.y - s.pose.t.y) * factor,
+            s.pose.t.z + (e.pose.t.z - s.pose.t.z) * factor};
+  double scale0, scale1;  // Eigen QuaternionBase::slerp; theta and sin(theta) of the interval come from the host
+  if (e.linear) {
+    scale0 = 1.0 - factor;
+    scale1 = factor;
+  } else {
+    scale0 = sin((1.0 - factor) * e.theta) / e.sin_theta;
+    scale1 = sin(factor * e.theta) / e.sin_theta;
+  }
+  if (e.negative) scale1 = -scale1;
+  out->q = {scale0 * s.pose.q.w + scale1 * e.pose.q.w, scale0 * s.pose.q.x + scale1 * e.pose.q.x,
+            scale0 * s.pose.q.y + scale1 * e.pose.q.y, scale0 * s.pose.q.z + scale1 * e.pose.q.z};
+  return true;
+}
+
+__global__ void __launch_bounds__(kBlock) mw_run_poses(SelectArgs a) {
+  const int64_t v = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  RowRef r{};
+  if (v < a.n) r = row_ref(a, v);
+  int total;
+  const int inc = block_inclusive_scan(r.head ? 1 : 0, &total);
+  if (v >= a.n) return;
+  const int run = a.head_tiles[blockIdx.x] + inc - 1;
+  a.run_of_row[v] = run;
+  if (!r.head) return;
+  const MsgRec& msg = a.msgs[r.m];
+  // FromSeconds: duration_cast of double seconds to int64 ticks, truncation toward zero
+  const int64_t tick = msg.stamp + (int64_t)((double)r.p.w * 1e7);
+  const TrajRec tr = a.trajs[msg.slot];
+  Rigidd tracking_to_map;
+  RunPose out{};
+  if (lookup(a.times + tr.first, a.nodes + tr.first, tr.count, tick, &tracking_to_map)) {
+    out.sensor_to_map = to_float(compose(tracking_to_map, msg.sensor_to_tracking));
+    out.valid = 1;
+    atomicMax(a.msg_last_run + r.m, run);
+  }
+  a.runs[run] = out;
+}
+
+// origin = sensor_to_map * Vector3f::Zero() of the message's last kept point
+__global__ void mw_origins(SelectArgs a) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= a.num_msgs) return;
+  const int run = a.msg_last_run[m];
+  Vec3f o{__int_as_float(0x7fc00000), __int_as_float(0x7fc00000), __int_as_float(0x7fc00000)};
+  if (run >= 0) o = apply(a.runs[run].sensor_to_map, Vec3f{0.f, 0.f, 0.f});
+  a.origins[3 * m] = o.x;
+  a.origins[3 * m + 1] = o.y;
+  a.origins[3 * m + 2] = o.z;
+}
+
+__device__ __forceinline__ bool in_extent(const Int3& c) {
+  return c.x >= -kGridHalf && c.x < kGridHalf && c.y >= -kGridHalf && c.y < kGridHalf && c.z >= -kGridHalf && c.z < kGridHalf;
+}
+__device__ __forceinline__ unsigned long long cell_key(const Int3& c) {
+  return ((unsigned long long)(c.x + kGridHalf) << 28) | ((unsigned long long)(c.y + kGridHalf) << 14) |
+         (unsigned long long)(c.z + kGridHalf);
+}
+__device__ __forceinline__ int64_t slot_of(const Table& t, unsigned long long key) {
+  return (int64_t)((key * 0x9E3779B97F4A7C15ull) >> t.shift);
+}
+
+// kind 0: count kept rows per tile; kind 1: scatter them in order (compact list and / or x y z output)
+template <int kind>
+__global__ void __launch_bounds__(kBlock) mw_select(SelectArgs a) {
+  const int64_t v = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  bool keep = false, no_pose = false, out_of_range = false, outside = false;
+  Vec3f q{};
+  int m = 0;
+  if (v < a.n) {
+    m = message_of(a.msgs, a.num_msgs, v);
+    const MsgRec& msg = a.msgs[m];
+    const float4 p = a.rows[msg.first_row + (v - msg.voff)];
+    const RunPose pose = a.runs[a.run_of_row[v]];
+    if (!pose.valid) {
+      no_pose = true;
+    } else {
+      q = apply(pose.sensor_to_map, Vec3f{p.x, p.y, p.z});
+      keep = true;
+      if (a.range_filter) {
+        const Vec3f o{a.origins[3 * m], a.origins[3 * m + 1], a.origins[3 * m + 2]};
+        const double range = (double)norm3(sub(q, o));
+        if (!(a.min_range <= range && range <= a.max_range)) {
+          keep = false;
+          out_of_range = true;
+        }
+      }
+      // Pass 1 also checks the batch origin: with both ends of every ray inside the extent a ray is at most ~28 400 voxels
+      // long, so pass 2's float step x += voxel_size always advances (a far origin would stall it and loop forever).
+      if (keep && kind == 0 && a.check_extent)
+        outside = !in_extent(cell_index(q, a.resolution)) ||
+                  !in_extent(cell_index(Vec3f{a.origins[3 * m], a.origins[3 * m + 1], a.origins[3 * m + 2]}, a.resolution));
+    }
+  }
+  if (kind == 0) {
+    const int c = __syncthreads_count(keep);
+    const int c_no_pose = __syncthreads_count(no_pose);
+    const int c_range = __syncthreads_count(out_of_range);
+    const int c_outside = __syncthreads_count(outside);
+    if (threadIdx.x == 0) {
+      a.keep_tiles[blockIdx.x] = c;
+      if (c_no_pose) atomicAdd(a.counters + kNoPose, (unsigned long long)c_no_pose);
+      if (c_range) atomicAdd(a.counters + kRange, (unsigned long long)c_range);
+      if (c_outside) atomicAdd(a.counters + kOutside, (unsigned long long)c_outside);
+    }
+    return;
+  }
+  int total;
+  const int inc = block_inclusive_scan(keep ? 1 : 0, &total);
+  if (!keep) return;
+  const int64_t pos = (int64_t)a.keep_tiles[blockIdx.x] + inc - 1;
+  if (a.compact) a.compact[pos] = make_float4(q.x, q.y, q.z, __int_as_float(m));
+  if (a.out_xyz) {
+    a.out_xyz[3 * pos] = q.x;
+    a.out_xyz[3 * pos + 1] = q.y;
+    a.out_xyz[3 * pos + 2] = q.z;
+  }
+}
+
+// pass 1: ++hits of every kept point's cell (ProcessInPhaseOne)
+__global__ void __launch_bounds__(kBlock) mw_insert_hits(Table t, const float4* pts, int64_t n, float resolution) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = pts[i];
+  const unsigned long long key = cell_key(cell_index(Vec3f{p.x, p.y, p.z}, resolution));
+  for (int64_t s = slot_of(t, key);; s = (s + 1) & t.mask) {
+    unsigned long long k = t.keys[s];
+    if (k == kEmpty) {
+      k = atomicCAS(t.keys + s, kEmpty, key);
+      if (k == kEmpty) {
+        atomicAdd(t.num_cells, 1);
+        k = key;
+      }
+    }
+    if (k == key) {
+      atomicAdd(t.hits + s, 1);
+      return;
+    }
+  }
+}
+
+__device__ __forceinline__ int64_t find(const Table& t, unsigned long long key) {
+  for (int64_t s = slot_of(t, key);; s = (s + 1) & t.mask) {
+    const unsigned long long k = t.keys[s];
+    if (k == key) return s;
+    if (k == kEmpty) return -1;
+  }
+}
+
+// table growth: every cell moves to the larger table with its counts
+__global__ void __launch_bounds__(kBlock) mw_rehash(Table to, Table from, int64_t from_cap) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (i >= from_cap) return;
+  const unsigned long long key = from.keys[i];
+  if (key == kEmpty) return;
+  int64_t s = slot_of(to, key);
+  while (atomicCAS(to.keys + s, kEmpty, key) != kEmpty) s = (s + 1) & to.mask;
+  to.hits[s] = from.hits[i];
+  to.rays[s] = from.rays[i];
+}
+
+// pass 2 (ProcessInPhaseTwo): samples at x = 0, voxel_size, ... (< length, x a float advanced in double) along the ray from the
+// batch origin; a sample's cell gains a ray if it has hits. Consecutive samples in one cell are counted with one lookup.
+__global__ void __launch_bounds__(kBlock) mw_rays(Table t, const float4* pts, int64_t n, const float* origins, float resolution,
+                                                  double voxel_size, unsigned long long* counters) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  long long samples = 0;
+  if (i < n) {
+    const float4 p = pts[i];
+    const int m = __float_as_int(p.w);
+    const Vec3f o{origins[3 * m], origins[3 * m + 1], origins[3 * m + 2]};
+    const Vec3f delta = sub(Vec3f{p.x, p.y, p.z}, o);
+    const float length = norm3(delta);
+    const CellDivider div = make_divider(resolution);
+    unsigned long long run_key = kEmpty;
+    int run_count = 0;
+    for (float x = 0.f; x < length; x = (float)((double)x + voxel_size)) {
+      ++samples;
+      const float s = x / length;
+      const Int3 c = cell_index(add(o, mul(s, delta)), div);
+      const unsigned long long key = in_extent(c) ? cell_key(c) : kEmpty;  // beyond the extent: reads 0 hits
+      if (key != run_key) {
+        if (run_count > 0 && run_key != kEmpty) {
+          const int64_t slot = find(t, run_key);
+          if (slot >= 0) atomicAdd(t.rays + slot, run_count);
+        }
+        run_key = key;
+        run_count = 0;
+      }
+      ++run_count;
+    }
+    if (run_count > 0 && run_key != kEmpty) {
+      const int64_t slot = find(t, run_key);
+      if (slot >= 0) atomicAdd(t.rays + slot, run_count);
+    }
+  }
+  // block sum of the sample counts, one 64-bit integer atomic per block
+  __shared__ long long warp_sums[kBlock / 32];
+  for (int d = 16; d > 0; d >>= 1) samples += __shfl_down_sync(0xffffffffu, samples, d);
+  if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = samples;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long s = 0;
+    for (int w = 0; w < kBlock / 32; ++w) s += warp_sums[w];
+    if (s) atomicAdd(counters + kSamples, (unsigned long long)s);
+  }
+}
+
+// pass 3 (ProcessInPhaseThree): keep iff rays < 3 * hits (kMissPerHitLimit, compared in double); kind 0 counts, 1 scatters
+template <int kind>
+__global__ void __launch_bounds__(kBlock) mw_gate(Table t, const float4* pts, int64_t n, float resolution, int32_t* tiles,
+                                                  float* out_xyz) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  bool keep = false;
+  float4 p{};
+  if (i < n) {
+    p = pts[i];
+    const Int3 c = cell_index(Vec3f{p.x, p.y, p.z}, resolution);
+    int hits = 0, rays = 0;
+    const int64_t slot = in_extent(c) ? find(t, cell_key(c)) : -1;
+    if (slot >= 0) {
+      hits = t.hits[slot];
+      rays = t.rays[slot];
+    }
+    keep = (double)rays < 3.0 * (double)hits;
+  }
+  if (kind == 0) {
+    const int c = __syncthreads_count(keep);
+    if (threadIdx.x == 0) tiles[blockIdx.x] = c;
+    return;
+  }
+  int total;
+  const int inc = block_inclusive_scan(keep ? 1 : 0, &total);
+  if (!keep) return;
+  const int64_t pos = (int64_t)tiles[blockIdx.x] + inc - 1;
+  out_xyz[3 * pos] = p.x;
+  out_xyz[3 * pos + 1] = p.y;
+  out_xyz[3 * pos + 2] = p.z;
+}
+
+unsigned tiles_of(int64_t n) { return (unsigned)((n + kBlock - 1) / kBlock); }
+
+#define MW_TRY(expr)                \
+  do {                              \
+    const int st__ = (expr);        \
+    if (st__ != DL_OK) return st__; \
+  } while (0)
+
+}  // namespace
+
+struct dl_map_writer {
+  dl_context* ctx = nullptr;
+  dl_map_writer_options options{};
+  float resolution = 0.f;          // (float)outlier_voxel_size: HybridGridBase's float resolution
+  std::map<int32_t, int32_t> slot_of;  // trajectory id -> slot
+  std::vector<TrajRec> trajs;
+  std::vector<int64_t> times;
+  std::vector<NodeRec> nodes;
+  bool tables_dirty = false;
+  int64_t* d_times = nullptr;
+  NodeRec* d_nodes = nullptr;
+  TrajRec* d_trajs = nullptr;
+  int pass = 0;                    // 0 .. num_passes - 1
+  bool started = false, finished = false;
+  RunPose* d_runs = nullptr;
+  int64_t runs_capacity = 0;
+  Table table{};                   // cell -> (hits, rays)
+  int64_t table_capacity = 0;
+  int64_t num_cells = 0;
+
+  int num_passes() const { return options.outlier_voxel_size > 0 ? 3 : 1; }
+  bool final_pass() const { return pass == num_passes() - 1; }
+
+  int upload_tables() {
+    if (!tables_dirty) return DL_OK;
+    cudaFree(d_times);
+    cudaFree(d_nodes);
+    cudaFree(d_trajs);
+    d_times = nullptr; d_nodes = nullptr; d_trajs = nullptr;
+    const size_t nn = std::max<size_t>(nodes.size(), 1), nt = std::max<size_t>(trajs.size(), 1);
+    DL_CUDA(ctx, cudaMalloc(&d_times, nn * sizeof(int64_t)));
+    DL_CUDA(ctx, cudaMalloc(&d_nodes, nn * sizeof(NodeRec)));
+    DL_CUDA(ctx, cudaMalloc(&d_trajs, nt * sizeof(TrajRec)));
+    DL_CUDA(ctx, cudaMemcpy(d_times, times.data(), times.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
+    DL_CUDA(ctx, cudaMemcpy(d_nodes, nodes.data(), nodes.size() * sizeof(NodeRec), cudaMemcpyHostToDevice));
+    DL_CUDA(ctx, cudaMemcpy(d_trajs, trajs.data(), trajs.size() * sizeof(TrajRec), cudaMemcpyHostToDevice));
+    tables_dirty = false;
+    return DL_OK;
+  }
+  int reserve_runs(int64_t n) {
+    if (n <= runs_capacity) return DL_OK;
+    const int64_t cap = std::max<int64_t>({n, 2 * runs_capacity, 4096});
+    DL_CUDA(ctx, ctx->wait_stream());
+    cudaFree(d_runs);
+    d_runs = nullptr;
+    runs_capacity = 0;
+    DL_CUDA(ctx, cudaMalloc(&d_runs, (size_t)cap * sizeof(RunPose)));
+    runs_capacity = cap;
+    return DL_OK;
+  }
+  static int alloc_table(dl_context* ctx, int64_t cap, Table* t) {
+    int shift = 64;
+    for (int64_t c = cap; c > 1; c >>= 1) --shift;
+    t->mask = cap - 1;
+    t->shift = shift;
+    DL_CUDA(ctx, cudaMalloc(&t->keys, (size_t)cap * sizeof(unsigned long long)));
+    DL_CUDA(ctx, cudaMalloc(&t->hits, (size_t)cap * sizeof(int32_t)));
+    DL_CUDA(ctx, cudaMalloc(&t->rays, (size_t)cap * sizeof(int32_t)));
+    DL_CUDA(ctx, cudaMemsetAsync(t->keys, 0xff, (size_t)cap * sizeof(unsigned long long), ctx->stream));
+    DL_CUDA(ctx, cudaMemsetAsync(t->hits, 0, (size_t)cap * sizeof(int32_t), ctx->stream));
+    DL_CUDA(ctx, cudaMemsetAsync(t->rays, 0, (size_t)cap * sizeof(int32_t), ctx->stream));
+    return DL_OK;
+  }
+  static void free_table(Table* t) {
+    cudaFree(t->keys);
+    cudaFree(t->hits);
+    cudaFree(t->rays);
+    t->keys = nullptr; t->hits = nullptr; t->rays = nullptr;
+  }
+  // Load factor <= 1/2 after `adding` more cells: sized from the count of kept points before they are inserted.
+  int reserve_table(int64_t adding) {
+    int64_t cap = 1024;
+    while (cap < 2 * (num_cells + adding)) cap <<= 1;
+    if (cap <= table_capacity) return DL_OK;
+    Table fresh{};
+    const int st = alloc_table(ctx, cap, &fresh);
+    if (st != DL_OK) {
+      free_table(&fresh);
+      return st;
+    }
+    if (table_capacity > 0) {
+      mw_rehash<<<tiles_of(table_capacity), kBlock, 0, ctx->stream>>>(fresh, table, table_capacity);
+      DL_LAUNCH_CHECK(ctx, "mw_rehash");
+    }
+    DL_CUDA(ctx, ctx->wait_stream());
+    fresh.num_cells = table.num_cells;
+    free_table(&table);
+    table = fresh;
+    table_capacity = cap;
+    return DL_OK;
+  }
+  int process(int32_t num_messages, const dl_map_message* messages, const float* rows_host, const float* rows_dev,
+              int64_t num_rows, float* points_host, float* points_dev, int64_t* num_points_out, float* origins_out,
+              dl_map_writer_info* info);
+};
+
+namespace {
+
+bool valid_pose7(const double* p) {
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(p[k])) return false;
+  return true;
+}
+
+}  // namespace
+
+int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages, const float* rows_host, const float* rows_dev,
+                           int64_t num_rows, float* points_host, float* points_dev, int64_t* num_points_out, float* origins_out,
+                           dl_map_writer_info* info) {
+  if (!num_points_out || num_messages < 0 || (num_messages > 0 && !messages) || num_rows < 0)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: bad arguments");
+  if (finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: the final pass was flushed");
+  // validate every message before any work
+  std::vector<MsgRec> msgs((size_t)std::max(num_messages, 1));
+  int64_t n = 0;
+  for (int32_t m = 0; m < num_messages; ++m) {
+    const dl_map_message& g = messages[m];
+    const auto it = slot_of.find(g.trajectory_id);
+    if (it == slot_of.end()) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: unknown trajectory " + std::to_string(g.trajectory_id));
+    if (g.first_row < 0 || g.num_rows < 0 || g.first_row > num_rows || g.num_rows > num_rows - g.first_row)
+      return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: message rows outside the row buffer");
+    if (!valid_pose7(g.sensor_to_tracking)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: sensor_to_tracking is not finite");
+    msgs[m] = MsgRec{g.stamp, g.first_row, n, it->second, 0, pose_from7(g.sensor_to_tracking)};
+    n += g.num_rows;
+  }
+  if (n >= (1ll << 31)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: more than 2^31 - 1 rows in one call");
+  if (n > 0 && !rows_host && !rows_dev) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: no rows");
+  if (n > 0 && final_pass() && !points_host && !points_dev) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: no points_out");
+  if (rows_dev && ((uintptr_t)rows_dev & 15) != 0) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: rows must be 16-byte aligned");
+  *num_points_out = 0;
+  dl_map_writer_info local{};
+  local.pass = pass;
+  local.final_pass = final_pass() ? 1 : 0;
+  local.num_rows = n;
+  local.messages_without_batch = num_messages;
+  if (n == 0) {
+    if (origins_out) for (int64_t k = 0; k < 3 * (int64_t)num_messages; ++k) origins_out[k] = NAN;
+    started = true;
+    if (info) *info = local;
+    return DL_OK;
+  }
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  MW_TRY(upload_tables());
+  const unsigned tiles = tiles_of(n);
+  SelectArgs a{};
+  float4* up_rows = nullptr;
+  MsgRec* d_msgs = nullptr;
+  int32_t* d_ints = nullptr;  // [0] runs, [1] kept, [2] gate survivors
+  float* d_out = nullptr;
+  int32_t* gate_tiles = nullptr;
+  MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+    if (rows_host) up_rows = ar.take<float4>((size_t)num_rows);
+    d_msgs = ar.take<MsgRec>((size_t)num_messages);
+    a.head_tiles = ar.take<int32_t>(tiles);
+    a.keep_tiles = ar.take<int32_t>(tiles);
+    gate_tiles = ar.take<int32_t>(tiles);
+    a.run_of_row = ar.take<int32_t>((size_t)n);
+    a.msg_last_run = ar.take<int32_t>((size_t)num_messages);
+    a.origins = ar.take<float>(3 * (size_t)num_messages);
+    a.counters = ar.take<unsigned long long>(kNumCounters);
+    d_ints = ar.take<int32_t>(3);
+    a.compact = ar.take<float4>((size_t)n);
+    if (points_host) d_out = ar.take<float>(3 * (size_t)n);
+  }));
+  if (rows_host) {
+    DL_CUDA(ctx, cudaMemcpyAsync(up_rows, rows_host, (size_t)num_rows * 16, cudaMemcpyHostToDevice, ctx->stream));
+    a.rows = up_rows;
+  } else {
+    a.rows = reinterpret_cast<const float4*>(rows_dev);
+  }
+  if (!d_out) d_out = points_dev;
+  DL_CUDA(ctx, cudaMemcpyAsync(d_msgs, msgs.data(), (size_t)num_messages * sizeof(MsgRec), cudaMemcpyHostToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(a.msg_last_run, 0xff, (size_t)num_messages * sizeof(int32_t), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(a.counters, 0, kNumCounters * sizeof(unsigned long long), ctx->stream));
+  a.num_rows = num_rows;
+  a.msgs = d_msgs;
+  a.num_msgs = num_messages;
+  a.n = n;
+  a.times = d_times;
+  a.nodes = d_nodes;
+  a.trajs = d_trajs;
+  a.num_runs = d_ints;
+  a.num_keep = d_ints + 1;
+  a.range_filter = options.range_filter;
+  a.min_range = options.min_range;
+  a.max_range = options.max_range;
+  a.resolution = resolution;
+  a.check_extent = options.outlier_voxel_size > 0 && pass == 0;
+
+  // runs and their poses: the number of runs is counted before the pose table is sized
+  mw_heads_count<<<tiles, kBlock, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "mw_heads_count");
+  mw_tile_prefix<<<1, kBlock, 0, ctx->stream>>>(a.head_tiles, (int)tiles, a.num_runs);
+  DL_LAUNCH_CHECK(ctx, "mw_tile_prefix");
+  int32_t num_runs = 0;
+  DL_CUDA(ctx, cudaMemcpyAsync(&num_runs, a.num_runs, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  MW_TRY(reserve_runs(num_runs));
+  a.runs = d_runs;
+  mw_run_poses<<<tiles, kBlock, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "mw_run_poses");
+  mw_origins<<<(num_messages + 127) / 128, 128, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "mw_origins");
+  // transform, Has, range gate, ordered compaction
+  mw_select<0><<<tiles, kBlock, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "mw_select<0>");
+  mw_tile_prefix<<<1, kBlock, 0, ctx->stream>>>(a.keep_tiles, (int)tiles, a.num_keep);
+  DL_LAUNCH_CHECK(ctx, "mw_tile_prefix");
+  const bool direct = final_pass() && options.outlier_voxel_size <= 0;
+  SelectArgs s = a;
+  if (direct) {
+    s.compact = nullptr;
+    s.out_xyz = d_out;
+  }
+  mw_select<1><<<tiles, kBlock, 0, ctx->stream>>>(s);
+  DL_LAUNCH_CHECK(ctx, "mw_select<1>");
+  unsigned long long counters[kNumCounters];
+  int32_t kept = 0;
+  std::vector<int32_t> last_run((size_t)num_messages);
+  DL_CUDA(ctx, cudaMemcpyAsync(counters, a.counters, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(&kept, a.num_keep, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(last_run.data(), a.msg_last_run, (size_t)num_messages * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                               ctx->stream));
+  if (origins_out)
+    DL_CUDA(ctx, cudaMemcpyAsync(origins_out, a.origins, 3 * (size_t)num_messages * sizeof(float), cudaMemcpyDeviceToHost,
+                                 ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  if (counters[kOutside] > 0)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: a point's or its batch origin's cell lies beyond +-8192 cells (the hybrid "
+                                 "grid's largest extent)");
+  local.dropped_no_pose = (int64_t)counters[kNoPose];
+  local.dropped_range = (int64_t)counters[kRange];
+  local.messages_without_batch = std::count(last_run.begin(), last_run.end(), -1);
+
+  if (options.outlier_voxel_size > 0) MW_TRY(reserve_table(pass == 0 ? kept : 0));
+  int64_t out_count = 0;
+  if (direct) {
+    out_count = kept;
+  } else if (pass == 0) {
+    if (kept > 0) {
+      mw_insert_hits<<<tiles_of(kept), kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution);
+      DL_LAUNCH_CHECK(ctx, "mw_insert_hits");
+    }
+  } else if (pass == 1) {
+    if (kept > 0) {
+      mw_rays<<<tiles_of(kept), kBlock, 0, ctx->stream>>>(table, a.compact, kept, a.origins, resolution, options.outlier_voxel_size,
+                                                          a.counters);
+      DL_LAUNCH_CHECK(ctx, "mw_rays");
+    }
+  } else if (kept > 0) {
+    const unsigned gt = tiles_of(kept);
+    mw_gate<0><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, nullptr);
+    DL_LAUNCH_CHECK(ctx, "mw_gate<0>");
+    mw_tile_prefix<<<1, kBlock, 0, ctx->stream>>>(gate_tiles, (int)gt, d_ints + 2);
+    DL_LAUNCH_CHECK(ctx, "mw_tile_prefix");
+    mw_gate<1><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, d_out);
+    DL_LAUNCH_CHECK(ctx, "mw_gate<1>");
+    int32_t survivors = 0;
+    DL_CUDA(ctx, cudaMemcpyAsync(&survivors, d_ints + 2, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
+    out_count = survivors;
+    local.dropped_moving = kept - survivors;
+  }
+  DL_CUDA(ctx, cudaMemcpyAsync(counters, a.counters, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
+  int32_t cells = 0;
+  if (table.num_cells) DL_CUDA(ctx, cudaMemcpyAsync(&cells, table.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  if (points_host && out_count > 0)
+    DL_CUDA(ctx, cudaMemcpyAsync(points_host, d_out, 3 * (size_t)out_count * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  num_cells = cells;
+  local.num_samples = (int64_t)counters[kSamples];
+  local.num_points_out = out_count;
+  *num_points_out = out_count;
+  started = true;
+  if (info) *info = local;
+  return DL_OK;
+}
+
+int dl_map_writer_create(dl_context* ctx, const dl_map_writer_options* options, dl_map_writer** out) {
+  if (!ctx || !options || !out) return DL_ERR_ARG;
+  const dl_map_writer_options& o = *options;
+  if (o.range_filter != 0 && o.range_filter != 1) return ctx->fail(DL_ERR_ARG, "range_filter must be 0 or 1");
+  if (o.range_filter && (std::isnan(o.min_range) || std::isnan(o.max_range)))
+    return ctx->fail(DL_ERR_ARG, "min_range / max_range must not be NaN");
+  if (!(o.outlier_voxel_size >= 0) || !std::isfinite(o.outlier_voxel_size) ||
+      (o.outlier_voxel_size > 0 && !((float)o.outlier_voxel_size > 0.f)))
+    return ctx->fail(DL_ERR_ARG, "outlier_voxel_size must be finite and >= 0");
+  dl_map_writer* w = new dl_map_writer();
+  w->ctx = ctx;
+  w->options = o;
+  w->resolution = (float)o.outlier_voxel_size;
+  if (o.outlier_voxel_size > 0) {
+    DL_CUDA(ctx, cudaSetDevice(ctx->device));
+    int32_t* counter = nullptr;
+    cudaError_t e = cudaMalloc(&counter, sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMemset(counter, 0, sizeof(int32_t));
+    if (e != cudaSuccess) {
+      cudaFree(counter);
+      delete w;
+      return ctx->cuda_fail(e, "dl_map_writer_create");
+    }
+    w->table.num_cells = counter;
+  }
+  *out = w;
+  return DL_OK;
+}
+
+void dl_map_writer_destroy(dl_map_writer* w) {
+  if (!w) return;
+  cudaSetDevice(w->ctx->device);
+  cudaStreamSynchronize(w->ctx->stream);
+  dl_map_writer::free_table(&w->table);
+  cudaFree(w->table.num_cells);
+  cudaFree(w->d_runs);
+  cudaFree(w->d_times);
+  cudaFree(w->d_nodes);
+  cudaFree(w->d_trajs);
+  delete w;
+}
+
+int dl_map_writer_add_trajectory(dl_map_writer* w, int32_t trajectory_id, int32_t num_nodes, const int64_t* times,
+                                 const double* poses) {
+  if (!w) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  if (num_nodes < 0 || (num_nodes > 0 && (!times || !poses))) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_trajectory: bad arguments");
+  if (w->started || w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_trajectory: processing has begun");
+  if (w->slot_of.count(trajectory_id)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_trajectory: trajectory added twice");
+  for (int32_t i = 0; i < num_nodes; ++i) {
+    if (!valid_pose7(poses + 7 * (size_t)i)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_trajectory: a pose is not finite");
+    // TransformInterpolationBuffer::Push: CHECK_GE(time, latest_time())
+    if (i > 0 && times[i] < times[i - 1]) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_trajectory: node times decrease");
+  }
+  const int64_t first = (int64_t)w->nodes.size();
+  for (int32_t i = 0; i < num_nodes; ++i) {
+    NodeRec r{};
+    r.pose = pose_from7(poses + 7 * (size_t)i);
+    if (i > 0) {
+      // the interval-constant half of Eigen's slerp, with the host's acos / sin
+      const Quatd& s = w->nodes.back().pose.q;
+      const Quatd& e = r.pose.q;
+      const double d = (s.x * e.x + s.y * e.y) + (s.z * e.z + s.w * e.w);
+      const double abs_d = std::fabs(d);
+      r.linear = abs_d >= 1.0 - DBL_EPSILON;
+      r.negative = d < 0.0;
+      r.theta = r.linear ? 0.0 : std::acos(abs_d);
+      r.sin_theta = r.linear ? 1.0 : std::sin(r.theta);
+    }
+    w->nodes.push_back(r);
+    w->times.push_back(times[i]);
+  }
+  w->slot_of[trajectory_id] = (int32_t)w->trajs.size();
+  w->trajs.push_back(TrajRec{first, num_nodes});
+  w->tables_dirty = true;
+  return DL_OK;
+}
+
+int dl_map_writer_process(dl_map_writer* w, int32_t num_messages, const dl_map_message* messages, const float* xyzt_rows,
+                          int64_t num_rows, float* points_out, int64_t* num_points_out, float* origins_out,
+                          dl_map_writer_info* info) {
+  if (!w) return DL_ERR_ARG;
+  return w->process(num_messages, messages, xyzt_rows, nullptr, num_rows, points_out, nullptr, num_points_out, origins_out, info);
+}
+
+int dl_map_writer_process_dev(dl_map_writer* w, int32_t num_messages, const dl_map_message* messages, const float* xyzt_rows_dev,
+                              int64_t num_rows, float* points_out_dev, int64_t* num_points_out, float* origins_out,
+                              dl_map_writer_info* info) {
+  if (!w) return DL_ERR_ARG;
+  return w->process(num_messages, messages, nullptr, xyzt_rows_dev, num_rows, nullptr, points_out_dev, num_points_out, origins_out,
+                    info);
+}
+
+int dl_map_writer_flush(dl_map_writer* w, int32_t* restart) {
+  if (!w || !restart) return DL_ERR_ARG;
+  if (w->finished) return w->ctx->fail(DL_ERR_ARG, "dl_map_writer_flush: the final pass was flushed");
+  if (w->final_pass()) {
+    w->finished = true;
+    *restart = 0;
+  } else {
+    ++w->pass;
+    *restart = 1;
+  }
+  return DL_OK;
+}
+
+int dl_map_writer_voxels(const dl_map_writer* w, int64_t capacity, int32_t* cells_xyz, int32_t* hits, int32_t* rays, int64_t* count) {
+  if (!w || !count || capacity < 0) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  *count = w->num_cells;
+  if (!cells_xyz) return DL_OK;
+  if (capacity < w->num_cells || !hits || !rays) return ctx->fail(DL_ERR_ARG, "dl_map_writer_voxels: capacity below the cell count");
+  if (w->table_capacity == 0) return DL_OK;
+  const size_t cap = (size_t)w->table_capacity;
+  std::vector<unsigned long long> keys(cap);
+  std::vector<int32_t> h(cap), r(cap);
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  DL_CUDA(ctx, cudaMemcpy(keys.data(), w->table.keys, cap * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  DL_CUDA(ctx, cudaMemcpy(h.data(), w->table.hits, cap * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  DL_CUDA(ctx, cudaMemcpy(r.data(), w->table.rays, cap * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  std::vector<size_t> order;
+  for (size_t i = 0; i < cap; ++i)
+    if (keys[i] != kEmpty) order.push_back(i);
+  std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return keys[a] < keys[b]; });  // key order = (x, y, z) order
+  for (size_t k = 0; k < order.size(); ++k) {
+    const unsigned long long key = keys[order[k]];
+    cells_xyz[3 * k] = (int32_t)((key >> 28) & 0x3fff) - kGridHalf;
+    cells_xyz[3 * k + 1] = (int32_t)((key >> 14) & 0x3fff) - kGridHalf;
+    cells_xyz[3 * k + 2] = (int32_t)(key & 0x3fff) - kGridHalf;
+    hits[k] = h[order[k]];
+    rays[k] = r[order[k]];
+  }
+  *count = (int64_t)order.size();
+  return DL_OK;
+}

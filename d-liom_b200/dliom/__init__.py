@@ -37,6 +37,8 @@ EXPORTS = [
     "dl_pose_graph_3d_create", "dl_pose_graph_3d_destroy", "dl_pose_graph_3d_add_node", "dl_pose_graph_3d_freeze_trajectory",
     "dl_pose_graph_3d_run_final_optimization", "dl_pose_graph_3d_poses", "dl_pose_graph_3d_local_to_global",
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
+    "dl_map_writer_create", "dl_map_writer_destroy", "dl_map_writer_add_trajectory", "dl_map_writer_process",
+    "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels",
 ]
 
 
@@ -353,6 +355,25 @@ class Pg3dSearch(C.Structure):   # dl_pg3d_search
                 ("node_index", C.c_int32), ("pose_guess", C.c_double * 7), ("result", Constraint)]
 
 
+class MapWriterOptions(C.Structure):   # dl_map_writer_options
+    _fields_ = [("range_filter", C.c_int32), ("reserved", C.c_int32), ("min_range", C.c_double), ("max_range", C.c_double),
+                ("outlier_voxel_size", C.c_double)]
+
+
+class MapMessage(C.Structure):   # dl_map_message
+    _fields_ = [("stamp", C.c_int64), ("first_row", C.c_int64), ("num_rows", C.c_int64), ("trajectory_id", C.c_int32),
+                ("reserved", C.c_int32), ("sensor_to_tracking", C.c_double * 7)]
+
+
+class MapWriterInfo(C.Structure):   # dl_map_writer_info
+    _fields_ = [("pass_", C.c_int32), ("final_pass", C.c_int32), ("num_rows", C.c_int64), ("dropped_no_pose", C.c_int64),
+                ("dropped_range", C.c_int64), ("dropped_moving", C.c_int64), ("messages_without_batch", C.c_int64),
+                ("num_samples", C.c_int64), ("num_points_out", C.c_int64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 PG3D_INTRA_SUBMAP, PG3D_INTER_SUBMAP = 0, 1
 PG3D_NODE_POSES, PG3D_SUBMAP_POSES, PG3D_OPTIMIZATION_NODES, PG3D_OPTIMIZATION_SUBMAPS = 0, 1, 2, 3
 
@@ -472,6 +493,14 @@ def lib():
     L.dl_pose_graph_3d_constraints.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
     L.dl_pose_graph_3d_last_searches.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
     L.dl_pose_graph_3d_store_bytes.argtypes = [vp, ip(C.c_int64), ip(C.c_int64)]
+    L.dl_map_writer_create.argtypes = [vp, ip(MapWriterOptions), ip(vp)]
+    L.dl_map_writer_destroy.argtypes = [vp]
+    L.dl_map_writer_destroy.restype = None
+    L.dl_map_writer_add_trajectory.argtypes = [vp, C.c_int32, C.c_int32, vp, vp]
+    L.dl_map_writer_process.argtypes = [vp, C.c_int32, vp, vp, C.c_int64, vp, ip(C.c_int64), vp, ip(MapWriterInfo)]
+    L.dl_map_writer_process_dev.argtypes = [vp, C.c_int32, vp, vp, C.c_int64, vp, ip(C.c_int64), vp, ip(MapWriterInfo)]
+    L.dl_map_writer_flush.argtypes = [vp, ip(C.c_int32)]
+    L.dl_map_writer_voxels.argtypes = [vp, C.c_int64, vp, vp, vp, ip(C.c_int64)]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
     L.dl_ltb_create.argtypes = [vp, ip(LtbOptions), ip(vp)]
     L.dl_ltb_destroy.argtypes = [vp]
@@ -1181,6 +1210,113 @@ class PoseGraph3D:
         up, cap = C.c_int64(0), C.c_int64(0)
         self.ctx.check(self.ctx.L.dl_pose_graph_3d_store_bytes(self.h, C.byref(up), C.byref(cap)))
         return up.value, cap.value
+
+
+def seconds_to_ticks(seconds):
+    """Seconds -> universal ticks of 100 ns, llround(t * 1e7) (rounded half away from zero), for node times given in seconds
+    (dl_pg3d_node::time) where the map writer takes ticks (proto::Trajectory::Node::timestamp)."""
+    t = np.asarray(seconds, np.float64) * 1e7
+    whole = np.trunc(t)
+    return (whole + np.sign(t) * (np.abs(t - whole) >= 0.5)).astype(np.int64)
+
+
+class MapWriter:
+    """The assets writer's point pipeline (dl_map_writer_*): trajectory lookup and transform to the map, optional
+    min_max_range_filter and voxel_filter_and_remove_moving_objects, with the restart protocol: stream every message through
+    process(), then flush(); repeat while flush() returns True. Output points come from the final pass only."""
+
+    def __init__(self, ctx, range_filter=None, outlier_voxel_size=0.0):
+        """range_filter: None or (min_range, max_range)."""
+        self.ctx = ctx
+        o = MapWriterOptions()
+        if range_filter is not None:
+            o.range_filter, o.min_range, o.max_range = 1, float(range_filter[0]), float(range_filter[1])
+        o.outlier_voxel_size = float(outlier_voxel_size)
+        self.h = C.c_void_p()
+        ctx.check(ctx.L.dl_map_writer_create(ctx.h, C.byref(o), C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.ctx.L.dl_map_writer_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):
+            self.close()
+
+    def add_trajectory(self, trajectory_id, times_ticks, poses):
+        t = np.ascontiguousarray(times_ticks, np.int64)
+        p = np.ascontiguousarray(poses, np.float64).reshape(-1, 7)
+        self.ctx.check(self.ctx.L.dl_map_writer_add_trajectory(self.h, int(trajectory_id), len(t), t.ctypes.data, p.ctypes.data))
+
+    def add_pose_graph_trajectory(self, graph, trajectory_id, node_times_seconds):
+        """A PoseGraph3D trajectory: its node poses (GetTrajectoryNodePoses) at the nodes' times, converted with seconds_to_ticks."""
+        self.add_trajectory(trajectory_id, seconds_to_ticks(node_times_seconds), graph.node_poses(trajectory_id))
+
+    @staticmethod
+    def messages(msgs):
+        """[(stamp ticks, first_row, num_rows, trajectory_id, sensor_to_tracking7)] -> a dl_map_message array"""
+        arr = (MapMessage * max(len(msgs), 1))()
+        for k, (stamp, first, n, traj, s2t) in enumerate(msgs):
+            arr[k].stamp, arr[k].first_row, arr[k].num_rows, arr[k].trajectory_id = int(stamp), int(first), int(n), int(traj)
+            arr[k].sensor_to_tracking[:] = [float(v) for v in s2t]
+        return arr
+
+    def process(self, msgs, rows):
+        """rows: (n, 4) float32 x y z t -> (points (k, 3) float32, origins (len(msgs), 3), info dict)"""
+        rows = np.ascontiguousarray(rows, np.float32).reshape(-1, 4)
+        m = self.messages(msgs)
+        total = sum(int(x[2]) for x in msgs)
+        out = np.zeros((max(total, 1), 3), np.float32)
+        origins = np.zeros((max(len(msgs), 1), 3), np.float32)
+        n, info = C.c_int64(0), MapWriterInfo()
+        self.ctx.check(self.ctx.L.dl_map_writer_process(self.h, len(msgs), C.cast(m, C.c_void_p), rows.ctypes.data, len(rows),
+                                                        out.ctypes.data, C.byref(n), origins.ctypes.data, C.byref(info)))
+        return out[:n.value], origins[:len(msgs)], info.as_dict()
+
+    def process_dev(self, msgs, rows_dev_ptr, num_rows, points_dev_ptr):
+        """Device rows in, device points out -> (number of points, origins, info dict)"""
+        m = self.messages(msgs)
+        origins = np.zeros((max(len(msgs), 1), 3), np.float32)
+        n, info = C.c_int64(0), MapWriterInfo()
+        self.ctx.check(self.ctx.L.dl_map_writer_process_dev(self.h, len(msgs), C.cast(m, C.c_void_p), rows_dev_ptr, int(num_rows),
+                                                            points_dev_ptr, C.byref(n), origins.ctypes.data, C.byref(info)))
+        return n.value, origins[:len(msgs)], info.as_dict()
+
+    def flush(self):
+        """True if every message must be streamed again."""
+        r = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_map_writer_flush(self.h, C.byref(r)))
+        return bool(r.value)
+
+    def voxels(self):
+        """(cells (k, 3) int32, hits, rays), sorted by cell index"""
+        n = C.c_int64(0)
+        self.ctx.check(self.ctx.L.dl_map_writer_voxels(self.h, 0, None, None, None, C.byref(n)))
+        cells = np.zeros((max(n.value, 1), 3), np.int32)
+        hits, rays = np.zeros(max(n.value, 1), np.int32), np.zeros(max(n.value, 1), np.int32)
+        self.ctx.check(self.ctx.L.dl_map_writer_voxels(self.h, n.value, cells.ctypes.data, hits.ctypes.data, rays.ctypes.data,
+                                                       C.byref(n)))
+        return cells[:n.value], hits[:n.value], rays[:n.value]
+
+    def write_map(self, msgs, rows):
+        """Every pass over the same messages; the final pass's points."""
+        while True:
+            pts, origins, info = self.process(msgs, rows)
+            if not self.flush():
+                return pts, origins, info
+
+
+def write_pcd(path, points):
+    """io::PcdWritingPointsProcessor (io/pcd_writing_points_processor.cc:35-66): binary PCD v0.7, x y z floats, no colour,
+    WIDTH and POINTS zero-padded to 15 digits, 12 bytes per point in order."""
+    pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+    n = len(pts)
+    header = ("# generated by Cartographer\nVERSION .7\nFIELDS x y z\nSIZE 4 4 4\nTYPE F F F\nCOUNT 1 1 1\n"
+              f"WIDTH {n:015d}\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS {n:015d}\nDATA binary\n")
+    with open(path, "wb") as f:
+        f.write(header.encode())
+        f.write(pts.tobytes())
 
 
 def comm_unique_id():

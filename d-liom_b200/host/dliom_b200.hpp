@@ -7,6 +7,7 @@
 //   scan_matching::CeresScanMatcher3D                        SM/ceres_scan_matcher_3d.h:34-61
 //   mapping::RangeDataSynchronizer                           C/mapping/internal/3d/range_data_synchronizer.h:30-68
 //   mapping::LocalTrajectoryBuilder3D                        C/mapping/internal/3d/local_trajectory_builder_3d.h:81-113
+//   io::MapWriter, io::PcdWritingPointsProcessor             cartographer_ros/assets_writer.cc:120-160, C/io/*_points_processor.cc
 // Eigen / protobuf types are replaced by the plain structs below (this image has neither); INTEGRATION.md shows
 // the three-line adapters for Eigen::Vector3f / transform::Rigid3d / proto options in a real Cartographer tree.
 // Errors: the reference CHECK-aborts; this shim throws dliom::Error carrying the C-ABI status and message.
@@ -14,6 +15,7 @@
 #include <algorithm>
 #include <array>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <deque>
 #include <map>
@@ -782,4 +784,121 @@ class PoseGraph3D {
 };
 
 }  // namespace mapping
+
+namespace io {
+
+// The assets writer's processors (cartographer_ros/assets_writer.cc with the fork's assets_writer_tongji.lua), on the device in
+// the fixed order HandleMessage -> MinMaxRangeFiteringPointsProcessor -> OutlierRemovingPointsProcessor (dl_map_writer_*).
+struct MinMaxRangeFilteringOptions {  // min_max_range_filter (io/min_max_range_filtering_points_processor.cc:26-33)
+  double min_range = 0.0, max_range = 0.0;
+};
+struct OutlierRemovingOptions {  // voxel_filter_and_remove_moving_objects (io/outlier_removing_points_processor.cc:26-32)
+  double voxel_size = 0.0;
+};
+struct MapWriterOptions {
+  bool min_max_range_filter = false;
+  MinMaxRangeFilteringOptions range;
+  bool remove_moving_objects = false;
+  OutlierRemovingOptions outlier;
+};
+struct Message {  // one sensor message = one PointsBatch: x y z t rows (t in seconds, relative to stamp), sensor frame
+  int64_t stamp = 0;  // universal ticks (common::ToUniversal)
+  int trajectory_id = 0;
+  Rigid3d sensor_to_tracking;
+  TimedPointCloud rows;
+};
+enum class FlushResult { kRestartStream, kFinished };  // PointsProcessor::FlushResult
+
+class MapWriter {
+ public:
+  MapWriter(Context* ctx, const MapWriterOptions& options) : ctx_(ctx) {
+    dl_map_writer_options o{};
+    o.range_filter = options.min_max_range_filter ? 1 : 0;
+    o.min_range = options.range.min_range;
+    o.max_range = options.range.max_range;
+    o.outlier_voxel_size = options.remove_moving_objects ? options.outlier.voxel_size : 0.0;
+    ctx->check(dl_map_writer_create(ctx->get(), &o, &writer_));
+  }
+  ~MapWriter() { dl_map_writer_destroy(writer_); }
+  MapWriter(const MapWriter&) = delete;
+  MapWriter& operator=(const MapWriter&) = delete;
+  // TransformInterpolationBuffer(proto::Trajectory): node timestamps (universal ticks, non-decreasing) and global poses
+  void AddTrajectory(int trajectory_id, const std::vector<int64_t>& times, const std::vector<Rigid3d>& poses) {
+    if (times.size() != poses.size()) throw Error(DL_ERR_ARG, "AddTrajectory: times and poses differ in length");
+    std::vector<double> p(7 * poses.size());
+    for (size_t i = 0; i < poses.size(); ++i) poses[i].to7(&p[7 * i]);
+    ctx_->check(dl_map_writer_add_trajectory(writer_, trajectory_id, (int32_t)times.size(), times.data(), p.data()));
+  }
+  // Streams messages (one call for many); returns the points of the final pass, in order, and nothing in earlier passes.
+  PointCloud Process(const std::vector<Message>& messages) {
+    std::vector<dl_map_message> m(messages.size());
+    TimedPointCloud rows;
+    for (size_t k = 0; k < messages.size(); ++k) {
+      m[k].stamp = messages[k].stamp;
+      m[k].first_row = (int64_t)rows.size();
+      m[k].num_rows = (int64_t)messages[k].rows.size();
+      m[k].trajectory_id = messages[k].trajectory_id;
+      messages[k].sensor_to_tracking.to7(m[k].sensor_to_tracking);
+      rows.insert(rows.end(), messages[k].rows.begin(), messages[k].rows.end());
+    }
+    PointCloud out(rows.size());
+    int64_t n = 0;
+    ctx_->check(dl_map_writer_process(writer_, (int32_t)m.size(), m.data(), rows.empty() ? nullptr : rows[0].data(),
+                                      (int64_t)rows.size(), out.empty() ? nullptr : out[0].data(), &n, nullptr, &last_info_));
+    out.resize((size_t)n);
+    return out;
+  }
+  FlushResult Flush() {
+    int32_t restart = 0;
+    ctx_->check(dl_map_writer_flush(writer_, &restart));
+    return restart ? FlushResult::kRestartStream : FlushResult::kFinished;
+  }
+  const dl_map_writer_info& last_info() const { return last_info_; }
+
+ private:
+  Context* ctx_;
+  dl_map_writer* writer_ = nullptr;
+  dl_map_writer_info last_info_{};
+};
+
+// io::PcdWritingPointsProcessor (io/pcd_writing_points_processor.cc:35-130): binary PCD v0.7, x y z floats, no colour. The header
+// (WIDTH and POINTS zero-padded to 15 digits) is written before the first points and rewritten with the count at Flush.
+class PcdWritingPointsProcessor {
+ public:
+  explicit PcdWritingPointsProcessor(const std::string& filename) : file_(std::fopen(filename.c_str(), "wb")) {
+    if (!file_) throw Error(DL_ERR_ARG, "cannot open " + filename);
+  }
+  ~PcdWritingPointsProcessor() { if (file_) std::fclose(file_); }
+  PcdWritingPointsProcessor(const PcdWritingPointsProcessor&) = delete;
+  PcdWritingPointsProcessor& operator=(const PcdWritingPointsProcessor&) = delete;
+  void Process(const PointCloud& points) {
+    if (points.empty()) return;
+    if (num_points_ == 0) WriteHeader(0);
+    for (const auto& p : points)
+      if (std::fwrite(p.data(), 4, 3, file_) != 3) throw Error(DL_ERR_ARG, "PCD write failed");
+    num_points_ += (int64_t)points.size();
+  }
+  void Flush() {
+    WriteHeader(num_points_);
+    const bool ok = std::fclose(file_) == 0;
+    file_ = nullptr;
+    if (!ok) throw Error(DL_ERR_ARG, "PCD close failed");
+  }
+
+ private:
+  void WriteHeader(int64_t num_points) {
+    char header[320];
+    const int len = std::snprintf(header, sizeof(header),
+                                  "# generated by Cartographer\nVERSION .7\nFIELDS x y z\nSIZE 4 4 4\nTYPE F F F\nCOUNT 1 1 1\n"
+                                  "WIDTH %015lld\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %015lld\nDATA binary\n",
+                                  (long long)num_points, (long long)num_points);
+    if (std::fseek(file_, 0, SEEK_SET) != 0 || std::fwrite(header, 1, (size_t)len, file_) != (size_t)len)
+      throw Error(DL_ERR_ARG, "PCD header write failed");
+    if (std::fseek(file_, 0, SEEK_END) != 0) throw Error(DL_ERR_ARG, "PCD seek failed");
+  }
+  std::FILE* file_;
+  int64_t num_points_ = 0;
+};
+
+}  // namespace io
 }  // namespace dliom

@@ -781,6 +781,76 @@ int dl_ltb_get_submap(dl_local_trajectory_builder* builder, int32_t index, dl_gr
                       dl_grid** low_resolution_grid, double* local_pose, int32_t* num_range_data, int32_t* finished);
 int dl_ltb_get_state(const dl_local_trajectory_builder* builder, dl_nav_state* state, int32_t* initialized);
 
+/* ---- map writer: the assets writer's point pipeline for a finished run (cartographer_ros/assets_writer.cc:120-160 HandleMessage,
+ *      the fork's config dlio/config/assets_writer_tongji.lua) on the device. Per message (one io::PointsBatch):
+ *        point time = stamp + FromSeconds(t) (ticks of 100 ns, truncated toward zero), a point with !Has(time) is dropped
+ *        (transform_interpolation_buffer.cc:45-66, Interpolate in timestamped_transform.cc:22-37: fp64 lerp + Eigen slerp),
+ *        sensor_to_map = (tracking_to_map(time) * sensor_to_tracking).cast<float>(), output point = sensor_to_map * p, the batch
+ *        origin = the translation of the last kept point's sensor_to_map; a message without a kept point makes no batch;
+ *      then, in this fixed order:
+ *        min_max_range_filter (io/min_max_range_filtering_points_processor.cc): keep iff min_range <= |p - origin| <= max_range,
+ *          the float norm compared in double;
+ *        voxel_filter_and_remove_moving_objects (io/outlier_removing_points_processor.cc), three passes over the whole input:
+ *          pass 1 counts hits per cell (lround(p / (float)voxel_size)), pass 2 walks every ray from the batch origin in steps of
+ *          voxel_size (for (float x = 0; x < length; x += voxel_size)) and adds one ray to the sample's cell if it has hits,
+ *          pass 3 removes a point iff !(rays < 3 * hits) of its cell. Hits and rays are integer counts (no float atomics), so
+ *          they do not depend on the order of the work.
+ *      Restart protocol (PointsProcessor::FlushResult): stream every message of every trajectory through
+ *      dl_map_writer_process(_dev), then call dl_map_writer_flush; if *restart is 1 (twice with moving-object removal), stream
+ *      all of it again. Output points come only from the final pass. Node times are universal ticks (100 ns, the value of
+ *      proto::Trajectory::Node::timestamp) and must be non-decreasing; trajectories are added before the first process call.
+ *      Rejected with DL_ERR_ARG, the writer unchanged: an unknown trajectory, a trajectory added twice or after processing began,
+ *      rows outside [0, num_rows), a call after the final flush, and (pass 1) a kept point whose cell lies beyond the hybrid
+ *      grid's largest extent, +-8192 cells per axis (the reference's grid CHECK-fails there, hybrid_grid.h:391), or whose batch
+ *      origin's cell does (a ray that long could stall pass 2's float step, where the reference loops forever). Not built:
+ *      X-ray images, colours, intensities, other writers, the fixed-ratio sampler, frame-id filters, bag / tf reading. ---- */
+typedef struct dl_map_writer dl_map_writer;
+typedef struct dl_map_writer_options {
+  int32_t range_filter;        /* 1: min_max_range_filter is in the pipeline */
+  int32_t reserved;
+  double min_range, max_range;
+  double outlier_voxel_size;   /* > 0: voxel_filter_and_remove_moving_objects is in the pipeline, with this voxel_size */
+} dl_map_writer_options;
+typedef struct dl_map_message {  /* one PointsBatch: rows [first_row, first_row + num_rows) of the call's x y z t rows */
+  int64_t stamp;                 /* universal ticks of the message (the time the row times t, in seconds, are relative to) */
+  int64_t first_row, num_rows;
+  int32_t trajectory_id, reserved;
+  double sensor_to_tracking[7];
+} dl_map_message;
+typedef struct dl_map_writer_info {  /* of one process call */
+  int32_t pass;                      /* 0, 1 or 2: the pass this call belonged to */
+  int32_t final_pass;                /* 1 if this pass produces the output points */
+  int64_t num_rows;                  /* rows of the call's messages */
+  int64_t dropped_no_pose;           /* !Has(time) */
+  int64_t dropped_range;             /* min_max_range_filter */
+  int64_t dropped_moving;            /* moving-object removal (final pass only) */
+  int64_t messages_without_batch;
+  int64_t num_samples;               /* pass 2: ray samples taken */
+  int64_t num_points_out;
+} dl_map_writer_info;
+int dl_map_writer_create(dl_context* ctx, const dl_map_writer_options* options, dl_map_writer** out);
+void dl_map_writer_destroy(dl_map_writer* writer);
+/* times: num_nodes universal ticks (non-decreasing), poses: 7 doubles per node (the node's global pose). */
+int dl_map_writer_add_trajectory(dl_map_writer* writer, int32_t trajectory_id, int32_t num_nodes, const int64_t* times,
+                                 const double* poses);
+/* xyzt_rows: num_rows rows of x y z t floats (sensor frame, t in seconds relative to the message stamp, e.g. the rows of
+ * dl_decode_point_cloud2 with an identity sensor_to_tracking). points_out: room for as many x y z points as the messages have
+ * rows (may be NULL when the call is not in the final pass). origins_out (optional): 3 floats per message, the batch origin, NaN
+ * for a message without a batch. info may be NULL. At most 2^31 - 1 message rows per call. */
+int dl_map_writer_process(dl_map_writer* writer, int32_t num_messages, const dl_map_message* messages, const float* xyzt_rows,
+                          int64_t num_rows, float* points_out, int64_t* num_points_out, float* origins_out,
+                          dl_map_writer_info* info);
+/* The same with device rows in and device points out (16-byte aligned rows, as dl_decode_point_cloud2_dev writes them). */
+int dl_map_writer_process_dev(dl_map_writer* writer, int32_t num_messages, const dl_map_message* messages,
+                              const float* xyzt_rows_dev, int64_t num_rows, float* points_out_dev, int64_t* num_points_out,
+                              float* origins_out, dl_map_writer_info* info);
+/* Ends a pass: *restart = 1 if every message must be streamed again, 0 when the final pass ended (the writer is then finished). */
+int dl_map_writer_flush(dl_map_writer* writer, int32_t* restart);
+/* The moving-object removal's cell table, sorted by cell index (x, then y, then z): 3 ints per cell, hits, rays. Pass
+ * cells_xyz = NULL to query *count. */
+int dl_map_writer_voxels(const dl_map_writer* writer, int64_t capacity, int32_t* cells_xyz, int32_t* hits, int32_t* rays,
+                         int64_t* count);
+
 /* Device memory helpers so a host language without CUDA bindings can stage buffers. */
 int dl_device_alloc(dl_context* ctx, int64_t bytes, void** out_dev);
 int dl_device_free(dl_context* ctx, void* dev);
