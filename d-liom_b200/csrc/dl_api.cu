@@ -1703,6 +1703,7 @@ struct FrontendBuffers {
   int64_t tcap2 = 0, bit_words = 0;
   unsigned long long* slots2;  // second filter: one 64-bit word per slot (dl_frontend.cu)
   uint32_t* bits;              // two survivor bitmaps per scan
+  uint32_t* first_bits;        // the first filter's survivor bitmap per scan
   int32_t *last_index, *error_flag;
   float* local4;
   uint8_t* adaptive_first;  // scratch of the adaptive filters' grid-wide first pass (dl_voxel.cu)
@@ -1741,6 +1742,7 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   f->tcap2 = next_pow2(cap);
   f->bit_words = (int64_t)((C + 31) / 32);
   f->slots2 = a.take<unsigned long long>(B * f->tcap2); f->bits = a.take<uint32_t>(B * 2 * f->bit_words);
+  f->first_bits = a.take<uint32_t>(B * f->bit_words);
   f->last_index = a.take<int32_t>(B); f->error_flag = a.take<int32_t>(B);
   f->local4 = a.take<float>(B * C * 4);
   f->adaptive_first = a.take<uint8_t>(adaptive_first_pass_bytes(2 * batch, cap) + 16 * 1024);
@@ -1778,7 +1780,7 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
   fa.first_resolution = 0.5f * o.voxel_filter_size;  // LTB:394
   fa.second_resolution = o.voxel_filter_size;        // LTB:479-484
   fa.min_range = o.min_range; fa.max_range = o.max_range; fa.scan_period = o.scan_period;
-  fa.table1 = f.table; fa.slots2 = f.slots2; fa.bits = f.bits; fa.bit_words = f.bit_words;
+  fa.table1 = f.table; fa.first_bits = f.first_bits; fa.slots2 = f.slots2; fa.bits = f.bits; fa.bit_words = f.bit_words;
   fa.idx_bits = 1;
   while (((int64_t)1 << fa.idx_bits) < f.cap) ++fa.idx_bits;      // point indices are < cap
   fa.axis_bits = std::min(21, (63 - fa.idx_bits) / 3);             // 15 bits per axis up to 256 k points per scan

@@ -1,14 +1,15 @@
 // Fused scan front half for the batched front end: 4 launches per sub-batch (5 with per-run deskew poses) instead of the 11 of the stage-wise path
 // (dl_voxel.cu + dl_ingest.cu, which stay as the standalone filter API and as a cross-check in the tests).
 //
-//   A  fe_first_filter_insert   first voxel filter (LTB:393-395): every point proposes its index for its voxel
-//                               (atomicCAS claim + atomicMin), one 128-bit load per point.
+//   A  fe_first_filter_tile     first voxel filter (LTB:393-395), per tile of 2048 rows: the tile's lowest row per voxel in
+//                               shared memory, then only those propose their index to the scan's table (atomicCAS claim +
+//                               atomicMin); the survivors end as a per-scan bitmap.
 //   B0 fe_run_poses             12-byte rows with the point times as runs: the deskew pose (fp64 slerp + composition, LTB:430-445) once
 //                               per RUN instead of once per survivor; kernel B then loads the finished Rigid3f.
-//   B  fe_ingest_second_insert  for each first-filter survivor: deskew + transform + range gate (LTB:426-472) and
-//                               immediately the SECOND voxel filter's insert (LTB:479-484) keyed on the local-frame
-//                               voxel — no compaction in between: ids stay the original input indices, which
-//                               preserves "first point in input order wins" for free.
+//   B  fe_ingest_tile           per tile, the first-filter survivors in index order (from the bitmap): deskew + transform +
+//                               range gate (LTB:426-472) and the SECOND voxel filter (LTB:479-484) keyed on the local-frame
+//                               voxel, again per tile in shared memory first — no compaction in between: ids stay the original
+//                               input indices, which preserves "first point in input order wins" for free.
 //   C1 fe_mark_bits             the second filter's winners (the index field of every non-empty slot) become bits of two
 //                               per-scan bitmaps (returns, misses): 4 KiB per 32 k points, L2-resident.
 //   C2 fe_emit_tracking         ordered compaction straight from the bitmaps (popcount prefix; no per-point class map, no
@@ -25,8 +26,8 @@
 // 2 max_range / voxel_filter_size cells — +-2.4 km at 0.15 m. A point outside it sets the scan's error flag and the scan's
 // result is invalid (ok = -1); the generic dl_voxel_filter has no such limit. Returns and misses share the table (bit 63).
 //
-// Algorithmic traffic per raw point: A reads 12/16 B; B reads 4 B slot (+12/16 B row + 4 B time, writes 16 B record + 8 B slot
-// for survivors); C1 reads 8 B per slot; C2 reads 16 B and writes 12 B per output point.
+// Algorithmic traffic per raw point: A reads 12/16 B; B reads 1 bit (+12/16 B row + 4 B time, writes
+// 16 B record + 8 B slot for survivors); C1 reads 8 B per slot; C2 reads 16 B and writes 12 B per output point.
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
 
@@ -57,16 +58,19 @@ __device__ __forceinline__ Vec3f load_xyz(const float* __restrict__ rows, int ro
   return {v.x, v.y, v.z};
 }
 
-// 12-byte rows: index (into the batch's run arrays) of the time run that contains row i of scan b. A binary search of the scan's
-// ~2 k run starts (L1-resident) per survivor: expanding the run index of every row once per batch (4 B per row, one more kernel
-// and 17 MB of writes per step) made the ingest kernel faster but the step slower.
-__device__ __forceinline__ int run_index(const FrontendArgs& a, int b, int i) {
-  int lo = a.run_offsets[b], hi = a.run_offsets[b + 1] - 1;  // last run whose first row is <= i
+// 12-byte rows: index (into the batch's run arrays) of the time run that contains row i, searched among runs [lo, hi] (the last
+// run whose first row is <= i). The ingest kernel bounds the search to the runs of its tile, a few dozen L1-resident starts:
+// expanding the run index of every row once per batch (4 B per row, one more kernel and 17 MB of writes per step) made the
+// ingest kernel faster but the step slower.
+__device__ __forceinline__ int run_search(const FrontendArgs& a, int lo, int hi, int i) {
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
     if (__ldg(a.run_first_row + mid) <= i) lo = mid; else hi = mid - 1;
   }
   return lo;
+}
+__device__ __forceinline__ int run_index(const FrontendArgs& a, int b, int i) {
+  return run_search(a, a.run_offsets[b], a.run_offsets[b + 1] - 1, i);
 }
 
 // Time of row i of scan b: the row's fourth float, or (12-byte rows) the value of the run that contains the row.
@@ -75,29 +79,125 @@ __device__ __forceinline__ float point_time(const FrontendArgs& a, int b, const 
   return a.run_value[run_index(a, b, i)];
 }
 
+__device__ __forceinline__ int warp_sum(int v) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+  return v;
+}
+__device__ __forceinline__ int warp_exclusive(int v) {
+  const int lane = threadIdx.x & 31;
+  int inc = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int o = __shfl_up_sync(0xffffffffu, inc, d);
+    if (lane >= d) inc += o;
+  }
+  return inc - v;
+}
+
+// Both voxel filters keep the lowest input index per voxel, and a minimum can be taken in two levels: within each tile of kTile
+// consecutive rows (shared memory), then over the tile winners (the scan's table in global memory). The survivors are the same
+// for any input order and any tiling; what the tiles buy is that rows arrive in firing order, so most duplicates of a voxel lie in
+// the same tile (first filter: 93 %, second filter: 91.5 % of a 64-beam sweep's duplicates, tools/frontend_locality.py) and never
+// reach the L2's atomic units. A tile table has 2 * kTile slots and holds at most kTile voxels: it cannot fill.
+constexpr int kTile = 2048;
+constexpr int kTileSlots = 2 * kTile;
+
+// Appends the index of every non-empty entry of a tile table to `list` (any order) and returns how many there are. The whole CTA
+// calls it; kTileSlots is a multiple of the block size, so every warp runs the same number of rounds.
+template <typename T>
+__device__ __forceinline__ int list_occupied(const T* table, T empty, uint16_t* list, int* count) {
+  const int lane = threadIdx.x & 31;
+  for (int k = threadIdx.x; k < kTileSlots; k += blockDim.x) {
+    const bool used = table[k] != empty;
+    const unsigned ballot = __ballot_sync(0xffffffffu, used);
+    int at = 0;
+    if (lane == 0 && ballot) at = atomicAdd(count, __popc(ballot));
+    at = __shfl_sync(0xffffffffu, at, 0);
+    if (used) list[at + __popc(ballot & ((1u << lane) - 1))] = (uint16_t)k;
+  }
+  __syncthreads();
+  return *count;
+}
+
 // ---------------------------------------------------------------------------------------------------- A
-// One point in flight per thread: the kernel runs at the L2's atomic throughput, and 2 or 4 points per thread (more outstanding
-// atomics) measured slower because they only lengthen the L2 queues.
-__global__ void __launch_bounds__(kBlock, 8) fe_first_filter_insert(FrontendArgs a) {
+// One CTA per tile: the rows' cells go to shared memory (consecutive lanes read consecutive rows, so every sector of the tile is
+// fetched once), a shared table keeps the lowest row per cell (comparing cells in shared memory), and only the tile winners
+// propose their index to the scan's table: CAS claim, atomicMin only when the newcomer is older. A collision there still compares
+// against the owner's row in global memory.
+constexpr int kTileBlock = 512;
+__global__ void __launch_bounds__(kTileBlock) fe_first_filter_tile(FrontendArgs a) {
+  __shared__ Int3 cell[kTile];
+  __shared__ uint32_t owner[kTileSlots];
+  __shared__ uint16_t winners[kTile];
+  __shared__ uint32_t tile_bits[kTile / 32];
+  __shared__ int num_winners;
   const int b = a.first_scan + blockIdx.y;
   const int n = a.counts[b];
+  const int base = blockIdx.x * kTile;
+  if (base >= n) return;
+  const int rows_here = min(kTile, n - base);
   const float* rows = a.ranges + (size_t)b * a.in_cap * a.row_floats;
+  const CellDivider res = make_divider(a.first_resolution);
+  for (int k = threadIdx.x; k < kTileSlots; k += kTileBlock) owner[k] = kEmpty32;
+  if (threadIdx.x == 0) num_winners = 0;
+  if (threadIdx.x < kTile / 32) tile_bits[threadIdx.x] = 0;
+  for (int k = threadIdx.x; k < rows_here; k += kTileBlock) cell[k] = cell_index(load_xyz(rows, a.row_floats, base + k), res);
+  __syncthreads();
+  for (int k = threadIdx.x; k < rows_here; k += kTileBlock) {
+    const Int3 c = cell[k];
+    uint32_t hh = table_slot(hash_cell(c), kTileSlots);
+    uint32_t p = atomicCAS(owner + hh, kEmpty32, (uint32_t)k);
+    while (p != kEmpty32) {  // the slot has an owner: same voxel -> the lower row stays; else probe on
+      const Int3 o = cell[p];
+      if (o.x == c.x && o.y == c.y && o.z == c.z) {
+        if ((uint32_t)k < p) atomicMin(owner + hh, (uint32_t)k);  // the owner only ever decreases
+        break;
+      }
+      hh = (hh + 1) & (kTileSlots - 1);
+      p = atomicCAS(owner + hh, kEmpty32, (uint32_t)k);
+    }
+  }
+  __syncthreads();
+  const int m = list_occupied(owner, kEmpty32, winners, &num_winners);
+  // The scan's first-filter bitmap (memset to 0): every tile winner sets its bit before it is inserted (fence, then barrier), and
+  // every insert that meets an equal voxel clears the bit of the one that lost, the newcomer or the owner it replaced. A voxel
+  // with k tile winners sees k - 1 such meetings, each with a different loser, so exactly the lowest index keeps its bit (4 % of
+  // the tile winners on a bench sweep are cleared). Streaming the scan's table into the bitmap instead cost a kernel as long as
+  // a third of this one.
+  for (int k = threadIdx.x; k < m; k += kTileBlock) {
+    const uint32_t w = owner[winners[k]];
+    atomicOr(tile_bits + (w >> 5), 1u << (w & 31));
+  }
+  __syncthreads();
+  uint32_t* bits = a.first_bits + (size_t)b * a.bit_words;
+  if (threadIdx.x < kTile / 32 && tile_bits[threadIdx.x]) {
+    atomicOr(bits + (base >> 5) + threadIdx.x, tile_bits[threadIdx.x]);
+    __threadfence();
+  }
+  __syncthreads();
   uint32_t* tab = a.table1 + (size_t)b * a.tcap1;
   const uint32_t tcap = (uint32_t)a.tcap1;  // any size (not a power of two): slot = hash * tcap >> 32
-  const CellDivider res = make_divider(a.first_resolution);
-  const int stride = gridDim.x * kBlock;
-  for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += stride) {
-    const Int3 c = cell_index(load_xyz(rows, a.row_floats, i), res);
+  for (int k = threadIdx.x; k < m; k += kTileBlock) {
+    const uint32_t w = owner[winners[k]];
+    const Int3 c = cell[w];
+    const uint32_t i = (uint32_t)base + w;
     uint32_t hh = table_slot(hash_cell(c), tcap);
-    uint32_t p = atomicCAS(tab + hh, kEmpty32, (uint32_t)i);
-    while (p != kEmpty32) {  // the slot has an owner: same voxel -> the lower index stays; else probe on
+    uint32_t p = atomicCAS(tab + hh, kEmpty32, i);
+    while (p != kEmpty32) {
       const Int3 o = cell_index(load_xyz(rows, a.row_floats, p), res);
       if (o.x == c.x && o.y == c.y && o.z == c.z) {
-        if ((uint32_t)i < p) atomicMin(tab + hh, (uint32_t)i);  // the owner only ever decreases
+        uint32_t loser = i;
+        if (i < p) {
+          const uint32_t q = atomicMin(tab + hh, i);  // the owner only ever decreases
+          if (q > i) loser = q;
+        }
+        __threadfence();  // the loser's bit was set before its insert that this thread has seen
+        atomicAnd(bits + (loser >> 5), ~(1u << (loser & 31)));
         break;
       }
       hh = hh + 1 == tcap ? 0u : hh + 1;
-      p = atomicCAS(tab + hh, kEmpty32, (uint32_t)i);
+      p = atomicCAS(tab + hh, kEmpty32, i);
     }
   }
 }
@@ -162,22 +262,46 @@ __device__ __forceinline__ bool pack_slot(const KeyLayout& k, const Int3& c, boo
   *slot = (miss ? (1ull << 63) : 0ull) | (key << k.idx_bits) | (unsigned long long)i;
   return true;
 }
+// The voxel of a slot word (inverse of pack_slot's key).
+__device__ __forceinline__ Int3 unpack_cell(const KeyLayout& k, unsigned long long slot) {
+  const unsigned long long key = slot >> k.idx_bits;  // the miss bit lies above the three axes and is masked off
+  const uint32_t m = (1u << k.axis_bits) - 1;
+  return {(int)(((uint32_t)(key >> (2 * k.axis_bits)) & m) + k.bx), (int)(((uint32_t)(key >> k.axis_bits) & m) + k.by),
+          (int)(((uint32_t)key & m) + k.bz)};
+}
+// Second-filter insert of a slot word into a table of mask + 1 slots (the tile's in shared memory or the scan's): CAS claim; among
+// equal keys (same class and voxel) atomicMin keeps the lowest index.
+__device__ __forceinline__ void slot_insert(unsigned long long* slots, uint32_t mask, int idx_bits, const Int3& c,
+                                            unsigned long long slot) {
+  uint32_t hh = (hash_cell(c) ^ ((slot >> 63) ? 0x9e3779b9u : 0u)) & mask;
+  for (;;) {
+    const unsigned long long prev = atomicCAS(slots + hh, kEmpty64, slot);
+    if (prev == kEmpty64) break;
+    if ((prev >> idx_bits) == (slot >> idx_bits)) {
+      if (slot < prev) atomicMin(slots + hh, slot);
+      break;
+    }
+    hh = (hh + 1) & mask;
+  }
+}
 
-// Heavy per-survivor work of kernel B (double slerp, pose composition, transform, gate, second-filter insert).
+// Per-survivor work of kernel B: deskew, transform, range gate, the local-frame record and the second filter's insert into the
+// tile table. [run_lo, run_hi]: the tile's time runs (12-byte rows).
 template <bool kRunPose>
 __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, const float* rows, int rf, const ScanConstants& sc,
-                                               bool no_deskew, const KeyLayout& kl, unsigned long long* slots, uint32_t mask2, int i) {
+                                               bool no_deskew, const KeyLayout& kl, int run_lo, int run_hi,
+                                               unsigned long long* tile_slots, int i) {
   float4 h;
   Rigidf pose;
   if (kRunPose) {  // 12-byte rows, per-run pose table
     const float* p = rows + (size_t)i * 3;
     h = make_float4(p[0], p[1], p[2], 0.f);
-    const float4* rp = (const float4*)(a.run_pose + (size_t)8 * run_index(a, b, i));
+    const float4* rp = (const float4*)(a.run_pose + (size_t)8 * run_search(a, run_lo, run_hi, i));
     const float4 p0 = __ldg(rp), p1 = __ldg(rp + 1);
     pose = Rigidf{{p0.x, p0.y, p0.z}, {p0.w, p1.x, p1.y, p1.z}};
   } else if (rf == 3) {
     const float* p = rows + (size_t)i * 3;
-    h = make_float4(p[0], p[1], p[2], point_time(a, b, rows, rf, i));
+    h = make_float4(p[0], p[1], p[2], a.run_value[run_search(a, run_lo, run_hi, i)]);
   } else {
     h = __ldg((const float4*)(rows + (size_t)i * rf));
   }
@@ -207,80 +331,77 @@ __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, con
       a.error_flag[b] = 1;  // per scan: only this scan's result is invalidated
       cls = 0;
     } else {
-      uint32_t hh = (hash_cell(c) ^ (cls == 2 ? 0x9e3779b9u : 0u)) & mask2;
-      for (;;) {
-        const unsigned long long prev = atomicCAS(slots + hh, kEmpty64, slot);
-        if (prev == kEmpty64) break;
-        if ((prev >> kl.idx_bits) == (slot >> kl.idx_bits)) {  // same class and voxel: the lowest index stays
-          if (slot < prev) atomicMin(slots + hh, slot);
-          break;
-        }
-        hh = (hh + 1) & mask2;
-      }
+      slot_insert(tile_slots, kTileSlots - 1, kl.idx_bits, c, slot);
     }
   }
   return cls;
 }
 
-// Only ~30 % of the raw points survive the first filter, so running the heavy path under the survivor predicate
-// would leave most lanes idle. Each warp instead appends its survivors to a small shared-memory queue and drains
-// it 32 at a time with all lanes busy.
+// One CTA per tile of kTile rows. Warp 0 expands the tile's first-filter bitmap words into a shared list of survivors in index
+// order (only ~40 % of the rows survive, so the heavy path runs over the list with all lanes busy): rows are read and local-frame
+// records written at nearly consecutive addresses, and the run search of 12-byte rows covers only the tile's few dozen runs
+// (L1-resident starts and poses). The survivors' second-filter words meet in the tile table; only the tile winners go on to the
+// scan's table, with the same protocol.
+constexpr int kWordsPerLane = kTile / 32 / 32;  // bitmap words of a tile per lane of warp 0
 template <bool kRunPose>
-__global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_second_insert(FrontendArgs a) {  // <= 40 / 64 registers
-  __shared__ int queue[kBlock / 32][64];
+__global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_tile(FrontendArgs a) {  // <= 40 / 64 registers
+  __shared__ unsigned long long tile_slots[kTileSlots];
+  __shared__ uint16_t list[kTile];
+  __shared__ int listed, num_winners, run_lo, run_hi;
   const int b = a.first_scan + blockIdx.y;
   const int n = a.counts[b];
+  const int base = blockIdx.x * kTile;
+  if (base >= n) return;
+  const int rows_here = min(kTile, n - base);
   const int rf = a.row_floats;
   const float* rows = a.ranges + (size_t)b * a.in_cap * rf;
-  const uint32_t* tab = a.table1 + (size_t)b * a.tcap1;
-  unsigned long long* slots = a.slots2 + (size_t)b * a.tcap2;
-  const uint32_t mask2 = (uint32_t)a.tcap2 - 1;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = threadIdx.x; k < kTileSlots; k += kBlock) tile_slots[k] = kEmpty64;
+  if (warp == 0) {
+    const uint32_t* bits = a.first_bits + (size_t)b * a.bit_words + (base >> 5);
+    const int words = (rows_here + 31) >> 5;
+    uint32_t w[kWordsPerLane];
+    int count = 0;
+#pragma unroll
+    for (int j = 0; j < kWordsPerLane; ++j) {
+      const int q = lane * kWordsPerLane + j;
+      w[j] = q < words ? __ldcg(bits + q) : 0u;
+      count += __popc(w[j]);
+    }
+    int pos = warp_exclusive(count);
+#pragma unroll
+    for (int j = 0; j < kWordsPerLane; ++j)
+      for (uint32_t x = w[j]; x; x &= x - 1) list[pos++] = (uint16_t)((lane * kWordsPerLane + j) * 32 + __ffs(x) - 1);
+    if (lane == 31) listed = pos;
+    if (lane == 0) num_winners = 0;
+  } else if (threadIdx.x == 32) {
+    run_lo = run_hi = 0;
+    if (rf == 3) {
+      run_lo = run_index(a, b, base);
+      run_hi = run_index(a, b, base + rows_here - 1);
+    }
+  }
   const ScanConstants& sc = a.scans[b];
   const KeyLayout kl = key_layout(a, sc);
-  const bool no_deskew = n > 0 && (double)fabsf(point_time(a, b, rows, rf, 0)) < 1e-3;  // first survivor is row 0 (LTB:430-433)
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int* q = queue[warp];
-  int queued = 0, survivors = 0, returns = 0, last = -1;
-  // The first filter's survivors are exactly the non-empty table slots: stream the table (coalesced) instead of
-  // probing it once per raw point. Order does not matter here: the second filter keys on the original index.
-  if (n == 0) return;
-  // (four slots per thread and step through one 16-byte load: same kernel time in the serial launch list, slightly slower in the
-  //  overlapped step, so the stream stays one slot per thread)
-  for (int h = blockIdx.x * kBlock + threadIdx.x; h < (int)a.tcap1; h += gridDim.x * kBlock) {
-    const uint32_t owner = __ldcg(tab + h);
-    const bool surv = owner != kEmpty32;
-    const unsigned ballot = __ballot_sync(0xffffffffu, surv);
-    if (surv) {
-      q[queued + __popc(ballot & ((1u << lane) - 1))] = (int)owner;
-      last = max(last, (int)owner);
-    }
-    queued += __popc(ballot);
-    survivors += surv;
-    __syncwarp();
-    if (queued >= 32) {
-      returns += ingest_survivor<kRunPose>(a, b, rows, rf, sc, no_deskew, kl, slots, mask2, q[lane]) == 1;
-      __syncwarp();
-      const int rest = queued - 32;
-      const int moved = lane < rest ? q[32 + lane] : 0;
-      __syncwarp();
-      if (lane < rest) q[lane] = moved;
-      queued = rest;
-      __syncwarp();
-    }
+  const bool no_deskew = !kRunPose && (double)fabsf(point_time(a, b, rows, rf, 0)) < 1e-3;  // LTB:430-433
+  __syncthreads();
+  if (threadIdx.x == 0 && listed > 0) {  // survivor count and the LAST survivor (hits_poses.back(), LTB:476)
+    atomicAdd(a.n_first + b, listed);
+    atomicMax(a.last_index + b, base + list[listed - 1]);
   }
-  if (lane < queued) returns += ingest_survivor<kRunPose>(a, b, rows, rf, sc, no_deskew, kl, slots, mask2, q[lane]) == 1;
-  // bookkeeping: survivor counts and the LAST first-filter survivor (hits_poses.back(), LTB:476)
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) {
-    survivors += __shfl_xor_sync(0xffffffffu, survivors, d);
-    returns += __shfl_xor_sync(0xffffffffu, returns, d);
-    last = max(last, __shfl_xor_sync(0xffffffffu, last, d));
+  int returns = 0;
+  for (int k = threadIdx.x; k < listed; k += kBlock)  // (shared operands read where used: fewer registers across the loop)
+    returns += ingest_survivor<kRunPose>(a, b, rows, rf, sc, no_deskew, kl, run_lo, run_hi, tile_slots, base + list[k]) == 1;
+  __syncthreads();
+  const int won = list_occupied(tile_slots, kEmpty64, list, &num_winners);
+  unsigned long long* slots = a.slots2 + (size_t)b * a.tcap2;
+  const uint32_t mask2 = (uint32_t)a.tcap2 - 1;
+  for (int k = threadIdx.x; k < won; k += kBlock) {
+    const unsigned long long s = tile_slots[list[k]];
+    slot_insert(slots, mask2, kl.idx_bits, unpack_cell(kl, s), s);
   }
-  if (lane == 0) {
-    if (survivors) atomicAdd(a.n_first + b, survivors);
-    if (returns) atomicAdd(a.n_returns_local + b, returns);
-    if (last >= 0) atomicMax(a.last_index + b, last);
-  }
+  returns = warp_sum(returns);
+  if (lane == 0 && returns) atomicAdd(a.n_returns_local + b, returns);
 }
 
 // ---------------------------------------------------------------------------------------------------- C
@@ -304,22 +425,6 @@ __global__ void __launch_bounds__(kBlock) fe_mark_bits(FrontendArgs a) {
       atomicOr(scan_bits(a, b, (int)(s >> 63)) + (i >> 5), 1u << (i & 31));  // result unused: a reduction, no round trip
     }
   }
-}
-
-__device__ __forceinline__ int warp_sum(int v) {
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-  return v;
-}
-__device__ __forceinline__ int warp_exclusive(int v) {
-  const int lane = threadIdx.x & 31;
-  int inc = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int o = __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= d) inc += o;
-  }
-  return inc - v;
 }
 
 // C2: gridDim.x CTAs per scan. Every CTA counts the bits of all 1024-point chunks of its scan (32 words per chunk: a few KiB from
@@ -453,6 +558,7 @@ int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch) {
   DL_CUDA(ctx, cudaMemsetAsync(a.table1, 0xFF, (size_t)batch * a.tcap1 * sizeof(uint32_t), ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(a.slots2, 0xFF, (size_t)batch * a.tcap2 * sizeof(unsigned long long), ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(a.bits, 0, (size_t)batch * 2 * a.bit_words * sizeof(uint32_t), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(a.first_bits, 0, (size_t)batch * a.bit_words * sizeof(uint32_t), ctx->stream));
   fe_reset_counters<<<(batch + 127) / 128, 128, 0, ctx->stream>>>(a, batch);
   DL_LAUNCH_CHECK(ctx, "fe_reset_counters");
   return DL_OK;
@@ -462,9 +568,9 @@ int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch) {
 int launch_fe_first_filter(dl_context* ctx, FrontendArgs a, int first_scan, int num_scans) {
   if (num_scans <= 0) return DL_OK;
   a.first_scan = first_scan;
-  const int tiles = (int)std::min<int64_t>((a.cap + kBlock - 1) / kBlock, 128);
-  fe_first_filter_insert<<<dim3(tiles, num_scans), kBlock, 0, ctx->stream>>>(a);
-  DL_LAUNCH_CHECK(ctx, "fe_first_filter_insert");
+  const int row_tiles = (int)((a.cap + kTile - 1) / kTile);
+  fe_first_filter_tile<<<dim3(row_tiles, num_scans), kTileBlock, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "fe_first_filter_tile");
   return DL_OK;
 }
 
@@ -472,15 +578,15 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
   if (batch <= 0) return DL_OK;
   a.first_scan = first_scan;
   const int tiles = (int)std::min<int64_t>((a.cap + kBlock - 1) / kBlock, 128);
-  const int per_scan = 48;  // measured best of {8, 20, 32, 48, 64}: enough CTAs in flight to hide the random-access latency
+  const int row_tiles = (int)((a.cap + kTile - 1) / kTile);
   if (a.run_pose && a.max_runs > 0) {
     fe_run_poses<<<dim3((a.max_runs + 127) / 128, batch), 128, 0, ctx->stream>>>(a);
     DL_LAUNCH_CHECK(ctx, "fe_run_poses");
-    fe_ingest_second_insert<true><<<dim3(per_scan, batch), kBlock, 0, ctx->stream>>>(a);
+    fe_ingest_tile<true><<<dim3(row_tiles, batch), kBlock, 0, ctx->stream>>>(a);
   } else {
-    fe_ingest_second_insert<false><<<dim3(per_scan, batch), kBlock, 0, ctx->stream>>>(a);
+    fe_ingest_tile<false><<<dim3(row_tiles, batch), kBlock, 0, ctx->stream>>>(a);
   }
-  DL_LAUNCH_CHECK(ctx, "fe_ingest_second_insert");
+  DL_LAUNCH_CHECK(ctx, "fe_ingest_tile");
   fe_mark_bits<<<dim3(tiles, batch), kBlock, 0, ctx->stream>>>(a);
   DL_LAUNCH_CHECK(ctx, "fe_mark_bits");
   const int max_chunks = (int)((a.bit_words + 31) / 32);

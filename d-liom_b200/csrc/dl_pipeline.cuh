@@ -88,6 +88,7 @@ struct FrontendArgs {
   float first_resolution, second_resolution, min_range, max_range;
   double scan_period;
   uint32_t* table1;              // first filter: slot -> min point index
+  uint32_t* first_bits;          // per scan one bitmap of bit_words words: bit i = point i survives the first filter
   unsigned long long* slots2;    // second filter: slot -> [miss | relative voxel key | point index] (dl_frontend.cu)
   int idx_bits, axis_bits;       // widths of the index field and of one axis of the key
   uint32_t* bits;                // per scan two bitmaps (returns, misses) of bit_words words: bit i = point i survives
