@@ -1,5 +1,5 @@
 // C-ABI of libdliom_b200.so (declared in include/dliom_b200.h): contexts, the device grid mirror, and the host
-// orchestration of the kernels in dl_voxel.cu / dl_rtcsm.cu / dl_nls.cu / dl_ingest.cu.
+// orchestration of the kernels in dl_voxel.cu / dl_rtcsm.cu / dl_nls.cu / dl_frontend.cu.
 // There is deliberately no CPU implementation of anything here: without a CUDA device every call fails.
 #include <algorithm>
 #include <cmath>
@@ -1692,13 +1692,10 @@ namespace {
 struct FrontendBuffers {
   int batch = 0;
   int64_t cap = 0, tcap = 0;
-  int tiles = 0;
-  int32_t *counts0, *n1, *n_ret, *n_miss, *n2, *n3, *countsA, *npassesA, *croppedA, *block_counts, *tile_counts;
-  uint32_t *table, *slot, *tableA, *scratchA;
-  int32_t *keep1, *keep2, *keep3, *keepA;
-  float *tmp_points, *returns_local, *misses_local, *returns_tracking, *misses_tracking, *clouds, *current_pose, *origins,
-      *passesA, *rtcsm_scores;
-  uint8_t* cls;
+  int32_t *counts0, *n1, *n_ret, *n2, *n3, *countsA, *npassesA, *croppedA;
+  uint32_t *table, *tableA, *scratchA;
+  int32_t* keepA;
+  float *returns_tracking, *misses_tracking, *clouds, *current_pose, *origins, *passesA, *rtcsm_scores;
   // fused front half
   int64_t tcap2 = 0, bit_words = 0;
   unsigned long long* slots2;  // second filter: one 64-bit word per slot (dl_frontend.cu)
@@ -1717,19 +1714,15 @@ struct FrontendBuffers {
   float *run_value = nullptr, *run_pose = nullptr;
 };
 
-// Device scratch of one front-end run. The stage-wise buffers (one voxel-filter pass per launch: dl_voxel.cu / dl_ingest.cu)
-// exist only for dl_ingest_scan, which cross-checks the fused front half against them; the batched path does not carve them
-// (round 1 did: ~150 B x cap x batch of dead scratch per context).
-void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f, bool stagewise = false) {
+// Device scratch of one front-end run.
+void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f) {
   const size_t B = (size_t)batch, C = (size_t)cap;
   f->batch = batch;
   f->cap = cap;
   f->tcap = next_pow2(2 * cap);
-  f->tiles = (int)((cap + 255) / 256);
-  f->counts0 = a.take<int32_t>(B); f->n1 = a.take<int32_t>(B); f->n_ret = a.take<int32_t>(B); f->n_miss = a.take<int32_t>(B);
+  f->counts0 = a.take<int32_t>(B); f->n1 = a.take<int32_t>(B); f->n_ret = a.take<int32_t>(B);
   f->n2 = a.take<int32_t>(B); f->n3 = a.take<int32_t>(B); f->countsA = a.take<int32_t>(2 * B); f->npassesA = a.take<int32_t>(2 * B);
   f->croppedA = a.take<int32_t>(2 * B);
-  f->tile_counts = a.take<int32_t>(B * f->tiles * 2);
   f->table = a.take<uint32_t>(B * f->tcap);
   f->tableA = a.take<uint32_t>(B * 2 * f->tcap); f->scratchA = a.take<uint32_t>(B * 4 * C);
   f->keepA = a.take<int32_t>(B * 2 * C);
@@ -1746,15 +1739,6 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   f->last_index = a.take<int32_t>(B); f->error_flag = a.take<int32_t>(B);
   f->local4 = a.take<float>(B * C * 4);
   f->adaptive_first = a.take<uint8_t>(adaptive_first_pass_bytes(2 * batch, cap) + 16 * 1024);
-  f->block_counts = nullptr; f->slot = nullptr; f->keep1 = f->keep2 = f->keep3 = nullptr;
-  f->tmp_points = f->returns_local = f->misses_local = nullptr; f->cls = nullptr;
-  if (stagewise) {
-    f->block_counts = a.take<int32_t>(B * f->tiles);
-    f->slot = a.take<uint32_t>(B * C);
-    f->keep1 = a.take<int32_t>(B * C); f->keep2 = a.take<int32_t>(B * C); f->keep3 = a.take<int32_t>(B * C);
-    f->tmp_points = a.take<float>(B * C * 3); f->returns_local = a.take<float>(B * C * 3); f->misses_local = a.take<float>(B * C * 3);
-    f->cls = a.take<uint8_t>(B * C);
-  }
 }
 
 // Device copies of the time_run_* arrays of 12-byte rows (validated by check_frontend) and, with many runs per scan, the table
@@ -1772,7 +1756,7 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
                                 int64_t in_cap, int row_floats) {
   FrontendArgs fa{};
   fa.ranges = d_ranges; fa.in_cap = in_cap; fa.row_floats = row_floats; fa.counts = f.counts0; fa.scans = f.scans;
-  fa.origins = f.origins; fa.cap = f.cap; fa.tiles = f.tiles; fa.tcap2 = f.tcap2;
+  fa.origins = f.origins; fa.cap = f.cap; fa.tcap2 = f.tcap2;
   // First-filter table of the fused path: the next power of two above 2 * cap (load ~0.18 on real sweeps). A compact table of
   // 1.25 slots per point (the kernels take any size: slot = hash * tcap >> 32) saves a third of the memset and of the ingest
   // kernel's table stream but costs the first filter more in collisions than it saves.
@@ -1795,34 +1779,6 @@ int row_floats_of(const dl_frontend_options& o) { return o.range_row_floats == 4
 
 ScanConstants make_scan_constants(const double* prev7, const double* cur7) {  // dl_pipeline.cuh has the arithmetic
   return dl::make_scan_constants(pose_from7(prev7), pose_from7(cur7));
-}
-
-// Stages 1-3: first voxel filter, deskew/transform/gate, second voxel filters, back to the tracking frame.
-int frontend_ingest(dl_context* ctx, const dl_frontend_options& o, const FrontendBuffers& f, const float* d_ranges,
-                    int64_t in_cap) {
-  {
-    StageScope st(ctx, "voxel_filter_first");
-    DL_TRY(launch_voxel_filter(ctx, d_ranges, 8, in_cap, f.counts0, f.batch, 0.5f * o.voxel_filter_size, f.table, f.tcap,
-                               f.slot, f.keep1, f.n1, f.block_counts));
-  }
-  IngestArgs ia{};
-  ia.ranges = d_ranges; ia.in_cap = in_cap; ia.scans = f.scans; ia.origins = f.origins; ia.keep = f.keep1;
-  ia.keep_counts = f.n1; ia.cap = f.cap; ia.tiles = f.tiles; ia.min_range = o.min_range; ia.max_range = o.max_range;
-  ia.scan_period = o.scan_period; ia.tmp_points = f.tmp_points; ia.cls = f.cls; ia.tile_counts = f.tile_counts;
-  ia.returns_local = f.returns_local; ia.misses_local = f.misses_local; ia.num_returns = f.n_ret; ia.num_misses = f.n_miss;
-  ia.current_pose = f.current_pose;
-  {
-    StageScope st(ctx, "deskew_transform_gate");
-    DL_TRY(launch_ingest(ctx, ia, f.batch));
-  }
-  StageScope st2(ctx, "voxel_filter_second");
-  DL_TRY(launch_voxel_filter(ctx, f.returns_local, 3, f.cap, f.n_ret, f.batch, o.voxel_filter_size, f.table, f.tcap, f.slot,
-                             f.keep2, f.n2, f.block_counts));
-  DL_TRY(launch_gather_to_tracking(ctx, f.returns_local, f.cap, f.keep2, f.n2, f.current_pose, f.returns_tracking, f.batch));
-  DL_TRY(launch_voxel_filter(ctx, f.misses_local, 3, f.cap, f.n_miss, f.batch, o.voxel_filter_size, f.table, f.tcap, f.slot,
-                             f.keep3, f.n3, f.block_counts));
-  DL_TRY(launch_gather_to_tracking(ctx, f.misses_local, f.cap, f.keep3, f.n3, f.current_pose, f.misses_tracking, f.batch));
-  return DL_OK;
 }
 
 // The pinned staging block of a front-end batch: the small per-call tables, then the results and estimated IMU states that a
@@ -2514,48 +2470,50 @@ int dl_ingest_scan(dl_context* ctx, const dl_frontend_options* options, const vo
   if (!ctx || !options || !ranges || n < 1 || n > 0x3fffffff || !origins || num_origins < 1 || !prev_pose || !predicted_pose ||
       !counts_out)
     return DL_ERR_ARG;
+  if (row_floats_of(*options) != 8) return ctx->fail(DL_ERR_ARG, "dl_ingest_scan takes RangeMeasurement rows (range_row_floats = 8)");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   float* d_ranges;
   FrontendBuffers f;
   DL_TRY(carve_scratch(ctx, [&](Arena& a) {
     d_ranges = a.take<float>((size_t)n * 8);
-    carve(a, 1, n, num_origins, &f, true);
+    carve(a, 1, n, num_origins, &f);
   }));
   DL_TRY(h2d(ctx, d_ranges, (const float*)ranges, (size_t)n * 8));
-  if (row_floats_of(*options) != 8) return ctx->fail(DL_ERR_ARG, "dl_ingest_scan takes RangeMeasurement rows (range_row_floats = 8)");
   DL_TRY(frontend_upload_small(ctx, *options, f, &n, origins, num_origins, prev_pose, predicted_pose, nullptr, nullptr));
-  // stage-wise kernels (first_keep, returns_local) ...
-  DL_TRY(frontend_ingest(ctx, *options, f, d_ranges, n));
-  int32_t stagewise[4];
-  DL_TRY(d2h(ctx, &stagewise[0], f.n1, 1));
-  DL_TRY(d2h(ctx, &stagewise[1], f.n_ret, 1));
-  DL_TRY(d2h(ctx, &stagewise[2], f.n2, 1));
-  DL_TRY(d2h(ctx, &stagewise[3], f.n3, 1));
-  DL_TRY(sync(ctx));
-  std::vector<int32_t> keep32(stagewise[0]);
-  DL_TRY(d2h(ctx, keep32.data(), f.keep1, stagewise[0]));
-  if (returns_local_out) DL_TRY(d2h(ctx, returns_local_out, f.returns_local, (size_t)stagewise[1] * 3));
-  DL_TRY(sync(ctx));
-  // ... then the fused kernels the batched front end uses, for everything in the tracking frame
+  // fe_ingest_tile writes the local record of a return or a miss only: zeroed records read as class 0 for every other row
+  DL_CUDA(ctx, cudaMemsetAsync(f.local4, 0, (size_t)n * 4 * sizeof(float), ctx->stream));
   const FrontendArgs fa = make_frontend_args(*options, f, d_ranges, n, 8);
   DL_TRY(launch_fe_prepare(ctx, fa, 1));
   DL_TRY(launch_fe_first_filter(ctx, fa, 0, 1));
   DL_TRY(launch_fe_rest(ctx, fa, 0, 1));
-  int32_t c[4];
+  int32_t c[4], error_flag;
   DL_TRY(d2h(ctx, &c[0], f.n1, 1));
   DL_TRY(d2h(ctx, &c[1], f.n_ret, 1));
   DL_TRY(d2h(ctx, &c[2], f.n2, 1));
   DL_TRY(d2h(ctx, &c[3], f.n3, 1));
+  DL_TRY(d2h(ctx, &error_flag, f.error_flag, 1));
+  std::vector<uint32_t> first_bits(f.bit_words);
+  DL_TRY(d2h(ctx, first_bits.data(), f.first_bits, first_bits.size()));
+  std::vector<float> local(returns_local_out ? (size_t)n * 4 : 0);  // float4 per row: local-frame point, class in .w
+  DL_TRY(d2h(ctx, local.data(), f.local4, local.size()));
   DL_TRY(sync(ctx));
   for (int i = 0; i < 4; ++i) counts_out[i] = c[i];
-  if (c[0] != stagewise[0] || c[1] != stagewise[1] || c[2] != stagewise[2] || c[3] != stagewise[3])
-    return ctx->fail(DL_ERR_ARG, "internal: fused and stage-wise front ends disagree on survivor counts");
+  if (error_flag)
+    return ctx->fail(DL_ERR_ARG, "a point lies outside the voxel-key span of the second voxel filter (dl_scan_result.ok = -1)");
   if (returns_tracking_out) DL_TRY(d2h(ctx, returns_tracking_out, f.returns_tracking, (size_t)c[2] * 3));
   if (misses_tracking_out) DL_TRY(d2h(ctx, misses_tracking_out, f.misses_tracking, (size_t)c[3] * 3));
   if (current_pose7f_out) DL_TRY(d2h(ctx, current_pose7f_out, f.current_pose, 7));
   DL_TRY(sync(ctx));
-  if (first_keep_out)
-    for (int i = 0; i < c[0]; ++i) first_keep_out[i] = keep32[i];
+  // first_keep: the rows of the first filter's bitmap in index order; returns_local: those of them in class 1 (a return)
+  int64_t kept = 0, returns = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    if (!(first_bits[i >> 5] >> (i & 31) & 1u)) continue;
+    if (first_keep_out) first_keep_out[kept++] = i;
+    if (!returns_local_out) continue;
+    int32_t cls;
+    std::memcpy(&cls, &local[4 * i + 3], sizeof(cls));
+    if (cls == 1) std::memcpy(returns_local_out + 3 * returns++, &local[4 * i], 3 * sizeof(float));
+  }
   return DL_OK;
 }
 

@@ -1,5 +1,5 @@
-// Fused scan front half for the batched front end: 4 launches per sub-batch (5 with per-run deskew poses) instead of the 11 of the stage-wise path
-// (dl_voxel.cu + dl_ingest.cu, which stay as the standalone filter API and as a cross-check in the tests).
+// Fused scan front half of the batched front end and of dl_ingest_scan: 4 launches per sub-batch (5 with per-run deskew poses),
+// then the small glue kernels of the batched front end (cloud gathers, pose algebra, result records).
 //
 //   A  fe_first_filter_tile     first voxel filter (LTB:393-395), per tile of 2048 rows: the tile's lowest row per voxel in
 //                               shared memory, then only those propose their index to the scan's table (atomicCAS claim +
@@ -323,7 +323,7 @@ __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, con
     }
   }
   if (cls) {
-    // one aligned 16-byte record per survivor: local-frame point (+ class in .w, for debugging only)
+    // one aligned 16-byte record per survivor: local-frame point (+ class in .w, which dl_ingest_scan reads for returns_local)
     ((float4*)a.local)[(size_t)b * a.cap + i] = make_float4(outp.x, outp.y, outp.z, __int_as_float(cls));
     const Int3 c = cell_index(outp, make_divider(a.second_resolution));
     unsigned long long slot;
@@ -552,6 +552,71 @@ __global__ void fe_reset_counters(FrontendArgs a, int batch) {
   a.error_flag[b] = 0;
 }
 
+// ---------------------------------------------------------------------------------------------------- glue
+// Plain gather of selected rows (adaptive filter survivors) into a dense cloud.
+__global__ void __launch_bounds__(kBlock) gather_rows_kernel(const float* __restrict__ in, int64_t cap_in, int pairs_per_cloud,
+                                                             const int32_t* __restrict__ keep, const int32_t* __restrict__ keep_counts,
+                                                             int64_t cap_out, float* __restrict__ out) {
+  const int pair = blockIdx.y;
+  const int b = pair / pairs_per_cloud;
+  const int count = keep_counts[pair];
+  // grid-stride: the survivors are a few hundred rows, so a handful of CTAs per cloud replaces one per 256 rows of capacity
+  for (int j = blockIdx.x * kBlock + threadIdx.x; j < count; j += gridDim.x * kBlock) {
+    const float* p = in + ((size_t)b * cap_in + keep[(size_t)pair * cap_in + j]) * 3;
+    float* o = out + ((size_t)pair * cap_out + j) * 3;
+    o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
+  }
+}
+
+// initial_ceres_pose = submap.local_pose^-1 * pose_prediction, pose_prediction = current_pose.cast<double>() (LTB:476-487, :504-505)
+__global__ void initial_pose_kernel(int batch, const float* __restrict__ current_pose, Rigidd submap_inverse,
+                                    double* __restrict__ initial_pose, double* __restrict__ target_translation) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  const float* cp = current_pose + 7 * b;
+  const Rigidd prediction = to_double(Rigidf{{cp[0], cp[1], cp[2]}, {cp[3], cp[4], cp[5], cp[6]}});
+  const Rigidd init = compose(submap_inverse, prediction);
+  pose_to7(init, initial_pose + 7 * b);
+  target_translation[3 * b] = init.t.x;
+  target_translation[3 * b + 1] = init.t.y;
+  target_translation[3 * b + 2] = init.t.z;
+}
+
+__global__ void finalize_results_kernel(ResultArgs a) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.batch) return;
+  dl_scan_result& r = a.results[b];
+  const int n_hi = a.adaptive_counts[2 * b], n_lo = a.adaptive_counts[2 * b + 1];
+  r.num_first_filter = a.first_counts[b];
+  r.num_returns = a.return_counts[b];
+  r.num_misses = a.miss_counts[b];
+  r.num_high_resolution = n_hi;
+  r.num_low_resolution = n_lo;
+  r.num_cropped_high = a.adaptive_cropped[2 * b];
+  r.num_cropped_low = a.adaptive_cropped[2 * b + 1];
+  r.num_passes_high = a.adaptive_passes[2 * b];
+  r.num_passes_low = a.adaptive_passes[2 * b + 1];
+  r.rtcsm_score = a.rtcsm_scores ? a.rtcsm_scores[b] : 0.f;
+  r.reserved = 0;
+  // the reference drops the scan when any of the three clouds is empty (LTB:497-500, :510-513, :531-534)
+  r.ok = (a.return_counts[b] > 0 && n_hi > 0 && n_lo > 0) ? 1 : 0;
+  if (a.error_flag && a.error_flag[b]) r.ok = -1;  // a point fell outside +-2^20 voxels: results are not valid
+  if (a.imu_ok && a.imu_ok[b] == 0) r.ok = -2;   // no IMU factor (no samples / covariance not positive definite): no solve ran
+  const double* pose = a.fused ? a.fused[b].state : a.nls[b].pose;
+  r.summary = a.fused ? a.fused[b].summary : a.nls[b].summary;
+  for (int i = 0; i < 7; ++i) r.pose_observation_in_submap[i] = pose[i];
+  const Rigidd est = compose(a.submap, pose_from7(pose));  // LTB:553-554
+  pose_to7(est, r.pose_estimate_local);
+  if (a.fused && a.states_out) {  // solver state (submap frame) -> dl_nav_state in the local frame
+    dl_nav_state& o = a.states_out[b];
+    const Vec3d v = rotate(a.submap.q, Vec3d{pose[7], pose[8], pose[9]});
+    o.p[0] = est.t.x; o.p[1] = est.t.y; o.p[2] = est.t.z;
+    o.q[0] = est.q.w; o.q[1] = est.q.x; o.q[2] = est.q.y; o.q[3] = est.q.z;
+    o.v[0] = v.x; o.v[1] = v.y; o.v[2] = v.z;
+    for (int k = 0; k < 3; ++k) { o.ba[k] = pose[10 + k]; o.bg[k] = pose[13 + k]; }
+  }
+}
+
 }  // namespace
 
 int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch) {
@@ -600,6 +665,31 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
   const int parts = 4;  // CTAs per scan: a 74-scan sub-batch x 4 = 296 CTAs of 512 threads, about two per SM of an H100
   fe_emit_tracking<<<dim3(parts, batch), kEmitBlock, smem, ctx->stream>>>(a, max_chunks);
   DL_LAUNCH_CHECK(ctx, "fe_emit_tracking");
+  return DL_OK;
+}
+
+int launch_gather_rows(dl_context* ctx, const float* in, int64_t cap_in, int pairs_per_cloud, const int32_t* keep,
+                       const int32_t* keep_counts, int64_t cap_out, float* out, int pairs) {
+  if (pairs <= 0) return DL_OK;
+  const dim3 grid((unsigned)std::min<int64_t>((cap_out + kBlock - 1) / kBlock, 8), pairs);
+  gather_rows_kernel<<<grid, kBlock, 0, ctx->stream>>>(in, cap_in, pairs_per_cloud, keep, keep_counts, cap_out, out);
+  DL_LAUNCH_CHECK(ctx, "gather_rows_kernel");
+  return DL_OK;
+}
+
+int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd& submap_inverse,
+                        double* initial_pose, double* target_translation) {
+  if (batch <= 0) return DL_OK;
+  initial_pose_kernel<<<(batch + 127) / 128, 128, 0, ctx->stream>>>(batch, current_pose, submap_inverse, initial_pose,
+                                                                    target_translation);
+  DL_LAUNCH_CHECK(ctx, "initial_pose_kernel");
+  return DL_OK;
+}
+
+int launch_finalize_results(dl_context* ctx, const ResultArgs& a) {
+  if (a.batch <= 0) return DL_OK;
+  finalize_results_kernel<<<(a.batch + 127) / 128, 128, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "finalize_results_kernel");
   return DL_OK;
 }
 

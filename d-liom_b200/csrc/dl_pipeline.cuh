@@ -1,4 +1,4 @@
-// Argument blocks of the batched front-end kernels (dl_ingest.cu) and their launchers.
+// Argument blocks of the batched front-end kernels (dl_frontend.cu, dl_imu.cu) and their launchers.
 #pragma once
 #include "dl_internal.cuh"
 
@@ -47,27 +47,6 @@ struct ImuPrepareArgs {
 };
 int launch_imu_prepare(dl_context* ctx, const ImuPrepareArgs& a);
 
-struct IngestArgs {
-  const float* ranges;        // all scans, RangeMeasurement rows (8 floats); scan b starts at row b * in_cap
-  int64_t in_cap;
-  const ScanConstants* scans;
-  const float* origins;       // 3 floats per sensor
-  const int32_t* keep;        // first voxel filter survivors, b * cap + k -> row within the scan
-  const int32_t* keep_counts;
-  int64_t cap;
-  int tiles;
-  float min_range, max_range;
-  double scan_period;
-  float* tmp_points;          // b * cap * 3
-  uint8_t* cls;               // b * cap
-  int32_t* tile_counts;       // b * tiles * 2
-  float* returns_local;       // b * cap * 3
-  float* misses_local;
-  int32_t* num_returns;
-  int32_t* num_misses;
-  float* current_pose;        // b * 7 floats (t, q wxyz)
-};
-
 // Fused front half (dl_frontend.cu).
 struct FrontendArgs {
   const float* ranges;   // scan b starts at row b * in_cap; rows of row_floats floats (3: x y z, 4: x y z t, 8: + u64 origin index)
@@ -83,7 +62,6 @@ struct FrontendArgs {
   const ScanConstants* scans;
   const float* origins;
   int64_t cap;           // per-scan capacity of every per-point array below
-  int tiles;             // ceil(cap / 256)
   int64_t tcap1, tcap2;  // table capacities (powers of two)
   float first_resolution, second_resolution, min_range, max_range;
   double scan_period;
@@ -122,9 +100,6 @@ struct ResultArgs {
   dl_scan_result* results;
 };
 
-int launch_ingest(dl_context* ctx, const IngestArgs& a, int batch);
-int launch_gather_to_tracking(dl_context* ctx, const float* in, int64_t cap, const int32_t* keep,
-                              const int32_t* keep_counts, const float* current_pose, float* out, int batch);
 int launch_gather_rows(dl_context* ctx, const float* in, int64_t cap_in, int pairs_per_cloud, const int32_t* keep,
                        const int32_t* keep_counts, int64_t cap_out, float* out, int pairs);
 int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd& submap_inverse,

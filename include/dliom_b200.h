@@ -613,9 +613,11 @@ int dl_decode_point_cloud2_dev(dl_context* ctx, const dl_point_cloud2_layout* la
                                int64_t num_points, const double* sensor_to_tracking, float* rows_out_dev,
                                int64_t* num_rows_out, double* stamp_offset_seconds);
 
-/* Scan ingest only (LTB:393-487). ranges: n RangeMeasurement rows (32 bytes: x y z t + uint64 origin index);
- * origins: 3 floats per sensor. Outputs have capacity n rows. counts_out[4] = {first filter survivors,
- * returns (local frame, before 2nd filter), returns in tracking frame, misses in tracking frame}. */
+/* Scan ingest only (LTB:393-487): the batched front half of dl_frontend_match_batch run on one scan.
+ * ranges: n RangeMeasurement rows (32 bytes: x y z t + uint64 origin index); origins: 3 floats per sensor.
+ * Outputs have capacity n rows. counts_out[4] = {first filter survivors, returns (local frame, before 2nd filter),
+ * returns in tracking frame, misses in tracking frame}. DL_ERR_ARG if a point lies outside the voxel-key span of
+ * the second voxel filter (where a batched call would report ok = -1 for the scan, see dl_scan_result). */
 int dl_ingest_scan(dl_context* ctx, const dl_frontend_options* options, const void* ranges, int64_t n,
                    const float* origins, int32_t num_origins, const double* prev_pose, const double* predicted_pose,
                    int64_t* first_keep_out, float* returns_local_out, float* returns_tracking_out,

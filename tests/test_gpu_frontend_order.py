@@ -22,8 +22,8 @@ def ctx():
 
 
 def assert_ingest_equal(ctx, orc, w, rows, s=0):
-    """dl_ingest_scan runs the fused kernels (and checks their counts against the stage-wise ones); the tracking-frame clouds
-    and the current pose come from the fused path."""
+    """dl_ingest_scan runs the fused kernels on one scan: first_keep and returns_local come from the first filter's bitmap and
+    the local-frame records, the tracking-frame clouds and the current pose from the compaction."""
     import dliom
     fo = dliom.FrontendOptions.from_oracle(w["opts"])
     want = orc.ingest_scan(w["opts"], rows, w["origin"], w["prev"][s], w["cur"][s])
@@ -132,3 +132,23 @@ def test_key_range_flag_inside_a_tile(ctx, orc):
     res = ctx.frontend_match_batch(fo, [near, flagged, near], w["origin"], w["prev"][[0, 0, 0]], w["cur"][[0, 0, 0]],
                                    w["submap_pose"], hi, lo)
     assert (res[0].ok, res[1].ok, res[2].ok) == (1, -1, 1)
+
+
+def test_key_range_flag_fails_ingest_scan(ctx):
+    """dl_ingest_scan on 32-byte rows with one point beyond the key span of a 0.4 mm second filter fails with DL_ERR_ARG."""
+    import dliom
+    w = workload()
+    fo = dliom.FrontendOptions.from_oracle(w["opts"])
+    fo.voxel_filter_size = 4e-4
+    full = w["scans"][0]
+    dist = np.sqrt(full["x"] ** 2 + full["y"] ** 2 + full["z"] ** 2)
+    near = full[dist < 5.0].copy()
+    near["t"][-1] = 0.0
+    assert len(near) > 500
+    flagged = near.copy()
+    for k in "xyz":
+        flagged[k][len(near) // 2] = full[dist > 20.0][0][k]
+    assert len(ctx.ingest_scan(fo, near, w["origin"], w["prev"][0], w["cur"][0])["returns_tracking"]) > 0
+    with pytest.raises(dliom.DlError) as e:
+        ctx.ingest_scan(fo, flagged, w["origin"], w["prev"][0], w["cur"][0])
+    assert e.value.status == -2 and "key span" in str(e.value)   # DL_ERR_ARG
