@@ -3,18 +3,23 @@
 // (LTB:605-610) and the loop-closure matcher compares (SM/rotational_scan_matcher.cc:31-121, :159-170).
 //
 // The reference buckets the cloud into 0.2 m slices (std::map -> ascending slice order, points in input order), sorts each
-// slice by the angle around its centroid and walks it sequentially, adding into ONE float histogram; every float sum here
-// keeps that order:
+// slice by the angle around its centroid (SortSlice, :94-121) and walks the SORTED slice (AddPointCloudSliceToHistogram,
+// :63-92), which takes the centroid again, of the points SortSlice kept and in their sorted order; it adds into ONE float
+// histogram. Every float sum here keeps the reference's order:
 //   1. key = (slice, input index) -> bitonic sort: slices contiguous, ascending, input order inside        (whole CTA)
-//   2. centroid of a slice = sequential float sum over its points, one thread per slice                     (:54-61)
-//   3. key = (slice, atan2 of the offset from the centroid, index); points closer than 0.2 m dropped -> sort (:94-121)
-//   4. one thread per slice walks its sorted points with the reference's `last`-point logic and emits one
-//      (bucket, value) event per point                                                                      (:63-92)
+//   2. first centroid of a slice = sequential float sum over its points in input order, one thread per slice (:54-61)
+//   3. key = (slice, atan2 of the offset from the first centroid, index); points closer than 0.2 m dropped -> sort (:94-121)
+//   4. one thread per slice: exact-angle fix-up of the sort, second centroid = sequential float sum over the kept points in
+//      sorted order, then the walk with the reference's `last`-point logic, one (bucket, value) event per point     (:63-92)
 //   5. one thread per bucket adds its events in (slice, point) order = the order of the reference's += chain (:31-52)
 // One CTA per cloud; the sorts run in global memory (the arrays are L2-resident: 8 B per point).
-// Float parity: the sums are ordered like the reference's, but atan2f / sqrtf are the device's (atan2f <= 2 ulp), so a point
-// whose angle sits on a bucket or ordering boundary can land differently than on the CPU: compared with a tolerance in the
-// tests, not bit for bit. Compiled -fmad=false like everything that mirrors the reference's float expressions.
+// Float parity: compiled -fmad=false, so every sqrt, division and sum is the reference's IEEE operation in the reference's
+// order, and the histogram is bit-identical to the reference's except through atan2f. The device's atan2f and glibc's are
+// each within a few ulps of the true angle, so only a point whose angle lies within a few ulps of another point's angle in
+// its slice (the sort) or of a bucket boundary (the walk) can be decided differently. Equal angles keep input order (the
+// order libstdc++'s insertion sort gives slices of at most 16 points; std::sort leaves it unspecified beyond), with -0 and +0
+// equal as std::sort's operator< sees them. tests/test_gpu_rotational_histogram.py checks bit equality on clouds cleared of
+// such points and, on scene clouds, that any difference comes from one.
 #include "dl_internal.cuh"
 
 namespace dl {
@@ -118,7 +123,7 @@ __global__ void __launch_bounds__(kThreads) rotational_histogram_kernel(Histogra
   bitonic_sort(a.keys, a.np2);
   find_slices(a, a.n);
   const int num_slices = a.counters[0];
-  // ---- 2. centroids (sequential float sums in input order, per slice)
+  // ---- 2. first centroids (sequential float sums in input order, per slice)
   for (int s = threadIdx.x; s < num_slices; s += kThreads) {
     float sx = 0.f, sy = 0.f;
     const int b = a.slice_first[s], e = a.slice_first[s + 1];
@@ -141,8 +146,11 @@ __global__ void __launch_bounds__(kThreads) rotational_histogram_kernel(Histogra
       const int i = (int)(key & 0xFFFFFFFFFFFull);
       const float dx = a.points[3 * i] - cx, dy = a.points[3 * i + 1] - cy;
       unsigned long long out = kPad;
-      if (!(sqrtf(dx * dx + dy * dy) < kMinDistance))
-        out = ((unsigned long long)s << 44) | ((unsigned long long)(order_bits(atan2f(dy, dx)) >> 8) << 20) | (unsigned long long)(k - b);
+      if (!(sqrtf(dx * dx + dy * dy) < kMinDistance)) {
+        float angle = atan2f(dy, dx);
+        if (angle == 0.f) angle = 0.f;  // -0 sorts with +0 (std::sort's operator< sees them equal): input order decides
+        out = ((unsigned long long)s << 44) | ((unsigned long long)(order_bits(angle) >> 8) << 20) | (unsigned long long)(k - b);
+      }
       // 20 bits slice ordinal | 24 bits angle | 20 bits position inside the slice (ties and the lost low angle bits resolve
       // towards input order; std::sort leaves that order unspecified)
       a.keys[k] = out;
@@ -189,13 +197,21 @@ __global__ void __launch_bounds__(kThreads) rotational_histogram_kernel(Histogra
         }
       }
     }
+    // the walk's centroid: AddPointCloudSliceToHistogram takes it of the sorted slice (kept points, sorted order)
+    float sx = 0.f, sy = 0.f;
+    for (int k = begin; k < end; ++k) {
+      const int i = point_of(k);
+      sx += a.points[3 * i];
+      sy += a.points[3 * i + 1];
+    }
+    const float wx = sx / (float)(end - begin), wy = sy / (float)(end - begin);
     int il = point_of(begin);
     float lx = a.points[3 * il], ly = a.points[3 * il + 1];
     for (int k = begin; k < end; ++k) {
       const int i = point_of(k);
       const float px = a.points[3 * i], py = a.points[3 * i + 1];
       const float dx = px - lx, dy = py - ly;
-      const float ccx = px - cx, ccy = py - cy;
+      const float ccx = px - wx, ccy = py - wy;
       const float distance = sqrtf(dx * dx + dy * dy);
       const float direction_norm = sqrtf(ccx * ccx + ccy * ccy);
       int bucket = -1;

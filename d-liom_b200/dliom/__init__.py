@@ -650,6 +650,14 @@ class Context:
                                                    C.byref(npass)))
         return keep[:m.value].copy(), passes[:npass.value].copy()
 
+    # ---- RotationalScanMatcher::ComputeHistogram
+    def rotational_histogram(self, points, size):
+        """Histogram of `size` buckets of the n x 3 cloud (gravity-aligned frame); size in [1, 1024], n <= 2^20."""
+        points = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+        out = np.zeros(max(int(size), 0), np.float32)
+        self.check(self.L.dl_rotational_histogram(self.h, points, len(points), int(size), out))
+        return out
+
     # ---- matchers
     def rtcsm_match(self, grid, points, initial_pose, linear_window, angular_window, w_t, w_r, want_scores=False):
         points = np.ascontiguousarray(points, np.float32).reshape(-1, 3)

@@ -169,32 +169,6 @@ def test_builder_initialisation_motion_filter_and_drops(orc):
     b.close(); b2.close(); ctx.close()
 
 
-def test_rotational_histogram_against_oracle(orc):
-    import dliom
-    ctx = dliom.Context(0)
-    times, scans = drive(2)
-    opts = orc.FrontEndOptions.defaults()
-    for rows, t in zip(scans, times):
-        import synth
-        pts = orc.ingest_scan(opts, rows, np.zeros((1, 3), np.float32), synth.pose7(t - 0.1), synth.pose7(t))["returns_tracking"]
-        want = orc.compute_histogram(pts, 120)
-        got = np.zeros(120, np.float32)
-        ctx.check(ctx.L.dl_rotational_histogram(ctx.h, np.ascontiguousarray(pts), len(pts), 120, got))
-        assert want.sum() > 1.0
-        assert abs(got.sum() - want.sum()) <= 2e-3 * want.sum()
-        assert np.abs(got - want).sum() <= 0.02 * want.sum()
-    # tiny hand-made slice: four corners of a square ring + an interior point (dropped: closer than 0.2 m to the centroid)
-    sq = np.array([[1, 0, 0.0], [0, 1, 0.0], [-1, 0, 0.0], [0, -1, 0.0], [0.05, 0.0, 0.0]], np.float32) * np.float32(0.5)
-    want = orc.compute_histogram(sq, 8)
-    got = np.zeros(8, np.float32)
-    ctx.check(ctx.L.dl_rotational_histogram(ctx.h, sq, len(sq), 8, got))
-    assert np.allclose(got, want, atol=1e-5)
-    empty = np.ones(8, np.float32)
-    ctx.check(ctx.L.dl_rotational_histogram(ctx.h, np.zeros((1, 3), np.float32), 0, 8, empty))   # no points: all zero
-    assert not empty.any()
-    ctx.close()
-
-
 def _synchronize(prior, secondary_queue):
     """Python twin of RangeDataSynchronizer::AddRangeData for the prior sensor (range_data_synchronizer.cc:43-109):
     prior = (time, xyzt float32 [n,4]); secondary_queue = list of (time, xyzt). Returns RangeMeasurement rows + number merged."""
