@@ -306,7 +306,7 @@ __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, con
     h = __ldg((const float4*)(rows + (size_t)i * rf));
   }
   const unsigned long long origin_index = rf >= 8 ? *(const unsigned long long*)(rows + (size_t)i * rf + 4) : 0ull;
-  const float* o = a.origins + 3 * origin_index;
+  const float* o = a.origins + 3 * (origin_index + (unsigned long long)a.origin_base[b]);
   if (!kRunPose) pose = point_pose(sc, no_deskew, a.scan_period, h.w);
   const Vec3f hit = apply(pose, Vec3f{h.x, h.y, h.z});
   const Vec3f org = apply(pose, Vec3f{o[0], o[1], o[2]});
@@ -569,13 +569,13 @@ __global__ void __launch_bounds__(kBlock) gather_rows_kernel(const float* __rest
 }
 
 // initial_ceres_pose = submap.local_pose^-1 * pose_prediction, pose_prediction = current_pose.cast<double>() (LTB:476-487, :504-505)
-__global__ void initial_pose_kernel(int batch, const float* __restrict__ current_pose, Rigidd submap_inverse,
+__global__ void initial_pose_kernel(int batch, const float* __restrict__ current_pose, const Rigidd* __restrict__ submap_inverse,
                                     double* __restrict__ initial_pose, double* __restrict__ target_translation) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= batch) return;
   const float* cp = current_pose + 7 * b;
   const Rigidd prediction = to_double(Rigidf{{cp[0], cp[1], cp[2]}, {cp[3], cp[4], cp[5], cp[6]}});
-  const Rigidd init = compose(submap_inverse, prediction);
+  const Rigidd init = compose(submap_inverse[b], prediction);
   pose_to7(init, initial_pose + 7 * b);
   target_translation[3 * b] = init.t.x;
   target_translation[3 * b + 1] = init.t.y;
@@ -605,11 +605,12 @@ __global__ void finalize_results_kernel(ResultArgs a) {
   const double* pose = a.fused ? a.fused[b].state : a.nls[b].pose;
   r.summary = a.fused ? a.fused[b].summary : a.nls[b].summary;
   for (int i = 0; i < 7; ++i) r.pose_observation_in_submap[i] = pose[i];
-  const Rigidd est = compose(a.submap, pose_from7(pose));  // LTB:553-554
+  const Rigidd submap = a.submap[b];
+  const Rigidd est = compose(submap, pose_from7(pose));  // LTB:553-554
   pose_to7(est, r.pose_estimate_local);
   if (a.fused && a.states_out) {  // solver state (submap frame) -> dl_nav_state in the local frame
     dl_nav_state& o = a.states_out[b];
-    const Vec3d v = rotate(a.submap.q, Vec3d{pose[7], pose[8], pose[9]});
+    const Vec3d v = rotate(submap.q, Vec3d{pose[7], pose[8], pose[9]});
     o.p[0] = est.t.x; o.p[1] = est.t.y; o.p[2] = est.t.z;
     o.q[0] = est.q.w; o.q[1] = est.q.x; o.q[2] = est.q.y; o.q[3] = est.q.z;
     o.v[0] = v.x; o.v[1] = v.y; o.v[2] = v.z;
@@ -677,7 +678,7 @@ int launch_gather_rows(dl_context* ctx, const float* in, int64_t cap_in, int pai
   return DL_OK;
 }
 
-int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd& submap_inverse,
+int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd* submap_inverse,
                         double* initial_pose, double* target_translation) {
   if (batch <= 0) return DL_OK;
   initial_pose_kernel<<<(batch + 127) / 128, 128, 0, ctx->stream>>>(batch, current_pose, submap_inverse, initial_pose,

@@ -12,7 +12,7 @@
 //   4. one thread per slice: exact-angle fix-up of the sort, second centroid = sequential float sum over the kept points in
 //      sorted order, then the walk with the reference's `last`-point logic, one (bucket, value) event per point     (:63-92)
 //   5. one thread per bucket adds its events in (slice, point) order = the order of the reference's += chain (:31-52)
-// One CTA per cloud; the sorts run in global memory (the arrays are L2-resident: 8 B per point).
+// One CTA per cloud (several clouds in one launch through an argument array); the sorts run in global memory (the arrays are L2-resident: 8 B per point).
 // Float parity: compiled -fmad=false, so every sqrt, division and sum is the reference's IEEE operation in the reference's
 // order, and the histogram is bit-identical to the reference's except through atan2f. The device's atan2f and glibc's are
 // each within a few ulps of the true angle, so only a point whose angle lies within a few ulps of another point's angle in
@@ -20,6 +20,8 @@
 // order libstdc++'s insertion sort gives slices of at most 16 points; std::sort leaves it unspecified beyond), with -0 and +0
 // equal as std::sort's operator< sees them. tests/test_gpu_rotational_histogram.py checks bit equality on clouds cleared of
 // such points and, on scene clouds, that any difference comes from one.
+#include <vector>
+
 #include "dl_internal.cuh"
 
 namespace dl {
@@ -105,7 +107,9 @@ __device__ void find_slices(const HistogramArgs& a, int count) {
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kThreads) rotational_histogram_kernel(HistogramArgs a) {
+// many == nullptr: the one cloud `one`; otherwise cloud blockIdx.x of `many`.
+__global__ void __launch_bounds__(kThreads) rotational_histogram_kernel(HistogramArgs one, const HistogramArgs* __restrict__ many) {
+  const HistogramArgs a = many ? many[blockIdx.x] : one;
   const float kSliceHeight = 0.2f, kMinDistance = 0.2f, kMaxDistance = 0.9f;
   const float kPi = 3.14159274101257324f;  // (float)M_PI
   // ---- 1. (slice, index) keys
@@ -273,11 +277,7 @@ void carve_rotational_histogram(Arena& a, int64_t n, HistogramScratch* s) {
   s->counters = a.take<int>(2);
 }
 
-// d_points: n x 3 floats on the device. d_histogram: `size` floats (size <= 1024). `s` is carved for n points.
-int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, const float* d_points, int64_t n, int size,
-                                float* d_histogram, int32_t** d_error_out) {
-  if (size < 1 || size > kThreads) return ctx->fail(DL_ERR_ARG, "histogram size must be in [1, 1024]");
-  if (n > (1 << 20)) return ctx->fail(DL_ERR_ARG, "more than 2^20 points in a rotational histogram");
+static HistogramArgs histogram_args(const HistogramScratch& s, const float* d_points, int64_t n, int size, float* d_histogram) {
   HistogramArgs h{};
   h.points = d_points;
   h.n = (int)n;
@@ -290,14 +290,41 @@ int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, cons
   h.ev_value = s.ev_value;
   h.counters = s.counters;
   h.histogram = d_histogram;
+  return h;
+}
+
+// d_points: n x 3 floats on the device. d_histogram: `size` floats (size <= 1024). `s` is carved for n points.
+int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, const float* d_points, int64_t n, int size,
+                                float* d_histogram, int32_t** d_error_out) {
+  if (size < 1 || size > kThreads) return ctx->fail(DL_ERR_ARG, "histogram size must be in [1, 1024]");
+  if (n > (1 << 20)) return ctx->fail(DL_ERR_ARG, "more than 2^20 points in a rotational histogram");
+  const HistogramArgs h = histogram_args(s, d_points, n, size, d_histogram);
   DL_CUDA(ctx, cudaMemsetAsync(h.counters, 0, 2 * sizeof(int), ctx->stream));
   if (n == 0) {
     DL_CUDA(ctx, cudaMemsetAsync(d_histogram, 0, sizeof(float) * size, ctx->stream));
   } else {
-    rotational_histogram_kernel<<<1, kThreads, 0, ctx->stream>>>(h);
+    rotational_histogram_kernel<<<1, kThreads, 0, ctx->stream>>>(h, nullptr);
     DL_LAUNCH_CHECK(ctx, "rotational_histogram_kernel");
   }
   if (d_error_out) *d_error_out = h.counters + 1;
+  return DL_OK;
+}
+
+size_t rotational_histograms_args_bytes(int count) { return sizeof(HistogramArgs) * (size_t)count; }
+
+int launch_rotational_histograms(dl_context* ctx, const HistogramScratch* s, const float* const* d_points, const int64_t* n,
+                                 int count, int size, float* const* d_histograms, void* d_args) {
+  if (count <= 0) return DL_OK;
+  if (size < 1 || size > kThreads) return ctx->fail(DL_ERR_ARG, "histogram size must be in [1, 1024]");
+  std::vector<HistogramArgs> h(count);
+  for (int k = 0; k < count; ++k) {
+    if (n[k] < 1 || n[k] > (1 << 20)) return ctx->fail(DL_ERR_ARG, "every cloud of a histogram batch needs 1 to 2^20 points");
+    h[k] = histogram_args(s[k], d_points[k], n[k], size, d_histograms[k]);
+    DL_CUDA(ctx, cudaMemsetAsync(h[k].counters, 0, 2 * sizeof(int), ctx->stream));
+  }
+  DL_CUDA(ctx, cudaMemcpyAsync(d_args, h.data(), sizeof(HistogramArgs) * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
+  rotational_histogram_kernel<<<count, kThreads, 0, ctx->stream>>>(h[0], (const HistogramArgs*)d_args);
+  DL_LAUNCH_CHECK(ctx, "rotational_histogram_kernel");
   return DL_OK;
 }
 

@@ -212,8 +212,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) imu_prepare_kernel(ImuPre
     const Rigidd prev{pi, qi}, cur{pj, qj};
     a.scans[b] = make_scan_constants(prev, cur);
     // the factor in the submap frame (the grids live there and the solve is frame-invariant)
-    const Rigidd pose_i = compose(a.to_submap, prev), pose_j = compose(a.to_submap, cur);
-    const Vec3d wi = rotate(a.to_submap.q, vi), wj = rotate(a.to_submap.q, vj), Gs = rotate(a.to_submap.q, G);
+    const Rigidd to_submap = a.to_submap[b];
+    const Rigidd pose_i = compose(to_submap, prev), pose_j = compose(to_submap, cur);
+    const Vec3d wi = rotate(to_submap.q, vi), wj = rotate(to_submap.q, vj), Gs = rotate(to_submap.q, G);
     t.pi[0] = pose_i.t.x; t.pi[1] = pose_i.t.y; t.pi[2] = pose_i.t.z;
     t.qi[0] = pose_i.q.w; t.qi[1] = pose_i.q.x; t.qi[2] = pose_i.q.y; t.qi[3] = pose_i.q.z;
     t.vi[0] = wi.x; t.vi[1] = wi.y; t.vi[2] = wi.z;

@@ -13,6 +13,12 @@
 // Structure growth is lock-free and spin-free: (1) claim missing top entries, (2) claim missing node entries — one
 // kernel each, so nobody ever waits for an allocation made in the same kernel — then (3) hits, (4) misses,
 // (5) FinishUpdate over the list of touched cells.
+// One call inserts into many grids (a list of jobs, blockIdx.y = job): jobs of distinct grids touch distinct cells, so they run
+// side by side, and the host steps (bounding boxes, pool growth) are taken once for all of them.
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
 
@@ -24,6 +30,7 @@ constexpr int kBlock = 256;
 struct InsertArgs {
   const float* returns;  // n x 3, already in the grid's frame
   int n;
+  const int32_t* n_dev;  // bounding-box pass only, optional: the point count on the device (n is then an upper bound)
   Vec3f origin;
   float resolution;
   int bits;
@@ -57,14 +64,16 @@ __device__ __forceinline__ void for_each_cell(const InsertArgs& a, int i, int ph
     f(Int3{o.x + d.x * position / num_samples, o.y + d.y * position / num_samples, o.z + d.z * position / num_samples});
 }
 
-__global__ void ins_bbox_kernel(InsertArgs a) {
+__global__ void ins_bbox_kernel(const InsertArgs* __restrict__ jobs) {
+  const InsertArgs a = jobs[blockIdx.y];
+  const int n = a.n_dev ? *a.n_dev : a.n;
   int lo[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, hi[3] = {-0x7fffffff, -0x7fffffff, -0x7fffffff};
   auto add = [&](const Int3& c) {
     lo[0] = min(lo[0], c.x); lo[1] = min(lo[1], c.y); lo[2] = min(lo[2], c.z);
     hi[0] = max(hi[0], c.x); hi[1] = max(hi[1], c.y); hi[2] = max(hi[2], c.z);
   };
-  for (int i = blockIdx.x * kBlock + threadIdx.x; i < a.n; i += gridDim.x * kBlock) add(hit_cell(a, i));
-  if (blockIdx.x == 0 && threadIdx.x == 0 && a.num_free > 0 && a.n > 0) add(cell_index(a.origin, a.resolution));
+  for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) add(hit_cell(a, i));
+  if (blockIdx.x == 0 && threadIdx.x == 0 && a.num_free > 0 && n > 0) add(cell_index(a.origin, a.resolution));
   for (int k = 0; k < 3; ++k) {
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) {
@@ -100,7 +109,8 @@ __device__ __forceinline__ void shifted(const InsertArgs& a, const Int3& c, unsi
 //   ASSIGN = 0  mark every missing entry this Insert touches (-1 -> -2) and count them in counters[3 + LEVEL];
 //   ASSIGN = 1  after the host has grown the pool by that count: give every marked entry its slot (-2 -> index).
 template <int LEVEL, int ASSIGN>
-__global__ void __launch_bounds__(kBlock) ins_claim_kernel(InsertArgs a, int phase) {
+__global__ void __launch_bounds__(kBlock) ins_claim_kernel(const InsertArgs* __restrict__ jobs, int phase) {
+  const InsertArgs a = jobs[blockIdx.y];
   for (int i = blockIdx.x * kBlock + threadIdx.x; i < a.n; i += gridDim.x * kBlock) {
     for_each_cell(a, i, phase, [&](const Int3& c) {
       unsigned sx, sy, sz;
@@ -122,7 +132,8 @@ __global__ void __launch_bounds__(kBlock) ins_claim_kernel(InsertArgs a, int pha
   }
 }
 
-__global__ void __launch_bounds__(kBlock) ins_apply_kernel(InsertArgs a, int phase) {
+__global__ void __launch_bounds__(kBlock) ins_apply_kernel(const InsertArgs* __restrict__ jobs, int phase) {
+  const InsertArgs a = jobs[blockIdx.y];
   const uint16_t* table = phase == 0 ? a.hit_table : a.miss_table;
   for (int i = blockIdx.x * kBlock + threadIdx.x; i < a.n; i += gridDim.x * kBlock) {
     for_each_cell(a, i, phase, [&](const Int3& c) {
@@ -150,7 +161,8 @@ __global__ void __launch_bounds__(kBlock) ins_apply_kernel(InsertArgs a, int pha
 }
 
 // FinishUpdate: remove the update marker from every cell touched by this Insert.
-__global__ void ins_finish_kernel(InsertArgs a) {
+__global__ void ins_finish_kernel(const InsertArgs* __restrict__ jobs) {
+  const InsertArgs a = jobs[blockIdx.y];
   const int count = a.counters[2];
   for (int k = blockIdx.x * kBlock + threadIdx.x; k < count; k += gridDim.x * kBlock) {
     const uint32_t cell = a.update_list[k];
@@ -158,10 +170,18 @@ __global__ void ins_finish_kernel(InsertArgs a) {
   }
 }
 
-__global__ void transform_filter_kernel(const float* __restrict__ in, int n, Rigidf to_submap, Vec3f origin_submap,
-                                        float max_range, float* __restrict__ all, float* __restrict__ near,
-                                        int32_t* near_count, int32_t* tile_counts, int pass) {
-  // pass 0: transform + per-tile count of in-range points; pass 1: ordered scatter of the in-range ones
+__global__ void transform_filter_kernel(const TransformJob* __restrict__ jobs, int pass) {
+  // pass 0: transform + per-tile count of in-range points; pass 1: ordered scatter of the in-range ones. blockIdx.y = job.
+  const TransformJob& job = jobs[blockIdx.y];
+  const int n = job.n;
+  if ((int)blockIdx.x * kBlock >= max(n, 1)) return;  // the launch covers the longest job (whole CTAs: the ballots below)
+  const float* __restrict__ in = job.in;
+  const Rigidf to_submap = job.to_submap;
+  const Vec3f origin_submap = job.origin_submap;
+  const float max_range = job.max_range;
+  float* __restrict__ all = job.all;
+  float* __restrict__ near = job.near;
+  int32_t* tile_counts = job.tile_counts;
   __shared__ int warp_sums[kBlock / 32];
   const int i = blockIdx.x * kBlock + threadIdx.x;
   Vec3f p{0, 0, 0};
@@ -190,7 +210,29 @@ __global__ void transform_filter_kernel(const float* __restrict__ in, int n, Rig
     float* o = near + 3 * (size_t)(tile_base + base + __popc(ballot & ((1u << lane) - 1)));
     o[0] = p.x; o[1] = p.y; o[2] = p.z;
   }
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *near_count = tile_base + total;
+  if ((int)blockIdx.x == (max(n, 1) + kBlock - 1) / kBlock - 1 && threadIdx.x == 0) *job.near_count = tile_base + total;
+}
+
+// range_data_in_local = opt_pose * returns / misses (LTB:559-560) and the gravity-aligned returns of the histogram
+// (Rotation(gravity_alignment) * returns, LTB:605-610), float arithmetic of dl_math.cuh without contraction: the bits of the
+// host loop it replaces. blockIdx.y = job; x covers returns, then misses.
+__global__ void local_frame_kernel(const LocalFrameJob* __restrict__ jobs) {
+  const LocalFrameJob& job = jobs[blockIdx.y];
+  const int n = job.num_returns + job.num_misses;
+  for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) {
+    const bool ret = i < job.num_returns;
+    const int k = ret ? i : i - job.num_returns;
+    const float* src = (ret ? job.returns : job.misses) + 3 * (size_t)k;
+    const Vec3f p{src[0], src[1], src[2]};
+    const Vec3f l = apply(job.pose, p);
+    float* dst = (ret ? job.returns_local : job.misses_local) + 3 * (size_t)k;
+    dst[0] = l.x; dst[1] = l.y; dst[2] = l.z;
+    if (ret) {
+      const Vec3f g = apply(job.gravity_alignment, p);
+      float* d = job.returns_aligned + 3 * (size_t)k;
+      d[0] = g.x; d[1] = g.y; d[2] = g.z;
+    }
+  }
 }
 
 }  // namespace
@@ -211,98 +253,217 @@ void compute_odds_table(float probability, uint16_t* table) {
   }
 }
 
-int grid_reserve_pools(dl_grid* g, int pending_counter, int level);
 int grid_ensure_device_state(dl_grid* g);
+int grid_grow_pool(dl_grid* g, int level, size_t used, size_t add);
 
-// One RangeDataInserter3D::Insert on the device grid. `d_returns` (n x 3 floats, grid frame) is device memory.
-int grid_insert_device(dl_context* ctx, dl_grid* g, const Vec3f& origin, const float* d_returns, int n, int num_free,
-                       const uint16_t* d_hit_table, const uint16_t* d_miss_table, int32_t* d_bbox, uint32_t* d_update_list) {
-  if (n <= 0) return DL_OK;
-  DL_TRY_STATUS(grid_ensure_device_state(g));
-  InsertArgs a{};
-  a.returns = d_returns; a.n = n; a.origin = origin; a.resolution = g->resolution; a.num_free = num_free;
-  a.bbox = d_bbox; a.update_list = d_update_list; a.hit_table = d_hit_table; a.miss_table = d_miss_table;
-  const int blocks = std::min(kNumSMs * 8, (n + kBlock - 1) / kBlock);
-  // 1. which cells will be touched -> does the top level have to grow (CHECK_LE(new_bits, 8))?
-  const int32_t init[6] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff, -0x7fffffff, -0x7fffffff};
-  DL_CUDA(ctx, cudaMemcpyAsync(d_bbox, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-  ins_bbox_kernel<<<blocks, kBlock, 0, ctx->stream>>>(a);
-  DL_LAUNCH_CHECK(ctx, "ins_bbox_kernel");
-  int32_t bbox[6];
-  DL_CUDA(ctx, cudaMemcpyAsync(bbox, d_bbox, sizeof(bbox), cudaMemcpyDeviceToHost, ctx->stream));
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  for (;;) {
-    const int half = (64 << g->bits) >> 1;
-    bool fits = true;
-    for (int k = 0; k < 3; ++k) fits = fits && bbox[k] >= -half && bbox[3 + k] < half;
-    if (fits) break;
-    if (g->bits + 1 > 8) return ctx->fail(DL_ERR_GRID_RANGE, "cell index outside +-8192 cells");
-    const size_t new_size = (size_t)8 << (3 * g->bits);
-    int32_t* grown = nullptr;
-    DL_CUDA(ctx, cudaMalloc((void**)&grown, new_size * sizeof(int32_t)));
-    DL_CUDA(ctx, cudaMemsetAsync(grown, 0xFF, new_size * sizeof(int32_t), ctx->stream));
-    const int old_cells = 1 << (3 * g->bits);
-    grid_grow_kernel<<<(old_cells + 255) / 256, 256, 0, ctx->stream>>>(g->d_top, g->bits, grown);
-    DL_LAUNCH_CHECK(ctx, "grid_grow_kernel");
-    DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    DL_CUDA(ctx, cudaFree(g->d_top));
-    g->d_top = grown;
-    g->d_top_cap = new_size;
-    g->bits += 1;
-    // from here on the device copy is ahead of the host mirror, whatever happens next: a later failure (range, out of
-    // memory) must not leave g->bits describing a host `top` of the old size
-    g->mirror_stale = true;
-    g->version++;
+size_t insert_args_bytes(int jobs) { return sizeof(InsertArgs) * (size_t)jobs; }
+
+namespace {
+
+// Grows every job's node pool (level 0) or brick pool (level 1) by exactly the number of entries its Insert marked
+// (counters[3 + level], written by ins_claim_kernel<level, 0>). The grids' counters are gathered on the device into d_gather
+// (8 ints per job) and read back in one copy: one host wait for all grids.
+int reserve_pools(dl_context* ctx, std::vector<InsertArgs>& args, const std::vector<dl_grid*>& grids, int level, int32_t* d_gather) {
+  for (size_t j = 0; j < grids.size(); ++j)
+    DL_CUDA(ctx, cudaMemcpyAsync(d_gather + 8 * j, grids[j]->d_counters, 5 * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  std::vector<int32_t> counters(8 * grids.size());
+  DL_CUDA(ctx, cudaMemcpyAsync(counters.data(), d_gather, counters.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  for (size_t j = 0; j < grids.size(); ++j) {
+    dl_grid* g = grids[j];
+    const int32_t* c = counters.data() + 8 * j;
+    DL_TRY_STATUS(grid_grow_pool(g, level, (size_t)c[level], (size_t)c[3 + level]));
+    if (level == 0) args[j].nodes = g->d_nodes;
+    else args[j].bricks = g->d_bricks;
   }
-  // 2. structure growth with exact reservations: mark + count the missing nodes, grow the node pool by that count, assign;
-  //    then the same for the bricks (whose node entries now exist)
-  a.bits = g->bits; a.top = g->d_top; a.nodes = g->d_nodes; a.bricks = g->d_bricks; a.counters = g->d_counters;
-  DL_CUDA(ctx, cudaMemsetAsync(g->d_counters + 2, 0, 3 * sizeof(int32_t), ctx->stream));
-  const int phases = num_free > 0 ? 2 : 1;
-  for (int phase = 0; phase < phases; ++phase) {
-    ins_claim_kernel<0, 0><<<blocks, kBlock, 0, ctx->stream>>>(a, phase);
-    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<0,0>");
-  }
-  g->mirror_stale = true;  // top entries are marked: the device copy is the only consistent one until the Insert completes
-  g->version++;
-  DL_TRY_STATUS(grid_reserve_pools(g, 3, 0));
-  a.nodes = g->d_nodes;
-  for (int phase = 0; phase < phases; ++phase) {
-    ins_claim_kernel<0, 1><<<blocks, kBlock, 0, ctx->stream>>>(a, phase);
-    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<0,1>");
-  }
-  for (int phase = 0; phase < phases; ++phase) {
-    ins_claim_kernel<1, 0><<<blocks, kBlock, 0, ctx->stream>>>(a, phase);
-    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<1,0>");
-  }
-  DL_TRY_STATUS(grid_reserve_pools(g, 4, 1));
-  a.bricks = g->d_bricks;
-  for (int phase = 0; phase < phases; ++phase) {
-    ins_claim_kernel<1, 1><<<blocks, kBlock, 0, ctx->stream>>>(a, phase);
-    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<1,1>");
-  }
-  ins_apply_kernel<<<blocks, kBlock, 0, ctx->stream>>>(a, 0);
-  DL_LAUNCH_CHECK(ctx, "ins_apply_kernel(hits)");
-  if (num_free > 0) {
-    ins_apply_kernel<<<blocks, kBlock, 0, ctx->stream>>>(a, 1);
-    DL_LAUNCH_CHECK(ctx, "ins_apply_kernel(misses)");
-  }
-  ins_finish_kernel<<<blocks, kBlock, 0, ctx->stream>>>(a);
-  DL_LAUNCH_CHECK(ctx, "ins_finish_kernel");
-  g->mirror_stale = true;
-  g->version++;
   return DL_OK;
 }
 
-int launch_transform_filter(dl_context* ctx, const float* in, int n, const Rigidf& to_submap, const Vec3f& origin_submap,
-                            float max_range, float* all, float* near, int32_t* near_count, int32_t* tile_counts) {
-  if (n <= 0) return DL_OK;
-  const int tiles = (n + kBlock - 1) / kBlock;
+// One round of insert_range_data_device: every grid at most once.
+int insert_round(dl_context* ctx, const InsertJob* const* jobs, int count, int num_free, const uint16_t* d_hit_table,
+                 const uint16_t* d_miss_table, int32_t* d_bbox, InsertArgs* d_args) {
+  std::vector<InsertArgs> args;
+  std::vector<dl_grid*> grids;
+  int widest = 0;
+  for (int j = 0; j < count; ++j) {
+    const InsertJob& job = *jobs[j];
+    if (job.n <= 0) continue;
+    DL_TRY_STATUS(grid_ensure_device_state(job.grid));
+    InsertArgs a{};
+    a.returns = job.returns; a.n = job.n; a.n_dev = job.n_dev; a.origin = job.origin; a.resolution = job.grid->resolution;
+    a.num_free = num_free; a.bbox = d_bbox + 8 * args.size(); a.update_list = job.update_list;
+    a.hit_table = d_hit_table; a.miss_table = d_miss_table;
+    args.push_back(a);
+    grids.push_back(job.grid);
+    widest = std::max(widest, job.n);
+  }
+  if (args.empty()) return DL_OK;
+  const unsigned J = (unsigned)args.size();
+  auto upload = [&]() -> int {
+    DL_CUDA(ctx, cudaMemcpyAsync(d_args, args.data(), sizeof(InsertArgs) * J, cudaMemcpyHostToDevice, ctx->stream));
+    return DL_OK;
+  };
+  // 1. which cells will be touched -> does a top level have to grow (CHECK_LE(new_bits, 8))? One pass over every job.
+  std::vector<int32_t> bbox(8 * J);
+  for (unsigned j = 0; j < J; ++j) {
+    const int32_t init[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff, -0x7fffffff, -0x7fffffff, 0, 0};
+    std::memcpy(bbox.data() + 8 * j, init, sizeof(init));
+  }
+  DL_CUDA(ctx, cudaMemcpyAsync(d_bbox, bbox.data(), sizeof(int32_t) * 8 * J, cudaMemcpyHostToDevice, ctx->stream));
+  DL_TRY_STATUS(upload());
+  ins_bbox_kernel<<<dim3(std::min(kNumSMs * 8, (widest + kBlock - 1) / kBlock), J), kBlock, 0, ctx->stream>>>(d_args);
+  DL_LAUNCH_CHECK(ctx, "ins_bbox_kernel");
+  // the device counts ride in the unused seventh int of each job's box: one read-back, one host wait for every job
+  for (unsigned j = 0; j < J; ++j)
+    if (args[j].n_dev)
+      DL_CUDA(ctx, cudaMemcpyAsync(d_bbox + 8 * j + 6, args[j].n_dev, sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(bbox.data(), d_bbox, sizeof(int32_t) * 8 * J, cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  // jobs whose count on the device is zero drop out; the others carry their exact count from here on
+  {
+    std::vector<InsertArgs> kept_args;
+    std::vector<dl_grid*> kept_grids;
+    std::vector<int32_t> kept_bbox;
+    for (unsigned j = 0; j < J; ++j) {
+      if (args[j].n_dev) args[j].n = bbox[8 * j + 6];
+      args[j].n_dev = nullptr;
+      if (args[j].n <= 0) continue;
+      kept_args.push_back(args[j]);
+      kept_grids.push_back(grids[j]);
+      kept_bbox.insert(kept_bbox.end(), bbox.begin() + 8 * j, bbox.begin() + 8 * j + 8);
+    }
+    args.swap(kept_args);
+    grids.swap(kept_grids);
+    bbox.swap(kept_bbox);
+  }
+  if (args.empty()) return DL_OK;
+  const unsigned K = (unsigned)args.size();
+  widest = 0;
+  for (const InsertArgs& a : args) widest = std::max(widest, a.n);
+  const dim3 blocks(std::min(kNumSMs * 8, (widest + kBlock - 1) / kBlock), K);
+  // 2. top-level growth of whichever grids need it
+  for (unsigned j = 0; j < K; ++j) {
+    dl_grid* g = grids[j];
+    const int32_t* bb = bbox.data() + 8 * j;
+    for (;;) {
+      const int half = (64 << g->bits) >> 1;
+      bool fits = true;
+      for (int k = 0; k < 3; ++k) fits = fits && bb[k] >= -half && bb[3 + k] < half;
+      if (fits) break;
+      if (g->bits + 1 > 8) return ctx->fail(DL_ERR_GRID_RANGE, "cell index outside +-8192 cells");
+      const size_t new_size = (size_t)8 << (3 * g->bits);
+      int32_t* grown = nullptr;
+      DL_CUDA(ctx, cudaMalloc((void**)&grown, new_size * sizeof(int32_t)));
+      DL_CUDA(ctx, cudaMemsetAsync(grown, 0xFF, new_size * sizeof(int32_t), ctx->stream));
+      const int old_cells = 1 << (3 * g->bits);
+      grid_grow_kernel<<<(old_cells + 255) / 256, 256, 0, ctx->stream>>>(g->d_top, g->bits, grown);
+      DL_LAUNCH_CHECK(ctx, "grid_grow_kernel");
+      DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      DL_CUDA(ctx, cudaFree(g->d_top));
+      g->d_top = grown;
+      g->d_top_cap = new_size;
+      g->bits += 1;
+      // from here on the device copy is ahead of the host mirror, whatever happens next: a later failure (range, out of
+      // memory) must not leave g->bits describing a host `top` of the old size
+      g->mirror_stale = true;
+      g->version++;
+    }
+  }
+  // 3. structure growth with exact reservations: mark + count the missing nodes, grow the node pools by those counts, assign;
+  //    then the same for the bricks (whose node entries now exist)
+  for (unsigned j = 0; j < K; ++j) {
+    dl_grid* g = grids[j];
+    InsertArgs& a = args[j];
+    a.bits = g->bits; a.top = g->d_top; a.nodes = g->d_nodes; a.bricks = g->d_bricks; a.counters = g->d_counters;
+    DL_CUDA(ctx, cudaMemsetAsync(g->d_counters + 2, 0, 3 * sizeof(int32_t), ctx->stream));
+  }
+  DL_TRY_STATUS(upload());
+  const int phases = num_free > 0 ? 2 : 1;
+  for (int phase = 0; phase < phases; ++phase) {
+    ins_claim_kernel<0, 0><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
+    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<0,0>");
+  }
+  for (dl_grid* g : grids) {  // top entries are marked: the device copy is the only consistent one until the Insert completes
+    g->mirror_stale = true;
+    g->version++;
+  }
+  DL_TRY_STATUS(reserve_pools(ctx, args, grids, 0, d_bbox));
+  DL_TRY_STATUS(upload());
+  for (int phase = 0; phase < phases; ++phase) {
+    ins_claim_kernel<0, 1><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
+    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<0,1>");
+  }
+  for (int phase = 0; phase < phases; ++phase) {
+    ins_claim_kernel<1, 0><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
+    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<1,0>");
+  }
+  DL_TRY_STATUS(reserve_pools(ctx, args, grids, 1, d_bbox));
+  DL_TRY_STATUS(upload());
+  for (int phase = 0; phase < phases; ++phase) {
+    ins_claim_kernel<1, 1><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
+    DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<1,1>");
+  }
+  ins_apply_kernel<<<blocks, kBlock, 0, ctx->stream>>>(d_args, 0);
+  DL_LAUNCH_CHECK(ctx, "ins_apply_kernel(hits)");
+  if (num_free > 0) {
+    ins_apply_kernel<<<blocks, kBlock, 0, ctx->stream>>>(d_args, 1);
+    DL_LAUNCH_CHECK(ctx, "ins_apply_kernel(misses)");
+  }
+  ins_finish_kernel<<<blocks, kBlock, 0, ctx->stream>>>(d_args);
+  DL_LAUNCH_CHECK(ctx, "ins_finish_kernel");
+  for (dl_grid* g : grids) {
+    g->mirror_stale = true;
+    g->version++;
+  }
+  return DL_OK;
+}
+
+}  // namespace
+
+int insert_range_data_device(dl_context* ctx, const InsertJob* jobs, int count, int num_free, const uint16_t* d_hit_table,
+                             const uint16_t* d_miss_table, int32_t* d_bbox, void* d_args) {
+  // A grid named by several jobs takes them in list order, one round each: within a round every grid appears once.
+  std::vector<const InsertJob*> pending;
+  for (int j = 0; j < count; ++j) pending.push_back(jobs + j);
+  while (!pending.empty()) {
+    std::vector<const InsertJob*> round, later;
+    for (const InsertJob* job : pending) {
+      bool taken = false;
+      for (const InsertJob* r : round) taken = taken || r->grid == job->grid;
+      bool waits = false;  // keep list order per grid: a job never overtakes an earlier one of its grid
+      for (const InsertJob* l : later) waits = waits || l->grid == job->grid;
+      (taken || waits ? later : round).push_back(job);
+    }
+    DL_TRY_STATUS(insert_round(ctx, round.data(), (int)round.size(), num_free, d_hit_table, d_miss_table, d_bbox, (InsertArgs*)d_args));
+    pending.swap(later);
+  }
+  return DL_OK;
+}
+
+size_t transform_jobs_bytes(int jobs) { return sizeof(TransformJob) * (size_t)jobs; }
+
+int launch_transform_filter(dl_context* ctx, const TransformJob* jobs, int count, void* d_jobs) {
+  int widest = 0;
+  for (int j = 0; j < count; ++j) widest = std::max(widest, jobs[j].n);
+  if (widest <= 0) return DL_OK;
+  DL_CUDA(ctx, cudaMemcpyAsync(d_jobs, jobs, sizeof(TransformJob) * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
+  const dim3 tiles((widest + kBlock - 1) / kBlock, count);
   for (int pass = 0; pass < 2; ++pass) {
-    transform_filter_kernel<<<tiles, kBlock, 0, ctx->stream>>>(in, n, to_submap, origin_submap, max_range, all, near,
-                                                               near_count, tile_counts, pass);
+    transform_filter_kernel<<<tiles, kBlock, 0, ctx->stream>>>((const TransformJob*)d_jobs, pass);
     DL_LAUNCH_CHECK(ctx, "transform_filter_kernel");
   }
+  return DL_OK;
+}
+
+size_t local_frame_jobs_bytes(int jobs) { return sizeof(LocalFrameJob) * (size_t)jobs; }
+
+int launch_local_frame(dl_context* ctx, const LocalFrameJob* jobs, int count, void* d_jobs) {
+  int widest = 0;
+  for (int j = 0; j < count; ++j) widest = std::max(widest, jobs[j].num_returns + jobs[j].num_misses);
+  if (widest <= 0) return DL_OK;
+  DL_CUDA(ctx, cudaMemcpyAsync(d_jobs, jobs, sizeof(LocalFrameJob) * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
+  local_frame_kernel<<<dim3(std::min(64, (widest + kBlock - 1) / kBlock), count), kBlock, 0, ctx->stream>>>((const LocalFrameJob*)d_jobs);
+  DL_LAUNCH_CHECK(ctx, "local_frame_kernel");
   return DL_OK;
 }
 

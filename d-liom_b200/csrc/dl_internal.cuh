@@ -329,10 +329,45 @@ int launch_fcsm_pruned(dl_context* ctx, const FcsmPair* pairs_dev, int count, in
 int launch_fcsm(dl_context* ctx, const FcsmPair* pairs_dev, int count, int max_points, long long max_threads,
                 unsigned long long* best_dev, FcsmPick* picks_dev, float* all_scores_dev);
 void compute_odds_table(float probability, uint16_t* table32768);
-int grid_insert_device(dl_context* ctx, dl_grid* g, const Vec3f& origin, const float* d_returns, int n, int num_free,
-                       const uint16_t* d_hit_table, const uint16_t* d_miss_table, int32_t* d_bbox, uint32_t* d_update_list);
-int launch_transform_filter(dl_context* ctx, const float* in, int n, const Rigidf& to_submap, const Vec3f& origin_submap,
-                            float max_range, float* all, float* near, int32_t* near_count, int32_t* tile_counts);
+// One RangeDataInserter3D::Insert per job (dl_inserter.cu). Device pointers; the grid's frame.
+struct InsertJob {
+  dl_grid* grid;
+  Vec3f origin;
+  const float* returns;     // n x 3
+  int n;                    // the point count, or an upper bound of it when n_dev is given
+  const int32_t* n_dev;     // optional: the point count on the device (a transform filter's near count)
+  uint32_t* update_list;    // n * (1 + num_free) entries
+};
+// Runs the jobs' Inserts with one set of host steps for all of them (one bounding-box read-back, then one counter read-back
+// per pool level); jobs of one grid run in list order, one after another. d_bbox: 8 ints per job; d_args:
+// insert_args_bytes(count) bytes.
+size_t insert_args_bytes(int jobs);
+int insert_range_data_device(dl_context* ctx, const InsertJob* jobs, int count, int num_free, const uint16_t* d_hit_table,
+                             const uint16_t* d_miss_table, int32_t* d_bbox, void* d_args);
+// TransformRangeData into the submap frame + FilterRangeDataByMaxRange (submap_3d.cc:42-51, :264-279) of one cloud per job:
+// `all` receives every point, `near` (count in *near_count) those within max_range of the origin, in input order.
+struct TransformJob {
+  const float* in;
+  int n;
+  Rigidf to_submap;
+  Vec3f origin_submap;
+  float max_range;
+  float *all, *near;
+  int32_t* near_count;
+  int32_t* tile_counts;     // ceil(n / 256)
+};
+size_t transform_jobs_bytes(int jobs);
+int launch_transform_filter(dl_context* ctx, const TransformJob* jobs, int count, void* d_jobs);
+// range_data_in_local and the histogram's gravity-aligned returns of one scan per job.
+struct LocalFrameJob {
+  const float *returns, *misses;   // tracking frame
+  int num_returns, num_misses;
+  Rigidf pose;                     // opt_pose.cast<float>()
+  Rigidf gravity_alignment;        // its rotation only
+  float *returns_local, *misses_local, *returns_aligned;
+};
+size_t local_frame_jobs_bytes(int jobs);
+int launch_local_frame(dl_context* ctx, const LocalFrameJob* jobs, int count, void* d_jobs);
 // dl_window.cu
 int launch_window_optimize(dl_context* ctx, int count, const dl_nav_state* states_i, const double* prior_information,
                            const dl_preintegration* preint, const double* matched_pose, const dl_nav_state* initial_j,
@@ -350,6 +385,12 @@ struct HistogramScratch {  // device scratch of one rotational histogram of n po
 void carve_rotational_histogram(Arena& a, int64_t n, HistogramScratch* s);
 int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, const float* d_points, int64_t n, int size,
                                 float* d_histogram, int32_t** d_error_out);
+// `count` clouds in one launch, one CTA each: cloud k = n[k] (>= 1) points at d_points[k], scratch s[k] carved for at least n[k],
+// histogram k (`size` floats) at d_histograms[k]. d_args: rotational_histograms_args_bytes(count) bytes of device memory. The error
+// flag of cloud k is s[k].counters[1].
+size_t rotational_histograms_args_bytes(int count);
+int launch_rotational_histograms(dl_context* ctx, const HistogramScratch* s, const float* const* d_points, const int64_t* n,
+                                 int count, int size, float* const* d_histograms, void* d_args);
 // dl_comm.cu: staging buffers of the constraint exchange and the timed all-gather
 int comm_reserve(dl_comm* c, size_t bytes_per_rank);
 void* comm_send_buffer(dl_comm* c);

@@ -36,7 +36,7 @@ struct ImuPrepareArgs {
   int count;
   const dl_preintegration* preint;
   const dl_nav_state* states_i;  // local frame
-  Rigidd to_submap;              // inverse of the submap's local pose
+  const Rigidd* to_submap;       // per scan: inverse of its matching submap's local pose
   double gravity[3];
   double imu_weight;
   ScanConstants* scans;
@@ -61,6 +61,7 @@ struct FrontendArgs {
   const int32_t* counts;
   const ScanConstants* scans;
   const float* origins;
+  const int32_t* origin_base;    // per scan: its first origin in `origins` (a row's origin index counts from there)
   int64_t cap;           // per-scan capacity of every per-point array below
   int64_t tcap1, tcap2;  // table capacities (powers of two)
   float first_resolution, second_resolution, min_range, max_range;
@@ -93,7 +94,7 @@ struct ResultArgs {
   const float* rtcsm_scores;       // optional
   const NlsOutput* nls;
   const FusedOutput* fused;        // optional: the fused (IMU) solve's output replaces `nls`
-  Rigidd submap;
+  const Rigidd* submap;            // per scan: the local pose of its matching submap
   const int32_t* error_flag;       // per scan: set by the fused front half when a voxel key could not be packed
   const int32_t* imu_ok;           // optional: 0 = the scan's IMU factor could not be formed (result ok = -2)
   dl_nav_state* states_out;        // optional (fused solve): the estimated state in the LOCAL frame
@@ -102,7 +103,7 @@ struct ResultArgs {
 
 int launch_gather_rows(dl_context* ctx, const float* in, int64_t cap_in, int pairs_per_cloud, const int32_t* keep,
                        const int32_t* keep_counts, int64_t cap_out, float* out, int pairs);
-int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd& submap_inverse,
+int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd* submap_inverse,
                         double* initial_pose, double* target_translation);
 int launch_finalize_results(dl_context* ctx, const ResultArgs& a);
 

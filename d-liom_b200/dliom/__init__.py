@@ -34,6 +34,7 @@ EXPORTS = [
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
     "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
+    "dl_ltb_add_range_data_batch",
     "dl_pose_graph_3d_create", "dl_pose_graph_3d_destroy", "dl_pose_graph_3d_add_node", "dl_pose_graph_3d_freeze_trajectory",
     "dl_pose_graph_3d_run_final_optimization", "dl_pose_graph_3d_poses", "dl_pose_graph_3d_local_to_global",
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
@@ -308,6 +309,11 @@ class MatchingResult(C.Structure):   # dl_matching_result
                 ("num_insertion_submaps", C.c_int32), ("insertion_submap_index", C.c_int32 * 2), ("reserved", C.c_int32)]
 
 
+class LtbBatchItem(C.Structure):   # dl_ltb_batch_item
+    _fields_ = [("builder", C.c_void_p), ("time", C.c_double), ("rows", C.c_void_p), ("n", C.c_int64), ("row_floats", C.c_int32),
+                ("num_origins", C.c_int32), ("origins", C.c_void_p)]
+
+
 class PoseGraph3DOptions(C.Structure):   # dl_pose_graph_3d_options
     _fields_ = [("optimize_every_n_nodes", C.c_int32), ("every_nodes_to_find_constraint", C.c_int32),
                 ("matcher_translation_weight", C.c_double), ("matcher_rotation_weight", C.c_double),
@@ -514,6 +520,7 @@ def lib():
     L.dl_ltb_num_submaps.argtypes = [vp]
     L.dl_ltb_get_submap.argtypes = [vp, C.c_int32, ip(vp), ip(vp), f64p, ip(C.c_int32), ip(C.c_int32)]
     L.dl_ltb_get_state.argtypes = [vp, ip(NavState), ip(C.c_int32)]
+    L.dl_ltb_add_range_data_batch.argtypes = [C.c_int32, ip(LtbBatchItem), ip(MatchingResult)]
     L.dl_frontend_submit.argtypes = [vp, ip(FrontendOptions), C.c_int32, ip(vp), i64p, f32p, C.c_int32, f64p, f64p, f64p, vp, vp]
     L.dl_frontend_collect.argtypes = [vp, C.c_int32, ip(ScanResult)]
     L.dl_frontend_match_batch_dev.argtypes = [vp, ip(FrontendOptions), C.c_int32, vp, C.c_int64, i64p, f32p, C.c_int32,
@@ -1108,6 +1115,39 @@ class LocalTrajectoryBuilder:
         init = C.c_int32(0)
         self.ctx.check(self.ctx.L.dl_ltb_get_state(self.h, C.byref(s), C.byref(init)))
         return s.to16(), bool(init.value)
+
+
+def _ltb_rows(scan, origins):
+    """-> (contiguous rows, row_floats, contiguous (k, 3) float32 origins) of one scan for the dl_ltb_* calls: an (n, 4) float
+    array of x y z t rows with one origin, or 32-byte RangeMeasurement records (x y z t + u64 origin index) with k origins."""
+    rows = np.ascontiguousarray(scan)
+    if rows.dtype.itemsize == 32 and rows.dtype.names:
+        row_floats = 8
+    else:
+        rows = np.ascontiguousarray(rows, np.float32).reshape(-1, 4)
+        row_floats = 4
+    origins = np.ascontiguousarray(np.zeros((1, 3)) if origins is None else origins, np.float32).reshape(-1, 3)
+    return rows, row_floats, origins
+
+
+def add_range_data_batch(builders, times, scans, origins=None):
+    """dl_ltb_add_range_data_batch: one add_range_data (x y z t rows) or add_synchronized_range_data (RangeMeasurement records)
+    per builder, all in one call; -> one MatchingResult per builder, byte for byte the single calls' results. origins: None (one
+    origin at zero each) or one origin array per builder. The builders must share a context and have equal options."""
+    builders = list(builders)
+    if not (len(times) == len(scans) == len(builders)) or (origins is not None and len(origins) != len(builders)):
+        raise ValueError("one time, scan (and origin array) per builder")
+    keep = []   # the arrays must outlive the call
+    items = (LtbBatchItem * max(len(builders), 1))()
+    for k, b in enumerate(builders):
+        rows, row_floats, o = _ltb_rows(scans[k], None if origins is None else origins[k])
+        keep += [rows, o]
+        items[k] = LtbBatchItem(b.h, float(times[k]), rows.ctypes.data, len(rows), row_floats, len(o), o.ctypes.data)
+    results = (MatchingResult * max(len(builders), 1))()
+    if builders:
+        ctx = builders[0].ctx
+        ctx.check(ctx.L.dl_ltb_add_range_data_batch(len(builders), items, results))
+    return [results[k] for k in range(len(builders))]
 
 
 class PoseGraph3D:

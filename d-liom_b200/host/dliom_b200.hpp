@@ -527,6 +527,56 @@ class LocalTrajectoryBuilder3D {  // local_trajectory_builder_3d.h:81-113
     dl_matching_result r{};
     ctx_->check(dl_ltb_add_synchronized_range_data(builder_, data.time, data.ranges.data(), (int64_t)data.ranges.size(), 8,
                                                    data.origins[0].data(), (int32_t)data.origins.size(), &r));
+    return Result(r);
+  }
+  // One AddRangeData of the batch form below.
+  struct RangeDataItem {
+    LocalTrajectoryBuilder3D* builder;
+    std::string sensor_id;
+    const sensor::TimedPointCloudData* data;
+  };
+  // AddRangeData of several trajectories in one dl_ltb_add_range_data_batch call: result k is what items[k].builder->AddRangeData(
+  // items[k].sensor_id, *items[k].data) would have returned, and every builder ends in the same state. Each builder's own
+  // RangeDataSynchronizer runs first; builders whose data is only queued return nullptr and take no part. The builders must share
+  // one Context and appear once each (Error(DL_ERR_ARG) before any synchroniser runs), and have equal options (Error(DL_ERR_ARG)
+  // from dl_ltb_add_range_data_batch, after the synchronisers have run but before any builder is touched).
+  static std::vector<std::unique_ptr<MatchingResult>> AddRangeData(const std::vector<RangeDataItem>& items) {
+    std::vector<std::unique_ptr<MatchingResult>> out(items.size());
+    if (items.empty()) return out;
+    Context* ctx = items[0].builder->ctx_;
+    for (size_t k = 0; k < items.size(); ++k) {
+      if (items[k].builder->ctx_ != ctx) throw Error(DL_ERR_ARG, "the builders of a batch must share one Context");
+      for (size_t j = 0; j < k; ++j)
+        if (items[j].builder == items[k].builder) throw Error(DL_ERR_ARG, "a builder appears twice in one batch");
+    }
+    std::vector<sensor::TimedPointCloudOriginData> data;
+    std::vector<size_t> which;
+    data.reserve(items.size());
+    for (size_t k = 0; k < items.size(); ++k) {
+      LocalTrajectoryBuilder3D* b = items[k].builder;
+      data.push_back(b->synchronizer_.AddRangeData(items[k].sensor_id, *items[k].data, b->options_.enable_manual_deskew));
+      if (!data.back().ranges.empty()) which.push_back(k);
+    }
+    std::vector<dl_ltb_batch_item> batch;
+    for (size_t k : which) {
+      const sensor::TimedPointCloudOriginData& d = data[k];
+      batch.push_back(dl_ltb_batch_item{items[k].builder->builder_, d.time, d.ranges.data(), (int64_t)d.ranges.size(), 8,
+                                        (int32_t)d.origins.size(), d.origins[0].data()});
+    }
+    std::vector<dl_matching_result> r(batch.size());
+    ctx->check(dl_ltb_add_range_data_batch((int32_t)batch.size(), batch.data(), r.data()));
+    for (size_t j = 0; j < which.size(); ++j) out[which[j]] = items[which[j]].builder->Result(r[j]);
+    return out;
+  }
+  void AddOdometryData(double /*time*/, const Rigid3d& /*pose*/) {}  // the fork never constructs its extrapolator (LTB:574-582)
+  // Replaces the NDT initialisation when the caller knows the state (tests, re-localisation).
+  void SetInitialState(const dl_nav_state& state) { ctx_->check(dl_ltb_set_initial_state(builder_, &state)); }
+  int num_submaps() const { return dl_ltb_num_submaps(builder_); }
+  dl_local_trajectory_builder* get() const { return builder_; }
+
+ private:
+  // MatchingResult / InsertionResult of a dl_matching_result this builder has just produced (LTB:559-622).
+  std::unique_ptr<MatchingResult> Result(const dl_matching_result& r) const {
     if (!r.has_result) return nullptr;
     std::unique_ptr<MatchingResult> out(new MatchingResult);
     out->time = r.time;
@@ -550,13 +600,6 @@ class LocalTrajectoryBuilder3D {  // local_trajectory_builder_3d.h:81-113
     }
     return out;
   }
-  void AddOdometryData(double /*time*/, const Rigid3d& /*pose*/) {}  // the fork never constructs its extrapolator (LTB:574-582)
-  // Replaces the NDT initialisation when the caller knows the state (tests, re-localisation).
-  void SetInitialState(const dl_nav_state& state) { ctx_->check(dl_ltb_set_initial_state(builder_, &state)); }
-  int num_submaps() const { return dl_ltb_num_submaps(builder_); }
-  dl_local_trajectory_builder* get() const { return builder_; }
-
- private:
   PointCloud Cloud(int which) const {
     int64_t n = 0;
     ctx_->check(dl_ltb_get_cloud(builder_, which, nullptr, 0, &n));

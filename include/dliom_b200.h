@@ -773,6 +773,32 @@ int dl_ltb_add_range_data(dl_local_trajectory_builder* builder, double time, con
  * sorted by time, and one origin per sensor. */
 int dl_ltb_add_synchronized_range_data(dl_local_trajectory_builder* builder, double time, const void* rows, int64_t n,
                                        int32_t row_floats, const float* origins, int32_t num_origins, dl_matching_result* result);
+/* Several trajectories in one call: item k is the arguments of one dl_ltb_add_synchronized_range_data on items[k].builder, and
+ * afterwards results[k] and everything observable on that builder (state, clouds, histogram, submaps and their grids' cells)
+ * are byte for byte what that single call would have produced. Members are independent, so their order does not matter. The
+ * scans of all members run through one front-end batch, each against its own builder's matching submap, and the insertions
+ * into all their active submaps share one set of host steps: the host waits a fixed number of times per call whatever
+ * `count` is, except once for each grid whose pools or top level have to grow and for each submap a member hands over to.
+ * A member to which one of the single call's early returns applies (initialising, n == 0, no IMU since the last scan) takes
+ * no part in the device work. Rules, checked before any builder is touched (DL_ERR_ARG, every builder unchanged):
+ * one dl_context for all builders, no builder twice, and equal dl_ltb_options on every builder, field by field (the batched
+ * front end takes one options block and one IMU noise). count == 0 is a no-op. Each builder's host state is committed
+ * only after the call's device work has succeeded. A call that fails after its device work has begun (a CUDA error, out of
+ * memory, a cloud the rotational histogram refuses — the latter is detected before any grid changes) commits no builder's host
+ * state, but after a failure inside the insertion the grids of the members' active submaps may already hold their scans: do not
+ * feed such a builder the same scan again. dl_ltb_add_range_data and dl_ltb_add_synchronized_range_data are the batch of one.
+ * The correlative pre-match (use_online_correlative_scan_matching) is not part of this path: dl_ltb_create refuses it, as the
+ * fused solve does, and the front end refuses a correlative batch whose scans match different grids. */
+typedef struct dl_ltb_batch_item {
+  dl_local_trajectory_builder* builder;
+  double time;
+  const void* rows;        /* as dl_ltb_add_synchronized_range_data: row_floats 4 (x y z t, one origin) or 8 (RangeMeasurement) */
+  int64_t n;
+  int32_t row_floats;
+  int32_t num_origins;
+  const float* origins;    /* num_origins x 3 */
+} dl_ltb_batch_item;
+int dl_ltb_add_range_data_batch(int32_t count, const dl_ltb_batch_item* items, dl_matching_result* results);
 /* Clouds of the last scan that produced a result. which: 0 returns / 1 misses of range_data_in_local, 2 / 3 the high / low
  * resolution point clouds in the tracking frame (TrajectoryNode::Data). Pass out = NULL to query *num_points. */
 int dl_ltb_get_cloud(const dl_local_trajectory_builder* builder, int32_t which, float* out, int64_t capacity_points, int64_t* num_points);
