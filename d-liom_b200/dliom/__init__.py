@@ -40,6 +40,7 @@ EXPORTS = [
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
     "dl_map_writer_create", "dl_map_writer_destroy", "dl_map_writer_add_trajectory", "dl_map_writer_process",
     "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels",
+    "dl_submap_textures", "dl_submap_projections",
 ]
 
 
@@ -384,6 +385,20 @@ PG3D_INTRA_SUBMAP, PG3D_INTER_SUBMAP = 0, 1
 PG3D_NODE_POSES, PG3D_SUBMAP_POSES, PG3D_OPTIMIZATION_NODES, PG3D_OPTIMIZATION_SUBMAPS = 0, 1, 2, 3
 
 
+class SubmapImageQuery(C.Structure):   # dl_submap_image_query
+    _fields_ = [("grid", C.c_void_p), ("pose", C.c_double * 7)]
+
+
+class SubmapTexture(C.Structure):   # dl_submap_texture
+    _fields_ = [("resolution", C.c_float), ("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32),
+                ("slice_pose", C.c_double * 7), ("offset", C.c_int64)]
+
+
+class SubmapProjection(C.Structure):   # dl_submap_projection
+    _fields_ = [("resolution", C.c_float), ("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32),
+                ("ox", C.c_double), ("oy", C.c_double), ("offset", C.c_int64)]
+
+
 def spa_constraints(constraints):
     """(submap, node, zbar7, translation_weight, rotation_weight) tuples -> a dl_spa_constraint array (numpy-packed: graphs of
     tens of thousands of constraints)."""
@@ -508,6 +523,9 @@ def lib():
     L.dl_map_writer_flush.argtypes = [vp, ip(C.c_int32)]
     L.dl_map_writer_voxels.argtypes = [vp, C.c_int64, vp, vp, vp, ip(C.c_int64)]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
+    L.dl_submap_textures.argtypes = [vp, C.c_int32, ip(SubmapImageQuery), ip(SubmapTexture), C.c_int64, vp, ip(C.c_int64)]
+    L.dl_submap_projections.argtypes = [vp, C.c_int32, ip(SubmapImageQuery), ip(SubmapProjection), C.c_int64, vp,
+                                        ip(C.c_int64)]
     L.dl_ltb_create.argtypes = [vp, ip(LtbOptions), ip(vp)]
     L.dl_ltb_destroy.argtypes = [vp]
     L.dl_ltb_destroy.restype = None
@@ -664,6 +682,34 @@ class Context:
         out = np.zeros(max(int(size), 0), np.float32)
         self.check(self.L.dl_rotational_histogram(self.h, points, len(points), int(size), out))
         return out
+
+    # ---- submap images
+    def _submap_images(self, fn, record, queries):
+        n = len(queries)
+        qs = (SubmapImageQuery * max(n, 1))()
+        for k, (grid, pose) in enumerate(queries):
+            qs[k].grid = grid.h if isinstance(grid, Grid) else grid
+            qs[k].pose[:] = [float(v) for v in np.asarray(pose, np.float64).reshape(7)]
+        recs = (record * max(n, 1))()
+        size = C.c_int64(0)
+        self.check(fn(self.h, n, qs, recs, 0, None, C.byref(size)))
+        out = np.zeros(max(size.value, 1), np.uint8)
+        self.check(fn(self.h, n, qs, recs, size.value, out.ctypes.data_as(C.c_void_p), C.byref(size)))
+        return [recs[k] for k in range(n)], out
+
+    def submap_textures(self, queries):
+        """Submap3D::ToResponseProto's textures of (grid, global pose 7-vector) queries, one call: a dict per query with
+        resolution, width, height, slice_pose and cells, a (height, width, 2) uint8 array of (value, alpha) (not gzipped)."""
+        recs, out = self._submap_images(self.L.dl_submap_textures, SubmapTexture, queries)
+        return [{"resolution": r.resolution, "width": r.width, "height": r.height, "slice_pose": np.array(r.slice_pose[:]),
+                 "cells": out[r.offset:r.offset + 2 * r.width * r.height].reshape(r.height, r.width, 2).copy()} for r in recs]
+
+    def project_submaps(self, queries):
+        """ProjectToCvMat of (grid, pose 7-vector) queries, one call: a dict per query with resolution, width, height, ox, oy and
+        pixels, a (height, width) uint8 array (row y - min_y, column x - min_x)."""
+        recs, out = self._submap_images(self.L.dl_submap_projections, SubmapProjection, queries)
+        return [{"resolution": r.resolution, "width": r.width, "height": r.height, "ox": r.ox, "oy": r.oy,
+                 "pixels": out[r.offset:r.offset + r.width * r.height].reshape(r.height, r.width).copy()} for r in recs]
 
     # ---- matchers
     def rtcsm_match(self, grid, points, initial_pose, linear_window, angular_window, w_t, w_r, want_scores=False):

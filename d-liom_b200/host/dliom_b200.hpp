@@ -613,6 +613,95 @@ class LocalTrajectoryBuilder3D {  // local_trajectory_builder_3d.h:81-113
   dl_local_trajectory_builder* builder_ = nullptr;
 };
 
+// A builder's submap (dl_ltb_get_submap): its device grids stay owned by the builder.
+struct Submap3D {
+  const dl_grid* high_resolution_grid = nullptr;
+  const dl_grid* low_resolution_grid = nullptr;
+  Rigid3d local_pose;
+  int num_range_data = 0;
+  bool finished = false;
+};
+inline Submap3D GetSubmap(Context* ctx, const LocalTrajectoryBuilder3D& builder, int index) {
+  dl_grid *hi = nullptr, *lo = nullptr;
+  double pose[7];
+  int32_t n = 0, finished = 0;
+  ctx->check(dl_ltb_get_submap(builder.get(), index, &hi, &lo, pose, &n, &finished));
+  return {hi, lo, Rigid3d::from7(pose), n, finished != 0};
+}
+
+// proto::SubmapQuery::Response (Submap3D::ToResponseProto, submap_3d.cc:253-262): textures[0] high, [1] low resolution. The
+// cells are raw interleaved (value, alpha) bytes; common::FastGzipString them when filling the proto.
+struct SubmapTexture {
+  std::vector<uint8_t> cells;
+  int width = 0, height = 0;
+  double resolution = 0;
+  Rigid3d slice_pose;
+};
+struct SubmapQueryResponse {
+  int submap_version = 0;
+  std::vector<SubmapTexture> textures;
+};
+// Every (submap, global submap pose) in one device call (dl_submap_textures).
+inline std::vector<SubmapQueryResponse> ToResponseProto(Context* ctx, const std::vector<std::pair<Submap3D, Rigid3d>>& submaps) {
+  std::vector<dl_submap_image_query> queries;
+  for (const auto& s : submaps)
+    for (const dl_grid* g : {s.first.high_resolution_grid, s.first.low_resolution_grid}) {
+      dl_submap_image_query q{g, {}};
+      s.second.to7(q.pose);
+      queries.push_back(q);
+    }
+  std::vector<dl_submap_texture> textures(queries.size());
+  int64_t bytes = 0;
+  ctx->check(dl_submap_textures(ctx->get(), (int32_t)queries.size(), queries.data(), textures.data(), 0, nullptr, &bytes));
+  std::vector<uint8_t> cells((size_t)bytes);
+  ctx->check(dl_submap_textures(ctx->get(), (int32_t)queries.size(), queries.data(), textures.data(), bytes, cells.data(), &bytes));
+  std::vector<SubmapQueryResponse> out(submaps.size());
+  for (size_t k = 0; k < submaps.size(); ++k) {
+    out[k].submap_version = submaps[k].first.num_range_data;
+    for (size_t j = 2 * k; j < 2 * k + 2; ++j) {
+      const dl_submap_texture& t = textures[j];
+      const uint8_t* first = cells.data() + t.offset;
+      out[k].textures.push_back({std::vector<uint8_t>(first, first + 2 * (size_t)t.width * t.height), t.width, t.height,
+                                 t.resolution, Rigid3d::from7(t.slice_pose)});
+    }
+  }
+  return out;
+}
+inline SubmapQueryResponse ToResponseProto(Context* ctx, const Submap3D& submap, const Rigid3d& global_submap_pose) {
+  return ToResponseProto(ctx, {{submap, global_submap_pose}})[0];
+}
+
+// The fork's ProjectToCvMat (submap_3d.cc:381-464): the 8-bit image of cv::Mat(height, width, CV_8UC1), row-major, before its
+// cv::threshold / cv::erode. Pass the submap's local pose, as ConstraintBuilder3D::ExtractFeaturesForSubmap does.
+struct SubmapProjection {
+  int width = 0, height = 0;
+  std::vector<uint8_t> pixels;
+  double ox = 0, oy = 0, resolution = 0;
+};
+// Every (grid, pose) in one device call (dl_submap_projections).
+inline std::vector<SubmapProjection> ProjectToCvMat(Context* ctx, const std::vector<std::pair<const dl_grid*, Rigid3d>>& grids) {
+  std::vector<dl_submap_image_query> queries;
+  for (const auto& g : grids) {
+    dl_submap_image_query q{g.first, {}};
+    g.second.to7(q.pose);
+    queries.push_back(q);
+  }
+  std::vector<dl_submap_projection> records(queries.size());
+  int64_t bytes = 0;
+  ctx->check(dl_submap_projections(ctx->get(), (int32_t)queries.size(), queries.data(), records.data(), 0, nullptr, &bytes));
+  std::vector<uint8_t> pixels((size_t)bytes);
+  ctx->check(dl_submap_projections(ctx->get(), (int32_t)queries.size(), queries.data(), records.data(), bytes, pixels.data(), &bytes));
+  std::vector<SubmapProjection> out;
+  for (const dl_submap_projection& r : records) {
+    const uint8_t* first = pixels.data() + r.offset;
+    out.push_back({r.width, r.height, std::vector<uint8_t>(first, first + (size_t)r.width * r.height), r.ox, r.oy, r.resolution});
+  }
+  return out;
+}
+inline SubmapProjection ProjectToCvMat(Context* ctx, const dl_grid* hybrid_grid, const Rigid3d& transform) {
+  return ProjectToCvMat(ctx, {{hybrid_grid, transform}})[0];
+}
+
 }  // namespace mapping
 
 namespace optimization {

@@ -809,6 +809,58 @@ int dl_ltb_get_submap(dl_local_trajectory_builder* builder, int32_t index, dl_gr
                       dl_grid** low_resolution_grid, double* local_pose, int32_t* num_range_data, int32_t* finished);
 int dl_ltb_get_state(const dl_local_trajectory_builder* builder, dl_nav_state* state, int32_t* initialized);
 
+/* ---- submap images: Submap3D::ToResponseProto's X-ray textures (C/mapping/3d/submap_3d.cc:53-178, :253-262) and the fork's
+ *      ProjectToCvMat (:381-464), the 8-bit image the loop detector's feature stage reads, computed on the device from the grids
+ *      in place, for any number of (grid, pose) queries per call (each its own grid and pose; a grid may appear many times).
+ *      Both walk every cell HybridGrid::Iterator yields (value != 0), skip it when ValueToProbability(value) < 0.501f, move the
+ *      cell centre index * resolution by a Rigid3f and take lround(c * (1.f / resolution)) per axis (ExtractVoxelData,
+ *      :82-112). Per pixel (x, y): the cell count, min / max z, the largest probability (from 0.5f) and the float sum of the
+ *      probabilities in iterator order — lexicographic in (z/64, y/64, x/64, z/8 % 8, y/8 % 8, x/8 % 8, z % 8, y % 8, x % 8),
+ *      as dl_grid_export_cells emits the cells.
+ *   Textures (AddToTextureProto): the transform is pose.cast<float>() (the submap's global pose); width = max_y - min_y + 1,
+ *      height = max_x - min_x + 1; cell (x, y) goes to pixel (max_x - x) * width + (max_y - y), two bytes (value, alpha) each,
+ *      ComputePixelValues (:116-146) exactly, ProbabilityToLogOddsInteger's logf included (a host-built table of its steps).
+ *      slice_pose = pose.inverse() * Translation(max_x * resolution, max_y * resolution, pose z), the two products in float.
+ *   Projections (ProjectToCvMat): the transform is the pose's rotation without its yaw: Embed3D(Rigid2d::Rotation(-GetYaw))
+ *      .cast<float>() * Rigid3d::Rotation(q).cast<float>() (:385-390, built on the host); width = max_x - min_x + 1, height =
+ *      max_y - min_y + 1, row-major, pixel (y - min_y) * width + (x - min_x) = (uint8) lround((sum - 0.1f) * (255.f / 0.8f)) for
+ *      every pixel: an empty pixel is 224, and the int -> uchar conversion wraps dense columns, as the reference does.
+ *      ox = min_x * (double)resolution, oy = min_y * (double)resolution. Pass the submap's LOCAL pose for the loop detector
+ *      (pose_graph_3d.cc:1078-1096 via ConstraintBuilder3D::ExtractFeaturesForSubmap).
+ * Deliberate differences:
+ *   - the texture's cells are returned raw, not through common::FastGzipString: compress them if a SubmapQuery needs it;
+ *   - the fork's cv::threshold / cv::erode after ProjectToCvMat are not applied (OpenCV, host, cheap on the 8-bit image);
+ *   - a grid without an obstructed cell (empty included) gives width = height = 0 and slice_pose / ox / oy all 0, where the
+ *     reference's bounding box is INT_MIN - INT_MAX (undefined behaviour).
+ * Pass cells / pixels = NULL to fill the per-query records and *num_bytes only (the images' bytes at each record's `offset`);
+ * otherwise `capacity` must be at least *num_bytes. Grids are read only; they must be synced (dl_grid_sync after
+ * dl_grid_set_cells) and not modified during the call. The host waits three times per call (two when sizing), whatever the
+ * query count, plus once when the context's device scratch has to grow; the grids' pool sizes are read with one 8-byte copy per
+ * query, the kernel launches do not depend on the query count. The size query runs the whole cell pass once, so sizing and then
+ * filling reads every cell three times. Fails with DL_ERR_ARG while a dl_frontend_submit batch is in flight on `ctx`. */
+typedef struct dl_submap_image_query {
+  const dl_grid* grid;
+  double pose[7];
+} dl_submap_image_query;
+typedef struct dl_submap_texture {
+  float resolution;
+  int32_t width, height;
+  int32_t reserved;
+  double slice_pose[7];
+  int64_t offset;  /* first byte of the 2 * width * height interleaved (value, alpha) bytes */
+} dl_submap_texture;
+typedef struct dl_submap_projection {
+  float resolution;
+  int32_t width, height;
+  int32_t reserved;
+  double ox, oy;
+  int64_t offset;  /* first byte of the width * height pixels */
+} dl_submap_projection;
+int dl_submap_textures(dl_context* ctx, int32_t count, const dl_submap_image_query* queries, dl_submap_texture* textures,
+                       int64_t capacity, uint8_t* cells, int64_t* num_bytes);
+int dl_submap_projections(dl_context* ctx, int32_t count, const dl_submap_image_query* queries, dl_submap_projection* projections,
+                          int64_t capacity, uint8_t* pixels, int64_t* num_bytes);
+
 /* ---- map writer: the assets writer's point pipeline for a finished run (cartographer_ros/assets_writer.cc:120-160 HandleMessage,
  *      the fork's config dlio/config/assets_writer_tongji.lua) on the device. Per message (one io::PointsBatch):
  *        point time = stamp + FromSeconds(t) (ticks of 100 ns, truncated toward zero), a point with !Has(time) is dropped
