@@ -1,4 +1,4 @@
-// Fused scan front half of the batched front end and of dl_ingest_scan: 4 launches per sub-batch (5 with per-run deskew poses),
+// Fused scan front half of the batched front end and of dl_ingest_scan: 3 launches per sub-batch (4 with per-run deskew poses),
 // then the small glue kernels of the batched front end (cloud gathers, pose algebra, result records).
 //
 //   A  fe_first_filter_tile     first voxel filter (LTB:393-395), per tile of 2048 rows: the tile's lowest row per voxel in
@@ -9,10 +9,10 @@
 //   B  fe_ingest_tile           per tile, the first-filter survivors in index order (from the bitmap): deskew + transform +
 //                               range gate (LTB:426-472) and the SECOND voxel filter (LTB:479-484) keyed on the local-frame
 //                               voxel, again per tile in shared memory first — no compaction in between: ids stay the original
-//                               input indices, which preserves "first point in input order wins" for free.
-//   C1 fe_mark_bits             the second filter's winners (the index field of every non-empty slot) become bits of two
-//                               per-scan bitmaps (returns, misses): 4 KiB per 32 k points, L2-resident.
-//   C2 fe_emit_tracking         ordered compaction straight from the bitmaps (popcount prefix; no per-point class map, no
+//                               input indices, which preserves "first point in input order wins" for free. Its survivors end as
+//                               two per-scan bitmaps (returns, misses; 4 KiB per 32 k points), with kernel A's set-then-clear
+//                               protocol.
+//   C  fe_emit_tracking         ordered compaction straight from the bitmaps (popcount prefix; no per-point class map, no
 //                               tile counts), fused with the scan's current pose (hits_poses.back(), LTB:476) and the frame
 //                               change back to tracking (TransformRangeData with current_pose^-1, LTB:485-487); output rows
 //                               are written coalesced.
@@ -27,7 +27,7 @@
 // result is invalid (ok = -1); the generic dl_voxel_filter has no such limit. Returns and misses share the table (bit 63).
 //
 // Algorithmic traffic per raw point: A reads 12/16 B; B reads 1 bit (+12/16 B row + 4 B time, writes
-// 16 B record + 8 B slot for survivors); C1 reads 8 B per slot; C2 reads 16 B and writes 12 B per output point.
+// 16 B record + 8 B slot for survivors) and writes 2 bits; C reads 16 B and writes 12 B per output point.
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
 
@@ -270,16 +270,20 @@ __device__ __forceinline__ Int3 unpack_cell(const KeyLayout& k, unsigned long lo
           (int)(((uint32_t)key & m) + k.bz)};
 }
 // Second-filter insert of a slot word into a table of mask + 1 slots (the tile's in shared memory or the scan's): CAS claim; among
-// equal keys (same class and voxel) atomicMin keeps the lowest index.
-__device__ __forceinline__ void slot_insert(unsigned long long* slots, uint32_t mask, int idx_bits, const Int3& c,
-                                            unsigned long long slot) {
+// equal keys (same class and voxel) atomicMin keeps the lowest index. Returns the word that lost the meeting, the newcomer's or
+// the one it replaced, or kEmpty64 when the insert claimed an empty slot.
+__device__ __forceinline__ unsigned long long slot_insert(unsigned long long* slots, uint32_t mask, int idx_bits, const Int3& c,
+                                                          unsigned long long slot) {
   uint32_t hh = (hash_cell(c) ^ ((slot >> 63) ? 0x9e3779b9u : 0u)) & mask;
   for (;;) {
     const unsigned long long prev = atomicCAS(slots + hh, kEmpty64, slot);
-    if (prev == kEmpty64) break;
+    if (prev == kEmpty64) return kEmpty64;
     if ((prev >> idx_bits) == (slot >> idx_bits)) {
-      if (slot < prev) atomicMin(slots + hh, slot);
-      break;
+      if (slot < prev) {
+        const unsigned long long q = atomicMin(slots + hh, slot);  // the owner only ever decreases
+        if (q > slot) return q;
+      }
+      return slot;
     }
     hh = (hh + 1) & mask;
   }
@@ -342,11 +346,26 @@ __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, con
 // records written at nearly consecutive addresses, and the run search of 12-byte rows covers only the tile's few dozen runs
 // (L1-resident starts and poses). The survivors' second-filter words meet in the tile table; only the tile winners go on to the
 // scan's table, with the same protocol.
+//
+// The second filter's survivors end as the scan's two bitmaps (returns, misses) with the first filter's set-then-clear protocol:
+// the CTA stores its tile's words of both bitmaps, one bit per tile winner, before any of its winners is inserted (fence, then
+// barrier), and every insert that meets an equal key clears the bit of the one that lost, the newcomer or the word it replaced.
+// A key with k tile winners sees k - 1 meetings, each with a different loser, so exactly the lowest index keeps its bit. A clear
+// only ever follows the store of its word (the loser was seen in the scan's table), so the stores need no cleared bitmap, and
+// every word the compaction reads is stored by the tile that owns it. This replaces a kernel that streamed the whole scan table
+// (8 bytes per slot, 2^17 slots per 64-beam scan) to find the winners.
 constexpr int kWordsPerLane = kTile / 32 / 32;  // bitmap words of a tile per lane of warp 0
+constexpr int kTileWords = kTile / 32;
+
+__device__ __forceinline__ uint32_t* scan_bits(const FrontendArgs& a, int b, int miss) {
+  return a.bits + ((size_t)b * 2 + miss) * a.bit_words;
+}
+
 template <bool kRunPose>
 __global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_tile(FrontendArgs a) {  // <= 40 / 64 registers
   __shared__ unsigned long long tile_slots[kTileSlots];
   __shared__ uint16_t list[kTile];
+  __shared__ uint32_t tile_bits[2][kTileWords];  // the tile winners: returns, misses
   __shared__ int listed, num_winners, run_lo, run_hi;
   const int b = a.first_scan + blockIdx.y;
   const int n = a.counts[b];
@@ -357,6 +376,7 @@ __global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_tile(Front
   const float* rows = a.ranges + (size_t)b * a.in_cap * rf;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int k = threadIdx.x; k < kTileSlots; k += kBlock) tile_slots[k] = kEmpty64;
+  if (threadIdx.x < 2 * kTileWords) tile_bits[threadIdx.x / kTileWords][threadIdx.x % kTileWords] = 0u;
   if (warp == 0) {
     const uint32_t* bits = a.first_bits + (size_t)b * a.bit_words + (base >> 5);
     const int words = (rows_here + 31) >> 5;
@@ -394,11 +414,29 @@ __global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_tile(Front
     returns += ingest_survivor<kRunPose>(a, b, rows, rf, sc, no_deskew, kl, run_lo, run_hi, tile_slots, base + list[k]) == 1;
   __syncthreads();
   const int won = list_occupied(tile_slots, kEmpty64, list, &num_winners);
+  const unsigned long long idx_mask = (1ull << kl.idx_bits) - 1;
+  for (int k = threadIdx.x; k < won; k += kBlock) {
+    const unsigned long long s = tile_slots[list[k]];
+    const uint32_t w = (uint32_t)(s & idx_mask) - (uint32_t)base;
+    atomicOr(&tile_bits[s >> 63][w >> 5], 1u << (w & 31));
+  }
+  __syncthreads();
+  if (threadIdx.x < 2 * kTileWords) {
+    const int miss = threadIdx.x / kTileWords, q = threadIdx.x % kTileWords;
+    if (q < ((rows_here + 31) >> 5)) __stcg(scan_bits(a, b, miss) + (base >> 5) + q, tile_bits[miss][q]);
+    __threadfence();
+  }
+  __syncthreads();
   unsigned long long* slots = a.slots2 + (size_t)b * a.tcap2;
   const uint32_t mask2 = (uint32_t)a.tcap2 - 1;
   for (int k = threadIdx.x; k < won; k += kBlock) {
     const unsigned long long s = tile_slots[list[k]];
-    slot_insert(slots, mask2, kl.idx_bits, unpack_cell(kl, s), s);
+    const unsigned long long loser = slot_insert(slots, mask2, kl.idx_bits, unpack_cell(kl, s), s);
+    if (loser != kEmpty64) {
+      const uint32_t i = (uint32_t)(loser & idx_mask);
+      __threadfence();  // the loser's bit was stored before its insert that this thread has seen
+      atomicAnd(scan_bits(a, b, (int)(loser >> 63)) + (i >> 5), ~(1u << (i & 31)));
+    }
   }
   returns = warp_sum(returns);
   if (lane == 0 && returns) atomicAdd(a.n_returns_local + b, returns);
@@ -408,26 +446,7 @@ __global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_tile(Front
 constexpr int kEmitBlock = 512, kEmitWarps = kEmitBlock / 32;
 constexpr int kChunkPoints = 1024;  // one warp handles 32 bitmap words = 1024 consecutive point indices at a time
 
-__device__ __forceinline__ uint32_t* scan_bits(const FrontendArgs& a, int b, int miss) {
-  return a.bits + ((size_t)b * 2 + miss) * a.bit_words;
-}
-
-// C1: the second filter's survivors are the index fields of its non-empty slots: stream the table once, set one bit each.
-__global__ void __launch_bounds__(kBlock) fe_mark_bits(FrontendArgs a) {
-  const int b = a.first_scan + blockIdx.y;
-  if (a.counts[b] == 0) return;
-  const unsigned long long* slots = a.slots2 + (size_t)b * a.tcap2;
-  const unsigned long long idx_mask = (1ull << a.idx_bits) - 1;
-  for (int h = blockIdx.x * kBlock + threadIdx.x; h < (int)a.tcap2; h += gridDim.x * kBlock) {
-    const unsigned long long s = __ldcg(slots + h);
-    if (s != kEmpty64) {
-      const uint32_t i = (uint32_t)(s & idx_mask);
-      atomicOr(scan_bits(a, b, (int)(s >> 63)) + (i >> 5), 1u << (i & 31));  // result unused: a reduction, no round trip
-    }
-  }
-}
-
-// C2: gridDim.x CTAs per scan. Every CTA counts the bits of all 1024-point chunks of its scan (32 words per chunk: a few KiB from
+// C: gridDim.x CTAs per scan. Every CTA counts the bits of all 1024-point chunks of its scan (32 words per chunk: a few KiB from
 // L2), scans the chunk counts, and emits the chunks it owns: the warp expands a chunk's set bits into a shared-memory list and
 // then walks the list with all lanes, so that output rows k, k+1, ... are written by neighbouring lanes (coalesced 12-byte rows).
 __global__ void __launch_bounds__(kEmitBlock) fe_emit_tracking(FrontendArgs a, int max_chunks) {
@@ -620,10 +639,13 @@ __global__ void finalize_results_kernel(ResultArgs a) {
 
 }  // namespace
 
+// The scan tables live in global memory and are cleared here on every call. Keeping them in a thread-block cluster's distributed
+// shared memory instead (one 8-CTA cluster per scan, no memsets) gave the same outputs but made the step 1.45x slower: one CTA
+// per SM cannot hide the tiles' latency as four per-tile CTAs do (DESIGN §6).
 int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch) {
   DL_CUDA(ctx, cudaMemsetAsync(a.table1, 0xFF, (size_t)batch * a.tcap1 * sizeof(uint32_t), ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(a.slots2, 0xFF, (size_t)batch * a.tcap2 * sizeof(unsigned long long), ctx->stream));
-  DL_CUDA(ctx, cudaMemsetAsync(a.bits, 0, (size_t)batch * 2 * a.bit_words * sizeof(uint32_t), ctx->stream));
+  // a.bits needs no clearing: fe_ingest_tile stores every word of it that fe_emit_tracking reads
   DL_CUDA(ctx, cudaMemsetAsync(a.first_bits, 0, (size_t)batch * a.bit_words * sizeof(uint32_t), ctx->stream));
   fe_reset_counters<<<(batch + 127) / 128, 128, 0, ctx->stream>>>(a, batch);
   DL_LAUNCH_CHECK(ctx, "fe_reset_counters");
@@ -643,7 +665,6 @@ int launch_fe_first_filter(dl_context* ctx, FrontendArgs a, int first_scan, int 
 int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
   if (batch <= 0) return DL_OK;
   a.first_scan = first_scan;
-  const int tiles = (int)std::min<int64_t>((a.cap + kBlock - 1) / kBlock, 128);
   const int row_tiles = (int)((a.cap + kTile - 1) / kTile);
   if (a.run_pose && a.max_runs > 0) {
     fe_run_poses<<<dim3((a.max_runs + 127) / 128, batch), 128, 0, ctx->stream>>>(a);
@@ -653,8 +674,6 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
     fe_ingest_tile<false><<<dim3(row_tiles, batch), kBlock, 0, ctx->stream>>>(a);
   }
   DL_LAUNCH_CHECK(ctx, "fe_ingest_tile");
-  fe_mark_bits<<<dim3(tiles, batch), kBlock, 0, ctx->stream>>>(a);
-  DL_LAUNCH_CHECK(ctx, "fe_mark_bits");
   const int max_chunks = (int)((a.bit_words + 31) / 32);
   const size_t smem = (size_t)2 * (max_chunks + 1) * sizeof(int) + (size_t)kEmitWarps * kChunkPoints * sizeof(uint16_t);
   if (smem > 200 * 1024) return ctx->fail(DL_ERR_ARG, "scan too large for the front end's compaction (> 20 M points)");
