@@ -272,7 +272,17 @@ void dl_grid_destroy(dl_grid* g) {
 }
 
 float dl_grid_resolution(const dl_grid* g) { return g ? g->resolution : 0.f; }
-int64_t dl_grid_num_bricks(const dl_grid* g) { return g ? (int64_t)(g->bricks.size() / 512) : 0; }
+// After a device insert the host mirror is behind until the next download: the device's brick counter is then the count in use.
+int64_t dl_grid_num_bricks(const dl_grid* g) {
+  if (!g) return 0;
+  if (!g->mirror_stale) return (int64_t)(g->bricks.size() / 512);
+  int32_t used = 0;
+  if (cudaSetDevice(g->ctx->device) != cudaSuccess ||
+      cudaMemcpyAsync(&used, g->d_counters + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, g->ctx->stream) != cudaSuccess ||
+      cudaStreamSynchronize(g->ctx->stream) != cudaSuccess)
+    return -1;
+  return used;
+}
 
 static int grid_download(dl_grid* g);
 static inline size_t top_flat(int x, int y, int z, int bits) { return ((((size_t)z << bits) + y) << bits) + x; }

@@ -49,6 +49,15 @@ __device__ __forceinline__ Int3 hit_cell(const InsertArgs& a, int i) {
   return cell_index(Vec3f{a.returns[3 * i], a.returns[3 * i + 1], a.returns[3 * i + 2]}, a.resolution);
 }
 
+// CHECK_LT(num_samples, 1 << 15) of range_data_inserter_3d.cc:37: the host refuses a job with a longer ray before any grid
+// changes, so that delta * position below stays inside int.
+constexpr int kMaxSamples = 1 << 15;
+
+// Sample `position` of a ray from cell o with delta d: origin_cell + delta * position / num_samples, C++ truncating division.
+__device__ __forceinline__ Int3 miss_cell(const Int3& o, const Int3& d, int num_samples, int position) {
+  return Int3{o.x + d.x * position / num_samples, o.y + d.y * position / num_samples, o.z + d.z * position / num_samples};
+}
+
 // Visits the hit cell (phase 0) or the miss cells (phase 1) of ray i, exactly as range_data_inserter_3d.cc:33-50.
 template <typename F>
 __device__ __forceinline__ void for_each_cell(const InsertArgs& a, int i, int phase, F f) {
@@ -60,20 +69,31 @@ __device__ __forceinline__ void for_each_cell(const InsertArgs& a, int i, int ph
   const Int3 o = cell_index(a.origin, a.resolution);
   const Int3 d{h.x - o.x, h.y - o.y, h.z - o.z};
   const int num_samples = max(abs(d.x), max(abs(d.y), abs(d.z)));
-  for (int position = max(0, num_samples - a.num_free); position < num_samples; ++position)
-    f(Int3{o.x + d.x * position / num_samples, o.y + d.y * position / num_samples, o.z + d.z * position / num_samples});
+  for (int position = max(0, num_samples - a.num_free); position < num_samples; ++position) f(miss_cell(o, d, num_samples, position));
 }
 
+// The box of every cell the job touches, in bbox[0..5], and its longest ray (num_samples) in bbox[7]. A ray touches its hit
+// cell and samples max(0, num_samples - num_free) .. num_samples - 1; sample cells move monotonically along each axis, so the
+// first of them and the hit cell bound them all (the origin cell only counts when it is a sample).
 __global__ void ins_bbox_kernel(const InsertArgs* __restrict__ jobs) {
   const InsertArgs a = jobs[blockIdx.y];
   const int n = a.n_dev ? *a.n_dev : a.n;
+  const Int3 o = cell_index(a.origin, a.resolution);
   int lo[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, hi[3] = {-0x7fffffff, -0x7fffffff, -0x7fffffff};
+  int longest = 0;
   auto add = [&](const Int3& c) {
     lo[0] = min(lo[0], c.x); lo[1] = min(lo[1], c.y); lo[2] = min(lo[2], c.z);
     hi[0] = max(hi[0], c.x); hi[1] = max(hi[1], c.y); hi[2] = max(hi[2], c.z);
   };
-  for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) add(hit_cell(a, i));
-  if (blockIdx.x == 0 && threadIdx.x == 0 && a.num_free > 0 && n > 0) add(cell_index(a.origin, a.resolution));
+  for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) {
+    const Int3 h = hit_cell(a, i);
+    add(h);
+    const Int3 d{h.x - o.x, h.y - o.y, h.z - o.z};
+    const int num_samples = max(abs(d.x), max(abs(d.y), abs(d.z)));
+    longest = max(longest, num_samples);
+    if (a.num_free > 0 && num_samples > 0 && num_samples < kMaxSamples)  // a longer ray fails the call: its box is not needed
+      add(miss_cell(o, d, num_samples, max(0, num_samples - a.num_free)));
+  }
   for (int k = 0; k < 3; ++k) {
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) {
@@ -81,11 +101,15 @@ __global__ void ins_bbox_kernel(const InsertArgs* __restrict__ jobs) {
       hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], d));
     }
   }
-  if ((threadIdx.x & 31) == 0)
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) longest = max(longest, __shfl_xor_sync(0xffffffffu, longest, d));
+  if ((threadIdx.x & 31) == 0) {
     for (int k = 0; k < 3; ++k) {
       atomicMin(a.bbox + k, lo[k]);
       atomicMax(a.bbox + 3 + k, hi[k]);
     }
+    atomicMax(a.bbox + 7, longest);
+  }
 }
 
 // Grow(): every axis doubles, the old content moves to the centre (hybrid_grid.h:389-407).
@@ -279,69 +303,18 @@ int reserve_pools(dl_context* ctx, std::vector<InsertArgs>& args, const std::vec
   return DL_OK;
 }
 
-// One round of insert_range_data_device: every grid at most once.
-int insert_round(dl_context* ctx, const InsertJob* const* jobs, int count, int num_free, const uint16_t* d_hit_table,
-                 const uint16_t* d_miss_table, int32_t* d_bbox, InsertArgs* d_args) {
-  std::vector<InsertArgs> args;
-  std::vector<dl_grid*> grids;
-  int widest = 0;
-  for (int j = 0; j < count; ++j) {
-    const InsertJob& job = *jobs[j];
-    if (job.n <= 0) continue;
-    DL_TRY_STATUS(grid_ensure_device_state(job.grid));
-    InsertArgs a{};
-    a.returns = job.returns; a.n = job.n; a.n_dev = job.n_dev; a.origin = job.origin; a.resolution = job.grid->resolution;
-    a.num_free = num_free; a.bbox = d_bbox + 8 * args.size(); a.update_list = job.update_list;
-    a.hit_table = d_hit_table; a.miss_table = d_miss_table;
-    args.push_back(a);
-    grids.push_back(job.grid);
-    widest = std::max(widest, job.n);
-  }
-  if (args.empty()) return DL_OK;
-  const unsigned J = (unsigned)args.size();
+// One round of insert_range_data_device: every grid at most once. bbox holds each job's box (8 ints, ins_bbox_kernel).
+int insert_round(dl_context* ctx, std::vector<InsertArgs> args, const std::vector<dl_grid*>& grids, const std::vector<int32_t>& bbox,
+                 int num_free, int32_t* d_bbox, InsertArgs* d_args) {
+  const unsigned K = (unsigned)args.size();
   auto upload = [&]() -> int {
-    DL_CUDA(ctx, cudaMemcpyAsync(d_args, args.data(), sizeof(InsertArgs) * J, cudaMemcpyHostToDevice, ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(d_args, args.data(), sizeof(InsertArgs) * K, cudaMemcpyHostToDevice, ctx->stream));
     return DL_OK;
   };
-  // 1. which cells will be touched -> does a top level have to grow (CHECK_LE(new_bits, 8))? One pass over every job.
-  std::vector<int32_t> bbox(8 * J);
-  for (unsigned j = 0; j < J; ++j) {
-    const int32_t init[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff, -0x7fffffff, -0x7fffffff, 0, 0};
-    std::memcpy(bbox.data() + 8 * j, init, sizeof(init));
-  }
-  DL_CUDA(ctx, cudaMemcpyAsync(d_bbox, bbox.data(), sizeof(int32_t) * 8 * J, cudaMemcpyHostToDevice, ctx->stream));
-  DL_TRY_STATUS(upload());
-  ins_bbox_kernel<<<dim3(std::min(kNumSMs * 8, (widest + kBlock - 1) / kBlock), J), kBlock, 0, ctx->stream>>>(d_args);
-  DL_LAUNCH_CHECK(ctx, "ins_bbox_kernel");
-  // the device counts ride in the unused seventh int of each job's box: one read-back, one host wait for every job
-  for (unsigned j = 0; j < J; ++j)
-    if (args[j].n_dev)
-      DL_CUDA(ctx, cudaMemcpyAsync(d_bbox + 8 * j + 6, args[j].n_dev, sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
-  DL_CUDA(ctx, cudaMemcpyAsync(bbox.data(), d_bbox, sizeof(int32_t) * 8 * J, cudaMemcpyDeviceToHost, ctx->stream));
-  DL_CUDA(ctx, ctx->wait_stream());
-  // jobs whose count on the device is zero drop out; the others carry their exact count from here on
-  {
-    std::vector<InsertArgs> kept_args;
-    std::vector<dl_grid*> kept_grids;
-    std::vector<int32_t> kept_bbox;
-    for (unsigned j = 0; j < J; ++j) {
-      if (args[j].n_dev) args[j].n = bbox[8 * j + 6];
-      args[j].n_dev = nullptr;
-      if (args[j].n <= 0) continue;
-      kept_args.push_back(args[j]);
-      kept_grids.push_back(grids[j]);
-      kept_bbox.insert(kept_bbox.end(), bbox.begin() + 8 * j, bbox.begin() + 8 * j + 8);
-    }
-    args.swap(kept_args);
-    grids.swap(kept_grids);
-    bbox.swap(kept_bbox);
-  }
-  if (args.empty()) return DL_OK;
-  const unsigned K = (unsigned)args.size();
-  widest = 0;
+  int widest = 0;
   for (const InsertArgs& a : args) widest = std::max(widest, a.n);
   const dim3 blocks(std::min(kNumSMs * 8, (widest + kBlock - 1) / kBlock), K);
-  // 2. top-level growth of whichever grids need it
+  // 1. top-level growth of whichever grids need it
   for (unsigned j = 0; j < K; ++j) {
     dl_grid* g = grids[j];
     const int32_t* bb = bbox.data() + 8 * j;
@@ -369,7 +342,7 @@ int insert_round(dl_context* ctx, const InsertJob* const* jobs, int count, int n
       g->version++;
     }
   }
-  // 3. structure growth with exact reservations: mark + count the missing nodes, grow the node pools by those counts, assign;
+  // 2. structure growth with exact reservations: mark + count the missing nodes, grow the node pools by those counts, assign;
   //    then the same for the bricks (whose node entries now exist)
   for (unsigned j = 0; j < K; ++j) {
     dl_grid* g = grids[j];
@@ -421,21 +394,82 @@ int insert_round(dl_context* ctx, const InsertJob* const* jobs, int count, int n
 }  // namespace
 
 int insert_range_data_device(dl_context* ctx, const InsertJob* jobs, int count, int num_free, const uint16_t* d_hit_table,
-                             const uint16_t* d_miss_table, int32_t* d_bbox, void* d_args) {
-  // A grid named by several jobs takes them in list order, one round each: within a round every grid appears once.
-  std::vector<const InsertJob*> pending;
-  for (int j = 0; j < count; ++j) pending.push_back(jobs + j);
-  while (!pending.empty()) {
-    std::vector<const InsertJob*> round, later;
-    for (const InsertJob* job : pending) {
-      bool taken = false;
-      for (const InsertJob* r : round) taken = taken || r->grid == job->grid;
-      bool waits = false;  // keep list order per grid: a job never overtakes an earlier one of its grid
-      for (const InsertJob* l : later) waits = waits || l->grid == job->grid;
-      (taken || waits ? later : round).push_back(job);
+                             const uint16_t* d_miss_table, int32_t* d_bbox, void* d_args_raw) {
+  InsertArgs* d_args = (InsertArgs*)d_args_raw;
+  std::vector<InsertArgs> args;
+  std::vector<dl_grid*> grids;
+  int widest = 0;
+  for (int j = 0; j < count; ++j) {
+    const InsertJob& job = jobs[j];
+    if (job.n <= 0) continue;
+    DL_TRY_STATUS(grid_ensure_device_state(job.grid));
+    InsertArgs a{};
+    a.returns = job.returns; a.n = job.n; a.n_dev = job.n_dev; a.origin = job.origin; a.resolution = job.grid->resolution;
+    a.num_free = num_free; a.bbox = d_bbox + 8 * args.size(); a.update_list = job.update_list;
+    a.hit_table = d_hit_table; a.miss_table = d_miss_table;
+    args.push_back(a);
+    grids.push_back(job.grid);
+    widest = std::max(widest, job.n);
+  }
+  if (args.empty()) return DL_OK;
+  const unsigned J = (unsigned)args.size();
+  // 1. which cells will be touched, and how long the rays are: one pass over every job of every round, one read-back
+  std::vector<int32_t> bbox(8 * J);
+  for (unsigned j = 0; j < J; ++j) {
+    const int32_t init[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, -0x7fffffff, -0x7fffffff, -0x7fffffff, 0, 0};
+    std::memcpy(bbox.data() + 8 * j, init, sizeof(init));
+  }
+  DL_CUDA(ctx, cudaMemcpyAsync(d_bbox, bbox.data(), sizeof(int32_t) * 8 * J, cudaMemcpyHostToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(d_args, args.data(), sizeof(InsertArgs) * J, cudaMemcpyHostToDevice, ctx->stream));
+  ins_bbox_kernel<<<dim3(std::min(kNumSMs * 8, (widest + kBlock - 1) / kBlock), J), kBlock, 0, ctx->stream>>>(d_args);
+  DL_LAUNCH_CHECK(ctx, "ins_bbox_kernel");
+  // the device counts ride in the unused seventh int of each job's box: one read-back, one host wait for every job
+  for (unsigned j = 0; j < J; ++j)
+    if (args[j].n_dev)
+      DL_CUDA(ctx, cudaMemcpyAsync(d_bbox + 8 * j + 6, args[j].n_dev, sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(bbox.data(), d_bbox, sizeof(int32_t) * 8 * J, cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  // jobs whose count on the device is zero drop out; the others carry their exact count from here on
+  {
+    std::vector<InsertArgs> kept_args;
+    std::vector<dl_grid*> kept_grids;
+    std::vector<int32_t> kept_bbox;
+    for (unsigned j = 0; j < J; ++j) {
+      if (args[j].n_dev) args[j].n = bbox[8 * j + 6];
+      args[j].n_dev = nullptr;
+      if (args[j].n <= 0) continue;
+      kept_args.push_back(args[j]);
+      kept_grids.push_back(grids[j]);
+      kept_bbox.insert(kept_bbox.end(), bbox.begin() + 8 * j, bbox.begin() + 8 * j + 8);
     }
-    DL_TRY_STATUS(insert_round(ctx, round.data(), (int)round.size(), num_free, d_hit_table, d_miss_table, d_bbox, (InsertArgs*)d_args));
-    pending.swap(later);
+    args.swap(kept_args);
+    grids.swap(kept_grids);
+    bbox.swap(kept_bbox);
+  }
+  // 2. the checks that refuse a call run before any grid changes: CHECK_LT(num_samples, 1 << 15) (range_data_inserter_3d.cc:37)
+  //    and CHECK_LE(new_bits, 8) (hybrid_grid.h:391), i.e. every touched cell within +-8192 cells
+  const unsigned K = (unsigned)args.size();
+  for (unsigned j = 0; j < K; ++j) {
+    const int32_t* bb = bbox.data() + 8 * j;
+    if (bb[7] >= kMaxSamples) return ctx->fail(DL_ERR_ARG, "a ray crosses 2^15 cells or more (CHECK_LT(num_samples, 1 << 15))");
+    for (int k = 0; k < 3; ++k)
+      if (bb[k] < -8192 || bb[3 + k] >= 8192) return ctx->fail(DL_ERR_GRID_RANGE, "cell index outside +-8192 cells");
+  }
+  // 3. a grid named by several jobs takes them in list order, one round each: a round takes the first pending job of every grid
+  std::vector<char> done(K, 0);
+  for (unsigned left = K; left > 0;) {
+    std::vector<InsertArgs> round_args;
+    std::vector<dl_grid*> round_grids;
+    std::vector<int32_t> round_bbox;
+    for (unsigned j = 0; j < K; ++j) {
+      if (done[j] || std::find(round_grids.begin(), round_grids.end(), grids[j]) != round_grids.end()) continue;
+      done[j] = 1;
+      --left;
+      round_args.push_back(args[j]);
+      round_grids.push_back(grids[j]);
+      round_bbox.insert(round_bbox.end(), bbox.begin() + 8 * j, bbox.begin() + 8 * j + 8);
+    }
+    DL_TRY_STATUS(insert_round(ctx, round_args, round_grids, round_bbox, num_free, d_bbox, d_args));
   }
   return DL_OK;
 }

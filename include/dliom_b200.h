@@ -75,6 +75,9 @@ int dl_grid_set_cells(dl_grid* grid, int64_t n, const int32_t* x, const int32_t*
                       const uint16_t* value);
 int dl_grid_sync(dl_grid* grid);
 float dl_grid_resolution(const dl_grid* grid);
+/* The 8^3 bricks in use: every brick the reference's HybridGrid would have allocated, set or inserted. After a device insert
+ * this is the device's count (one 4-byte read-back; -1 on a CUDA error), until an export or dl_grid_set_cells brings the
+ * host mirror up to date. */
 int64_t dl_grid_num_bricks(const dl_grid* grid);
 /* HybridGrid::value() for n cell indices (xyz interleaved), evaluated ON THE DEVICE (hybrid_grid.h:263-281). */
 int dl_grid_lookup(dl_context* ctx, const dl_grid* grid, int64_t n, const int32_t* xyz, uint16_t* value_out);
@@ -92,7 +95,14 @@ typedef struct dl_range_data_inserter_options {
   int32_t num_free_space_voxels;
   int32_t reserved;
 } dl_range_data_inserter_options;
-/* returns: n x 3 floats already in the grid's (submap) frame; origin: 3 floats in the same frame. */
+/* returns: n x 3 floats already in the grid's (submap) frame; origin: 3 floats in the same frame.
+ * The grid grows to hold exactly the cells the Insert touches: each hit cell and the last num_free_space_voxels samples of
+ * its ray. The origin cell counts only when it is one of those samples, so the origin may lie beyond +-8192 cells.
+ * Refused before any grid changes (the reference CHECK-fails instead):
+ *   DL_ERR_ARG         a ray of 2^15 cells or more (num_samples, the largest |hit cell - origin cell| component), whatever
+ *                      num_free_space_voxels is (CHECK_LT(num_samples, 1 << 15), range_data_inserter_3d.cc:37);
+ *   DL_ERR_GRID_RANGE  a touched cell outside +-8192 cells.
+ * The submap and batched forms check every job of the call before the first one writes. */
 int dl_grid_insert_range_data(dl_context* ctx, dl_grid* grid, const dl_range_data_inserter_options* options,
                               const float* origin, const float* returns, int64_t n);
 /* Submap3D::InsertRangeData: range data in the LOCAL frame is moved into the submap frame (local_pose^-1, float), the

@@ -107,6 +107,8 @@ def lib():
     L.orc_grid_num_cells.argtypes = [C.c_void_p]
     L.orc_grid_export.argtypes = [C.c_void_p, i32p, i32p, i32p, u16p]
     L.orc_grid_insert_range_data.argtypes = [C.c_void_p, f32p, f32p, C.c_int64, C.c_double, C.c_double, C.c_int]
+    L.orc_submap_insert_range_data.argtypes = [C.c_void_p, C.c_void_p, f64p, f32p, f32p, C.c_int64, C.c_double, C.c_double,
+                                               C.c_int, C.c_int]
     L.orc_interpolate.restype = C.c_double
     L.orc_interpolate.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_double]
     L.orc_interpolate_grad.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_double, f64p]
@@ -242,8 +244,9 @@ class Grid:
 
     def insert_range_data(self, origin, returns, hit=0.55, miss=0.49, num_free=2):
         returns = np.ascontiguousarray(returns, np.float32).reshape(-1, 3)
-        self.L.orc_grid_insert_range_data(self.h, np.ascontiguousarray(origin, np.float32), returns, len(returns),
-                                          hit, miss, num_free)
+        if self.L.orc_grid_insert_range_data(self.h, np.ascontiguousarray(origin, np.float32), returns, len(returns),
+                                             hit, miss, num_free):
+            raise RuntimeError("grid growth limit (CHECK_LE(new_bits, 8))")
 
     def interpolate(self, x, y, z):
         return self.L.orc_interpolate(self.h, x, y, z)
@@ -252,6 +255,23 @@ class Grid:
         out = np.zeros(4)
         self.L.orc_interpolate_grad(self.h, x, y, z, out)
         return out
+
+
+def submap_insert_range_data(hi, lo, local_pose, origin, returns, high_resolution_max_range=20, hit=0.55, miss=0.49,
+                             num_free=2):
+    """Submap3D::InsertRangeData of local-frame range data into the grids (hi may be lo) of the submap at local_pose."""
+    returns = np.ascontiguousarray(returns, np.float32).reshape(-1, 3)
+    if lib().orc_submap_insert_range_data(hi.h, lo.h, np.ascontiguousarray(local_pose, np.float64),
+                                          np.ascontiguousarray(origin, np.float32), returns, len(returns), hit, miss, num_free,
+                                          int(high_resolution_max_range)):
+        raise RuntimeError("grid growth limit (CHECK_LE(new_bits, 8))")
+
+
+def lookup_table_to_apply_odds(odds):
+    """ComputeLookupTableToApplyOdds(odds) (float odds): uint16[32768], update marker included."""
+    out = np.zeros(32768, np.uint16)
+    lib().orc_lookup_table_to_apply_odds(np.float32(odds), out)
+    return out
 
 
 def voxel_filter(points, resolution):

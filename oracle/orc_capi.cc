@@ -88,10 +88,23 @@ void orc_grid_export(void* g, int* xs, int* ys, int* zs, uint16_t* vs) {
   int64_t n = 0;
   ((HybridGrid*)g)->ForEachCell([&](const I3& i, uint16_t v) { xs[n] = i.x; ys[n] = i.y; zs[n] = i.z; vs[n] = v; ++n; });
 }
-void orc_grid_insert_range_data(void* g, const float* origin, const float* returns, int64_t n, double hit_p,
-                                double miss_p, int num_free) {
+// Returns 1 past the growth limit (the grid then holds whatever the Insert wrote before it stopped).
+int orc_grid_insert_range_data(void* g, const float* origin, const float* returns, int64_t n, double hit_p,
+                               double miss_p, int num_free) {
   RangeDataInserter ins(RangeDataInserterOptions{hit_p, miss_p, num_free});
-  ins.Insert({origin[0], origin[1], origin[2]}, returns, n, (HybridGrid*)g);
+  try { ins.Insert({origin[0], origin[1], origin[2]}, returns, n, (HybridGrid*)g); } catch (...) { return 1; }
+  return 0;
+}
+// Submap::InsertRangeData into two caller-owned grids (which may be one grid): the transform and range filter of
+// Submap3D::InsertRangeData, then Insert(near) into hi and Insert(all) into lo. Returns 1 past the growth limit.
+int orc_submap_insert_range_data(void* hi, void* lo, const double* local_pose, const float* origin, const float* returns,
+                                 int64_t n, double hit_p, double miss_p, int num_free, int high_resolution_max_range) {
+  RangeDataInserter ins(RangeDataInserterOptions{hit_p, miss_p, num_free});
+  try {
+    submap_insert_range_data(pose_in(local_pose), {origin[0], origin[1], origin[2]}, returns, n, ins,
+                             high_resolution_max_range, (HybridGrid*)hi, (HybridGrid*)lo);
+  } catch (...) { return 1; }
+  return 0;
 }
 
 // ---- interpolation

@@ -60,26 +60,32 @@ class RangeDataInserter {
   std::vector<uint16_t> hit_table_, miss_table_;
 };
 
+// Submap3D::InsertRangeData of range data in the local frame (origin + returns; misses are not inserted by the reference)
+// into the grids of the submap at local_pose.
+inline void submap_insert_range_data(const Rigid3d& local_pose, const V3f& origin, const float* returns, int64_t n,
+                                     const RangeDataInserter& ins, int high_resolution_max_range, HybridGrid* hi, HybridGrid* lo) {
+  const Rigid3f to_submap = cast_f(inverse(local_pose));
+  const V3f o = apply(to_submap, origin);
+  std::vector<float> all, near;
+  all.reserve(3 * n);
+  for (int64_t i = 0; i < n; ++i) {
+    const V3f p = apply(to_submap, V3f{returns[3 * i], returns[3 * i + 1], returns[3 * i + 2]});
+    all.insert(all.end(), {p.x, p.y, p.z});
+    if (norm(p - o) <= (float)high_resolution_max_range) near.insert(near.end(), {p.x, p.y, p.z});
+  }
+  ins.Insert(o, near.data(), (int64_t)near.size() / 3, hi);
+  ins.Insert(o, all.data(), n, lo);
+}
+
 struct Submap {
   Rigid3d local_pose;
   HybridGrid hi, lo;
   int num_range_data = 0;
   Submap(float hi_res, float lo_res, const Rigid3d& pose) : local_pose(pose), hi(hi_res), lo(lo_res) {}
 
-  // range data given in the local frame (origin + returns); misses are not inserted by the reference.
   void InsertRangeData(const V3f& origin, const float* returns, int64_t n, const RangeDataInserter& ins,
                        int high_resolution_max_range) {
-    const Rigid3f to_submap = cast_f(inverse(local_pose));
-    const V3f o = apply(to_submap, origin);
-    std::vector<float> all, near;
-    all.reserve(3 * n);
-    for (int64_t i = 0; i < n; ++i) {
-      const V3f p = apply(to_submap, V3f{returns[3 * i], returns[3 * i + 1], returns[3 * i + 2]});
-      all.insert(all.end(), {p.x, p.y, p.z});
-      if (norm(p - o) <= (float)high_resolution_max_range) near.insert(near.end(), {p.x, p.y, p.z});
-    }
-    ins.Insert(o, near.data(), (int64_t)near.size() / 3, &hi);
-    ins.Insert(o, all.data(), n, &lo);
+    submap_insert_range_data(local_pose, origin, returns, n, ins, high_resolution_max_range, &hi, &lo);
     ++num_range_data;
   }
 };
