@@ -1745,14 +1745,16 @@ struct FrontendBuffers {
   int batch = 0;
   int64_t cap = 0, tcap = 0;
   int32_t *counts0, *n1, *n_ret, *n2, *n3, *countsA, *npassesA, *croppedA;
-  uint32_t *table, *tableA, *scratchA;
+  uint32_t *tableA, *scratchA;
   int32_t* keepA;
   float *returns_tracking, *misses_tracking, *clouds, *current_pose, *origins, *passesA, *rtcsm_scores;
   // fused front half
-  int64_t tcap2 = 0, bit_words = 0;
-  unsigned long long* slots2;  // second filter: one 64-bit word per slot (dl_frontend.cu)
+  int64_t bit_words = 0;
   uint32_t* bits;              // two survivor bitmaps per scan
   uint32_t* first_bits;        // the first filter's survivor bitmap per scan
+  int4* stage;                 // tile winners by hash partition, and their ends per tile (dl_frontend.cu)
+  int32_t *part_ends, *spill_used;
+  uint32_t* spill;
   int32_t *last_index, *error_flag;
   float* local4;
   uint8_t* adaptive_first;  // scratch of the adaptive filters' grid-wide first pass (dl_voxel.cu)
@@ -1777,7 +1779,6 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   f->counts0 = a.take<int32_t>(B); f->n1 = a.take<int32_t>(B); f->n_ret = a.take<int32_t>(B);
   f->n2 = a.take<int32_t>(B); f->n3 = a.take<int32_t>(B); f->countsA = a.take<int32_t>(2 * B); f->npassesA = a.take<int32_t>(2 * B);
   f->croppedA = a.take<int32_t>(2 * B);
-  f->table = a.take<uint32_t>(B * f->tcap);
   f->tableA = a.take<uint32_t>(B * 2 * f->tcap); f->scratchA = a.take<uint32_t>(B * 4 * C);
   f->keepA = a.take<int32_t>(B * 2 * C);
   f->returns_tracking = a.take<float>(B * C * 3); f->misses_tracking = a.take<float>(B * C * 3);
@@ -1787,10 +1788,14 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   f->submap = a.take<Rigidd>(B); f->submap_inverse = a.take<Rigidd>(B); f->origin_base = a.take<int32_t>(B);
   f->initial_pose = a.take<double>(B * 7); f->target = a.take<double>(B * 3);
   f->problems = a.take<NlsProblem>(B); f->nls_out = a.take<NlsOutput>(B);
-  f->tcap2 = next_pow2(cap);
   f->bit_words = (int64_t)((C + 31) / 32);
-  f->slots2 = a.take<unsigned long long>(B * f->tcap2); f->bits = a.take<uint32_t>(B * 2 * f->bit_words);
+  f->bits = a.take<uint32_t>(B * 2 * f->bit_words);
   f->first_bits = a.take<uint32_t>(B * f->bit_words);
+  const size_t tiles = (C + kFrontendTile - 1) / kFrontendTile;
+  f->stage = a.take<int4>(B * tiles * kFrontendTile);
+  f->part_ends = a.take<int32_t>(B * tiles * kFrontendParts);
+  f->spill = a.take<uint32_t>(B * 2 * tiles * kFrontendTile);
+  f->spill_used = a.take<int32_t>(2 * B);
   f->last_index = a.take<int32_t>(B); f->error_flag = a.take<int32_t>(B);
   f->local4 = a.take<float>(B * C * 4);
   f->adaptive_first = a.take<uint8_t>(adaptive_first_pass_bytes(2 * batch, cap) + 16 * 1024);
@@ -1811,15 +1816,12 @@ FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuff
                                 int64_t in_cap, int row_floats) {
   FrontendArgs fa{};
   fa.ranges = d_ranges; fa.in_cap = in_cap; fa.row_floats = row_floats; fa.counts = f.counts0; fa.scans = f.scans;
-  fa.origins = f.origins; fa.origin_base = f.origin_base; fa.cap = f.cap; fa.tcap2 = f.tcap2;
-  // First-filter table of the fused path: the next power of two above 2 * cap (load ~0.18 on real sweeps). A compact table of
-  // 1.25 slots per point (the kernels take any size: slot = hash * tcap >> 32) saves a third of the memset and of the ingest
-  // kernel's table stream but costs the first filter more in collisions than it saves.
-  fa.tcap1 = f.tcap;
+  fa.origins = f.origins; fa.origin_base = f.origin_base; fa.cap = f.cap;
   fa.first_resolution = 0.5f * o.voxel_filter_size;  // LTB:394
   fa.second_resolution = o.voxel_filter_size;        // LTB:479-484
   fa.min_range = o.min_range; fa.max_range = o.max_range; fa.scan_period = o.scan_period;
-  fa.table1 = f.table; fa.first_bits = f.first_bits; fa.slots2 = f.slots2; fa.bits = f.bits; fa.bit_words = f.bit_words;
+  fa.first_bits = f.first_bits; fa.bits = f.bits; fa.bit_words = f.bit_words;
+  fa.stage = f.stage; fa.part_ends = f.part_ends; fa.spill = f.spill; fa.spill_used = f.spill_used;
   fa.idx_bits = 1;
   while (((int64_t)1 << fa.idx_bits) < f.cap) ++fa.idx_bits;      // point indices are < cap
   fa.axis_bits = std::min(21, (63 - fa.idx_bits) / 3);             // 15 bits per axis up to 256 k points per scan

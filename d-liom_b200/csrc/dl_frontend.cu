@@ -1,33 +1,38 @@
-// Fused scan front half of the batched front end and of dl_ingest_scan: 3 launches per sub-batch (4 with per-run deskew poses),
+// Fused scan front half of the batched front end and of dl_ingest_scan: 5 launches per sub-batch (6 with per-run deskew poses),
 // then the small glue kernels of the batched front end (cloud gathers, pose algebra, result records).
 //
 //   A  fe_first_filter_tile     first voxel filter (LTB:393-395), per tile of 2048 rows: the tile's lowest row per voxel in
-//                               shared memory, then only those propose their index to the scan's table (atomicCAS claim +
-//                               atomicMin); the survivors end as a per-scan bitmap.
+//                               shared memory; the tile stores its words of the scan's survivor bitmap and writes its winners
+//                               to the scan's hash partitions.
+//   A2 fe_merge_partitions      per (scan, partition): the lowest row per voxel over all tiles, in shared memory; clears the
+//                               bits of the tile winners that lost.
 //   B0 fe_run_poses             12-byte rows with the point times as runs: the deskew pose (fp64 slerp + composition, LTB:430-445) once
 //                               per RUN instead of once per survivor; kernel B then loads the finished Rigid3f.
 //   B  fe_ingest_tile           per tile, the first-filter survivors in index order (from the bitmap): deskew + transform +
 //                               range gate (LTB:426-472) and the SECOND voxel filter (LTB:479-484) keyed on the local-frame
 //                               voxel, again per tile in shared memory first — no compaction in between: ids stay the original
-//                               input indices, which preserves "first point in input order wins" for free. Its survivors end as
-//                               two per-scan bitmaps (returns, misses; 4 KiB per 32 k points), with kernel A's set-then-clear
-//                               protocol.
-//   C  fe_emit_tracking         ordered compaction straight from the bitmaps (popcount prefix; no per-point class map, no
+//                               input indices, which preserves "first point in input order wins" for free. Its tile winners
+//                               end as two per-scan bitmaps (returns, misses; 4 KiB per 32 k points) and go to partitions as
+//                               kernel A's do.
+//   B2 fe_merge_partitions      as A2, for the second filter's words.
+//   C  fe_emit_tracking        ordered compaction straight from the bitmaps (popcount prefix; no per-point class map, no
 //                               tile counts), fused with the scan's current pose (hits_poses.back(), LTB:476) and the frame
 //                               change back to tracking (TransformRangeData with current_pose^-1, LTB:485-487); output rows
 //                               are written coalesced.
 //
-// The second filter's table has ONE 64-bit word per slot: [miss | voxel key relative to the scan's pose | point index]. The
-// key sits above the index, so for equal keys atomicMin keeps the lowest index ("first point in input order", voxel_filter.cc:
-// 81-131) and a slot's key never changes once claimed: a collision compares keys inside the word, never reads another thread's
-// point, and a survivor touches one 8-byte slot (round 1: an 8-byte key slot + a 4-byte min slot). The key holds 3 x axis_bits
+// The second filter's entries are ONE 64-bit word: [miss | voxel key relative to the scan's pose | point index]. The key sits
+// above the index, so for equal keys atomicMin keeps the lowest index ("first point in input order", voxel_filter.cc:81-131)
+// and a claimed word's key never changes: a collision compares keys inside the word. The key holds 3 x axis_bits
 // (axis_bits = min(21, (63 - index_bits) / 3): 15 bits for scans up to 256 k points) of the voxel index RELATIVE to the voxel of
 // the scan's predicted pose: every output point lies within max_range of the (moving) sensor origin, so the reachable span is
 // 2 max_range / voxel_filter_size cells — +-2.4 km at 0.15 m. A point outside it sets the scan's error flag and the scan's
 // result is invalid (ok = -1); the generic dl_voxel_filter has no such limit. Returns and misses share the table (bit 63).
 //
-// Algorithmic traffic per raw point: A reads 12/16 B; B reads 1 bit (+12/16 B row + 4 B time, writes
-// 16 B record + 8 B slot for survivors) and writes 2 bits; C reads 16 B and writes 12 B per output point.
+// Algorithmic traffic per raw point: A reads 12/16 B and writes 1 bit (+16 B entry per tile winner, read back by A2); B reads
+// 1 bit (+12/16 B row + 4 B time, writes 16 B record for survivors, 8 B entry per tile winner, read back by B2) and writes
+// 2 bits; C reads 16 B and writes 12 B per output point.
+#include <type_traits>
+
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
 
@@ -95,12 +100,12 @@ __device__ __forceinline__ int warp_exclusive(int v) {
   return inc - v;
 }
 
-// Both voxel filters keep the lowest input index per voxel, and a minimum can be taken in two levels: within each tile of kTile
-// consecutive rows (shared memory), then over the tile winners (the scan's table in global memory). The survivors are the same
-// for any input order and any tiling; what the tiles buy is that rows arrive in firing order, so most duplicates of a voxel lie in
-// the same tile (first filter: 93 %, second filter: 91.5 % of a 64-beam sweep's duplicates, tools/frontend_locality.py) and never
-// reach the L2's atomic units. A tile table has 2 * kTile slots and holds at most kTile voxels: it cannot fill.
-constexpr int kTile = 2048;
+// Both voxel filters keep the lowest input index per voxel, and a minimum can be taken in any grouping: within each tile of kTile
+// consecutive rows (shared memory), then over the tile winners of one hash partition (shared memory again, see "partitions"
+// below). The survivors are the same for any input order and any tiling; what the tiles buy is that rows arrive in firing order,
+// so most duplicates of a voxel lie in the same tile (first filter: 93 %, second filter: 91.5 % of a 64-beam sweep's duplicates,
+// tools/frontend_locality.py). A tile table has 2 * kTile slots and holds at most kTile voxels: it cannot fill.
+constexpr int kTile = kFrontendTile;
 constexpr int kTileSlots = 2 * kTile;
 
 // Appends the index of every non-empty entry of a tile table to `list` (any order) and returns how many there are. The whole CTA
@@ -120,17 +125,78 @@ __device__ __forceinline__ int list_occupied(const T* table, T empty, uint16_t* 
   return *count;
 }
 
+// ---------------------------------------------------------------------------------------------------- partitions
+// The tile winners of a scan meet by hash partition, not in a scan-wide table. A tile writes its winners to its own kTile-entry
+// segment of the scan's stage, grouped by partition, and the end of every partition to its row of part_ends: it writes the whole
+// row, so nothing needs clearing. Then one CTA per (scan, partition) (kernels A2 and B2, fe_merge_partitions) reads that
+// partition's entries from every tile and keeps the lowest index per voxel in a shared table, as the tiles did; every entry that
+// loses there clears its bit in the scan's bitmap, whose words the tiles stored whole. The kernel boundary orders the clears
+// after the stores.
+//
+// A scan has two partitions per row tile (at most kParts), so a partition expects at most half of its shared table's kTile
+// entries even when every row is its own voxel. A partition with more entries than that (hash collisions, or scans of more than
+// kParts / 2 tiles) runs the same protocol in a global table of 2 slots per entry, carved from the scan's `spill` and cleared by
+// the CTA itself. The partition takes hash bits that the tile table's slot does not use, and the merge's table takes the slot's
+// bits, which vary freely within a partition.
+//
+// A tile counts its winners per partition in 16-bit halves of 32-bit words (a count, start or cursor is at most kTile), so that
+// kernel B's count fits in its tile's bitmap words once they are stored.
+constexpr int kParts = kFrontendParts;
+static_assert(kParts % 64 == 0 && kParts / 2 <= 2 * kTile / 32, "kernel B counts partitions in its tile's bitmap words");
+
+__device__ __forceinline__ int num_parts(int n) { return min(2 * ((n + kTile - 1) / kTile), kParts); }
+__device__ __forceinline__ size_t row_tiles(const FrontendArgs& a) { return (size_t)((a.cap + kTile - 1) / kTile); }
+__device__ __forceinline__ int4* scan_stage(const FrontendArgs& a, int b) { return a.stage + (size_t)b * row_tiles(a) * kTile; }
+__device__ __forceinline__ int32_t* part_ends(const FrontendArgs& a, int b, int tile) {
+  return a.part_ends + ((size_t)b * row_tiles(a) + tile) * kParts;
+}
+// First filter: the tile slot is the hash's top 12 bits (table_slot), the partition its low 20 bits.
+__device__ __forceinline__ int first_part(uint32_t hash, int parts) { return (int)__umulhi(hash << 12, (uint32_t)parts); }
+
+// Adds one to the 16-bit counter of partition q in hist[kParts / 2] and returns its value before.
+__device__ __forceinline__ int part_add(uint32_t* hist, int q) {
+  const int shift = (q & 1) * 16;
+  return (int)(atomicAdd(hist + (q >> 1), 1u << shift) >> shift) & 0xFFFF;
+}
+
+// The whole CTA calls this once hist holds the tile's winners per partition: warp 0 turns the counts into the start of every
+// partition in the tile's segment (hist) and stores their ends to the tile's row of part_ends. The caller then places each
+// winner at part_add(hist, partition).
+__device__ __forceinline__ void partition_starts(uint32_t* hist, int parts, int32_t* ends) {
+  if (threadIdx.x < 32) {
+    constexpr int kWords = kParts / 64;  // per lane: 2 partitions per word
+    uint32_t c[kWords];
+    int sum = 0;
+#pragma unroll
+    for (int j = 0; j < kWords; ++j) {
+      c[j] = hist[threadIdx.x * kWords + j];
+      sum += (int)(c[j] & 0xFFFF) + (int)(c[j] >> 16);
+    }
+    int run = warp_exclusive(sum);
+#pragma unroll
+    for (int j = 0; j < kWords; ++j) {
+      const int q = 2 * (threadIdx.x * kWords + j);
+      const int lo = run, hi = run + (int)(c[j] & 0xFFFF);
+      run = hi + (int)(c[j] >> 16);
+      hist[threadIdx.x * kWords + j] = (uint32_t)lo | ((uint32_t)hi << 16);
+      if (q < parts) ends[q] = hi;
+      if (q + 1 < parts) ends[q + 1] = run;
+    }
+  }
+  __syncthreads();
+}
+
 // ---------------------------------------------------------------------------------------------------- A
 // One CTA per tile: the rows' cells go to shared memory (consecutive lanes read consecutive rows, so every sector of the tile is
-// fetched once), a shared table keeps the lowest row per cell (comparing cells in shared memory), and only the tile winners
-// propose their index to the scan's table: CAS claim, atomicMin only when the newcomer is older. A collision there still compares
-// against the owner's row in global memory.
+// fetched once), and a shared table keeps the lowest row per cell (comparing cells in shared memory). The tile stores its words
+// of the scan's first-filter bitmap, one bit per tile winner, and writes each winner to its partition as {cell x, y, z, row}.
 constexpr int kTileBlock = 512;
 __global__ void __launch_bounds__(kTileBlock) fe_first_filter_tile(FrontendArgs a) {
   __shared__ Int3 cell[kTile];
   __shared__ uint32_t owner[kTileSlots];
   __shared__ uint16_t winners[kTile];
   __shared__ uint32_t tile_bits[kTile / 32];
+  __shared__ uint32_t hist[kParts / 2];
   __shared__ int num_winners;
   const int b = a.first_scan + blockIdx.y;
   const int n = a.counts[b];
@@ -142,6 +208,7 @@ __global__ void __launch_bounds__(kTileBlock) fe_first_filter_tile(FrontendArgs 
   for (int k = threadIdx.x; k < kTileSlots; k += kTileBlock) owner[k] = kEmpty32;
   if (threadIdx.x == 0) num_winners = 0;
   if (threadIdx.x < kTile / 32) tile_bits[threadIdx.x] = 0;
+  if (threadIdx.x < kParts / 2) hist[threadIdx.x] = 0;
   for (int k = threadIdx.x; k < rows_here; k += kTileBlock) cell[k] = cell_index(load_xyz(rows, a.row_floats, base + k), res);
   __syncthreads();
   for (int k = threadIdx.x; k < rows_here; k += kTileBlock) {
@@ -160,45 +227,23 @@ __global__ void __launch_bounds__(kTileBlock) fe_first_filter_tile(FrontendArgs 
   }
   __syncthreads();
   const int m = list_occupied(owner, kEmpty32, winners, &num_winners);
-  // The scan's first-filter bitmap (memset to 0): every tile winner sets its bit before it is inserted (fence, then barrier), and
-  // every insert that meets an equal voxel clears the bit of the one that lost, the newcomer or the owner it replaced. A voxel
-  // with k tile winners sees k - 1 such meetings, each with a different loser, so exactly the lowest index keeps its bit (4 % of
-  // the tile winners on a bench sweep are cleared). Streaming the scan's table into the bitmap instead cost a kernel as long as
-  // a third of this one.
+  // One bit per tile winner; the merge (A2) clears the bits of the winners that lose to another tile's (4 % of the tile winners
+  // on a bench sweep).
+  const int parts = num_parts(n);
   for (int k = threadIdx.x; k < m; k += kTileBlock) {
     const uint32_t w = owner[winners[k]];
     atomicOr(tile_bits + (w >> 5), 1u << (w & 31));
+    part_add(hist, first_part(hash_cell(cell[w]), parts));
   }
   __syncthreads();
-  uint32_t* bits = a.first_bits + (size_t)b * a.bit_words;
-  if (threadIdx.x < kTile / 32 && tile_bits[threadIdx.x]) {
-    atomicOr(bits + (base >> 5) + threadIdx.x, tile_bits[threadIdx.x]);
-    __threadfence();
-  }
-  __syncthreads();
-  uint32_t* tab = a.table1 + (size_t)b * a.tcap1;
-  const uint32_t tcap = (uint32_t)a.tcap1;  // any size (not a power of two): slot = hash * tcap >> 32
+  if (threadIdx.x < ((rows_here + 31) >> 5))
+    a.first_bits[(size_t)b * a.bit_words + (base >> 5) + threadIdx.x] = tile_bits[threadIdx.x];
+  partition_starts(hist, parts, part_ends(a, b, blockIdx.x));
+  int4* seg = scan_stage(a, b) + base;
   for (int k = threadIdx.x; k < m; k += kTileBlock) {
     const uint32_t w = owner[winners[k]];
     const Int3 c = cell[w];
-    const uint32_t i = (uint32_t)base + w;
-    uint32_t hh = table_slot(hash_cell(c), tcap);
-    uint32_t p = atomicCAS(tab + hh, kEmpty32, i);
-    while (p != kEmpty32) {
-      const Int3 o = cell_index(load_xyz(rows, a.row_floats, p), res);
-      if (o.x == c.x && o.y == c.y && o.z == c.z) {
-        uint32_t loser = i;
-        if (i < p) {
-          const uint32_t q = atomicMin(tab + hh, i);  // the owner only ever decreases
-          if (q > i) loser = q;
-        }
-        __threadfence();  // the loser's bit was set before its insert that this thread has seen
-        atomicAnd(bits + (loser >> 5), ~(1u << (loser & 31)));
-        break;
-      }
-      hh = hh + 1 == tcap ? 0u : hh + 1;
-      p = atomicCAS(tab + hh, kEmpty32, i);
-    }
+    seg[part_add(hist, first_part(hash_cell(c), parts))] = make_int4(c.x, c.y, c.z, base + (int)w);
   }
 }
 
@@ -269,23 +314,25 @@ __device__ __forceinline__ Int3 unpack_cell(const KeyLayout& k, unsigned long lo
   return {(int)(((uint32_t)(key >> (2 * k.axis_bits)) & m) + k.bx), (int)(((uint32_t)(key >> k.axis_bits) & m) + k.by),
           (int)(((uint32_t)key & m) + k.bz)};
 }
-// Second-filter insert of a slot word into a table of mask + 1 slots (the tile's in shared memory or the scan's): CAS claim; among
-// equal keys (same class and voxel) atomicMin keeps the lowest index. Returns the word that lost the meeting, the newcomer's or
-// the one it replaced, or kEmpty64 when the insert claimed an empty slot.
-__device__ __forceinline__ unsigned long long slot_insert(unsigned long long* slots, uint32_t mask, int idx_bits, const Int3& c,
-                                                          unsigned long long slot) {
-  uint32_t hh = (hash_cell(c) ^ ((slot >> 63) ? 0x9e3779b9u : 0u)) & mask;
+// Second-filter hash of a slot word in voxel c: returns and misses apart. The tile slot is its low 12 bits, the partition the 20
+// bits above.
+__device__ __forceinline__ uint32_t second_hash(const Int3& c, unsigned long long slot) {
+  return hash_cell(c) ^ ((slot >> 63) ? 0x9e3779b9u : 0u);
+}
+__device__ __forceinline__ int second_part(uint32_t hash, int parts) { return (int)__umulhi(hash & 0xFFFFF000u, (uint32_t)parts); }
+
+// Second-filter insert of a slot word into the tile's table: CAS claim; among equal keys (same class and voxel) atomicMin keeps
+// the lowest index.
+__device__ __forceinline__ void slot_insert(unsigned long long* slots, int idx_bits, const Int3& c, unsigned long long slot) {
+  uint32_t hh = second_hash(c, slot) & (kTileSlots - 1);
   for (;;) {
     const unsigned long long prev = atomicCAS(slots + hh, kEmpty64, slot);
-    if (prev == kEmpty64) return kEmpty64;
+    if (prev == kEmpty64) return;
     if ((prev >> idx_bits) == (slot >> idx_bits)) {
-      if (slot < prev) {
-        const unsigned long long q = atomicMin(slots + hh, slot);  // the owner only ever decreases
-        if (q > slot) return q;
-      }
-      return slot;
+      if (slot < prev) atomicMin(slots + hh, slot);  // the owner only ever decreases
+      return;
     }
-    hh = (hh + 1) & mask;
+    hh = (hh + 1) & (kTileSlots - 1);
   }
 }
 
@@ -335,7 +382,7 @@ __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, con
       a.error_flag[b] = 1;  // per scan: only this scan's result is invalidated
       cls = 0;
     } else {
-      slot_insert(tile_slots, kTileSlots - 1, kl.idx_bits, c, slot);
+      slot_insert(tile_slots, kl.idx_bits, c, slot);
     }
   }
   return cls;
@@ -344,16 +391,9 @@ __device__ __forceinline__ int ingest_survivor(const FrontendArgs& a, int b, con
 // One CTA per tile of kTile rows. Warp 0 expands the tile's first-filter bitmap words into a shared list of survivors in index
 // order (only ~40 % of the rows survive, so the heavy path runs over the list with all lanes busy): rows are read and local-frame
 // records written at nearly consecutive addresses, and the run search of 12-byte rows covers only the tile's few dozen runs
-// (L1-resident starts and poses). The survivors' second-filter words meet in the tile table; only the tile winners go on to the
-// scan's table, with the same protocol.
-//
-// The second filter's survivors end as the scan's two bitmaps (returns, misses) with the first filter's set-then-clear protocol:
-// the CTA stores its tile's words of both bitmaps, one bit per tile winner, before any of its winners is inserted (fence, then
-// barrier), and every insert that meets an equal key clears the bit of the one that lost, the newcomer or the word it replaced.
-// A key with k tile winners sees k - 1 meetings, each with a different loser, so exactly the lowest index keeps its bit. A clear
-// only ever follows the store of its word (the loser was seen in the scan's table), so the stores need no cleared bitmap, and
-// every word the compaction reads is stored by the tile that owns it. This replaces a kernel that streamed the whole scan table
-// (8 bytes per slot, 2^17 slots per 64-beam scan) to find the winners.
+// (L1-resident starts and poses). The survivors' second-filter words meet in the tile table. The CTA stores its tile's words of
+// the scan's two bitmaps (returns, misses), one bit per tile winner, and writes the winners' words (self-describing: miss | key
+// | index) to their partitions, where B2 clears the bits of those that lose to another tile's.
 constexpr int kWordsPerLane = kTile / 32 / 32;  // bitmap words of a tile per lane of warp 0
 constexpr int kTileWords = kTile / 32;
 
@@ -424,22 +464,124 @@ __global__ void __launch_bounds__(kBlock, kRunPose ? 6 : 4) fe_ingest_tile(Front
   if (threadIdx.x < 2 * kTileWords) {
     const int miss = threadIdx.x / kTileWords, q = threadIdx.x % kTileWords;
     if (q < ((rows_here + 31) >> 5)) __stcg(scan_bits(a, b, miss) + (base >> 5) + q, tile_bits[miss][q]);
-    __threadfence();
   }
   __syncthreads();
-  unsigned long long* slots = a.slots2 + (size_t)b * a.tcap2;
-  const uint32_t mask2 = (uint32_t)a.tcap2 - 1;
+  uint32_t* hist = &tile_bits[0][0];  // stored: the words count the winners per partition now (6 CTAs per SM leave no room)
+  if (threadIdx.x < kParts / 2) hist[threadIdx.x] = 0;
+  __syncthreads();
+  const int parts = num_parts(n);
   for (int k = threadIdx.x; k < won; k += kBlock) {
     const unsigned long long s = tile_slots[list[k]];
-    const unsigned long long loser = slot_insert(slots, mask2, kl.idx_bits, unpack_cell(kl, s), s);
-    if (loser != kEmpty64) {
-      const uint32_t i = (uint32_t)(loser & idx_mask);
-      __threadfence();  // the loser's bit was stored before its insert that this thread has seen
-      atomicAnd(scan_bits(a, b, (int)(loser >> 63)) + (i >> 5), ~(1u << (i & 31)));
-    }
+    part_add(hist, second_part(second_hash(unpack_cell(kl, s), s), parts));
+  }
+  __syncthreads();
+  partition_starts(hist, parts, part_ends(a, b, blockIdx.x));
+  unsigned long long* seg = reinterpret_cast<unsigned long long*>(scan_stage(a, b)) + base;
+  for (int k = threadIdx.x; k < won; k += kBlock) {
+    const unsigned long long s = tile_slots[list[k]];
+    seg[part_add(hist, second_part(second_hash(unpack_cell(kl, s), s), parts))] = s;
   }
   returns = warp_sum(returns);
   if (lane == 0 && returns) atomicAdd(a.n_returns_local + b, returns);
+}
+
+// ---------------------------------------------------------------------------------------------------- A2, B2
+// Merge of entry k into a table of n slots that holds entry positions (Slot: 16 bits in shared memory, 32 in the spill): CAS
+// claim; an equal voxel keeps the lower index in the claimer's entry (atomicMin) and clears the bit of the one that lost, the
+// newcomer or the index it replaced. A voxel with k entries sees k - 1 meetings, each with a different loser, so exactly the
+// lowest index keeps its bit. An entry's index changes only once it has claimed a slot, so entry k is read unchanged here.
+template <typename Slot>
+__device__ __forceinline__ void merge_entry(const FrontendArgs& a, int b, const KeyLayout&, int4* ent, uint32_t k, Slot* table,
+                                            uint32_t n) {
+  const int4 e = ent[k];
+  const uint32_t i = (uint32_t)e.w;
+  uint32_t hh = __umulhi(hash_cell(Int3{e.x, e.y, e.z}), n);  // the top bits: the partition took the low ones
+  for (;;) {
+    const Slot o = atomicCAS(table + hh, (Slot)~0u, (Slot)k);
+    if (o == (Slot)~0u) return;
+    const int4 f = ent[o];
+    if (f.x == e.x && f.y == e.y && f.z == e.z) {
+      const uint32_t loser = max(atomicMin(reinterpret_cast<unsigned*>(&ent[o].w), i), i);
+      atomicAnd(a.first_bits + (size_t)b * a.bit_words + (loser >> 5), ~(1u << (loser & 31)));
+      return;
+    }
+    hh = hh + 1 == n ? 0u : hh + 1;
+  }
+}
+template <typename Slot>
+__device__ __forceinline__ void merge_entry(const FrontendArgs& a, int b, const KeyLayout& kl, unsigned long long* ent, uint32_t k,
+                                            Slot* table, uint32_t n) {
+  const unsigned long long s = ent[k];
+  const uint32_t h = second_hash(unpack_cell(kl, s), s);
+  uint32_t hh = __umulhi(__funnelshift_l(h, h, 20), n);  // the low 12 bits first: the partition took the ones above
+  for (;;) {
+    const Slot o = atomicCAS(table + hh, (Slot)~0u, (Slot)k);
+    if (o == (Slot)~0u) return;
+    if ((ent[o] >> kl.idx_bits) == (s >> kl.idx_bits)) {  // the key bits of a claimed entry never change
+      const unsigned long long loser = max(atomicMin(ent + o, s), s);
+      const uint32_t i = (uint32_t)(loser & ((1ull << kl.idx_bits) - 1));
+      atomicAnd(scan_bits(a, b, (int)(loser >> 63)) + (i >> 5), ~(1u << (i & 31)));
+      return;
+    }
+    hh = hh + 1 == n ? 0u : hh + 1;
+  }
+}
+
+// One CTA per (scan, partition), kSecond: B2, else A2. The partition's entries are copied from every tile's segment into shared
+// memory and merged there; when they exceed kTile they are merged where they lie, through a table in the scan's spill.
+constexpr int kMergeBlock = 256;
+template <bool kSecond>
+__global__ void __launch_bounds__(kMergeBlock) fe_merge_partitions(FrontendArgs a) {
+  using Entry = typename std::conditional<kSecond, unsigned long long, int4>::type;
+  __shared__ Entry ent[kTile];
+  __shared__ uint32_t table[kTileSlots / 2];  // kTileSlots 16-bit slots
+  __shared__ int fill;
+  __shared__ uint32_t* spill;
+  const int b = a.first_scan + blockIdx.y;
+  const int n = a.counts[b];
+  const int p = blockIdx.x;
+  if (p >= num_parts(n)) return;
+  const int tiles = (n + kTile - 1) / kTile;
+  const int32_t* ends = part_ends(a, b, 0) + p;  // tile t: ends[t * kParts]
+  Entry* stage = reinterpret_cast<Entry*>(scan_stage(a, b));
+  const KeyLayout kl = kSecond ? key_layout(a, a.scans[b]) : KeyLayout{};
+  if (threadIdx.x == 0) fill = 0;
+  for (int k = threadIdx.x; k < kTileSlots / 2; k += kMergeBlock) table[k] = kEmpty32;
+  __syncthreads();
+  // a thread per tile reserves room for the tile's entries and copies them while the partition still fits (kCopy loads in
+  // flight: a tile holds a few entries of a partition)
+  constexpr int kCopy = 4;
+  for (int t = threadIdx.x; t < tiles; t += kMergeBlock) {
+    const int from = p ? ends[(size_t)t * kParts - 1] : 0, to = ends[(size_t)t * kParts];
+    const int at = atomicAdd(&fill, to - from) - from;
+    if (at + to > kTile) continue;
+    for (int j = from; j < to; j += kCopy) {
+      Entry v[kCopy];
+#pragma unroll
+      for (int u = 0; u < kCopy; ++u)
+        if (j + u < to) v[u] = stage[(size_t)t * kTile + j + u];
+#pragma unroll
+      for (int u = 0; u < kCopy; ++u)
+        if (j + u < to) ent[at + j + u] = v[u];
+    }
+  }
+  __syncthreads();
+  const int count = fill;
+  if (count <= kTile) {
+    for (int k = threadIdx.x; k < count; k += kMergeBlock)
+      merge_entry(a, b, kl, ent, (uint32_t)k, reinterpret_cast<uint16_t*>(table), (uint32_t)kTileSlots);
+    return;
+  }
+  const uint32_t slots = 2u * (uint32_t)count;
+  if (threadIdx.x == 0) spill = a.spill + (size_t)b * 2 * row_tiles(a) * kTile + atomicAdd(a.spill_used + 2 * b + kSecond, (int)slots);
+  __syncthreads();
+  uint32_t* tab = spill;
+  for (uint32_t k = threadIdx.x; k < slots; k += kMergeBlock) tab[k] = kEmpty32;
+  __syncthreads();
+  for (int t = threadIdx.x; t < tiles; t += kMergeBlock) {
+    const int from = p ? ends[(size_t)t * kParts - 1] : 0, to = ends[(size_t)t * kParts];
+    for (int j = from; j < to; ++j) merge_entry(a, b, kl, stage, (uint32_t)(t * kTile + j), tab, slots);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------- C
@@ -569,6 +711,7 @@ __global__ void fe_reset_counters(FrontendArgs a, int batch) {
     cp[0] = cur.t.x; cp[1] = cur.t.y; cp[2] = cur.t.z; cp[3] = cur.q.w; cp[4] = cur.q.x; cp[5] = cur.q.y; cp[6] = cur.q.z;
   }
   a.error_flag[b] = 0;
+  a.spill_used[2 * b] = a.spill_used[2 * b + 1] = 0;
 }
 
 // ---------------------------------------------------------------------------------------------------- glue
@@ -639,27 +782,30 @@ __global__ void finalize_results_kernel(ResultArgs a) {
 
 }  // namespace
 
-// The scan tables live in global memory and are cleared here on every call. Keeping them in a thread-block cluster's distributed
-// shared memory instead (one 8-CTA cluster per scan, no memsets) gave the same outputs but made the step 1.45x slower: one CTA
-// per SM cannot hide the tiles' latency as four per-tile CTAs do (DESIGN §6).
+// Nothing of the front half needs clearing: the tiles store every bitmap word and part_ends row that is read, and a spilled
+// partition clears its own table.
 int launch_fe_prepare(dl_context* ctx, const FrontendArgs& a, int batch) {
-  DL_CUDA(ctx, cudaMemsetAsync(a.table1, 0xFF, (size_t)batch * a.tcap1 * sizeof(uint32_t), ctx->stream));
-  DL_CUDA(ctx, cudaMemsetAsync(a.slots2, 0xFF, (size_t)batch * a.tcap2 * sizeof(unsigned long long), ctx->stream));
-  // a.bits needs no clearing: fe_ingest_tile stores every word of it that fe_emit_tracking reads
-  DL_CUDA(ctx, cudaMemsetAsync(a.first_bits, 0, (size_t)batch * a.bit_words * sizeof(uint32_t), ctx->stream));
   fe_reset_counters<<<(batch + 127) / 128, 128, 0, ctx->stream>>>(a, batch);
   DL_LAUNCH_CHECK(ctx, "fe_reset_counters");
   return DL_OK;
 }
 
-// Kernel A for scans [first_scan, first_scan + num_scans): lets the host overlap the upload of later scans.
+static int launch_merge(dl_context* ctx, const FrontendArgs& a, int row_tiles, int num_scans, bool second) {
+  const dim3 grid(std::min(2 * row_tiles, kParts), num_scans);
+  if (second) fe_merge_partitions<true><<<grid, kMergeBlock, 0, ctx->stream>>>(a);
+  else fe_merge_partitions<false><<<grid, kMergeBlock, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "fe_merge_partitions");
+  return DL_OK;
+}
+
+// Kernels A and A2 for scans [first_scan, first_scan + num_scans): lets the host overlap the upload of later scans.
 int launch_fe_first_filter(dl_context* ctx, FrontendArgs a, int first_scan, int num_scans) {
   if (num_scans <= 0) return DL_OK;
   a.first_scan = first_scan;
   const int row_tiles = (int)((a.cap + kTile - 1) / kTile);
   fe_first_filter_tile<<<dim3(row_tiles, num_scans), kTileBlock, 0, ctx->stream>>>(a);
   DL_LAUNCH_CHECK(ctx, "fe_first_filter_tile");
-  return DL_OK;
+  return launch_merge(ctx, a, row_tiles, num_scans, false);
 }
 
 int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
@@ -674,6 +820,7 @@ int launch_fe_rest(dl_context* ctx, FrontendArgs a, int first_scan, int batch) {
     fe_ingest_tile<false><<<dim3(row_tiles, batch), kBlock, 0, ctx->stream>>>(a);
   }
   DL_LAUNCH_CHECK(ctx, "fe_ingest_tile");
+  if (const int st = launch_merge(ctx, a, row_tiles, batch, true)) return st;
   const int max_chunks = (int)((a.bit_words + 31) / 32);
   const size_t smem = (size_t)2 * (max_chunks + 1) * sizeof(int) + (size_t)kEmitWarps * kChunkPoints * sizeof(uint16_t);
   if (smem > 200 * 1024) return ctx->fail(DL_ERR_ARG, "scan too large for the front end's compaction (> 20 M points)");

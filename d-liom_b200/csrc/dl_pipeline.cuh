@@ -47,7 +47,9 @@ struct ImuPrepareArgs {
 };
 int launch_imu_prepare(dl_context* ctx, const ImuPrepareArgs& a);
 
-// Fused front half (dl_frontend.cu).
+// Fused front half (dl_frontend.cu): rows per tile, and the most hash partitions a scan's tile winners are split into.
+constexpr int kFrontendTile = 2048;
+constexpr int kFrontendParts = 256;
 struct FrontendArgs {
   const float* ranges;   // scan b starts at row b * in_cap; rows of row_floats floats (3: x y z, 4: x y z t, 8: + u64 origin index)
   const int32_t* run_offsets;    // row_floats == 3: per-point times as runs (dl_frontend_options::time_run_*), device copies
@@ -63,12 +65,13 @@ struct FrontendArgs {
   const float* origins;
   const int32_t* origin_base;    // per scan: its first origin in `origins` (a row's origin index counts from there)
   int64_t cap;           // per-scan capacity of every per-point array below
-  int64_t tcap1, tcap2;  // table capacities (powers of two)
   float first_resolution, second_resolution, min_range, max_range;
   double scan_period;
-  uint32_t* table1;              // first filter: slot -> min point index
   uint32_t* first_bits;          // per scan one bitmap of bit_words words: bit i = point i survives the first filter
-  unsigned long long* slots2;    // second filter: slot -> [miss | relative voxel key | point index] (dl_frontend.cu)
+  int4* stage;                   // per scan one 2048-entry segment per row tile: the tile winners grouped by hash partition
+  int32_t* part_ends;            // per scan and row tile, kFrontendParts ints: end of each partition's entries in its segment
+  uint32_t* spill;               // per scan 2 slots per stage entry: tables of the partitions too large for shared memory
+  int32_t* spill_used;           // per scan 2 (first, second filter): slots of `spill` taken so far
   int idx_bits, axis_bits;       // widths of the index field and of one axis of the key
   uint32_t* bits;                // per scan two bitmaps (returns, misses) of bit_words words: bit i = point i survives
   int64_t bit_words;             // ceil(cap / 32)
