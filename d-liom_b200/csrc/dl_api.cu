@@ -1102,9 +1102,11 @@ void search_window(const dl_fcsm_options& o, const dl_grid* hi, int* wxy, int* w
 }
 // Decides, before the scratch is carved, whether pairs [first, first + n) get the pruned search and how many pruning blocks
 // its bounds table needs per pair. The pruned search needs the index of every high-resolution grid of the chunk
-// (DLIOM_FCSM_EXHAUSTIVE=1 forces the fallback) and at most 60 000 blocks per pair (one CTA per block and pair in grid.x).
-int plan_coarse(dl_context* ctx, const dl_fcsm_options& o, int first, int n, const dl_grid* const* hi_grids, CoarseSearch* cs) {
-  cs->pruned = std::getenv("DLIOM_FCSM_EXHAUSTIVE") == nullptr;
+// (DLIOM_FCSM_EXHAUSTIVE=1 or allow_pruned = false forces the fallback, and then no index is built) and at most 60 000 blocks
+// per pair (one CTA per block and pair in grid.x).
+int plan_coarse(dl_context* ctx, const dl_fcsm_options& o, int first, int n, const dl_grid* const* hi_grids, CoarseSearch* cs,
+                bool allow_pruned = true) {
+  cs->pruned = allow_pruned && std::getenv("DLIOM_FCSM_EXHAUSTIVE") == nullptr;
   cs->max_blocks = 1;
   for (int k = 0; k < n && cs->pruned; ++k) {
     bool have = false;
@@ -1140,9 +1142,10 @@ void carve_coarse(Arena& a, const PairClouds& pc, int first, int n, CoarseSearch
 }
 
 // Runs the coarse search for pairs [first, first + n) in the buffers carve_coarse took, uploading their clouds first unless they
-// are device-resident; leaves the picks on the device.
+// are device-resident; leaves the picks on the device. all_scores_dev (exhaustive search of one pair only): every leaf score.
 int coarse_search(dl_context* ctx, const dl_fcsm_options& o, float min_score, int first, int n, const double* guesses,
-                  const PairClouds& pc, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, CoarseSearch* out) {
+                  const PairClouds& pc, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, CoarseSearch* out,
+                  float* all_scores_dev = nullptr) {
   const int64_t* hi_off = pc.hi_off;
   const int64_t* lo_off = pc.lo_off;
   const int64_t hi0 = hi_off[first], lo0 = lo_off[first];
@@ -1192,7 +1195,7 @@ int coarse_search(dl_context* ctx, const dl_fcsm_options& o, float min_score, in
   if (out->pruned)
     return launch_fcsm_pruned(ctx, out->d_pairs, n, max_points, out->max_blocks, out->d_bounds, out->d_max_bound, out->d_best,
                               out->d_picks);
-  return launch_fcsm(ctx, out->d_pairs, n, max_points, max_candidates, out->d_best, out->d_picks, nullptr);
+  return launch_fcsm(ctx, out->d_pairs, n, max_points, max_candidates, out->d_best, out->d_picks, all_scores_dev);
 }
 int check_pairs(dl_context* ctx, int count, const double* guesses, const float* hi_pts, const int64_t* hi_off, const float* lo_pts,
                 const int64_t* lo_off, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids) {
@@ -1212,7 +1215,7 @@ extern "C" {
 
 int dl_fcsm_match_3dof(dl_context* ctx, const dl_fcsm_options* o, const double* guess, const float* hi_pts, int64_t n_hi,
                        const float* lo_pts, int64_t n_lo, const dl_grid* hi, const dl_grid* lo, float min_score,
-                       dl_fcsm_result* result) {
+                       dl_fcsm_result* result, float* all_scores, int64_t all_scores_capacity) {
   if (!ctx || !o || !result || n_hi < 0 || n_lo < 0) return DL_ERR_ARG;
   const int64_t hi_off[2] = {0, n_hi}, lo_off[2] = {0, n_lo};
   if (guess && hi && lo && (n_hi == 0 || n_lo == 0)) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
@@ -1225,11 +1228,20 @@ int dl_fcsm_match_3dof(dl_context* ctx, const dl_fcsm_options* o, const double* 
   pc.lo_pts = lo_pts;
   pc.hi_off = hi_off;
   pc.lo_off = lo_off;
-  DL_TRY(plan_coarse(ctx, *o, 0, 1, &hi, &cs));
-  DL_TRY(carve_scratch(ctx, [&](Arena& a) { carve_coarse(a, pc, 0, 1, &cs); }));
-  DL_TRY(coarse_search(ctx, *o, min_score, 0, 1, guess, pc, &hi, &lo, &cs));
+  int wxy, wz;
+  search_window(*o, hi, &wxy, &wz);
+  const int64_t K = (2ll * wxy + 1) * (2ll * wxy + 1) * (2ll * wz + 1);
+  if (all_scores && all_scores_capacity < K) return ctx->fail(DL_ERR_ARG, "all_scores has room for fewer than num_candidates floats");
+  DL_TRY(plan_coarse(ctx, *o, 0, 1, &hi, &cs, all_scores == nullptr));  // only the exhaustive kernel scores every leaf
+  float* d_scores = nullptr;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    carve_coarse(a, pc, 0, 1, &cs);
+    d_scores = all_scores ? a.take<float>(K) : nullptr;
+  }));
+  DL_TRY(coarse_search(ctx, *o, min_score, 0, 1, guess, pc, &hi, &lo, &cs, d_scores));
   FcsmPick pick;
   DL_TRY(d2h(ctx, &pick, cs.d_picks, 1));
+  if (all_scores) DL_TRY(d2h(ctx, all_scores, d_scores, K));
   DL_TRY(sync(ctx));
   std::memset(result, 0, sizeof(*result));
   result->num_candidates = pick.num_candidates;

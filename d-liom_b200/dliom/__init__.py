@@ -458,7 +458,7 @@ def lib():
                                            ip(C.c_int64), f32p, ip(C.c_int)]
     L.dl_rtcsm_match.argtypes = [vp, ip(RtcsmOptions), f64p, f32p, C.c_int64, vp, f64p, ip(C.c_float), ip(RtcsmInfo), vp]
     L.dl_fcsm_match_3dof.argtypes = [vp, ip(FcsmOptions), f64p, f32p, C.c_int64, f32p, C.c_int64, vp, vp, C.c_float,
-                                     ip(FcsmResult)]
+                                     ip(FcsmResult), vp, C.c_int64]
     L.dl_fcsm_match.argtypes = [vp, ip(FcsmOptions), f32p, f32p, C.c_int32, f64p, f64p, f64p, f32p, C.c_int64, f32p, C.c_int64, vp, vp,
                                 C.c_float, ip(FcsmResult)]
     L.dl_constraint_search_batch.argtypes = [vp, ip(ConstraintOptions), C.c_int32, f64p, f32p, i64p, f32p, i64p, C.c_void_p,
@@ -734,15 +734,25 @@ class Context:
                 "scores": scores}
 
     def fcsm_match_3dof(self, hi_grid, lo_grid, hi_points, lo_points, pose_guess, min_score, xy_window=5.0, z_window=1.0,
-                        min_low_resolution_score=0.55, min_rotational_score=0.77, depth=8, full_depth=3):
+                        min_low_resolution_score=0.55, min_rotational_score=0.77, depth=8, full_depth=3, want_scores=False):
+        """MatchWith3DofInitial -> FcsmResult; with want_scores, (FcsmResult, float32 score of every leaf as a
+        [2 wz + 1, 2 wxy + 1, 2 wxy + 1] (z, y, x) array), from the exhaustive search. The array is sized by the header's
+        formula; the library checks its capacity against its own count and refuses a call it would overrun."""
         hi_points = np.ascontiguousarray(hi_points, np.float32).reshape(-1, 3)
         lo_points = np.ascontiguousarray(lo_points, np.float32).reshape(-1, 3)
         opt = FcsmOptions(depth, full_depth, min_rotational_score, min_low_resolution_score, xy_window, z_window, 0.26)
         r = FcsmResult()
+        scores = None
+        if want_scores:
+            res = float(self.L.dl_grid_resolution(hi_grid.h))    # window / float resolution in double, then lround
+            wxy, wz = (int(np.floor(q)) + int(q - np.floor(q) >= 0.5) for q in (xy_window / res, z_window / res))
+            scores = np.zeros((2 * wz + 1, 2 * wxy + 1, 2 * wxy + 1), np.float32) if min(wxy, wz) >= 0 else np.zeros(1, np.float32)
         self.check(self.L.dl_fcsm_match_3dof(self.h, C.byref(opt), np.ascontiguousarray(pose_guess, np.float64), hi_points,
                                              len(hi_points), lo_points, len(lo_points), hi_grid.h, lo_grid.h,
-                                             np.float32(min_score), C.byref(r)))
-        return r
+                                             np.float32(min_score), C.byref(r),
+                                             None if scores is None else scores.ctypes.data_as(C.c_void_p),
+                                             0 if scores is None else scores.size))
+        return r if scores is None else (r, scores)
 
     def fcsm_match(self, hi_grid, lo_grid, hi_points, lo_points, node_pose, submap_pose, min_score, submap_histogram=None,
                    scan_histogram=None, histogram_size=10, gravity_alignment=(1.0, 0.0, 0.0, 0.0), xy_window=5.0, z_window=1.0,

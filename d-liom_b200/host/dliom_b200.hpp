@@ -241,7 +241,7 @@ class FastCorrelativeScanMatcher3D {
                                    high_resolution_point_cloud.empty() ? nullptr : high_resolution_point_cloud[0].data(),
                                    (int64_t)high_resolution_point_cloud.size(),
                                    low_resolution_point_cloud.empty() ? nullptr : low_resolution_point_cloud[0].data(),
-                                   (int64_t)low_resolution_point_cloud.size(), hi_->get(), lo_->get(), min_score, &r));
+                                   (int64_t)low_resolution_point_cloud.size(), hi_->get(), lo_->get(), min_score, &r, nullptr, 0));
     if (!r.found) return nullptr;
     return std::unique_ptr<Result>(new Result{r.score, Rigid3d::from7(r.pose_estimate), r.rotational_score, r.low_resolution_score});
   }

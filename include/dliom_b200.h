@@ -180,10 +180,14 @@ typedef struct dl_fcsm_result { /* FastCorrelativeScanMatcher3D::Result; found =
   int32_t scan_index;     /* dl_fcsm_match: which of the yaw steps that passed the rotational score won (0 otherwise) */
   int64_t num_candidates; /* leaves scored */
 } dl_fcsm_result;
+/* all_scores (optional) receives the score of every leaf, index (z * side + y) * side + x, offsets counted from the window's
+ * low corner, and asking for it runs the exhaustive search. With wxy = lround(linear_xy_search_window / (double)resolution),
+ * wz = lround(linear_z_search_window / (double)resolution) and side = 2 * wxy + 1 there are num_candidates =
+ * side * side * (2 * wz + 1) leaves; an all_scores_capacity (in floats) below that fails with DL_ERR_ARG before any work. */
 int dl_fcsm_match_3dof(dl_context* ctx, const dl_fcsm_options* options, const double* pose_in_submap_guess,
                        const float* high_resolution_points, int64_t n_high, const float* low_resolution_points,
                        int64_t n_low, const dl_grid* high_resolution_grid, const dl_grid* low_resolution_grid,
-                       float min_score, dl_fcsm_result* result);
+                       float min_score, dl_fcsm_result* result, float* all_scores, int64_t all_scores_capacity);
 
 /* FastCorrelativeScanMatcher3D::Match (SM/fast_correlative_scan_matcher_3d.cc:145-162, :221-250, :296-350): the yaw search
  * around the node's orientation x the translation window. The yaw steps, the rotational scores (RotationalScanMatcher::Match on
