@@ -12,12 +12,25 @@
 //   pass 3  mw_gate (count/scatter) remove iff !(rays < 3 * hits), ordered compaction into the output
 // The acos / sin of a node interval's slerp are computed on the host (glibc), once per interval; the per-run sin of the
 // interpolation factor is the device's (DESIGN §4).
+//
+// X-ray stages (final pass only, every stage in one read of the output points, in chunks of kXrayChunk points):
+//   mw_xray_check     every stage's cell inside +-8192, before anything changes
+//   mw_xray_insert    per stage: claim the voxel key (64-bit CAS), count the point in its column and, if the voxel is new, the
+//                     column's occupied voxels (integer atomics), extend the bounding box (warp min / max, then integer atomics);
+//                     for a stage with colours, one (stage, column slot) sort key per point
+//   stable radix sort of the keys (values: point indices), then mw_xray_fold: one thread per column adds its points' colours
+//                     in stream order onto the column's float sums, which is the reference's order of float additions
+//   mw_xray_pixels    IntoImage after the final flush, with log(n) from a host-built glibc table
 #include <algorithm>
 #include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <mutex>
 #include <vector>
+
+#include <cub/cub.cuh>
 
 #include "dl_internal.cuh"
 
@@ -39,7 +52,7 @@ struct TrajRec {
 };
 struct MsgRec {
   int64_t stamp, first_row, voff;  // voff: first virtual row of the message
-  int32_t slot, pad;
+  int32_t slot, frame;
   Rigidd sensor_to_tracking;
 };
 struct RunPose {
@@ -69,6 +82,7 @@ struct SelectArgs {
   int32_t* num_keep;
   float4* compact;           // x y z + message index (bits) of every kept point, in order
   float* out_xyz;            // or x y z only, straight into the output
+  int32_t* out_msg;          // with out_xyz, optional: the message of every output point (the X-ray stages' colours)
   int check_extent;
   float resolution;
   unsigned long long* counters;
@@ -78,6 +92,7 @@ struct Table {
   unsigned long long* keys;
   int32_t* hits;
   int32_t* rays;
+  float4* sums;              // optional per-slot payload (the X-ray table's column colour sums), moved by the rehash
   int64_t mask;
   int shift;
   int32_t* num_cells;
@@ -288,6 +303,24 @@ __global__ void __launch_bounds__(kBlock) mw_select(SelectArgs a) {
     a.out_xyz[3 * pos] = q.x;
     a.out_xyz[3 * pos + 1] = q.y;
     a.out_xyz[3 * pos + 2] = q.z;
+    if (a.out_msg) a.out_msg[pos] = m;
+  }
+}
+
+// the slot of `key`, inserting it if absent (*fresh: this thread's CAS inserted it)
+__device__ __forceinline__ int64_t claim(const Table& t, unsigned long long key, bool* fresh) {
+  *fresh = false;
+  for (int64_t s = slot_of(t, key);; s = (s + 1) & t.mask) {
+    unsigned long long k = t.keys[s];
+    if (k == kEmpty) {
+      k = atomicCAS(t.keys + s, kEmpty, key);
+      if (k == kEmpty) {
+        atomicAdd(t.num_cells, 1);
+        *fresh = true;
+        return s;
+      }
+    }
+    if (k == key) return s;
   }
 }
 
@@ -296,21 +329,8 @@ __global__ void __launch_bounds__(kBlock) mw_insert_hits(Table t, const float4* 
   const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   const float4 p = pts[i];
-  const unsigned long long key = cell_key(cell_index(Vec3f{p.x, p.y, p.z}, resolution));
-  for (int64_t s = slot_of(t, key);; s = (s + 1) & t.mask) {
-    unsigned long long k = t.keys[s];
-    if (k == kEmpty) {
-      k = atomicCAS(t.keys + s, kEmpty, key);
-      if (k == kEmpty) {
-        atomicAdd(t.num_cells, 1);
-        k = key;
-      }
-    }
-    if (k == key) {
-      atomicAdd(t.hits + s, 1);
-      return;
-    }
-  }
+  bool fresh;
+  atomicAdd(t.hits + claim(t, cell_key(cell_index(Vec3f{p.x, p.y, p.z}, resolution)), &fresh), 1);
 }
 
 __device__ __forceinline__ int64_t find(const Table& t, unsigned long long key) {
@@ -331,6 +351,7 @@ __global__ void __launch_bounds__(kBlock) mw_rehash(Table to, Table from, int64_
   while (atomicCAS(to.keys + s, kEmpty, key) != kEmpty) s = (s + 1) & to.mask;
   to.hits[s] = from.hits[i];
   to.rays[s] = from.rays[i];
+  if (to.sums) to.sums[s] = from.sums[i];
 }
 
 // pass 2 (ProcessInPhaseTwo): samples at x = 0, voxel_size, ... (< length, x a float advanced in double) along the ray from the
@@ -383,7 +404,7 @@ __global__ void __launch_bounds__(kBlock) mw_rays(Table t, const float4* pts, in
 // pass 3 (ProcessInPhaseThree): keep iff rays < 3 * hits (kMissPerHitLimit, compared in double); kind 0 counts, 1 scatters
 template <int kind>
 __global__ void __launch_bounds__(kBlock) mw_gate(Table t, const float4* pts, int64_t n, float resolution, int32_t* tiles,
-                                                  float* out_xyz) {
+                                                  float* out_xyz, int32_t* out_msg) {
   const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   bool keep = false;
   float4 p{};
@@ -410,6 +431,166 @@ __global__ void __launch_bounds__(kBlock) mw_gate(Table t, const float4* pts, in
   out_xyz[3 * pos] = p.x;
   out_xyz[3 * pos + 1] = p.y;
   out_xyz[3 * pos + 2] = p.z;
+  if (out_msg) out_msg[pos] = __float_as_int(p.w);
+}
+
+// ---- X-ray stages. Keys of the X-ray table: bit 46 voxel (1) or column (0), bits 42..45 the stage, bits 0..41 cell_key(x, y, z)
+// (x = -kGridHalf for a column). Per column slot: hits = points, rays = occupied voxels, sums = colour sums (r, g, b).
+constexpr int kMaxStages = DL_MAP_WRITER_MAX_STAGES;
+constexpr unsigned long long kVoxelBit = 1ull << 46;
+constexpr int kLogTable = 2 * kGridHalf;     // a column holds at most 16384 distinct voxels
+constexpr int64_t kXrayChunk = 1 << 21;      // points per insert: bounds the table's growth per reservation
+
+struct XrayStage {
+  Rigidf transform;
+  float resolution;
+  int32_t num_colors;        // colour stages added before this stage: colors[0, num_colors)
+  int32_t sum_index;         // index among the stages with colours, -1 for a stage without (its sums stay 0)
+};
+struct ColorStage {
+  int32_t frame;
+  float r, g, b;             // Uint8ComponentToFloat
+};
+struct XrayArgs {
+  const float* points;       // x y z of the final pass's output, in order
+  const int32_t* point_msg;  // message of every point
+  const MsgRec* msgs;
+  int64_t first, n;          // points [first, first + n) of the call
+  int num_stages;
+  XrayStage stages[kMaxStages];
+  ColorStage colors[kMaxStages];
+  int32_t sum_stage[kMaxStages];  // stage of every sum_index
+  int32_t* bbox;             // 6 per stage: min x y z, max x y z
+  unsigned long long* sort_keys;  // [sum_index * n + i]: sum_index << slot_bits | column slot
+  int32_t* sort_vals;        // point index
+  int slot_bits;
+  unsigned long long* outside;
+};
+
+__device__ __forceinline__ Int3 xray_cell(const XrayStage& s, float x, float y, float z) {
+  return cell_index(apply(s.transform, Vec3f{x, y, z}), s.resolution);
+}
+
+__global__ void __launch_bounds__(kBlock) mw_xray_check(XrayArgs a) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  bool outside = false;
+  if (i < a.n) {
+    const float* p = a.points + 3 * (a.first + i);
+    for (int s = 0; s < a.num_stages; ++s) outside |= !in_extent(xray_cell(a.stages[s], p[0], p[1], p[2]));
+  }
+  const int c = __syncthreads_count(outside);
+  if (threadIdx.x == 0 && c) atomicAdd(a.outside, (unsigned long long)c);
+}
+
+__global__ void __launch_bounds__(kBlock) mw_xray_insert(Table t, XrayArgs a) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  const bool active = i < a.n;
+  float x = 0.f, y = 0.f, z = 0.f;
+  if (active) {
+    const float* p = a.points + 3 * (a.first + i);
+    x = p[0]; y = p[1]; z = p[2];
+  }
+  for (int s = 0; s < a.num_stages; ++s) {
+    Int3 c{INT_MAX, INT_MAX, INT_MAX}, d{INT_MIN, INT_MIN, INT_MIN};
+    if (active) {
+      c = xray_cell(a.stages[s], x, y, z);
+      d = c;
+      const unsigned long long stage = (unsigned long long)s << 42;
+      bool fresh_voxel, fresh_column;
+      claim(t, kVoxelBit | stage | cell_key(c), &fresh_voxel);
+      const int64_t col = claim(t, stage | cell_key(Int3{-kGridHalf, c.y, c.z}), &fresh_column);
+      atomicAdd(t.hits + col, 1);
+      if (fresh_voxel) atomicAdd(t.rays + col, 1);
+      const int k = a.stages[s].sum_index;
+      if (k >= 0) {
+        a.sort_keys[k * a.n + i] = ((unsigned long long)k << a.slot_bits) | (unsigned long long)col;
+        a.sort_vals[k * a.n + i] = (int32_t)i;
+      }
+    }
+    // Eigen::AlignedBox3i::extend: integer min / max, one atomic per warp and bound
+    const int lo[3] = {__reduce_min_sync(0xffffffffu, c.x), __reduce_min_sync(0xffffffffu, c.y), __reduce_min_sync(0xffffffffu, c.z)};
+    const int hi[3] = {__reduce_max_sync(0xffffffffu, d.x), __reduce_max_sync(0xffffffffu, d.y), __reduce_max_sync(0xffffffffu, d.z)};
+    if ((threadIdx.x & 31) == 0 && lo[0] != INT_MAX) {
+      int32_t* box = a.bbox + 6 * s;
+      for (int k = 0; k < 3; ++k) {
+        atomicMin(box + k, lo[k]);
+        atomicMax(box + 3 + k, hi[k]);
+      }
+    }
+  }
+}
+
+// the colour stage `s` gives a point of frame `frame`: the last matching colour stage before it, else kDefaultColor
+__device__ __forceinline__ float4 point_color(const XrayArgs& a, int s, int32_t frame) {
+  for (int c = a.stages[s].num_colors - 1; c >= 0; --c)
+    if (a.colors[c].frame == frame) return make_float4(a.colors[c].r, a.colors[c].g, a.colors[c].b, 0.f);
+  return make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// one thread per run of equal sorted keys (one column of one stage): the run's points in stream order onto the float sums
+__global__ void __launch_bounds__(kBlock) mw_xray_fold(Table t, XrayArgs a, const unsigned long long* keys, const int32_t* vals,
+                                                       int64_t count) {
+  const int64_t j = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (j >= count || (j > 0 && keys[j - 1] == keys[j])) return;
+  const unsigned long long key = keys[j];
+  const int64_t slot = (int64_t)(key & ((1ull << a.slot_bits) - 1));
+  const int s = a.sum_stage[key >> a.slot_bits];
+  float4 sum = t.sums[slot];
+  for (int64_t k = j; k < count && keys[k] == key; ++k) {
+    const float4 c = point_color(a, s, a.msgs[a.point_msg[a.first + vals[k]]].frame);
+    sum.x += c.x;
+    sum.y += c.y;
+    sum.z += c.z;
+  }
+  t.sums[slot] = sum;
+}
+
+__global__ void __launch_bounds__(kBlock) mw_xray_max_voxels(Table t, int64_t cap, int stage, int32_t* max_voxels) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  int v = 0;
+  if (i < cap) {
+    const unsigned long long key = t.keys[i];
+    if (key != kEmpty && !(key & kVoxelBit) && (int)((key >> 42) & 15) == stage) v = t.rays[i];
+  }
+  v = __reduce_max_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0 && v) atomicMax(max_voxels, v);
+}
+
+// Mix (xray_points_processor.cc): a * (1. - t) in double, t * b in float, the sum in double, returned as float
+__device__ __forceinline__ float mix(float a, float b, float t) { return (float)((double)a * (1.0 - (double)t) + (double)(t * b)); }
+// FloatComponentToUint8: lround(Clamp(c, 0.f, 1.f) * 255), the product in float
+__device__ __forceinline__ uint32_t to_uint8(float c) {
+  const float v = c > 1.f ? 1.f : (c < 0.f ? 0.f : c);
+  return (uint32_t)(uint8_t)lroundf(v * 255.f);
+}
+
+// IntoImage: one thread per slot; the column pixels of the stage (the image starts white: empty columns)
+__global__ void __launch_bounds__(kBlock) mw_xray_pixels(Table t, int64_t cap, int stage, const double* log_n, float max_log,
+                                                         int max_y, int max_z, int width, uint32_t* argb) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (i >= cap) return;
+  const unsigned long long key = t.keys[i];
+  if (key == kEmpty || (key & kVoxelBit) || (int)((key >> 42) & 15) != stage) return;
+  const int y = (int)((key >> 14) & 0x3fff) - kGridHalf, z = (int)(key & 0x3fff) - kGridHalf;
+  const float count = (float)(uint32_t)t.hits[i];
+  const float4 sum = t.sums[i];
+  const float saturation = (float)(log_n[t.rays[i]] / (double)max_log);
+  const uint32_t r = to_uint8(mix(1.f, sum.x / count, saturation));
+  const uint32_t g = to_uint8(mix(1.f, sum.y / count, saturation));
+  const uint32_t b = to_uint8(mix(1.f, sum.z / count, saturation));
+  argb[(int64_t)(max_z - z) * width + (max_y - y)] = 0xFF000000u | r << 16 | g << 8 | b;  // Uint8ColorToCairo
+}
+
+// std::log(double n) for n = 0 .. kLogTable, glibc's (through a volatile pointer, never the compiler's folding)
+const std::vector<double>& log_table() {
+  static std::vector<double> table;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    double (*volatile glibc_log)(double) = ::log;
+    table.resize(kLogTable + 1);
+    for (int n = 0; n <= kLogTable; ++n) table[n] = glibc_log((double)n);
+  });
+  return table;
 }
 
 unsigned tiles_of(int64_t n) { return (unsigned)((n + kBlock - 1) / kBlock); }
@@ -441,6 +622,15 @@ struct dl_map_writer {
   Table table{};                   // cell -> (hits, rays)
   int64_t table_capacity = 0;
   int64_t num_cells = 0;
+  // X-ray and colour stages, in pipeline order
+  std::vector<XrayStage> xrays;
+  std::vector<ColorStage> colors;
+  std::vector<int32_t> sum_stage;  // stage of every sum_index
+  Table xray{};                    // voxel and column keys of every X-ray stage (see the key layout above), with colour sums
+  int64_t xray_capacity = 0;
+  int64_t xray_entries = 0;
+  int32_t* d_bbox = nullptr;       // 6 per stage
+  double* d_log = nullptr;         // log_table()
 
   int num_passes() const { return options.outlier_voxel_size > 0 ? 3 : 1; }
   bool final_pass() const { return pass == num_passes() - 1; }
@@ -472,7 +662,7 @@ struct dl_map_writer {
     runs_capacity = cap;
     return DL_OK;
   }
-  static int alloc_table(dl_context* ctx, int64_t cap, Table* t) {
+  static int alloc_table(dl_context* ctx, int64_t cap, bool sums, Table* t) {
     int shift = 64;
     for (int64_t c = cap; c > 1; c >>= 1) --shift;
     t->mask = cap - 1;
@@ -483,34 +673,81 @@ struct dl_map_writer {
     DL_CUDA(ctx, cudaMemsetAsync(t->keys, 0xff, (size_t)cap * sizeof(unsigned long long), ctx->stream));
     DL_CUDA(ctx, cudaMemsetAsync(t->hits, 0, (size_t)cap * sizeof(int32_t), ctx->stream));
     DL_CUDA(ctx, cudaMemsetAsync(t->rays, 0, (size_t)cap * sizeof(int32_t), ctx->stream));
+    if (sums) {
+      DL_CUDA(ctx, cudaMalloc(&t->sums, (size_t)cap * sizeof(float4)));
+      DL_CUDA(ctx, cudaMemsetAsync(t->sums, 0, (size_t)cap * sizeof(float4), ctx->stream));
+    }
     return DL_OK;
   }
   static void free_table(Table* t) {
     cudaFree(t->keys);
     cudaFree(t->hits);
     cudaFree(t->rays);
-    t->keys = nullptr; t->hits = nullptr; t->rays = nullptr;
+    cudaFree(t->sums);
+    t->keys = nullptr; t->hits = nullptr; t->rays = nullptr; t->sums = nullptr;
   }
-  // Load factor <= 1/2 after `adding` more cells: sized from the count of kept points before they are inserted.
-  int reserve_table(int64_t adding) {
+  // Load factor <= 1/2 after `adding` more entries: sized from a count of the points about to be inserted.
+  int reserve_table(Table* t, int64_t* capacity, int64_t used, int64_t adding, bool sums) {
     int64_t cap = 1024;
-    while (cap < 2 * (num_cells + adding)) cap <<= 1;
-    if (cap <= table_capacity) return DL_OK;
+    while (cap < 2 * (used + adding)) cap <<= 1;
+    if (cap <= *capacity) return DL_OK;
     Table fresh{};
-    const int st = alloc_table(ctx, cap, &fresh);
+    const int st = alloc_table(ctx, cap, sums, &fresh);
     if (st != DL_OK) {
       free_table(&fresh);
       return st;
     }
-    if (table_capacity > 0) {
-      mw_rehash<<<tiles_of(table_capacity), kBlock, 0, ctx->stream>>>(fresh, table, table_capacity);
+    if (*capacity > 0) {
+      mw_rehash<<<tiles_of(*capacity), kBlock, 0, ctx->stream>>>(fresh, *t, *capacity);
       DL_LAUNCH_CHECK(ctx, "mw_rehash");
     }
     DL_CUDA(ctx, ctx->wait_stream());
-    fresh.num_cells = table.num_cells;
-    free_table(&table);
-    table = fresh;
-    table_capacity = cap;
+    fresh.num_cells = t->num_cells;
+    free_table(t);
+    *t = fresh;
+    *capacity = cap;
+    return DL_OK;
+  }
+  int insert_xray(const float* points, const int32_t* point_msg, const MsgRec* msgs, int64_t n, void* sort_scratch,
+                  size_t sort_bytes, unsigned long long* keys, int32_t* vals, unsigned long long* outside);
+  XrayArgs xray_args() const {
+    XrayArgs a{};
+    a.num_stages = (int)xrays.size();
+    std::copy(xrays.begin(), xrays.end(), a.stages);
+    std::copy(colors.begin(), colors.end(), a.colors);
+    std::copy(sum_stage.begin(), sum_stage.end(), a.sum_stage);
+    a.bbox = d_bbox;
+    return a;
+  }
+  // the X-ray table, the bounding boxes and the log table, at the first X-ray stage
+  int init_xray() {
+    if (xray.num_cells) return DL_OK;
+    DL_CUDA(ctx, cudaSetDevice(ctx->device));
+    std::vector<int32_t> box(6 * kMaxStages);
+    for (int s = 0; s < kMaxStages; ++s)
+      for (int k = 0; k < 3; ++k) {
+        box[6 * s + k] = INT_MAX;
+        box[6 * s + 3 + k] = INT_MIN;
+      }
+    const std::vector<double>& logs = log_table();
+    int32_t* counter = nullptr;
+    int32_t* bbox = nullptr;
+    double* logs_dev = nullptr;
+    cudaError_t e = cudaMalloc(&counter, sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&bbox, box.size() * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&logs_dev, logs.size() * sizeof(double));
+    if (e == cudaSuccess) e = cudaMemset(counter, 0, sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMemcpy(bbox, box.data(), box.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(logs_dev, logs.data(), logs.size() * sizeof(double), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      cudaFree(counter);
+      cudaFree(bbox);
+      cudaFree(logs_dev);
+      return ctx->cuda_fail(e, "dl_map_writer_add_xray");
+    }
+    xray.num_cells = counter;
+    d_bbox = bbox;
+    d_log = logs_dev;
     return DL_OK;
   }
   int process(int32_t num_messages, const dl_map_message* messages, const float* rows_host, const float* rows_dev,
@@ -544,7 +781,7 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
     if (g.first_row < 0 || g.num_rows < 0 || g.first_row > num_rows || g.num_rows > num_rows - g.first_row)
       return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: message rows outside the row buffer");
     if (!valid_pose7(g.sensor_to_tracking)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: sensor_to_tracking is not finite");
-    msgs[m] = MsgRec{g.stamp, g.first_row, n, it->second, 0, pose_from7(g.sensor_to_tracking)};
+    msgs[m] = MsgRec{g.stamp, g.first_row, n, it->second, g.frame_id, pose_from7(g.sensor_to_tracking)};
     n += g.num_rows;
   }
   if (n >= (1ll << 31)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: more than 2^31 - 1 rows in one call");
@@ -572,7 +809,26 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   int32_t* d_ints = nullptr;  // [0] runs, [1] kept, [2] gate survivors
   float* d_out = nullptr;
   int32_t* gate_tiles = nullptr;
+  // X-ray stages: the message of every output point, and the sort of one chunk's (stage, column) keys
+  const bool with_xray = final_pass() && !xrays.empty();
+  const int64_t sort_items = with_xray ? std::min<int64_t>(n, kXrayChunk) * (int64_t)sum_stage.size() : 0;
+  size_t sort_bytes = 0;
+  if (sort_items > 0) {
+    cub::DoubleBuffer<unsigned long long> k(nullptr, nullptr);
+    cub::DoubleBuffer<int32_t> v(nullptr, nullptr);
+    DL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k, v, (int)sort_items, 0, 64, ctx->stream));
+  }
+  int32_t* out_msg = nullptr;
+  unsigned long long* sort_keys = nullptr;
+  int32_t* sort_vals = nullptr;
+  void* sort_scratch = nullptr;
   MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+    if (with_xray) {
+      out_msg = ar.take<int32_t>((size_t)n);
+      sort_keys = ar.take<unsigned long long>(2 * (size_t)sort_items);
+      sort_vals = ar.take<int32_t>(2 * (size_t)sort_items);
+      sort_scratch = ar.take<char>(sort_bytes);
+    }
     if (rows_host) up_rows = ar.take<float4>((size_t)num_rows);
     d_msgs = ar.take<MsgRec>((size_t)num_messages);
     a.head_tiles = ar.take<int32_t>(tiles);
@@ -635,6 +891,7 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   if (direct) {
     s.compact = nullptr;
     s.out_xyz = d_out;
+    s.out_msg = out_msg;
   }
   mw_select<1><<<tiles, kBlock, 0, ctx->stream>>>(s);
   DL_LAUNCH_CHECK(ctx, "mw_select<1>");
@@ -656,7 +913,7 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   local.dropped_range = (int64_t)counters[kRange];
   local.messages_without_batch = std::count(last_run.begin(), last_run.end(), -1);
 
-  if (options.outlier_voxel_size > 0) MW_TRY(reserve_table(pass == 0 ? kept : 0));
+  if (options.outlier_voxel_size > 0) MW_TRY(reserve_table(&table, &table_capacity, num_cells, pass == 0 ? kept : 0, false));
   int64_t out_count = 0;
   if (direct) {
     out_count = kept;
@@ -673,11 +930,11 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
     }
   } else if (kept > 0) {
     const unsigned gt = tiles_of(kept);
-    mw_gate<0><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, nullptr);
+    mw_gate<0><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, nullptr, nullptr);
     DL_LAUNCH_CHECK(ctx, "mw_gate<0>");
     mw_tile_prefix<<<1, kBlock, 0, ctx->stream>>>(gate_tiles, (int)gt, d_ints + 2);
     DL_LAUNCH_CHECK(ctx, "mw_tile_prefix");
-    mw_gate<1><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, d_out);
+    mw_gate<1><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, d_out, out_msg);
     DL_LAUNCH_CHECK(ctx, "mw_gate<1>");
     int32_t survivors = 0;
     DL_CUDA(ctx, cudaMemcpyAsync(&survivors, d_ints + 2, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -685,6 +942,8 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
     out_count = survivors;
     local.dropped_moving = kept - survivors;
   }
+  if (with_xray && out_count > 0)
+    MW_TRY(insert_xray(d_out, out_msg, d_msgs, out_count, sort_scratch, sort_bytes, sort_keys, sort_vals, a.counters + kOutside));
   DL_CUDA(ctx, cudaMemcpyAsync(counters, a.counters, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
   int32_t cells = 0;
   if (table.num_cells) DL_CUDA(ctx, cudaMemcpyAsync(&cells, table.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -697,6 +956,57 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   *num_points_out = out_count;
   started = true;
   if (info) *info = local;
+  return DL_OK;
+}
+
+// The final pass's output points [0, n) of one call into every X-ray stage. Every cell is checked before anything changes; then
+// chunks of kXrayChunk points, each with its table reservation (two new entries per point and stage at most), insert, sort and
+// fold, so that the colour sums take the points in stream order across chunks and calls.
+int dl_map_writer::insert_xray(const float* points, const int32_t* point_msg, const MsgRec* msgs, int64_t n, void* sort_scratch,
+                               size_t sort_bytes, unsigned long long* keys, int32_t* vals, unsigned long long* outside) {
+  XrayArgs a = xray_args();
+  a.points = points;
+  a.point_msg = point_msg;
+  a.msgs = msgs;
+  a.outside = outside;
+  a.n = n;
+  DL_CUDA(ctx, cudaMemsetAsync(outside, 0, sizeof(unsigned long long), ctx->stream));
+  mw_xray_check<<<tiles_of(n), kBlock, 0, ctx->stream>>>(a);
+  DL_LAUNCH_CHECK(ctx, "mw_xray_check");
+  unsigned long long num_outside = 0;
+  DL_CUDA(ctx, cudaMemcpyAsync(&num_outside, outside, sizeof(num_outside), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  if (num_outside > 0)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: a point's X-ray cell lies beyond +-8192 cells (the hybrid grid's largest "
+                                 "extent)");
+  const int64_t num_sums = (int64_t)sum_stage.size();
+  const int64_t items_cap = std::min<int64_t>(n, kXrayChunk) * num_sums;  // the carve's size of each sort buffer
+  int sum_bits = 0;
+  while ((1 << sum_bits) < num_sums) ++sum_bits;
+  for (int64_t first = 0; first < n; first += kXrayChunk) {
+    const int64_t m = std::min(kXrayChunk, n - first);
+    MW_TRY(reserve_table(&xray, &xray_capacity, xray_entries, 2 * m * (int64_t)xrays.size(), true));
+    a.first = first;
+    a.n = m;
+    a.slot_bits = 64 - xray.shift;
+    a.sort_keys = keys;
+    a.sort_vals = vals;
+    mw_xray_insert<<<tiles_of(m), kBlock, 0, ctx->stream>>>(xray, a);
+    DL_LAUNCH_CHECK(ctx, "mw_xray_insert");
+    if (num_sums > 0) {
+      const int items = (int)(m * num_sums);
+      cub::DoubleBuffer<unsigned long long> k(keys, keys + items_cap);
+      cub::DoubleBuffer<int32_t> v(vals, vals + items_cap);
+      // the scratch was sized for all 64 bits and items_cap items, the most any chunk sorts
+      DL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(sort_scratch, sort_bytes, k, v, items, 0, a.slot_bits + sum_bits, ctx->stream));
+      mw_xray_fold<<<tiles_of(items), kBlock, 0, ctx->stream>>>(xray, a, k.Current(), v.Current(), items);
+      DL_LAUNCH_CHECK(ctx, "mw_xray_fold");
+    }
+    int32_t entries = 0;
+    DL_CUDA(ctx, cudaMemcpyAsync(&entries, xray.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
+    xray_entries = entries;
+  }
   return DL_OK;
 }
 
@@ -735,6 +1045,10 @@ void dl_map_writer_destroy(dl_map_writer* w) {
   cudaStreamSynchronize(w->ctx->stream);
   dl_map_writer::free_table(&w->table);
   cudaFree(w->table.num_cells);
+  dl_map_writer::free_table(&w->xray);
+  cudaFree(w->xray.num_cells);
+  cudaFree(w->d_bbox);
+  cudaFree(w->d_log);
   cudaFree(w->d_runs);
   cudaFree(w->d_times);
   cudaFree(w->d_nodes);
@@ -834,5 +1148,87 @@ int dl_map_writer_voxels(const dl_map_writer* w, int64_t capacity, int32_t* cell
     rays[k] = r[order[k]];
   }
   *count = (int64_t)order.size();
+  return DL_OK;
+}
+
+int dl_map_writer_add_color(dl_map_writer* w, const dl_map_writer_color* color) {
+  if (!w) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  if (!color) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_color: bad arguments");
+  if (w->started || w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_color: processing has begun");
+  if ((int)(w->xrays.size() + w->colors.size()) >= kMaxStages)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_color: more than DL_MAP_WRITER_MAX_STAGES stages");
+  // ToFloatColor: Uint8ComponentToFloat(c) = c / 255.f
+  w->colors.push_back(ColorStage{color->frame_id, color->rgb[0] / 255.f, color->rgb[1] / 255.f, color->rgb[2] / 255.f});
+  return DL_OK;
+}
+
+int dl_map_writer_add_xray(dl_map_writer* w, const dl_map_writer_xray* xray, int32_t* stage) {
+  if (!w) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  if (!xray || !stage) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: bad arguments");
+  if (w->started || w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: processing has begun");
+  if ((int)(w->xrays.size() + w->colors.size()) >= kMaxStages)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: more than DL_MAP_WRITER_MAX_STAGES stages");
+  if (!(xray->voxel_size > 0) || !std::isfinite(xray->voxel_size) || !((float)xray->voxel_size > 0.f))
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: voxel_size must be finite and > 0");
+  if (!valid_pose7(xray->transform)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: transform is not finite");
+  const double* q = xray->transform + 3;  // Eigen's squaredNorm order
+  const double norm = std::sqrt(q[1] * q[1] + q[2] * q[2] + q[3] * q[3] + q[0] * q[0]);
+  if (!(std::fabs(norm - 1.0) <= 1e-9)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: the rotation is not a unit quaternion");
+  MW_TRY(w->init_xray());
+  XrayStage s{};
+  s.transform = to_float(pose_from7(xray->transform));
+  s.resolution = (float)xray->voxel_size;
+  s.num_colors = (int32_t)w->colors.size();
+  s.sum_index = -1;
+  if (s.num_colors > 0) {
+    s.sum_index = (int32_t)w->sum_stage.size();
+    w->sum_stage.push_back((int32_t)w->xrays.size());
+  }
+  *stage = (int32_t)w->xrays.size();
+  w->xrays.push_back(s);
+  return DL_OK;
+}
+
+int dl_map_writer_xray_image(const dl_map_writer* w, int32_t stage, int64_t capacity, uint32_t* argb, int32_t* width,
+                             int32_t* height) {
+  if (!w || !width || !height) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  if (stage < 0 || stage >= (int32_t)w->xrays.size()) return ctx->fail(DL_ERR_ARG, "dl_map_writer_xray_image: unknown stage");
+  if (!w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_xray_image: the final pass has not been flushed");
+  int32_t box[6];
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  DL_CUDA(ctx, cudaMemcpy(box, w->d_bbox + 6 * stage, sizeof(box), cudaMemcpyDeviceToHost));
+  const bool empty = box[1] > box[4];  // Eigen::AlignedBox::isEmpty
+  const int32_t wd = empty ? 0 : box[4] - box[1] + 1, ht = empty ? 0 : box[5] - box[2] + 1;
+  *width = wd;
+  *height = ht;
+  if (!argb || empty) return DL_OK;
+  const int64_t pixels = (int64_t)wd * ht;
+  if (capacity < pixels) return ctx->fail(DL_ERR_ARG, "dl_map_writer_xray_image: capacity below width * height");
+  int32_t* d_max = nullptr;
+  uint32_t* d_img = nullptr;
+  MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+    d_max = ar.take<int32_t>(1);
+    d_img = ar.take<uint32_t>((size_t)pixels);
+  }));
+  const unsigned tiles = tiles_of(w->xray_capacity);
+  DL_CUDA(ctx, cudaMemsetAsync(d_max, 0, sizeof(int32_t), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(d_img, 0xff, (size_t)pixels * sizeof(uint32_t), ctx->stream));  // white
+  mw_xray_max_voxels<<<tiles, kBlock, 0, ctx->stream>>>(w->xray, w->xray_capacity, stage, d_max);
+  DL_LAUNCH_CHECK(ctx, "mw_xray_max_voxels");
+  int32_t max_voxels = 0;
+  DL_CUDA(ctx, cudaMemcpyAsync(&max_voxels, d_max, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  // IntoImage: max starts at numeric_limits<float>::min() and takes std::max<float>(max, log(n)); log is monotone, so the
+  // largest n gives the largest (float)log(n)
+  const float max_log = std::max<float>(FLT_MIN, (float)log_table()[max_voxels]);
+  mw_xray_pixels<<<tiles, kBlock, 0, ctx->stream>>>(w->xray, w->xray_capacity, stage, w->d_log, max_log, box[4], box[5], wd,
+                                                     d_img);
+  DL_LAUNCH_CHECK(ctx, "mw_xray_pixels");
+  DL_CUDA(ctx, cudaMemcpyAsync(argb, d_img, (size_t)pixels * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
   return DL_OK;
 }

@@ -4,7 +4,9 @@ The product is the shared library; this module only marshals numpy arrays into i
 There is no fallback: if the library is missing, or no CUDA device is present, calls raise.
 """
 import ctypes as C
+import math
 import os
+import struct
 
 import numpy as np
 
@@ -39,7 +41,8 @@ EXPORTS = [
     "dl_pose_graph_3d_run_final_optimization", "dl_pose_graph_3d_poses", "dl_pose_graph_3d_local_to_global",
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
     "dl_map_writer_create", "dl_map_writer_destroy", "dl_map_writer_add_trajectory", "dl_map_writer_process",
-    "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels",
+    "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels", "dl_map_writer_add_color",
+    "dl_map_writer_add_xray", "dl_map_writer_xray_image",
     "dl_submap_textures", "dl_submap_projections",
 ]
 
@@ -369,7 +372,15 @@ class MapWriterOptions(C.Structure):   # dl_map_writer_options
 
 class MapMessage(C.Structure):   # dl_map_message
     _fields_ = [("stamp", C.c_int64), ("first_row", C.c_int64), ("num_rows", C.c_int64), ("trajectory_id", C.c_int32),
-                ("reserved", C.c_int32), ("sensor_to_tracking", C.c_double * 7)]
+                ("frame_id", C.c_int32), ("sensor_to_tracking", C.c_double * 7)]
+
+
+class MapWriterColor(C.Structure):   # dl_map_writer_color
+    _fields_ = [("frame_id", C.c_int32), ("rgb", C.c_uint8 * 3), ("pad", C.c_uint8)]
+
+
+class MapWriterXray(C.Structure):   # dl_map_writer_xray
+    _fields_ = [("voxel_size", C.c_double), ("transform", C.c_double * 7)]
 
 
 class MapWriterInfo(C.Structure):   # dl_map_writer_info
@@ -522,6 +533,9 @@ def lib():
     L.dl_map_writer_process_dev.argtypes = [vp, C.c_int32, vp, vp, C.c_int64, vp, ip(C.c_int64), vp, ip(MapWriterInfo)]
     L.dl_map_writer_flush.argtypes = [vp, ip(C.c_int32)]
     L.dl_map_writer_voxels.argtypes = [vp, C.c_int64, vp, vp, vp, ip(C.c_int64)]
+    L.dl_map_writer_add_color.argtypes = [vp, ip(MapWriterColor)]
+    L.dl_map_writer_add_xray.argtypes = [vp, ip(MapWriterXray), ip(C.c_int32)]
+    L.dl_map_writer_xray_image.argtypes = [vp, C.c_int32, C.c_int64, vp, ip(C.c_int32), ip(C.c_int32)]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
     L.dl_submap_textures.argtypes = [vp, C.c_int32, ip(SubmapImageQuery), ip(SubmapTexture), C.c_int64, vp, ip(C.c_int64)]
     L.dl_submap_projections.argtypes = [vp, C.c_int32, ip(SubmapImageQuery), ip(SubmapProjection), C.c_int64, vp,
@@ -1357,12 +1371,41 @@ class MapWriter:
         """A PoseGraph3D trajectory: its node poses (GetTrajectoryNodePoses) at the nodes' times, converted with seconds_to_ticks."""
         self.add_trajectory(trajectory_id, seconds_to_ticks(node_times_seconds), graph.node_poses(trajectory_id))
 
+    def add_color(self, frame_id, rgb):
+        """color_points: messages whose frame_id (an integer) equals this one get every point coloured rgb / 255.f; rgb are
+        the Lua values, converted with static_cast<uint8>. Added before processing begins, in pipeline order."""
+        c = MapWriterColor()
+        c.frame_id = int(frame_id)
+        c.rgb[:] = [int(v) & 0xFF for v in rgb]
+        self.ctx.check(self.ctx.L.dl_map_writer_add_color(self.h, C.byref(c)))
+
+    def add_xray(self, voxel_size, transform7):
+        """write_xray_image of the final pass's points (transform: Rigid3d t, q wxyz) -> the stage number for xray_image()."""
+        x = MapWriterXray()
+        x.voxel_size = float(voxel_size)
+        x.transform[:] = [float(v) for v in transform7]
+        stage = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_map_writer_add_xray(self.h, C.byref(x), C.byref(stage)))
+        return stage.value
+
+    def xray_image(self, stage):
+        """After the final flush: (height, width) uint32 Cairo ARGB32 words, (0, 0) for an empty bounding box."""
+        w, h = C.c_int32(0), C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_map_writer_xray_image(self.h, int(stage), 0, None, C.byref(w), C.byref(h)))
+        img = np.zeros((h.value, w.value), np.uint32)
+        if img.size:
+            self.ctx.check(self.ctx.L.dl_map_writer_xray_image(self.h, int(stage), img.size, img.ctypes.data, C.byref(w),
+                                                               C.byref(h)))
+        return img
+
     @staticmethod
     def messages(msgs):
-        """[(stamp ticks, first_row, num_rows, trajectory_id, sensor_to_tracking7)] -> a dl_map_message array"""
+        """[(stamp ticks, first_row, num_rows, trajectory_id, sensor_to_tracking7[, frame_id])] -> a dl_map_message array"""
         arr = (MapMessage * max(len(msgs), 1))()
-        for k, (stamp, first, n, traj, s2t) in enumerate(msgs):
+        for k, msg in enumerate(msgs):
+            stamp, first, n, traj, s2t = msg[:5]
             arr[k].stamp, arr[k].first_row, arr[k].num_rows, arr[k].trajectory_id = int(stamp), int(first), int(n), int(traj)
+            arr[k].frame_id = int(msg[5]) if len(msg) > 5 else 0
             arr[k].sensor_to_tracking[:] = [float(v) for v in s2t]
         return arr
 
@@ -1421,6 +1464,78 @@ def write_pcd(path, points):
     with open(path, "wb") as f:
         f.write(header.encode())
         f.write(pts.tobytes())
+
+
+def roll_pitch_yaw(roll, pitch, yaw):
+    """transform::RollPitchYaw (transform/rigid_transform.cc:40-46): AngleAxisd(yaw, Z) * AngleAxisd(pitch, Y) *
+    AngleAxisd(roll, X), each AngleAxis (cos(a/2), sin(a/2) * axis), the products in Eigen's order -> (w, x, y, z)."""
+    def product(a, b):
+        aw, ax, ay, az = a
+        bw, bx, by, bz = b
+        return (aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+                aw * by + ay * bw + az * bx - ax * bz, aw * bz + az * bw + ax * by - ay * bx)
+    r = (math.cos(0.5 * roll), math.sin(0.5 * roll), 0.0, 0.0)
+    p = (math.cos(0.5 * pitch), 0.0, math.sin(0.5 * pitch), 0.0)
+    y = (math.cos(0.5 * yaw), 0.0, 0.0, math.sin(0.5 * yaw))
+    return product(product(y, p), r)
+
+
+def png_bytes(argb):
+    """An 8-bit RGB PNG (colour type 2, every X-ray pixel is opaque) of (height, width) Cairo ARGB32 words: filter 0 on every
+    row, a zlib stream of stored deflate blocks (at most 65535 bytes each), one IDAT chunk. The same bytes as
+    io::WritePng (dliom_b200.hpp)."""
+    img = np.ascontiguousarray(argb, np.uint32)
+    h, w = img.shape
+    if h == 0 or w == 0:
+        raise ValueError("png_bytes: an empty image has no PNG")
+    rgb = np.stack([(img >> 16) & 0xFF, (img >> 8) & 0xFF, img & 0xFF], axis=-1).astype(np.uint8)
+    raw = np.concatenate([np.zeros((h, 1), np.uint8), rgb.reshape(h, 3 * w)], axis=1).tobytes()
+    blocks = [raw[k:k + 65535] for k in range(0, len(raw), 65535)]
+    z = bytearray(b"\x78\x01")
+    for k, b in enumerate(blocks):
+        z += struct.pack("<BHH", int(k == len(blocks) - 1), len(b), len(b) ^ 0xFFFF) + b
+    z += struct.pack(">I", _adler32(raw))
+
+    def chunk(kind, data):
+        return struct.pack(">I", len(data)) + kind + data + struct.pack(">I", _crc32(kind + data))
+    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 2, 0, 0, 0)) + chunk(b"IDAT", bytes(z))
+            + chunk(b"IEND", b""))
+
+
+def write_png(path, argb):
+    """png_bytes(argb) into path."""
+    data = png_bytes(argb)
+    with open(path, "wb") as f:
+        f.write(data)
+
+
+_CRC_TABLE = None
+
+
+def _crc32(data):
+    """CRC-32 of PNG (ISO 3309, reflected polynomial 0xEDB88320), table-driven."""
+    global _CRC_TABLE
+    if _CRC_TABLE is None:
+        t = np.arange(256, dtype=np.uint32)
+        for _ in range(8):
+            t = np.where(t & 1, np.uint32(0xEDB88320) ^ (t >> 1), t >> 1).astype(np.uint32)
+        _CRC_TABLE = [int(v) for v in t]
+    c = 0xFFFFFFFF
+    for b in data:
+        c = _CRC_TABLE[(c ^ b) & 0xFF] ^ (c >> 8)
+    return c ^ 0xFFFFFFFF
+
+
+def _adler32(data):
+    """Adler-32 of zlib (RFC 1950): sums modulo 65521, over blocks of 5552 bytes so that int64 sums cannot overflow."""
+    a, b = 1, 0
+    arr = np.frombuffer(data, np.uint8).astype(np.int64)
+    for k in range(0, len(arr), 5552):
+        blk = arr[k:k + 5552]
+        n = len(blk)
+        b = (b + n * a + int(np.dot(np.arange(n, 0, -1, dtype=np.int64), blk))) % 65521
+        a = (a + int(blk.sum())) % 65521
+    return (b << 16) | a
 
 
 def comm_unique_id():

@@ -8,12 +8,15 @@
 //   mapping::RangeDataSynchronizer                           C/mapping/internal/3d/range_data_synchronizer.h:30-68
 //   mapping::LocalTrajectoryBuilder3D                        C/mapping/internal/3d/local_trajectory_builder_3d.h:81-113
 //   io::MapWriter, io::PcdWritingPointsProcessor             cartographer_ros/assets_writer.cc:120-160, C/io/*_points_processor.cc
+//   io::ColoringPointsProcessor, io::XRayPointsProcessor     C/io/coloring_points_processor.cc, C/io/xray_points_processor.cc
+//   transform::RollPitchYaw                                  C/transform/rigid_transform.cc:40-46
 // Eigen / protobuf types are replaced by the plain structs below (this image has neither); INTEGRATION.md shows
 // the three-line adapters for Eigen::Vector3f / transform::Rigid3d / proto options in a real Cartographer tree.
 // Errors: the reference CHECK-aborts; this shim throws dliom::Error carrying the C-ABI status and message.
 #pragma once
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -917,6 +920,23 @@ class PoseGraph3D {
 
 }  // namespace mapping
 
+namespace transform {
+
+// RollPitchYaw (transform/rigid_transform.cc:40-46): AngleAxisd(yaw, Z) * AngleAxisd(pitch, Y) * AngleAxisd(roll, X), each angle
+// axis as (cos(a / 2), sin(a / 2) * axis), multiplied in Eigen's quaternion-product order. Returns (w, x, y, z).
+inline std::array<double, 4> RollPitchYaw(double roll, double pitch, double yaw) {
+  auto product = [](const std::array<double, 4>& a, const std::array<double, 4>& b) -> std::array<double, 4> {
+    return {a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3], a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2],
+            a[0] * b[2] + a[2] * b[0] + a[3] * b[1] - a[1] * b[3], a[0] * b[3] + a[3] * b[0] + a[1] * b[2] - a[2] * b[1]};
+  };
+  const std::array<double, 4> r = {std::cos(0.5 * roll), std::sin(0.5 * roll), 0.0, 0.0};
+  const std::array<double, 4> p = {std::cos(0.5 * pitch), 0.0, std::sin(0.5 * pitch), 0.0};
+  const std::array<double, 4> y = {std::cos(0.5 * yaw), 0.0, 0.0, std::sin(0.5 * yaw)};
+  return product(product(y, p), r);
+}
+
+}  // namespace transform
+
 namespace io {
 
 // The assets writer's processors (cartographer_ros/assets_writer.cc with the fork's assets_writer_tongji.lua), on the device in
@@ -936,6 +956,7 @@ struct MapWriterOptions {
 struct Message {  // one sensor message = one PointsBatch: x y z t rows (t in seconds, relative to stamp), sensor frame
   int64_t stamp = 0;  // universal ticks (common::ToUniversal)
   int trajectory_id = 0;
+  std::string frame_id;  // PointsBatch::frame_id: what color_points stages match, exactly
   Rigid3d sensor_to_tracking;
   TimedPointCloud rows;
 };
@@ -970,6 +991,7 @@ class MapWriter {
       m[k].first_row = (int64_t)rows.size();
       m[k].num_rows = (int64_t)messages[k].rows.size();
       m[k].trajectory_id = messages[k].trajectory_id;
+      m[k].frame_id = FrameId(messages[k].frame_id);
       messages[k].sensor_to_tracking.to7(m[k].sensor_to_tracking);
       rows.insert(rows.end(), messages[k].rows.begin(), messages[k].rows.end());
     }
@@ -986,11 +1008,137 @@ class MapWriter {
     return restart ? FlushResult::kRestartStream : FlushResult::kFinished;
   }
   const dl_map_writer_info& last_info() const { return last_info_; }
+  // Stages after the final multi-pass stage, added before the first Process in pipeline order (what ColoringPointsProcessor
+  // and XRayPointsProcessor call).
+  void AddColor(const std::string& frame_id, const std::array<uint8_t, 3>& rgb) {
+    dl_map_writer_color c{};
+    c.frame_id = FrameId(frame_id);
+    for (int i = 0; i < 3; ++i) c.rgb[i] = rgb[i];
+    ctx_->check(dl_map_writer_add_color(writer_, &c));
+  }
+  int AddXRay(double voxel_size, const Rigid3d& transform) {
+    dl_map_writer_xray x{};
+    x.voxel_size = voxel_size;
+    transform.to7(x.transform);
+    int32_t stage = 0;
+    ctx_->check(dl_map_writer_add_xray(writer_, &x, &stage));
+    return stage;
+  }
+  // After the final Flush: Cairo ARGB32 words, row-major; 0 x 0 for an empty bounding box.
+  std::vector<uint32_t> XRayImage(int stage, int* width, int* height) const {
+    int32_t w = 0, h = 0;
+    ctx_->check(dl_map_writer_xray_image(writer_, stage, 0, nullptr, &w, &h));
+    std::vector<uint32_t> argb((size_t)w * (size_t)h);
+    if (!argb.empty()) ctx_->check(dl_map_writer_xray_image(writer_, stage, (int64_t)argb.size(), argb.data(), &w, &h));
+    *width = w;
+    *height = h;
+    return argb;
+  }
 
  private:
+  // PointsBatch::frame_id strings as the C-ABI's integers: equal strings, equal integers
+  int32_t FrameId(const std::string& frame_id) {
+    const auto it = frame_ids_.emplace(frame_id, (int32_t)frame_ids_.size()).first;
+    return it->second;
+  }
   Context* ctx_;
   dl_map_writer* writer_ = nullptr;
   dl_map_writer_info last_info_{};
+  std::map<std::string, int32_t> frame_ids_;
+};
+
+// io::ColoringPointsProcessor (io/coloring_points_processor.cc): batches of `frame_id` get `color` (the Lua values after
+// static_cast<uint8>) for the X-ray stages added after it.
+class ColoringPointsProcessor {
+ public:
+  ColoringPointsProcessor(MapWriter* writer, const std::array<uint8_t, 3>& color, const std::string& frame_id) {
+    writer->AddColor(frame_id, color);
+  }
+};
+
+// PNG bytes of an X-ray image: 8-bit RGB (colour type 2: every pixel is opaque), filter 0 on every row, one IDAT chunk holding a
+// zlib stream of stored deflate blocks, CRC-32 and Adler-32 computed here. The same bytes as dliom.png_bytes.
+inline std::vector<uint8_t> PngBytes(const std::vector<uint32_t>& argb, int width, int height) {
+  auto be32 = [](std::vector<uint8_t>* out, uint32_t v) {
+    for (int s = 24; s >= 0; s -= 8) out->push_back((uint8_t)(v >> s));
+  };
+  std::vector<uint8_t> raw;
+  raw.reserve((size_t)height * (1 + 3 * (size_t)width));
+  for (int y = 0; y < height; ++y) {
+    raw.push_back(0);
+    for (int x = 0; x < width; ++x) {
+      const uint32_t c = argb[(size_t)y * width + x];
+      raw.push_back((uint8_t)(c >> 16));
+      raw.push_back((uint8_t)(c >> 8));
+      raw.push_back((uint8_t)c);
+    }
+  }
+  std::vector<uint8_t> z = {0x78, 0x01};
+  for (size_t k = 0; k < raw.size(); k += 65535) {
+    const size_t n = std::min<size_t>(65535, raw.size() - k);
+    z.push_back(k + n >= raw.size() ? 1 : 0);
+    z.push_back((uint8_t)n);
+    z.push_back((uint8_t)(n >> 8));
+    z.push_back((uint8_t)~n);
+    z.push_back((uint8_t)(~n >> 8));
+    z.insert(z.end(), raw.begin() + k, raw.begin() + k + n);
+  }
+  uint32_t a = 1, b = 0;  // Adler-32
+  for (uint8_t v : raw) {
+    a = (a + v) % 65521;
+    b = (b + a) % 65521;
+  }
+  be32(&z, b << 16 | a);
+  uint32_t table[256];  // CRC-32, reflected polynomial 0xEDB88320
+  for (uint32_t n = 0; n < 256; ++n) {
+    uint32_t c = n;
+    for (int k = 0; k < 8; ++k) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+    table[n] = c;
+  }
+  std::vector<uint8_t> png = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1a, '\n'};
+  auto chunk = [&](const char* kind, const std::vector<uint8_t>& data) {
+    be32(&png, (uint32_t)data.size());
+    const size_t start = png.size();
+    png.insert(png.end(), kind, kind + 4);
+    png.insert(png.end(), data.begin(), data.end());
+    uint32_t c = 0xFFFFFFFFu;
+    for (size_t i = start; i < png.size(); ++i) c = table[(c ^ png[i]) & 0xFF] ^ (c >> 8);
+    be32(&png, c ^ 0xFFFFFFFFu);
+  };
+  std::vector<uint8_t> ihdr;
+  be32(&ihdr, (uint32_t)width);
+  be32(&ihdr, (uint32_t)height);
+  ihdr.insert(ihdr.end(), {8, 2, 0, 0, 0});
+  chunk("IHDR", ihdr);
+  chunk("IDAT", z);
+  chunk("IEND", {});
+  return png;
+}
+
+// io::XRayPointsProcessor (io/xray_points_processor.cc) with draw_trajectories = false and without separate_floors: the final
+// pass's points seen through `transform` at `voxel_size`; Flush, after the writer's final Flush, writes <output_filename>.png
+// (nothing for an empty bounding box, where the reference only warns).
+class XRayPointsProcessor {
+ public:
+  XRayPointsProcessor(MapWriter* writer, double voxel_size, const Rigid3d& transform, const std::string& output_filename)
+      : writer_(writer), stage_(writer->AddXRay(voxel_size, transform)), output_filename_(output_filename) {}
+  void Flush() const {
+    int width = 0, height = 0;
+    const std::vector<uint32_t> argb = writer_->XRayImage(stage_, &width, &height);
+    if (argb.empty()) return;
+    const std::vector<uint8_t> png = PngBytes(argb, width, height);
+    const std::string path = output_filename_ + ".png";
+    std::FILE* f = std::fopen(path.c_str(), "wb");
+    if (!f) throw Error(DL_ERR_ARG, "cannot open " + path);
+    const bool ok = std::fwrite(png.data(), 1, png.size(), f) == png.size();
+    if (std::fclose(f) != 0 || !ok) throw Error(DL_ERR_ARG, "PNG write failed: " + path);
+  }
+  int stage() const { return stage_; }
+
+ private:
+  MapWriter* writer_;
+  int stage_;
+  std::string output_filename_;
 };
 
 // io::PcdWritingPointsProcessor (io/pcd_writing_points_processor.cc:35-130): binary PCD v0.7, x y z floats, no colour. The header

@@ -896,8 +896,10 @@ int dl_submap_projections(dl_context* ctx, int32_t count, const dl_submap_image_
  *      Rejected with DL_ERR_ARG, the writer unchanged: an unknown trajectory, a trajectory added twice or after processing began,
  *      rows outside [0, num_rows), a call after the final flush, and (pass 1) a kept point whose cell lies beyond the hybrid
  *      grid's largest extent, +-8192 cells per axis (the reference's grid CHECK-fails there, hybrid_grid.h:391), or whose batch
- *      origin's cell does (a ray that long could stall pass 2's float step, where the reference loops forever). Not built:
- *      X-ray images, colours, intensities, other writers, the fixed-ratio sampler, frame-id filters, bag / tf reading. ---- */
+ *      origin's cell does (a ray that long could stall pass 2's float step, where the reference loops forever).
+ *      X-ray images (io/xray_points_processor.cc) and color_points (io/coloring_points_processor.cc) of the final pass's points,
+ *      see dl_map_writer_add_xray. Not built: intensities, other writers, the fixed-ratio sampler, frame-id filters, bag / tf
+ *      reading. ---- */
 typedef struct dl_map_writer dl_map_writer;
 typedef struct dl_map_writer_options {
   int32_t range_filter;        /* 1: min_max_range_filter is in the pipeline */
@@ -908,7 +910,8 @@ typedef struct dl_map_writer_options {
 typedef struct dl_map_message {  /* one PointsBatch: rows [first_row, first_row + num_rows) of the call's x y z t rows */
   int64_t stamp;                 /* universal ticks of the message (the time the row times t, in seconds, are relative to) */
   int64_t first_row, num_rows;
-  int32_t trajectory_id, reserved;
+  int32_t trajectory_id;
+  int32_t frame_id;              /* caller-chosen integer for PointsBatch::frame_id; only colour stages read it */
   double sensor_to_tracking[7];
 } dl_map_message;
 typedef struct dl_map_writer_info {  /* of one process call */
@@ -944,6 +947,42 @@ int dl_map_writer_flush(dl_map_writer* writer, int32_t* restart);
  * cells_xyz = NULL to query *count. */
 int dl_map_writer_voxels(const dl_map_writer* writer, int64_t capacity, int32_t* cells_xyz, int32_t* hits, int32_t* rays,
                          int64_t* count);
+
+/* ---- X-ray images and point colours of the final pass (io/xray_points_processor.cc, io/coloring_points_processor.cc).
+ *      Stages are added after create and before the first process call, in pipeline order, and sit after the last multi-pass
+ *      stage: they see exactly the final pass's output points, messages in call order, rows in message order (the reference
+ *      LOG(FATAL)s when X-ray generation comes before a multi-pass stage). At most DL_MAP_WRITER_MAX_STAGES stages of both
+ *      kinds together.
+ *        color_points: a message whose frame_id equals the stage's gets every point coloured rgb[i] / 255.f. An X-ray stage sees
+ *          the colour stages added before it, the last matching one wins; a message none of them touched has no colours and adds
+ *          kDefaultColor (0, 0, 0).
+ *        write_xray_image: camera_point = transform.cast<float>() * p, cell = lround(camera_point / (float)voxel_size) per axis;
+ *          the cell becomes occupied, extends the bounding box, and its column (y, z) adds the colour to float sums in stream
+ *          order and counts the point. The image is (max.y - min.y + 1) x (max.z - min.z + 1), cell (y, z) at pixel
+ *          (max.y - y, max.z - z); a pixel mixes white with the column's mean colour by log(occupied voxels) / max over columns
+ *          of that log (IntoImage, including its double / float promotions); an empty column is white. Images equal the
+ *          reference's with draw_trajectories = false (trajectory strokes are Cairo's antialiasing and are not drawn).
+ *      Rejected with DL_ERR_ARG, the writer unchanged: a stage added after processing began or beyond the cap, voxel_size <= 0 or
+ *      not finite, a quaternion with |norm - 1| > 1e-9 (FromDictionary's CHECK_NEAR), and (final pass) a point whose X-ray cell
+ *      lies beyond +-8192 on any axis (where HybridGridBase<bool>::mutable_value CHECK-fails). ---- */
+#define DL_MAP_WRITER_MAX_STAGES 16
+typedef struct dl_map_writer_color {
+  int32_t frame_id;
+  uint8_t rgb[3];                /* the Lua values after static_cast<uint8> */
+  uint8_t pad;
+} dl_map_writer_color;
+typedef struct dl_map_writer_xray {
+  double voxel_size;
+  double transform[7];           /* Rigid3d: t x y z, q w x y z */
+} dl_map_writer_xray;
+int dl_map_writer_add_color(dl_map_writer* writer, const dl_map_writer_color* color);
+/* *stage receives the X-ray stage's number (0, 1, ... in the order X-ray stages were added). */
+int dl_map_writer_add_xray(dl_map_writer* writer, const dl_map_writer_xray* xray, int32_t* stage);
+/* After the final flush: the image of an X-ray stage as Cairo ARGB32 words 0xFF000000 | r << 16 | g << 8 | b, row-major,
+ * *width * *height of them. Pass argb = NULL to query the size; capacity is in words. An empty bounding box gives 0 x 0 (the
+ * reference writes no file then). Rejected with DL_ERR_ARG: an unknown stage, a call before the final flush, capacity too small. */
+int dl_map_writer_xray_image(const dl_map_writer* writer, int32_t stage, int64_t capacity, uint32_t* argb, int32_t* width,
+                             int32_t* height);
 
 /* Device memory helpers so a host language without CUDA bindings can stage buffers. */
 int dl_device_alloc(dl_context* ctx, int64_t bytes, void** out_dev);

@@ -5,8 +5,15 @@ oracle arm on a subset of the scans, and the GPU's name and power limit. The ora
 (tests/map_writer_oracle.py): it checks the output bit for bit; its time is that of a correctness reference, not of a CPU
 implementation.
 
+With --xray the same invocation also times the final pass with the six X-ray stages of the reference's backpack pipeline
+(assets_writer_backpack_3d.lua: gray YZ / XY / XZ at 5 cm, color_points for two LiDAR frames, the three again in colour; messages
+alternate between the two frame ids) against the final pass without them, alternating the two, and reports the X-ray share of
+the final pass, point-stages per second, the device bytes the stages hold (cudaMemGetInfo difference) and the image sizes.
+
     python tools/bench_map_writer.py --scans 300 --voxel 0.05 --repeat 3
+    python tools/bench_map_writer.py --scans 300 --voxel 0.05 --repeat 3 --xray
 """
+import math
 import argparse
 import json
 import os
@@ -57,6 +64,7 @@ def main():
     ap.add_argument("--max-range", type=float, default=60.0)
     ap.add_argument("--repeat", type=int, default=3)
     ap.add_argument("--cpu-scans", type=int, default=2)
+    ap.add_argument("--xray", action="store_true", help="also time the final pass with the backpack pipeline's X-ray stages")
     args = ap.parse_args()
 
     import torch
@@ -116,7 +124,70 @@ def main():
                        "points_per_s": round(len(sub_rows) * 3 / cpu_s), "samples_per_s": round(want["num_samples"] / cpu_s),
                        "bit_identical": bool(got.tobytes() == want["points"].tobytes())},
     }
+    if args.xray:
+        line["xray"] = bench_xray(ctx, args, times, poses, msgs, rows, rows_dev, out_dev)
     print(json.dumps(line))
+
+
+XRAY_VOXEL = 5e-2
+
+
+def backpack_stages():
+    """assets_writer_backpack_3d.lua after its range filter (transform.lua's rotations), frame ids 0 and 1."""
+    import dliom
+    xy, xz, yz = [(0.0, 0.0, 0.0) + tuple(dliom.roll_pitch_yaw(*a))
+                  for a in ((0.0, -math.pi / 2.0, 0.0), (0.0, 0.0, -math.pi / 2), (0.0, 0.0, math.pi))]
+    gray = [("xray", yz), ("xray", xy), ("xray", xz)]
+    return gray + [("color", 0, (255, 0, 0)), ("color", 1, (0, 255, 0))] + gray
+
+
+def bench_xray(ctx, args, times, poses, msgs, rows, rows_dev, out_dev):
+    import torch
+    import dliom
+    msgs = [m + (k % 2,) for k, m in enumerate(msgs)]
+
+    def final_pass(with_stages):
+        torch.cuda.synchronize()
+        free0 = torch.cuda.mem_get_info()[0]
+        w = dliom.MapWriter(ctx, range_filter=(args.min_range, args.max_range), outlier_voxel_size=args.voxel)
+        w.add_trajectory(0, times, poses)
+        ids = []
+        if with_stages:
+            for s in backpack_stages():
+                if s[0] == "xray":
+                    ids.append(w.add_xray(XRAY_VOXEL, s[1]))
+                else:
+                    w.add_color(s[1], s[2])
+        while True:
+            t0 = time.perf_counter()
+            n, _, info = w.process_dev(msgs, rows_dev.data_ptr(), len(rows), out_dev.data_ptr())
+            ms = (time.perf_counter() - t0) * 1e3    # the call ends in a device synchronise
+            if not w.flush():
+                break
+        held = free0 - torch.cuda.mem_get_info()[0]
+        t0 = time.perf_counter()
+        shapes = [list(w.xray_image(i).shape) for i in ids]
+        image_ms = (time.perf_counter() - t0) * 1e3
+        w.close()
+        return ms, n, held, shapes, image_ms
+
+    final_pass(True)    # warm-up: the X-ray table, the sort's scratch
+    with_ms, without_ms = [], []
+    for _ in range(args.repeat):
+        a = final_pass(False)
+        b = final_pass(True)
+        without_ms.append(a[0])
+        with_ms.append(b[0])
+    n, held_with, shapes, image_ms = b[1], b[2], b[3], b[4]
+    held_without = a[2]
+    best_with, best_without = min(with_ms), min(without_ms)
+    stages = sum(1 for s in backpack_stages() if s[0] == "xray")
+    return {"stages": stages, "voxel_size": XRAY_VOXEL, "points": int(n),
+            "final_pass_ms_without": [round(v, 3) for v in without_ms], "final_pass_ms_with": [round(v, 3) for v in with_ms],
+            "xray_share_of_final_pass": round((best_with - best_without) / best_with, 4),
+            "point_stages_per_s": round(n * stages / ((best_with - best_without) / 1e3)),
+            "device_bytes_held_by_stages": int(held_with - held_without), "image_ms_all_stages": round(image_ms, 3),
+            "image_sizes_hw": shapes}
 
 
 if __name__ == "__main__":
