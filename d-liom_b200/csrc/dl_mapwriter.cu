@@ -581,6 +581,214 @@ __global__ void __launch_bounds__(kBlock) mw_xray_pixels(Table t, int64_t cap, i
   argb[(int64_t)(max_z - z) * width + (max_y - y)] = 0xFF000000u | r << 16 | g << 8 | b;  // Uint8ColorToCairo
 }
 
+// ---- Probability-grid stages (write_probability_grid, write_ros_map). Cells are uint16 correspondence-cost values without the
+// update marker; a per-cell 32-bit stamp replaces it: batch k (counted from 1 over the writer's life) claims a cell with
+// atomicMax(stamp, 2k + 1) for a hit and 2k for a walk, and the claimer that lifts the stamp past 2k - 1 applies the table once.
+// Hits run in one launch before the walks, so a hit wins over every miss of its batch and no FinishUpdate pass is needed.
+constexpr int kSubpixel = 1000;              // ray_casting.cc kSubpixelScale
+constexpr int kGridBoxChunk = 32;            // points per lane of mw_grid_boxes
+
+// Per message of a call: the float box of its output points' x y as order-preserving keys, and its first / last output point.
+struct GridBoxes {
+  uint32_t* keys;            // 4 per message: ~key of min x, min y, key of max x, max y (0: no point)
+  int32_t* first;            // per message: first and last output point (first = INT_MAX: no point)
+  int32_t* last;
+  unsigned long long* nonfinite;
+};
+
+__device__ __forceinline__ uint32_t float_key(float f) {
+  const uint32_t b = __float_as_uint(f);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+// one warp per 32 * kGridBoxChunk consecutive points, lane l takes every 32nd; runs of one message are reduced per lane, then
+// per warp when every lane holds the same message
+__global__ void __launch_bounds__(kBlock) mw_grid_boxes(const float* pts, const int32_t* msg, int64_t n, GridBoxes b) {
+  const int lane = threadIdx.x & 31;
+  const int64_t base = ((int64_t)blockIdx.x * kBlock + (threadIdx.x & ~31)) * kGridBoxChunk;
+  int cur = -1, first = INT_MAX, last = -1;
+  uint32_t lo_x = ~0u, lo_y = ~0u, hi_x = 0, hi_y = 0;
+  bool bad = false;
+  auto flush = [&](bool warp_wide) {
+    if (warp_wide) {
+      lo_x = __reduce_min_sync(0xffffffffu, lo_x);
+      lo_y = __reduce_min_sync(0xffffffffu, lo_y);
+      hi_x = __reduce_max_sync(0xffffffffu, hi_x);
+      hi_y = __reduce_max_sync(0xffffffffu, hi_y);
+      first = __reduce_min_sync(0xffffffffu, first);
+      last = __reduce_max_sync(0xffffffffu, last);
+      if (lane != 0) return;
+    }
+    if (cur < 0) return;
+    atomicMax(b.keys + 4 * cur, ~lo_x);
+    atomicMax(b.keys + 4 * cur + 1, ~lo_y);
+    atomicMax(b.keys + 4 * cur + 2, hi_x);
+    atomicMax(b.keys + 4 * cur + 3, hi_y);
+    atomicMin(b.first + cur, first);
+    atomicMax(b.last + cur, last);
+  };
+  for (int k = 0; k < kGridBoxChunk; ++k) {
+    const int64_t i = base + (int64_t)k * 32 + lane;
+    if (i >= n) break;
+    const int m = msg[i];
+    if (m != cur) {
+      flush(false);
+      cur = m;
+      first = INT_MAX; last = -1;
+      lo_x = ~0u; lo_y = ~0u; hi_x = 0; hi_y = 0;
+    }
+    const float x = pts[3 * i], y = pts[3 * i + 1];
+    if (!isfinite(x) || !isfinite(y)) {
+      bad = true;
+      continue;
+    }
+    first = min(first, (int)i);
+    last = (int)i;
+    lo_x = min(lo_x, float_key(x)); lo_y = min(lo_y, float_key(y));
+    hi_x = max(hi_x, float_key(x)); hi_y = max(hi_y, float_key(y));
+  }
+  flush(__all_sync(0xffffffffu, cur == __shfl_sync(0xffffffffu, cur, 0)));
+  const unsigned bad_lanes = __ballot_sync(0xffffffffu, bad);
+  if (lane == 0 && bad_lanes) atomicAdd(b.nonfinite, (unsigned long long)__popc(bad_lanes));
+}
+
+// One batch of one grid stage, at the batch's own limits; cells land at (x + off_x, y + off_y) of the allocated grid.
+struct GridBatch {
+  const float* pts;          // the batch's x y z points
+  int32_t n;
+  int32_t begin_x, begin_y;  // the origin's superscaled cell
+  int32_t off_x, off_y;
+  int32_t stride;            // num_x_cells of the allocated grid
+  double max_x, max_y, resolution;  // the superscaled limits' max and resolution / 1000
+  uint16_t* cells;
+  uint32_t* stamps;
+  const uint16_t* table;     // the hit or the miss table, without the update marker
+  uint32_t claim;            // 2k + 1 (hits) or 2k (walks)
+};
+
+// ApplyLookupTable with the stamp in place of kUpdateMarker (a plain load first: most revisits near the origin stop there)
+__device__ __forceinline__ void grid_visit(const GridBatch& g, int x, int y) {
+  const int64_t idx = (int64_t)(y + g.off_y) * g.stride + (x + g.off_x);
+  const uint32_t lowest = g.claim & ~1u;  // 2k: any claim of this batch
+  if (*(volatile uint32_t*)(g.stamps + idx) >= lowest) return;
+  if (atomicMax(g.stamps + idx, g.claim) < lowest) g.cells[idx] = __ldg(g.table + g.cells[idx]);
+}
+
+// MapLimits::GetCellIndex at the superscaled limits: the float promoted to double, IEEE division, lround
+__device__ __forceinline__ int2 grid_end(const GridBatch& g, int i) {
+  const double px = (double)g.pts[3 * i], py = (double)g.pts[3 * i + 1];
+  return make_int2((int)llround((g.max_y - py) / g.resolution - 0.5), (int)llround((g.max_x - px) / g.resolution - 0.5));
+}
+
+__global__ void __launch_bounds__(kBlock) mw_grid_hits(GridBatch g) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= g.n) return;
+  const int2 e = grid_end(g, i);
+  grid_visit(g, e.x / kSubpixel, e.y / kSubpixel);
+}
+
+// CastRay (ray_casting.cc:29-146): x ascending, the vertical special case, int64 sub_y with the sub_y == denominator corner rule
+__global__ void __launch_bounds__(kBlock) mw_grid_walks(GridBatch g) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= g.n) return;
+  const int2 e = grid_end(g, i);
+  int2 b = make_int2(g.begin_x, g.begin_y), end = e;
+  if (b.x > end.x) {
+    b = e;
+    end = make_int2(g.begin_x, g.begin_y);
+  }
+  if (b.x / kSubpixel == end.x / kSubpixel) {
+    const int x = b.x / kSubpixel, last = max(b.y, end.y) / kSubpixel;
+    for (int y = min(b.y, end.y) / kSubpixel; y <= last; ++y) grid_visit(g, x, y);
+    return;
+  }
+  const int64_t dx = end.x - b.x, dy = end.y - b.y, denominator = 2 * kSubpixel * dx;
+  int cx = b.x / kSubpixel, cy = b.y / kSubpixel;
+  int64_t sub_y = (2 * (b.y % kSubpixel) + 1) * dx;
+  const int first_pixel = 2 * kSubpixel - 2 * (b.x % kSubpixel) - 1;
+  const int last_pixel = 2 * (end.x % kSubpixel) + 1;
+  const int end_x = end.x / kSubpixel;
+  sub_y += dy * first_pixel;
+  if (dy > 0) {
+    while (true) {
+      grid_visit(g, cx, cy);
+      while (sub_y > denominator) {
+        sub_y -= denominator;
+        ++cy;
+        grid_visit(g, cx, cy);
+      }
+      ++cx;
+      if (sub_y == denominator) {
+        sub_y -= denominator;
+        ++cy;
+      }
+      if (cx == end_x) break;
+      sub_y += dy * 2 * kSubpixel;
+    }
+    sub_y += dy * last_pixel;
+    grid_visit(g, cx, cy);
+    while (sub_y > denominator) {
+      sub_y -= denominator;
+      ++cy;
+      grid_visit(g, cx, cy);
+    }
+    return;
+  }
+  while (true) {
+    grid_visit(g, cx, cy);
+    while (sub_y < 0) {
+      sub_y += denominator;
+      --cy;
+      grid_visit(g, cx, cy);
+    }
+    ++cx;
+    if (sub_y == 0) {
+      sub_y += denominator;
+      --cy;
+    }
+    if (cx == end_x) break;
+    sub_y += dy * 2 * kSubpixel;
+  }
+  sub_y += dy * last_pixel;
+  grid_visit(g, cx, cy);
+  while (sub_y < 0) {
+    sub_y += denominator;
+    --cy;
+    grid_visit(g, cx, cy);
+  }
+}
+
+// The known-cells box: no table entry returns a cell to 0 (unknown), so it is the box of the cells != 0
+__global__ void __launch_bounds__(kBlock) mw_grid_known_box(const uint16_t* cells, int nx, int64_t count, int32_t* box) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  int x0 = INT_MAX, y0 = INT_MAX, x1 = INT_MIN, y1 = INT_MIN;
+  if (i < count && cells[i] != 0) {
+    x0 = x1 = (int)(i % nx);
+    y0 = y1 = (int)(i / nx);
+  }
+  x0 = __reduce_min_sync(0xffffffffu, x0);
+  y0 = __reduce_min_sync(0xffffffffu, y0);
+  x1 = __reduce_max_sync(0xffffffffu, x1);
+  y1 = __reduce_max_sync(0xffffffffu, y1);
+  if ((threadIdx.x & 31) == 0 && x0 != INT_MAX) {
+    atomicMin(box, x0);
+    atomicMin(box + 1, y0);
+    atomicMax(box + 2, x1);
+    atomicMax(box + 3, y1);
+  }
+}
+
+// the cropped box's cells and DrawProbabilityGrid's grey values (colour table indexed by the cell value)
+__global__ void __launch_bounds__(kBlock) mw_grid_crop(const uint16_t* cells, int nx, int ox, int oy, int width, int64_t count,
+                                                       const uint8_t* colors, uint16_t* out_cells, uint8_t* out_pixels) {
+  const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+  if (i >= count) return;
+  const int64_t x = i % width, y = i / width;
+  const uint16_t v = cells[(oy + y) * (int64_t)nx + ox + x];
+  out_cells[i] = v;
+  out_pixels[i] = colors[v];
+}
+
 // std::log(double n) for n = 0 .. kLogTable, glibc's (through a volatile pointer, never the compiler's folding)
 const std::vector<double>& log_table() {
   static std::vector<double> table;
@@ -591,6 +799,98 @@ const std::vector<double>& log_table() {
     for (int n = 0; n <= kLogTable; ++n) table[n] = glibc_log((double)n);
   });
   return table;
+}
+
+// kValueToCorrespondenceCost (probability_values.cc:27-36, 59-63): SlowValueToBoundedFloat in float, host arithmetic
+// (-ffp-contract=off)
+float value_to_correspondence_cost(int value) {
+  const float lo = 1.f - (1.f - 0.1f), hi = 1.f - 0.1f;  // kMinCorrespondenceCost, kMaxCorrespondenceCost
+  if (value == 0) return hi;
+  const float scale = (hi - lo) / 32766.f;
+  return (float)value * scale + (lo - scale);
+}
+// CorrespondenceCostToValue (probability_values.h:32-44, 85-88)
+uint16_t correspondence_cost_to_value(float c) {
+  const float lo = 1.f - (1.f - 0.1f), hi = 1.f - 0.1f;
+  const float clamped = c > hi ? hi : (c < lo ? lo : c);
+  return (uint16_t)((int)lroundf((clamped - lo) * (32766.f / (hi - lo))) + 1);
+}
+// ComputeLookupTableToApplyCorrespondenceCostOdds(Odds((float)probability)) (probability_values.cc:85-100), without the update
+// marker
+void compute_correspondence_cost_table(double probability, uint16_t* table) {
+  const float p = (float)probability;
+  const float odds = p / (1.f - p);
+  auto from_odds = [](float o) { return o / (o + 1.f); };
+  table[0] = correspondence_cost_to_value(1.f - from_odds(odds));
+  for (int cell = 1; cell != 32768; ++cell) {
+    const float q = 1.f - value_to_correspondence_cost(cell);  // CorrespondenceCostToProbability
+    table[cell] = correspondence_cost_to_value(1.f - from_odds(odds * (q / (1.f - q))));
+  }
+}
+// DrawProbabilityGrid's grey value of every cell value: 128 if unknown, else ProbabilityToColor(GetProbability)
+// (probability_grid_points_processor.cc:49-54, 137-146)
+std::vector<uint8_t> grid_color_table() {
+  std::vector<uint8_t> colors(32768);
+  colors[0] = 128;
+  for (int v = 1; v < 32768; ++v) {
+    const float p = 1.f - value_to_correspondence_cost(v);
+    const float probability = 1.f - p;
+    colors[v] = (uint8_t)(int)lroundf(255 * ((probability - 0.1f) / ((1.f - 0.1f) - 0.1f)));
+  }
+  return colors;
+}
+
+struct GridLimits {          // MapLimits: max (double), cell counts
+  double max_x, max_y;
+  int32_t nx, ny;
+};
+struct GridStage {
+  double resolution;
+  int32_t insert_free_space;
+  GridLimits limits;         // after the last call
+  uint16_t* cells = nullptr;   // allocated at `limits` once a batch arrived (before that every cell is unknown)
+  uint32_t* stamps = nullptr;
+  uint16_t* tables = nullptr;  // hit [0, 32768), miss [32768, 65536)
+  int64_t batches = 0;       // k of the last batch
+};
+// One call's growth of one stage, decided before anything changes: every batch's limits and cell offset in the grid of the
+// call's final limits, and the new buffers when the grid grows (or is first allocated).
+struct GridPlan {
+  GridLimits final_limits;
+  std::vector<GridLimits> at;
+  std::vector<int2> offset;
+  int32_t grow_x = 0, grow_y = 0;  // where the previous content lands
+  uint16_t* cells = nullptr;
+  uint32_t* stamps = nullptr;
+};
+
+// MapLimits::GetCellIndex (map_limits.h:69-76)
+void grid_cell_index(const GridLimits& l, double resolution, float px, float py, long* x, long* y) {
+  *x = std::lround((l.max_y - (double)py) / resolution - 0.5);
+  *y = std::lround((l.max_x - (double)px) / resolution - 0.5);
+}
+// Grid2D::GrowLimits (grid_2d.cc:116-145) on the limits alone; false where a doubling would pass DL_MAP_WRITER_MAX_GRID_CELLS.
+// (*add_x, *add_y) accumulate the translation of the cells.
+bool grid_grow_limits(GridLimits* l, double resolution, float px, float py, int32_t* add_x, int32_t* add_y) {
+  for (;;) {
+    long x, y;
+    grid_cell_index(*l, resolution, px, py, &x, &y);
+    if (x >= 0 && y >= 0 && x < l->nx && y < l->ny) return true;
+    if (2 * (int64_t)l->nx > DL_MAP_WRITER_MAX_GRID_CELLS || 2 * (int64_t)l->ny > DL_MAP_WRITER_MAX_GRID_CELLS) return false;
+    const int32_t xo = l->nx / 2, yo = l->ny / 2;
+    l->max_x = l->max_x + resolution * (double)yo;
+    l->max_y = l->max_y + resolution * (double)xo;
+    l->nx *= 2;
+    l->ny *= 2;
+    *add_x += xo;
+    *add_y += yo;
+  }
+}
+float key_float(uint32_t k) {
+  const uint32_t b = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
+  float f;
+  std::memcpy(&f, &b, sizeof(f));
+  return f;
 }
 
 unsigned tiles_of(int64_t n) { return (unsigned)((n + kBlock - 1) / kBlock); }
@@ -631,8 +931,17 @@ struct dl_map_writer {
   int64_t xray_entries = 0;
   int32_t* d_bbox = nullptr;       // 6 per stage
   double* d_log = nullptr;         // log_table()
+  // probability-grid stages, in the order they were added
+  std::vector<GridStage> grids;
+  uint8_t* d_grid_colors = nullptr;  // grid_color_table()
+  struct GridCall {                // the batches of one final-pass call and every stage's plan
+    std::vector<int32_t> first, count;
+    std::vector<float> origins;    // x y per batch
+    std::vector<GridPlan> plans;
+  };
 
   int num_passes() const { return options.outlier_voxel_size > 0 ? 3 : 1; }
+  int num_stages() const { return (int)(xrays.size() + colors.size() + grids.size()); }
   bool final_pass() const { return pass == num_passes() - 1; }
 
   int upload_tables() {
@@ -753,6 +1062,17 @@ struct dl_map_writer {
   int process(int32_t num_messages, const dl_map_message* messages, const float* rows_host, const float* rows_dev,
               int64_t num_rows, float* points_host, float* points_dev, int64_t* num_points_out, float* origins_out,
               dl_map_writer_info* info);
+  int plan_grids(const float* points, const int32_t* point_msg, int64_t n, const float* origins, int num_messages,
+                 const std::vector<int32_t>& last_run, const GridBoxes& boxes, GridCall* call);
+  int apply_grids(const float* points, GridCall* call);
+  static void drop_plans(GridCall* call) {
+    for (GridPlan& p : call->plans) {
+      cudaFree(p.cells);
+      cudaFree(p.stamps);
+      p.cells = nullptr;
+      p.stamps = nullptr;
+    }
+  }
 };
 
 namespace {
@@ -809,8 +1129,10 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   int32_t* d_ints = nullptr;  // [0] runs, [1] kept, [2] gate survivors
   float* d_out = nullptr;
   int32_t* gate_tiles = nullptr;
-  // X-ray stages: the message of every output point, and the sort of one chunk's (stage, column) keys
+  // X-ray and grid stages: the message of every output point; X-ray stages: the sort of one chunk's (stage, column) keys
   const bool with_xray = final_pass() && !xrays.empty();
+  const bool with_grid = final_pass() && !grids.empty();
+  GridBoxes boxes{};
   const int64_t sort_items = with_xray ? std::min<int64_t>(n, kXrayChunk) * (int64_t)sum_stage.size() : 0;
   size_t sort_bytes = 0;
   if (sort_items > 0) {
@@ -823,8 +1145,14 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   int32_t* sort_vals = nullptr;
   void* sort_scratch = nullptr;
   MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+    if (with_xray || with_grid) out_msg = ar.take<int32_t>((size_t)n);
+    if (with_grid) {
+      boxes.keys = ar.take<uint32_t>(4 * (size_t)num_messages);
+      boxes.first = ar.take<int32_t>((size_t)num_messages);
+      boxes.last = ar.take<int32_t>((size_t)num_messages);
+      boxes.nonfinite = ar.take<unsigned long long>(1);
+    }
     if (with_xray) {
-      out_msg = ar.take<int32_t>((size_t)n);
       sort_keys = ar.take<unsigned long long>(2 * (size_t)sort_items);
       sort_vals = ar.take<int32_t>(2 * (size_t)sort_items);
       sort_scratch = ar.take<char>(sort_bytes);
@@ -942,8 +1270,18 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
     out_count = survivors;
     local.dropped_moving = kept - survivors;
   }
-  if (with_xray && out_count > 0)
-    MW_TRY(insert_xray(d_out, out_msg, d_msgs, out_count, sort_scratch, sort_bytes, sort_keys, sort_vals, a.counters + kOutside));
+  // every stage checks its input before any of them changes: the grids' growth first, then the X-ray cells
+  GridCall grid_call;
+  if (with_grid) MW_TRY(plan_grids(d_out, out_msg, out_count, a.origins, num_messages, last_run, boxes, &grid_call));
+  if (with_xray && out_count > 0) {
+    const int st = insert_xray(d_out, out_msg, d_msgs, out_count, sort_scratch, sort_bytes, sort_keys, sort_vals,
+                               a.counters + kOutside);
+    if (st != DL_OK) {
+      drop_plans(&grid_call);
+      return st;
+    }
+  }
+  if (with_grid) MW_TRY(apply_grids(d_out, &grid_call));
   DL_CUDA(ctx, cudaMemcpyAsync(counters, a.counters, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
   int32_t cells = 0;
   if (table.num_cells) DL_CUDA(ctx, cudaMemcpyAsync(&cells, table.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1010,6 +1348,146 @@ int dl_map_writer::insert_xray(const float* points, const int32_t* point_msg, co
   return DL_OK;
 }
 
+// The grid stages' half of a final-pass call that changes nothing: one reduction of every batch's float box and point range over
+// the call's output points, one read-back, then GrowAsNeeded replayed on the host for every stage and batch in order. A stage
+// whose grid grows (or gets its first batch) gets its buffers at the call's final limits here, so that apply_grids cannot fail
+// halfway.
+int dl_map_writer::plan_grids(const float* points, const int32_t* point_msg, int64_t n, const float* origins, int num_messages,
+                              const std::vector<int32_t>& last_run, const GridBoxes& b, GridCall* call) {
+  std::vector<int32_t> batch_msgs;
+  for (int m = 0; m < num_messages; ++m)
+    if (last_run[m] >= 0) batch_msgs.push_back(m);
+  if (batch_msgs.empty()) return DL_OK;
+  const size_t nm = (size_t)num_messages;
+  DL_CUDA(ctx, cudaMemsetAsync(b.keys, 0, 4 * nm * sizeof(uint32_t), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(b.first, 0x7f, nm * sizeof(int32_t), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(b.last, 0xff, nm * sizeof(int32_t), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(b.nonfinite, 0, sizeof(unsigned long long), ctx->stream));
+  if (n > 0) {
+    const int64_t per_block = (int64_t)kBlock * kGridBoxChunk;
+    mw_grid_boxes<<<(unsigned)((n + per_block - 1) / per_block), kBlock, 0, ctx->stream>>>(points, point_msg, n, b);
+    DL_LAUNCH_CHECK(ctx, "mw_grid_boxes");
+  }
+  std::vector<uint32_t> keys(4 * nm);
+  std::vector<int32_t> first(nm), last(nm);
+  std::vector<float> org(3 * nm);
+  unsigned long long nonfinite = 0;
+  DL_CUDA(ctx, cudaMemcpyAsync(keys.data(), b.keys, keys.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(first.data(), b.first, nm * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(last.data(), b.last, nm * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(org.data(), origins, org.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(&nonfinite, b.nonfinite, sizeof(nonfinite), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  if (nonfinite > 0) return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: a point's x or y is not finite (probability grid stage)");
+  // GrowAsNeeded's float box: the origin, extended by every point (min / max do not depend on the order)
+  std::vector<float> lo(2 * batch_msgs.size()), hi(2 * batch_msgs.size());
+  for (size_t j = 0; j < batch_msgs.size(); ++j) {
+    const int m = batch_msgs[j];
+    float x0 = org[3 * m], y0 = org[3 * m + 1], x1 = x0, y1 = y0;
+    const bool points_in = first[m] <= last[m];
+    if (points_in) {
+      x0 = std::min(x0, key_float(~keys[4 * m]));
+      y0 = std::min(y0, key_float(~keys[4 * m + 1]));
+      x1 = std::max(x1, key_float(keys[4 * m + 2]));
+      y1 = std::max(y1, key_float(keys[4 * m + 3]));
+    }
+    const float pad = 1e-6f;  // kPadding
+    lo[2 * j] = x0 - pad;
+    lo[2 * j + 1] = y0 - pad;
+    hi[2 * j] = x1 + pad;
+    hi[2 * j + 1] = y1 + pad;
+    call->first.push_back(points_in ? first[m] : 0);
+    call->count.push_back(points_in ? last[m] - first[m] + 1 : 0);
+    call->origins.push_back(org[3 * m]);
+    call->origins.push_back(org[3 * m + 1]);
+  }
+  for (const GridStage& g : grids) {
+    GridPlan p;
+    p.final_limits = g.limits;
+    std::vector<int2> at_growth;
+    for (size_t j = 0; j < batch_msgs.size(); ++j) {
+      if (!grid_grow_limits(&p.final_limits, g.resolution, lo[2 * j], lo[2 * j + 1], &p.grow_x, &p.grow_y) ||
+          !grid_grow_limits(&p.final_limits, g.resolution, hi[2 * j], hi[2 * j + 1], &p.grow_x, &p.grow_y)) {
+        drop_plans(call);
+        return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: a batch would grow a probability grid beyond "
+                                     "DL_MAP_WRITER_MAX_GRID_CELLS cells per axis");
+      }
+      p.at.push_back(p.final_limits);
+      at_growth.push_back(make_int2(p.grow_x, p.grow_y));
+    }
+    for (const int2& c : at_growth) p.offset.push_back(make_int2(p.grow_x - c.x, p.grow_y - c.y));
+    call->plans.push_back(p);
+  }
+  for (size_t s = 0; s < grids.size(); ++s) {
+    GridPlan& p = call->plans[s];
+    if (grids[s].cells && p.grow_x == 0 && p.grow_y == 0) continue;
+    const size_t cells = (size_t)p.final_limits.nx * (size_t)p.final_limits.ny;
+    cudaError_t e = cudaMalloc(&p.cells, cells * sizeof(uint16_t));
+    if (e == cudaSuccess) e = cudaMalloc(&p.stamps, cells * sizeof(uint32_t));
+    if (e != cudaSuccess) {
+      drop_plans(call);
+      return ctx->cuda_fail(e, "dl_map_writer_process (probability grid)");
+    }
+  }
+  return DL_OK;
+}
+
+// Moves grown grids into their new buffers, then per stage and batch in order one launch for the hits and one for the walks.
+int dl_map_writer::apply_grids(const float* points, GridCall* call) {
+  for (size_t s = 0; s < grids.size() && !call->count.empty(); ++s) {
+    GridStage& g = grids[s];
+    GridPlan& p = call->plans[s];
+    const GridLimits& l = p.final_limits;
+    if (p.cells) {
+      const size_t cells = (size_t)l.nx * (size_t)l.ny;
+      DL_CUDA(ctx, cudaMemsetAsync(p.cells, 0, cells * sizeof(uint16_t), ctx->stream));
+      DL_CUDA(ctx, cudaMemsetAsync(p.stamps, 0, cells * sizeof(uint32_t), ctx->stream));  // below every claim
+      if (g.cells)
+        DL_CUDA(ctx, cudaMemcpy2DAsync(p.cells + (size_t)p.grow_y * l.nx + p.grow_x, (size_t)l.nx * sizeof(uint16_t), g.cells,
+                                       (size_t)g.limits.nx * sizeof(uint16_t), (size_t)g.limits.nx * sizeof(uint16_t),
+                                       (size_t)g.limits.ny, cudaMemcpyDeviceToDevice, ctx->stream));
+      if (g.cells) DL_CUDA(ctx, ctx->wait_stream());  // the copy out of the old buffers has ended
+      cudaFree(g.cells);
+      cudaFree(g.stamps);
+      g.cells = p.cells;
+      g.stamps = p.stamps;
+      p.cells = nullptr;
+      p.stamps = nullptr;
+    }
+    g.limits = l;
+    const double superscaled = g.resolution / kSubpixel;
+    for (size_t j = 0; j < call->count.size(); ++j) {
+      const int64_t k = ++g.batches;
+      GridBatch gb{};
+      gb.pts = points + 3 * (size_t)call->first[j];
+      gb.n = call->count[j];
+      long bx, by;
+      grid_cell_index(p.at[j], superscaled, call->origins[2 * j], call->origins[2 * j + 1], &bx, &by);
+      gb.begin_x = (int32_t)bx;
+      gb.begin_y = (int32_t)by;
+      gb.off_x = p.offset[j].x;
+      gb.off_y = p.offset[j].y;
+      gb.stride = l.nx;
+      gb.max_x = p.at[j].max_x;
+      gb.max_y = p.at[j].max_y;
+      gb.resolution = superscaled;
+      gb.cells = g.cells;
+      gb.stamps = g.stamps;
+      if (gb.n == 0) continue;  // the batch only grew the grid
+      gb.table = g.tables;
+      gb.claim = (uint32_t)(2 * k + 1);
+      mw_grid_hits<<<tiles_of(gb.n), kBlock, 0, ctx->stream>>>(gb);
+      DL_LAUNCH_CHECK(ctx, "mw_grid_hits");
+      if (!g.insert_free_space) continue;
+      gb.table = g.tables + 32768;
+      gb.claim = (uint32_t)(2 * k);
+      mw_grid_walks<<<tiles_of(gb.n), kBlock, 0, ctx->stream>>>(gb);
+      DL_LAUNCH_CHECK(ctx, "mw_grid_walks");
+    }
+  }
+  return DL_OK;
+}
+
 int dl_map_writer_create(dl_context* ctx, const dl_map_writer_options* options, dl_map_writer** out) {
   if (!ctx || !options || !out) return DL_ERR_ARG;
   const dl_map_writer_options& o = *options;
@@ -1049,6 +1527,12 @@ void dl_map_writer_destroy(dl_map_writer* w) {
   cudaFree(w->xray.num_cells);
   cudaFree(w->d_bbox);
   cudaFree(w->d_log);
+  for (GridStage& g : w->grids) {
+    cudaFree(g.cells);
+    cudaFree(g.stamps);
+    cudaFree(g.tables);
+  }
+  cudaFree(w->d_grid_colors);
   cudaFree(w->d_runs);
   cudaFree(w->d_times);
   cudaFree(w->d_nodes);
@@ -1156,7 +1640,7 @@ int dl_map_writer_add_color(dl_map_writer* w, const dl_map_writer_color* color) 
   dl_context* ctx = w->ctx;
   if (!color) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_color: bad arguments");
   if (w->started || w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_color: processing has begun");
-  if ((int)(w->xrays.size() + w->colors.size()) >= kMaxStages)
+  if (w->num_stages() >= kMaxStages)
     return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_color: more than DL_MAP_WRITER_MAX_STAGES stages");
   // ToFloatColor: Uint8ComponentToFloat(c) = c / 255.f
   w->colors.push_back(ColorStage{color->frame_id, color->rgb[0] / 255.f, color->rgb[1] / 255.f, color->rgb[2] / 255.f});
@@ -1168,7 +1652,7 @@ int dl_map_writer_add_xray(dl_map_writer* w, const dl_map_writer_xray* xray, int
   dl_context* ctx = w->ctx;
   if (!xray || !stage) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: bad arguments");
   if (w->started || w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: processing has begun");
-  if ((int)(w->xrays.size() + w->colors.size()) >= kMaxStages)
+  if (w->num_stages() >= kMaxStages)
     return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: more than DL_MAP_WRITER_MAX_STAGES stages");
   if (!(xray->voxel_size > 0) || !std::isfinite(xray->voxel_size) || !((float)xray->voxel_size > 0.f))
     return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: voxel_size must be finite and > 0");
@@ -1229,6 +1713,107 @@ int dl_map_writer_xray_image(const dl_map_writer* w, int32_t stage, int64_t capa
                                                      d_img);
   DL_LAUNCH_CHECK(ctx, "mw_xray_pixels");
   DL_CUDA(ctx, cudaMemcpyAsync(argb, d_img, (size_t)pixels * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  return DL_OK;
+}
+
+int dl_map_writer_add_probability_grid(dl_map_writer* w, const dl_map_writer_grid_options* options, int32_t* stage) {
+  if (!w) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  if (!options || !stage) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_probability_grid: bad arguments");
+  if (w->started || w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_probability_grid: processing has begun");
+  if (w->num_stages() >= kMaxStages)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_probability_grid: more than DL_MAP_WRITER_MAX_STAGES stages");
+  const dl_map_writer_grid_options& o = *options;
+  if (!(o.resolution > 0) || !std::isfinite(o.resolution))
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_probability_grid: resolution must be finite and > 0");
+  // CreateProbabilityGridRangeDataInserterOptions2D: CHECK_GT(hit_probability, 0.5), CHECK_LT(miss_probability, 0.5)
+  if (!(o.hit_probability > 0.5) || !std::isfinite(o.hit_probability) || !(o.miss_probability < 0.5) ||
+      !std::isfinite(o.miss_probability))
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_probability_grid: hit_probability must be > 0.5 and miss_probability < 0.5");
+  if (o.insert_free_space != 0 && o.insert_free_space != 1)
+    return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_probability_grid: insert_free_space must be 0 or 1");
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  std::vector<uint16_t> tables(2 * 32768);
+  compute_correspondence_cost_table(o.hit_probability, tables.data());
+  compute_correspondence_cost_table(o.miss_probability, tables.data() + 32768);
+  const std::vector<uint8_t> colors = grid_color_table();
+  uint16_t* d_tables = nullptr;
+  uint8_t* d_colors = nullptr;
+  cudaError_t e = cudaMalloc(&d_tables, tables.size() * sizeof(uint16_t));
+  if (e == cudaSuccess) e = cudaMemcpy(d_tables, tables.data(), tables.size() * sizeof(uint16_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && !w->d_grid_colors) {
+    e = cudaMalloc(&d_colors, colors.size());
+    if (e == cudaSuccess) e = cudaMemcpy(d_colors, colors.data(), colors.size(), cudaMemcpyHostToDevice);
+  }
+  if (e != cudaSuccess) {
+    cudaFree(d_tables);
+    cudaFree(d_colors);
+    return ctx->cuda_fail(e, "dl_map_writer_add_probability_grid");
+  }
+  if (d_colors) w->d_grid_colors = d_colors;
+  GridStage g{};
+  g.resolution = o.resolution;
+  g.insert_free_space = o.insert_free_space;
+  // CreateProbabilityGrid (probability_grid_points_processor.cc:150-158): 100 x 100 cells, max = 0.5 * 100 * resolution
+  const double max = 0.5 * 100 * o.resolution;
+  g.limits = GridLimits{max, max, 100, 100};
+  g.tables = d_tables;
+  *stage = (int32_t)w->grids.size();
+  w->grids.push_back(g);
+  return DL_OK;
+}
+
+int dl_map_writer_probability_grid(const dl_map_writer* w, int32_t stage, dl_map_writer_grid_info* info, int64_t capacity,
+                                   uint16_t* cells, uint8_t* pixels) {
+  if (!w || !info) return DL_ERR_ARG;
+  dl_context* ctx = w->ctx;
+  if (stage < 0 || stage >= (int32_t)w->grids.size()) return ctx->fail(DL_ERR_ARG, "dl_map_writer_probability_grid: unknown stage");
+  if (!w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_probability_grid: the final pass has not been flushed");
+  const GridStage& g = w->grids[stage];
+  const int64_t num_cells = (int64_t)g.limits.nx * g.limits.ny;
+  int32_t box[4] = {INT_MAX, INT_MAX, INT_MIN, INT_MIN};
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (g.cells) {
+    int32_t* d_box = nullptr;
+    MW_TRY(carve_scratch(ctx, [&](Arena& ar) { d_box = ar.take<int32_t>(4); }));
+    DL_CUDA(ctx, cudaMemcpyAsync(d_box, box, sizeof(box), cudaMemcpyHostToDevice, ctx->stream));
+    mw_grid_known_box<<<tiles_of(num_cells), kBlock, 0, ctx->stream>>>(g.cells, g.limits.nx, num_cells, d_box);
+    DL_LAUNCH_CHECK(ctx, "mw_grid_known_box");
+    DL_CUDA(ctx, cudaMemcpyAsync(box, d_box, sizeof(box), cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
+  }
+  dl_map_writer_grid_info r{};
+  r.resolution = g.resolution;
+  r.max_x = g.limits.max_x;
+  r.max_y = g.limits.max_y;
+  r.num_x_cells = g.limits.nx;
+  r.num_y_cells = g.limits.ny;
+  const bool empty = box[0] > box[2];  // ComputeCroppedLimits: an empty box gives offset 0 and 1 x 1
+  r.offset_x = empty ? 0 : box[0];
+  r.offset_y = empty ? 0 : box[1];
+  r.width = empty ? 1 : box[2] - box[0] + 1;
+  r.height = empty ? 1 : box[3] - box[1] + 1;
+  *info = r;
+  if (!cells && !pixels) return DL_OK;
+  const int64_t count = (int64_t)r.width * r.height;
+  if (capacity < count) return ctx->fail(DL_ERR_ARG, "dl_map_writer_probability_grid: capacity below width * height");
+  if (!g.cells) {  // no batch reached the stage: cell (0, 0) of the initial grid, unknown
+    if (cells) cells[0] = 0;
+    if (pixels) pixels[0] = 128;
+    return DL_OK;
+  }
+  uint16_t* d_cells = nullptr;
+  uint8_t* d_pixels = nullptr;
+  MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+    d_cells = ar.take<uint16_t>((size_t)count);
+    d_pixels = ar.take<uint8_t>((size_t)count);
+  }));
+  mw_grid_crop<<<tiles_of(count), kBlock, 0, ctx->stream>>>(g.cells, g.limits.nx, r.offset_x, r.offset_y, r.width, count,
+                                                             w->d_grid_colors, d_cells, d_pixels);
+  DL_LAUNCH_CHECK(ctx, "mw_grid_crop");
+  if (cells) DL_CUDA(ctx, cudaMemcpyAsync(cells, d_cells, (size_t)count * sizeof(uint16_t), cudaMemcpyDeviceToHost, ctx->stream));
+  if (pixels) DL_CUDA(ctx, cudaMemcpyAsync(pixels, d_pixels, (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));
   DL_CUDA(ctx, ctx->wait_stream());
   return DL_OK;
 }

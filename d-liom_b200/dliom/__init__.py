@@ -42,7 +42,7 @@ EXPORTS = [
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
     "dl_map_writer_create", "dl_map_writer_destroy", "dl_map_writer_add_trajectory", "dl_map_writer_process",
     "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels", "dl_map_writer_add_color",
-    "dl_map_writer_add_xray", "dl_map_writer_xray_image",
+    "dl_map_writer_add_xray", "dl_map_writer_xray_image", "dl_map_writer_add_probability_grid", "dl_map_writer_probability_grid",
     "dl_submap_textures", "dl_submap_projections",
 ]
 
@@ -383,6 +383,20 @@ class MapWriterXray(C.Structure):   # dl_map_writer_xray
     _fields_ = [("voxel_size", C.c_double), ("transform", C.c_double * 7)]
 
 
+class MapWriterGridOptions(C.Structure):   # dl_map_writer_grid_options
+    _fields_ = [("resolution", C.c_double), ("hit_probability", C.c_double), ("miss_probability", C.c_double),
+                ("insert_free_space", C.c_int32), ("reserved", C.c_int32)]
+
+
+class MapWriterGridInfo(C.Structure):   # dl_map_writer_grid_info
+    _fields_ = [("resolution", C.c_double), ("max_x", C.c_double), ("max_y", C.c_double), ("num_x_cells", C.c_int32),
+                ("num_y_cells", C.c_int32), ("offset_x", C.c_int32), ("offset_y", C.c_int32), ("width", C.c_int32),
+                ("height", C.c_int32)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class MapWriterInfo(C.Structure):   # dl_map_writer_info
     _fields_ = [("pass_", C.c_int32), ("final_pass", C.c_int32), ("num_rows", C.c_int64), ("dropped_no_pose", C.c_int64),
                 ("dropped_range", C.c_int64), ("dropped_moving", C.c_int64), ("messages_without_batch", C.c_int64),
@@ -536,6 +550,8 @@ def lib():
     L.dl_map_writer_add_color.argtypes = [vp, ip(MapWriterColor)]
     L.dl_map_writer_add_xray.argtypes = [vp, ip(MapWriterXray), ip(C.c_int32)]
     L.dl_map_writer_xray_image.argtypes = [vp, C.c_int32, C.c_int64, vp, ip(C.c_int32), ip(C.c_int32)]
+    L.dl_map_writer_add_probability_grid.argtypes = [vp, ip(MapWriterGridOptions), ip(C.c_int32)]
+    L.dl_map_writer_probability_grid.argtypes = [vp, C.c_int32, ip(MapWriterGridInfo), C.c_int64, vp, vp]
     L.dl_rotational_histogram.argtypes = [vp, f32p, C.c_int64, C.c_int32, f32p]
     L.dl_submap_textures.argtypes = [vp, C.c_int32, ip(SubmapImageQuery), ip(SubmapTexture), C.c_int64, vp, ip(C.c_int64)]
     L.dl_submap_projections.argtypes = [vp, C.c_int32, ip(SubmapImageQuery), ip(SubmapProjection), C.c_int64, vp,
@@ -1398,6 +1414,27 @@ class MapWriter:
                                                                C.byref(h)))
         return img
 
+    def add_probability_grid(self, resolution, hit, miss, insert_free_space=True):
+        """write_probability_grid / write_ros_map of the final pass's batches (range_data_inserter: hit_probability,
+        miss_probability, insert_free_space) -> the stage number for probability_grid()."""
+        o = MapWriterGridOptions()
+        o.resolution, o.hit_probability, o.miss_probability = float(resolution), float(hit), float(miss)
+        o.insert_free_space = int(bool(insert_free_space))
+        stage = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_map_writer_add_probability_grid(self.h, C.byref(o), C.byref(stage)))
+        return stage.value
+
+    def probability_grid(self, stage):
+        """After the final flush: (info dict, cells (height, width) uint16, pixels (height, width) uint8) of the cropped box
+        (ComputeCroppedLimits; DrawProbabilityGrid's grey values, unrotated)."""
+        info = MapWriterGridInfo()
+        self.ctx.check(self.ctx.L.dl_map_writer_probability_grid(self.h, int(stage), C.byref(info), 0, None, None))
+        cells = np.zeros((info.height, info.width), np.uint16)
+        pixels = np.zeros((info.height, info.width), np.uint8)
+        self.ctx.check(self.ctx.L.dl_map_writer_probability_grid(self.h, int(stage), C.byref(info), cells.size,
+                                                                 cells.ctypes.data, pixels.ctypes.data))
+        return info.as_dict(), cells, pixels
+
     @staticmethod
     def messages(msgs):
         """[(stamp ticks, first_row, num_rows, trajectory_id, sensor_to_tracking7[, frame_id])] -> a dl_map_message array"""
@@ -1507,6 +1544,40 @@ def write_png(path, argb):
     data = png_bytes(argb)
     with open(path, "wb") as f:
         f.write(data)
+
+
+def grey_argb(pixels):
+    """(height, width) uint8 grey values -> Cairo ARGB32 words (r = g = b), what png_bytes takes."""
+    v = np.asarray(pixels, np.uint32)
+    return 0xFF000000 | (v << 16) | (v << 8) | v
+
+
+def write_probability_grid_png(path, pixels):
+    """write_probability_grid (draw_trajectories = false): the grey image of MapWriter.probability_grid as an RGB PNG."""
+    write_png(path, grey_argb(pixels))
+
+
+def ros_map_bytes(info, pixels, pgm_filename):
+    """write_ros_map (ros_map_writing_points_processor.cc:59-80, ros_map.cc): the image rotated 90 degrees clockwise
+    (Image::Rotate90DegreesClockwise), WritePgm's bytes and WriteYaml's bytes (std::to_string is %f) -> (pgm, yaml)."""
+    rotated = np.rot90(np.asarray(pixels, np.uint8), -1)
+    height, width = rotated.shape
+    res = info["resolution"]
+    pgm = (f"P5\n# Cartographer map; {res:f} m/pixel\n{width} {height}\n255\n").encode() + rotated.tobytes()
+    origin_x = info["max_x"] - (info["offset_y"] + width) * res
+    origin_y = info["max_y"] - (info["offset_x"] + height) * res
+    yaml = (f"image: {pgm_filename}\nresolution: {res:f}\norigin: [{origin_x:f}, {origin_y:f}, 0.0]\nnegate: 0\n"
+            "occupied_thresh: 0.65\nfree_thresh: 0.196\n").encode()
+    return pgm, yaml
+
+
+def write_ros_map(filestem, info, pixels):
+    """<filestem>.pgm and <filestem>.yaml as the reference writes them (the YAML names the PGM as opened)."""
+    pgm, yaml = ros_map_bytes(info, pixels, filestem + ".pgm")
+    with open(filestem + ".pgm", "wb") as f:
+        f.write(pgm)
+    with open(filestem + ".yaml", "wb") as f:
+        f.write(yaml)
 
 
 _CRC_TABLE = None

@@ -9,6 +9,8 @@
 //   mapping::LocalTrajectoryBuilder3D                        C/mapping/internal/3d/local_trajectory_builder_3d.h:81-113
 //   io::MapWriter, io::PcdWritingPointsProcessor             cartographer_ros/assets_writer.cc:120-160, C/io/*_points_processor.cc
 //   io::ColoringPointsProcessor, io::XRayPointsProcessor     C/io/coloring_points_processor.cc, C/io/xray_points_processor.cc
+//   io::ProbabilityGridPointsProcessor, io::DrawProbabilityGrid  C/io/probability_grid_points_processor.cc
+//   cartographer_ros::RosMapWritingPointsProcessor           cartographer_ros/ros_map_writing_points_processor.cc, ros_map.cc
 //   transform::RollPitchYaw                                  C/transform/rigid_transform.cc:40-46
 // Eigen / protobuf types are replaced by the plain structs below (this image has neither); INTEGRATION.md shows
 // the three-line adapters for Eigen::Vector3f / transform::Rigid3d / proto options in a real Cartographer tree.
@@ -1024,6 +1026,28 @@ class MapWriter {
     ctx_->check(dl_map_writer_add_xray(writer_, &x, &stage));
     return stage;
   }
+  // A probability-grid stage (what ProbabilityGridPointsProcessor and RosMapWritingPointsProcessor call).
+  int AddProbabilityGrid(double resolution, double hit_probability, double miss_probability, bool insert_free_space = true) {
+    dl_map_writer_grid_options o{};
+    o.resolution = resolution;
+    o.hit_probability = hit_probability;
+    o.miss_probability = miss_probability;
+    o.insert_free_space = insert_free_space ? 1 : 0;
+    int32_t stage = 0;
+    ctx_->check(dl_map_writer_add_probability_grid(writer_, &o, &stage));
+    return stage;
+  }
+  // After the final Flush: the grid's limits and cropped box; the cropped cells and grey pixels, row-major.
+  dl_map_writer_grid_info ProbabilityGrid(int stage, std::vector<uint16_t>* cells, std::vector<uint8_t>* pixels) const {
+    dl_map_writer_grid_info info{};
+    ctx_->check(dl_map_writer_probability_grid(writer_, stage, &info, 0, nullptr, nullptr));
+    const size_t n = (size_t)info.width * (size_t)info.height;
+    if (cells) cells->assign(n, 0);
+    if (pixels) pixels->assign(n, 0);
+    ctx_->check(dl_map_writer_probability_grid(writer_, stage, &info, (int64_t)n, cells ? cells->data() : nullptr,
+                                               pixels ? pixels->data() : nullptr));
+    return info;
+  }
   // After the final Flush: Cairo ARGB32 words, row-major; 0 x 0 for an empty bounding box.
   std::vector<uint32_t> XRayImage(int stage, int* width, int* height) const {
     int32_t w = 0, h = 0;
@@ -1141,6 +1165,62 @@ class XRayPointsProcessor {
   std::string output_filename_;
 };
 
+inline void WriteFile(const std::string& path, const std::string& bytes) {
+  std::FILE* f = std::fopen(path.c_str(), "wb");
+  if (!f) throw Error(DL_ERR_ARG, "cannot open " + path);
+  const bool ok = std::fwrite(bytes.data(), 1, bytes.size(), f) == bytes.size();
+  if (std::fclose(f) != 0 || !ok) throw Error(DL_ERR_ARG, "write failed: " + path);
+}
+
+// io::Image of DrawProbabilityGrid: grey values (r = g = b), row-major.
+struct GreyImage {
+  int width = 0, height = 0;
+  std::vector<uint8_t> pixels;
+  // Image::Rotate90DegreesClockwise (io/image.cc:67-76)
+  void Rotate90DegreesClockwise() {
+    std::vector<uint8_t> out;
+    out.reserve(pixels.size());
+    for (int x = 0; x < width; ++x)
+      for (int y = height - 1; y >= 0; --y) out.push_back(pixels[(size_t)y * width + x]);
+    pixels.swap(out);
+    std::swap(width, height);
+  }
+};
+
+// io::DrawProbabilityGrid (io/probability_grid_points_processor.cc:127-148) of a grid stage after the writer's final Flush:
+// the cropped box (1 x 1 at offset 0 for an empty grid), 128 for unknown cells; *info receives the limits and the offset.
+inline GreyImage DrawProbabilityGrid(const MapWriter& writer, int stage, dl_map_writer_grid_info* info) {
+  GreyImage image;
+  *info = writer.ProbabilityGrid(stage, nullptr, &image.pixels);
+  image.width = info->width;
+  image.height = info->height;
+  return image;
+}
+
+// io::ProbabilityGridPointsProcessor with draw_trajectories = false: Flush, after the writer's final Flush, writes
+// <filename>.png (grey in 8-bit RGB, PngBytes).
+class ProbabilityGridPointsProcessor {
+ public:
+  ProbabilityGridPointsProcessor(MapWriter* writer, double resolution, double hit_probability, double miss_probability,
+                                 bool insert_free_space, const std::string& filename)
+      : writer_(writer), stage_(writer->AddProbabilityGrid(resolution, hit_probability, miss_probability, insert_free_space)),
+        filename_(filename) {}
+  void Flush() const {
+    dl_map_writer_grid_info info;
+    const GreyImage image = DrawProbabilityGrid(*writer_, stage_, &info);
+    std::vector<uint32_t> argb(image.pixels.size());
+    for (size_t i = 0; i < argb.size(); ++i) argb[i] = 0xFF000000u | image.pixels[i] * 0x010101u;
+    const std::vector<uint8_t> png = PngBytes(argb, image.width, image.height);
+    WriteFile(filename_ + ".png", std::string(png.begin(), png.end()));
+  }
+  int stage() const { return stage_; }
+
+ private:
+  MapWriter* writer_;
+  int stage_;
+  std::string filename_;
+};
+
 // io::PcdWritingPointsProcessor (io/pcd_writing_points_processor.cc:35-130): binary PCD v0.7, x y z floats, no colour. The header
 // (WIDTH and POINTS zero-padded to 15 digits) is written before the first points and rewritten with the count at Flush.
 class PcdWritingPointsProcessor {
@@ -1181,4 +1261,55 @@ class PcdWritingPointsProcessor {
 };
 
 }  // namespace io
+
+namespace cartographer_ros {
+
+// std::to_string(double): "%f"
+inline std::string ToString(double v) {
+  char buf[512];
+  std::snprintf(buf, sizeof(buf), "%f", v);
+  return buf;
+}
+
+// WritePgm (ros_map.cc): the header, then the red channel row by row
+inline std::string PgmBytes(const io::GreyImage& image, double resolution) {
+  std::string out = "P5\n# Cartographer map; " + ToString(resolution) + " m/pixel\n" + std::to_string(image.width) + " " +
+                    std::to_string(image.height) + "\n255\n";
+  out.append(image.pixels.begin(), image.pixels.end());
+  return out;
+}
+
+// WriteYaml (ros_map.cc): map_saver's constants
+inline std::string YamlBytes(double resolution, double origin_x, double origin_y, const std::string& pgm_filename) {
+  return "image: " + pgm_filename + "\n" + "resolution: " + ToString(resolution) + "\n" + "origin: [" + ToString(origin_x) +
+         ", " + ToString(origin_y) + ", 0.0]\nnegate: 0\noccupied_thresh: 0.65\nfree_thresh: 0.196\n";
+}
+
+// cartographer_ros::RosMapWritingPointsProcessor (ros_map_writing_points_processor.cc): Flush, after the writer's final Flush,
+// writes <filestem>.pgm (the image rotated 90 degrees clockwise) and <filestem>.yaml.
+class RosMapWritingPointsProcessor {
+ public:
+  RosMapWritingPointsProcessor(io::MapWriter* writer, double resolution, double hit_probability, double miss_probability,
+                               bool insert_free_space, const std::string& filestem)
+      : writer_(writer), stage_(writer->AddProbabilityGrid(resolution, hit_probability, miss_probability, insert_free_space)),
+        filestem_(filestem) {}
+  void Flush() const {
+    dl_map_writer_grid_info info;
+    io::GreyImage image = io::DrawProbabilityGrid(*writer_, stage_, &info);
+    const std::string pgm_filename = filestem_ + ".pgm";
+    image.Rotate90DegreesClockwise();
+    io::WriteFile(pgm_filename, PgmBytes(image, info.resolution));
+    const double origin_x = info.max_x - (info.offset_y + image.width) * info.resolution;
+    const double origin_y = info.max_y - (info.offset_x + image.height) * info.resolution;
+    io::WriteFile(filestem_ + ".yaml", YamlBytes(info.resolution, origin_x, origin_y, pgm_filename));
+  }
+  int stage() const { return stage_; }
+
+ private:
+  io::MapWriter* writer_;
+  int stage_;
+  std::string filestem_;
+};
+
+}  // namespace cartographer_ros
 }  // namespace dliom

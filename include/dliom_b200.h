@@ -898,8 +898,9 @@ int dl_submap_projections(dl_context* ctx, int32_t count, const dl_submap_image_
  *      grid's largest extent, +-8192 cells per axis (the reference's grid CHECK-fails there, hybrid_grid.h:391), or whose batch
  *      origin's cell does (a ray that long could stall pass 2's float step, where the reference loops forever).
  *      X-ray images (io/xray_points_processor.cc) and color_points (io/coloring_points_processor.cc) of the final pass's points,
- *      see dl_map_writer_add_xray. Not built: intensities, other writers, the fixed-ratio sampler, frame-id filters, bag / tf
- *      reading. ---- */
+ *      see dl_map_writer_add_xray. 2D occupancy grids of the final pass (io/probability_grid_points_processor.cc,
+ *      cartographer_ros/ros_map_writing_points_processor.cc), see dl_map_writer_add_probability_grid. Not built: intensities,
+ *      write_hybrid_grid, write_ply / write_xyz, the fixed-ratio sampler, frame-id filters, bag / tf reading. ---- */
 typedef struct dl_map_writer dl_map_writer;
 typedef struct dl_map_writer_options {
   int32_t range_filter;        /* 1: min_max_range_filter is in the pipeline */
@@ -983,6 +984,46 @@ int dl_map_writer_add_xray(dl_map_writer* writer, const dl_map_writer_xray* xray
  * reference writes no file then). Rejected with DL_ERR_ARG: an unknown stage, a call before the final flush, capacity too small. */
 int dl_map_writer_xray_image(const dl_map_writer* writer, int32_t stage, int64_t capacity, uint32_t* argb, int32_t* width,
                              int32_t* height);
+
+/* ---- 2D occupancy grids of the final pass: write_probability_grid (io/probability_grid_points_processor.cc) and write_ros_map
+ *      (cartographer_ros/ros_map_writing_points_processor.cc) share this stage. Added like an X-ray stage (after create, before
+ *      the first process call, counted against DL_MAP_WRITER_MAX_STAGES with the other kinds); several may coexist.
+ *      Every batch of the final pass (a message whose origin is not NaN, also when the range filter or the moving-object
+ *      removal emptied it) is one ProbabilityGridRangeDataInserter2D::Insert({origin, points, {}}): only x and y are used.
+ *        the grid starts as CreateProbabilityGrid(resolution): 100 x 100 cells, max = 50 * resolution per axis (double);
+ *        GrowAsNeeded: the float box of the origin and the points, GrowLimits(min - 1e-6f) and GrowLimits(max + 1e-6f), each
+ *          doubling both axes around the centre until the cell is contained (grid_2d.cc:116);
+ *        GetCellIndex(p) = (lround((max.y - p.y) / res - 0.5), lround((max.x - p.x) / res - 0.5)) in double;
+ *        CastRays at res / 1000 (ray_casting.cc:166): the hit table on every point's cell, then (insert_free_space) the
+ *          subpixel walk CastRay(origin, point) with the miss table; a cell is updated at most once per batch and a hit wins over
+ *          any miss (kUpdateMarker). The tables are ComputeLookupTableToApplyCorrespondenceCostOdds(Odds((float)p)).
+ *      Rejected with DL_ERR_ARG, the writer unchanged: a stage added after processing began or beyond the cap, a resolution <= 0
+ *      or not finite, hit_probability <= 0.5 or miss_probability >= 0.5 (the reference's CHECKs) or either not finite, and (final
+ *      pass) a point whose x or y is not finite or a batch whose growth would take a grid beyond DL_MAP_WRITER_MAX_GRID_CELLS
+ *      cells per axis (the reference's superscaled num_cells * 1000 must fit an int). A failed allocation returns DL_ERR_CUDA,
+ *      the writer unchanged. A writer returns the same points, origins and info with or without grid stages. ---- */
+#define DL_MAP_WRITER_MAX_GRID_CELLS (100 << 14)
+typedef struct dl_map_writer_grid_options {
+  double resolution;
+  double hit_probability, miss_probability;  /* range_data_inserter: > 0.5 and < 0.5 */
+  int32_t insert_free_space;                 /* 1 (the reference's default) or 0 */
+  int32_t reserved;
+} dl_map_writer_grid_options;
+typedef struct dl_map_writer_grid_info {
+  double resolution, max_x, max_y;           /* MapLimits after the final flush */
+  int32_t num_x_cells, num_y_cells;
+  int32_t offset_x, offset_y;                /* ComputeCroppedLimits: the known-cells box, or 0, 0 and 1 x 1 when it is empty */
+  int32_t width, height;                     /* cropped num_x_cells, num_y_cells */
+} dl_map_writer_grid_info;
+/* *stage receives the grid stage's number (0, 1, ... in the order grid stages were added). */
+int dl_map_writer_add_probability_grid(dl_map_writer* writer, const dl_map_writer_grid_options* options, int32_t* stage);
+/* After the final flush: the grid's limits and cropped box in *info; cells (optional) receives the Grid2D uint16 correspondence-cost
+ * values of the cropped box, row-major (cell (offset_x + x, offset_y + y) at y * width + x, 0 = unknown); pixels (optional)
+ * receives DrawProbabilityGrid's grey values of the same box, unrotated (128 for an unknown cell, else
+ * lround(255 * (((1 - p) - 0.1f) / ((1 - 0.1f) - 0.1f))) in float). Both NULL queries the size; capacity is in cells. Rejected with
+ * DL_ERR_ARG: an unknown stage, a call before the final flush, capacity below width * height. */
+int dl_map_writer_probability_grid(const dl_map_writer* writer, int32_t stage, dl_map_writer_grid_info* info, int64_t capacity,
+                                   uint16_t* cells, uint8_t* pixels);
 
 /* Device memory helpers so a host language without CUDA bindings can stage buffers. */
 int dl_device_alloc(dl_context* ctx, int64_t bytes, void** out_dev);

@@ -10,8 +10,15 @@ With --xray the same invocation also times the final pass with the six X-ray sta
 alternate between the two frame ids) against the final pass without them, alternating the two, and reports the X-ray share of
 the final pass, point-stages per second, the device bytes the stages hold (cudaMemGetInfo difference) and the image sizes.
 
+With --ros-map it times the final pass with one write_ros_map grid stage (assets_writer_ros_map.lua: 0.05 m, hit 0.55, miss
+0.49, insert_free_space) against the final pass without it, alternating the two, and reports the stage's milliseconds, walk cells
+per second, the grid's size and the device bytes the stage holds. Walk cells are counted from the shapes in an untimed run with
+one message per call: per walk |dx| + |dy| + 1 pixels of CastRay's ends at the grid's final limits (a walk through an exact pixel
+corner visits one cell fewer, which this count ignores).
+
     python tools/bench_map_writer.py --scans 300 --voxel 0.05 --repeat 3
     python tools/bench_map_writer.py --scans 300 --voxel 0.05 --repeat 3 --xray
+    python tools/bench_map_writer.py --scans 300 --voxel 0.05 --repeat 3 --ros-map
 """
 import math
 import argparse
@@ -65,6 +72,7 @@ def main():
     ap.add_argument("--repeat", type=int, default=3)
     ap.add_argument("--cpu-scans", type=int, default=2)
     ap.add_argument("--xray", action="store_true", help="also time the final pass with the backpack pipeline's X-ray stages")
+    ap.add_argument("--ros-map", action="store_true", help="also time the final pass with one 0.05 m write_ros_map grid stage")
     args = ap.parse_args()
 
     import torch
@@ -126,6 +134,8 @@ def main():
     }
     if args.xray:
         line["xray"] = bench_xray(ctx, args, times, poses, msgs, rows, rows_dev, out_dev)
+    if args.ros_map:
+        line["ros_map"] = bench_ros_map(ctx, args, times, poses, msgs, rows, rows_dev, out_dev)
     print(json.dumps(line))
 
 
@@ -188,6 +198,74 @@ def bench_xray(ctx, args, times, poses, msgs, rows, rows_dev, out_dev):
             "point_stages_per_s": round(n * stages / ((best_with - best_without) / 1e3)),
             "device_bytes_held_by_stages": int(held_with - held_without), "image_ms_all_stages": round(image_ms, 3),
             "image_sizes_hw": shapes}
+
+
+ROS_MAP = (0.05, 0.55, 0.49)   # assets_writer_ros_map.lua's write_ros_map
+
+
+def walk_cells(ctx, args, times, poses, msgs, rows, info):
+    """Sum over walks of |dx| + |dy| + 1 pixels between CastRay's superscaled ends, at the grid's final limits; the batches
+    come from an untimed writer fed one message per call."""
+    import dliom
+    import probability_grid_reference as pg
+    w = dliom.MapWriter(ctx, range_filter=(args.min_range, args.max_range), outlier_voxel_size=args.voxel)
+    w.add_trajectory(0, times, poses)
+    while True:
+        out = [w.process([m], rows) for m in msgs]
+        if not w.flush():
+            break
+    w.close()
+    ss = pg.Limits(info["resolution"], info["max_x"], info["max_y"], info["num_x_cells"], info["num_y_cells"]).superscaled()
+    total = 0
+    for pts, origin, _ in out:
+        if np.isnan(origin[0][0]) or len(pts) == 0:
+            continue
+        bx, by = ss.cell_index(origin[0][0], origin[0][1])
+        ex, ey = ss.cell_indices(pts[:, 0], pts[:, 1])
+        total += int((np.abs(ex // 1000 - bx // 1000) + np.abs(ey // 1000 - by // 1000) + 1).sum())
+    return total
+
+
+def bench_ros_map(ctx, args, times, poses, msgs, rows, rows_dev, out_dev):
+    import torch
+    import dliom
+
+    def final_pass(with_stage):
+        torch.cuda.synchronize()
+        free0 = torch.cuda.mem_get_info()[0]
+        w = dliom.MapWriter(ctx, range_filter=(args.min_range, args.max_range), outlier_voxel_size=args.voxel)
+        w.add_trajectory(0, times, poses)
+        stage = w.add_probability_grid(*ROS_MAP) if with_stage else None
+        while True:
+            t0 = time.perf_counter()
+            n, _, _ = w.process_dev(msgs, rows_dev.data_ptr(), len(rows), out_dev.data_ptr())
+            ms = (time.perf_counter() - t0) * 1e3    # the call ends in a device synchronise
+            if not w.flush():
+                break
+        held = free0 - torch.cuda.mem_get_info()[0]
+        info = None
+        if with_stage:
+            t0 = time.perf_counter()
+            info, _, _ = w.probability_grid(stage)
+            read_ms = (time.perf_counter() - t0) * 1e3
+        w.close()
+        return ms, n, held, info, (read_ms if with_stage else None)
+
+    final_pass(True)    # warm-up
+    with_ms, without_ms = [], []
+    for _ in range(args.repeat):
+        a = final_pass(False)
+        b = final_pass(True)
+        without_ms.append(a[0])
+        with_ms.append(b[0])
+    n, held_with, info, read_ms = b[1], b[2], b[3], b[4]
+    stage_ms = min(with_ms) - min(without_ms)
+    cells = walk_cells(ctx, args, times, poses, msgs, rows, info)
+    return {"resolution": ROS_MAP[0], "hit": ROS_MAP[1], "miss": ROS_MAP[2], "points": int(n),
+            "final_pass_ms_without": [round(v, 3) for v in without_ms], "final_pass_ms_with": [round(v, 3) for v in with_ms],
+            "stage_ms": round(stage_ms, 3), "walk_cells": cells, "walk_cells_per_s": round(cells / (stage_ms / 1e3)),
+            "grid_cells_xy": [info["num_x_cells"], info["num_y_cells"]], "cropped_wh": [info["width"], info["height"]],
+            "device_bytes_held_by_stage": int(held_with - a[2]), "read_back_ms": round(read_ms, 3)}
 
 
 if __name__ == "__main__":
