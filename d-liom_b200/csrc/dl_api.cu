@@ -752,124 +752,101 @@ struct RtcsmBatchItem {
   float max_scan_range;
   float* d_scores;  // optional
 };
+// plan_rtcsm_batch builds the tables and lays out the one upload (every scan's tables, the descriptors, the CTA prefix); take()
+// carves that upload and the argmax words, so a caller can count the scratch before it reserves it; run_rtcsm_batch uploads
+// and launches.
 struct RtcsmBatchPlan {
   std::vector<RtcsmTables> tables;
+  std::vector<size_t> off_q, off_t, off_pr, off_pt;
+  std::vector<int32_t> prefix;
+  size_t off_scans = 0, off_prefix = 0, blob = 0;
+  unsigned char* d_blob = nullptr;
   RtcsmScan* d_scans = nullptr;
   unsigned long long* d_best = nullptr;
+  void take(Arena& a) {
+    d_blob = a.take<unsigned char>(blob);
+    d_best = a.take<unsigned long long>(tables.size());
+    d_scans = (RtcsmScan*)(d_blob + off_scans);
+  }
 };
-int rtcsm_batch_device(dl_context* ctx, const dl_rtcsm_options& opt, const dl_grid* grid, const std::vector<RtcsmBatchItem>& items,
-                       Arena& a, RtcsmBatchPlan* plan) {
+int plan_rtcsm_batch(dl_context* ctx, const dl_rtcsm_options& opt, float resolution, const std::vector<RtcsmBatchItem>& items,
+                     RtcsmBatchPlan* plan) {
   const int B = (int)items.size();
-  if (B == 0) return DL_OK;
-  plan->tables.resize(B);
-  size_t blob = 0;
+  plan->tables.assign(B, RtcsmTables{});
+  plan->off_q.resize(B); plan->off_t.resize(B); plan->off_pr.resize(B); plan->off_pt.resize(B);
+  plan->prefix.assign(B + 1, 0);
   auto align16 = [](size_t v) { return (v + 15) & ~size_t(15); };
-  std::vector<size_t> off_q(B), off_t(B), off_pr(B), off_pt(B);
-  std::vector<int32_t> prefix(B + 1, 0);
+  size_t blob = 0;
   for (int k = 0; k < B; ++k) {
-    build_rtcsm_tables(opt, grid->resolution, items[k].max_scan_range, to_float(items[k].initial), &plan->tables[k]);
+    build_rtcsm_tables(opt, resolution, items[k].max_scan_range, to_float(items[k].initial), &plan->tables[k]);
     const RtcsmTables& t = plan->tables[k];
     const int64_t R = (int64_t)t.cand_q.size(), L = (int64_t)t.cand_t.size();
     if (R * L >= 0xFFFFFFFFll) return ctx->fail(DL_ERR_ARG, "more than 2^32-1 correlative candidates");
-    off_q[k] = blob; blob = align16(blob + R * sizeof(Quatf));
-    off_t[k] = blob; blob = align16(blob + L * sizeof(Vec3f));
-    off_pr[k] = blob; blob = align16(blob + R * sizeof(double));
-    off_pt[k] = blob; blob = align16(blob + L * sizeof(double));
-    prefix[k + 1] = prefix[k] + rtcsm_ctas_for(R, L);
+    plan->off_q[k] = blob; blob = align16(blob + R * sizeof(Quatf));
+    plan->off_t[k] = blob; blob = align16(blob + L * sizeof(Vec3f));
+    plan->off_pr[k] = blob; blob = align16(blob + R * sizeof(double));
+    plan->off_pt[k] = blob; blob = align16(blob + L * sizeof(double));
+    plan->prefix[k + 1] = plan->prefix[k] + rtcsm_ctas_for(R, L);
   }
-  const size_t off_scans = blob; blob = align16(blob + (size_t)B * sizeof(RtcsmScan));
-  const size_t off_prefix = blob; blob = align16(blob + (size_t)(B + 1) * sizeof(int32_t));
-  unsigned char* d_blob = a.take<unsigned char>(blob);
-  unsigned long long* d_best = a.take<unsigned long long>(B);
-  if (a.off > ctx->d_scratch_bytes) return ctx->fail(DL_ERR_ARG, "internal: RT-CSM scratch underestimated");
-  std::vector<unsigned char> host(blob);
+  plan->off_scans = blob; blob = align16(blob + (size_t)B * sizeof(RtcsmScan));
+  plan->off_prefix = blob; blob = align16(blob + (size_t)(B + 1) * sizeof(int32_t));
+  plan->blob = blob;
+  return DL_OK;
+}
+// `plan` has taken its scratch; items[k].d_points / d_scores are read here.
+int run_rtcsm_batch(dl_context* ctx, const dl_grid* grid, const std::vector<RtcsmBatchItem>& items, const RtcsmBatchPlan& plan) {
+  const int B = (int)items.size();
+  if (B == 0) return DL_OK;
+  std::vector<unsigned char> host(plan.blob);
   for (int k = 0; k < B; ++k) {
-    const RtcsmTables& t = plan->tables[k];
-    std::memcpy(host.data() + off_q[k], t.cand_q.data(), t.cand_q.size() * sizeof(Quatf));
-    std::memcpy(host.data() + off_t[k], t.cand_t.data(), t.cand_t.size() * sizeof(Vec3f));
-    std::memcpy(host.data() + off_pr[k], t.pen_r.data(), t.pen_r.size() * sizeof(double));
-    std::memcpy(host.data() + off_pt[k], t.pen_t.data(), t.pen_t.size() * sizeof(double));
+    const RtcsmTables& t = plan.tables[k];
+    std::memcpy(host.data() + plan.off_q[k], t.cand_q.data(), t.cand_q.size() * sizeof(Quatf));
+    std::memcpy(host.data() + plan.off_t[k], t.cand_t.data(), t.cand_t.size() * sizeof(Vec3f));
+    std::memcpy(host.data() + plan.off_pr[k], t.pen_r.data(), t.pen_r.size() * sizeof(double));
+    std::memcpy(host.data() + plan.off_pt[k], t.pen_t.data(), t.pen_t.size() * sizeof(double));
     RtcsmScan sc{};
     sc.points = items[k].d_points;
     sc.n = (int32_t)items[k].n;
-    sc.cand_q = (const Quatf*)(d_blob + off_q[k]);
-    sc.cand_t = (const Vec3f*)(d_blob + off_t[k]);
-    sc.pen_r = (const double*)(d_blob + off_pr[k]);
-    sc.pen_t = (const double*)(d_blob + off_pt[k]);
+    sc.cand_q = (const Quatf*)(plan.d_blob + plan.off_q[k]);
+    sc.cand_t = (const Vec3f*)(plan.d_blob + plan.off_t[k]);
+    sc.pen_r = (const double*)(plan.d_blob + plan.off_pr[k]);
+    sc.pen_t = (const double*)(plan.d_blob + plan.off_pt[k]);
     sc.R = (int32_t)t.cand_q.size();
     sc.L = (int32_t)t.cand_t.size();
     sc.scores = items[k].d_scores;
-    sc.best = d_best + k;
-    std::memcpy(host.data() + off_scans + (size_t)k * sizeof(RtcsmScan), &sc, sizeof(sc));
+    sc.best = plan.d_best + k;
+    std::memcpy(host.data() + plan.off_scans + (size_t)k * sizeof(RtcsmScan), &sc, sizeof(sc));
   }
-  std::memcpy(host.data() + off_prefix, prefix.data(), (size_t)(B + 1) * sizeof(int32_t));
-  DL_TRY(h2d(ctx, d_blob, host.data(), blob));
-  DL_CUDA(ctx, cudaMemsetAsync(d_best, 0, sizeof(unsigned long long) * B, ctx->stream));
+  std::memcpy(host.data() + plan.off_prefix, plan.prefix.data(), (size_t)(B + 1) * sizeof(int32_t));
+  DL_TRY(h2d(ctx, plan.d_blob, host.data(), plan.blob));
+  DL_CUDA(ctx, cudaMemsetAsync(plan.d_best, 0, sizeof(unsigned long long) * B, ctx->stream));
   DL_TRY(sync(ctx));  // `host` is pageable and local
-  plan->d_scans = (RtcsmScan*)(d_blob + off_scans);
-  plan->d_best = d_best;
-  return launch_rtcsm_batch(ctx, grid->view(), plan->d_scans, (const int32_t*)(d_blob + off_prefix), B, prefix[B]);
+  return launch_rtcsm_batch(ctx, grid->view(), plan.d_scans, (const int32_t*)(plan.d_blob + plan.off_prefix), B, plan.prefix[B]);
 }
 
-// Runs the search for ONE cloud already on the device (the standalone matcher call). Leaves the best pose in pose_out.
-int rtcsm_device(dl_context* ctx, const dl_rtcsm_options& opt, const Rigidd& initial, const float* d_points, int64_t n,
-                 const dl_grid* grid, Arena& a, Rigidd* pose_out, float* score_out, dl_rtcsm_info* info,
-                 float* all_scores_host) {
-  float* d_max = a.take<float>(1);
-  int32_t* d_n = a.take<int32_t>(1);
-  const int32_t n32 = (int32_t)n;
-  DL_TRY(h2d(ctx, d_n, &n32, 1));
-  DL_TRY(launch_max_range_batch(ctx, d_points, 0, d_n, 0, 1, 3.f * grid->resolution, d_max));
-  float max_scan_range = 0.f;
-  DL_TRY(d2h(ctx, &max_scan_range, d_max, 1));
-  DL_TRY(sync(ctx));
-  // size of the score cube is known once the tables are: build them here once to size the optional score buffer
-  RtcsmTables probe;
-  build_rtcsm_tables(opt, grid->resolution, max_scan_range, to_float(initial), &probe);
-  const int64_t R = (int64_t)probe.cand_q.size(), L = (int64_t)probe.cand_t.size(), K = R * L;
-  if (K >= 0xFFFFFFFFll) return ctx->fail(DL_ERR_ARG, "more than 2^32-1 correlative candidates");
-  float* d_scores = all_scores_host ? a.take<float>(K) : nullptr;
-  RtcsmBatchPlan plan;
-  DL_TRY(rtcsm_batch_device(ctx, opt, grid, {RtcsmBatchItem{d_points, n, initial, max_scan_range, d_scores}}, a, &plan));
-  unsigned long long best = 0;
-  DL_TRY(d2h(ctx, &best, plan.d_best, 1));
-  if (all_scores_host) DL_TRY(d2h(ctx, all_scores_host, d_scores, K));
-  DL_TRY(sync(ctx));
-  if (best == 0) return ctx->fail(DL_ERR_SCORE, "no candidate with a positive score (CHECK_GT(score, 0))");
-  const RtcsmTables& t = plan.tables[0];
-  const uint32_t score_bits = (uint32_t)(best >> 32);
-  const int64_t index = (int64_t)(0xFFFFFFFFull - (best & 0xFFFFFFFFull));
-  float score;
-  std::memcpy(&score, &score_bits, 4);
-  const int64_t l = index / R, r = index - l * R;
-  *pose_out = to_double(Rigidf{t.cand_t[l], t.cand_q[r]});
-  if (score_out) *score_out = score;
-  if (info) {
-    info->best_index = index;
-    info->num_candidates = K;
-    info->linear_window = t.linear;
-    info->angular_window = t.angular;
-    info->angular_step = t.step;
-    info->max_scan_range = max_scan_range;
-  }
-  return DL_OK;
+// The farthest point of a host cloud, floored at 3 * resolution (cc:63-71), with the norm the device reduction uses.
+float max_scan_range_host(const float* points, int64_t n, float resolution) {
+  float m = 3.f * resolution;
+  for (int64_t i = 0; i < n; ++i) m = std::max(m, norm3(Vec3f{points[3 * i], points[3 * i + 1], points[3 * i + 2]}));
+  return m;
 }
 
-// Upper bound of the scratch rtcsm_device takes for one cloud, from the options alone. This is the one reservation that cannot
-// be counted from a carve: the candidate tables' size follows from the cloud's farthest point, which a device reduction finds
-// in the middle of the call, when the scratch already holds the call's inputs and cannot grow. So the angular window is
-// bounded by the window / smallest possible step. rtcsm_batch_device checks the bound before it uploads the tables.
-size_t rtcsm_scratch_bound(const dl_rtcsm_options& opt, float resolution, bool scores) {
+// Upper bound of the scratch one scan of the front end's correlative pre-match takes (tables, descriptor, prefix, argmax word).
+// The tables' size follows from the cloud's farthest point, which a device reduction finds after the front end has carved its
+// scratch, so it is bounded from the options. Every point the pre-match sees has passed the high-resolution filter's
+// norm3(p) <= max_range, so max_scan_range <= max(3 * resolution, max_range). The float step does not grow with the range, so
+// A is largest at that range, until the argument of acosf rounds to 1 (about 4096 resolutions): there the step is 0 and A is 0,
+// and below it the step is never smaller than 0.999f * acosf(1 - 2^-24). So A is bounded by its value at max_range, or by the
+// smallest positive step when max_range is past that cliff.
+size_t rtcsm_scratch_bound(const dl_rtcsm_options& opt, float resolution, float max_range) {
   const int L1 = 2 * (int)std::lround(opt.linear_search_window / resolution) + 1;
-  // step >= 0.999 * acos(1 - res^2 / (2 r^2)) with r <= 200 m (beyond any LiDAR the front end accepts)
-  const float r = 200.f;
-  const float step = 0.999f * std::acos(1.f - (resolution * resolution) / (2.f * r * r));
+  const float r = max_range > 3.f * resolution ? max_range : 3.f * resolution;
+  const float kSafetyMargin = 1.f - 1e-3f;
+  float step = kSafetyMargin * std::acos(1.f - (resolution * resolution) / (2.f * (r * r)));
+  if (!(step > 0.f)) step = kSafetyMargin * std::acos(std::nextafter(1.f, 0.f));
   const int A1 = 2 * (int)std::lround(opt.angular_search_window / step) + 1;
   const size_t R = (size_t)A1 * A1 * A1, L = (size_t)L1 * L1 * L1;
-  Arena bound(nullptr);  // rtcsm_device's takes at the largest tables, with room for the blob's 16-byte alignment
-  bound.take<float>(1);
-  bound.take<int32_t>(1);
-  bound.take<float>(scores ? R * L : 0);
+  Arena bound(nullptr);  // the plan's takes at the largest tables, with room for the blob's 16-byte alignment
   bound.take<unsigned char>(R * 16 + L * 12 + R * 8 + L * 8 + 256 + sizeof(RtcsmScan) + 64);
   bound.take<unsigned long long>(1);
   return bound.off + 4096;
@@ -886,14 +863,44 @@ int dl_rtcsm_match(dl_context* ctx, const dl_rtcsm_options* options, const doubl
   if (n == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
   if (grid->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  // The cloud is on the host: its farthest point, hence the tables and the exact scratch, are known before the carve.
+  const float max_scan_range = max_scan_range_host(points, n, grid->resolution);
+  std::vector<RtcsmBatchItem> items{RtcsmBatchItem{nullptr, n, pose_from7(initial_pose), max_scan_range, nullptr}};
+  RtcsmBatchPlan plan;
+  DL_TRY(plan_rtcsm_batch(ctx, *options, grid->resolution, items, &plan));
+  const RtcsmTables& t = plan.tables[0];
+  const int64_t R = (int64_t)t.cand_q.size(), K = R * (int64_t)t.cand_t.size();
   float* d_pts;
-  Arena a(nullptr);
-  DL_TRY(carve_scratch(ctx, [&](Arena& c) { d_pts = c.take<float>(3 * n); },
-                       rtcsm_scratch_bound(*options, grid->resolution, all_scores != nullptr), &a));
+  float* d_scores = nullptr;
+  DL_TRY(carve_scratch(ctx, [&](Arena& c) {
+    d_pts = c.take<float>(3 * n);
+    if (all_scores) d_scores = c.take<float>(K);
+    plan.take(c);
+  }));
   DL_TRY(h2d(ctx, d_pts, points, 3 * n));
-  Rigidd best;
-  DL_TRY(rtcsm_device(ctx, *options, pose_from7(initial_pose), d_pts, n, grid, a, &best, score_out, info, all_scores));
-  pose_to7(best, pose_out);
+  items[0].d_points = d_pts;
+  items[0].d_scores = d_scores;
+  DL_TRY(run_rtcsm_batch(ctx, grid, items, plan));
+  unsigned long long best = 0;
+  DL_TRY(d2h(ctx, &best, plan.d_best, 1));
+  if (all_scores) DL_TRY(d2h(ctx, all_scores, d_scores, K));
+  DL_TRY(sync(ctx));
+  if (best == 0) return ctx->fail(DL_ERR_SCORE, "no candidate with a positive score (CHECK_GT(score, 0))");
+  const uint32_t score_bits = (uint32_t)(best >> 32);
+  const int64_t index = (int64_t)(0xFFFFFFFFull - (best & 0xFFFFFFFFull));
+  float score;
+  std::memcpy(&score, &score_bits, 4);
+  const int64_t l = index / R, r = index - l * R;
+  pose_to7(to_double(Rigidf{t.cand_t[l], t.cand_q[r]}), pose_out);
+  if (score_out) *score_out = score;
+  if (info) {
+    info->best_index = index;
+    info->num_candidates = K;
+    info->linear_window = t.linear;
+    info->angular_window = t.angular;
+    info->angular_step = t.step;
+    info->max_scan_range = max_scan_range;
+  }
   return DL_OK;
 }
 
@@ -2165,7 +2172,10 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
         DL_CUDA(ctx, cudaMemsetAsync(f.rtcsm_scores, 0, sizeof(float) * f.batch, ctx->stream));
         if (!items.empty()) {
           RtcsmBatchPlan plan;
-          DL_TRY(rtcsm_batch_device(ctx, o.real_time_correlative_scan_matcher, hi, items, a, &plan));
+          DL_TRY(plan_rtcsm_batch(ctx, o.real_time_correlative_scan_matcher, hi->resolution, items, &plan));
+          plan.take(a);
+          if (a.off > ctx->d_scratch_bytes) return ctx->fail(DL_ERR_ARG, "internal: RT-CSM scratch underestimated");
+          DL_TRY(run_rtcsm_batch(ctx, hi, items, plan));
           int32_t* d_slots = a.take<int32_t>(items.size());
           DL_TRY(h2d(ctx, d_slots, slots.data(), slots.size()));
           DL_TRY(launch_rtcsm_pick(ctx, plan.d_scans, (int)items.size(), f.initial_pose, d_slots, f.rtcsm_scores, d_slots));
@@ -2281,7 +2291,8 @@ int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int nu
   const int64_t cap = in.on_device ? in.cap_rows : std::max<int64_t>(max_size, 1);
   // The correlative pre-match takes its candidate tables after the carve (see rtcsm_scratch_bound).
   const size_t rtcsm_extra = options->use_online_correlative_scan_matching
-      ? (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, submaps.high(0)->resolution, false)
+      ? (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, submaps.high(0)->resolution,
+                                                options->high_resolution_adaptive_voxel_filter.max_range)
       : 0;
   float* d_ranges;
   dl_scan_result* d_results;
