@@ -1596,11 +1596,7 @@ bool build_imu_term(const Rigidd& to_submap, const dl_nav_state& si, const dl_na
   t->pi[0] = pose_i.t.x; t->pi[1] = pose_i.t.y; t->pi[2] = pose_i.t.z;
   t->qi[0] = pose_i.q.w; t->qi[1] = pose_i.q.x; t->qi[2] = pose_i.q.y; t->qi[3] = pose_i.q.z;
   t->vi[0] = vi.x; t->vi[1] = vi.y; t->vi[2] = vi.z;
-  for (int k = 0; k < 3; ++k) {
-    t->bai[k] = si.ba[k]; t->bgi[k] = si.bg[k];
-    t->dp[k] = m.delta_p[k]; t->dv[k] = m.delta_v[k];
-  }
-  for (int k = 0; k < 4; ++k) t->dq[k] = m.delta_q[k];
+  imu_term_deltas(m, si.ba, si.bg, t);
   t->G[0] = G.x; t->G[1] = G.y; t->G[2] = G.z;
   t->sum_dt = m.sum_dt;
   if (!information_matrix(m.covariance, imu_weight, t->W)) return false;
@@ -1665,6 +1661,70 @@ int dl_imu_predict(const dl_nav_state* si, const dl_preintegration* m, const dou
   sj->p[0] = p.x; sj->p[1] = p.y; sj->p[2] = p.z;
   sj->v[0] = v.x; sj->v[1] = v.y; sj->v[2] = v.z;
   sj->q[0] = q.w; sj->q[1] = q.x; sj->q[2] = q.y; sj->q[3] = q.z;
+  return DL_OK;
+}
+
+int dl_imu_factor_evaluate(dl_context* ctx, int32_t count, const dl_nav_state* states_i, const dl_preintegration* preintegrations,
+                           const double* submap_local_poses, const double* gravity, double imu_weight, const double* x16,
+                           int32_t* ok, dl_nav_state* predicted, double* information, double* residual, double* hessian,
+                           double* gradient, double* cost2) {
+  if (!ctx || count < 0 || !gravity || !(imu_weight >= 0.) ||
+      (count > 0 && (!states_i || !preintegrations || !submap_local_poses || !ok || !predicted || !information || !residual ||
+                     !hessian || !gradient || !cost2)))
+    return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  dl_preintegration* d_pre;
+  dl_nav_state *d_si, *d_pred;
+  Rigidd* d_to_submap;
+  ScanConstants* d_scans;
+  HostImuTerm* d_terms;
+  double *d_init, *d_x, *d_out;
+  int32_t* d_ok;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pre = a.take<dl_preintegration>(count);
+    d_si = a.take<dl_nav_state>(count);
+    d_pred = a.take<dl_nav_state>(count);
+    d_to_submap = a.take<Rigidd>(count);
+    d_scans = a.take<ScanConstants>(count);
+    d_terms = a.take<HostImuTerm>(count);
+    d_init = a.take<double>((size_t)count * 16);
+    d_x = x16 ? a.take<double>((size_t)count * 16) : nullptr;
+    d_out = a.take<double>((size_t)count * kImuFactorOutDoubles);
+    d_ok = a.take<int32_t>(count);
+  }));
+  std::vector<Rigidd> to_submap(count);
+  for (int c = 0; c < count; ++c) to_submap[c] = inverse(pose_from7(submap_local_poses + 7 * c));
+  DL_TRY(h2d(ctx, d_pre, preintegrations, count));
+  DL_TRY(h2d(ctx, d_si, states_i, count));
+  DL_TRY(h2d(ctx, d_to_submap, to_submap.data(), count));
+  if (x16) DL_TRY(h2d(ctx, d_x, x16, (size_t)count * 16));
+  ImuPrepareArgs pa{};
+  pa.count = count; pa.preint = d_pre; pa.states_i = d_si; pa.to_submap = d_to_submap;
+  for (int k = 0; k < 3; ++k) pa.gravity[k] = gravity[k];
+  pa.imu_weight = imu_weight; pa.scans = d_scans; pa.terms = d_terms; pa.init16 = d_init; pa.predicted = d_pred; pa.ok = d_ok;
+  DL_TRY(launch_imu_prepare(ctx, pa));
+  DL_TRY(launch_imu_factor_evaluate(ctx, count, d_terms, d_ok, x16 ? d_x : d_init, d_out));
+  std::vector<HostImuTerm> terms(count);
+  std::vector<double> out((size_t)count * kImuFactorOutDoubles);
+  DL_TRY(d2h(ctx, ok, d_ok, count));
+  DL_TRY(d2h(ctx, predicted, d_pred, count));
+  DL_TRY(d2h(ctx, terms.data(), d_terms, count));
+  DL_TRY(d2h(ctx, out.data(), d_out, out.size()));
+  DL_TRY(sync(ctx));
+  for (int c = 0; c < count; ++c) {
+    const double* o = out.data() + (size_t)c * kImuFactorOutDoubles;
+    const bool good = ok[c] != 0;
+    for (int e = 0; e < 225; ++e) {
+      information[225 * (size_t)c + e] = good ? terms[c].W[e] : 0.0;
+      hessian[225 * (size_t)c + e] = good ? o[15 + e] : 0.0;
+    }
+    for (int e = 0; e < 15; ++e) {
+      residual[15 * (size_t)c + e] = good ? o[e] : 0.0;
+      gradient[15 * (size_t)c + e] = good ? o[240 + e] : 0.0;
+    }
+    cost2[c] = good ? o[255] : 0.0;
+  }
   return DL_OK;
 }
 

@@ -218,11 +218,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) imu_prepare_kernel(ImuPre
     t.pi[0] = pose_i.t.x; t.pi[1] = pose_i.t.y; t.pi[2] = pose_i.t.z;
     t.qi[0] = pose_i.q.w; t.qi[1] = pose_i.q.x; t.qi[2] = pose_i.q.y; t.qi[3] = pose_i.q.z;
     t.vi[0] = wi.x; t.vi[1] = wi.y; t.vi[2] = wi.z;
-    for (int k = 0; k < 3; ++k) {
-      t.bai[k] = si.ba[k]; t.bgi[k] = si.bg[k];
-      t.dp[k] = m.delta_p[k]; t.dv[k] = m.delta_v[k];
-    }
-    for (int k = 0; k < 4; ++k) t.dq[k] = m.delta_q[k];
+    imu_term_deltas(m, si.ba, si.bg, &t);
     t.G[0] = Gs.x; t.G[1] = Gs.y; t.G[2] = Gs.z;
     t.sum_dt = m.sum_dt;
     double* x = a.init16 + 16 * (size_t)b;

@@ -272,6 +272,7 @@ struct FusedOutput {
 };
 // IMU term of the fused solve in the SUBMAP frame (built by dl_api.cu on the host or by imu_prepare_kernel on the device):
 // state i (fixed), the pre-integrated deltas, gravity, and W = weight^2 * Sigma^-1 (row-major 15x15, order p, theta, v, ba, bg).
+// dp, dq, dv carry the bias correction of imu_term_deltas: the residual reads conj(dq) as the inverse of the corrected delta_q.
 struct ImuTerm {
   double pi[3], qi[4], vi[3], bai[3], bgi[3];
   double dp[3], dq[4], dv[3];
@@ -281,10 +282,48 @@ struct ImuTerm {
 };
 constexpr int kImuTermDoubles = 16 + 10 + 3 + 1 + 225;
 static_assert(sizeof(ImuTerm) == kImuTermDoubles * sizeof(double), "ImuTerm layout");
+
+// State i's biases and the pre-integrated deltas of its factor, with the first-order bias correction of
+// integration_base.h:283-290 folded in once per scan (dba = ba_i - linearized_ba, dbg = bg_i - linearized_bg):
+//   dp + J_p,ba dba + J_p,bg dbg,   dv + J_v,ba dba + J_v,bg dbg,   c = delta_q (x) (1, 1/2 J_q,bg dbg).
+// dq holds c / |c|^2, so that its conjugate is Eigen's c.inverse() (the corrected quaternion is not unit). Sums run left to
+// right, like the window smoother's copy of this residual (dl_window.cu). Biases equal to the linearisation point leave the
+// raw deltas, bit for bit. Host (build_imu_term) and device (imu_prepare_kernel).
+DL_HD void imu_term_deltas(const dl_preintegration& m, const double* ba_i, const double* bg_i, ImuTerm* t) {
+  double dba[3], dbg[3];
+  bool at_linearisation = true;
+  for (int k = 0; k < 3; ++k) {
+    t->bai[k] = ba_i[k]; t->bgi[k] = bg_i[k];
+    t->dp[k] = m.delta_p[k]; t->dv[k] = m.delta_v[k];
+    dba[k] = ba_i[k] - m.linearized_ba[k];
+    dbg[k] = bg_i[k] - m.linearized_bg[k];
+    at_linearisation = at_linearisation && dba[k] == 0.0 && dbg[k] == 0.0;
+  }
+  for (int k = 0; k < 4; ++k) t->dq[k] = m.delta_q[k];
+  if (at_linearisation) return;
+  const double* J = m.jacobian;
+  auto blk = [&](int r, int c, const double* d) {  // row r of the 3x3 block at (r, c) times d
+    return J[r * 15 + c] * d[0] + J[r * 15 + c + 1] * d[1] + J[r * 15 + c + 2] * d[2];
+  };
+  double th[3];
+  for (int k = 0; k < 3; ++k) {
+    t->dp[k] = m.delta_p[k] + blk(k, 9, dba) + blk(k, 12, dbg);
+    t->dv[k] = m.delta_v[k] + blk(6 + k, 9, dba) + blk(6 + k, 12, dbg);
+    th[k] = blk(3 + k, 12, dbg);
+  }
+  const Quatd c = qmul(Quatd{m.delta_q[0], m.delta_q[1], m.delta_q[2], m.delta_q[3]}, Quatd{1.0, 0.5 * th[0], 0.5 * th[1], 0.5 * th[2]});
+  const double n2 = (c.x * c.x + c.y * c.y) + (c.z * c.z + c.w * c.w);
+  t->dq[0] = c.w / n2; t->dq[1] = c.x / n2; t->dq[2] = c.y / n2; t->dq[3] = c.z / n2;
+}
 int launch_nls_fused(dl_context* ctx, const NlsOptions& opt, const NlsProblem* problems_dev, const ImuTerm* imu_terms_dev,
                      const double* initial16_dev, int count, FusedOutput* out_dev);
 int launch_nls_normal_equations(dl_context* ctx, const NlsOptions& opt, const NlsProblem* problems_dev,
                                 const double* at_pose_dev, double* out28_dev);
+// The fused solve's IMU normal equations of each prepared factor at x16_dev (16 doubles per factor, submap frame), into
+// kImuFactorOutDoubles doubles per factor: residual (15), H (225, row-major), g (15), r^T W r. Factors with ok == 0 are skipped.
+constexpr int kImuFactorOutDoubles = 15 + 225 + 15 + 1;
+int launch_imu_factor_evaluate(dl_context* ctx, int count, const ImuTerm* terms_dev, const int32_t* ok_dev, const double* x16_dev,
+                               double* out_dev);
 int launch_imu_preintegrate(dl_context* ctx, int count, const int32_t* offsets, const double* dts, const double* accs,
                             const double* gyrs, const double* biases, int bias_stride, const dl_imu_noise& noise,
                             dl_preintegration* out);

@@ -861,6 +861,27 @@ __global__ void __launch_bounds__(kBlock) nls_normal_equations_kernel(NlsOptions
   }
 }
 
+// The IMU term of the fused solve alone, one warp per prepared factor: residual, H = J^T W J, g = J^T W r and r^T W r at x16
+// (submap frame). Factors whose covariance was not positive definite (ok == 0) are skipped.
+__global__ void __launch_bounds__(32) imu_factor_evaluate_kernel(const ImuTerm* __restrict__ terms, const int32_t* __restrict__ ok,
+                                                                 const double* __restrict__ x16, double* __restrict__ out) {
+  __shared__ ImuShared is;
+  __shared__ double x[16];
+  const int b = blockIdx.x, lane = threadIdx.x;
+  if (!ok[b]) return;
+  for (int e = lane; e < 225; e += 32) is.W[e] = terms[b].W[e];
+  if (lane < 16) x[lane] = x16[16 * (size_t)b + lane];
+  __syncwarp();
+  imu_normal_equations(terms[b], x, is, lane);
+  double* o = out + (size_t)b * kImuFactorOutDoubles;  // r(15) H(225) g(15) cost2
+  if (lane < 15) {
+    o[lane] = is.r[lane];
+    o[240 + lane] = is.g[lane];
+  }
+  for (int e = lane; e < 225; e += 32) o[15 + e] = is.H[e / 15][e % 15];
+  if (lane == 0) o[255] = is.cost2;
+}
+
 __global__ void interpolate_kernel(GridView g, int64_t n, const double* __restrict__ xyz, double* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -916,6 +937,14 @@ int launch_nls_normal_equations(dl_context* ctx, const NlsOptions& opt, const Nl
                                 const double* at_pose_dev, double* out28_dev) {
   nls_normal_equations_kernel<<<1, kBlock, 0, ctx->stream>>>(opt, problems_dev, at_pose_dev, out28_dev);
   DL_LAUNCH_CHECK(ctx, "nls_normal_equations_kernel");
+  return DL_OK;
+}
+
+int launch_imu_factor_evaluate(dl_context* ctx, int count, const ImuTerm* terms_dev, const int32_t* ok_dev, const double* x16_dev,
+                               double* out_dev) {
+  if (count <= 0) return DL_OK;
+  imu_factor_evaluate_kernel<<<count, 32, 0, ctx->stream>>>(terms_dev, ok_dev, x16_dev, out_dev);
+  DL_LAUNCH_CHECK(ctx, "imu_factor_evaluate_kernel");
   return DL_OK;
 }
 

@@ -27,7 +27,7 @@ EXPORTS = [
     "dl_grid_sync", "dl_grid_resolution", "dl_grid_num_bricks", "dl_grid_lookup", "dl_grid_interpolate",
     "dl_grid_insert_range_data", "dl_submap_insert_range_data", "dl_grid_export_cells",
     "dl_voxel_filter", "dl_voxel_indices", "dl_adaptive_voxel_filter", "dl_rtcsm_match", "dl_fcsm_match_3dof", "dl_fcsm_match", "dl_constraint_search_batch", "dl_ceres_match",
-    "dl_ceres_match_batch", "dl_ceres_normal_equations", "dl_imu_preintegrate", "dl_imu_predict", "dl_fused_match_batch", "dl_ingest_scan", "dl_decode_point_cloud2", "dl_decode_point_cloud2_dev", "dl_frontend_match_batch", "dl_frontend_match_batch_imu", "dl_frontend_submit", "dl_frontend_collect",
+    "dl_ceres_match_batch", "dl_ceres_normal_equations", "dl_imu_preintegrate", "dl_imu_predict", "dl_imu_factor_evaluate", "dl_fused_match_batch", "dl_ingest_scan", "dl_decode_point_cloud2", "dl_decode_point_cloud2_dev", "dl_frontend_match_batch", "dl_frontend_match_batch_imu", "dl_frontend_submit", "dl_frontend_collect",
     "dl_frontend_match_batch_dev", "dl_frontend_fetch_results", "dl_device_alloc", "dl_device_free",
     "dl_copy_to_device", "dl_copy_to_host",
     "dl_frontend_match_batch_imu_samples", "dl_frontend_match_batch_imu_samples_dev", "dl_frontend_submit_imu_samples",
@@ -496,6 +496,8 @@ def lib():
                                             f64p, f64p, f64p]
     L.dl_imu_preintegrate.argtypes = [vp, ip(ImuNoise), C.c_int32, i32p, f64p, f64p, f64p, f64p, ip(Preintegration)]
     L.dl_imu_predict.argtypes = [ip(NavState), ip(Preintegration), f64p, ip(NavState)]
+    L.dl_imu_factor_evaluate.argtypes = [vp, C.c_int32, ip(NavState), ip(Preintegration), f64p, f64p, C.c_double, vp, i32p,
+                                         ip(NavState), f64p, f64p, f64p, f64p, f64p]
     L.dl_fused_match_batch.argtypes = [vp, ip(CeresOptions), C.c_double, f64p, C.c_int32, C.c_int32, f64p, ip(NavState),
                                        ip(NavState), ip(Preintegration), ip(vp), i64p, ip(vp), ip(NavState),
                                        ip(SolveSummary)]
@@ -963,6 +965,24 @@ class Context:
         si, sj = NavState.from16(state_i16), NavState()
         self.check(self.L.dl_imu_predict(C.byref(si), C.byref(m), np.ascontiguousarray(gravity, np.float64), C.byref(sj)))
         return sj.to16()
+
+    def imu_factor_evaluate(self, states_i, preints, submap_poses, imu_weight=1.0, gravity=(0.0, 0.0, 9.8), x16=None):
+        """The fused solve's IMU factor alone (dl_imu_factor_evaluate). states_i: [n,16] local frame; preints: Preintegration
+        structs; submap_poses: [n,7]; x16: [n,16] in the submap frame or None (the prepared start). -> dict of ok [n],
+        predicted [n,16], information [n,15,15], residual [n,15], hessian [n,15,15], gradient [n,15], cost2 [n]."""
+        n = len(preints)
+        si = (NavState * n)(*[NavState.from16(x) for x in states_i])
+        pm = (Preintegration * n)(*preints)
+        pred = (NavState * n)()
+        ok = np.zeros(n, np.int32)
+        info, hess = np.zeros((n, 15, 15)), np.zeros((n, 15, 15))
+        res, grad, cost2 = np.zeros((n, 15)), np.zeros((n, 15)), np.zeros(n)
+        x = None if x16 is None else np.ascontiguousarray(x16, np.float64).reshape(n, 16)
+        self.check(self.L.dl_imu_factor_evaluate(self.h, n, si, pm, np.ascontiguousarray(submap_poses, np.float64).reshape(n, 7),
+                                                 np.ascontiguousarray(gravity, np.float64), float(imu_weight),
+                                                 None if x is None else x.ctypes.data, ok, pred, info, res, hess, grad, cost2))
+        return {"ok": ok, "predicted": np.array([p.to16() for p in pred]), "information": info, "residual": res,
+                "hessian": hess, "gradient": grad, "cost2": cost2}
 
     def fused_match_batch(self, problems, grids_per_problem, occ_weights, trans_w, rot_w, submap_poses, states_i,
                           initial_states_j, preints, imu_weight=1.0, gravity=(0.0, 0.0, 9.8), nonmono=False, max_iter=12):

@@ -511,10 +511,24 @@ int dl_imu_preintegrate(dl_context* ctx, const dl_imu_noise* noise, int32_t coun
                         dl_preintegration* out);
 /* State at the end of the interval (the front end's pose prediction, LTB:188-199). gravity: 3 doubles (+9.8 z). */
 int dl_imu_predict(const dl_nav_state* state_i, const dl_preintegration* m, const double* gravity, dl_nav_state* state_j);
+/* The IMU factor of the fused solve alone, for kernel-level checks: the device preparation of dl_frontend_match_batch_imu_samples
+ * (prediction, factor in the submap frame, information matrix) followed by the solve's IMU normal equations, for `count`
+ * independent (states_i[k], preintegrations[k], submap_local_poses[k]) triples. x16: 16 doubles per factor (p q v ba bg of
+ * state j in the SUBMAP frame) at which the equations are evaluated, or NULL for the prepared start (the prediction).
+ * Outputs per factor: ok (0: the covariance is not positive definite, every other output of the factor is zero), the
+ * predicted state (local frame), information = imu_weight^2 * covariance^-1 (225, row-major), residual (15), hessian = J^T W J
+ * (225), gradient = J^T W r (15) and cost2 = r^T W r. Order p, theta, v, b_a, b_g; theta perturbs q on the left
+ * (q <- (cos|d|, sin|d|/|d| d) (x) q). */
+int dl_imu_factor_evaluate(dl_context* ctx, int32_t count, const dl_nav_state* states_i, const dl_preintegration* preintegrations,
+                           const double* submap_local_poses, const double* gravity, double imu_weight, const double* x16,
+                           int32_t* ok, dl_nav_state* predicted, double* information, double* residual, double* hessian,
+                           double* gradient, double* cost2);
 /* Fused scan match for `count` independent problems: state i fixed, the 15 local parameters of state j estimated
  * from the occupied-space residuals (+ optional translation / rotation priors of `options`) and the IMU residual
  * weighted by imu_weight^2 * covariance^-1. States are in the local frame; submap_local_poses (7 doubles each) place
- * the grids. Arrays indexed like dl_ceres_match_batch. */
+ * the grids. Arrays indexed like dl_ceres_match_batch. preintegrations[k] may be linearised at other biases than
+ * states_i[k]'s: the factor then takes the first-order bias correction of integration_base.h:283-290 (delta_p, delta_v
+ * and delta_q moved by the bias blocks of the pre-integration's Jacobian), as the window smoother does. */
 int dl_fused_match_batch(dl_context* ctx, const dl_ceres_options* options, double imu_weight, const double* gravity,
                          int32_t count, int32_t num_pairs, const double* submap_local_poses,
                          const dl_nav_state* states_i, const dl_nav_state* initial_states_j,
@@ -649,7 +663,8 @@ int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options,
  * scan, predicted_states[k] = dl_imu_predict(states_i[k], preintegrations[k]) provides the pose prediction (its pose is what
  * the plain call takes as predicted_poses; prev_poses[k] is states_i[k]'s pose) and the initial velocity and biases.
  * states_out[k] receives the estimated state of scan k (local frame); results[k] as in the plain call, with the pose part
- * of the state. An EXTENSION like dl_fused_match_batch: the reference chains the plain match and a GTSAM update. */
+ * of the state. preintegrations[k] may be linearised at other biases than states_i[k]'s (bias correction as in
+ * dl_fused_match_batch). An EXTENSION like dl_fused_match_batch: the reference chains the plain match and a GTSAM update. */
 typedef struct dl_frontend_imu {
   double imu_weight;
   double gravity[3];

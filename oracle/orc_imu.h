@@ -188,16 +188,36 @@ inline NavState imu_predict(const NavState& i, const Preintegration& m, const V3
   return j;
 }
 
-// The 15 residuals (order p, theta, v, ba, bg) of integration_base.h:267-301 with state i's biases equal to the
-// linearisation biases, and their Jacobian (15 x 15) w.r.t. the local parameters of state j.
+// The 15 residuals (order p, theta, v, ba, bg) of integration_base.h:267-301, and their Jacobian (15 x 15) w.r.t. the
+// local parameters of state j. State i's biases may differ from the linearisation biases m.ba / m.bg: the deltas then take
+// the first-order correction of :283-290 (corrected_delta_p / _v, corrected_delta_q = delta_q * deltaQ(J_q,bg dbg), whose
+// Eigen inverse() divides the conjugate by the squared norm). Sums run left to right. At the linearisation biases the raw
+// deltas are used as they are.
 inline void imu_residual(const NavState& si, const NavState& sj, const Preintegration& m, const V3d& G, double* r,
                          double (*J)[15]) {
   const double T = m.sum_dt;
+  const V3d dba = si.ba - m.ba, dbg = si.bg - m.bg;
+  V3d dp = m.delta_p, dv = m.delta_v;
+  Quatd dq_inv = conj(m.delta_q);
+  if (!(dba.x == 0 && dba.y == 0 && dba.z == 0 && dbg.x == 0 && dbg.y == 0 && dbg.z == 0)) {
+    auto blk = [&](int r0, int c0, const V3d& d) {
+      const double(*Jm)[15] = m.jacobian;
+      return V3d{Jm[r0][c0] * d.x + Jm[r0][c0 + 1] * d.y + Jm[r0][c0 + 2] * d.z,
+                 Jm[r0 + 1][c0] * d.x + Jm[r0 + 1][c0 + 1] * d.y + Jm[r0 + 1][c0 + 2] * d.z,
+                 Jm[r0 + 2][c0] * d.x + Jm[r0 + 2][c0 + 1] * d.y + Jm[r0 + 2][c0 + 2] * d.z};
+    };
+    dp = m.delta_p + blk(0, 9, dba) + blk(0, 12, dbg);
+    dv = m.delta_v + blk(6, 9, dba) + blk(6, 12, dbg);
+    const V3d th = blk(3, 12, dbg);
+    const Quatd c = qmul(m.delta_q, Quatd{1.0, 0.5 * th.x, 0.5 * th.y, 0.5 * th.z});
+    const double n2 = (c.x * c.x + c.y * c.y) + (c.z * c.z + c.w * c.w);
+    dq_inv = {c.w / n2, -c.x / n2, -c.y / n2, -c.z / n2};
+  }
   const Quatd qi_inv = conj(si.q);
-  const V3d rp = rotate(qi_inv, scale(0.5 * T * T, G) + sj.p - si.p - scale(T, si.v)) - m.delta_p;
-  const Quatd A = qmul(conj(m.delta_q), qi_inv);
+  const V3d rp = rotate(qi_inv, scale(0.5 * T * T, G) + sj.p - si.p - scale(T, si.v)) - dp;
+  const Quatd A = qmul(dq_inv, qi_inv);
   const Quatd e = qmul(A, sj.q);
-  const V3d rv = rotate(qi_inv, scale(T, G) + sj.v - si.v) - m.delta_v;
+  const V3d rv = rotate(qi_inv, scale(T, G) + sj.v - si.v) - dv;
   r[0] = rp.x; r[1] = rp.y; r[2] = rp.z;
   r[3] = 2 * e.x; r[4] = 2 * e.y; r[5] = 2 * e.z;
   r[6] = rv.x; r[7] = rv.y; r[8] = rv.z;
