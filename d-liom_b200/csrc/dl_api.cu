@@ -3412,6 +3412,21 @@ int dl_ltb_get_submap(dl_local_trajectory_builder* b, int32_t index, dl_grid** h
   return b->ctx->fail(DL_ERR_ARG, "no submap with this index");
 }
 
+int dl_ltb_release_submap(dl_local_trajectory_builder* b, int32_t index) {
+  if (!b) return DL_ERR_ARG;
+  for (LtbSubmap& s : b->finished)
+    if (s.index == index) {
+      if (!s.hi) return b->ctx->fail(DL_ERR_ARG, "the submap's grids were already released");
+      dl_grid_destroy(s.hi);
+      dl_grid_destroy(s.lo);
+      s.hi = s.lo = nullptr;
+      return DL_OK;
+    }
+  for (const LtbSubmap& s : b->active)
+    if (s.index == index) return b->ctx->fail(DL_ERR_ARG, "an active submap cannot be released");
+  return b->ctx->fail(DL_ERR_ARG, "no submap with this index");
+}
+
 int dl_ltb_get_state(const dl_local_trajectory_builder* b, dl_nav_state* state, int32_t* initialized) {
   if (!b) return DL_ERR_ARG;
   if (state) *state = b->prev_state;

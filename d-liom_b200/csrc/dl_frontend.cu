@@ -249,18 +249,8 @@ __global__ void __launch_bounds__(kTileBlock) fe_first_filter_tile(FrontendArgs 
 
 // ---------------------------------------------------------------------------------------------------- B
 __device__ __forceinline__ Rigidd interpolate_pose(double s, const ScanConstants& c) {
-  double scale0, scale1;
-  if (c.linear_slerp) {
-    scale0 = 1.0 - s;
-    scale1 = s;
-  } else {
-    scale0 = sin((1.0 - s) * c.theta) / c.sin_theta;
-    scale1 = sin(s * c.theta) / c.sin_theta;
-  }
-  if (c.negative_dot) scale1 = -scale1;
   Rigidd out;
-  out.q = {scale0 * 1.0 + scale1 * c.rel.q.w, scale0 * 0.0 + scale1 * c.rel.q.x, scale0 * 0.0 + scale1 * c.rel.q.y,
-           scale0 * 0.0 + scale1 * c.rel.q.z};
+  out.q = slerp(Quatd{1.0, 0.0, 0.0, 0.0}, c.rel.q, s, c.slerp);
   out.t = mul(s, c.rel.t);
   return out;
 }

@@ -33,6 +33,7 @@
 #include <cub/cub.cuh>
 
 #include "dl_internal.cuh"
+#include "dl_pipeline.cuh"
 
 using namespace dl;
 
@@ -44,8 +45,7 @@ constexpr unsigned long long kEmpty = ~0ull;
 
 struct NodeRec {          // node i of a trajectory, and the slerp constants of the interval (i - 1, i), computed on the host
   Rigidd pose;
-  double theta, sin_theta;
-  int32_t linear, negative;
+  SlerpConstants slerp;
 };
 struct TrajRec {
   int64_t first, count;   // nodes [first, first + count) of the writer's node arrays
@@ -188,17 +188,7 @@ __device__ bool lookup(const int64_t* times, const NodeRec* nodes, int64_t count
   const double factor = ((double)(tick - times[lo - 1]) / 1e7) / duration;
   out->t = {s.pose.t.x + (e.pose.t.x - s.pose.t.x) * factor, s.pose.t.y + (e.pose.t.y - s.pose.t.y) * factor,
             s.pose.t.z + (e.pose.t.z - s.pose.t.z) * factor};
-  double scale0, scale1;  // Eigen QuaternionBase::slerp; theta and sin(theta) of the interval come from the host
-  if (e.linear) {
-    scale0 = 1.0 - factor;
-    scale1 = factor;
-  } else {
-    scale0 = sin((1.0 - factor) * e.theta) / e.sin_theta;
-    scale1 = sin(factor * e.theta) / e.sin_theta;
-  }
-  if (e.negative) scale1 = -scale1;
-  out->q = {scale0 * s.pose.q.w + scale1 * e.pose.q.w, scale0 * s.pose.q.x + scale1 * e.pose.q.x,
-            scale0 * s.pose.q.y + scale1 * e.pose.q.y, scale0 * s.pose.q.z + scale1 * e.pose.q.z};
+  out->q = slerp(s.pose.q, e.pose.q, factor, e.slerp);  // theta and sin(theta) of the interval come from the host
   return true;
 }
 
@@ -1557,15 +1547,7 @@ int dl_map_writer_add_trajectory(dl_map_writer* w, int32_t trajectory_id, int32_
     NodeRec r{};
     r.pose = pose_from7(poses + 7 * (size_t)i);
     if (i > 0) {
-      // the interval-constant half of Eigen's slerp, with the host's acos / sin
-      const Quatd& s = w->nodes.back().pose.q;
-      const Quatd& e = r.pose.q;
-      const double d = (s.x * e.x + s.y * e.y) + (s.z * e.z + s.w * e.w);
-      const double abs_d = std::fabs(d);
-      r.linear = abs_d >= 1.0 - DBL_EPSILON;
-      r.negative = d < 0.0;
-      r.theta = r.linear ? 0.0 : std::acos(abs_d);
-      r.sin_theta = r.linear ? 1.0 : std::sin(r.theta);
+      r.slerp = slerp_constants(w->nodes.back().pose.q, r.pose.q);  // the interval-constant half, with the host's acos / sin
     }
     w->nodes.push_back(r);
     w->times.push_back(times[i]);

@@ -4,13 +4,42 @@
 
 namespace dl {
 
+// Eigen's QuaternionBase::slerp(t, b) from a, in two halves: the part that depends on the two quaternions only (theta =
+// acos|d|, sin(theta), the |d| >= 1 - eps and d < 0 switches) and the per-t blend. Host and device, double arithmetic.
+struct SlerpConstants {
+  double theta, sin_theta;
+  int linear, negative_dot;
+};
+DL_HD SlerpConstants slerp_constants(const Quatd& a, const Quatd& b) {
+  SlerpConstants c;
+  const double d = (a.x * b.x + a.y * b.y) + (a.z * b.z + a.w * b.w);  // a.dot(b)
+  const double abs_d = fabs(d);
+  const double one = 1.0 - 2.220446049250313e-16;
+  c.linear = abs_d >= one;
+  c.negative_dot = d < 0;
+  c.theta = c.linear ? 0.0 : acos(abs_d);
+  c.sin_theta = c.linear ? 1.0 : sin(c.theta);
+  return c;
+}
+DL_HD Quatd slerp(const Quatd& a, const Quatd& b, double t, const SlerpConstants& c) {
+  double scale0, scale1;
+  if (c.linear) {
+    scale0 = 1.0 - t;
+    scale1 = t;
+  } else {
+    scale0 = sin((1.0 - t) * c.theta) / c.sin_theta;
+    scale1 = sin(t * c.theta) / c.sin_theta;
+  }
+  if (c.negative_dot) scale1 = -scale1;
+  return {scale0 * a.w + scale1 * b.w, scale0 * a.x + scale1 * b.x, scale0 * a.y + scale1 * b.y, scale0 * a.z + scale1 * b.z};
+}
+
 // Per-scan constants of the deskew, prepared on the host with the reference's double arithmetic (LTB:426-428,
 // LTB:871-879): prev = previous optimised pose, cur = IMU-predicted pose at scan end, rel = prev^-1 * cur, and the
-// scan-constant part of Eigen's slerp (theta = acos|d|, sin(theta), the |d| >= 1 - eps and d < 0 switches).
+// scan-constant half of Eigen's slerp from the identity to rel.q.
 struct ScanConstants {
   Rigidd prev, cur, rel;
-  double theta, sin_theta;
-  int linear_slerp, negative_dot;
+  SlerpConstants slerp;
 };
 
 // LTB:426-428 and the scan-constant half of Eigen's slerp, in the reference's double arithmetic. Host and device.
@@ -19,13 +48,7 @@ DL_HD ScanConstants make_scan_constants(const Rigidd& prev, const Rigidd& cur) {
   c.prev = prev;
   c.cur = cur;
   c.rel = compose(inverse(c.prev), c.cur);
-  const double d = (0.0 * c.rel.q.x + 0.0 * c.rel.q.y) + (0.0 * c.rel.q.z + 1.0 * c.rel.q.w);  // Identity.dot(rel.q)
-  const double abs_d = fabs(d);
-  const double one = 1.0 - 2.220446049250313e-16;
-  c.linear_slerp = abs_d >= one;
-  c.negative_dot = d < 0;
-  c.theta = c.linear_slerp ? 0.0 : acos(abs_d);
-  c.sin_theta = c.linear_slerp ? 1.0 : sin(c.theta);
+  c.slerp = slerp_constants(Quatd{1.0, 0.0, 0.0, 0.0}, c.rel.q);
   return c;
 }
 

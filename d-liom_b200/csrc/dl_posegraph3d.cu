@@ -5,7 +5,11 @@
 // node store, uploaded once per node, and every search reads them there through dl::constraint_search — the kernels of
 // dl_constraint_search_batch. The optimization calls dl_pose_graph_solve_sparse on the graph's poses: that call is the block-sparse
 // solve's one host entry (it takes host poses, sets up the CSR lists and runs the LM state machine on the host), and the poses
-// it moves are 56 bytes per submap or node, so there is no second copy of its set-up here. See include/dliom_b200.h.
+// it moves are 56 bytes per submap or node, so there is no second copy of its set-up here. Pure localization adds trimming
+// (TrimmingHandle::MarkSubmapAsTrimmed, :1002-1058, and PureLocalizationTrimmer, C/mapping/pose_graph_trimmer.cc:24-45),
+// FinishTrajectory (:535-547) and SetInitialTrajectoryPose (:849-876); a trimmed node's clouds become dead ranges of the
+// node store, and pg3d_store_compact copies the live ones into a fresh store once the dead outweigh them. See
+// include/dliom_b200.h.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -16,6 +20,7 @@
 #include <vector>
 
 #include "dl_internal.cuh"
+#include "dl_pipeline.cuh"
 
 using namespace dl;
 
@@ -39,10 +44,32 @@ struct Node {
   int64_t hi_begin = 0, n_hi = 0, lo_begin = 0, n_lo = 0;  // points in the node store
 };
 struct Trajectory {
-  std::vector<Submap> submaps;
-  std::vector<Node> nodes;
+  // MapById (C/mapping/id.h): indices in order; a trimmed index is a hole
+  std::map<int32_t, Submap> submaps;
+  std::map<int32_t, Node> nodes;
+  int32_t num_submaps = 0, num_nodes = 0;  // indices handed out so far: the index of the next append
+  // Trim of the highest index forbids later appends (id.h:289-300). The ban outlives the last element: a trajectory whose
+  // every submap was trimmed takes no new nodes.
+  bool submaps_can_append = true, nodes_can_append = true;
 };
 using Id = std::pair<int32_t, int32_t>;  // (trajectory_id, index)
+struct InitialTrajectoryPose {  // PoseGraph3D::InitialTrajectoryPose
+  int32_t to_trajectory_id;
+  Rigidd relative_pose;
+  double time;
+};
+struct StoreSegment {  // one live node's clouds (high- then low-resolution xyz floats) in the old and the fresh store
+  int64_t src, dst, floats;
+};
+constexpr int64_t kMinDeadFloats = (int64_t)1 << 20;  // compaction waits for at least this many dead floats (4 MiB)
+constexpr int kCompactBlock = 256;
+
+// One block per live node: its contiguous segment is copied with consecutive threads on consecutive floats (coalesced).
+__global__ void __launch_bounds__(kCompactBlock) pg3d_store_compact(const float* __restrict__ src, float* __restrict__ dst,
+                                                                    const StoreSegment* __restrict__ segments) {
+  const StoreSegment s = segments[blockIdx.x];
+  for (int64_t i = threadIdx.x; i < s.floats; i += kCompactBlock) dst[s.dst + i] = src[s.src + i];
+}
 
 double ms_since(std::chrono::steady_clock::time_point t0) {
   return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -77,16 +104,61 @@ struct dl_pose_graph_3d {
   std::vector<dl_pg3d_search> last_searches;             // of the last add_node call
   float* d_store = nullptr;                             // node store: xyz floats, each node's high- then low-resolution cloud
   int64_t store_capacity = 0, store_used = 0;            // in floats
+  int64_t store_live = 0;                                // floats of the nodes still in the graph; the rest of store_used is dead
   int64_t bytes_uploaded = 0;
+  std::set<int32_t> finished_trajectories;               // finished_trajectories_
+  std::map<int32_t, InitialTrajectoryPose> initial_poses;  // initial_trajectory_poses_
+  struct PureLocalizationTrimmer {
+    int32_t trajectory_id, num_submaps_to_keep;
+  };
+  std::vector<PureLocalizationTrimmer> trimmers;         // trimmers_, in the order they were added
+  std::vector<dl_pg3d_submap_id> last_trimmed;
 
-  // ComputeLocalToGlobalTransform (:914-935) over global_submap_poses_ (optimized) or submap_data (the problem's poses)
-  Rigidd local_to_global(int32_t trajectory_id, bool optimized) const {
+  // GetInterpolatedGlobalTrajectoryPose (:858-876): lower_bound by node time, clamped to the first and last node, else
+  // transform::Interpolate of the two nodes around `time`. false: the trajectory has no nodes (the reference CHECKs).
+  bool interpolated_global_pose(int32_t trajectory_id, double time, Rigidd* out) const {
     const auto it = trajectories.find(trajectory_id);
-    if (it == trajectories.end()) return identity();
-    const std::vector<Submap>& s = it->second.submaps;
-    for (int i = (int)s.size() - 1; i >= 0; --i)
-      if (!optimized || s[i].optimized) return compose(optimized ? s[i].optimized_global : s[i].global, inverse(s[i].local));
-    return identity();
+    if (it == trajectories.end() || it->second.nodes.empty()) return false;
+    const std::map<int32_t, Node>& nodes = it->second.nodes;
+    const auto end = std::find_if(nodes.begin(), nodes.end(), [time](const std::pair<const int32_t, Node>& n) {
+      return !(n.second.time < time);
+    });
+    if (end == nodes.begin()) {
+      *out = end->second.global;
+      return true;
+    }
+    if (end == nodes.end()) {
+      *out = std::prev(end)->second.global;
+      return true;
+    }
+    const Node& a = std::prev(end)->second;
+    const Node& b = end->second;
+    const double factor = (time - a.time) / (b.time - a.time);  // timestamped_transform.cc:22-37, on the double node times
+    out->t = {a.global.t.x + (b.global.t.x - a.global.t.x) * factor, a.global.t.y + (b.global.t.y - a.global.t.y) * factor,
+              a.global.t.z + (b.global.t.z - a.global.t.z) * factor};
+    out->q = slerp(a.global.q, b.global.q, factor, slerp_constants(a.global.q, b.global.q));
+    return true;
+  }
+  // ComputeLocalToGlobalTransform (:914-935) over global_submap_poses_ (optimized) or submap_data (the problem's poses): the
+  // last optimized submap that is still in the graph; before any, the initial trajectory pose if one was set. false: that
+  // pose needs a trajectory without nodes.
+  bool local_to_global(int32_t trajectory_id, bool optimized, Rigidd* out) const {
+    const auto it = trajectories.find(trajectory_id);
+    if (it != trajectories.end())
+      for (auto s = it->second.submaps.rbegin(); s != it->second.submaps.rend(); ++s)
+        if (!optimized || s->second.optimized) {
+          *out = compose(optimized ? s->second.optimized_global : s->second.global, inverse(s->second.local));
+          return true;
+        }
+    const auto ip = initial_poses.find(trajectory_id);
+    if (ip == initial_poses.end()) {
+      *out = identity();
+      return true;
+    }
+    Rigidd at;
+    if (!interpolated_global_pose(ip->second.to_trajectory_id, ip->second.time, &at)) return false;
+    *out = compose(at, ip->second.relative_pose);
+    return true;
   }
   int reserve_store(int64_t floats) {
     if (store_used + floats <= store_capacity) return DL_OK;
@@ -108,6 +180,10 @@ struct dl_pose_graph_3d {
     return DL_OK;
   }
   int optimize(dl_solve_summary* summary);
+  int run_trimmers();
+  int check_trimmable(int32_t trajectory_id, int32_t submap_index) const;
+  int mark_submap_as_trimmed(const Id& submap_id);
+  int compact_store();
 };
 
 namespace {
@@ -141,38 +217,39 @@ int dl_pose_graph_3d::optimize(dl_solve_summary* summary) {
     if (!has_added) constraints.push_back(c);
   }
   if (summary) std::memset(summary, 0, sizeof(*summary));
-  // poses: submaps then nodes, each in (trajectory, index) order
-  std::map<int32_t, int32_t> submap_base, node_base;
+  // poses: submaps then nodes, each in (trajectory, index) order over the ids still in the graph. The solve holds its first
+  // submap, so after a trim of the first one the next remaining submap is the anchor (optimization_problem_3d.cc:286-316).
+  std::map<Id, int32_t> submap_row, node_row;
   int32_t S = 0, N = 0;
   for (const auto& [id, t] : trajectories) {
-    submap_base[id] = S;
-    node_base[id] = N;
-    S += (int32_t)t.submaps.size();
-    N += (int32_t)t.nodes.size();
+    for (const auto& kv : t.submaps) submap_row[Id{id, kv.first}] = S++;
+    for (const auto& kv : t.nodes) node_row[Id{id, kv.first}] = N++;
   }
   if (S == 0) {  // RunOptimization: nothing to optimize
     pending.clear();
-    return DL_OK;
+    return run_trimmers();
   }
   std::vector<double> poses(7 * (size_t)(S + N));
   std::vector<uint8_t> frozen_mask(S + N, 0);
   for (const auto& [id, t] : trajectories) {
     const uint8_t f = frozen.count(id) ? 1 : 0;
-    for (size_t i = 0; i < t.submaps.size(); ++i) {
-      pose_to7(t.submaps[i].global, &poses[7 * (submap_base[id] + i)]);
-      frozen_mask[submap_base[id] + i] = f;
+    for (const auto& [i, s] : t.submaps) {
+      const int32_t r = submap_row[Id{id, i}];
+      pose_to7(s.global, &poses[7 * (size_t)r]);
+      frozen_mask[r] = f;
     }
-    for (size_t i = 0; i < t.nodes.size(); ++i) {
-      pose_to7(t.nodes[i].problem_global, &poses[7 * (S + node_base[id] + i)]);
-      frozen_mask[S + node_base[id] + i] = f;
+    for (const auto& [i, n] : t.nodes) {
+      const int32_t r = S + node_row[Id{id, i}];
+      pose_to7(n.problem_global, &poses[7 * (size_t)r]);
+      frozen_mask[r] = f;
     }
   }
   std::vector<dl_spa_constraint> spa(constraints.size());
   for (size_t k = 0; k < constraints.size(); ++k) {
     const dl_pg3d_constraint& c = constraints[k];
     dl_spa_constraint& s = spa[k];
-    s.submap = submap_base[c.submap_trajectory_id] + c.submap_index;
-    s.node = node_base[c.node_trajectory_id] + c.node_index;
+    s.submap = submap_row.at(Id{c.submap_trajectory_id, c.submap_index});
+    s.node = node_row.at(Id{c.node_trajectory_id, c.node_index});
     std::memcpy(s.zbar, c.zbar, sizeof(s.zbar));
     s.translation_weight = c.translation_weight;
     s.rotation_weight = c.rotation_weight;
@@ -187,20 +264,144 @@ int dl_pose_graph_3d::optimize(dl_solve_summary* summary) {
   pending.clear();
   if (summary) *summary = local;
   for (auto& [id, t] : trajectories) {
-    for (size_t i = 0; i < t.submaps.size(); ++i) t.submaps[i].global = pose_from7(&poses[7 * (submap_base[id] + i)]);
-    for (size_t i = 0; i < t.nodes.size(); ++i) {
-      t.nodes[i].problem_global = pose_from7(&poses[7 * (S + node_base[id] + i)]);
+    for (auto& [i, s] : t.submaps) s.global = pose_from7(&poses[7 * (size_t)submap_row[Id{id, i}]]);
+    for (auto& [i, n] : t.nodes) {
+      n.problem_global = pose_from7(&poses[7 * (size_t)(S + node_row[Id{id, i}])]);
       // every node is in node_data here (the calls are synchronous), so RunOptimization's extrapolation of the nodes added
       // after the solve started (:748-762) has nothing to move
-      t.nodes[i].global = t.nodes[i].problem_global;
+      n.global = n.problem_global;
     }
   }
   for (auto& [id, t] : trajectories)  // global_submap_poses_ = submap_data
-    for (Submap& s : t.submaps) {
+    for (auto& [i, s] : t.submaps) {
       s.optimized = true;
       s.optimized_global = s.global;
     }
   num_nodes_since_last_loop_closure = 0;
+  return run_trimmers();
+}
+
+// HandleWorkQueue (:492-501): every trimmer in the order added, then the finished ones are dropped.
+// PureLocalizationTrimmer::Trim (pose_graph_trimmer.cc:30-43): all but the newest num_submaps_to_keep submaps, all of them
+// once the trajectory is finished, which also finishes the trimmer.
+int dl_pose_graph_3d::run_trimmers() {
+  for (PureLocalizationTrimmer& tr : trimmers) {
+    if (finished_trajectories.count(tr.trajectory_id)) tr.num_submaps_to_keep = 0;
+    std::vector<int32_t> ids;
+    const auto it = trajectories.find(tr.trajectory_id);
+    if (it != trajectories.end())
+      for (const auto& kv : it->second.submaps) ids.push_back(kv.first);
+    for (size_t i = 0; i + (size_t)tr.num_submaps_to_keep < ids.size(); ++i) {
+      DL_TRY_STATUS(check_trimmable(tr.trajectory_id, ids[i]));
+      DL_TRY_STATUS(mark_submap_as_trimmed(Id{tr.trajectory_id, ids[i]}));
+    }
+  }
+  trimmers.erase(std::remove_if(trimmers.begin(), trimmers.end(),
+                                [](const PureLocalizationTrimmer& tr) { return tr.num_submaps_to_keep == 0; }),
+                 trimmers.end());
+  return DL_OK;
+}
+
+int dl_pose_graph_3d::check_trimmable(int32_t trajectory_id, int32_t submap_index) const {
+  const auto it = trajectories.find(trajectory_id);
+  if (it == trajectories.end() || !it->second.submaps.count(submap_index))
+    return ctx->fail(DL_ERR_ARG, "trim: no such submap in the graph (unknown or already trimmed)");
+  if (!it->second.submaps.at(submap_index).finished) return ctx->fail(DL_ERR_ARG, "trim: the submap is not finished");
+  if (!pending.empty()) return ctx->fail(DL_ERR_ARG, "trim: constraints are pending; trim right after an optimization");
+  return DL_OK;
+}
+
+// TrimmingHandle::MarkSubmapAsTrimmed (:1002-1058) and OptimizationProblem3D::TrimSubmap / TrimTrajectoryNode
+// (optimization_problem_3d.cc:229-251): the submap, its constraints, and the nodes left without an INTRA_SUBMAP constraint
+// together with all of theirs leave the graph. Their clouds become dead ranges of the node store.
+int dl_pose_graph_3d::mark_submap_as_trimmed(const Id& submap_id) {
+  const auto submap_of = [](const dl_pg3d_constraint& c) { return Id{c.submap_trajectory_id, c.submap_index}; };
+  const auto node_of = [](const dl_pg3d_constraint& c) { return Id{c.node_trajectory_id, c.node_index}; };
+  std::set<Id> nodes_to_retain;
+  for (const dl_pg3d_constraint& c : constraints)
+    if (c.tag == DL_PG3D_INTRA_SUBMAP && submap_of(c) != submap_id) nodes_to_retain.insert(node_of(c));
+  std::set<Id> nodes_to_remove;
+  std::vector<dl_pg3d_constraint> kept;
+  for (const dl_pg3d_constraint& c : constraints) {
+    if (submap_of(c) == submap_id) {
+      if (c.tag == DL_PG3D_INTRA_SUBMAP && !nodes_to_retain.count(node_of(c))) nodes_to_remove.insert(node_of(c));
+    } else {
+      kept.push_back(c);
+    }
+  }
+  constraints.clear();
+  for (const dl_pg3d_constraint& c : kept)
+    if (!nodes_to_remove.count(node_of(c))) constraints.push_back(c);
+  Trajectory& t = trajectories.at(submap_id.first);
+  const auto s = t.submaps.find(submap_id.second);
+  if (std::next(s) == t.submaps.end()) t.submaps_can_append = false;
+  t.submaps.erase(s);
+  computed.erase(submap_id);  // ConstraintBuilder3D::DeleteScanMatcher: the submap is never a search target again
+  for (const Id& node_id : nodes_to_remove) {
+    Trajectory& nt = trajectories.at(node_id.first);
+    const auto n = nt.nodes.find(node_id.second);
+    if (std::next(n) == nt.nodes.end()) nt.nodes_can_append = false;
+    store_live -= 3 * (n->second.n_hi + n->second.n_lo);
+    nt.nodes.erase(n);
+    for (auto& kv : computed) kv.second.erase(node_id);
+  }
+  last_trimmed.push_back(dl_pg3d_submap_id{submap_id.first, submap_id.second});
+  if (store_used - store_live > store_live && store_used - store_live >= kMinDeadFloats) return compact_store();
+  return DL_OK;
+}
+
+// Every live node's clouds into a fresh store, in (trajectory, index) order, by one launch of pg3d_store_compact; then the old
+// buffer is freed and the offsets are rewritten. Each compaction copies at most as many floats as died since the last one,
+// so the copying costs O(1) per uploaded float. A failure leaves the old store and every offset as they were.
+int dl_pose_graph_3d::compact_store() {
+  std::vector<StoreSegment> segments;
+  int64_t live = 0;
+  for (const auto& [id, t] : trajectories)
+    for (const auto& [i, n] : t.nodes) {
+      segments.push_back(StoreSegment{3 * n.hi_begin, live, 3 * (n.n_hi + n.n_lo)});
+      live += 3 * (n.n_hi + n.n_lo);
+    }
+  if (live == 0) {  // nothing left to copy: the store is freed, and the next add_node grows a new one
+    DL_CUDA(ctx, cudaSetDevice(ctx->device));
+    DL_CUDA(ctx, ctx->wait_stream());
+    cudaFree(d_store);
+    d_store = nullptr;
+    store_capacity = store_used = store_live = 0;
+    return DL_OK;
+  }
+  const int64_t cap = std::max<int64_t>(2 * live, (int64_t)1 << 20);
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  DL_TRY_STATUS(ctx->reserve_device(std::max<size_t>(segments.size(), 1) * sizeof(StoreSegment)));
+  float* fresh = nullptr;
+  cudaError_t e = cudaMalloc(&fresh, (size_t)cap * sizeof(float));
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // an allocation failure is not sticky: clear it for the next launch check
+    return ctx->cuda_fail(e, "node store compaction");
+  }
+  if (!segments.empty()) {
+    StoreSegment* d_segments = static_cast<StoreSegment*>(ctx->d_scratch);
+    e = cudaMemcpyAsync(d_segments, segments.data(), segments.size() * sizeof(StoreSegment), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) {
+      pg3d_store_compact<<<(unsigned)segments.size(), kCompactBlock, 0, ctx->stream>>>(d_store, fresh, d_segments);
+      ctx->launches++;
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = ctx->wait_stream();
+    if (e != cudaSuccess) {
+      cudaFree(fresh);
+      return ctx->cuda_fail(e, "pg3d_store_compact");
+    }
+  }
+  cudaFree(d_store);
+  d_store = fresh;
+  store_capacity = cap;
+  store_used = store_live = live;
+  size_t k = 0;
+  for (auto& [id, t] : trajectories)
+    for (auto& [i, n] : t.nodes) {
+      n.hi_begin = segments[k++].dst / 3;
+      n.lo_begin = n.hi_begin + n.n_hi;
+    }
   return DL_OK;
 }
 
@@ -230,6 +431,7 @@ void dl_pose_graph_3d_destroy(dl_pose_graph_3d* g) {
 int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int32_t num_matches,
                               const dl_pg3d_submap_match* matches, dl_pg3d_add_node_info* info) {
   if (!g || !node || num_matches < 0 || (num_matches > 0 && !matches)) return DL_ERR_ARG;
+  g->last_trimmed.clear();
   dl_context* ctx = g->ctx;
   const auto t0 = std::chrono::steady_clock::now();
   const int m = node->num_insertion_submaps;
@@ -242,8 +444,11 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
     if (!ins[i].high_resolution_grid || !ins[i].low_resolution_grid) return ctx->fail(DL_ERR_ARG, "insertion submap without grids");
   const int32_t tid = node->trajectory_id;
   if (tid < 0) return ctx->fail(DL_ERR_ARG, "negative trajectory id");
+  if (g->finished_trajectories.count(tid)) return ctx->fail(DL_ERR_ARG, "the trajectory is finished");
   const auto tit = g->trajectories.find(tid);
-  const int32_t S = tit == g->trajectories.end() ? 0 : (int32_t)tit->second.submaps.size();
+  if (tit != g->trajectories.end() && !tit->second.nodes_can_append)
+    return ctx->fail(DL_ERR_ARG, "the trajectory's highest node index was trimmed: no more nodes can be appended");
+  const int32_t S = tit == g->trajectories.end() ? 0 : tit->second.num_submaps;  // submap indices handed out, holes included
   // AddNode's "is insertion_submaps.back() new" and InitializeGlobalSubmapPoses' CHECKs, as index rules
   bool back_is_new;
   if (m == 1) {
@@ -255,10 +460,18 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
     else if (S >= 2 && a == S - 2 && b == S - 1) back_is_new = false;
     else return ctx->fail(DL_ERR_ARG, "insertion submaps do not continue the trajectory's submap sequence");
   }
+  if (back_is_new && tit != g->trajectories.end() && !tit->second.submaps_can_append)
+    return ctx->fail(DL_ERR_ARG, "the trajectory's highest submap index was trimmed: no more submaps can be appended");
   if (tit != g->trajectories.end())
-    for (int i = 0; i < m; ++i)
-      if (ins[i].submap_index < S && tit->second.submaps[ins[i].submap_index].finished)
-        return ctx->fail(DL_ERR_ARG, "insertion submap is already finished");
+    for (int i = 0; i < m; ++i) {
+      if (ins[i].submap_index >= S) continue;
+      const auto it = tit->second.submaps.find(ins[i].submap_index);
+      if (it == tit->second.submaps.end()) return ctx->fail(DL_ERR_ARG, "insertion submap was trimmed");
+      if (it->second.finished) return ctx->fail(DL_ERR_ARG, "insertion submap is already finished");
+    }
+  Rigidd local_to_global;  // GetLocalToGlobalTransform, for the node's pose (:115-116) and a first submap (:67-110)
+  if (!g->local_to_global(tid, true, &local_to_global))
+    return ctx->fail(DL_ERR_ARG, "the initial trajectory pose refers to a trajectory without nodes");
   const bool newly_finished = ins[0].finished != 0;
   if (!newly_finished && num_matches > 0) return ctx->fail(DL_ERR_ARG, "submap matches passed but no insertion submap finished");
   const Id front_id{tid, ins[0].submap_index};
@@ -272,9 +485,9 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
     if (to.first == tid && std::abs(to.second - front_id.second) <= 2)
       return ctx->fail(DL_ERR_ARG, "a match names a same-trajectory submap within two indices");
     const auto it = g->trajectories.find(to.first);
-    if (it == g->trajectories.end() || to.second < 0 || to.second >= (int32_t)it->second.submaps.size())
-      return ctx->fail(DL_ERR_ARG, "a match names an unknown submap");
-    if (!it->second.submaps[to.second].finished) return ctx->fail(DL_ERR_ARG, "a match names an unfinished submap");
+    if (it == g->trajectories.end() || !it->second.submaps.count(to.second))
+      return ctx->fail(DL_ERR_ARG, "a match names an unknown or trimmed submap");
+    if (!it->second.submaps.at(to.second).finished) return ctx->fail(DL_ERR_ARG, "a match names an unfinished submap");
     if (k > 0 && to == Id{sorted[k - 1].trajectory_id, sorted[k - 1].submap_index})
       return ctx->fail(DL_ERR_ARG, "a submap is matched twice");
   }
@@ -293,21 +506,25 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
 
   // ---- 4. fan-out and searches of a newly finished submap, before anything is committed
   const Rigidd local_pose = pose_from7(node->local_pose);
-  const int32_t node_index = tit == g->trajectories.end() ? 0 : (int32_t)tit->second.nodes.size();
+  const int32_t node_index = tit == g->trajectories.end() ? 0 : tit->second.num_nodes;
   std::vector<Pair> pairs;
   std::vector<dl_constraint> results;
   double search_ms = 0.0;
   if (newly_finished && !sorted.empty()) {
     const Trajectory* tr = tit == g->trajectories.end() ? nullptr : &tit->second;
     const Rigidd local_from = pose_from7(ins[0].local_pose);  // a finished submap was seen before: the same pose
-    const Rigidd from_local = tr && front_id.second < S ? tr->submaps[front_id.second].local : local_from;
-    std::vector<int32_t> nodes_in_submap = tr && front_id.second < S ? tr->submaps[front_id.second].node_ids : std::vector<int32_t>();
+    const Submap* from = tr && front_id.second < S ? &tr->submaps.at(front_id.second) : nullptr;
+    const Rigidd from_local = from ? from->local : local_from;
+    std::vector<int32_t> nodes_in_submap;
+    if (from)
+      for (const int32_t n : from->node_ids)
+        if (tr->nodes.count(n)) nodes_in_submap.push_back(n);  // trimmed nodes are holes
     nodes_in_submap.push_back(node_index);  // this node was just inserted into it
     const Rigidd T_S2_G2 = yaw_free_alignment(from_local);
     const Rigidd from_local_inv = inverse(from_local);
     for (const dl_pg3d_submap_match& mt : sorted) {
       const Id to{mt.trajectory_id, mt.submap_index};
-      const Submap& target = g->trajectories.at(to.first).submaps[to.second];
+      const Submap& target = g->trajectories.at(to.first).submaps.at(to.second);
       const Rigidd T_G1_S1 = inverse(yaw_free_alignment(target.local));
       const Rigidd submap_to_submap_2d{{mt.x, mt.y, 0.0}, yaw_quaternion(mt.theta)};  // Embed3D(Rigid2d)
       const Rigidd left = compose(compose(T_G1_S1, submap_to_submap_2d), T_S2_G2);
@@ -317,7 +534,7 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
         if (j++ % g->options.every_nodes_to_find_constraint != 0) continue;
         if (done != g->computed.end() && done->second.count(Id{tid, n})) continue;
         const bool is_new = n == node_index;
-        const Node* nd = is_new ? nullptr : &tr->nodes[n];
+        const Node* nd = is_new ? nullptr : &tr->nodes.at(n);
         Pair p;
         p.submap = to;
         p.node = Id{tid, n};
@@ -342,7 +559,7 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
         lo_off[k + 1] = lo_off[k] + p.n_lo;
         hib[k] = p.hi_begin;
         lob[k] = p.lo_begin;
-        const Submap& target = g->trajectories.at(p.submap.first).submaps[p.submap.second];
+        const Submap& target = g->trajectories.at(p.submap.first).submaps.at(p.submap.second);
         if (target.hi->structure_dirty || target.lo->structure_dirty)
           return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
         hg[k] = target.hi;
@@ -364,11 +581,12 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
   // ---- commit: 1. AddNode, 3. ComputeConstraintsForNode, 4. the searches' results
   Trajectory& t = g->trajectories[tid];
   g->store_used += 3 * (n_hi + n_lo);
+  g->store_live += 3 * (n_hi + n_lo);
   g->bytes_uploaded += uploaded;
   Node nd;
   nd.time = node->time;
   nd.local = local_pose;
-  nd.global = compose(g->local_to_global(tid, true), local_pose);  // GetLocalToGlobalTransform * local_pose (:115-116)
+  nd.global = compose(local_to_global, local_pose);  // GetLocalToGlobalTransform * local_pose (:115-116)
   nd.hi_begin = hi_begin;
   nd.n_hi = n_hi;
   nd.lo_begin = lo_begin;
@@ -379,15 +597,18 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
     s.lo = ins[m - 1].low_resolution_grid;
     s.local = pose_from7(ins[m - 1].local_pose);
     // InitializeGlobalSubmapPoses (:67-110)
-    if (m == 1) s.global = compose(g->local_to_global(tid, true), s.local);
-    else s.global = compose(compose(t.submaps[ins[0].submap_index].global, inverse(t.submaps[ins[0].submap_index].local)), s.local);
-    t.submaps.push_back(s);
+    if (m == 1) s.global = compose(local_to_global, s.local);
+    else {
+      const Submap& front = t.submaps.at(ins[0].submap_index);
+      s.global = compose(compose(front.global, inverse(front.local)), s.local);
+    }
+    t.submaps[t.num_submaps++] = s;
   }
-  const Submap& matching = t.submaps[ins[0].submap_index];
+  const Submap& matching = t.submaps.at(ins[0].submap_index);
   nd.problem_global = compose(compose(matching.global, inverse(matching.local)), local_pose);  // :345-347
-  t.nodes.push_back(nd);
+  t.nodes[t.num_nodes++] = nd;
   for (int i = 0; i < m; ++i) {
-    Submap& s = t.submaps[ins[i].submap_index];
+    Submap& s = t.submaps.at(ins[i].submap_index);
     s.node_ids.push_back(node_index);
     dl_pg3d_constraint c{};
     c.submap_trajectory_id = tid;
@@ -412,7 +633,7 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
     s.result = results[k];
   }
   if (newly_finished) {
-    t.submaps[ins[0].submap_index].finished = true;
+    t.submaps.at(ins[0].submap_index).finished = true;
     for (size_t k = 0; k < pairs.size(); ++k) {
       if (!results[k].found) continue;
       ++found;
@@ -465,6 +686,7 @@ int dl_pose_graph_3d_freeze_trajectory(dl_pose_graph_3d* g, int32_t trajectory_i
 
 int dl_pose_graph_3d_run_final_optimization(dl_pose_graph_3d* g, dl_solve_summary* summary) {
   if (!g) return DL_ERR_ARG;
+  g->last_trimmed.clear();
   // max_num_final_iterations is set and then overwritten with the regular cap (pose_graph_3d.cc:677-682): the same solve
   return g->optimize(summary);
 }
@@ -478,24 +700,29 @@ int dl_pose_graph_3d_poses(const dl_pose_graph_3d* g, int32_t trajectory_id, int
   *count = n;
   if (!poses) return DL_OK;
   if (capacity < n) return g->ctx->fail(DL_ERR_ARG, "capacity smaller than the trajectory");
-  const Rigidd extrapolate = g->local_to_global(trajectory_id, true);
-  for (int32_t i = 0; i < n; ++i) {
-    Rigidd p;
-    if (which == DL_PG3D_NODE_POSES) p = it->second.nodes[i].global;
-    else if (which == DL_PG3D_OPTIMIZATION_NODES) p = it->second.nodes[i].problem_global;
-    else if (which == DL_PG3D_OPTIMIZATION_SUBMAPS) p = it->second.submaps[i].global;
-    else {
-      const Submap& s = it->second.submaps[i];
-      p = s.optimized ? s.optimized_global : compose(extrapolate, s.local);
+  if (n == 0) return DL_OK;
+  Rigidd extrapolate = identity();
+  if (which == DL_PG3D_SUBMAP_POSES && !g->local_to_global(trajectory_id, true, &extrapolate))
+    return g->ctx->fail(DL_ERR_ARG, "the initial trajectory pose refers to a trajectory without nodes");
+  size_t i = 0;
+  if (nodes)
+    for (const auto& kv : it->second.nodes)
+      pose_to7(which == DL_PG3D_NODE_POSES ? kv.second.global : kv.second.problem_global, poses + 7 * i++);
+  else
+    for (const auto& kv : it->second.submaps) {
+      const Submap& s = kv.second;
+      const Rigidd p = which == DL_PG3D_OPTIMIZATION_SUBMAPS ? s.global : s.optimized ? s.optimized_global : compose(extrapolate, s.local);
+      pose_to7(p, poses + 7 * i++);
     }
-    pose_to7(p, poses + 7 * (size_t)i);
-  }
   return DL_OK;
 }
 
 int dl_pose_graph_3d_local_to_global(const dl_pose_graph_3d* g, int32_t trajectory_id, double* pose) {
   if (!g || !pose) return DL_ERR_ARG;
-  pose_to7(g->local_to_global(trajectory_id, true), pose);
+  Rigidd p;
+  if (!g->local_to_global(trajectory_id, true, &p))
+    return g->ctx->fail(DL_ERR_ARG, "the initial trajectory pose refers to a trajectory without nodes");
+  pose_to7(p, pose);
   return DL_OK;
 }
 
@@ -523,6 +750,82 @@ int dl_pose_graph_3d_store_bytes(const dl_pose_graph_3d* g, int64_t* uploaded, i
   if (!g) return DL_ERR_ARG;
   if (uploaded) *uploaded = g->bytes_uploaded;
   if (capacity) *capacity = g->store_capacity * (int64_t)sizeof(float);
+  return DL_OK;
+}
+
+int dl_pg3d_trim_submap(dl_pose_graph_3d* g, int32_t trajectory_id, int32_t submap_index) {
+  if (!g) return DL_ERR_ARG;
+  g->last_trimmed.clear();
+  DL_TRY_STATUS(g->check_trimmable(trajectory_id, submap_index));
+  return g->mark_submap_as_trimmed(Id{trajectory_id, submap_index});
+}
+
+int dl_pg3d_add_pure_localization_trimmer(dl_pose_graph_3d* g, int32_t trajectory_id, int32_t num_submaps_to_keep) {
+  if (!g || trajectory_id < 0) return DL_ERR_ARG;
+  if (num_submaps_to_keep < 3) return g->ctx->fail(DL_ERR_ARG, "a pure-localization trimmer keeps at least 3 submaps");
+  g->trimmers.push_back(dl_pose_graph_3d::PureLocalizationTrimmer{trajectory_id, num_submaps_to_keep});
+  return DL_OK;
+}
+
+int dl_pg3d_finish_trajectory(dl_pose_graph_3d* g, int32_t trajectory_id) {
+  if (!g || trajectory_id < 0) return DL_ERR_ARG;
+  g->last_trimmed.clear();
+  if (!g->finished_trajectories.insert(trajectory_id).second) return g->ctx->fail(DL_ERR_ARG, "the trajectory is already finished");
+  const auto it = g->trajectories.find(trajectory_id);
+  if (it != g->trajectories.end())
+    for (auto& kv : it->second.submaps) kv.second.finished = true;
+  return g->optimize(nullptr);  // DispatchOptimization: the step of dl_pose_graph_3d_run_final_optimization
+}
+
+int dl_pg3d_is_trajectory_finished(const dl_pose_graph_3d* g, int32_t trajectory_id, int32_t* finished) {
+  if (!g || !finished) return DL_ERR_ARG;
+  *finished = g->finished_trajectories.count(trajectory_id) ? 1 : 0;
+  return DL_OK;
+}
+
+int dl_pg3d_set_initial_trajectory_pose(dl_pose_graph_3d* g, int32_t from_trajectory_id, int32_t to_trajectory_id,
+                                        const double* relative_pose, double time) {
+  if (!g || !relative_pose || from_trajectory_id < 0 || to_trajectory_id < 0) return DL_ERR_ARG;
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(relative_pose[k])) return g->ctx->fail(DL_ERR_ARG, "the relative pose is not finite");
+  if (!std::isfinite(time)) return g->ctx->fail(DL_ERR_ARG, "the time is not finite");
+  g->initial_poses[from_trajectory_id] = InitialTrajectoryPose{to_trajectory_id, pose_from7(relative_pose), time};
+  return DL_OK;
+}
+
+int dl_pg3d_ids(const dl_pose_graph_3d* g, int32_t trajectory_id, int32_t which, int32_t capacity, int32_t* indices,
+                int32_t* count) {
+  if (!g || !count || which < DL_PG3D_NODE_POSES || which > DL_PG3D_OPTIMIZATION_SUBMAPS || capacity < 0) return DL_ERR_ARG;
+  const auto it = g->trajectories.find(trajectory_id);
+  const bool nodes = which == DL_PG3D_NODE_POSES || which == DL_PG3D_OPTIMIZATION_NODES;
+  const int32_t n = it == g->trajectories.end() ? 0 : (int32_t)(nodes ? it->second.nodes.size() : it->second.submaps.size());
+  *count = n;
+  if (!indices) return DL_OK;
+  if (capacity < n) return g->ctx->fail(DL_ERR_ARG, "capacity smaller than the trajectory");
+  if (n == 0) return DL_OK;
+  int32_t i = 0;
+  if (nodes)
+    for (const auto& kv : it->second.nodes) indices[i++] = kv.first;
+  else
+    for (const auto& kv : it->second.submaps) indices[i++] = kv.first;
+  return DL_OK;
+}
+
+int dl_pg3d_last_trimmed(const dl_pose_graph_3d* g, int32_t capacity, dl_pg3d_submap_id* out, int32_t* count) {
+  if (!g || !count || capacity < 0) return DL_ERR_ARG;
+  const int32_t n = (int32_t)g->last_trimmed.size();
+  *count = n;
+  if (!out) return DL_OK;
+  if (capacity < n) return g->ctx->fail(DL_ERR_ARG, "capacity smaller than the trimmed list");
+  std::copy(g->last_trimmed.begin(), g->last_trimmed.end(), out);
+  return DL_OK;
+}
+
+int dl_pg3d_store_usage(const dl_pose_graph_3d* g, int64_t* live_bytes, int64_t* used_bytes, int64_t* capacity_bytes) {
+  if (!g) return DL_ERR_ARG;
+  if (live_bytes) *live_bytes = g->store_live * (int64_t)sizeof(float);
+  if (used_bytes) *used_bytes = g->store_used * (int64_t)sizeof(float);
+  if (capacity_bytes) *capacity_bytes = g->store_capacity * (int64_t)sizeof(float);
   return DL_OK;
 }
 

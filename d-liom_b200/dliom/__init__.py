@@ -36,10 +36,12 @@ EXPORTS = [
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
     "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
-    "dl_ltb_add_range_data_batch",
+    "dl_ltb_add_range_data_batch", "dl_ltb_release_submap",
     "dl_pose_graph_3d_create", "dl_pose_graph_3d_destroy", "dl_pose_graph_3d_add_node", "dl_pose_graph_3d_freeze_trajectory",
     "dl_pose_graph_3d_run_final_optimization", "dl_pose_graph_3d_poses", "dl_pose_graph_3d_local_to_global",
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
+    "dl_pg3d_trim_submap", "dl_pg3d_add_pure_localization_trimmer", "dl_pg3d_finish_trajectory", "dl_pg3d_is_trajectory_finished",
+    "dl_pg3d_set_initial_trajectory_pose", "dl_pg3d_ids", "dl_pg3d_last_trimmed", "dl_pg3d_store_usage",
     "dl_map_writer_create", "dl_map_writer_destroy", "dl_map_writer_add_trajectory", "dl_map_writer_process",
     "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels", "dl_map_writer_add_color",
     "dl_map_writer_add_xray", "dl_map_writer_xray_image", "dl_map_writer_add_probability_grid", "dl_map_writer_probability_grid",
@@ -365,6 +367,10 @@ class Pg3dSearch(C.Structure):   # dl_pg3d_search
                 ("node_index", C.c_int32), ("pose_guess", C.c_double * 7), ("result", Constraint)]
 
 
+class Pg3dSubmapId(C.Structure):   # dl_pg3d_submap_id
+    _fields_ = [("trajectory_id", C.c_int32), ("submap_index", C.c_int32)]
+
+
 class MapWriterOptions(C.Structure):   # dl_map_writer_options
     _fields_ = [("range_filter", C.c_int32), ("reserved", C.c_int32), ("min_range", C.c_double), ("max_range", C.c_double),
                 ("outlier_voxel_size", C.c_double)]
@@ -541,6 +547,14 @@ def lib():
     L.dl_pose_graph_3d_constraints.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
     L.dl_pose_graph_3d_last_searches.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
     L.dl_pose_graph_3d_store_bytes.argtypes = [vp, ip(C.c_int64), ip(C.c_int64)]
+    L.dl_pg3d_trim_submap.argtypes = [vp, C.c_int32, C.c_int32]
+    L.dl_pg3d_add_pure_localization_trimmer.argtypes = [vp, C.c_int32, C.c_int32]
+    L.dl_pg3d_finish_trajectory.argtypes = [vp, C.c_int32]
+    L.dl_pg3d_is_trajectory_finished.argtypes = [vp, C.c_int32, ip(C.c_int32)]
+    L.dl_pg3d_set_initial_trajectory_pose.argtypes = [vp, C.c_int32, C.c_int32, vp, C.c_double]
+    L.dl_pg3d_ids.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, ip(C.c_int32)]
+    L.dl_pg3d_last_trimmed.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
+    L.dl_pg3d_store_usage.argtypes = [vp, ip(C.c_int64), ip(C.c_int64), ip(C.c_int64)]
     L.dl_map_writer_create.argtypes = [vp, ip(MapWriterOptions), ip(vp)]
     L.dl_map_writer_destroy.argtypes = [vp]
     L.dl_map_writer_destroy.restype = None
@@ -571,6 +585,7 @@ def lib():
     L.dl_ltb_get_submap.argtypes = [vp, C.c_int32, ip(vp), ip(vp), f64p, ip(C.c_int32), ip(C.c_int32)]
     L.dl_ltb_get_state.argtypes = [vp, ip(NavState), ip(C.c_int32)]
     L.dl_ltb_add_range_data_batch.argtypes = [C.c_int32, ip(LtbBatchItem), ip(MatchingResult)]
+    L.dl_ltb_release_submap.argtypes = [vp, C.c_int32]
     L.dl_frontend_submit.argtypes = [vp, ip(FrontendOptions), C.c_int32, ip(vp), i64p, f32p, C.c_int32, f64p, f64p, f64p, vp, vp]
     L.dl_frontend_collect.argtypes = [vp, C.c_int32, ip(ScanResult)]
     L.dl_frontend_match_batch_dev.argtypes = [vp, ip(FrontendOptions), C.c_int32, vp, C.c_int64, i64p, f32p, C.c_int32,
@@ -1216,6 +1231,10 @@ class LocalTrajectoryBuilder:
         self.ctx.check(self.ctx.L.dl_ltb_get_submap(self.h, index, C.byref(hi), C.byref(lo), pose, C.byref(n), C.byref(fin)))
         return Grid.borrowed(self.ctx, hi), Grid.borrowed(self.ctx, lo), pose, n.value, bool(fin.value)
 
+    def release_submap(self, index):
+        """Frees the device grids of a finished submap (dl_ltb_release_submap); submap(index) then returns NULL grid handles."""
+        self.ctx.check(self.ctx.L.dl_ltb_release_submap(self.h, int(index)))
+
     def state(self):
         s = NavState()
         init = C.c_int32(0)
@@ -1265,6 +1284,8 @@ class PoseGraph3D:
         self.ctx, self.options = ctx, options if options is not None else PoseGraph3DOptions.defaults()
         self.h = C.c_void_p()
         self._grids = {}   # the borrowed grids' Python handles stay alive with the graph, one entry per grid
+        self._submap_grids = {}   # (trajectory, submap index) -> its two keys in _grids
+        self._feeders = {}        # (trajectory, submap index) -> the LocalTrajectoryBuilder whose grids add_node_from_builder passed
         ctx.check(ctx.L.dl_pose_graph_3d_create(ctx.h, C.byref(self.options), C.byref(self.h)))
 
     def close(self):
@@ -1291,13 +1312,14 @@ class PoseGraph3D:
             s.submap_index, s.finished = int(index), int(bool(finished))
             s.high_resolution_grid, s.low_resolution_grid = hg.h, lg.h
             s.local_pose[:] = [float(v) for v in pose]
-            self._grids[hg.h.value if isinstance(hg.h, C.c_void_p) else hg.h] = hg
-            self._grids[lg.h.value if isinstance(lg.h, C.c_void_p) else lg.h] = lg
+            keys = [g.h.value if isinstance(g.h, C.c_void_p) else g.h for g in (hg, lg)]
+            self._grids[keys[0]], self._grids[keys[1]] = hg, lg
+            self._submap_grids[(int(trajectory_id), int(index))] = keys
         m = (Pg3dSubmapMatch * max(len(matches), 1))(*[Pg3dSubmapMatch(int(t), int(i), float(x), float(y), float(th))
                                                         for t, i, x, y, th in matches])
         info = Pg3dAddNodeInfo()
-        self.ctx.check(self.ctx.L.dl_pose_graph_3d_add_node(self.h, C.byref(n), len(matches), C.cast(m, C.c_void_p),
-                                                            C.byref(info)))
+        self._checked_forgetting_trimmed(self.ctx.L.dl_pose_graph_3d_add_node(self.h, C.byref(n), len(matches),
+                                                                              C.cast(m, C.c_void_p), C.byref(info)))
         return info
 
     def add_node_from_builder(self, trajectory_id, builder, result, matches=()):
@@ -1308,16 +1330,80 @@ class PoseGraph3D:
             index = result.insertion_submap_index[i]
             hg, lg, pose, _, finished = builder.submap(index)
             subs.append((index, finished, hg, lg, pose))
+            self._feeders[(int(trajectory_id), int(index))] = builder
         return self.add_node(trajectory_id, result.time, np.array(result.local_pose[:]), builder.cloud(2), builder.cloud(3),
                              subs, matches)
+
+    def _checked_forgetting_trimmed(self, status):
+        """After a call that may have trimmed, whatever its status (the call empties the trimmed list when it starts, so a
+        failure after some trims reports those): the graph no longer reads the trimmed submaps' grids. Their handles are
+        dropped unless another submap in the graph passed the same grid, and a submap fed by add_node_from_builder has its
+        grids released on that builder if the builder has finished it (its active submaps, trimmed by finish_trajectory, stay
+        until the builder is closed). Then the status is checked."""
+        for t, i in self.last_trimmed():
+            keys = self._submap_grids.pop((t, i), ())
+            still_used = {k for ks in self._submap_grids.values() for k in ks}
+            for key in keys:
+                if key not in still_used:
+                    self._grids.pop(key, None)
+            builder = self._feeders.pop((t, i), None)
+            if builder is not None and builder.submap(i)[4]:
+                builder.release_submap(i)
+        self.ctx.check(status)
 
     def freeze_trajectory(self, trajectory_id):
         self.ctx.check(self.ctx.L.dl_pose_graph_3d_freeze_trajectory(self.h, int(trajectory_id)))
 
     def run_final_optimization(self):
         s = SolveSummary()
-        self.ctx.check(self.ctx.L.dl_pose_graph_3d_run_final_optimization(self.h, C.byref(s)))
+        self._checked_forgetting_trimmed(self.ctx.L.dl_pose_graph_3d_run_final_optimization(self.h, C.byref(s)))
         return s.as_dict()
+
+    def trim_submap(self, trajectory_id, submap_index):
+        """TrimmingHandle::MarkSubmapAsTrimmed (dl_pg3d_trim_submap)."""
+        self._checked_forgetting_trimmed(self.ctx.L.dl_pg3d_trim_submap(self.h, int(trajectory_id), int(submap_index)))
+
+    def add_pure_localization_trimmer(self, trajectory_id, num_submaps_to_keep=3):
+        """PureLocalizationTrimmer (dl_pg3d_add_pure_localization_trimmer): runs after every optimization."""
+        self.ctx.check(self.ctx.L.dl_pg3d_add_pure_localization_trimmer(self.h, int(trajectory_id), int(num_submaps_to_keep)))
+
+    def finish_trajectory(self, trajectory_id):
+        """FinishTrajectory (dl_pg3d_finish_trajectory): every submap finished, then the final optimization and the trimmers."""
+        self._checked_forgetting_trimmed(self.ctx.L.dl_pg3d_finish_trajectory(self.h, int(trajectory_id)))
+
+    def is_trajectory_finished(self, trajectory_id):
+        f = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_pg3d_is_trajectory_finished(self.h, int(trajectory_id), C.byref(f)))
+        return bool(f.value)
+
+    def set_initial_trajectory_pose(self, from_trajectory_id, to_trajectory_id, relative_pose, time):
+        """SetInitialTrajectoryPose (dl_pg3d_set_initial_trajectory_pose): relative_pose 7 (t xyz, q wxyz), time in seconds."""
+        p = np.ascontiguousarray(relative_pose, np.float64).reshape(7)
+        self.ctx.check(self.ctx.L.dl_pg3d_set_initial_trajectory_pose(self.h, int(from_trajectory_id), int(to_trajectory_id),
+                                                                      p.ctypes.data, float(time)))
+
+    def ids(self, trajectory_id, which=None):
+        """Indices of the rows of node_poses (which = PG3D_NODE_POSES, the default) or submap_poses (PG3D_SUBMAP_POSES)."""
+        which = PG3D_NODE_POSES if which is None else which
+        n = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_pg3d_ids(self.h, int(trajectory_id), which, 0, None, C.byref(n)))
+        out = np.zeros(max(n.value, 1), np.int32)
+        self.ctx.check(self.ctx.L.dl_pg3d_ids(self.h, int(trajectory_id), which, n.value, out.ctypes.data, C.byref(n)))
+        return out[:n.value].tolist()
+
+    def last_trimmed(self):
+        """[(trajectory, submap index)] trimmed by the last call that could trim."""
+        n = C.c_int32(0)
+        self.ctx.check(self.ctx.L.dl_pg3d_last_trimmed(self.h, 0, None, C.byref(n)))
+        out = (Pg3dSubmapId * max(n.value, 1))()
+        self.ctx.check(self.ctx.L.dl_pg3d_last_trimmed(self.h, n.value, C.cast(out, C.c_void_p), C.byref(n)))
+        return [(s.trajectory_id, s.submap_index) for s in list(out)[:n.value]]
+
+    def store_usage(self):
+        """Node store bytes: (live, used, capacity)."""
+        v = [C.c_int64(0) for _ in range(3)]
+        self.ctx.check(self.ctx.L.dl_pg3d_store_usage(self.h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
 
     def _poses(self, trajectory_id, which):
         n = C.c_int32(0)

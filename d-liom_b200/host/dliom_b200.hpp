@@ -827,6 +827,38 @@ struct PoseGraphConstraint {  // PoseGraphInterface::Constraint with its tag
   Tag tag;
 };
 
+class PoseGraph3D;
+
+// PoseGraphInterface's trimming side (pose_graph_trimmer.h): what a trimmer sees of the graph, and the trimmer itself.
+class Trimmable {
+ public:
+  virtual ~Trimmable() = default;
+  virtual std::vector<optimization::SubmapId> GetSubmapIds(int trajectory_id) const = 0;
+  virtual std::vector<PoseGraphConstraint> GetConstraints() const = 0;
+  virtual bool IsFinished(int trajectory_id) const = 0;
+  virtual void MarkSubmapAsTrimmed(const optimization::SubmapId& submap_id) = 0;  // dl_pg3d_trim_submap
+};
+class PoseGraphTrimmer {
+ public:
+  virtual ~PoseGraphTrimmer() = default;
+  virtual void Trim(Trimmable* pose_graph) = 0;
+  virtual bool IsFinished() = 0;
+};
+// PureLocalizationTrimmer (pose_graph_trimmer.cc:24-45). Its policy lives in the C object (dl_pg3d_add_pure_localization_trimmer):
+// PoseGraph3D::AddTrimmer registers it there, and the graph runs it after each optimization, so Trim is never called on it.
+class PureLocalizationTrimmer : public PoseGraphTrimmer {
+ public:
+  PureLocalizationTrimmer(int trajectory_id, int num_submaps_to_keep)
+      : trajectory_id_(trajectory_id), num_submaps_to_keep_(num_submaps_to_keep) {}
+  void Trim(Trimmable*) override {}
+  bool IsFinished() override { return false; }
+  int trajectory_id() const { return trajectory_id_; }
+  int num_submaps_to_keep() const { return num_submaps_to_keep_; }
+
+ private:
+  int trajectory_id_, num_submaps_to_keep_;
+};
+
 // mapping::PoseGraph3D (pose_graph_3d.cc) on the live loop-closure path: a thin owner of the C object dl_pose_graph_3d, which
 // holds the graph, the device node store and the constraint table, runs the searches and the solve (include/dliom_b200.h).
 // AddNode is the call GlobalTrajectoryBuilder makes (global_trajectory_builder.cc:80-82) with the builder whose submaps the
@@ -847,6 +879,47 @@ class PoseGraph3D {
   ~PoseGraph3D() { dl_pose_graph_3d_destroy(graph_); }
   PoseGraph3D(const PoseGraph3D&) = delete;
   PoseGraph3D& operator=(const PoseGraph3D&) = delete;
+
+  // Pure localization. After every call that may trim (AddNode, RunFinalOptimization, FinishTrajectory), the grids of the
+  // submaps the graph trimmed are released on the LocalTrajectoryBuilder3D that AddNode got them from, if that builder has
+  // finished them (dl_ltb_release_submap); then, if the call optimized, the host trimmers run in the order added, after the
+  // ones the C object runs itself, and finished host trimmers are dropped (HandleWorkQueue, :492-501).
+  void AddTrimmer(std::unique_ptr<PoseGraphTrimmer> trimmer) {
+    if (const auto* p = dynamic_cast<const PureLocalizationTrimmer*>(trimmer.get())) {
+      ctx_->check(dl_pg3d_add_pure_localization_trimmer(graph_, p->trajectory_id(), p->num_submaps_to_keep()));
+      return;
+    }
+    trimmers_.push_back(std::move(trimmer));
+  }
+  void FinishTrajectory(int trajectory_id) {  // every submap finished, then the final optimization and the trimmers
+    const int st = dl_pg3d_finish_trajectory(graph_, trajectory_id);
+    AfterCall(st, st == DL_OK);
+  }
+  bool IsTrajectoryFinished(int trajectory_id) const {
+    int32_t finished = 0;
+    ctx_->check(dl_pg3d_is_trajectory_finished(graph_, trajectory_id, &finished));
+    return finished != 0;
+  }
+  void SetInitialTrajectoryPose(int from_trajectory_id, int to_trajectory_id, const Rigid3d& pose, double time) {
+    double p[7];
+    pose.to7(p);
+    ctx_->check(dl_pg3d_set_initial_trajectory_pose(graph_, from_trajectory_id, to_trajectory_id, p, time));
+  }
+  // The node and submap poses of one trajectory keyed by their ids (MapById's view: trimmed ids are absent).
+  std::map<optimization::NodeId, Rigid3d> GetTrajectoryNodePosesById(int trajectory_id) const {
+    std::map<optimization::NodeId, Rigid3d> out;
+    const std::vector<Rigid3d> poses = Poses(trajectory_id, DL_PG3D_NODE_POSES);
+    const std::vector<int32_t> ids = Ids(trajectory_id, DL_PG3D_NODE_POSES);
+    for (size_t i = 0; i < ids.size() && i < poses.size(); ++i) out[{trajectory_id, ids[i]}] = poses[i];
+    return out;
+  }
+  std::map<optimization::SubmapId, Rigid3d> GetAllSubmapPosesById(int trajectory_id) const {
+    std::map<optimization::SubmapId, Rigid3d> out;
+    const std::vector<Rigid3d> poses = Poses(trajectory_id, DL_PG3D_SUBMAP_POSES);
+    const std::vector<int32_t> ids = Ids(trajectory_id, DL_PG3D_SUBMAP_POSES);
+    for (size_t i = 0; i < ids.size() && i < poses.size(); ++i) out[{trajectory_id, ids[i]}] = poses[i];
+    return out;
+  }
 
   // -> the node's id; the submaps' grids, local poses and finished flags come from the builder (dl_ltb_get_submap).
   optimization::NodeId AddNode(int trajectory_id, const LocalTrajectoryBuilder3D& builder,
@@ -875,14 +948,18 @@ class PoseGraph3D {
     std::vector<dl_pg3d_submap_match> m;
     for (const SubmapMatch& sm : matches) m.push_back({sm.submap_id.trajectory_id, sm.submap_id.submap_index, sm.x, sm.y, sm.theta});
     dl_pg3d_add_node_info local{};
-    ctx_->check(dl_pose_graph_3d_add_node(graph_, &node, (int32_t)m.size(), m.data(), &local));
+    const int st = dl_pose_graph_3d_add_node(graph_, &node, (int32_t)m.size(), m.data(), &local);
+    if (st == DL_OK)
+      for (int i = 0; i < node.num_insertion_submaps; ++i) feeders_[{trajectory_id, node.insertion_submaps[i].submap_index}] = &builder;
+    AfterCall(st, st == DL_OK && local.optimized);
     if (info) *info = local;
     return {trajectory_id, local.node_index};
   }
   void FreezeTrajectory(int trajectory_id) { ctx_->check(dl_pose_graph_3d_freeze_trajectory(graph_, trajectory_id)); }
   dl_solve_summary RunFinalOptimization() {
     dl_solve_summary s{};
-    ctx_->check(dl_pose_graph_3d_run_final_optimization(graph_, &s));
+    const int st = dl_pose_graph_3d_run_final_optimization(graph_, &s);
+    AfterCall(st, st == DL_OK);
     return s;
   }
   std::vector<Rigid3d> GetTrajectoryNodePoses(int trajectory_id) const { return Poses(trajectory_id, DL_PG3D_NODE_POSES); }
@@ -907,6 +984,56 @@ class PoseGraph3D {
   dl_pose_graph_3d* get() const { return graph_; }
 
  private:
+  // TrimmingHandle (pose_graph_3d.cc:955-1058) over the C calls.
+  class TrimmingHandle : public Trimmable {
+   public:
+    explicit TrimmingHandle(PoseGraph3D* parent) : parent_(parent) {}
+    std::vector<optimization::SubmapId> GetSubmapIds(int trajectory_id) const override {
+      std::vector<optimization::SubmapId> out;
+      for (const int32_t i : parent_->Ids(trajectory_id, DL_PG3D_SUBMAP_POSES)) out.push_back({trajectory_id, i});
+      return out;
+    }
+    std::vector<PoseGraphConstraint> GetConstraints() const override { return parent_->constraints(); }
+    bool IsFinished(int trajectory_id) const override { return parent_->IsTrajectoryFinished(trajectory_id); }
+    void MarkSubmapAsTrimmed(const optimization::SubmapId& submap_id) override {
+      const int st = dl_pg3d_trim_submap(parent_->graph_, submap_id.trajectory_id, submap_id.submap_index);
+      parent_->AfterCall(st, false);
+    }
+
+   private:
+    PoseGraph3D* parent_;
+  };
+  // The trimmed submaps' grids back to their builders (also after a failed call: it reports what it trimmed before failing),
+  // then the call's status, then the host trimmers if it optimized.
+  void AfterCall(int status, bool optimized) {
+    int32_t n = 0;
+    ctx_->check(dl_pg3d_last_trimmed(graph_, 0, nullptr, &n));
+    std::vector<dl_pg3d_submap_id> trimmed((size_t)n);
+    if (n) ctx_->check(dl_pg3d_last_trimmed(graph_, n, trimmed.data(), &n));
+    for (const dl_pg3d_submap_id& id : trimmed) {
+      const auto it = feeders_.find({id.trajectory_id, id.submap_index});
+      if (it == feeders_.end()) continue;
+      const LocalTrajectoryBuilder3D* builder = it->second;
+      feeders_.erase(it);
+      int32_t finished = 0;
+      ctx_->check(dl_ltb_get_submap(builder->get(), id.submap_index, nullptr, nullptr, nullptr, nullptr, &finished));
+      if (finished) ctx_->check(dl_ltb_release_submap(builder->get(), id.submap_index));
+    }
+    ctx_->check(status);
+    if (!optimized || trimmers_.empty()) return;
+    TrimmingHandle handle(this);
+    for (auto& trimmer : trimmers_) trimmer->Trim(&handle);
+    trimmers_.erase(std::remove_if(trimmers_.begin(), trimmers_.end(),
+                                   [](std::unique_ptr<PoseGraphTrimmer>& t) { return t->IsFinished(); }),
+                    trimmers_.end());
+  }
+  std::vector<int32_t> Ids(int trajectory_id, int which) const {
+    int32_t n = 0;
+    ctx_->check(dl_pg3d_ids(graph_, trajectory_id, which, 0, nullptr, &n));
+    std::vector<int32_t> ids((size_t)n);
+    if (n) ctx_->check(dl_pg3d_ids(graph_, trajectory_id, which, n, ids.data(), &n));
+    return ids;
+  }
   std::vector<Rigid3d> Poses(int trajectory_id, int which) const {
     int32_t n = 0;
     ctx_->check(dl_pose_graph_3d_poses(graph_, trajectory_id, which, 0, nullptr, &n));
@@ -918,6 +1045,8 @@ class PoseGraph3D {
   }
   Context* ctx_;
   dl_pose_graph_3d* graph_ = nullptr;
+  std::map<optimization::SubmapId, const LocalTrajectoryBuilder3D*> feeders_;  // where AddNode got each submap's grids
+  std::vector<std::unique_ptr<PoseGraphTrimmer>> trimmers_;                     // host trimmers, in the order added
 };
 
 }  // namespace mapping

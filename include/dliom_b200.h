@@ -396,9 +396,28 @@ int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const dl_pose_gra
  *      the found constraints stay pending (the next optimization appends them); the call returns the solve's status.
  *      Deliberate differences: execution is synchronous and deterministic (the reference's thread pool may or may not finish a
  *      search before WhenDone); not built: the per-node proximity search (its MaybeAdd*Constraint bodies are commented out in
- *      this fork, :205-323, :367-381), trimming and trajectory connectivity, landmark / fixed-frame / odometry / IMU terms,
- *      .pbstream loading, and a communicator (one GPU; the search and the solve it calls have NCCL variants).
- *      The submap grids are borrowed (owner: the caller, e.g. the dl_local_trajectory_builder) and must outlive the graph. ---- */
+ *      this fork, :205-323, :367-381), trajectory connectivity and global-localization sampling, landmark / fixed-frame /
+ *      odometry / IMU terms, .pbstream loading, and a communicator (one GPU; the search and the solve it calls have NCCL
+ *      variants).
+ *      The submap grids are borrowed (owner: the caller, e.g. the dl_local_trajectory_builder) and must outlive the graph, or
+ *      their submap's trim (see dl_pg3d_last_trimmed).
+ *
+ *      Pure localization (MapBuilder with pure_localization, map_builder.cc:147-151): the dl_pg3d_* calls below. Their prefix is
+ *      the block's type prefix; the dl_pose_graph_3d_* entry points above are the mapping path.
+ *      Ids with holes: submaps and nodes are MapById per trajectory (C/mapping/id.h). A trim removes one id; trimming a
+ *      trajectory's highest submap (node) index forbids appending submaps (nodes) to it (id.h:289-300), and an add_node that
+ *      would append one returns DL_ERR_ARG, the graph unchanged. The solve's submap and node order, the fan-out over a
+ *      finished submap's node ids and GetLocalToGlobalTransform's last optimized submap skip the holes; the solve holds its
+ *      first remaining submap (OptimizationProblem3D::Solve's first_submap, optimization_problem_3d.cc:286-316). A match or
+ *      an insertion submap naming a trimmed submap is rejected like an unknown one.
+ *      Trimmers (HandleWorkQueue, :492-501) run at the end of every successful optimization (the periodic one of add_node,
+ *      dl_pose_graph_3d_run_final_optimization, dl_pg3d_finish_trajectory) in the order they were added; a finished trimmer
+ *      is dropped; a failed solve runs none. Trimmed nodes' clouds become dead ranges of the node store; when the dead floats
+ *      exceed the live ones and number at least 2^20 (4 MiB), kernel pg3d_store_compact copies every live node's clouds into
+ *      a fresh store in one launch and the old one is freed, so after every trim used <= 2 * live or used - live < 4 MiB
+ *      (dl_pg3d_store_usage), and the copying costs O(1) per uploaded float. A failed compaction leaves the old store and
+ *      offsets as they were and returns DL_ERR_CUDA; the trim itself stands. A graph on which no dl_pg3d_* call is made
+ *      behaves exactly as without them. ---- */
 typedef struct dl_pose_graph_3d dl_pose_graph_3d;
 typedef struct dl_pose_graph_3d_options { /* proto::PoseGraphOptions, the fields this path reads */
   int32_t optimize_every_n_nodes;         /* 0: only on dl_pose_graph_3d_run_final_optimization */
@@ -486,6 +505,45 @@ typedef struct dl_pg3d_search {
 int dl_pose_graph_3d_last_searches(const dl_pose_graph_3d* graph, int32_t capacity, dl_pg3d_search* out, int32_t* count);
 /* Bytes of clouds uploaded into the node store since creation, and its capacity in bytes. */
 int dl_pose_graph_3d_store_bytes(const dl_pose_graph_3d* graph, int64_t* uploaded, int64_t* capacity);
+typedef struct dl_pg3d_submap_id {         /* SubmapId */
+  int32_t trajectory_id, submap_index;
+} dl_pg3d_submap_id;
+/* TrimmingHandle::MarkSubmapAsTrimmed (:1002-1058): nodes_to_retain = the nodes with an INTRA_SUBMAP constraint to another
+ * submap; every constraint of the submap is dropped; the nodes left without an INTRA_SUBMAP constraint and every constraint
+ * of theirs are dropped; the submap and those nodes leave the graph and the optimization problem (optimization_problem_3d.cc:
+ * 229-251). DL_ERR_ARG, the graph unchanged: an unknown or already trimmed submap, an unfinished submap (the reference
+ * CHECKs), or constraints still pending (there are none right after an optimization, which is where trimmers run). */
+int dl_pg3d_trim_submap(dl_pose_graph_3d* graph, int32_t trajectory_id, int32_t submap_index);
+/* PureLocalizationTrimmer (C/mapping/pose_graph_trimmer.cc:24-45): after each optimization, every submap of the trajectory but
+ * the newest num_submaps_to_keep (in index order) is trimmed; once the trajectory is finished all of them are, and the trimmer
+ * is done. num_submaps_to_keep < 3: DL_ERR_ARG. */
+int dl_pg3d_add_pure_localization_trimmer(dl_pose_graph_3d* graph, int32_t trajectory_id, int32_t num_submaps_to_keep);
+/* FinishTrajectory (:535-547): every submap of the trajectory becomes finished, then the step of
+ * dl_pose_graph_3d_run_final_optimization runs (pending constraints appended, solve, update, trimmers). The trajectory stays
+ * finished if that solve fails. Finishing twice returns DL_ERR_ARG; so does dl_pose_graph_3d_add_node on a finished
+ * trajectory. */
+int dl_pg3d_finish_trajectory(dl_pose_graph_3d* graph, int32_t trajectory_id);
+int dl_pg3d_is_trajectory_finished(const dl_pose_graph_3d* graph, int32_t trajectory_id, int32_t* finished);
+/* SetInitialTrajectoryPose (:849-856) with GetInterpolatedGlobalTrajectoryPose (:858-876, used at :914-928): while trajectory
+ * `from` has no optimized submap, its local-to-global transform is the `to` trajectory's node global poses interpolated at
+ * `time`, times relative_pose (t xyz, q wxyz). The interpolation takes the first node whose time is not below `time`
+ * (lower_bound); before the first node it is the first node's pose, past the last the last one's; else
+ * transform::Interpolate of the node before it and it: factor = (time - t0) / (t1 - t0) from the dl_pg3d_node::time doubles,
+ * translation t0 + (t1 - t0) * factor, rotation Eigen's slerp. `to` without nodes when the transform is needed: the call
+ * that needs it (add_node of `from`, the poses or local_to_global query) returns DL_ERR_ARG (the reference CHECKs). */
+int dl_pg3d_set_initial_trajectory_pose(dl_pose_graph_3d* graph, int32_t from_trajectory_id, int32_t to_trajectory_id,
+                                        const double* relative_pose, double time);
+/* The indices of the rows dl_pose_graph_3d_poses returns for the same `which` (submaps or nodes still in the graph, in index
+ * order). Pass indices = NULL to query *count. */
+int dl_pg3d_ids(const dl_pose_graph_3d* graph, int32_t trajectory_id, int32_t which, int32_t capacity, int32_t* indices,
+                int32_t* count);
+/* The submaps trimmed by the last dl_pose_graph_3d_add_node, dl_pose_graph_3d_run_final_optimization, dl_pg3d_finish_trajectory
+ * or dl_pg3d_trim_submap call, in trim order; each of these calls empties the list when it starts, so after a call that failed
+ * (a rejection, or a failure after some trims had already been made) it holds exactly what that call trimmed. Their grids are
+ * no longer read by the graph: the caller may release them (dl_ltb_release_submap). Pass out = NULL to query *count. */
+int dl_pg3d_last_trimmed(const dl_pose_graph_3d* graph, int32_t capacity, dl_pg3d_submap_id* out, int32_t* count);
+/* The node store in bytes: live (the clouds of the nodes still in the graph), used (written, dead ranges included), capacity. */
+int dl_pg3d_store_usage(const dl_pose_graph_3d* graph, int64_t* live_bytes, int64_t* used_bytes, int64_t* capacity_bytes);
 
 /* ---- IMU: pre-integration (LocalTrajectoryBuilder3D::AddImuData, LTB:164-201, with the in-repo mid-point integrator
  *      C/mapping/internal/3d/initialization/integration_base.h:109-265 instead of the un-vendored GTSAM one) and the
@@ -833,9 +891,14 @@ int dl_ltb_add_range_data_batch(int32_t count, const dl_ltb_batch_item* items, d
 int dl_ltb_get_cloud(const dl_local_trajectory_builder* builder, int32_t which, float* out, int64_t capacity_points, int64_t* num_points);
 int dl_ltb_get_histogram(const dl_local_trajectory_builder* builder, float* out, int32_t capacity);
 int32_t dl_ltb_num_submaps(const dl_local_trajectory_builder* builder);
-/* Submap `index` (0 = the first ever created): its device grids (owned by the builder), local pose, insert count, finished flag. */
+/* Submap `index` (0 = the first ever created): its device grids (owned by the builder; NULL once released), local pose, insert
+ * count, finished flag. */
 int dl_ltb_get_submap(dl_local_trajectory_builder* builder, int32_t index, dl_grid** high_resolution_grid,
                       dl_grid** low_resolution_grid, double* local_pose, int32_t* num_range_data, int32_t* finished);
+/* Frees the two device grids of finished submap `index` (the reference's shared_ptr<const Submap3D> dropping to zero once the
+ * pose graph trimmed it); the record (local pose, insert count, finished flag) stays. An active submap, an unknown index or
+ * a second release: DL_ERR_ARG, nothing freed. */
+int dl_ltb_release_submap(dl_local_trajectory_builder* builder, int32_t index);
 int dl_ltb_get_state(const dl_local_trajectory_builder* builder, dl_nav_state* state, int32_t* initialized);
 
 /* ---- submap images: Submap3D::ToResponseProto's X-ray textures (C/mapping/3d/submap_3d.cc:53-178, :253-262) and the fork's
