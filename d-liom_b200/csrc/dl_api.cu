@@ -163,8 +163,6 @@ void dl_context_destroy(dl_context* ctx) {
   if (ctx->batch_done) cudaEventDestroy(ctx->batch_done);
   if (ctx->sync_event) cudaEventDestroy(ctx->sync_event);
   if (ctx->d_fcsm_lut) cudaFree(ctx->d_fcsm_lut);
-  if (ctx->h_adaptive_stats) cudaFreeHost(ctx->h_adaptive_stats);
-  if (ctx->d_adaptive_stats) cudaFree(ctx->d_adaptive_stats);
   if (ctx->staging_done) cudaEventDestroy(ctx->staging_done);
   delete ctx;
 }
@@ -654,14 +652,12 @@ int dl_adaptive_voxel_filter(dl_context* ctx, const dl_adaptive_voxel_filter_opt
   float *d_pts, *d_passes;
   uint32_t *d_table, *d_scratch;
   int32_t *d_keep, *d_counts;
-  uint8_t* d_first;
   AdaptiveParams* d_params;
   DL_TRY(carve_scratch(ctx, [&](Arena& a) {
     d_pts = a.take<float>(n * stride);
     d_table = a.take<uint32_t>(tcap);
     d_scratch = a.take<uint32_t>(2 * n);
     d_keep = a.take<int32_t>(n);
-    d_first = a.take<uint8_t>(adaptive_first_pass_bytes(1, n));
     d_counts = a.take<int32_t>(3);  // n, survivors, passes
     d_params = a.take<AdaptiveParams>(1);
     d_passes = a.take<float>(32);
@@ -672,7 +668,7 @@ int dl_adaptive_voxel_filter(dl_context* ctx, const dl_adaptive_voxel_filter_opt
   DL_TRY(h2d(ctx, d_counts, &n32, 1));
   DL_TRY(h2d(ctx, d_params, &params, 1));
   DL_TRY(launch_adaptive_voxel_filter(ctx, d_pts, stride, n, d_counts, 1, d_params, 1, d_table, tcap, d_scratch, d_keep,
-                                      d_counts + 1, d_passes, d_counts + 2, nullptr, d_first));
+                                      d_counts + 1, d_passes, d_counts + 2, nullptr));
   int32_t res[2] = {0, 0};
   float passes[32];
   DL_TRY(d2h(ctx, res, d_counts + 1, 2));
@@ -1836,7 +1832,6 @@ struct FrontendBuffers {
   uint32_t* spill;
   int32_t *last_index, *error_flag;
   float* local4;
-  uint8_t* adaptive_first;  // scratch of the adaptive filters' grid-wide first pass (dl_voxel.cu)
   ScanConstants* scans;
   AdaptiveParams* filters;
   Rigidd *submap, *submap_inverse;  // per scan: its matching submap's local pose and the inverse (host arithmetic)
@@ -1877,7 +1872,6 @@ void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f
   f->spill_used = a.take<int32_t>(2 * B);
   f->last_index = a.take<int32_t>(B); f->error_flag = a.take<int32_t>(B);
   f->local4 = a.take<float>(B * C * 4);
-  f->adaptive_first = a.take<uint8_t>(adaptive_first_pass_bytes(2 * batch, cap) + 16 * 1024);
 }
 
 // Device copies of the time_run_* arrays of 12-byte rows (validated by check_frontend) and, with many runs per scan, the table
@@ -2201,8 +2195,7 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
         DL_TRY(launch_adaptive_voxel_filter(ctx, f.returns_tracking + (size_t)b0 * f.cap * 3, 3, f.cap, f.n2 + b0, nb, f.filters, 2,
                                             f.tableA + (size_t)2 * b0 * f.tcap, f.tcap, f.scratchA + (size_t)4 * b0 * f.cap,
                                             f.keepA + (size_t)2 * b0 * f.cap, f.countsA + 2 * b0, f.passesA + 64 * b0,
-                                            f.npassesA + 2 * b0, f.croppedA + 2 * b0,
-                                            f.adaptive_first + adaptive_first_pass_bytes(2 * b0, f.cap) + (size_t)k * 1024));
+                                            f.npassesA + 2 * b0, f.croppedA + 2 * b0));
       }
       DL_TRY(launch_gather_rows(ctx, f.returns_tracking + (size_t)b0 * f.cap * 3, f.cap, 2, f.keepA + (size_t)2 * b0 * f.cap,
                                 f.countsA + 2 * b0, f.cap, f.clouds + (size_t)2 * b0 * f.cap * 3, 2 * nb));

@@ -52,11 +52,6 @@ struct dl_context {
   cudaStream_t tail_stream = nullptr;   // high priority: the front end's raw-IMU chain (pre-integration, prediction), next to the first filter
   cudaEvent_t staging_done = nullptr;   // the pinned staging block of the previous call has been consumed
   cudaEvent_t batch_done = nullptr;     // dl_frontend_submit: everything of the batch in flight, incl. the result download
-  // adaptive voxel filter: how many (cloud, filter) pairs of the last probed launch needed the single-CTA search
-  // ([0] pairs that fell through, [1] pairs probed); pinned host copy of a device counter, read without synchronising
-  int32_t* h_adaptive_stats = nullptr;
-  int32_t* d_adaptive_stats = nullptr;
-  int64_t adaptive_calls = 0;
   uint8_t* d_fcsm_lut = nullptr;        // loop-closure search: cell value -> 8-bit precomputation value (dl_fcsm.cu), built on first use
   int in_flight = 0;                    // scans of the submitted, not yet collected batch
   bool in_flight_states = false;        // ... and whether it also stages the estimated IMU states
@@ -218,9 +213,7 @@ int launch_adaptive_voxel_filter(dl_context* ctx, const float* points, int strid
                                  int batch, const AdaptiveParams* filters_dev, int num_filters, uint32_t* table,
                                  int64_t table_cap, uint32_t* scratch /* pairs * 2 * cap */, int32_t* keep, int32_t* keep_counts,
                                  float* passes /* (batch*num_filters) * 32 */, int32_t* num_passes,
-                                 int32_t* cropped_counts /* optional, batch*num_filters */,
-                                 void* first_pass_scratch /* optional, adaptive_first_pass_bytes(batch * num_filters, cap) */);
-size_t adaptive_first_pass_bytes(int pairs, int64_t cap);
+                                 int32_t* cropped_counts /* optional, batch*num_filters */);
 
 struct RtcsmScan {  // one scan of a batched correlative search (dl_rtcsm.cu), device pointers
   const float* points;  // n x 3

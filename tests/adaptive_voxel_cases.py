@@ -4,7 +4,6 @@ name says: the cropped size, the voxel count or the cell box at the edge that de
 limit. A case is (name, rows, (max_length, min_num_points, max_range)).
 
 The device limits the generators aim at:
-  FIRST_PASS_SLOTS  8 192  slots of the grid-wide first-pass table per (cloud, filter) pair
   REGISTER_POINTS   8 192  cropped points the single-CTA search holds in registers (8 per thread)
   FAST_CAPACITY    22 528  cropped points of the fast mode: registers plus 14 336 in shared memory; above it, generic mode
   HASH_SLOTS        4 096  slots of the fast mode's shared hash table
@@ -19,7 +18,6 @@ import numpy as np
 import adaptive_voxel_reference as R
 
 f32 = np.float32
-FIRST_PASS_SLOTS = 8192
 REGISTER_POINTS = 8192
 FAST_CAPACITY = 22528
 HASH_SLOTS = 4096
@@ -28,9 +26,7 @@ PACK_MIN, PACK_MAX = -2 ** 20, 2 ** 20 - 2
 # round_div's shortcut keeps x * (1 / edge) only when 0.5 - |distance to the nearest integer| > |q| * 4.8e-7: from this |q| on
 # it never can, and every quotient takes the division
 ALWAYS_DIVIDES = 0.5 / 4.8e-7
-# dl_adaptive_voxel_filter sizes its table next_pow2(2 n) slots of 4 B; the first pass needs 8 192 x 12 B of it, so the
-# standalone call takes the first pass only for n > 8 192.
-STANDALONE_FIRST_PASS_MIN_N = 8193
+PADDED_ROWS = 8193  # padded() fills every cloud up to at least this many rows
 
 Case = collections.namedtuple("Case", "name rows opts")
 
@@ -57,8 +53,8 @@ def interleave(inside, outside, rng):
 
 
 def padded(inside, max_range, rng, extra=500):
-    """`inside` with out-of-range rows interleaved, at least STANDALONE_FIRST_PASS_MIN_N rows in all."""
-    k = max(extra, STANDALONE_FIRST_PASS_MIN_N - len(inside))
+    """`inside` with out-of-range rows interleaved, at least PADDED_ROWS rows in all."""
+    k = max(extra, PADDED_ROWS - len(inside))
     return interleave(np.asarray(inside, f32), outside_points(k, max_range, rng), rng)
 
 
@@ -142,22 +138,22 @@ def hash_case(voxels, expect):
     return case
 
 
-def first_pass_table_case(voxels, expect):
-    """`voxels` occupied 1 m cells of a 32 x 16 x 17 block, three points each; the first edge suffices."""
+def many_voxels_case(voxels):
+    """`voxels` occupied 1 m cells of a 32 x 16 x 17 block, three points each; the first edge suffices, with far more voxels
+    than the search's result table holds (generic mode)."""
     rng = np.random.RandomState(voxels)
     opts = (1.0, 150.0, 100.0)
     grid = np.stack(np.meshgrid(np.arange(32), np.arange(16), np.arange(17), indexing="ij"), -1).reshape(-1, 3)
     centres = grid[rng.choice(len(grid), voxels, replace=False)].astype(f32)
     pts = np.repeat(centres, 3, axis=0) + rng.uniform(-0.45, 0.45, (3 * voxels, 3))
-    case = Case(f"first_pass_{voxels}_voxels_at_max_length", padded(pts[rng.permutation(len(pts))], opts[2], rng), opts)
+    case = Case(f"voxels_{voxels}_at_max_length", padded(pts[rng.permutation(len(pts))], opts[2], rng), opts)
     n = R.num_voxels(cropped(case), opts[0])
-    assert side(n, FIRST_PASS_SLOTS) == expect and n >= opts[1]
+    assert n == voxels and n >= opts[1]
     return case
 
 
 def table_cases():
-    return [hash_case(HASH_SLOTS, 0), hash_case(HASH_SLOTS + 1, 1), first_pass_table_case(FIRST_PASS_SLOTS, 0),
-            first_pass_table_case(FIRST_PASS_SLOTS + 1, 1)]
+    return [hash_case(HASH_SLOTS, 0), hash_case(HASH_SLOTS + 1, 1), many_voxels_case(8192), many_voxels_case(8193)]
 
 
 # ------------------------------------------------------------------------------------------- byte-map box
@@ -306,7 +302,6 @@ def street_cases(orc):
     opts = orc.FrontEndOptions.defaults(voxel_filter_size=0.05)
     pts = orc.ingest_scan(opts, w["scans"][0], w["origin"], w["prev"][0], w["cur"][0])["returns_tracking"]
     pts = pts[np.random.RandomState(3).permutation(len(pts))]
-    assert len(pts) > STANDALONE_FIRST_PASS_MIN_N
     return [Case("shuffled_street_scan_high_resolution", pts, (2.0, 150.0, 15.0)),
             Case("shuffled_street_scan_low_resolution", pts, (4.0, 200.0, 60.0))]
 
@@ -331,7 +326,7 @@ def format_cases():
         rows = np.full((len(pts), stride), np.nan, f32)
         rows[:, :3] = pts
         out.append(Case(f"stride_{stride}_nan_rows_point_at_max_range", rows, opts))
-    for n in (0, 1, STANDALONE_FIRST_PASS_MIN_N):
+    for n in (0, 1, PADDED_ROWS):
         out.append(Case(f"rows_{n}", rng.uniform(-5, 5, (n, 3)).astype(f32), (2.0, 150.0, 15.0)))
     return out
 
@@ -343,9 +338,3 @@ def all_cases(orc=None):
         cases += street_cases(orc)
     return cases
 
-
-def primer():
-    """A search-route primer for the standalone call: n > 8 192 rows in one voxel, so its single pair falls through the first
-    pass (one voxel of 1 m against min_num_points 150) to the single-CTA search."""
-    pts = np.tile(np.array([[0.2, 0.2, 0.2]], f32), (STANDALONE_FIRST_PASS_MIN_N + 100, 1))
-    return Case("primer", pts, (1.0, 150.0, 15.0))

@@ -1,18 +1,7 @@
 """The device adaptive voxel filter (dl_voxel.cu) against the oracle, bit for bit (survivor indices and pass edges), on clouds built
-to sit on its edges (adaptive_voxel_cases.py: each generator checks with the numpy reference that it lands on its edge), each
-on both routes of launch_adaptive_voxel_filter, and the batched front end with pairs of every kind in one launch.
-
-Routes. launch_adaptive_voxel_filter runs the grid-wide first pass (8 192-slot table per pair) unless it is skipped, and the
-single-CTA search (fast mode, or generic mode) for the pairs the first pass did not finish. The choice is self-tuned from the
-context's call history: every call that can take the first pass counts one in `adaptive_calls`; a call with
-`adaptive_calls % 16 == 0` probes (runs the first pass and records how many pairs fell through), and the next 15 calls skip the
-first pass when more than half the pairs of the last probe fell through. So, without any switch in the library:
-  first_pass  a fresh dliom.Context whose first adaptive call is the case (a probe: the first pass runs);
-  search      a fresh context whose first call is a primer whose single pair falls through (n > 8 192 rows in one voxel), so
-              the case, its second call, skips the first pass and the single-CTA search does everything.
-dl_adaptive_voxel_filter sizes its table next_pow2(2 n) slots of 4 B and the first pass needs 8 192 x 12 B of it, so the
-standalone call can take the first pass only for n > 8 192 rows: below that both routes are the single-CTA search. Every case
-checks its route by the kernel launches it made (first pass: 5 kernels + the search kernel; search: 1)."""
+to sit on its edges (adaptive_voxel_cases.py: each generator checks with the numpy reference that it lands on its edge), and the
+batched front end with pairs of every kind in one launch. Every case runs once on a fresh dliom.Context, and the standalone call
+makes exactly one kernel launch (none for an empty cloud)."""
 import functools
 
 import numpy as np
@@ -25,10 +14,7 @@ from helpers import workload
 pytestmark = pytest.mark.gpu
 
 f32 = np.float32
-ROUTES = ["first_pass", "search"]
-FIRST_PASS_LAUNCHES = 6
 CASES = K.all_cases()
-RESULTS = {}   # case name -> route -> (keep, passes): both routes must agree with each other as well as with the oracle
 
 
 @functools.lru_cache(maxsize=None)
@@ -37,16 +23,11 @@ def oracle(name):
     return tuple(np.asarray(x) for x in __import__("orc").adaptive_voxel_filter(case.rows, *case.opts))
 
 
-def run(case, route):
-    """-> (survivors, pass edges, kernel launches of the call) on a fresh context, along `route`."""
+def run(case):
+    """-> (survivors, pass edges, kernel launches of the call) on a fresh context."""
     import dliom
     ctx = dliom.Context(0)
     try:
-        if route == "search":
-            p = K.primer()
-            before = ctx.launches
-            keep, passes = ctx.adaptive_voxel_filter(p.rows, *p.opts)
-            assert ctx.launches - before == FIRST_PASS_LAUNCHES and len(keep) == 1 and len(passes) == 8
         before = ctx.launches
         keep, passes = ctx.adaptive_voxel_filter(case.rows, *case.opts)
         return keep, passes, ctx.launches - before
@@ -54,45 +35,31 @@ def run(case, route):
         ctx.close()
 
 
-def expected_launches(case, route):
-    if len(case.rows) == 0:
-        return 0
-    if route == "first_pass" and len(case.rows) >= K.STANDALONE_FIRST_PASS_MIN_N:
-        return FIRST_PASS_LAUNCHES
-    return 1
-
-
-def check(case, route, want_keep, want_passes):
-    keep, passes, launches = run(case, route)
-    assert launches == expected_launches(case, route)
+def check(case, want_keep, want_passes):
+    keep, passes, launches = run(case)
+    assert launches == (1 if len(case.rows) else 0)
     assert np.array_equal(passes.view(np.uint32), np.asarray(want_passes, f32).view(np.uint32)), (passes, want_passes)
     assert np.array_equal(keep, want_keep)
-    for other in RESULTS.get(case.name, {}).values():
-        assert np.array_equal(other[0], keep) and np.array_equal(other[1].view(np.uint32), passes.view(np.uint32))
-    RESULTS.setdefault(case.name, {})[route] = (keep, passes)
 
 
-@pytest.mark.parametrize("route", ROUTES)
 @pytest.mark.parametrize("case", CASES, ids=[c.name for c in CASES])
-def test_device_matches_the_oracle(orc, case, route):
+def test_device_matches_the_oracle(orc, case):
     want_keep, want_passes = oracle(case.name)
-    check(case, route, want_keep, want_passes)
+    check(case, want_keep, want_passes)
 
 
-@pytest.mark.parametrize("route", ROUTES)
 @pytest.mark.parametrize("which", [0, 1], ids=["shuffled_street_scan_high_resolution", "shuffled_street_scan_low_resolution"])
-def test_device_matches_the_oracle_on_a_shuffled_street_scan(orc, which, route):
+def test_device_matches_the_oracle_on_a_shuffled_street_scan(orc, which):
     case = K.street_cases(orc)[which]
     want_keep, want_passes = orc.adaptive_voxel_filter(case.rows, *case.opts)
-    check(case, route, want_keep, want_passes)
+    check(case, want_keep, want_passes)
 
 
 # ------------------------------------------------------------------------------------------- batched front end
 # A 5 cm first voxel filter leaves ~18 000 returns per 16-beam sweep. High-resolution filter 2 m / 300 / 15 m, low-resolution
 # filter 10 cm / 200 / 60 m. Per scan, in a period of five: a sweep (high: bisection, 120 to 210 voxels at 2 m; low: ~11 000 voxels at
-# 10 cm, beyond the first-pass table), the same sweep scaled by 0.3 toward the sensor (high: bisection; low: first edge
-# sufficient), twice, and the first 150 rows of a sweep (sparse enough for both). Six of every ten pairs fall through the first
-# pass, so calls after a probe skip it: the batch runs both routes.
+# 10 cm, far beyond the search's result table), the same sweep scaled by 0.3 toward the sensor (high: bisection; low: first edge
+# sufficient), twice, and the first 150 rows of a sweep (sparse enough for both).
 def batch_scans(w, count):
     scans, prev, cur = [], [], []
     for i in range(count):
@@ -114,8 +81,8 @@ def pair_kind(pts, max_length, min_num_points, max_range):
     if f32(len(c)) <= f32(min_num_points):
         return "sparse"
     v = R.num_voxels(c, max_length)
-    if v > K.FIRST_PASS_SLOTS:
-        return "first_pass_overflow"
+    if v > 8192:
+        return "first_edge_over_8192_voxels"
     return "first_edge" if f32(v) >= f32(min_num_points) else "bisection"
 
 
@@ -141,9 +108,8 @@ def batch_case():
         kinds.append(tuple(pair_kind(pts, *f) for f in filters))
     # every five consecutive scans (any launch of at least five) hold pairs of all four kinds
     for s in range(len(scans) - 4):
-        assert {k for ks in kinds[s:s + 5] for k in ks} == {"sparse", "first_edge", "bisection", "first_pass_overflow"}, kinds
-    fell = sum(k in ("bisection", "first_pass_overflow") for ks in kinds for k in ks)
-    assert fell > len(scans)                        # more than half of the 2 pairs per scan
+        assert {k for ks in kinds[s:s + 5] for k in ks} == {"sparse", "first_edge", "bisection", "first_edge_over_8192_voxels"}, \
+            kinds
     return w, opts, scans, prev, cur, want
 
 
@@ -182,11 +148,11 @@ def repeat_identical(ctx, call, first, calls):
     return launches
 
 
-def test_frontend_batch_pairs_of_every_kind_against_the_oracle(orc):
+def test_frontend_batch_pairs_of_every_kind_against_the_oracle_with_steady_launches(orc):
     """Host scans (5 sub-batches per call) and device-resident scans (2 per call), 40 scans: every pair's cropped size, pass
     count and survivor count against the oracle, the pose within 1e-7 m / 1e-8 rad of orc.match_scan with the same iteration
-    count; then 4 (host) and 8 (device) more calls on the same context, i.e. 20 and 16 more sub-batch launches, probing and
-    not probing, which must repeat every pose and count bit for bit."""
+    count; then 4 (host) and 8 (device) more calls on the same context, i.e. 20 and 16 more sub-batch launches, which must
+    repeat every pose and count bit for bit with the same number of kernel launches."""
     import ctypes as C
     import dliom
     w, opts, scans, prev, cur, want = batch_case()
@@ -200,7 +166,7 @@ def test_frontend_batch_pairs_of_every_kind_against_the_oracle(orc):
     launches = {ctx.launches - before}
     check_against_oracle(first, want)
     launches |= repeat_identical(ctx, lambda: ctx.frontend_match_batch(fo, scans, *args), first, 4)
-    assert len(launches) > 1, launches          # some calls ran the first pass and some skipped it
+    assert len(launches) == 1, launches
     ctx.close()
 
     ctx = dliom.Context(0)
@@ -222,7 +188,7 @@ def test_frontend_batch_pairs_of_every_kind_against_the_oracle(orc):
     check_against_oracle(first_dev, want)
     for a, b in zip(first_dev, first):
         assert list(a.pose_estimate_local) == list(b.pose_estimate_local) and counts(a) == counts(b)
-    repeat_identical(ctx, dev, first_dev, 8)
+    assert len(repeat_identical(ctx, dev, first_dev, 8)) == 1
     for p in (d_rows, d_res):
         ctx.device_free(p)
     ctx.close()

@@ -2,7 +2,7 @@
 sweeps, bit for bit against the oracle (survivors and pass edges). Each sweep streams the cloud and counts the voxels of a few edges
 on byte maps over the cloud's cell box; the search replays on the stored counts, and an edge it asks for that was not counted costs
 one more sweep. Every generator checks with the numpy reference (adaptive_voxel_reference.py) that its cloud lands where its name
-says. The clouds have at most 8 192 rows, so the standalone call always takes the single-CTA search (one launch).
+says. Every standalone call is one launch of the search.
 
 The limits:
   MAP_BYTES     32 768  cells of byte map per sweep; an edge whose box alone is larger sends the pair to generic mode
@@ -19,7 +19,6 @@ import adaptive_voxel_reference as R
 f32 = np.float32
 MAP_BYTES = 32768
 RESULT_SLOTS = 2048
-MAX_ROWS = K.STANDALONE_FIRST_PASS_MIN_N - 1
 
 
 def line_case(name, cells, voxels, opts=(1.0, 150.0, 1e5)):
@@ -57,7 +56,7 @@ def plane_case(name, side, target_passes, min_from):
     """8 000 uniform points on a side x side plane; min_num_points = the voxel count at edge `min_from`, so that the search walks
     exactly `target_passes` (edges as multiples of max_length 1)."""
     rng = np.random.RandomState(int(side * 7))
-    pts = np.zeros((MAX_ROWS - 192, 3), f32)
+    pts = np.zeros((8000, 3), f32)
     pts[:, :2] = rng.uniform(0, side, (len(pts), 2))
     opts = (1.0, float(R.num_voxels(pts, f32(min_from))), 1e3)
     keep, passes, _ = R.search(pts, *opts)
