@@ -742,11 +742,13 @@ void build_rtcsm_tables(const dl_rtcsm_options& opt, float resolution, float max
 // — the angular window depends on each cloud's farthest point through acosf, which must be the host's to stay bit-exact —
 // and go up in ONE copy; one launch scores all (scan, rotation, translation) candidates.
 struct RtcsmBatchItem {
+  const dl_grid* grid;  // the grid this scan is scored against; every grid of a batch has the plan's resolution
   const float* d_points;
   int64_t n;
   Rigidd initial;
   float max_scan_range;
-  float* d_scores;  // optional
+  float* d_scores;          // optional
+  int32_t* d_nonpositive;   // optional: set to 1 when a candidate's score is not > 0
 };
 // plan_rtcsm_batch builds the tables and lays out the one upload (every scan's tables, the descriptors, the CTA prefix); take()
 // carves that upload and the argmax words, so a caller can count the scratch before it reserves it; run_rtcsm_batch uploads
@@ -789,8 +791,8 @@ int plan_rtcsm_batch(dl_context* ctx, const dl_rtcsm_options& opt, float resolut
   plan->blob = blob;
   return DL_OK;
 }
-// `plan` has taken its scratch; items[k].d_points / d_scores are read here.
-int run_rtcsm_batch(dl_context* ctx, const dl_grid* grid, const std::vector<RtcsmBatchItem>& items, const RtcsmBatchPlan& plan) {
+// `plan` has taken its scratch; items[k].d_points / d_scores / d_nonpositive are read here.
+int run_rtcsm_batch(dl_context* ctx, const std::vector<RtcsmBatchItem>& items, const RtcsmBatchPlan& plan) {
   const int B = (int)items.size();
   if (B == 0) return DL_OK;
   std::vector<unsigned char> host(plan.blob);
@@ -801,6 +803,7 @@ int run_rtcsm_batch(dl_context* ctx, const dl_grid* grid, const std::vector<Rtcs
     std::memcpy(host.data() + plan.off_pr[k], t.pen_r.data(), t.pen_r.size() * sizeof(double));
     std::memcpy(host.data() + plan.off_pt[k], t.pen_t.data(), t.pen_t.size() * sizeof(double));
     RtcsmScan sc{};
+    sc.grid = items[k].grid->view();
     sc.points = items[k].d_points;
     sc.n = (int32_t)items[k].n;
     sc.cand_q = (const Quatf*)(plan.d_blob + plan.off_q[k]);
@@ -811,13 +814,14 @@ int run_rtcsm_batch(dl_context* ctx, const dl_grid* grid, const std::vector<Rtcs
     sc.L = (int32_t)t.cand_t.size();
     sc.scores = items[k].d_scores;
     sc.best = plan.d_best + k;
+    sc.nonpositive = items[k].d_nonpositive;
     std::memcpy(host.data() + plan.off_scans + (size_t)k * sizeof(RtcsmScan), &sc, sizeof(sc));
   }
   std::memcpy(host.data() + plan.off_prefix, plan.prefix.data(), (size_t)(B + 1) * sizeof(int32_t));
   DL_TRY(h2d(ctx, plan.d_blob, host.data(), plan.blob));
   DL_CUDA(ctx, cudaMemsetAsync(plan.d_best, 0, sizeof(unsigned long long) * B, ctx->stream));
   DL_TRY(sync(ctx));  // `host` is pageable and local
-  return launch_rtcsm_batch(ctx, grid->view(), plan.d_scans, (const int32_t*)(plan.d_blob + plan.off_prefix), B, plan.prefix[B]);
+  return launch_rtcsm_batch(ctx, plan.d_scans, (const int32_t*)(plan.d_blob + plan.off_prefix), B, plan.prefix[B]);
 }
 
 // The farthest point of a host cloud, floored at 3 * resolution (cc:63-71), with the norm the device reduction uses.
@@ -861,7 +865,7 @@ int dl_rtcsm_match(dl_context* ctx, const dl_rtcsm_options* options, const doubl
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   // The cloud is on the host: its farthest point, hence the tables and the exact scratch, are known before the carve.
   const float max_scan_range = max_scan_range_host(points, n, grid->resolution);
-  std::vector<RtcsmBatchItem> items{RtcsmBatchItem{nullptr, n, pose_from7(initial_pose), max_scan_range, nullptr}};
+  std::vector<RtcsmBatchItem> items{RtcsmBatchItem{grid, nullptr, n, pose_from7(initial_pose), max_scan_range, nullptr, nullptr}};
   RtcsmBatchPlan plan;
   DL_TRY(plan_rtcsm_batch(ctx, *options, grid->resolution, items, &plan));
   const RtcsmTables& t = plan.tables[0];
@@ -876,7 +880,7 @@ int dl_rtcsm_match(dl_context* ctx, const dl_rtcsm_options* options, const doubl
   DL_TRY(h2d(ctx, d_pts, points, 3 * n));
   items[0].d_points = d_pts;
   items[0].d_scores = d_scores;
-  DL_TRY(run_rtcsm_batch(ctx, grid, items, plan));
+  DL_TRY(run_rtcsm_batch(ctx, items, plan));
   unsigned long long best = 0;
   DL_TRY(d2h(ctx, &best, plan.d_best, 1));
   if (all_scores) DL_TRY(d2h(ctx, all_scores, d_scores, K));
@@ -1823,6 +1827,7 @@ struct FrontendBuffers {
   uint32_t *tableA, *scratchA;
   int32_t* keepA;
   float *returns_tracking, *misses_tracking, *clouds, *current_pose, *origins, *passesA, *rtcsm_scores;
+  int32_t* rtcsm_nonpositive = nullptr;  // pre-match only (carve_prematch): per scan, a candidate scored <= 0 (CHECK_GT)
   // fused front half
   int64_t bit_words = 0;
   uint32_t* bits;              // two survivor bitmaps per scan
@@ -1883,6 +1888,11 @@ void carve_time_runs(Arena& a, const dl_frontend_options& o, int num_scans, Fron
   f->run_first_row = a.take<int32_t>(runs);
   f->run_value = a.take<float>(runs);
   if (runs > (size_t)8 * num_scans) f->run_pose = a.take<float>(runs * 8);
+}
+
+// The pre-match's per-scan flags, carved last so that every other buffer sits where it does without the pre-match.
+void carve_prematch(Arena& a, const dl_frontend_options& o, int num_scans, FrontendBuffers* f) {
+  if (o.use_online_correlative_scan_matching) f->rtcsm_nonpositive = a.take<int32_t>((size_t)num_scans);
 }
 
 FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuffers& f, const float* d_ranges,
@@ -2088,11 +2098,8 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
     }
   }
   DL_TRY(launch_fe_prepare(ctx, fa, f.batch));
-  const dl_grid* hi = submaps.high(0);
+  const float hi_resolution = submaps.high(0)->resolution;  // one for the batch (check_frontend)
   const bool rtcsm = o.use_online_correlative_scan_matching != 0;
-  if (rtcsm)
-    for (int b = 1; b < num_scans; ++b)
-      if (submaps.high(b) != hi) return ctx->fail(DL_ERR_ARG, "the correlative pre-match takes one matching grid per batch");
   int chunks = rtcsm ? 1 : (host_ranges ? 5 : 2);
   if (f.batch < 8 * chunks) chunks = std::max(1, f.batch / 8);
   // Sub-batches alternate between two equal-priority streams. Every back half (latency-bound, one or two CTAs per scan) on one
@@ -2203,13 +2210,15 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
       if (rtcsm) {
         // The angular window depends on the farthest point of each cloud through acosf, which must be the host's to stay
         // bit-exact: ONE synchronisation per batch brings back the clouds' sizes, farthest points and initial poses; the
-        // candidate tables of all scans then go up in one copy and one launch scores every (scan, rotation, translation).
-        // The best poses are written into f.initial_pose on the device, where the solve reads them.
+        // candidate tables of all scans then go up in one copy and one launch scores every (scan, rotation, translation),
+        // each scan against its own matching submap's high-resolution grid. The best poses are written into f.initial_pose on
+        // the device, where the solve reads them (the fused solve takes them as the pose part of state j's initial value);
+        // f.target keeps the prediction's translation (LTB:536).
         std::vector<int32_t> countsA(2 * f.batch);
         std::vector<double> init(7 * f.batch);
         std::vector<float> far(f.batch);
         float* d_far = a.take<float>(f.batch);
-        DL_TRY(launch_max_range_batch(ctx, f.clouds, (int64_t)2 * f.cap * 3, f.countsA, 2, f.batch, 3.f * hi->resolution, d_far));
+        DL_TRY(launch_max_range_batch(ctx, f.clouds, (int64_t)2 * f.cap * 3, f.countsA, 2, f.batch, 3.f * hi_resolution, d_far));
         DL_TRY(d2h(ctx, countsA.data(), f.countsA, 2 * f.batch));
         DL_TRY(d2h(ctx, init.data(), f.initial_pose, 7 * f.batch));
         DL_TRY(d2h(ctx, far.data(), d_far, f.batch));
@@ -2219,16 +2228,18 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
         std::vector<int32_t> slots;
         for (int b = 0; b < f.batch; ++b) {
           if (countsA[2 * b] <= 0) continue;
-          items.push_back(RtcsmBatchItem{f.clouds + (size_t)(2 * b) * f.cap * 3, countsA[2 * b], pose_from7(init.data() + 7 * b), far[b], nullptr});
+          items.push_back(RtcsmBatchItem{submaps.high(b), f.clouds + (size_t)(2 * b) * f.cap * 3, countsA[2 * b],
+                                         pose_from7(init.data() + 7 * b), far[b], nullptr, f.rtcsm_nonpositive + b});
           slots.push_back(b);
         }
         DL_CUDA(ctx, cudaMemsetAsync(f.rtcsm_scores, 0, sizeof(float) * f.batch, ctx->stream));
+        DL_CUDA(ctx, cudaMemsetAsync(f.rtcsm_nonpositive, 0, sizeof(int32_t) * f.batch, ctx->stream));
         if (!items.empty()) {
           RtcsmBatchPlan plan;
-          DL_TRY(plan_rtcsm_batch(ctx, o.real_time_correlative_scan_matcher, hi->resolution, items, &plan));
+          DL_TRY(plan_rtcsm_batch(ctx, o.real_time_correlative_scan_matcher, hi_resolution, items, &plan));
           plan.take(a);
           if (a.off > ctx->d_scratch_bytes) return ctx->fail(DL_ERR_ARG, "internal: RT-CSM scratch underestimated");
-          DL_TRY(run_rtcsm_batch(ctx, hi, items, plan));
+          DL_TRY(run_rtcsm_batch(ctx, items, plan));
           int32_t* d_slots = a.take<int32_t>(items.size());
           DL_TRY(h2d(ctx, d_slots, slots.data(), slots.size()));
           DL_TRY(launch_rtcsm_pick(ctx, plan.d_scans, (int)items.size(), f.initial_pose, d_slots, f.rtcsm_scores, d_slots));
@@ -2274,6 +2285,9 @@ int check_frontend(dl_context* ctx, const dl_frontend_options* o, int num_scans,
     if (!submaps.high(b) || !submaps.low(b)) return DL_ERR_ARG;
     if (submaps.high(b)->structure_dirty || submaps.low(b)->structure_dirty)
       return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+    // the pre-match's candidate tables and the 3 * resolution floor of the farthest point take one resolution per batch
+    if (o->use_online_correlative_scan_matching && submaps.high(b)->resolution != submaps.high(0)->resolution)
+      return ctx->fail(DL_ERR_ARG, "the correlative pre-match takes one high-resolution grid resolution per batch");
   }
   DL_TRY(check_ceres_options(ctx, &o->ceres_scan_matcher, 2));
   int64_t m = 0;
@@ -2358,6 +2372,7 @@ int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int nu
     if (imu) carve_imu(a, num_scans, imu);
     carve_time_runs(a, *options, num_scans, &f);
     if (more) (*more)(a);
+    carve_prematch(a, *options, num_scans, &f);
   }, rtcsm_extra, &rest));
   if (d_results_out) *d_results_out = d_results;
   if (buffers_out) *buffers_out = f;
@@ -2411,8 +2426,6 @@ int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options,
 static int check_imu_options(dl_context* ctx, const dl_frontend_options* options) {
   if (options && options->ceres_scan_matcher.only_optimize_yaw)
     return ctx->fail(DL_ERR_ARG, "only_optimize_yaw is not supported by the fused solve");
-  if (options && options->use_online_correlative_scan_matching)
-    return ctx->fail(DL_ERR_ARG, "the correlative pre-match is not combined with the fused solve");
   return DL_OK;
 }
 
@@ -3061,10 +3074,16 @@ int ltb_batch_device(dl_context* ctx, const dl_ltb_options& opt, bool two_stage,
   std::vector<dl_scan_result> r(P);
   std::vector<dl_nav_state> fused_states(P);
   std::vector<float> cur7(7 * (size_t)P);
+  std::vector<int32_t> nonpositive(fo.use_online_correlative_scan_matching ? P : 0, 0);
   DL_TRY(d2h(ctx, r.data(), d_results, P));
   if (!two_stage) DL_TRY(d2h(ctx, fused_states.data(), run.d_states, P));
   DL_TRY(d2h(ctx, cur7.data(), f.current_pose, 7 * (size_t)P));
+  DL_TRY(d2h(ctx, nonpositive.data(), f.rtcsm_nonpositive, nonpositive.size()));
   DL_TRY(sync(ctx));
+  // The reference CHECK-fails on a pre-match candidate whose score is not > 0 (real_time_correlative_scan_matcher_3d.cc:111).
+  // The pre-match runs before the insertion, so no grid has changed yet: the call fails and no builder is committed.
+  for (int32_t flag : nonpositive)
+    if (flag) return ctx->fail(DL_ERR_SCORE, "a correlative pre-match candidate scored <= 0 (CHECK_GT(score, 0))");
   std::vector<int> ok;  // slots whose scan was matched (scan.ok == 1)
   for (int s = 0; s < P; ++s) {
     LtbMember& m = ms[part[s]];
@@ -3245,7 +3264,7 @@ int dl_ltb_create(dl_context* ctx, const dl_ltb_options* options, dl_local_traje
     return ctx->fail(DL_ERR_ARG, "dl_ltb_options: resolutions, num_range_data or rotational_histogram_size out of range");
   DL_TRY(check_ceres_options(ctx, &options->frontend.ceres_scan_matcher, 2));
   DL_TRY(check_inserter(ctx, &options->range_data_inserter));
-  DL_TRY(check_imu_options(ctx, &options->frontend));
+  if (!options->two_stage) DL_TRY(check_imu_options(ctx, &options->frontend));  // the two-stage chain's plain solve takes only_optimize_yaw
   dl_local_trajectory_builder* b = new dl_local_trajectory_builder;
   b->ctx = ctx;
   b->opt = *options;

@@ -216,6 +216,7 @@ int launch_adaptive_voxel_filter(dl_context* ctx, const float* points, int strid
                                  int32_t* cropped_counts /* optional, batch*num_filters */);
 
 struct RtcsmScan {  // one scan of a batched correlative search (dl_rtcsm.cu), device pointers
+  GridView grid;        // the grid this scan is scored against
   const float* points;  // n x 3
   int32_t n;
   const Quatf* cand_q;  // R rotations (composed with the initial pose, normalised)
@@ -225,10 +226,10 @@ struct RtcsmScan {  // one scan of a batched correlative search (dl_rtcsm.cu), d
   int32_t R, L;
   float* scores;                     // optional, R * L
   unsigned long long* best;          // (score bits << 32) | ~index, zeroed before the launch
+  int32_t* nonpositive;              // optional, zeroed before the launch: set to 1 when a candidate's score is not > 0
 };
 int rtcsm_ctas_for(int64_t R, int64_t L);
-int launch_rtcsm_batch(dl_context* ctx, const GridView& grid, const RtcsmScan* scans_dev, const int32_t* cta_prefix_dev, int num_scans,
-                       int total_ctas);
+int launch_rtcsm_batch(dl_context* ctx, const RtcsmScan* scans_dev, const int32_t* cta_prefix_dev, int num_scans, int total_ctas);
 int launch_rtcsm_pick(dl_context* ctx, const RtcsmScan* scans_dev, int num_scans, double* pose_out, const int32_t* pose_slot,
                       float* score_out, const int32_t* score_slot);
 int launch_max_range_batch(dl_context* ctx, const float* points, int64_t stride_floats, const int32_t* counts, int count_stride,

@@ -16,7 +16,8 @@
 //   * The cloud is staged into shared memory by the TMA unit: cp.async.bulk global -> shared, completion on an mbarrier,
 //     two tiles in flight (the next tile streams in while the current one is scored). All warps of a CTA belong to one scan
 //     and share the staged tiles.
-//   * All scans of a front-end batch are scored by ONE launch: CTA -> scan through a prefix table; the argmax of each scan is
+//   * All scans of a front-end batch are scored by ONE launch: CTA -> scan through a prefix table, each scan against the grid
+//     its descriptor names (the trajectory builders' batch matches every scan against its own submap); the argmax of each scan is
 //     a packed 64-bit atomicMax (score bits << 32 | ~index: among equal scores the lowest index wins, the reference's strict
 //     '>' in emplace order), and rtcsm_pick_kernel turns it into the matcher's initial pose on the device.
 //
@@ -63,8 +64,8 @@ __device__ __forceinline__ void tma_load_bulk(void* dst_smem, const void* src_gm
                : "memory");
 }
 
-__global__ void __launch_bounds__(kBlock) rtcsm_score_kernel(GridView grid, const RtcsmScan* __restrict__ scans,
-                                                             const int32_t* __restrict__ cta_prefix, int num_scans) {
+__global__ void __launch_bounds__(kBlock) rtcsm_score_kernel(const RtcsmScan* __restrict__ scans, const int32_t* __restrict__ cta_prefix,
+                                                             int num_scans) {
   // two staged tiles (+16 B: the copy starts at the 16-byte boundary below the scan's first point)
   __shared__ __align__(128) unsigned char stage[2][kTileBytes + 32];
   __shared__ __align__(8) uint64_t full[2];
@@ -90,7 +91,7 @@ __global__ void __launch_bounds__(kBlock) rtcsm_score_kernel(GridView grid, cons
   const bool active = warp_active && l < sc.L;
   const Quatf q = sc.cand_q[r];
   const Vec3f t = active ? sc.cand_t[l] : Vec3f{0.f, 0.f, 0.f};
-  const CellDivider res = make_divider(grid.resolution);
+  const CellDivider res = make_divider(sc.grid.resolution);
 
   // tile k of the cloud = bytes [k * kTileBytes, ...) of the scan's points, fetched from the 16-byte boundary below
   const unsigned char* src = reinterpret_cast<const unsigned char*>(sc.points);
@@ -136,7 +137,7 @@ __global__ void __launch_bounds__(kBlock) rtcsm_score_kernel(GridView grid, cons
           for (int jj = 0; jj < m; ++jj) {
             const Vec3f w = add(Vec3f{my[3 * jj], my[3 * jj + 1], my[3 * jj + 2]}, t);
             const Int3 c = cell_index(w, res);
-            score += value_to_probability(grid_value(grid, c.x, c.y, c.z));
+            score += value_to_probability(grid_value(sc.grid, c.x, c.y, c.z));
           }
         }
         __syncwarp();
@@ -154,6 +155,7 @@ __global__ void __launch_bounds__(kBlock) rtcsm_score_kernel(GridView grid, cons
     const double a = sc.pen_t[l] + sc.pen_r[r];
     score = (float)((double)score * exp(-(a * a)));
     if (sc.scores) sc.scores[idx] = score;
+    if (sc.nonpositive && !(score > 0.f)) *sc.nonpositive = 1;  // where the reference's CHECK_GT(score, 0.f) aborts (cc:111)
     if (score > 0.f) packed = ((unsigned long long)__float_as_uint(score) << 32) | (0xFFFFFFFFull - (unsigned long long)idx);
   }
 #pragma unroll
@@ -204,10 +206,9 @@ int rtcsm_ctas_for(int64_t R, int64_t L) {
   return (int)((R * chunks + kWarps - 1) / kWarps);
 }
 
-int launch_rtcsm_batch(dl_context* ctx, const GridView& grid, const RtcsmScan* scans_dev, const int32_t* cta_prefix_dev, int num_scans,
-                       int total_ctas) {
+int launch_rtcsm_batch(dl_context* ctx, const RtcsmScan* scans_dev, const int32_t* cta_prefix_dev, int num_scans, int total_ctas) {
   if (num_scans <= 0 || total_ctas <= 0) return DL_OK;
-  rtcsm_score_kernel<<<total_ctas, kBlock, 0, ctx->stream>>>(grid, scans_dev, cta_prefix_dev, num_scans);
+  rtcsm_score_kernel<<<total_ctas, kBlock, 0, ctx->stream>>>(scans_dev, cta_prefix_dev, num_scans);
   DL_LAUNCH_CHECK(ctx, "rtcsm_score_kernel");
   return DL_OK;
 }

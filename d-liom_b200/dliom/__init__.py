@@ -301,6 +301,13 @@ class LtbOptions(C.Structure):   # dl_ltb_options
         o.rotational_histogram_size = kw.pop("rotational_histogram_size", 120)
         o.frames_for_static_initialization = kw.pop("frames_for_static_initialization", 7)
         o.two_stage = int(kw.pop("two_stage", 0))
+        # the correlative pre-match (LTB:514-521) and the yaw-only solve, over what `frontend` carries
+        if "use_rtcsm" in kw:
+            o.frontend.use_online_correlative_scan_matching = int(kw.pop("use_rtcsm"))
+        if "rtcsm" in kw:   # (linear_search_window, angular_search_window, translation / rotation_delta_cost_weight)
+            o.frontend.real_time_correlative_scan_matcher = RtcsmOptions(*[float(v) for v in kw.pop("rtcsm")])
+        if "only_optimize_yaw" in kw:
+            o.frontend.ceres_scan_matcher.only_optimize_yaw = int(kw.pop("only_optimize_yaw"))
         o.ceres_pose_noise_t, o.ceres_pose_noise_r = kw.pop("ceres_pose_noise_t", 1e-2), kw.pop("ceres_pose_noise_r", 1e-2)
         o.prior_pose_noise = kw.pop("prior_pose_noise", 1e-2)
         o.prior_velocity_noise, o.prior_bias_noise = kw.pop("prior_velocity_noise", 1e4), kw.pop("prior_bias_noise", 1e-2)
@@ -313,6 +320,11 @@ class MatchingResult(C.Structure):   # dl_matching_result
                 ("state", NavState), ("scan", ScanResult), ("origin_in_local", C.c_float * 3), ("num_returns", C.c_int32),
                 ("num_misses", C.c_int32), ("num_high_resolution", C.c_int32), ("num_low_resolution", C.c_int32),
                 ("num_insertion_submaps", C.c_int32), ("insertion_submap_index", C.c_int32 * 2), ("reserved", C.c_int32)]
+
+    @property
+    def rtcsm_score(self):
+        """The correlative pre-match's best score (0 when use_online_correlative_scan_matching is off)."""
+        return self.scan.rtcsm_score
 
 
 class LtbBatchItem(C.Structure):   # dl_ltb_batch_item

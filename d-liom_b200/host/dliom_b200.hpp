@@ -477,6 +477,8 @@ struct LocalTrajectoryBuilderOptions3D {  // proto::LocalTrajectoryBuilderOption
     f.high_resolution_adaptive_voxel_filter = {2.f, 150.f, 15.f};
     f.low_resolution_adaptive_voxel_filter = {4.f, 200.f, 60.f};
     f.scan_period = 0.1;
+    f.use_online_correlative_scan_matching = 0;  // 1: the correlative pre-match seeds the solve (LTB:514-521)
+    f.real_time_correlative_scan_matcher = {0.15, 3.14159265358979323846 / 180., 1e-1, 1e-1};
     f.ceres_scan_matcher.num_occupied_space_weights = 2;
     f.ceres_scan_matcher.occupied_space_weight[0] = 1.; f.ceres_scan_matcher.occupied_space_weight[1] = 6.;
     f.ceres_scan_matcher.translation_weight = 5.; f.ceres_scan_matcher.rotation_weight = 4e2;
@@ -511,6 +513,7 @@ class LocalTrajectoryBuilder3D {  // local_trajectory_builder_3d.h:81-113
     Rigid3d local_pose;
     sensor::RangeData range_data_in_local;
     std::unique_ptr<const InsertionResult> insertion_result;  // nullptr if dropped by the motion filter
+    float rtcsm_score = 0.f;  // the correlative pre-match's score (kRealTimeCorrelativeScanMatcherScoreMetric); 0 when it is off
   };
   LocalTrajectoryBuilder3D(Context* ctx, const LocalTrajectoryBuilderOptions3D& options,
                            const std::vector<std::string>& expected_range_sensor_ids)
@@ -586,6 +589,7 @@ class LocalTrajectoryBuilder3D {  // local_trajectory_builder_3d.h:81-113
     std::unique_ptr<MatchingResult> out(new MatchingResult);
     out->time = r.time;
     out->local_pose = Rigid3d::from7(r.local_pose);
+    out->rtcsm_score = r.scan.rtcsm_score;
     out->range_data_in_local.origin = {r.origin_in_local[0], r.origin_in_local[1], r.origin_in_local[2]};
     out->range_data_in_local.returns = Cloud(0);
     out->range_data_in_local.misses = Cloud(1);

@@ -722,7 +722,11 @@ int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options,
  * the plain call takes as predicted_poses; prev_poses[k] is states_i[k]'s pose) and the initial velocity and biases.
  * states_out[k] receives the estimated state of scan k (local frame); results[k] as in the plain call, with the pose part
  * of the state. preintegrations[k] may be linearised at other biases than states_i[k]'s (bias correction as in
- * dl_fused_match_batch). An EXTENSION like dl_fused_match_batch: the reference chains the plain match and a GTSAM update. */
+ * dl_fused_match_batch). An EXTENSION like dl_fused_match_batch: the reference chains the plain match and a GTSAM update.
+ * With use_online_correlative_scan_matching the correlative pre-match runs first (LTB:514-521) and its pose replaces the
+ * pose part of state j's initial value; velocity and biases stay the prediction's, and the translation target of the
+ * solve stays the prediction's translation (LTB:536). Combining the pre-match with the fused solve is part of the same
+ * extension. This and every fused entry below refuse only_optimize_yaw (DL_ERR_ARG). */
 typedef struct dl_frontend_imu {
   double imu_weight;
   double gravity[3];
@@ -828,7 +832,10 @@ typedef struct dl_ltb_options { /* proto::LocalTrajectoryBuilderOptions3D, the f
   int32_t frames_for_static_initialization;        /* 7 in the reference (LTB:376) */
   /* 0: the fused solve (scan match + IMU residual in one problem) gives the node's state. 1: the reference's TWO-STAGE chain —
    * plain CeresScanMatcher3D::Match from the IMU-predicted pose (LTB:535-542), then the window update with that pose as a prior
-   * (dl_window_optimize_batch; LTB:555, :693-863); the carried information starts from the reference's priors (LTB:84-90). */
+   * (dl_window_optimize_batch; LTB:555, :693-863); the carried information starts from the reference's priors (LTB:84-90).
+   * Both modes take frontend.use_online_correlative_scan_matching: the correlative pre-match (LTB:514-521) then seeds the
+   * solve from its pose, the translation target staying the prediction's (LTB:536). frontend.ceres_scan_matcher
+   * .only_optimize_yaw is taken by the two-stage chain's plain solve; dl_ltb_create refuses it for the fused solve. */
   int32_t two_stage;
   int32_t reserved;
   double ceres_pose_noise_t, ceres_pose_noise_r;   /* imu_options: sigmas of the matched pose in the window */
@@ -874,8 +881,11 @@ int dl_ltb_add_synchronized_range_data(dl_local_trajectory_builder* builder, dou
  * memory, a cloud the rotational histogram refuses — the latter is detected before any grid changes) commits no builder's host
  * state, but after a failure inside the insertion the grids of the members' active submaps may already hold their scans: do not
  * feed such a builder the same scan again. dl_ltb_add_range_data and dl_ltb_add_synchronized_range_data are the batch of one.
- * The correlative pre-match (use_online_correlative_scan_matching) is not part of this path: dl_ltb_create refuses it, as the
- * fused solve does, and the front end refuses a correlative batch whose scans match different grids. */
+ * With use_online_correlative_scan_matching every member's scan is pre-matched against its own matching submap's
+ * high-resolution grid in the batch's one scoring launch (a fixed number of extra host waits per call); dl_matching_result.scan.rtcsm_score
+ * carries the score (0 when the pre-match is off). Where the reference CHECK-fails on a candidate whose score is not > 0
+ * (real_time_correlative_scan_matcher_3d.cc:111), the call fails with DL_ERR_SCORE before any grid changes and commits no
+ * builder. */
 typedef struct dl_ltb_batch_item {
   dl_local_trajectory_builder* builder;
   double time;
