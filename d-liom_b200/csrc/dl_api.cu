@@ -18,29 +18,12 @@ using namespace dl;
 // ------------------------------------------------------------------------------------------------ context
 int dl_context::reserve_device(size_t bytes) {
   if (in_flight) return fail(DL_ERR_ARG, "a submitted batch is in flight on this context: call dl_frontend_collect first");
-  if (bytes <= d_scratch_bytes) return DL_OK;
-  if (d_scratch) {
-    DL_CUDA(this, cudaStreamSynchronize(stream));
-    DL_CUDA(this, cudaFree(d_scratch));
-    d_scratch = nullptr;
-    d_scratch_bytes = 0;
-  }
-  const size_t want = bytes + bytes / 4;
-  DL_CUDA(this, cudaMalloc(&d_scratch, want));
-  d_scratch_bytes = want;
-  return DL_OK;
+  if (bytes <= d_scratch.cap) return DL_OK;
+  return grow(this, d_scratch, bytes + bytes / 4);
 }
 int dl_context::reserve_pinned(size_t bytes) {
-  if (bytes <= h_pinned_bytes) return DL_OK;
-  if (h_pinned) {
-    DL_CUDA(this, cudaStreamSynchronize(stream));
-    DL_CUDA(this, cudaFreeHost(h_pinned));
-    h_pinned = nullptr;
-    h_pinned_bytes = 0;
-  }
-  DL_CUDA(this, cudaMallocHost(&h_pinned, bytes + bytes / 4));
-  h_pinned_bytes = bytes + bytes / 4;
-  return DL_OK;
+  if (bytes <= h_pinned.cap) return DL_OK;
+  return grow(this, h_pinned, bytes + bytes / 4);
 }
 
 int dl_context::stage_id(const char* name) {
@@ -71,45 +54,6 @@ int64_t next_pow2(int64_t v) {
   return p;
 }
 
-#define DL_TRY(expr)            \
-  do {                          \
-    const int st__ = (expr);    \
-    if (st__ != DL_OK) return st__; \
-  } while (0)
-
-template <typename T>
-int h2d(dl_context* ctx, T* dst, const T* src, size_t count) {
-  if (count == 0) return DL_OK;
-  DL_CUDA(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  return DL_OK;
-}
-// (Re)allocates a pool to at least `need` elements, preserving the first `used` elements and initialising the rest
-// with `fill` bytes: free node slots must read -1 and free brick slots 0 for the lock-free device-side growth.
-template <typename T>
-int realloc_pool(dl_context* ctx, T** ptr, size_t* cap, size_t need, size_t used, int fill) {
-  if (need <= *cap) return DL_OK;
-  const size_t want = need + need / 4 + 16 * 512;  // exact need + 25 % headroom (the callers count what they add)
-  T* fresh = nullptr;
-  DL_CUDA(ctx, cudaMalloc((void**)&fresh, want * sizeof(T)));
-  DL_CUDA(ctx, cudaMemsetAsync(fresh, fill, want * sizeof(T), ctx->stream));
-  if (*ptr && used) DL_CUDA(ctx, cudaMemcpyAsync(fresh, *ptr, used * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (*ptr) DL_CUDA(ctx, cudaFree(*ptr));
-  *ptr = fresh;
-  *cap = want;
-  return DL_OK;
-}
-
-template <typename T>
-int d2h(dl_context* ctx, T* dst, const T* src, size_t count) {
-  if (count == 0) return DL_OK;
-  DL_CUDA(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
-  return DL_OK;
-}
-int sync(dl_context* ctx) {
-  DL_CUDA(ctx, ctx->wait_stream());
-  return DL_OK;
-}
 }  // namespace
 
 extern "C" {
@@ -151,18 +95,15 @@ int dl_context_create(int device_ordinal, dl_context** out) {
 void dl_context_destroy(dl_context* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
-  if (ctx->stream) cudaStreamSynchronize(ctx->stream);
+  if (ctx->stream) ctx->wait_stream();
   for (const dl_context::Mark& m : ctx->marks) { cudaEventDestroy(m.begin); cudaEventDestroy(m.end); }
   for (cudaEvent_t e : ctx->event_pool) cudaEventDestroy(e);
-  if (ctx->d_scratch) cudaFree(ctx->d_scratch);
-  if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
   if (ctx->aux_stream) cudaStreamDestroy(ctx->aux_stream);
   if (ctx->tail_stream) cudaStreamDestroy(ctx->tail_stream);
   if (ctx->batch_done) cudaEventDestroy(ctx->batch_done);
   if (ctx->sync_event) cudaEventDestroy(ctx->sync_event);
-  if (ctx->d_fcsm_lut) cudaFree(ctx->d_fcsm_lut);
   if (ctx->staging_done) cudaEventDestroy(ctx->staging_done);
   delete ctx;
 }
@@ -198,7 +139,7 @@ int dl_context_set_profiling(dl_context* ctx, int enabled) {
 }
 int dl_context_read_profile(dl_context* ctx, dl_stage_time* out, int32_t capacity, int32_t* num_stages) {
   if (!ctx || !num_stages || capacity < 0 || (capacity > 0 && !out)) return DL_ERR_ARG;
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
   for (const dl_context::Mark& m : ctx->marks) {
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, m.begin, m.end) == cudaSuccess) {
@@ -260,12 +201,7 @@ int dl_grid_create(dl_context* ctx, float resolution, dl_grid** out) {
 void dl_grid_destroy(dl_grid* g) {
   if (!g) return;
   cudaSetDevice(g->ctx->device);
-  cudaStreamSynchronize(g->ctx->stream);
-  cudaFree(g->d_m8);
-  cudaFree(g->d_top);
-  cudaFree(g->d_nodes);
-  cudaFree(g->d_bricks);
-  cudaFree(g->d_counters);
+  g->ctx->wait_stream();
   delete g;
 }
 
@@ -276,8 +212,8 @@ int64_t dl_grid_num_bricks(const dl_grid* g) {
   if (!g->mirror_stale) return (int64_t)(g->bricks.size() / 512);
   int32_t used = 0;
   if (cudaSetDevice(g->ctx->device) != cudaSuccess ||
-      cudaMemcpyAsync(&used, g->d_counters + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, g->ctx->stream) != cudaSuccess ||
-      cudaStreamSynchronize(g->ctx->stream) != cudaSuccess)
+      cudaMemcpyAsync(&used, g->d_counters.get() + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, g->ctx->stream) != cudaSuccess ||
+      g->ctx->wait_stream() != cudaSuccess)
     return -1;
   return used;
 }
@@ -342,15 +278,15 @@ static int grid_download(dl_grid* g) {
   if (!g->mirror_stale) return DL_OK;
   dl_context* ctx = g->ctx;
   int32_t counters[2] = {0, 0};
-  DL_TRY(d2h(ctx, counters, g->d_counters, 2));
+  DL_TRY(d2h(ctx, counters, g->d_counters.get(), 2));
   DL_TRY(sync(ctx));
   g->top.resize((size_t)1 << (3 * g->bits));
   g->nodes.resize((size_t)counters[0] * 512);
   g->bricks.resize((size_t)counters[1] * 512);
   g->brick_dirty.assign(counters[1], 0);
-  DL_TRY(d2h(ctx, g->top.data(), g->d_top, g->top.size()));
-  DL_TRY(d2h(ctx, g->nodes.data(), g->d_nodes, g->nodes.size()));
-  DL_TRY(d2h(ctx, g->bricks.data(), g->d_bricks, g->bricks.size()));
+  DL_TRY(d2h(ctx, g->top.data(), g->d_top.get(), g->top.size()));
+  DL_TRY(d2h(ctx, g->nodes.data(), g->d_nodes.get(), g->nodes.size()));
+  DL_TRY(d2h(ctx, g->bricks.data(), g->d_bricks.get(), g->bricks.size()));
   DL_TRY(sync(ctx));
   g->mirror_stale = false;
   g->structure_dirty = false;
@@ -364,20 +300,15 @@ int dl_grid_sync(dl_grid* g) {
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
   if (g->mirror_stale) return ctx->fail(DL_ERR_ARG, "internal: host mirror is behind the device grid");
   const size_t nbricks = g->bricks.size() / 512;
-  if (!g->d_counters) DL_CUDA(ctx, cudaMalloc((void**)&g->d_counters, 8 * sizeof(int32_t)));
+  if (!g->d_counters.get()) DL_TRY(alloc(ctx, g->d_counters, 8));
   if (g->structure_dirty) {
-    if (g->top.size() > g->d_top_cap) {
-      if (g->d_top) { DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); DL_CUDA(ctx, cudaFree(g->d_top)); }
-      g->d_top = nullptr;
-      DL_CUDA(ctx, cudaMalloc((void**)&g->d_top, g->top.size() * sizeof(int32_t)));
-      g->d_top_cap = g->top.size();
-    }
-    DL_TRY(realloc_pool(ctx, &g->d_nodes, &g->d_nodes_cap, std::max<size_t>(g->nodes.size(), 512), 0, 0xFF));
-    const size_t old_cap = g->d_bricks_cap;
-    DL_TRY(realloc_pool(ctx, &g->d_bricks, &g->d_bricks_cap, std::max<size_t>(g->bricks.size(), 512), 0, 0));
-    if (g->d_bricks_cap != old_cap) std::fill(g->brick_dirty.begin(), g->brick_dirty.end(), 1);  // reallocated
-    DL_TRY(h2d(ctx, g->d_top, g->top.data(), g->top.size()));
-    DL_TRY(h2d(ctx, g->d_nodes, g->nodes.data(), g->nodes.size()));
+    if (g->top.size() > g->d_top.cap) DL_TRY(grow(ctx, g->d_top, g->top.size()));
+    DL_TRY(grid_grow_pool(g, 0, 0, std::max<size_t>(g->nodes.size() / 512, 1)));
+    const size_t old_cap = g->d_bricks.cap;
+    DL_TRY(grid_grow_pool(g, 1, 0, std::max<size_t>(nbricks, 1)));
+    if (g->d_bricks.cap != old_cap) std::fill(g->brick_dirty.begin(), g->brick_dirty.end(), 1);  // reallocated
+    DL_TRY(h2d(ctx, g->d_top.get(), g->top.data(), g->top.size()));
+    DL_TRY(h2d(ctx, g->d_nodes.get(), g->nodes.data(), g->nodes.size()));
     g->structure_dirty = false;
   }
   // upload dirty bricks, coalescing runs of consecutive dirty bricks into one copy
@@ -386,11 +317,11 @@ int dl_grid_sync(dl_grid* g) {
     if (!g->brick_dirty[b]) { ++b; continue; }
     size_t e = b;
     while (e < nbricks && g->brick_dirty[e]) g->brick_dirty[e++] = 0;
-    DL_TRY(h2d(ctx, g->d_bricks + b * 512, g->bricks.data() + b * 512, (e - b) * 512));
+    DL_TRY(h2d(ctx, g->d_bricks.get() + b * 512, g->bricks.data() + b * 512, (e - b) * 512));
     b = e;
   }
   const int32_t counters[8] = {(int32_t)(g->nodes.size() / 512), (int32_t)nbricks, 0, 0, 0, 0, 0, 0};
-  DL_TRY(h2d(ctx, g->d_counters, counters, 8));
+  DL_TRY(h2d(ctx, g->d_counters.get(), counters, 8));
   return sync(ctx);
 }
 
@@ -431,16 +362,19 @@ int dl_grid_interpolate(dl_context* ctx, const dl_grid* g, int64_t n, const doub
 namespace dl {
 int grid_ensure_device_state(dl_grid* g) {
   if (g->mirror_stale) return DL_OK;  // the device copy is authoritative and complete
-  bool dirty = g->structure_dirty || !g->d_counters;
+  bool dirty = g->structure_dirty || !g->d_counters.get();
   for (size_t b = 0; b < g->brick_dirty.size() && !dirty; ++b) dirty = g->brick_dirty[b] != 0;
   return dirty ? dl_grid_sync(g) : DL_OK;
 }
 // Grows the node pool (level 0) or the brick pool (level 1) from `used` entries in use by `add` more (dl_inserter.cu counts
-// them exactly: the entries the running Insert marked).
+// them exactly: the entries the running Insert marked), to the exact need + 25 % headroom, keeping the entries in use. Free
+// node slots must read -1 and free brick slots 0 for the lock-free device-side growth.
 int grid_grow_pool(dl_grid* g, int level, size_t used, size_t add) {
-  dl_context* ctx = g->ctx;
-  if (level == 0) return realloc_pool(ctx, &g->d_nodes, &g->d_nodes_cap, (used + add) * 512, used * 512, 0xFF);
-  return realloc_pool(ctx, &g->d_bricks, &g->d_bricks_cap, (used + add) * 512, used * 512, 0);
+  const size_t need = (used + add) * 512;
+  auto grow_pool = [&](auto& pool, int fill) {
+    return need <= pool.cap ? DL_OK : grow(g->ctx, pool, need + need / 4 + 16 * 512, used * 512, fill);
+  };
+  return level == 0 ? grow_pool(g->d_nodes, 0xFF) : grow_pool(g->d_bricks, 0);
 }
 }  // namespace dl
 
@@ -1054,7 +988,7 @@ int check_fcsm_options(dl_context* ctx, const dl_fcsm_options& o) {
 int ensure_search_index(dl_context* ctx, dl_grid* g, bool* have) {
   std::lock_guard<std::mutex> lock(g->index_mutex);  // grids are shared read-only between contexts: build once
   *have = false;
-  if (g->m8_version == g->version && g->d_m8) {
+  if (g->m8_version == g->version && g->d_m8.get()) {
     *have = true;
     return DL_OK;
   }
@@ -1082,19 +1016,11 @@ int ensure_search_index(dl_context* ctx, dl_grid* g, bool* have) {
   const size_t bytes = (size_t)dim[0] * dim[1] * dim[2];
   if (bytes > ((size_t)3 << 30)) return DL_OK;    // > 3 GiB per submap: stay exhaustive
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (g->d_m8_bytes < bytes) {
-    DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (g->d_m8) DL_CUDA(ctx, cudaFree(g->d_m8));
-    g->d_m8 = nullptr;
-    g->d_m8_bytes = 0;
-    DL_CUDA(ctx, cudaMalloc(&g->d_m8, bytes));
-    g->d_m8_bytes = bytes;
-  }
-  uint8_t* tmp = nullptr;
-  DL_CUDA(ctx, cudaMalloc(&tmp, bytes));
-  const int st = launch_fcsm_index(ctx, g->view(), org[0], org[1], org[2], dim[0], dim[1], dim[2], tmp, g->d_m8);
-  cudaStreamSynchronize(ctx->stream);
-  cudaFree(tmp);
+  if (g->d_m8.cap < bytes) DL_TRY(grow(ctx, g->d_m8, bytes));
+  DeviceBuffer<uint8_t> tmp;
+  DL_TRY(alloc(ctx, tmp, bytes));
+  const int st = launch_fcsm_index(ctx, g->view(), org[0], org[1], org[2], dim[0], dim[1], dim[2], tmp.get(), g->d_m8.get());
+  ctx->wait_stream();  // tmp is freed on return
   DL_TRY(st);
   for (int a = 0; a < 3; ++a) { g->m8_org[a] = org[a]; g->m8_dim[a] = dim[a]; }
   g->m8_version = g->version;
@@ -1189,7 +1115,7 @@ int coarse_search(dl_context* ctx, const dl_fcsm_options& o, float min_score, in
     p.min_score = min_score;
     p.min_low = o.min_low_resolution_score;
     if (out->pruned) {
-      p.m8 = hi_grids[g]->d_m8;
+      p.m8 = hi_grids[g]->d_m8.get();
       for (int a3 = 0; a3 < 3; ++a3) { p.m8_org[a3] = hi_grids[g]->m8_org[a3]; p.m8_dim[a3] = hi_grids[g]->m8_dim[a3]; }
     }
     const long long side = 2ll * p.wxy + 1;
@@ -1959,7 +1885,7 @@ int frontend_upload_small(dl_context* ctx, const dl_frontend_options& o, const F
   carve_staging(count, f.batch, num_origins, &s);
   DL_TRY(ctx->reserve_pinned(count.off));
   DL_CUDA(ctx, cudaEventSynchronize(ctx->staging_done));
-  Arena h(ctx->h_pinned);
+  Arena h(ctx->h_pinned.get());
   carve_staging(h, f.batch, num_origins, &s);
   for (int b = 0; b < f.batch; ++b) {
     s.counts[b] = (int32_t)sizes[b];
@@ -2238,7 +2164,7 @@ int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, f
           RtcsmBatchPlan plan;
           DL_TRY(plan_rtcsm_batch(ctx, o.real_time_correlative_scan_matcher, hi_resolution, items, &plan));
           plan.take(a);
-          if (a.off > ctx->d_scratch_bytes) return ctx->fail(DL_ERR_ARG, "internal: RT-CSM scratch underestimated");
+          if (a.off > ctx->d_scratch.cap) return ctx->fail(DL_ERR_ARG, "internal: RT-CSM scratch underestimated");
           DL_TRY(run_rtcsm_batch(ctx, items, plan));
           int32_t* d_slots = a.take<int32_t>(items.size());
           DL_TRY(h2d(ctx, d_slots, slots.data(), slots.size()));
@@ -2510,7 +2436,7 @@ int dl_frontend_match_batch_imu_samples_dev(dl_context* ctx, const dl_frontend_o
 static int submit_finish(dl_context* ctx, int num_scans, int num_origins, const dl_scan_result* d_results,
                          const dl_nav_state* d_states) {
   Staging s;
-  Arena h(ctx->h_pinned);  // the block frontend_upload_small reserved for this batch
+  Arena h(ctx->h_pinned.get());  // the block frontend_upload_small reserved for this batch
   carve_staging(h, num_scans, num_origins, &s);
   DL_CUDA(ctx, cudaMemcpyAsync(s.results, d_results, (size_t)num_scans * sizeof(dl_scan_result), cudaMemcpyDeviceToHost,
                                ctx->stream));

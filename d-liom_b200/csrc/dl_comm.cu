@@ -78,30 +78,21 @@ struct dl_comm {
   dl_context* ctx = nullptr;
   ncclComm_t comm = nullptr;
   int rank = 0, world = 1;
-  void* d_send = nullptr;   // staging for the constraint exchange: `cap` bytes
-  void* d_recv = nullptr;   // world * cap bytes
-  size_t cap = 0;
+  dl::DeviceBuffer<uint8_t> d_send;   // staging for the constraint exchange
+  dl::DeviceBuffer<uint8_t> d_recv;   // world times d_send's bytes
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 
 namespace dl {
 
 int comm_reserve(dl_comm* c, size_t bytes_per_rank) {
-  if (bytes_per_rank <= c->cap) return DL_OK;
-  dl_context* ctx = c->ctx;
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (c->d_send) cudaFree(c->d_send);
-  if (c->d_recv) cudaFree(c->d_recv);
-  c->d_send = c->d_recv = nullptr;
-  c->cap = 0;
+  if (bytes_per_rank <= c->d_send.cap && bytes_per_rank * c->world <= c->d_recv.cap) return DL_OK;
   const size_t want = bytes_per_rank + bytes_per_rank / 2 + 1024;
-  DL_CUDA(ctx, cudaMalloc(&c->d_send, want));
-  DL_CUDA(ctx, cudaMalloc(&c->d_recv, want * (size_t)c->world));
-  c->cap = want;
-  return DL_OK;
+  DL_TRY(grow(c->ctx, c->d_recv, want * (size_t)c->world));
+  return grow(c->ctx, c->d_send, want);
 }
-void* comm_send_buffer(dl_comm* c) { return c->d_send; }
-void* comm_recv_buffer(dl_comm* c) { return c->d_recv; }
+void* comm_send_buffer(dl_comm* c) { return c->d_send.get(); }
+void* comm_recv_buffer(dl_comm* c) { return c->d_recv.get(); }
 
 // recv[r * bytes .. (r+1) * bytes) = rank r's send[0 .. bytes); device-timed with events on the context's stream.
 int comm_all_gather(dl_comm* c, const void* send_dev, void* recv_dev, size_t bytes, float* ms) {
@@ -163,10 +154,8 @@ int dl_comm_create(dl_context* ctx, const uint8_t* id128, int32_t rank, int32_t 
 void dl_comm_destroy(dl_comm* c) {
   if (!c) return;
   cudaSetDevice(c->ctx->device);
-  cudaStreamSynchronize(c->ctx->stream);
+  c->ctx->wait_stream();
   if (c->comm) nccl_api()->CommDestroy(c->comm);
-  if (c->d_send) cudaFree(c->d_send);
-  if (c->d_recv) cudaFree(c->d_recv);
   if (c->e0) cudaEventDestroy(c->e0);
   if (c->e1) cudaEventDestroy(c->e1);
   delete c;

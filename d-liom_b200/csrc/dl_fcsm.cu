@@ -475,9 +475,9 @@ __global__ void __launch_bounds__(128) fcsm_finish_kernel(const FcsmPair* __rest
 }  // namespace
 
 int ensure_fcsm_lut(dl_context* ctx) {
-  if (!ctx->d_fcsm_lut) {
-    DL_CUDA(ctx, cudaMalloc(&ctx->d_fcsm_lut, kLutSize));
-    fcsm_lut_kernel<<<kLutSize / 256, 256, 0, ctx->stream>>>(ctx->d_fcsm_lut);
+  if (!ctx->d_fcsm_lut.get()) {
+    DL_TRY(alloc(ctx, ctx->d_fcsm_lut, kLutSize));
+    fcsm_lut_kernel<<<kLutSize / 256, 256, 0, ctx->stream>>>(ctx->d_fcsm_lut.get());
     DL_LAUNCH_CHECK(ctx, "fcsm_lut_kernel");
   }
   return DL_OK;
@@ -486,9 +486,9 @@ int ensure_fcsm_lut(dl_context* ctx) {
 // Dense sliding-maximum volume of one grid: out has nx * ny * nz bytes, element (0, 0, 0) = cell (ox, oy, oz); tmp same size.
 // nx is a multiple of 8 and (ox + grid_size / 2) % 8 == 0.
 int launch_fcsm_index(dl_context* ctx, const GridView& g, int ox, int oy, int oz, int nx, int ny, int nz, uint8_t* tmp, uint8_t* out) {
-  DL_TRY_STATUS(ensure_fcsm_lut(ctx));
+  DL_TRY(ensure_fcsm_lut(ctx));
   const long long total = (long long)nx * ny * nz, runs = total / 8;
-  m8_pass_x_kernel<<<(unsigned)((runs + 255) / 256), 256, 0, ctx->stream>>>(g, ctx->d_fcsm_lut, ox, oy, oz, nx, ny, nz, out);
+  m8_pass_x_kernel<<<(unsigned)((runs + 255) / 256), 256, 0, ctx->stream>>>(g, ctx->d_fcsm_lut.get(), ox, oy, oz, nx, ny, nz, out);
   DL_LAUNCH_CHECK(ctx, "m8_pass_x_kernel");
   m8_pass_axis_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(out, tmp, total, nx, nx, ny);
   DL_LAUNCH_CHECK(ctx, "m8_pass_axis_kernel(y)");
@@ -500,7 +500,7 @@ int launch_fcsm_index(dl_context* ctx, const GridView& g, int ox, int oy, int oz
 // Pruned search: bounds of every 8^3 block, then two rounds of block evaluation. bounds_dev: count * stride ints.
 int launch_fcsm_pruned(dl_context* ctx, const FcsmPair* pairs_dev, int count, int max_points, int max_blocks, int* bounds_dev,
                        int* max_bound_dev, unsigned long long* best_dev, FcsmPick* picks_dev) {
-  DL_TRY_STATUS(ensure_fcsm_lut(ctx));
+  DL_TRY(ensure_fcsm_lut(ctx));
   DL_CUDA(ctx, cudaMemsetAsync(best_dev, 0, sizeof(unsigned long long) * count, ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(max_bound_dev, 0, sizeof(int) * count, ctx->stream));
   fcsm_prepare_kernel<<<dim3((max_points + 255) / 256, count), 256, 0, ctx->stream>>>(pairs_dev);
@@ -509,7 +509,7 @@ int launch_fcsm_pruned(dl_context* ctx, const FcsmPair* pairs_dev, int count, in
   DL_LAUNCH_CHECK(ctx, "fcsm_bounds_kernel");
   for (int round = 0; round < 2; ++round) {
     fcsm_block_kernel<<<dim3(max_blocks, count), 64 * kPointGroups, 0, ctx->stream>>>(pairs_dev, bounds_dev, max_blocks, max_bound_dev, best_dev,
-                                                                       ctx->d_fcsm_lut, round);
+                                                                       ctx->d_fcsm_lut.get(), round);
     DL_LAUNCH_CHECK(ctx, "fcsm_block_kernel");
   }
   fcsm_finish_kernel<<<count, 128, 0, ctx->stream>>>(pairs_dev, best_dev, count, picks_dev);
@@ -551,12 +551,12 @@ int launch_pack_constraint_rows(dl_context* ctx, int n, const FcsmPick* picks, c
 
 int launch_fcsm(dl_context* ctx, const FcsmPair* pairs_dev, int count, int max_points, long long max_threads,
                 unsigned long long* best_dev, FcsmPick* picks_dev, float* all_scores_dev) {
-  DL_TRY_STATUS(ensure_fcsm_lut(ctx));
+  DL_TRY(ensure_fcsm_lut(ctx));
   DL_CUDA(ctx, cudaMemsetAsync(best_dev, 0, sizeof(unsigned long long) * count, ctx->stream));
   fcsm_prepare_kernel<<<dim3((max_points + 255) / 256, count), 256, 0, ctx->stream>>>(pairs_dev);
   DL_LAUNCH_CHECK(ctx, "fcsm_prepare_kernel");
   fcsm_search_kernel<<<dim3((unsigned)((max_threads + kBlock - 1) / kBlock), count), kBlock, 0, ctx->stream>>>(pairs_dev, best_dev,
-                                                                                                           all_scores_dev, ctx->d_fcsm_lut);
+                                                                                                           all_scores_dev, ctx->d_fcsm_lut.get());
   DL_LAUNCH_CHECK(ctx, "fcsm_search_kernel");
   fcsm_finish_kernel<<<count, 128, 0, ctx->stream>>>(pairs_dev, best_dev, count, picks_dev);
   DL_LAUNCH_CHECK(ctx, "fcsm_finish_kernel");

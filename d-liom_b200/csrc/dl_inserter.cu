@@ -277,9 +277,6 @@ void compute_odds_table(float probability, uint16_t* table) {
   }
 }
 
-int grid_ensure_device_state(dl_grid* g);
-int grid_grow_pool(dl_grid* g, int level, size_t used, size_t add);
-
 size_t insert_args_bytes(int jobs) { return sizeof(InsertArgs) * (size_t)jobs; }
 
 namespace {
@@ -289,16 +286,16 @@ namespace {
 // (8 ints per job) and read back in one copy: one host wait for all grids.
 int reserve_pools(dl_context* ctx, std::vector<InsertArgs>& args, const std::vector<dl_grid*>& grids, int level, int32_t* d_gather) {
   for (size_t j = 0; j < grids.size(); ++j)
-    DL_CUDA(ctx, cudaMemcpyAsync(d_gather + 8 * j, grids[j]->d_counters, 5 * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(d_gather + 8 * j, grids[j]->d_counters.get(), 5 * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
   std::vector<int32_t> counters(8 * grids.size());
   DL_CUDA(ctx, cudaMemcpyAsync(counters.data(), d_gather, counters.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   DL_CUDA(ctx, ctx->wait_stream());
   for (size_t j = 0; j < grids.size(); ++j) {
     dl_grid* g = grids[j];
     const int32_t* c = counters.data() + 8 * j;
-    DL_TRY_STATUS(grid_grow_pool(g, level, (size_t)c[level], (size_t)c[3 + level]));
-    if (level == 0) args[j].nodes = g->d_nodes;
-    else args[j].bricks = g->d_bricks;
+    DL_TRY(grid_grow_pool(g, level, (size_t)c[level], (size_t)c[3 + level]));
+    if (level == 0) args[j].nodes = g->d_nodes.get();
+    else args[j].bricks = g->d_bricks.get();
   }
   return DL_OK;
 }
@@ -325,16 +322,13 @@ int insert_round(dl_context* ctx, std::vector<InsertArgs> args, const std::vecto
       if (fits) break;
       if (g->bits + 1 > 8) return ctx->fail(DL_ERR_GRID_RANGE, "cell index outside +-8192 cells");
       const size_t new_size = (size_t)8 << (3 * g->bits);
-      int32_t* grown = nullptr;
-      DL_CUDA(ctx, cudaMalloc((void**)&grown, new_size * sizeof(int32_t)));
-      DL_CUDA(ctx, cudaMemsetAsync(grown, 0xFF, new_size * sizeof(int32_t), ctx->stream));
+      DeviceBuffer<int32_t> grown;
+      DL_TRY(alloc(ctx, grown, new_size, 0xFF));
       const int old_cells = 1 << (3 * g->bits);
-      grid_grow_kernel<<<(old_cells + 255) / 256, 256, 0, ctx->stream>>>(g->d_top, g->bits, grown);
+      grid_grow_kernel<<<(old_cells + 255) / 256, 256, 0, ctx->stream>>>(g->d_top.get(), g->bits, grown.get());
       DL_LAUNCH_CHECK(ctx, "grid_grow_kernel");
-      DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      DL_CUDA(ctx, cudaFree(g->d_top));
-      g->d_top = grown;
-      g->d_top_cap = new_size;
+      DL_CUDA(ctx, ctx->wait_stream());
+      g->d_top = std::move(grown);
       g->bits += 1;
       // from here on the device copy is ahead of the host mirror, whatever happens next: a later failure (range, out of
       // memory) must not leave g->bits describing a host `top` of the old size
@@ -347,10 +341,10 @@ int insert_round(dl_context* ctx, std::vector<InsertArgs> args, const std::vecto
   for (unsigned j = 0; j < K; ++j) {
     dl_grid* g = grids[j];
     InsertArgs& a = args[j];
-    a.bits = g->bits; a.top = g->d_top; a.nodes = g->d_nodes; a.bricks = g->d_bricks; a.counters = g->d_counters;
-    DL_CUDA(ctx, cudaMemsetAsync(g->d_counters + 2, 0, 3 * sizeof(int32_t), ctx->stream));
+    a.bits = g->bits; a.top = g->d_top.get(); a.nodes = g->d_nodes.get(); a.bricks = g->d_bricks.get(); a.counters = g->d_counters.get();
+    DL_CUDA(ctx, cudaMemsetAsync(g->d_counters.get() + 2, 0, 3 * sizeof(int32_t), ctx->stream));
   }
-  DL_TRY_STATUS(upload());
+  DL_TRY(upload());
   const int phases = num_free > 0 ? 2 : 1;
   for (int phase = 0; phase < phases; ++phase) {
     ins_claim_kernel<0, 0><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
@@ -360,8 +354,8 @@ int insert_round(dl_context* ctx, std::vector<InsertArgs> args, const std::vecto
     g->mirror_stale = true;
     g->version++;
   }
-  DL_TRY_STATUS(reserve_pools(ctx, args, grids, 0, d_bbox));
-  DL_TRY_STATUS(upload());
+  DL_TRY(reserve_pools(ctx, args, grids, 0, d_bbox));
+  DL_TRY(upload());
   for (int phase = 0; phase < phases; ++phase) {
     ins_claim_kernel<0, 1><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
     DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<0,1>");
@@ -370,8 +364,8 @@ int insert_round(dl_context* ctx, std::vector<InsertArgs> args, const std::vecto
     ins_claim_kernel<1, 0><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
     DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<1,0>");
   }
-  DL_TRY_STATUS(reserve_pools(ctx, args, grids, 1, d_bbox));
-  DL_TRY_STATUS(upload());
+  DL_TRY(reserve_pools(ctx, args, grids, 1, d_bbox));
+  DL_TRY(upload());
   for (int phase = 0; phase < phases; ++phase) {
     ins_claim_kernel<1, 1><<<blocks, kBlock, 0, ctx->stream>>>(d_args, phase);
     DL_LAUNCH_CHECK(ctx, "ins_claim_kernel<1,1>");
@@ -402,7 +396,7 @@ int insert_range_data_device(dl_context* ctx, const InsertJob* jobs, int count, 
   for (int j = 0; j < count; ++j) {
     const InsertJob& job = jobs[j];
     if (job.n <= 0) continue;
-    DL_TRY_STATUS(grid_ensure_device_state(job.grid));
+    DL_TRY(grid_ensure_device_state(job.grid));
     InsertArgs a{};
     a.returns = job.returns; a.n = job.n; a.n_dev = job.n_dev; a.origin = job.origin; a.resolution = job.grid->resolution;
     a.num_free = num_free; a.bbox = d_bbox + 8 * args.size(); a.update_list = job.update_list;
@@ -469,7 +463,7 @@ int insert_range_data_device(dl_context* ctx, const InsertJob* jobs, int count, 
       round_grids.push_back(grids[j]);
       round_bbox.insert(round_bbox.end(), bbox.begin() + 8 * j, bbox.begin() + 8 * j + 8);
     }
-    DL_TRY_STATUS(insert_round(ctx, round_args, round_grids, round_bbox, num_free, d_bbox, d_args));
+    DL_TRY(insert_round(ctx, round_args, round_grids, round_bbox, num_free, d_bbox, d_args));
   }
   return DL_OK;
 }

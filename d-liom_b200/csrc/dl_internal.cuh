@@ -4,6 +4,7 @@
 
 #include <cstdint>
 #include <cstdio>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -41,6 +42,29 @@ __device__ __forceinline__ uint16_t grid_value(const GridView& g, int x, int y, 
   return __ldg(g.bricks + (size_t)brick * 512 + (((sz & 7) << 6) | ((sy & 7) << 3) | (sx & 7)));
 }
 
+// ------------------------------------------------------------------------------------------------ owned memory
+// A handle's device allocation (Pinned: page-locked host memory) and its capacity in elements, freed by the destructor.
+// Structs that kernels take by value keep raw pointers, filled from these owners on the host side.
+// Invariant: a buffer that work queued on the context's stream may still read or write is released or replaced only after a
+// ctx->wait_stream() that covers that work. grow() waits before it frees or swaps, the destroy functions wait before they
+// delete their handle, and a buffer a kernel re-lays into is move-assigned only after a wait.
+template <typename T, bool Pinned = false>
+struct Buffer {
+  struct Free {
+    void operator()(T* p) const { Pinned ? cudaFreeHost(p) : cudaFree(p); }
+  };
+  std::unique_ptr<T, Free> ptr;
+  size_t cap = 0;
+  T* get() const { return ptr.get(); }
+  void reset() {
+    ptr.reset();
+    cap = 0;
+  }
+};
+template <typename T>
+using DeviceBuffer = Buffer<T>;
+using PinnedBuffer = Buffer<uint8_t, true>;
+
 }  // namespace dl
 
 // ------------------------------------------------------------------------------------------------ handles
@@ -52,7 +76,7 @@ struct dl_context {
   cudaStream_t tail_stream = nullptr;   // high priority: the front end's raw-IMU chain (pre-integration, prediction), next to the first filter
   cudaEvent_t staging_done = nullptr;   // the pinned staging block of the previous call has been consumed
   cudaEvent_t batch_done = nullptr;     // dl_frontend_submit: everything of the batch in flight, incl. the result download
-  uint8_t* d_fcsm_lut = nullptr;        // loop-closure search: cell value -> 8-bit precomputation value (dl_fcsm.cu), built on first use
+  dl::DeviceBuffer<uint8_t> d_fcsm_lut; // loop-closure search: cell value -> 8-bit precomputation value (dl_fcsm.cu), built on first use
   int in_flight = 0;                    // scans of the submitted, not yet collected batch
   bool in_flight_states = false;        // ... and whether it also stages the estimated IMU states
   dl_scan_result* staged_results = nullptr;  // where in h_pinned the in-flight batch's results land
@@ -60,10 +84,8 @@ struct dl_context {
   std::string error;
   int64_t launches = 0;
   // growable scratch arenas (device + pinned host), reused across calls
-  void* d_scratch = nullptr;
-  size_t d_scratch_bytes = 0;
-  void* h_pinned = nullptr;
-  size_t h_pinned_bytes = 0;
+  dl::DeviceBuffer<uint8_t> d_scratch;
+  dl::PinnedBuffer h_pinned;
   // optional per-stage timing (events recorded on `stream`)
   bool profiling = false;
   struct Mark {
@@ -114,20 +136,18 @@ struct dl_grid {
   std::vector<uint8_t> brick_dirty;         // per brick
   bool structure_dirty = true;
   // device copies
-  int32_t* d_top = nullptr;
-  int32_t* d_nodes = nullptr;
-  uint16_t* d_bricks = nullptr;
-  size_t d_top_cap = 0, d_nodes_cap = 0, d_bricks_cap = 0;  // element capacities
-  int32_t* d_counters = nullptr;  // [0] nodes in use, [1] bricks in use, [2] scratch (update-list length)
+  dl::DeviceBuffer<int32_t> d_top;
+  dl::DeviceBuffer<int32_t> d_nodes;
+  dl::DeviceBuffer<uint16_t> d_bricks;
+  dl::DeviceBuffer<int32_t> d_counters;  // [0] nodes in use, [1] bricks in use, [2] scratch (update-list length)
   bool mirror_stale = false;      // the device copy was modified by dl_grid_insert_range_data: the host mirror is behind
   uint64_t version = 1;           // bumped by every modification (cells set, sync, device insert)
   // loop-closure search index (dl_fcsm.cu), built on first use and rebuilt when `version` moved on
-  uint8_t* d_m8 = nullptr;
-  size_t d_m8_bytes = 0;
+  dl::DeviceBuffer<uint8_t> d_m8;
   uint64_t m8_version = 0;        // 0 = none
   int m8_org[3] = {0, 0, 0}, m8_dim[3] = {0, 0, 0};
   std::mutex index_mutex;
-  dl::GridView view() const { return {d_top, d_nodes, d_bricks, resolution, bits}; }
+  dl::GridView view() const { return {d_top.get(), d_nodes.get(), d_bricks.get(), resolution, bits}; }
 };
 
 #define DL_CUDA(ctx, call)                                  \
@@ -136,7 +156,7 @@ struct dl_grid {
     if (e__ != cudaSuccess) return (ctx)->cuda_fail(e__, #call); \
   } while (0)
 
-#define DL_TRY_STATUS(expr)         \
+#define DL_TRY(expr)                \
   do {                              \
     const int st__ = (expr);        \
     if (st__ != DL_OK) return st__; \
@@ -150,6 +170,59 @@ struct dl_grid {
   } while (0)
 
 namespace dl {
+
+// Allocates `count` elements into `b`, replacing what it held (see the invariant at Buffer), and sets their bytes to `fill` on
+// the context's stream unless fill < 0. On failure `b` is unchanged.
+template <typename T, bool Pinned>
+int alloc(dl_context* ctx, Buffer<T, Pinned>& b, size_t count, int fill = -1) {
+  void* p = nullptr;
+  const cudaError_t e = Pinned ? cudaMallocHost(&p, count * sizeof(T)) : cudaMalloc(&p, count * sizeof(T));
+  if (e != cudaSuccess) return ctx->cuda_fail(e, Pinned ? "cudaMallocHost" : "cudaMalloc");
+  Buffer<T, Pinned> fresh;
+  fresh.ptr.reset(static_cast<T*>(p));
+  fresh.cap = count;
+  if (fill >= 0) DL_CUDA(ctx, cudaMemsetAsync(p, fill, count * sizeof(T), ctx->stream));
+  b = std::move(fresh);
+  return DL_OK;
+}
+// Replaces `b` by `want` elements (the caller decides when and by how much to grow), keeping its first `keep` elements and
+// setting the others' bytes to `fill` unless fill < 0.
+//   keep == 0: wait, free, allocate, so that the old and the new buffer never coexist. A failed allocation leaves `b` empty.
+//   keep > 0:  allocate and fill, copy the prefix on the context's stream, wait, swap. On failure `b` is unchanged.
+template <typename T, bool Pinned>
+int grow(dl_context* ctx, Buffer<T, Pinned>& b, size_t want, size_t keep = 0, int fill = -1) {
+  if (keep == 0) {
+    if (b.get()) {
+      DL_CUDA(ctx, ctx->wait_stream());
+      b.reset();
+    }
+    return alloc(ctx, b, want, fill);
+  }
+  Buffer<T, Pinned> fresh;
+  DL_TRY(alloc(ctx, fresh, want, fill));
+  DL_CUDA(ctx, cudaMemcpyAsync(fresh.get(), b.get(), keep * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
+  b = std::move(fresh);
+  return DL_OK;
+}
+
+// Copies of `count` elements on the context's stream; the host waits for them (and everything before) with sync().
+template <typename T>
+int h2d(dl_context* ctx, T* dst, const T* src, size_t count) {
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+  return DL_OK;
+}
+template <typename T>
+int d2h(dl_context* ctx, T* dst, const T* src, size_t count) {
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+  return DL_OK;
+}
+inline int sync(dl_context* ctx) {
+  DL_CUDA(ctx, ctx->wait_stream());
+  return DL_OK;
+}
 
 // RAII stage bracket: records begin/end events on the context stream when profiling is on.
 struct StageScope {
@@ -188,7 +261,7 @@ int carve_scratch(dl_context* ctx, Carve&& carve, size_t extra = 0, Arena* rest 
   carve(count);
   const int st = ctx->reserve_device(count.off + extra);
   if (st != DL_OK) return st;
-  Arena a(ctx->d_scratch);
+  Arena a(ctx->d_scratch.get());
   carve(a);
   if (rest) *rest = a;
   return DL_OK;
@@ -454,6 +527,10 @@ int check_constraint_options(dl_context* ctx, const dl_constraint_options& optio
 int constraint_search(dl_context* ctx, const dl_constraint_options& options, int count, const double* guesses,
                       const PairClouds& clouds, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids,
                       dl_constraint* constraints);
+// dl_api.cu: uploads a grid's host mirror where the device copy is behind; grows its node pool (level 0) or brick pool (level 1)
+// from `used` entries in use by `add` more, keeping those in use
+int grid_ensure_device_state(dl_grid* g);
+int grid_grow_pool(dl_grid* g, int level, size_t used, size_t add);
 int launch_interpolate(dl_context* ctx, const GridView& grid, int64_t n, const double* xyz, double* out);
 int launch_grid_lookup(dl_context* ctx, const GridView& grid, int64_t n, const int32_t* xyz, uint16_t* out);
 

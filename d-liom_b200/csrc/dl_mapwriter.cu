@@ -97,6 +97,17 @@ struct Table {
   int shift;
   int32_t* num_cells;
 };
+// The owners behind a Table, which kernels take by value.
+struct TableBuffers {
+  DeviceBuffer<unsigned long long> keys;
+  DeviceBuffer<int32_t> hits, rays, num_cells;
+  DeviceBuffer<float4> sums;
+  Table view() const {
+    int shift = 64;
+    for (size_t c = keys.cap; c > 1; c >>= 1) --shift;
+    return Table{keys.get(), hits.get(), rays.get(), sums.get(), (int64_t)keys.cap - 1, shift, num_cells.get()};
+  }
+};
 
 __device__ __forceinline__ int message_of(const MsgRec* msgs, int num_msgs, int64_t v) {
   int lo = 0, hi = num_msgs;  // last message with voff <= v (empty messages share the next one's voff)
@@ -838,9 +849,9 @@ struct GridStage {
   double resolution;
   int32_t insert_free_space;
   GridLimits limits;         // after the last call
-  uint16_t* cells = nullptr;   // allocated at `limits` once a batch arrived (before that every cell is unknown)
-  uint32_t* stamps = nullptr;
-  uint16_t* tables = nullptr;  // hit [0, 32768), miss [32768, 65536)
+  DeviceBuffer<uint16_t> cells;   // allocated at `limits` once a batch arrived (before that every cell is unknown)
+  DeviceBuffer<uint32_t> stamps;
+  DeviceBuffer<uint16_t> tables;  // hit [0, 32768), miss [32768, 65536)
   int64_t batches = 0;       // k of the last batch
 };
 // One call's growth of one stage, decided before anything changes: every batch's limits and cell offset in the grid of the
@@ -850,8 +861,8 @@ struct GridPlan {
   std::vector<GridLimits> at;
   std::vector<int2> offset;
   int32_t grow_x = 0, grow_y = 0;  // where the previous content lands
-  uint16_t* cells = nullptr;
-  uint32_t* stamps = nullptr;
+  DeviceBuffer<uint16_t> cells;
+  DeviceBuffer<uint32_t> stamps;
 };
 
 // MapLimits::GetCellIndex (map_limits.h:69-76)
@@ -885,12 +896,6 @@ float key_float(uint32_t k) {
 
 unsigned tiles_of(int64_t n) { return (unsigned)((n + kBlock - 1) / kBlock); }
 
-#define MW_TRY(expr)                \
-  do {                              \
-    const int st__ = (expr);        \
-    if (st__ != DL_OK) return st__; \
-  } while (0)
-
 }  // namespace
 
 struct dl_map_writer {
@@ -902,28 +907,25 @@ struct dl_map_writer {
   std::vector<int64_t> times;
   std::vector<NodeRec> nodes;
   bool tables_dirty = false;
-  int64_t* d_times = nullptr;
-  NodeRec* d_nodes = nullptr;
-  TrajRec* d_trajs = nullptr;
+  DeviceBuffer<int64_t> d_times;
+  DeviceBuffer<NodeRec> d_nodes;
+  DeviceBuffer<TrajRec> d_trajs;
   int pass = 0;                    // 0 .. num_passes - 1
   bool started = false, finished = false;
-  RunPose* d_runs = nullptr;
-  int64_t runs_capacity = 0;
-  Table table{};                   // cell -> (hits, rays)
-  int64_t table_capacity = 0;
+  DeviceBuffer<RunPose> d_runs;
+  TableBuffers table;              // cell -> (hits, rays)
   int64_t num_cells = 0;
   // X-ray and colour stages, in pipeline order
   std::vector<XrayStage> xrays;
   std::vector<ColorStage> colors;
   std::vector<int32_t> sum_stage;  // stage of every sum_index
-  Table xray{};                    // voxel and column keys of every X-ray stage (see the key layout above), with colour sums
-  int64_t xray_capacity = 0;
+  TableBuffers xray;               // voxel and column keys of every X-ray stage (see the key layout above), with colour sums
   int64_t xray_entries = 0;
-  int32_t* d_bbox = nullptr;       // 6 per stage
-  double* d_log = nullptr;         // log_table()
+  DeviceBuffer<int32_t> d_bbox;    // 6 per stage
+  DeviceBuffer<double> d_log;      // log_table()
   // probability-grid stages, in the order they were added
   std::vector<GridStage> grids;
-  uint8_t* d_grid_colors = nullptr;  // grid_color_table()
+  DeviceBuffer<uint8_t> d_grid_colors;  // grid_color_table()
   struct GridCall {                // the batches of one final-pass call and every stage's plan
     std::vector<int32_t> first, count;
     std::vector<float> origins;    // x y per batch
@@ -936,75 +938,38 @@ struct dl_map_writer {
 
   int upload_tables() {
     if (!tables_dirty) return DL_OK;
-    cudaFree(d_times);
-    cudaFree(d_nodes);
-    cudaFree(d_trajs);
-    d_times = nullptr; d_nodes = nullptr; d_trajs = nullptr;
     const size_t nn = std::max<size_t>(nodes.size(), 1), nt = std::max<size_t>(trajs.size(), 1);
-    DL_CUDA(ctx, cudaMalloc(&d_times, nn * sizeof(int64_t)));
-    DL_CUDA(ctx, cudaMalloc(&d_nodes, nn * sizeof(NodeRec)));
-    DL_CUDA(ctx, cudaMalloc(&d_trajs, nt * sizeof(TrajRec)));
-    DL_CUDA(ctx, cudaMemcpy(d_times, times.data(), times.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
-    DL_CUDA(ctx, cudaMemcpy(d_nodes, nodes.data(), nodes.size() * sizeof(NodeRec), cudaMemcpyHostToDevice));
-    DL_CUDA(ctx, cudaMemcpy(d_trajs, trajs.data(), trajs.size() * sizeof(TrajRec), cudaMemcpyHostToDevice));
+    DL_TRY(grow(ctx, d_times, nn));
+    DL_TRY(grow(ctx, d_nodes, nn));
+    DL_TRY(grow(ctx, d_trajs, nt));
+    DL_TRY(h2d(ctx, d_times.get(), times.data(), times.size()));
+    DL_TRY(h2d(ctx, d_nodes.get(), nodes.data(), nodes.size()));
+    DL_TRY(h2d(ctx, d_trajs.get(), trajs.data(), trajs.size()));
     tables_dirty = false;
     return DL_OK;
   }
   int reserve_runs(int64_t n) {
-    if (n <= runs_capacity) return DL_OK;
-    const int64_t cap = std::max<int64_t>({n, 2 * runs_capacity, 4096});
-    DL_CUDA(ctx, ctx->wait_stream());
-    cudaFree(d_runs);
-    d_runs = nullptr;
-    runs_capacity = 0;
-    DL_CUDA(ctx, cudaMalloc(&d_runs, (size_t)cap * sizeof(RunPose)));
-    runs_capacity = cap;
-    return DL_OK;
-  }
-  static int alloc_table(dl_context* ctx, int64_t cap, bool sums, Table* t) {
-    int shift = 64;
-    for (int64_t c = cap; c > 1; c >>= 1) --shift;
-    t->mask = cap - 1;
-    t->shift = shift;
-    DL_CUDA(ctx, cudaMalloc(&t->keys, (size_t)cap * sizeof(unsigned long long)));
-    DL_CUDA(ctx, cudaMalloc(&t->hits, (size_t)cap * sizeof(int32_t)));
-    DL_CUDA(ctx, cudaMalloc(&t->rays, (size_t)cap * sizeof(int32_t)));
-    DL_CUDA(ctx, cudaMemsetAsync(t->keys, 0xff, (size_t)cap * sizeof(unsigned long long), ctx->stream));
-    DL_CUDA(ctx, cudaMemsetAsync(t->hits, 0, (size_t)cap * sizeof(int32_t), ctx->stream));
-    DL_CUDA(ctx, cudaMemsetAsync(t->rays, 0, (size_t)cap * sizeof(int32_t), ctx->stream));
-    if (sums) {
-      DL_CUDA(ctx, cudaMalloc(&t->sums, (size_t)cap * sizeof(float4)));
-      DL_CUDA(ctx, cudaMemsetAsync(t->sums, 0, (size_t)cap * sizeof(float4), ctx->stream));
-    }
-    return DL_OK;
-  }
-  static void free_table(Table* t) {
-    cudaFree(t->keys);
-    cudaFree(t->hits);
-    cudaFree(t->rays);
-    cudaFree(t->sums);
-    t->keys = nullptr; t->hits = nullptr; t->rays = nullptr; t->sums = nullptr;
+    if (n <= (int64_t)d_runs.cap) return DL_OK;
+    return grow(ctx, d_runs, (size_t)std::max<int64_t>({n, 2 * (int64_t)d_runs.cap, 4096}));
   }
   // Load factor <= 1/2 after `adding` more entries: sized from a count of the points about to be inserted.
-  int reserve_table(Table* t, int64_t* capacity, int64_t used, int64_t adding, bool sums) {
+  int reserve_table(TableBuffers* t, int64_t used, int64_t adding, bool sums) {
     int64_t cap = 1024;
     while (cap < 2 * (used + adding)) cap <<= 1;
-    if (cap <= *capacity) return DL_OK;
-    Table fresh{};
-    const int st = alloc_table(ctx, cap, sums, &fresh);
-    if (st != DL_OK) {
-      free_table(&fresh);
-      return st;
-    }
-    if (*capacity > 0) {
-      mw_rehash<<<tiles_of(*capacity), kBlock, 0, ctx->stream>>>(fresh, *t, *capacity);
+    const int64_t capacity = (int64_t)t->keys.cap;
+    if (cap <= capacity) return DL_OK;
+    TableBuffers fresh;
+    DL_TRY(alloc(ctx, fresh.keys, (size_t)cap, 0xff));
+    DL_TRY(alloc(ctx, fresh.hits, (size_t)cap, 0));
+    DL_TRY(alloc(ctx, fresh.rays, (size_t)cap, 0));
+    if (sums) DL_TRY(alloc(ctx, fresh.sums, (size_t)cap, 0));
+    if (capacity > 0) {
+      mw_rehash<<<tiles_of(capacity), kBlock, 0, ctx->stream>>>(fresh.view(), t->view(), capacity);
       DL_LAUNCH_CHECK(ctx, "mw_rehash");
     }
     DL_CUDA(ctx, ctx->wait_stream());
-    fresh.num_cells = t->num_cells;
-    free_table(t);
-    *t = fresh;
-    *capacity = cap;
+    fresh.num_cells = std::move(t->num_cells);
+    *t = std::move(fresh);
     return DL_OK;
   }
   int insert_xray(const float* points, const int32_t* point_msg, const MsgRec* msgs, int64_t n, void* sort_scratch,
@@ -1015,12 +980,12 @@ struct dl_map_writer {
     std::copy(xrays.begin(), xrays.end(), a.stages);
     std::copy(colors.begin(), colors.end(), a.colors);
     std::copy(sum_stage.begin(), sum_stage.end(), a.sum_stage);
-    a.bbox = d_bbox;
+    a.bbox = d_bbox.get();
     return a;
   }
   // the X-ray table, the bounding boxes and the log table, at the first X-ray stage
   int init_xray() {
-    if (xray.num_cells) return DL_OK;
+    if (xray.num_cells.get()) return DL_OK;
     DL_CUDA(ctx, cudaSetDevice(ctx->device));
     std::vector<int32_t> box(6 * kMaxStages);
     for (int s = 0; s < kMaxStages; ++s)
@@ -1029,25 +994,12 @@ struct dl_map_writer {
         box[6 * s + 3 + k] = INT_MIN;
       }
     const std::vector<double>& logs = log_table();
-    int32_t* counter = nullptr;
-    int32_t* bbox = nullptr;
-    double* logs_dev = nullptr;
-    cudaError_t e = cudaMalloc(&counter, sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&bbox, box.size() * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&logs_dev, logs.size() * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemset(counter, 0, sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMemcpy(bbox, box.data(), box.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(logs_dev, logs.data(), logs.size() * sizeof(double), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      cudaFree(counter);
-      cudaFree(bbox);
-      cudaFree(logs_dev);
-      return ctx->cuda_fail(e, "dl_map_writer_add_xray");
-    }
-    xray.num_cells = counter;
-    d_bbox = bbox;
-    d_log = logs_dev;
-    return DL_OK;
+    DL_TRY(alloc(ctx, d_bbox, box.size()));
+    DL_TRY(alloc(ctx, d_log, logs.size()));
+    DL_TRY(h2d(ctx, d_bbox.get(), box.data(), box.size()));
+    DL_TRY(h2d(ctx, d_log.get(), logs.data(), logs.size()));
+    DL_TRY(sync(ctx));                         // `box` is pageable and local
+    return alloc(ctx, xray.num_cells, 1, 0);  // last: the counter marks the X-ray state as made
   }
   int process(int32_t num_messages, const dl_map_message* messages, const float* rows_host, const float* rows_dev,
               int64_t num_rows, float* points_host, float* points_dev, int64_t* num_points_out, float* origins_out,
@@ -1055,14 +1007,6 @@ struct dl_map_writer {
   int plan_grids(const float* points, const int32_t* point_msg, int64_t n, const float* origins, int num_messages,
                  const std::vector<int32_t>& last_run, const GridBoxes& boxes, GridCall* call);
   int apply_grids(const float* points, GridCall* call);
-  static void drop_plans(GridCall* call) {
-    for (GridPlan& p : call->plans) {
-      cudaFree(p.cells);
-      cudaFree(p.stamps);
-      p.cells = nullptr;
-      p.stamps = nullptr;
-    }
-  }
 };
 
 namespace {
@@ -1111,7 +1055,7 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
     return DL_OK;
   }
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  MW_TRY(upload_tables());
+  DL_TRY(upload_tables());
   const unsigned tiles = tiles_of(n);
   SelectArgs a{};
   float4* up_rows = nullptr;
@@ -1134,7 +1078,7 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   unsigned long long* sort_keys = nullptr;
   int32_t* sort_vals = nullptr;
   void* sort_scratch = nullptr;
-  MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+  DL_TRY(carve_scratch(ctx, [&](Arena& ar) {
     if (with_xray || with_grid) out_msg = ar.take<int32_t>((size_t)n);
     if (with_grid) {
       boxes.keys = ar.take<uint32_t>(4 * (size_t)num_messages);
@@ -1174,9 +1118,9 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   a.msgs = d_msgs;
   a.num_msgs = num_messages;
   a.n = n;
-  a.times = d_times;
-  a.nodes = d_nodes;
-  a.trajs = d_trajs;
+  a.times = d_times.get();
+  a.nodes = d_nodes.get();
+  a.trajs = d_trajs.get();
   a.num_runs = d_ints;
   a.num_keep = d_ints + 1;
   a.range_filter = options.range_filter;
@@ -1193,8 +1137,8 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   int32_t num_runs = 0;
   DL_CUDA(ctx, cudaMemcpyAsync(&num_runs, a.num_runs, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   DL_CUDA(ctx, ctx->wait_stream());
-  MW_TRY(reserve_runs(num_runs));
-  a.runs = d_runs;
+  DL_TRY(reserve_runs(num_runs));
+  a.runs = d_runs.get();
   mw_run_poses<<<tiles, kBlock, 0, ctx->stream>>>(a);
   DL_LAUNCH_CHECK(ctx, "mw_run_poses");
   mw_origins<<<(num_messages + 127) / 128, 128, 0, ctx->stream>>>(a);
@@ -1231,28 +1175,29 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   local.dropped_range = (int64_t)counters[kRange];
   local.messages_without_batch = std::count(last_run.begin(), last_run.end(), -1);
 
-  if (options.outlier_voxel_size > 0) MW_TRY(reserve_table(&table, &table_capacity, num_cells, pass == 0 ? kept : 0, false));
+  if (options.outlier_voxel_size > 0) DL_TRY(reserve_table(&table, num_cells, pass == 0 ? kept : 0, false));
+  const Table t = table.view();
   int64_t out_count = 0;
   if (direct) {
     out_count = kept;
   } else if (pass == 0) {
     if (kept > 0) {
-      mw_insert_hits<<<tiles_of(kept), kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution);
+      mw_insert_hits<<<tiles_of(kept), kBlock, 0, ctx->stream>>>(t, a.compact, kept, resolution);
       DL_LAUNCH_CHECK(ctx, "mw_insert_hits");
     }
   } else if (pass == 1) {
     if (kept > 0) {
-      mw_rays<<<tiles_of(kept), kBlock, 0, ctx->stream>>>(table, a.compact, kept, a.origins, resolution, options.outlier_voxel_size,
+      mw_rays<<<tiles_of(kept), kBlock, 0, ctx->stream>>>(t, a.compact, kept, a.origins, resolution, options.outlier_voxel_size,
                                                           a.counters);
       DL_LAUNCH_CHECK(ctx, "mw_rays");
     }
   } else if (kept > 0) {
     const unsigned gt = tiles_of(kept);
-    mw_gate<0><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, nullptr, nullptr);
+    mw_gate<0><<<gt, kBlock, 0, ctx->stream>>>(t, a.compact, kept, resolution, gate_tiles, nullptr, nullptr);
     DL_LAUNCH_CHECK(ctx, "mw_gate<0>");
     mw_tile_prefix<<<1, kBlock, 0, ctx->stream>>>(gate_tiles, (int)gt, d_ints + 2);
     DL_LAUNCH_CHECK(ctx, "mw_tile_prefix");
-    mw_gate<1><<<gt, kBlock, 0, ctx->stream>>>(table, a.compact, kept, resolution, gate_tiles, d_out, out_msg);
+    mw_gate<1><<<gt, kBlock, 0, ctx->stream>>>(t, a.compact, kept, resolution, gate_tiles, d_out, out_msg);
     DL_LAUNCH_CHECK(ctx, "mw_gate<1>");
     int32_t survivors = 0;
     DL_CUDA(ctx, cudaMemcpyAsync(&survivors, d_ints + 2, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1262,19 +1207,13 @@ int dl_map_writer::process(int32_t num_messages, const dl_map_message* messages,
   }
   // every stage checks its input before any of them changes: the grids' growth first, then the X-ray cells
   GridCall grid_call;
-  if (with_grid) MW_TRY(plan_grids(d_out, out_msg, out_count, a.origins, num_messages, last_run, boxes, &grid_call));
-  if (with_xray && out_count > 0) {
-    const int st = insert_xray(d_out, out_msg, d_msgs, out_count, sort_scratch, sort_bytes, sort_keys, sort_vals,
-                               a.counters + kOutside);
-    if (st != DL_OK) {
-      drop_plans(&grid_call);
-      return st;
-    }
-  }
-  if (with_grid) MW_TRY(apply_grids(d_out, &grid_call));
+  if (with_grid) DL_TRY(plan_grids(d_out, out_msg, out_count, a.origins, num_messages, last_run, boxes, &grid_call));
+  if (with_xray && out_count > 0)
+    DL_TRY(insert_xray(d_out, out_msg, d_msgs, out_count, sort_scratch, sort_bytes, sort_keys, sort_vals, a.counters + kOutside));
+  if (with_grid) DL_TRY(apply_grids(d_out, &grid_call));
   DL_CUDA(ctx, cudaMemcpyAsync(counters, a.counters, sizeof(counters), cudaMemcpyDeviceToHost, ctx->stream));
   int32_t cells = 0;
-  if (table.num_cells) DL_CUDA(ctx, cudaMemcpyAsync(&cells, table.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  if (t.num_cells) DL_CUDA(ctx, cudaMemcpyAsync(&cells, t.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   if (points_host && out_count > 0)
     DL_CUDA(ctx, cudaMemcpyAsync(points_host, d_out, 3 * (size_t)out_count * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   DL_CUDA(ctx, ctx->wait_stream());
@@ -1313,13 +1252,14 @@ int dl_map_writer::insert_xray(const float* points, const int32_t* point_msg, co
   while ((1 << sum_bits) < num_sums) ++sum_bits;
   for (int64_t first = 0; first < n; first += kXrayChunk) {
     const int64_t m = std::min(kXrayChunk, n - first);
-    MW_TRY(reserve_table(&xray, &xray_capacity, xray_entries, 2 * m * (int64_t)xrays.size(), true));
+    DL_TRY(reserve_table(&xray, xray_entries, 2 * m * (int64_t)xrays.size(), true));
+    const Table t = xray.view();
     a.first = first;
     a.n = m;
-    a.slot_bits = 64 - xray.shift;
+    a.slot_bits = 64 - t.shift;
     a.sort_keys = keys;
     a.sort_vals = vals;
-    mw_xray_insert<<<tiles_of(m), kBlock, 0, ctx->stream>>>(xray, a);
+    mw_xray_insert<<<tiles_of(m), kBlock, 0, ctx->stream>>>(t, a);
     DL_LAUNCH_CHECK(ctx, "mw_xray_insert");
     if (num_sums > 0) {
       const int items = (int)(m * num_sums);
@@ -1327,11 +1267,11 @@ int dl_map_writer::insert_xray(const float* points, const int32_t* point_msg, co
       cub::DoubleBuffer<int32_t> v(vals, vals + items_cap);
       // the scratch was sized for all 64 bits and items_cap items, the most any chunk sorts
       DL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(sort_scratch, sort_bytes, k, v, items, 0, a.slot_bits + sum_bits, ctx->stream));
-      mw_xray_fold<<<tiles_of(items), kBlock, 0, ctx->stream>>>(xray, a, k.Current(), v.Current(), items);
+      mw_xray_fold<<<tiles_of(items), kBlock, 0, ctx->stream>>>(t, a, k.Current(), v.Current(), items);
       DL_LAUNCH_CHECK(ctx, "mw_xray_fold");
     }
     int32_t entries = 0;
-    DL_CUDA(ctx, cudaMemcpyAsync(&entries, xray.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(&entries, t.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     DL_CUDA(ctx, ctx->wait_stream());
     xray_entries = entries;
   }
@@ -1397,27 +1337,21 @@ int dl_map_writer::plan_grids(const float* points, const int32_t* point_msg, int
     std::vector<int2> at_growth;
     for (size_t j = 0; j < batch_msgs.size(); ++j) {
       if (!grid_grow_limits(&p.final_limits, g.resolution, lo[2 * j], lo[2 * j + 1], &p.grow_x, &p.grow_y) ||
-          !grid_grow_limits(&p.final_limits, g.resolution, hi[2 * j], hi[2 * j + 1], &p.grow_x, &p.grow_y)) {
-        drop_plans(call);
+          !grid_grow_limits(&p.final_limits, g.resolution, hi[2 * j], hi[2 * j + 1], &p.grow_x, &p.grow_y))
         return ctx->fail(DL_ERR_ARG, "dl_map_writer_process: a batch would grow a probability grid beyond "
                                      "DL_MAP_WRITER_MAX_GRID_CELLS cells per axis");
-      }
       p.at.push_back(p.final_limits);
       at_growth.push_back(make_int2(p.grow_x, p.grow_y));
     }
     for (const int2& c : at_growth) p.offset.push_back(make_int2(p.grow_x - c.x, p.grow_y - c.y));
-    call->plans.push_back(p);
+    call->plans.push_back(std::move(p));
   }
   for (size_t s = 0; s < grids.size(); ++s) {
     GridPlan& p = call->plans[s];
-    if (grids[s].cells && p.grow_x == 0 && p.grow_y == 0) continue;
+    if (grids[s].cells.get() && p.grow_x == 0 && p.grow_y == 0) continue;
     const size_t cells = (size_t)p.final_limits.nx * (size_t)p.final_limits.ny;
-    cudaError_t e = cudaMalloc(&p.cells, cells * sizeof(uint16_t));
-    if (e == cudaSuccess) e = cudaMalloc(&p.stamps, cells * sizeof(uint32_t));
-    if (e != cudaSuccess) {
-      drop_plans(call);
-      return ctx->cuda_fail(e, "dl_map_writer_process (probability grid)");
-    }
+    DL_TRY(alloc(ctx, p.cells, cells));
+    DL_TRY(alloc(ctx, p.stamps, cells));
   }
   return DL_OK;
 }
@@ -1428,21 +1362,18 @@ int dl_map_writer::apply_grids(const float* points, GridCall* call) {
     GridStage& g = grids[s];
     GridPlan& p = call->plans[s];
     const GridLimits& l = p.final_limits;
-    if (p.cells) {
+    if (p.cells.get()) {
       const size_t cells = (size_t)l.nx * (size_t)l.ny;
-      DL_CUDA(ctx, cudaMemsetAsync(p.cells, 0, cells * sizeof(uint16_t), ctx->stream));
-      DL_CUDA(ctx, cudaMemsetAsync(p.stamps, 0, cells * sizeof(uint32_t), ctx->stream));  // below every claim
-      if (g.cells)
-        DL_CUDA(ctx, cudaMemcpy2DAsync(p.cells + (size_t)p.grow_y * l.nx + p.grow_x, (size_t)l.nx * sizeof(uint16_t), g.cells,
-                                       (size_t)g.limits.nx * sizeof(uint16_t), (size_t)g.limits.nx * sizeof(uint16_t),
+      DL_CUDA(ctx, cudaMemsetAsync(p.cells.get(), 0, cells * sizeof(uint16_t), ctx->stream));
+      DL_CUDA(ctx, cudaMemsetAsync(p.stamps.get(), 0, cells * sizeof(uint32_t), ctx->stream));  // below every claim
+      if (g.cells.get()) {
+        DL_CUDA(ctx, cudaMemcpy2DAsync(p.cells.get() + (size_t)p.grow_y * l.nx + p.grow_x, (size_t)l.nx * sizeof(uint16_t),
+                                       g.cells.get(), (size_t)g.limits.nx * sizeof(uint16_t), (size_t)g.limits.nx * sizeof(uint16_t),
                                        (size_t)g.limits.ny, cudaMemcpyDeviceToDevice, ctx->stream));
-      if (g.cells) DL_CUDA(ctx, ctx->wait_stream());  // the copy out of the old buffers has ended
-      cudaFree(g.cells);
-      cudaFree(g.stamps);
-      g.cells = p.cells;
-      g.stamps = p.stamps;
-      p.cells = nullptr;
-      p.stamps = nullptr;
+        DL_CUDA(ctx, ctx->wait_stream());  // the copy out of the old buffers has ended
+      }
+      g.cells = std::move(p.cells);
+      g.stamps = std::move(p.stamps);
     }
     g.limits = l;
     const double superscaled = g.resolution / kSubpixel;
@@ -1461,15 +1392,15 @@ int dl_map_writer::apply_grids(const float* points, GridCall* call) {
       gb.max_x = p.at[j].max_x;
       gb.max_y = p.at[j].max_y;
       gb.resolution = superscaled;
-      gb.cells = g.cells;
-      gb.stamps = g.stamps;
+      gb.cells = g.cells.get();
+      gb.stamps = g.stamps.get();
       if (gb.n == 0) continue;  // the batch only grew the grid
-      gb.table = g.tables;
+      gb.table = g.tables.get();
       gb.claim = (uint32_t)(2 * k + 1);
       mw_grid_hits<<<tiles_of(gb.n), kBlock, 0, ctx->stream>>>(gb);
       DL_LAUNCH_CHECK(ctx, "mw_grid_hits");
       if (!g.insert_free_space) continue;
-      gb.table = g.tables + 32768;
+      gb.table = g.tables.get() + 32768;
       gb.claim = (uint32_t)(2 * k);
       mw_grid_walks<<<tiles_of(gb.n), kBlock, 0, ctx->stream>>>(gb);
       DL_LAUNCH_CHECK(ctx, "mw_grid_walks");
@@ -1487,46 +1418,22 @@ int dl_map_writer_create(dl_context* ctx, const dl_map_writer_options* options, 
   if (!(o.outlier_voxel_size >= 0) || !std::isfinite(o.outlier_voxel_size) ||
       (o.outlier_voxel_size > 0 && !((float)o.outlier_voxel_size > 0.f)))
     return ctx->fail(DL_ERR_ARG, "outlier_voxel_size must be finite and >= 0");
-  dl_map_writer* w = new dl_map_writer();
+  std::unique_ptr<dl_map_writer> w(new dl_map_writer());
   w->ctx = ctx;
   w->options = o;
   w->resolution = (float)o.outlier_voxel_size;
   if (o.outlier_voxel_size > 0) {
     DL_CUDA(ctx, cudaSetDevice(ctx->device));
-    int32_t* counter = nullptr;
-    cudaError_t e = cudaMalloc(&counter, sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMemset(counter, 0, sizeof(int32_t));
-    if (e != cudaSuccess) {
-      cudaFree(counter);
-      delete w;
-      return ctx->cuda_fail(e, "dl_map_writer_create");
-    }
-    w->table.num_cells = counter;
+    DL_TRY(alloc(ctx, w->table.num_cells, 1, 0));
   }
-  *out = w;
+  *out = w.release();
   return DL_OK;
 }
 
 void dl_map_writer_destroy(dl_map_writer* w) {
   if (!w) return;
   cudaSetDevice(w->ctx->device);
-  cudaStreamSynchronize(w->ctx->stream);
-  dl_map_writer::free_table(&w->table);
-  cudaFree(w->table.num_cells);
-  dl_map_writer::free_table(&w->xray);
-  cudaFree(w->xray.num_cells);
-  cudaFree(w->d_bbox);
-  cudaFree(w->d_log);
-  for (GridStage& g : w->grids) {
-    cudaFree(g.cells);
-    cudaFree(g.stamps);
-    cudaFree(g.tables);
-  }
-  cudaFree(w->d_grid_colors);
-  cudaFree(w->d_runs);
-  cudaFree(w->d_times);
-  cudaFree(w->d_nodes);
-  cudaFree(w->d_trajs);
+  w->ctx->wait_stream();
   delete w;
 }
 
@@ -1592,15 +1499,15 @@ int dl_map_writer_voxels(const dl_map_writer* w, int64_t capacity, int32_t* cell
   *count = w->num_cells;
   if (!cells_xyz) return DL_OK;
   if (capacity < w->num_cells || !hits || !rays) return ctx->fail(DL_ERR_ARG, "dl_map_writer_voxels: capacity below the cell count");
-  if (w->table_capacity == 0) return DL_OK;
-  const size_t cap = (size_t)w->table_capacity;
+  const size_t cap = w->table.keys.cap;
+  if (cap == 0) return DL_OK;
   std::vector<unsigned long long> keys(cap);
   std::vector<int32_t> h(cap), r(cap);
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  DL_CUDA(ctx, cudaMemcpy(keys.data(), w->table.keys, cap * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  DL_CUDA(ctx, cudaMemcpy(h.data(), w->table.hits, cap * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  DL_CUDA(ctx, cudaMemcpy(r.data(), w->table.rays, cap * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  DL_TRY(d2h(ctx, keys.data(), w->table.keys.get(), cap));
+  DL_TRY(d2h(ctx, h.data(), w->table.hits.get(), cap));
+  DL_TRY(d2h(ctx, r.data(), w->table.rays.get(), cap));
+  DL_TRY(sync(ctx));
   std::vector<size_t> order;
   for (size_t i = 0; i < cap; ++i)
     if (keys[i] != kEmpty) order.push_back(i);
@@ -1642,7 +1549,7 @@ int dl_map_writer_add_xray(dl_map_writer* w, const dl_map_writer_xray* xray, int
   const double* q = xray->transform + 3;  // Eigen's squaredNorm order
   const double norm = std::sqrt(q[1] * q[1] + q[2] * q[2] + q[3] * q[3] + q[0] * q[0]);
   if (!(std::fabs(norm - 1.0) <= 1e-9)) return ctx->fail(DL_ERR_ARG, "dl_map_writer_add_xray: the rotation is not a unit quaternion");
-  MW_TRY(w->init_xray());
+  DL_TRY(w->init_xray());
   XrayStage s{};
   s.transform = to_float(pose_from7(xray->transform));
   s.resolution = (float)xray->voxel_size;
@@ -1665,8 +1572,8 @@ int dl_map_writer_xray_image(const dl_map_writer* w, int32_t stage, int64_t capa
   if (!w->finished) return ctx->fail(DL_ERR_ARG, "dl_map_writer_xray_image: the final pass has not been flushed");
   int32_t box[6];
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  DL_CUDA(ctx, cudaMemcpy(box, w->d_bbox + 6 * stage, sizeof(box), cudaMemcpyDeviceToHost));
+  DL_TRY(d2h(ctx, box, w->d_bbox.get() + 6 * stage, 6));
+  DL_TRY(sync(ctx));
   const bool empty = box[1] > box[4];  // Eigen::AlignedBox::isEmpty
   const int32_t wd = empty ? 0 : box[4] - box[1] + 1, ht = empty ? 0 : box[5] - box[2] + 1;
   *width = wd;
@@ -1676,14 +1583,16 @@ int dl_map_writer_xray_image(const dl_map_writer* w, int32_t stage, int64_t capa
   if (capacity < pixels) return ctx->fail(DL_ERR_ARG, "dl_map_writer_xray_image: capacity below width * height");
   int32_t* d_max = nullptr;
   uint32_t* d_img = nullptr;
-  MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+  DL_TRY(carve_scratch(ctx, [&](Arena& ar) {
     d_max = ar.take<int32_t>(1);
     d_img = ar.take<uint32_t>((size_t)pixels);
   }));
-  const unsigned tiles = tiles_of(w->xray_capacity);
+  const Table xray = w->xray.view();
+  const int64_t xray_capacity = (int64_t)w->xray.keys.cap;
+  const unsigned tiles = tiles_of(xray_capacity);
   DL_CUDA(ctx, cudaMemsetAsync(d_max, 0, sizeof(int32_t), ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(d_img, 0xff, (size_t)pixels * sizeof(uint32_t), ctx->stream));  // white
-  mw_xray_max_voxels<<<tiles, kBlock, 0, ctx->stream>>>(w->xray, w->xray_capacity, stage, d_max);
+  mw_xray_max_voxels<<<tiles, kBlock, 0, ctx->stream>>>(xray, xray_capacity, stage, d_max);
   DL_LAUNCH_CHECK(ctx, "mw_xray_max_voxels");
   int32_t max_voxels = 0;
   DL_CUDA(ctx, cudaMemcpyAsync(&max_voxels, d_max, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1691,7 +1600,7 @@ int dl_map_writer_xray_image(const dl_map_writer* w, int32_t stage, int64_t capa
   // IntoImage: max starts at numeric_limits<float>::min() and takes std::max<float>(max, log(n)); log is monotone, so the
   // largest n gives the largest (float)log(n)
   const float max_log = std::max<float>(FLT_MIN, (float)log_table()[max_voxels]);
-  mw_xray_pixels<<<tiles, kBlock, 0, ctx->stream>>>(w->xray, w->xray_capacity, stage, w->d_log, max_log, box[4], box[5], wd,
+  mw_xray_pixels<<<tiles, kBlock, 0, ctx->stream>>>(xray, xray_capacity, stage, w->d_log.get(), max_log, box[4], box[5], wd,
                                                      d_img);
   DL_LAUNCH_CHECK(ctx, "mw_xray_pixels");
   DL_CUDA(ctx, cudaMemcpyAsync(argb, d_img, (size_t)pixels * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1720,29 +1629,23 @@ int dl_map_writer_add_probability_grid(dl_map_writer* w, const dl_map_writer_gri
   compute_correspondence_cost_table(o.hit_probability, tables.data());
   compute_correspondence_cost_table(o.miss_probability, tables.data() + 32768);
   const std::vector<uint8_t> colors = grid_color_table();
-  uint16_t* d_tables = nullptr;
-  uint8_t* d_colors = nullptr;
-  cudaError_t e = cudaMalloc(&d_tables, tables.size() * sizeof(uint16_t));
-  if (e == cudaSuccess) e = cudaMemcpy(d_tables, tables.data(), tables.size() * sizeof(uint16_t), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && !w->d_grid_colors) {
-    e = cudaMalloc(&d_colors, colors.size());
-    if (e == cudaSuccess) e = cudaMemcpy(d_colors, colors.data(), colors.size(), cudaMemcpyHostToDevice);
-  }
-  if (e != cudaSuccess) {
-    cudaFree(d_tables);
-    cudaFree(d_colors);
-    return ctx->cuda_fail(e, "dl_map_writer_add_probability_grid");
-  }
-  if (d_colors) w->d_grid_colors = d_colors;
   GridStage g{};
+  DeviceBuffer<uint8_t> d_colors;
+  DL_TRY(alloc(ctx, g.tables, tables.size()));
+  DL_TRY(h2d(ctx, g.tables.get(), tables.data(), tables.size()));
+  if (!w->d_grid_colors.get()) {
+    DL_TRY(alloc(ctx, d_colors, colors.size()));
+    DL_TRY(h2d(ctx, d_colors.get(), colors.data(), colors.size()));
+  }
+  DL_TRY(sync(ctx));  // `tables` and `colors` are pageable and local
+  if (d_colors.get()) w->d_grid_colors = std::move(d_colors);
   g.resolution = o.resolution;
   g.insert_free_space = o.insert_free_space;
   // CreateProbabilityGrid (probability_grid_points_processor.cc:150-158): 100 x 100 cells, max = 0.5 * 100 * resolution
   const double max = 0.5 * 100 * o.resolution;
   g.limits = GridLimits{max, max, 100, 100};
-  g.tables = d_tables;
   *stage = (int32_t)w->grids.size();
-  w->grids.push_back(g);
+  w->grids.push_back(std::move(g));
   return DL_OK;
 }
 
@@ -1756,11 +1659,11 @@ int dl_map_writer_probability_grid(const dl_map_writer* w, int32_t stage, dl_map
   const int64_t num_cells = (int64_t)g.limits.nx * g.limits.ny;
   int32_t box[4] = {INT_MAX, INT_MAX, INT_MIN, INT_MIN};
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (g.cells) {
+  if (g.cells.get()) {
     int32_t* d_box = nullptr;
-    MW_TRY(carve_scratch(ctx, [&](Arena& ar) { d_box = ar.take<int32_t>(4); }));
+    DL_TRY(carve_scratch(ctx, [&](Arena& ar) { d_box = ar.take<int32_t>(4); }));
     DL_CUDA(ctx, cudaMemcpyAsync(d_box, box, sizeof(box), cudaMemcpyHostToDevice, ctx->stream));
-    mw_grid_known_box<<<tiles_of(num_cells), kBlock, 0, ctx->stream>>>(g.cells, g.limits.nx, num_cells, d_box);
+    mw_grid_known_box<<<tiles_of(num_cells), kBlock, 0, ctx->stream>>>(g.cells.get(), g.limits.nx, num_cells, d_box);
     DL_LAUNCH_CHECK(ctx, "mw_grid_known_box");
     DL_CUDA(ctx, cudaMemcpyAsync(box, d_box, sizeof(box), cudaMemcpyDeviceToHost, ctx->stream));
     DL_CUDA(ctx, ctx->wait_stream());
@@ -1780,19 +1683,19 @@ int dl_map_writer_probability_grid(const dl_map_writer* w, int32_t stage, dl_map
   if (!cells && !pixels) return DL_OK;
   const int64_t count = (int64_t)r.width * r.height;
   if (capacity < count) return ctx->fail(DL_ERR_ARG, "dl_map_writer_probability_grid: capacity below width * height");
-  if (!g.cells) {  // no batch reached the stage: cell (0, 0) of the initial grid, unknown
+  if (!g.cells.get()) {  // no batch reached the stage: cell (0, 0) of the initial grid, unknown
     if (cells) cells[0] = 0;
     if (pixels) pixels[0] = 128;
     return DL_OK;
   }
   uint16_t* d_cells = nullptr;
   uint8_t* d_pixels = nullptr;
-  MW_TRY(carve_scratch(ctx, [&](Arena& ar) {
+  DL_TRY(carve_scratch(ctx, [&](Arena& ar) {
     d_cells = ar.take<uint16_t>((size_t)count);
     d_pixels = ar.take<uint8_t>((size_t)count);
   }));
-  mw_grid_crop<<<tiles_of(count), kBlock, 0, ctx->stream>>>(g.cells, g.limits.nx, r.offset_x, r.offset_y, r.width, count,
-                                                             w->d_grid_colors, d_cells, d_pixels);
+  mw_grid_crop<<<tiles_of(count), kBlock, 0, ctx->stream>>>(g.cells.get(), g.limits.nx, r.offset_x, r.offset_y, r.width,
+                                                             count, w->d_grid_colors.get(), d_cells, d_pixels);
   DL_LAUNCH_CHECK(ctx, "mw_grid_crop");
   if (cells) DL_CUDA(ctx, cudaMemcpyAsync(cells, d_cells, (size_t)count * sizeof(uint16_t), cudaMemcpyDeviceToHost, ctx->stream));
   if (pixels) DL_CUDA(ctx, cudaMemcpyAsync(pixels, d_pixels, (size_t)count, cudaMemcpyDeviceToHost, ctx->stream));

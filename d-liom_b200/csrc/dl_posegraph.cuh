@@ -147,7 +147,7 @@ struct LmCallbacks {
 inline int run_trust_region(const LmCallbacks& cb, int max_iter, dl_solve_summary* out) {
   const double kMinRelDecrease = 1e-3, kFunctionTol = 1e-6, kGradientTol = 1e-10, kParameterTol = 1e-8, kMinRadius = 1e-32, kMaxRadius = 1e16;
   double cur_cost = 0, gmax = 0, x_norm = 0;
-  DL_TRY_STATUS(cb.initial(&cur_cost, &gmax, &x_norm));
+  DL_TRY(cb.initial(&cur_cost, &gmax, &x_norm));
   dl_solve_summary sum{};
   sum.initial_cost = sum.final_cost = cur_cost;
   sum.termination = 1;
@@ -161,7 +161,7 @@ inline int run_trust_region(const LmCallbacks& cb, int max_iter, dl_solve_summar
       ++sum.num_successful_steps;
       if (cur_cost < minimum_cost) {
         minimum_cost = cur_cost;
-        DL_TRY_STATUS(cb.save_best());
+        DL_TRY(cb.save_best());
       }
     } else {
       ++sum.num_unsuccessful_steps;
@@ -177,7 +177,7 @@ inline int run_trust_region(const LmCallbacks& cb, int max_iter, dl_solve_summar
       ++iteration;
       bool valid = false;
       double mcc = 0;
-      DL_TRY_STATUS(cb.step(radius, reuse_diagonal, first_step, &valid, &mcc));
+      DL_TRY(cb.step(radius, reuse_diagonal, first_step, &valid, &mcc));
       first_step = false;
       reuse_diagonal = true;
       if (valid) {
@@ -197,7 +197,7 @@ inline int run_trust_region(const LmCallbacks& cb, int max_iter, dl_solve_summar
     }
     if (stop) break;
     double cand_cost = 0, step_norm = 0;
-    DL_TRY_STATUS(cb.candidate(&cand_cost, &step_norm));  // candidate cost + speculative normal equations in one pass
+    DL_TRY(cb.candidate(&cand_cost, &step_norm));  // candidate cost + speculative normal equations in one pass
     ++sum.num_evaluations;
     if (!std::isfinite(cand_cost)) cand_cost = 1.7976931348623157e308;
     if (step_norm <= kParameterTol * (x_norm + kParameterTol)) { sum.termination = 0; break; }
@@ -205,7 +205,7 @@ inline int run_trust_region(const LmCallbacks& cb, int max_iter, dl_solve_summar
     const double relative_decrease = (cur_cost - cand_cost) / model_cost_change;  // monotonic steps only (pose_graph.lua)
     if (relative_decrease > kMinRelDecrease) {
       cur_cost = cand_cost;
-      DL_TRY_STATUS(cb.accept(&gmax, &x_norm));
+      DL_TRY(cb.accept(&gmax, &x_norm));
       last_successful = true;
       last_cost = cand_cost;
       const double t = 2.0 * relative_decrease - 1.0;

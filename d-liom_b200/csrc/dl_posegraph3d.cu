@@ -102,8 +102,8 @@ struct dl_pose_graph_3d {
   std::map<Id, std::set<Id>> computed;                   // ConstraintBuilder3D::computed_constraints_: submap -> nodes
   int32_t num_nodes_since_last_loop_closure = 0;
   std::vector<dl_pg3d_search> last_searches;             // of the last add_node call
-  float* d_store = nullptr;                             // node store: xyz floats, each node's high- then low-resolution cloud
-  int64_t store_capacity = 0, store_used = 0;            // in floats
+  DeviceBuffer<float> d_store;                           // node store: xyz floats, each node's high- then low-resolution cloud
+  int64_t store_used = 0;                                // in floats
   int64_t store_live = 0;                                // floats of the nodes still in the graph; the rest of store_used is dead
   int64_t bytes_uploaded = 0;
   std::set<int32_t> finished_trajectories;               // finished_trajectories_
@@ -161,23 +161,11 @@ struct dl_pose_graph_3d {
     return true;
   }
   int reserve_store(int64_t floats) {
-    if (store_used + floats <= store_capacity) return DL_OK;
-    const int64_t cap = std::max<int64_t>({store_used + floats, 2 * store_capacity, (int64_t)1 << 20});
-    float* fresh = nullptr;
+    const int64_t capacity = (int64_t)d_store.cap;
+    if (store_used + floats <= capacity) return DL_OK;
+    const int64_t cap = std::max<int64_t>({store_used + floats, 2 * capacity, (int64_t)1 << 20});
     DL_CUDA(ctx, cudaSetDevice(ctx->device));
-    DL_CUDA(ctx, cudaMalloc(&fresh, (size_t)cap * sizeof(float)));
-    if (store_used > 0) {
-      cudaError_t e = cudaMemcpyAsync(fresh, d_store, (size_t)store_used * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream);
-      if (e == cudaSuccess) e = ctx->wait_stream();
-      if (e != cudaSuccess) {
-        cudaFree(fresh);
-        return ctx->cuda_fail(e, "node store growth");
-      }
-    }
-    if (d_store) cudaFree(d_store);
-    d_store = fresh;
-    store_capacity = cap;
-    return DL_OK;
+    return grow(ctx, d_store, (size_t)cap, (size_t)store_used);
   }
   int optimize(dl_solve_summary* summary);
   int run_trimmers();
@@ -292,8 +280,8 @@ int dl_pose_graph_3d::run_trimmers() {
     if (it != trajectories.end())
       for (const auto& kv : it->second.submaps) ids.push_back(kv.first);
     for (size_t i = 0; i + (size_t)tr.num_submaps_to_keep < ids.size(); ++i) {
-      DL_TRY_STATUS(check_trimmable(tr.trajectory_id, ids[i]));
-      DL_TRY_STATUS(mark_submap_as_trimmed(Id{tr.trajectory_id, ids[i]}));
+      DL_TRY(check_trimmable(tr.trajectory_id, ids[i]));
+      DL_TRY(mark_submap_as_trimmed(Id{tr.trajectory_id, ids[i]}));
     }
   }
   trimmers.erase(std::remove_if(trimmers.begin(), trimmers.end(),
@@ -364,37 +352,25 @@ int dl_pose_graph_3d::compact_store() {
   if (live == 0) {  // nothing left to copy: the store is freed, and the next add_node grows a new one
     DL_CUDA(ctx, cudaSetDevice(ctx->device));
     DL_CUDA(ctx, ctx->wait_stream());
-    cudaFree(d_store);
-    d_store = nullptr;
-    store_capacity = store_used = store_live = 0;
+    d_store.reset();
+    store_used = store_live = 0;
     return DL_OK;
   }
   const int64_t cap = std::max<int64_t>(2 * live, (int64_t)1 << 20);
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_TRY_STATUS(ctx->reserve_device(std::max<size_t>(segments.size(), 1) * sizeof(StoreSegment)));
-  float* fresh = nullptr;
-  cudaError_t e = cudaMalloc(&fresh, (size_t)cap * sizeof(float));
-  if (e != cudaSuccess) {
+  DL_TRY(ctx->reserve_device(std::max<size_t>(segments.size(), 1) * sizeof(StoreSegment)));
+  DeviceBuffer<float> fresh;
+  const int st = alloc(ctx, fresh, (size_t)cap);
+  if (st != DL_OK) {
     cudaGetLastError();  // an allocation failure is not sticky: clear it for the next launch check
-    return ctx->cuda_fail(e, "node store compaction");
+    return st;
   }
-  if (!segments.empty()) {
-    StoreSegment* d_segments = static_cast<StoreSegment*>(ctx->d_scratch);
-    e = cudaMemcpyAsync(d_segments, segments.data(), segments.size() * sizeof(StoreSegment), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) {
-      pg3d_store_compact<<<(unsigned)segments.size(), kCompactBlock, 0, ctx->stream>>>(d_store, fresh, d_segments);
-      ctx->launches++;
-      e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = ctx->wait_stream();
-    if (e != cudaSuccess) {
-      cudaFree(fresh);
-      return ctx->cuda_fail(e, "pg3d_store_compact");
-    }
-  }
-  cudaFree(d_store);
-  d_store = fresh;
-  store_capacity = cap;
+  StoreSegment* d_segments = reinterpret_cast<StoreSegment*>(ctx->d_scratch.get());  // live > 0: segments is not empty
+  DL_TRY(h2d(ctx, d_segments, segments.data(), segments.size()));
+  pg3d_store_compact<<<(unsigned)segments.size(), kCompactBlock, 0, ctx->stream>>>(d_store.get(), fresh.get(), d_segments);
+  DL_LAUNCH_CHECK(ctx, "pg3d_store_compact");
+  DL_CUDA(ctx, ctx->wait_stream());
+  d_store = std::move(fresh);
   store_used = store_live = live;
   size_t k = 0;
   for (auto& [id, t] : trajectories)
@@ -410,7 +386,7 @@ extern "C" {
 int dl_pose_graph_3d_create(dl_context* ctx, const dl_pose_graph_3d_options* options, dl_pose_graph_3d** out) {
   if (!ctx || !options || !out) return DL_ERR_ARG;
   *out = nullptr;
-  DL_TRY_STATUS(check_options(ctx, *options));
+  DL_TRY(check_options(ctx, *options));
   dl_pose_graph_3d* g = new dl_pose_graph_3d;
   g->ctx = ctx;
   g->options = *options;
@@ -420,10 +396,9 @@ int dl_pose_graph_3d_create(dl_context* ctx, const dl_pose_graph_3d_options* opt
 
 void dl_pose_graph_3d_destroy(dl_pose_graph_3d* g) {
   if (!g) return;
-  if (g->d_store) {
+  if (g->d_store.get()) {
     cudaSetDevice(g->ctx->device);
-    cudaStreamSynchronize(g->ctx->stream);
-    cudaFree(g->d_store);
+    g->ctx->wait_stream();
   }
   delete g;
 }
@@ -494,14 +469,12 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
 
   // ---- 2. the node's clouds into the node store (store_used moves on only at the commit below)
   const int64_t n_hi = node->num_high_resolution, n_lo = node->num_low_resolution;
-  DL_TRY_STATUS(g->reserve_store(3 * (n_hi + n_lo)));
+  DL_TRY(g->reserve_store(3 * (n_hi + n_lo)));
   const int64_t hi_begin = g->store_used / 3, lo_begin = hi_begin + n_hi;
   DL_CUDA(ctx, cudaSetDevice(ctx->device));
-  DL_CUDA(ctx, cudaMemcpyAsync(g->d_store + 3 * hi_begin, node->high_resolution_points, (size_t)n_hi * 12, cudaMemcpyHostToDevice,
-                               ctx->stream));
-  DL_CUDA(ctx, cudaMemcpyAsync(g->d_store + 3 * lo_begin, node->low_resolution_points, (size_t)n_lo * 12, cudaMemcpyHostToDevice,
-                               ctx->stream));
-  DL_CUDA(ctx, ctx->wait_stream());  // pageable host memory
+  DL_TRY(h2d(ctx, g->d_store.get() + 3 * hi_begin, node->high_resolution_points, 3 * (size_t)n_hi));
+  DL_TRY(h2d(ctx, g->d_store.get() + 3 * lo_begin, node->low_resolution_points, 3 * (size_t)n_lo));
+  DL_TRY(sync(ctx));  // pageable host memory
   const int64_t uploaded = 12 * (n_hi + n_lo);
 
   // ---- 4. fan-out and searches of a newly finished submap, before anything is committed
@@ -568,12 +541,12 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
       PairClouds pc;
       pc.hi_off = hi_off.data();
       pc.lo_off = lo_off.data();
-      pc.hi_store = g->d_store;
-      pc.lo_store = g->d_store;
+      pc.hi_store = g->d_store.get();
+      pc.lo_store = g->d_store.get();
       pc.hi_begin = hib.data();
       pc.lo_begin = lob.data();
       results.resize(n);
-      DL_TRY_STATUS(constraint_search(ctx, g->options.constraint_builder, n, guesses.data(), pc, hg.data(), lg.data(), results.data()));
+      DL_TRY(constraint_search(ctx, g->options.constraint_builder, n, guesses.data(), pc, hg.data(), lg.data(), results.data()));
       search_ms = ms_since(ts);
     }
   }
@@ -659,7 +632,7 @@ int dl_pose_graph_3d_add_node(dl_pose_graph_3d* g, const dl_pg3d_node* node, int
   double solve_ms = 0.0;
   if (g->options.optimize_every_n_nodes > 0 && g->num_nodes_since_last_loop_closure > g->options.optimize_every_n_nodes) {
     const auto ts = std::chrono::steady_clock::now();
-    DL_TRY_STATUS(g->optimize(&summary));
+    DL_TRY(g->optimize(&summary));
     solve_ms = ms_since(ts);
     optimized = 1;
   }
@@ -749,14 +722,14 @@ int dl_pose_graph_3d_last_searches(const dl_pose_graph_3d* g, int32_t capacity, 
 int dl_pose_graph_3d_store_bytes(const dl_pose_graph_3d* g, int64_t* uploaded, int64_t* capacity) {
   if (!g) return DL_ERR_ARG;
   if (uploaded) *uploaded = g->bytes_uploaded;
-  if (capacity) *capacity = g->store_capacity * (int64_t)sizeof(float);
+  if (capacity) *capacity = (int64_t)g->d_store.cap * (int64_t)sizeof(float);
   return DL_OK;
 }
 
 int dl_pg3d_trim_submap(dl_pose_graph_3d* g, int32_t trajectory_id, int32_t submap_index) {
   if (!g) return DL_ERR_ARG;
   g->last_trimmed.clear();
-  DL_TRY_STATUS(g->check_trimmable(trajectory_id, submap_index));
+  DL_TRY(g->check_trimmable(trajectory_id, submap_index));
   return g->mark_submap_as_trimmed(Id{trajectory_id, submap_index});
 }
 
@@ -825,7 +798,7 @@ int dl_pg3d_store_usage(const dl_pose_graph_3d* g, int64_t* live_bytes, int64_t*
   if (!g) return DL_ERR_ARG;
   if (live_bytes) *live_bytes = g->store_live * (int64_t)sizeof(float);
   if (used_bytes) *used_bytes = g->store_used * (int64_t)sizeof(float);
-  if (capacity_bytes) *capacity_bytes = g->store_capacity * (int64_t)sizeof(float);
+  if (capacity_bytes) *capacity_bytes = (int64_t)g->d_store.cap * (int64_t)sizeof(float);
   return DL_OK;
 }
 

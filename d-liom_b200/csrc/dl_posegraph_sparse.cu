@@ -498,12 +498,6 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     return ctx->fail(DL_ERR_ARG, "pose graph has more submap parameters than the reduced system's one-CTA factor holds (> 3072)");
   cudaError_t e0 = cudaSetDevice(ctx->device);
   if (e0 != cudaSuccess) return ctx->cuda_fail(e0, "cudaSetDevice");
-#define PG_CUDA(call)                                              \
-  do {                                                             \
-    cudaError_t e__ = (call);                                      \
-    if (e__ != cudaSuccess) return ctx->cuda_fail(e__, #call);     \
-  } while (0)
-
   // ---- setup: live constraints first, then those between two frozen poses (fixed cost only)
   std::vector<dl_spa_constraint> cons;
   cons.reserve(num_constraints);
@@ -526,24 +520,21 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   // pair lists padded to the largest count. Every scratch reservation made after the first collective is agreed on by a one-int
   // all-gather of its status, so that a rank that cannot reserve does not leave its peers waiting in the next collective.
   const int world = comm ? dl_comm_world_size(comm) : 1;
-  struct Control {
-    int32_t* d = nullptr;
-    ~Control() { if (d) cudaFree(d); }
-  } control;
+  DeviceBuffer<int32_t> control;
   constexpr int kMeta = 8;
-  if (comm) PG_CUDA(cudaMalloc(&control.d, (size_t)(kMeta + 1) * (world + 1) * sizeof(int32_t)));
-  int32_t* d_meta = control.d;
-  int32_t* d_meta_all = control.d ? control.d + kMeta : nullptr;
-  int32_t* d_st = control.d ? control.d + kMeta * (world + 1) : nullptr;
+  if (comm) DL_TRY(alloc(ctx, control, (size_t)(kMeta + 1) * (world + 1)));
+  int32_t* d_meta = control.get();
+  int32_t* d_meta_all = d_meta ? d_meta + kMeta : nullptr;
+  int32_t* d_st = d_meta ? d_meta + kMeta * (world + 1) : nullptr;
   int32_t* d_st_all = d_st ? d_st + 1 : nullptr;
   auto agree = [&](int st) -> int {  // the first failing rank's status on every rank
     if (!comm) return st;
     const int32_t mine = st;
-    PG_CUDA(cudaMemcpyAsync(d_st, &mine, 4, cudaMemcpyHostToDevice, ctx->stream));
-    DL_TRY_STATUS(dl_comm_all_gather_dev(comm, d_st, d_st_all, 4));
+    DL_CUDA(ctx, cudaMemcpyAsync(d_st, &mine, 4, cudaMemcpyHostToDevice, ctx->stream));
+    DL_TRY(dl_comm_all_gather_dev(comm, d_st, d_st_all, 4));
     std::vector<int32_t> all(world);
-    PG_CUDA(cudaMemcpyAsync(all.data(), d_st_all, 4 * (size_t)world, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(all.data(), d_st_all, 4 * (size_t)world, cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
     setup_bytes += 4 * (int64_t)world;
     if (st != DL_OK) return st;
     for (int r = 0; r < world; ++r)
@@ -555,11 +546,11 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     for (int p = 0; p < P; ++p) hash = (hash ^ (uint32_t)(dim[p] == 0 ? 1 : 0)) * 16777619u;
     const int32_t meta[kMeta] = {(int32_t)local_pairs.size(), n_red, S, N, (int32_t)hash, options->fix_z ? 1 : 0,
                                  options->max_num_iterations, 0};
-    PG_CUDA(cudaMemcpyAsync(d_meta, meta, sizeof(meta), cudaMemcpyHostToDevice, ctx->stream));
-    DL_TRY_STATUS(dl_comm_all_gather_dev(comm, d_meta, d_meta_all, (int64_t)sizeof(meta)));
+    DL_CUDA(ctx, cudaMemcpyAsync(d_meta, meta, sizeof(meta), cudaMemcpyHostToDevice, ctx->stream));
+    DL_TRY(dl_comm_all_gather_dev(comm, d_meta, d_meta_all, (int64_t)sizeof(meta)));
     std::vector<int32_t> all(kMeta * world);
-    PG_CUDA(cudaMemcpyAsync(all.data(), d_meta_all, sizeof(meta) * world, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(all.data(), d_meta_all, sizeof(meta) * world, cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
     setup_bytes += (int64_t)sizeof(meta) * world;
     int most = 0;
     for (int r = 0; r < world; ++r) {
@@ -571,17 +562,17 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     if (most > 0) {
       const size_t per = (size_t)most * sizeof(int2);
       int2 *d_send, *d_recv;
-      DL_TRY_STATUS(agree(carve_scratch(ctx, [&](Arena& a) {
+      DL_TRY(agree(carve_scratch(ctx, [&](Arena& a) {
         d_send = a.take<int2>(most);
         d_recv = a.take<int2>((size_t)most * world);
       })));
       std::vector<int2> send(most, make_int2(-1, -1));
       for (size_t i = 0; i < local_pairs.size(); ++i) send[i] = make_int2(local_pairs[i].first, local_pairs[i].second);
-      PG_CUDA(cudaMemcpyAsync(d_send, send.data(), per, cudaMemcpyHostToDevice, ctx->stream));
-      DL_TRY_STATUS(dl_comm_all_gather_dev(comm, d_send, d_recv, (int64_t)per));
+      DL_CUDA(ctx, cudaMemcpyAsync(d_send, send.data(), per, cudaMemcpyHostToDevice, ctx->stream));
+      DL_TRY(dl_comm_all_gather_dev(comm, d_send, d_recv, (int64_t)per));
       std::vector<int2> recv((size_t)most * world);
-      PG_CUDA(cudaMemcpyAsync(recv.data(), d_recv, per * world, cudaMemcpyDeviceToHost, ctx->stream));
-      PG_CUDA(cudaStreamSynchronize(ctx->stream));
+      DL_CUDA(ctx, cudaMemcpyAsync(recv.data(), d_recv, per * world, cudaMemcpyDeviceToHost, ctx->stream));
+      DL_CUDA(ctx, ctx->wait_stream());
       setup_bytes += (int64_t)per * world;
       pairs.clear();
       for (const int2& v : recv)
@@ -649,7 +640,7 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   dl_spa_constraint* d_c;
   int *d_dim, *d_roff, *d_pose_ptr, *d_pose_con, *d_pair_ptr, *d_pair_con, *d_sub_ptr, *d_node_ptr, *d_node_pairs, *d_blk_ptr;
   int2 *d_pairs, *d_blocks, *d_terms;
-  DL_TRY_STATUS(agree(carve_scratch(ctx, [&](Arena& a) {
+  DL_TRY(agree(carve_scratch(ctx, [&](Arena& a) {
     d_sys[0] = a.take<double>(sys);
     d_sys[1] = a.take<double>(sys);
     d_x = a.take<double>((size_t)7 * P);
@@ -687,27 +678,25 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     d_blk_ptr = a.take<int>(I(blk.ptr.size()));
     d_terms = a.take<int2>(I(terms.size()));
   })));
-  auto up = [&](void* d, const auto& v) {
-    if (!v.empty()) cudaMemcpyAsync(d, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice, ctx->stream);
-  };
-  up(d_pose_ptr, pose_con.ptr);
-  up(d_pose_con, pose_con.idx);
-  up(d_pair_ptr, pair_con.ptr);
-  up(d_pair_con, pair_con.idx);
-  up(d_pairs, pairs2);
-  up(d_sub_ptr, sub_pairs.ptr);
-  up(d_node_ptr, node_pairs.ptr);
-  up(d_node_pairs, node_pairs.idx);
-  up(d_blocks, blocks);
-  up(d_blk_ptr, blk.ptr);
-  up(d_terms, terms);
-  PG_CUDA(cudaMemcpyAsync(d_dim, dim.data(), (size_t)P * 4, cudaMemcpyHostToDevice, ctx->stream));
-  PG_CUDA(cudaMemcpyAsync(d_roff, roff.data(), (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
-  PG_CUDA(cudaMemcpyAsync(d_x, poses, (size_t)P * 56, cudaMemcpyHostToDevice, ctx->stream));
-  PG_CUDA(cudaMemcpyAsync(d_best, poses, (size_t)P * 56, cudaMemcpyHostToDevice, ctx->stream));
+  auto up = [&](auto* d, const auto& v) { return h2d(ctx, d, v.data(), v.size()); };
+  DL_TRY(up(d_pose_ptr, pose_con.ptr));
+  DL_TRY(up(d_pose_con, pose_con.idx));
+  DL_TRY(up(d_pair_ptr, pair_con.ptr));
+  DL_TRY(up(d_pair_con, pair_con.idx));
+  DL_TRY(up(d_pairs, pairs2));
+  DL_TRY(up(d_sub_ptr, sub_pairs.ptr));
+  DL_TRY(up(d_node_ptr, node_pairs.ptr));
+  DL_TRY(up(d_node_pairs, node_pairs.idx));
+  DL_TRY(up(d_blocks, blocks));
+  DL_TRY(up(d_blk_ptr, blk.ptr));
+  DL_TRY(up(d_terms, terms));
+  DL_CUDA(ctx, cudaMemcpyAsync(d_dim, dim.data(), (size_t)P * 4, cudaMemcpyHostToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(d_roff, roff.data(), (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(d_x, poses, (size_t)P * 56, cudaMemcpyHostToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(d_best, poses, (size_t)P * 56, cudaMemcpyHostToDevice, ctx->stream));
   if (!cons.empty())
-    PG_CUDA(cudaMemcpyAsync(d_c, cons.data(), cons.size() * sizeof(dl_spa_constraint), cudaMemcpyHostToDevice, ctx->stream));
-  PG_CUDA(cudaGetLastError());
+    DL_CUDA(ctx, cudaMemcpyAsync(d_c, cons.data(), cons.size() * sizeof(dl_spa_constraint), cudaMemcpyHostToDevice, ctx->stream));
+  DL_CUDA(ctx, cudaGetLastError());
   const SparseGraph gr{S, N, tdof, d_dim, d_roff, n_red};
   // the constraints between frozen poses: their cost once
   if (F > 0) {
@@ -734,10 +723,10 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     sp_cost_kernel<<<1, 256, 0, ctx->stream>>>(d_c2, M, d_misc, d_sys[buf]);
     DL_LAUNCH_CHECK(ctx, "sp_cost_kernel");
     if (comm) {
-      PG_CUDA(cudaEventRecord(ev0, ctx->stream));
-      DL_TRY_STATUS(dl_comm_all_reduce_f64_dev(comm, d_sys[buf], (int64_t)sys));
-      PG_CUDA(cudaEventRecord(ev1, ctx->stream));
-      PG_CUDA(cudaEventSynchronize(ev1));
+      DL_CUDA(ctx, cudaEventRecord(ev0, ctx->stream));
+      DL_TRY(dl_comm_all_reduce_f64_dev(comm, d_sys[buf], (int64_t)sys));
+      DL_CUDA(ctx, cudaEventRecord(ev1, ctx->stream));
+      DL_CUDA(ctx, cudaEventSynchronize(ev1));
       float ms = 0.f;
       cudaEventElapsedTime(&ms, ev0, ev1);
       reduce_ms += ms;
@@ -749,8 +738,8 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   double fixed_cost = 0;
   auto cost_of = [&](int buf, double* c) -> int {
     double c2[2];
-    PG_CUDA(cudaMemcpyAsync(c2, d_sys[buf], 16, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(c2, d_sys[buf], 16, cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
     *c = 0.5 * c2[0];
     fixed_cost = 0.5 * c2[1];
     return DL_OK;
@@ -758,8 +747,8 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   auto norms = [&](const double* x, const double* y, double* o) -> int {
     sp_norms_kernel<<<1, 256, 0, ctx->stream>>>(P, d_dim, x, y, d_misc + 1);
     DL_LAUNCH_CHECK(ctx, "sp_norms_kernel");
-    PG_CUDA(cudaMemcpyAsync(o, d_misc + 1, 24, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    DL_CUDA(ctx, cudaMemcpyAsync(o, d_misc + 1, 24, cudaMemcpyDeviceToHost, ctx->stream));
+    DL_CUDA(ctx, ctx->wait_stream());
     return DL_OK;
   };
   // projected gradient max norm at (at, system buf): || at - Plus(at, -g) ||_max, and ||at||
@@ -767,7 +756,7 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     sp_plus_kernel<<<(P + 127) / 128, 128, 0, ctx->stream>>>(P, d_dim, at, d_sys[buf], 2, -1.0, d_tmp);
     DL_LAUNCH_CHECK(ctx, "sp_plus_kernel");
     double o[3];
-    DL_TRY_STATUS(norms(at, d_tmp, o));
+    DL_TRY(norms(at, d_tmp, o));
     *gmax = o[0];
     *xnorm = o[1];
     return DL_OK;
@@ -775,26 +764,26 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   int cur = 0;
   dl_solve_summary sum{};
   if (n_local == 0) {  // nothing to optimise: Ceres reports the fixed cost and converges without iterating
-    DL_TRY_STATUS(evaluate(d_x, cur));
+    DL_TRY(evaluate(d_x, cur));
     double c = 0;
-    DL_TRY_STATUS(cost_of(cur, &c));
+    DL_TRY(cost_of(cur, &c));
     sum.initial_cost = sum.final_cost = c + fixed_cost;
     sum.termination = 0;
     sum.num_evaluations = 1;
   } else {
     LmCallbacks cb;
     cb.initial = [&](double* cost, double* gmax, double* x_norm) -> int {
-      DL_TRY_STATUS(evaluate(d_x, cur));
-      DL_TRY_STATUS(cost_of(cur, cost));
+      DL_TRY(evaluate(d_x, cur));
+      DL_TRY(cost_of(cur, cost));
       return gradient_norms(d_x, cur, gmax, x_norm);
     };
     cb.save_best = [&]() -> int {
-      PG_CUDA(cudaMemcpyAsync(d_best, d_x, (size_t)P * 56, cudaMemcpyDeviceToDevice, ctx->stream));
+      DL_CUDA(ctx, cudaMemcpyAsync(d_best, d_x, (size_t)P * 56, cudaMemcpyDeviceToDevice, ctx->stream));
       return DL_OK;
     };
     cb.step = [&](double radius, bool reuse_diagonal, bool first_step, bool* valid, double* model_cost_change) -> int {
       const double sc[3] = {radius, reuse_diagonal ? 1. : 0., first_step ? 1. : 0.};
-      PG_CUDA(cudaMemcpyAsync(sb.scalars, sc, 24, cudaMemcpyHostToDevice, ctx->stream));
+      DL_CUDA(ctx, cudaMemcpyAsync(sb.scalars, sc, 24, cudaMemcpyHostToDevice, ctx->stream));
       sb.sys = d_sys[cur];
       sp_scale_kernel<<<(6 * P + 127) / 128, 128, 0, ctx->stream>>>(pl, d_dim, sb);
       DL_LAUNCH_CHECK(ctx, "sp_scale_kernel");
@@ -807,7 +796,7 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
         DL_LAUNCH_CHECK(ctx, "sp_pair_kernel");
       }
       if (R > 0) {
-        PG_CUDA(cudaMemsetAsync(sb.A, 0, (size_t)n_red * n_red * 8, ctx->stream));
+        DL_CUDA(ctx, cudaMemsetAsync(sb.A, 0, (size_t)n_red * n_red * 8, ctx->stream));
         sp_reduce_kernel<<<R, 64, 0, ctx->stream>>>(pl, S, d_dim, d_roff, n_red, d_blocks, d_blk_ptr, d_terms, d_pairs, d_sub_ptr, sb);
         DL_LAUNCH_CHECK(ctx, "sp_reduce_kernel");
         sp_reduced_solve_kernel<<<1, 1024, 0, ctx->stream>>>(n_red, sb);
@@ -818,8 +807,8 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
       sp_finish_kernel<<<1, 256, 0, ctx->stream>>>(P, sb);
       DL_LAUNCH_CHECK(ctx, "sp_finish_kernel");
       double outv[2];
-      PG_CUDA(cudaMemcpyAsync(outv, sb.scalars + 3, 16, cudaMemcpyDeviceToHost, ctx->stream));
-      PG_CUDA(cudaStreamSynchronize(ctx->stream));
+      DL_CUDA(ctx, cudaMemcpyAsync(outv, sb.scalars + 3, 16, cudaMemcpyDeviceToHost, ctx->stream));
+      DL_CUDA(ctx, ctx->wait_stream());
       *valid = outv[0] != 0.;
       *model_cost_change = outv[1];
       return DL_OK;
@@ -827,10 +816,10 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     cb.candidate = [&](double* cand_cost, double* step_norm) -> int {
       sp_plus_kernel<<<(P + 127) / 128, 128, 0, ctx->stream>>>(P, d_dim, d_x, sb.delta, 0, 1.0, d_cand);
       DL_LAUNCH_CHECK(ctx, "sp_plus_kernel");
-      DL_TRY_STATUS(evaluate(d_cand, cur ^ 1));
-      DL_TRY_STATUS(cost_of(cur ^ 1, cand_cost));
+      DL_TRY(evaluate(d_cand, cur ^ 1));
+      DL_TRY(cost_of(cur ^ 1, cand_cost));
       double o[3];
-      DL_TRY_STATUS(norms(d_x, d_cand, o));
+      DL_TRY(norms(d_x, d_cand, o));
       *step_norm = o[2];
       return DL_OK;
     };
@@ -839,15 +828,15 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
       cur ^= 1;
       return gradient_norms(d_x, cur, gmax, x_norm);
     };
-    DL_TRY_STATUS(run_trust_region(cb, options->max_num_iterations, &sum));
+    DL_TRY(run_trust_region(cb, options->max_num_iterations, &sum));
     // Ceres 1.13 reports x_cost + fixed_cost; its tolerances above saw x_cost only
     sum.initial_cost += fixed_cost;
     sum.final_cost += fixed_cost;
   }
   cudaEventDestroy(ev0);
   cudaEventDestroy(ev1);
-  PG_CUDA(cudaMemcpyAsync(poses, d_best, (size_t)P * 56, cudaMemcpyDeviceToHost, ctx->stream));
-  PG_CUDA(cudaStreamSynchronize(ctx->stream));
+  DL_CUDA(ctx, cudaMemcpyAsync(poses, d_best, (size_t)P * 56, cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, ctx->wait_stream());
   if (summary) *summary = sum;
   if (info) {
     info->num_local_parameters = n_local;
@@ -859,6 +848,5 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     info->num_pairs = K;
     info->setup_exchange_bytes = setup_bytes;
   }
-#undef PG_CUDA
   return DL_OK;
 }

@@ -192,20 +192,6 @@ Rigidf projection_transform(const Rigidd& pose) {
   return compose(to_float(inverse_yaw), rotation);
 }
 
-// The call's scratch bytes in use so far are preserved when it has to grow (reserve_device would drop them).
-int reserve_device_keeping(dl_context* ctx, size_t bytes, size_t keep) {
-  if (bytes <= ctx->d_scratch_bytes) return DL_OK;
-  const size_t want = bytes + bytes / 4;
-  void* fresh = nullptr;
-  DL_CUDA(ctx, cudaMalloc(&fresh, want));
-  if (keep) DL_CUDA(ctx, cudaMemcpyAsync(fresh, ctx->d_scratch, keep, cudaMemcpyDeviceToDevice, ctx->stream));
-  DL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  DL_CUDA(ctx, cudaFree(ctx->d_scratch));
-  ctx->d_scratch = fresh;
-  ctx->d_scratch_bytes = want;
-  return DL_OK;
-}
-
 int bits_for(int64_t n) {  // least b >= 1 with n <= 2^b
   int b = 1;
   while (((int64_t)1 << b) < n) ++b;
@@ -225,7 +211,7 @@ int submap_images(dl_context* ctx, int mode, int32_t count, const dl_submap_imag
   for (int k = 0; k < count; ++k) {
     const dl_grid* g = queries[k].grid;
     if (!g) return ctx->fail(DL_ERR_ARG, "submap image query without a grid");
-    if (g->structure_dirty || !g->d_counters) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+    if (g->structure_dirty || !g->d_counters.get()) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
     if (g->ctx->device != ctx->device) return ctx->fail(DL_ERR_ARG, "submap image query of a grid on another device");
   }
   // the pinned block below holds a submitted front-end batch's staged results until dl_frontend_collect
@@ -237,10 +223,10 @@ int submap_images(dl_context* ctx, int mode, int32_t count, const dl_submap_imag
   StageScope stage(ctx, mode == kTexture ? "submap_textures" : "submap_projections");
 
   // 1. the pools' sizes: a grid the device inserter grew is ahead of its host mirror
-  DL_TRY_STATUS(ctx->reserve_pinned((size_t)count * 8 * sizeof(int32_t)));
-  int32_t* h_words = (int32_t*)ctx->h_pinned;
+  DL_TRY(ctx->reserve_pinned((size_t)count * 8 * sizeof(int32_t)));
+  int32_t* h_words = (int32_t*)ctx->h_pinned.get();
   for (int k = 0; k < count; ++k)
-    DL_CUDA(ctx, cudaMemcpyAsync(h_words + 2 * k, queries[k].grid->d_counters, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost,
+    DL_CUDA(ctx, cudaMemcpyAsync(h_words + 2 * k, queries[k].grid->d_counters.get(), 2 * sizeof(int32_t), cudaMemcpyDeviceToHost,
                                  ctx->stream));
   DL_CUDA(ctx, ctx->wait_stream());
   std::vector<ImageQuery> qs(count);
@@ -292,7 +278,7 @@ int submap_images(dl_context* ctx, int mode, int32_t count, const dl_submap_imag
   };
   Arena counted_a(nullptr);  // the bytes phase 4 must keep
   carve_a(counted_a);
-  DL_TRY_STATUS(carve_scratch(ctx, carve_a));
+  DL_TRY(carve_scratch(ctx, carve_a));
   DL_CUDA(ctx, cudaMemcpyAsync(d_qs, qs.data(), count * sizeof(ImageQuery), cudaMemcpyHostToDevice, ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(d_node_top, 0xFF, std::max<int64_t>(nodes, 1) * sizeof(int32_t), ctx->stream));
   DL_CUDA(ctx, cudaMemsetAsync(d_keys_in, 0xFF, (size_t)num_bricks * sizeof(uint64_t), ctx->stream));
@@ -370,8 +356,9 @@ int submap_images(dl_context* ctx, int mode, int32_t count, const dl_submap_imag
   };
   Arena counted_b(nullptr);
   carve_b(counted_b);
-  DL_TRY_STATUS(reserve_device_keeping(ctx, counted_b.off, counted_a.off));
-  Arena arena(ctx->d_scratch);
+  // the call's scratch bytes in use so far are kept when it has to grow (reserve_device would drop them)
+  if (counted_b.off > ctx->d_scratch.cap) DL_TRY(grow(ctx, ctx->d_scratch, counted_b.off + counted_b.off / 4, counted_a.off));
+  Arena arena(ctx->d_scratch.get());
   carve_b(arena);
   DL_CUDA(ctx, cudaMemcpyAsync(d_qs, qs.data(), count * sizeof(ImageQuery), cudaMemcpyHostToDevice, ctx->stream));
   image_cells_kernel<true><<<num_bricks, 512, 0, ctx->stream>>>(d_qs, d_keys, d_bricks, mode, nullptr, nullptr, d_brick_first,

@@ -1,8 +1,8 @@
 """Device block-sparse pose adjustment (csrc/dl_posegraph_sparse.cu, dl_pose_graph_solve_sparse; reference
 OptimizationProblem3D::Solve, optimization_problem_3d.cc:259-589) against the dense oracle (oracle/orc_posegraph.h, pinned to the
 reference's ReducesNoise test) and the block-sparse CPU oracle (tests/schur_oracle.py): same LM trajectory (iterations,
-termination), poses to 1e-8 on small graphs and 1e-6 at trajectory scale; frozen poses; run-to-run bit identity; the all-reduce
-bookkeeping; argument errors."""
+termination), poses to 1e-8 on small graphs and 1e-6 at trajectory scale; frozen poses; run-to-run bit identity, also with
+blocking host waits; the all-reduce bookkeeping; argument errors."""
 import os
 import subprocess
 import sys
@@ -131,6 +131,15 @@ def test_bit_identical_runs_and_world_of_one(ctx):
     P, K = len(submaps) + len(nodes), info.num_pairs
     assert info.all_reduce_bytes == 8 * (2 + 42 * P + 36 * K)
     assert info.setup_exchange_bytes == 32 + 4 + 4 + 8 * K    # meta, two agreed reservations, the pair list
+    blocking = dliom.Context(0)
+    blocking.set_blocking_sync(True)    # every host wait of the solve sleeps on an event instead of spinning
+    comm = dliom.Comm(blocking, dliom.comm_unique_id(), 0, 1)
+    d = blocking.pose_graph_solve_sparse(submaps, nodes, cons)
+    e = blocking.pose_graph_solve_sparse(submaps, nodes, cons, comm=comm)
+    comm.close()
+    blocking.close()
+    for r in (d, e):
+        assert np.array_equal(a[0], r[0]) and np.array_equal(a[1], r[1]) and a[2] == r[2]
 
 
 def test_argument_errors_before_any_collective(ctx):
