@@ -479,6 +479,10 @@ int launch_window_optimize(dl_context* ctx, int count, const dl_nav_state* state
                            const dl_preintegration* preint, const double* matched_pose, const dl_nav_state* initial_j,
                            const dl_window_options& opt, dl_nav_state* states_i_out, dl_nav_state* states_j_out,
                            double* information_out, dl_solve_summary* summaries);
+constexpr int kWindowEvalDoubles = 38 + 38 * 30 + 38 * 38;  // per problem: residual, Jacobian, weight
+int launch_window_evaluate(dl_context* ctx, int count, const dl_nav_state* states_i, const double* prior_information,
+                           const dl_preintegration* preint, const double* matched_pose, const dl_window_options& opt, const double* x,
+                           int32_t* ok, double* out);
 // dl_histogram.cu
 struct HistogramScratch {  // device scratch of one rotational histogram of n points
   unsigned long long* keys;

@@ -13,12 +13,17 @@
 //                                 rows are the bias random walk between the two keys
 //              pose prior on x_j: the matched pose, diagonal sigmas (translation, rotation)
 //              optional gravity prior on x_j's roll / pitch (gravity_factor.cc:10-31): the body-frame reference direction must
-//                                 map to the estimated gravity direction
-//   solve      Gauss-Newton on the 30 x 30 normal equations (Jacobians by forward-mode duals: one code path for every factor),
+//                                 map to the estimated gravity direction. Both are directions: the host refuses a zero or
+//                                 non-finite one and normalises both (Unit3 does the same), so their lengths do not enter
+//   solve     Gauss-Newton on the 30 x 30 normal equations (Jacobians by forward-mode duals: one code path for every factor),
 //              then the Schur complement on x_i gives the information of x_j = the prior of the next step
 //   difference from GTSAM, stated: GTSAM's PreintegratedImuMeasurements / ImuFactor integrate on the manifold with a 9-dim
 //              residual and a separate bias BetweenFactor; the integrator here is the reference's own IntegrationBase. Neither
 //              library is in this image, so the row's parity is pinned oracle <-> device only (DESIGN.md).
+//   difference from gravity_factor.cc, stated: the reference rotates b_ref by x_j's roll and pitch only (Rot3::RzRyRx(r.x, r.y, 0),
+//              :20, :25) and adds k_cost_value = 1e-5 to both error components (:12, :27-28); here b_ref is rotated by the whole
+//              R_j and the residual has no offset.
+// dl_window_evaluate runs window_weights and window_residuals alone at given (x_i, x_j), so the factors can be checked on their own.
 // One warp per trajectory: lane 0 forms the residuals and their duals, the 32 lanes share the 30 x 30 linear algebra.
 #include "dl_internal.cuh"
 
@@ -209,16 +214,15 @@ __device__ void window_residuals(const WindowArgs& a, int b, WindowShared& sh) {
     if (e.w.a < 0.) e = {-1.0 * e.w, -1.0 * e.x, -1.0 * e.y, -1.0 * e.z};
     store(2.0 * e.x, sh, 33); store(2.0 * e.y, sh, 34); store(2.0 * e.z, sh, 35);
   }
-  // ---- gravity direction on x_j: R_j * b_ref should point along g_dir (both unit); residual = the two components of R_j b_ref
-  //      orthogonal to g_dir in a fixed basis of its tangent plane (the role of Unit3::error in gravity_factor.cc:10-31)
+  // ---- gravity direction on x_j: R_j * b_ref should point along g_dir (both unit: the host normalised them, as Unit3 does);
+  //      residual = the two components of R_j b_ref orthogonal to g_dir in a fixed basis of its tangent plane (the role of
+  //      Unit3::error in gravity_factor.cc:10-31)
   if (a.opt.use_gravity_factor) {
     const double* gd = a.opt.gravity_direction;
     const double* br = a.opt.body_reference_direction;
     const DV n = dqrotate(sj.q, DV{dc(br[0]), dc(br[1]), dc(br[2])});
     // basis of the plane orthogonal to gd
-    Vec3d g{gd[0], gd[1], gd[2]};
-    const double gn = norm3(g);
-    g = mul(1.0 / gn, g);
+    const Vec3d g{gd[0], gd[1], gd[2]};
     const Vec3d helper = fabs(g.x) < 0.9 ? Vec3d{1, 0, 0} : Vec3d{0, 1, 0};
     Vec3d b1 = cross3(g, helper);
     b1 = mul(1.0 / norm3(b1), b1);
@@ -263,15 +267,10 @@ __device__ void warp_solve(double (*L)[kVars], int n, double* x /* rhs in, solut
 
 constexpr int kWarpsPerBlock = 2;
 
-__global__ void __launch_bounds__(kWarpsPerBlock * 32) window_optimize_kernel(WindowArgs a) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  WindowShared* all = reinterpret_cast<WindowShared*>(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.x * kWarpsPerBlock + warp;
-  if (b >= a.count) return;
-  WindowShared& sh = all[warp];
+// The block-diagonal weight of problem b into sh.W (whole warp): prior information, imu_weight^2 covariance^-1, the pose prior's and
+// the gravity factor's 1 / sigma^2. Returns (uniform) false when the covariance is not positive definite; the IMU block is then 0.
+__device__ bool window_weights(const WindowArgs& a, int b, WindowShared& sh, int lane) {
   const dl_preintegration& m = a.preint[b];
-  // weights
   for (int e = lane; e < kRes * kRes; e += 32) sh.W[e / kRes][e % kRes] = 0.;
   __syncwarp();
   for (int e = lane; e < 225; e += 32) sh.W[e / 15][e % 15] = a.prior_information[(size_t)b * 225 + e];
@@ -295,6 +294,20 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) window_optimize_kernel(Wi
     for (int k = 0; k < 3; ++k) { sh.W[30 + k][30 + k] = wt; sh.W[33 + k][33 + k] = wr; }
     const double wg = a.opt.use_gravity_factor ? 1.0 / (a.opt.gravity_sigma * a.opt.gravity_sigma) : 0.;
     sh.W[36][36] = sh.W[37][37] = wg;
+  }
+  return ok;
+}
+
+__global__ void __launch_bounds__(kWarpsPerBlock * 32) window_optimize_kernel(WindowArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  WindowShared* all = reinterpret_cast<WindowShared*>(smem);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x * kWarpsPerBlock + warp;
+  if (b >= a.count) return;
+  WindowShared& sh = all[warp];
+  const dl_preintegration& m = a.preint[b];
+  bool ok = window_weights(a, b, sh, lane);
+  if (lane == 0) {
     nav_to16(a.states_i[b], sh.xi);
     if (a.initial_j) {
       nav_to16(a.initial_j[b], sh.xj);
@@ -411,7 +424,41 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) window_optimize_kernel(Wi
   }
 }
 
+// The factors alone at given (x_i, x_j) (dl_window_evaluate): the weight and residual code of window_optimize_kernel, written out.
+// x: 32 doubles per problem (x_i then x_j, p q v ba bg each); out: kWindowEvalDoubles per problem, r (38), J (38 x 30), W (38 x 38).
+__global__ void __launch_bounds__(kWarpsPerBlock * 32) window_evaluate_kernel(WindowArgs a, const double* __restrict__ x,
+                                                                              int32_t* __restrict__ ok_out, double* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  WindowShared* all = reinterpret_cast<WindowShared*>(smem);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x * kWarpsPerBlock + warp;
+  if (b >= a.count) return;
+  WindowShared& sh = all[warp];
+  const bool ok = window_weights(a, b, sh, lane);
+  if (lane < 16) { sh.xi[lane] = x[(size_t)b * 32 + lane]; sh.xj[lane] = x[(size_t)b * 32 + 16 + lane]; }
+  __syncwarp();
+  if (ok && lane == 0) window_residuals(a, b, sh);
+  __syncwarp();
+  double* o = out + (size_t)b * kWindowEvalDoubles;
+  for (int e = lane; e < kRes; e += 32) o[e] = ok ? sh.r[e] : 0.;
+  for (int e = lane; e < kRes * kVars; e += 32) o[kRes + e] = ok ? sh.J[e / kVars][e % kVars] : 0.;
+  for (int e = lane; e < kRes * kRes; e += 32) o[kRes + kRes * kVars + e] = ok ? sh.W[e / kRes][e % kRes] : 0.;
+  if (lane == 0) ok_out[b] = ok ? 1 : 0;
+}
+
 }  // namespace
+
+int launch_window_evaluate(dl_context* ctx, int count, const dl_nav_state* states_i, const double* prior_information,
+                           const dl_preintegration* preint, const double* matched_pose, const dl_window_options& opt, const double* x,
+                           int32_t* ok, double* out) {
+  if (count <= 0) return DL_OK;
+  WindowArgs a{count, states_i, prior_information, preint, matched_pose, nullptr, opt, nullptr, nullptr, nullptr, nullptr};
+  const size_t smem = sizeof(WindowShared) * kWarpsPerBlock;
+  DL_CUDA(ctx, cudaFuncSetAttribute(window_evaluate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  window_evaluate_kernel<<<(count + kWarpsPerBlock - 1) / kWarpsPerBlock, kWarpsPerBlock * 32, smem, ctx->stream>>>(a, x, ok, out);
+  DL_LAUNCH_CHECK(ctx, "window_evaluate_kernel");
+  return DL_OK;
+}
 
 int launch_window_optimize(dl_context* ctx, int count, const dl_nav_state* states_i, const double* prior_information,
                            const dl_preintegration* preint, const double* matched_pose, const dl_nav_state* initial_j,

@@ -34,7 +34,7 @@ EXPORTS = [
     "dl_frontend_collect_imu",
     "dl_comm_unique_id", "dl_comm_create", "dl_comm_destroy", "dl_comm_rank", "dl_comm_world_size", "dl_comm_last_error",
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
-    "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
+    "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_window_evaluate", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
     "dl_ltb_add_range_data_batch", "dl_ltb_release_submap",
     "dl_pose_graph_3d_create", "dl_pose_graph_3d_destroy", "dl_pose_graph_3d_add_node", "dl_pose_graph_3d_freeze_trajectory",
@@ -546,6 +546,7 @@ def lib():
     L.dl_constraint_search_exchange.argtypes = [vp, vp, ip(ConstraintOptions), C.c_int32, C.c_int32, i32p, i32p, f64p, f32p, i64p,
                                                 f32p, i64p, C.c_void_p, C.c_void_p, ip(ConstraintRow), ip(ExchangeInfo)]
     L.dl_window_optimize_batch.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, vp, f64p, vp]
+    L.dl_window_evaluate.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, i32p, f64p, f64p, f64p]
     L.dl_pose_graph_solve_sparse.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, vp, C.c_int32,
                                              ip(SolveSummary), ip(PoseGraphSparseInfo)]
     L.dl_pose_graph_3d_create.argtypes = [vp, ip(PoseGraph3DOptions), ip(vp)]
@@ -882,14 +883,12 @@ class Context:
         return run
 
     def window_optimize_batch(self, means_i, prior_infos, preints, matched_poses, sigma_t=0.05, sigma_r=0.01, imu_weight=1.0,
-                              gravity=(0.0, 0.0, 9.8), max_iter=10, gravity_factor=None, initial_j=None):
+                              gravity=(0.0, 0.0, 9.8), max_iter=10, gravity_factor=None, initial_j=None, states_i_out=True):
         """WindowOptimize's stand-in (dl_window_optimize_batch) for len(means_i) trajectories. means_i / initial_j: 16-vectors;
-        prior_infos: (n, 15, 15); preints: ctypes Preintegration objects. -> (states_i smoothed, states_j, informations, summaries)."""
+        prior_infos: (n, 15, 15); preints: ctypes Preintegration objects. -> (states_i smoothed, states_j, informations, summaries);
+        states_i_out=False passes NULL for the smoothed previous keys and returns None in their place."""
         n = len(means_i)
-        opt = WindowOptions(sigma_t, sigma_r, imu_weight, (C.c_double * 3)(*gravity), int(max_iter), 1 if gravity_factor else 0,
-                            float(gravity_factor[0]) if gravity_factor else 1.0,
-                            (C.c_double * 3)(*(gravity_factor[1] if gravity_factor else (0, 0, 1))),
-                            (C.c_double * 3)(*(gravity_factor[2] if gravity_factor else (0, 0, 1))))
+        opt = self._window_options(sigma_t, sigma_r, imu_weight, gravity, max_iter, gravity_factor)
         si = (NavState * n)(*[NavState.from16(x) for x in means_i])
         pm = (Preintegration * n)(*preints)
         init = (NavState * n)(*[NavState.from16(x) for x in initial_j]) if initial_j is not None else None
@@ -899,9 +898,36 @@ class Context:
         self.check(self.L.dl_window_optimize_batch(self.h, C.byref(opt), n, C.cast(si, C.c_void_p),
                                                    np.ascontiguousarray(prior_infos, np.float64).reshape(-1), C.cast(pm, C.c_void_p),
                                                    np.ascontiguousarray(matched_poses, np.float64).reshape(-1),
-                                                   C.cast(init, C.c_void_p) if init is not None else None, C.cast(out_i, C.c_void_p),
+                                                   C.cast(init, C.c_void_p) if init is not None else None,
+                                                   C.cast(out_i, C.c_void_p) if states_i_out else None,
                                                    C.cast(out_j, C.c_void_p), info.reshape(-1), C.cast(sums, C.c_void_p)))
-        return (np.array([o.to16() for o in out_i]), np.array([o.to16() for o in out_j]), info, [s.as_dict() for s in sums])
+        return (np.array([o.to16() for o in out_i]) if states_i_out else None, np.array([o.to16() for o in out_j]), info,
+                [s.as_dict() for s in sums])
+
+    @staticmethod
+    def _window_options(sigma_t, sigma_r, imu_weight, gravity, max_iter, gravity_factor):
+        return WindowOptions(sigma_t, sigma_r, imu_weight, (C.c_double * 3)(*gravity), int(max_iter), 1 if gravity_factor else 0,
+                             float(gravity_factor[0]) if gravity_factor else 1.0,
+                             (C.c_double * 3)(*(gravity_factor[1] if gravity_factor else (0, 0, 1))),
+                             (C.c_double * 3)(*(gravity_factor[2] if gravity_factor else (0, 0, 1))))
+
+    def window_evaluate(self, means_i, prior_infos, preints, matched_poses, x_i, x_j, sigma_t=0.05, sigma_r=0.01, imu_weight=1.0,
+                        gravity=(0.0, 0.0, 9.8), gravity_factor=None):
+        """The window's factors at given (x_i, x_j) (dl_window_evaluate); arguments as window_optimize_batch, x_i / x_j: 16-vectors.
+        -> dict of ok [n], residual [n,38], jacobian [n,38,30], weight [n,38,38]."""
+        n = len(means_i)
+        opt = self._window_options(sigma_t, sigma_r, imu_weight, gravity, 10, gravity_factor)
+        si = (NavState * n)(*[NavState.from16(x) for x in means_i])
+        pm = (Preintegration * n)(*preints)
+        xi = (NavState * n)(*[NavState.from16(x) for x in x_i])
+        xj = (NavState * n)(*[NavState.from16(x) for x in x_j])
+        ok = np.zeros(n, np.int32)
+        r, J, W = np.zeros((n, 38)), np.zeros((n, 38, 30)), np.zeros((n, 38, 38))
+        self.check(self.L.dl_window_evaluate(self.h, C.byref(opt), n, C.cast(si, C.c_void_p),
+                                             np.ascontiguousarray(prior_infos, np.float64).reshape(-1), C.cast(pm, C.c_void_p),
+                                             np.ascontiguousarray(matched_poses, np.float64).reshape(-1), C.cast(xi, C.c_void_p),
+                                             C.cast(xj, C.c_void_p), ok, r.reshape(-1), J.reshape(-1), W.reshape(-1)))
+        return {"ok": ok, "residual": r, "jacobian": J, "weight": W}
 
     def pose_graph_solve_sparse(self, submap_poses, node_poses, constraints, fix_z=False, max_iter=50, comm=None, frozen=None):
         """OptimizationProblem3D::Solve (SPA only) on the device, block-sparse (Schur complement of the node blocks), for whole

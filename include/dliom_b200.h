@@ -611,9 +611,13 @@ typedef struct dl_window_options {
   int32_t max_num_iterations;    /* Gauss-Newton iterations (10 when 0) */
   int32_t use_gravity_factor;
   double gravity_sigma;          /* imu_options.prior_gravity_noise */
-  double gravity_direction[3];   /* estimated up direction in the local frame (g_vec_est_G_ normalised) */
+  double gravity_direction[3];   /* estimated up direction in the local frame (g_vec_est_G_) */
   double body_reference_direction[3]; /* the reference direction in the body frame that should map to it */
 } dl_window_options;
+/* gravity_direction and body_reference_direction are directions: with use_gravity_factor set, a zero or non-finite one is
+ * DL_ERR_ARG and both are normalised before use (as gtsam::Unit3 does), so their lengths do not change the result. The factor
+ * differs from gravity_factor.cc in two stated ways: b_ref is rotated by the whole R_j, not by its roll and pitch only
+ * (Rot3::RzRyRx(r.x, r.y, 0)), and the residual carries no k_cost_value = 1e-5 offset. */
 /* `count` independent trajectories. prior_information: 225 doubles each (row-major 15 x 15). matched_poses: 7 each.
  * initial_states_j may be NULL (start from the IMU prediction). states_i_out (optional) receives the smoothed previous keys.
  * summaries[k].termination: 0 converged, 1 iteration limit, 2 a covariance / system was not positive definite (no output). */
@@ -621,6 +625,16 @@ int dl_window_optimize_batch(dl_context* ctx, const dl_window_options* options, 
                              const double* prior_information, const dl_preintegration* preintegrations, const double* matched_poses,
                              const dl_nav_state* initial_states_j, dl_nav_state* states_i_out, dl_nav_state* states_j_out,
                              double* information_out, dl_solve_summary* summaries);
+/* The window's factors alone, for kernel-level checks: for `count` problems (arguments as dl_window_optimize_batch) evaluated at
+ * the given (x_i[k], x_j[k]) — x_i need not be the prior mean states_i[k]. Outputs per problem: ok (0: the IMU covariance is not
+ * positive definite, every other output of the problem is zero), residuals (38: 15 prior, 15 IMU, 6 pose, 2 gravity; the gravity
+ * rows are 0 without the factor), jacobians (38 x 30 row-major, d r / d (delta_i, delta_j) in the tangent order and chart above)
+ * and weights (38 x 38 row-major, block diagonal: prior information, imu_weight^2 covariance^-1, 1 / sigma^2 of the pose and
+ * gravity rows). The solve minimises 1/2 r^T W r. */
+int dl_window_evaluate(dl_context* ctx, const dl_window_options* options, int32_t count, const dl_nav_state* states_i,
+                       const double* prior_information, const dl_preintegration* preintegrations, const double* matched_poses,
+                       const dl_nav_state* x_i, const dl_nav_state* x_j, int32_t* ok, double* residuals, double* jacobians,
+                       double* weights);
 
 /* ---- the per-scan front end of LocalTrajectoryBuilder3D::AddRangeData / AddAccumulatedRangeData
  *      (LTB:393-554): voxel filter -> deskew/transform/range gate -> voxel filter -> adaptive filters ->

@@ -85,10 +85,8 @@ inline void window_residuals(const WindowOptions& o, const double* mean_i, const
   // gravity direction
   r[36] = r[37] = 0;
   if (o.use_gravity_factor) {
-    const V3d n = rotate(qj, o.body_reference_direction);
-    const double gn = std::sqrt(o.gravity_direction.x * o.gravity_direction.x + o.gravity_direction.y * o.gravity_direction.y +
-                                o.gravity_direction.z * o.gravity_direction.z);
-    const V3d g = scale(1.0 / gn, o.gravity_direction);
+    const V3d n = rotate(qj, o.body_reference_direction);   // both directions unit (window_optimize normalised them)
+    const V3d& g = o.gravity_direction;
     const V3d helper = std::fabs(g.x) < 0.9 ? V3d{1, 0, 0} : V3d{0, 1, 0};
     auto cross = [](const V3d& a, const V3d& b) { return V3d{a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; };
     V3d b1 = cross(g, helper);
@@ -99,11 +97,20 @@ inline void window_residuals(const WindowOptions& o, const double* mean_i, const
   }
 }
 
-// Returns false if a matrix is not positive definite. xi_out / xj_out: 16 doubles; info_out: 225.
-inline bool window_optimize(const WindowOptions& o, const double* mean_i, const double* prior_info, const Preintegration& m,
+// Returns false if a matrix is not positive definite or, with the gravity factor on, a direction is zero or not finite.
+// xi_out / xj_out: 16 doubles; info_out: 225.
+inline bool window_optimize(const WindowOptions& o_in, const double* mean_i, const double* prior_info, const Preintegration& m,
                             const Rigid3d& matched, const double* initial_j, double* xi_out, double* xj_out, double* info_out,
                             int* iterations_out, double* initial_cost_out, double* final_cost_out, int* termination_out) {
+  WindowOptions o = o_in;
   constexpr int R = 38, N = 30;
+  if (o_in.use_gravity_factor) {  // both are directions (Unit3): only their orientation enters the factor
+    for (V3d* d : {&o.gravity_direction, &o.body_reference_direction}) {
+      const double n = std::sqrt(d->x * d->x + d->y * d->y + d->z * d->z);
+      if (!std::isfinite(n) || !(n > 0.)) return false;
+      *d = scale(1.0 / n, *d);
+    }
+  }
   std::vector<double> W((size_t)R * R, 0.0);
   for (int a = 0; a < 15; ++a)
     for (int b = 0; b < 15; ++b) W[(size_t)a * R + b] = prior_info[a * 15 + b];
