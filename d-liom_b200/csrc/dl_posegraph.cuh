@@ -130,7 +130,9 @@ __device__ inline void cta_cholesky_solve(const double* U, int n, double* y) {
 }
 
 // ---- Ceres 1.13 TrustRegionMinimizer as pose_graph.lua runs it (LM, monotonic steps), scalars on the host. The solver keeps the
-// current point, the candidate and the best point; the driver only sees costs, norms and the step's validity.
+// current point, the candidate and the best point; the driver only sees costs, norms and the step's validity. The minimised
+// program holds the parameters of the poses that are neither frozen nor unreferenced (no constraint refers to them), so x, ||x||
+// and the parameter tolerance built from it cover those poses only.
 struct LmCallbacks {
   // evaluate at the starting point: cost (the minimised program's: fixed cost excluded), projected-gradient max norm, ||x||
   std::function<int(double* cost, double* gradient_max_norm, double* x_norm)> initial;

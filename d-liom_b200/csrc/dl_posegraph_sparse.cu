@@ -8,7 +8,8 @@
 // Cholesky; the node steps follow by back-substitution. In exact arithmetic this is the LM step of the dense normal equations,
 // as the oracle (oracle/orc_posegraph.h) takes it.
 //
-// Every pose owns a 6-slot block; its first dim(p) slots are live: 0 if frozen (Ceres removes constant blocks), 2 for the first
+// Every pose owns a 6-slot block; its first dim(p) slots are live: 0 if frozen or if no constraint (on any rank) refers to it
+// (Ceres's Program::RemoveFixedBlocks removes constant and unused blocks, so neither moves nor enters ||x||), 2 for the first
 // submap (constant translation, ConstantYawQuaternionPlus), else 3 + tdof (fix_z: tdof = 2). Dead slots carry zeros in the
 // Jacobian and an identity in the damped node blocks, so that they leave the live entries of every factor bit-unchanged.
 //
@@ -487,27 +488,25 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   for (int k = 0; k < num_constraints; ++k)
     if (constraints[k].submap < 0 || constraints[k].submap >= S || constraints[k].node < 0 || constraints[k].node >= N)
       return ctx->fail(DL_ERR_ARG, "constraint refers to a submap / node outside the graph");
-  std::vector<int> dim(P), roff(S);
-  int n_red = 0, n_local = 0;
-  for (int p = 0; p < P; ++p) {
-    dim[p] = (frozen && frozen[p]) ? 0 : p == 0 ? 2 : 3 + tdof;
-    if (p < S) { roff[p] = n_red; n_red += dim[p]; }
-    n_local += dim[p];
-  }
-  if (n_red > kMaxReduced)
+  auto is_frozen = [&](int p) { return frozen && frozen[p]; };
+  // The reduced system's limit holds for every submap that is not frozen, referenced or not, so that every rank can check it
+  // before the first collective (which submaps the constraints refer to is only known after the exchange).
+  int submap_capacity = 0;
+  for (int s = 0; s < S; ++s) submap_capacity += is_frozen(s) ? 0 : s == 0 ? 2 : 3 + tdof;
+  if (submap_capacity > kMaxReduced)
     return ctx->fail(DL_ERR_ARG, "pose graph has more submap parameters than the reduced system's one-CTA factor holds (> 3072)");
   cudaError_t e0 = cudaSetDevice(ctx->device);
   if (e0 != cudaSuccess) return ctx->cuda_fail(e0, "cudaSetDevice");
-  // ---- setup: live constraints first, then those between two frozen poses (fixed cost only)
+  // ---- setup: live constraints (not between two frozen poses) first, then those between two frozen poses (fixed cost only)
   std::vector<dl_spa_constraint> cons;
   cons.reserve(num_constraints);
   for (int pass = 0; pass < 2; ++pass)
     for (int k = 0; k < num_constraints; ++k) {
-      const bool live = dim[constraints[k].submap] + dim[S + constraints[k].node] > 0;
+      const bool live = !(is_frozen(constraints[k].submap) && is_frozen(S + constraints[k].node));
       if (live == (pass == 0)) cons.push_back(constraints[k]);
     }
   int M = 0;
-  while (M < (int)cons.size() && dim[cons[M].submap] + dim[S + cons[M].node] > 0) ++M;
+  while (M < (int)cons.size() && !(is_frozen(cons[M].submap) && is_frozen(S + cons[M].node))) ++M;
   const int F = (int)cons.size() - M;
   std::vector<std::pair<int, int>> local_pairs(M);
   for (int i = 0; i < M; ++i) local_pairs[i] = {cons[i].submap, cons[i].node};
@@ -516,9 +515,10 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   std::vector<std::pair<int, int>> pairs = local_pairs;
   int64_t setup_bytes = 0;
   // With a communicator every rank must take the same path through the collectives below. The set-up exchange: (pair count,
-  // reduced size, S, N, hash of the frozen mask, fix_z, max_num_iterations) from every rank, checked on every rank alike; then the
-  // pair lists padded to the largest count. Every scratch reservation made after the first collective is agreed on by a one-int
-  // all-gather of its status, so that a rank that cannot reserve does not leave its peers waiting in the next collective.
+  // non-frozen submap parameters, S, N, hash of the frozen flags, fix_z, max_num_iterations) from every rank, checked on every rank
+  // alike; then the pair lists padded to the largest count. Every scratch reservation made after the first collective is agreed on
+  // by a one-int all-gather of its status, so that a rank that cannot reserve does not leave its peers waiting in the next
+  // collective.
   const int world = comm ? dl_comm_world_size(comm) : 1;
   DeviceBuffer<int32_t> control;
   constexpr int kMeta = 8;
@@ -543,8 +543,8 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
   };
   if (comm) {
     uint32_t hash = 2166136261u;  // FNV-1a over the frozen flags
-    for (int p = 0; p < P; ++p) hash = (hash ^ (uint32_t)(dim[p] == 0 ? 1 : 0)) * 16777619u;
-    const int32_t meta[kMeta] = {(int32_t)local_pairs.size(), n_red, S, N, (int32_t)hash, options->fix_z ? 1 : 0,
+    for (int p = 0; p < P; ++p) hash = (hash ^ (uint32_t)(is_frozen(p) ? 1 : 0)) * 16777619u;
+    const int32_t meta[kMeta] = {(int32_t)local_pairs.size(), submap_capacity, S, N, (int32_t)hash, options->fix_z ? 1 : 0,
                                  options->max_num_iterations, 0};
     DL_CUDA(ctx, cudaMemcpyAsync(d_meta, meta, sizeof(meta), cudaMemcpyHostToDevice, ctx->stream));
     DL_TRY(dl_comm_all_gather_dev(comm, d_meta, d_meta_all, (int64_t)sizeof(meta)));
@@ -580,6 +580,19 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
       std::sort(pairs.begin(), pairs.end());
       pairs.erase(std::unique(pairs.begin(), pairs.end()), pairs.end());
     }
+  }
+  // A pose that no constraint refers to is not in Ceres's minimised program (Program::RemoveFixedBlocks drops unused parameter
+  // blocks as well as constant ones): like a frozen pose it gets no parameters, so it neither moves nor enters ||x||. A pose that
+  // is not frozen and is referenced on some rank sits in a live constraint there, so it is in the pair list every rank now holds:
+  // the pairs decide, and every rank forms the same dims without another exchange.
+  std::vector<uint8_t> used(P, 0);
+  for (const auto& pr : pairs) used[pr.first] = used[S + pr.second] = 1;
+  std::vector<int> dim(P), roff(S);
+  int n_red = 0, n_local = 0;
+  for (int p = 0; p < P; ++p) {
+    dim[p] = (is_frozen(p) || !used[p]) ? 0 : p == 0 ? 2 : 3 + tdof;
+    if (p < S) { roff[p] = n_red; n_red += dim[p]; }
+    n_local += dim[p];
   }
   const int K = (int)pairs.size();
   std::vector<int> con_pair(M);
@@ -849,4 +862,43 @@ extern "C" int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const 
     info->setup_exchange_bytes = setup_bytes;
   }
   return DL_OK;
+}
+
+// The factors alone: each constraint's residual and local Jacobian at the given poses, from sp_evaluate_kernel as the solve
+// launches it. Every pose of a constraint is referenced, so its dim is 0 if frozen, 2 for the first submap, else 3 + tdof.
+extern "C" int dl_pose_graph_evaluate(dl_context* ctx, const dl_pose_graph_options* options, int32_t num_submaps, int32_t num_nodes,
+                                      const double* poses, const uint8_t* frozen, const dl_spa_constraint* constraints,
+                                      int32_t num_constraints, double* residuals, double* jacobians) {
+  if (!ctx || !options || num_submaps < 1 || num_nodes < 0 || !poses || num_constraints < 0 ||
+      (num_constraints > 0 && (!constraints || !residuals || !jacobians)))
+    return DL_ERR_ARG;
+  const int S = num_submaps, N = num_nodes, P = S + N, M = num_constraints, tdof = options->fix_z ? 2 : 3;
+  for (int k = 0; k < M; ++k)
+    if (constraints[k].submap < 0 || constraints[k].submap >= S || constraints[k].node < 0 || constraints[k].node >= N)
+      return ctx->fail(DL_ERR_ARG, "constraint refers to a submap / node outside the graph");
+  if (M == 0) return DL_OK;
+  std::vector<int> dim(P);
+  for (int p = 0; p < P; ++p) dim[p] = (frozen && frozen[p]) ? 0 : p == 0 ? 2 : 3 + tdof;
+  cudaError_t e0 = cudaSetDevice(ctx->device);
+  if (e0 != cudaSuccess) return ctx->cuda_fail(e0, "cudaSetDevice");
+  double *d_x, *d_J, *d_e, *d_c2;
+  dl_spa_constraint* d_c;
+  int* d_dim;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_x = a.take<double>((size_t)7 * P);
+    d_J = a.take<double>((size_t)M * 72);
+    d_e = a.take<double>((size_t)M * 6);
+    d_c2 = a.take<double>((size_t)M);
+    d_c = a.take<dl_spa_constraint>((size_t)M);
+    d_dim = a.take<int>((size_t)P);
+  }));
+  DL_TRY(h2d(ctx, d_x, poses, (size_t)7 * P));
+  DL_TRY(h2d(ctx, d_c, constraints, (size_t)M));
+  DL_TRY(h2d(ctx, d_dim, dim.data(), (size_t)P));
+  const SparseGraph gr{S, N, tdof, d_dim, nullptr, 0};
+  sp_evaluate_kernel<<<(M + 63) / 64, 64, 0, ctx->stream>>>(gr, d_x, d_c, M, 1, d_J, d_e, d_c2);
+  DL_LAUNCH_CHECK(ctx, "sp_evaluate_kernel");
+  DL_TRY(d2h(ctx, residuals, d_e, (size_t)M * 6));
+  DL_TRY(d2h(ctx, jacobians, d_J, (size_t)M * 72));
+  return sync(ctx);
 }

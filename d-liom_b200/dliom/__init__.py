@@ -34,7 +34,7 @@ EXPORTS = [
     "dl_frontend_collect_imu",
     "dl_comm_unique_id", "dl_comm_create", "dl_comm_destroy", "dl_comm_rank", "dl_comm_world_size", "dl_comm_last_error",
     "dl_comm_all_gather_dev", "dl_comm_all_reduce_f64_dev", "dl_comm_broadcast_dev", "dl_constraint_search_exchange",
-    "dl_pose_graph_solve_sparse", "dl_window_optimize_batch", "dl_window_evaluate", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
+    "dl_pose_graph_solve_sparse", "dl_pose_graph_evaluate", "dl_window_optimize_batch", "dl_window_evaluate", "dl_rotational_histogram", "dl_ltb_create", "dl_ltb_destroy", "dl_ltb_set_initial_state", "dl_ltb_add_imu_data",
     "dl_ltb_add_range_data", "dl_ltb_add_synchronized_range_data", "dl_ltb_get_cloud", "dl_ltb_get_histogram", "dl_ltb_num_submaps", "dl_ltb_get_submap", "dl_ltb_get_state",
     "dl_ltb_add_range_data_batch", "dl_ltb_release_submap",
     "dl_pose_graph_3d_create", "dl_pose_graph_3d_destroy", "dl_pose_graph_3d_add_node", "dl_pose_graph_3d_freeze_trajectory",
@@ -547,6 +547,7 @@ def lib():
                                                 f32p, i64p, C.c_void_p, C.c_void_p, ip(ConstraintRow), ip(ExchangeInfo)]
     L.dl_window_optimize_batch.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, vp, f64p, vp]
     L.dl_window_evaluate.argtypes = [vp, ip(WindowOptions), C.c_int32, vp, f64p, vp, f64p, vp, vp, i32p, f64p, f64p, f64p]
+    L.dl_pose_graph_evaluate.argtypes = [vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, vp, C.c_int32, f64p, f64p]
     L.dl_pose_graph_solve_sparse.argtypes = [vp, vp, ip(PoseGraphOptions), C.c_int32, C.c_int32, f64p, vp, vp, C.c_int32,
                                              ip(SolveSummary), ip(PoseGraphSparseInfo)]
     L.dl_pose_graph_3d_create.argtypes = [vp, ip(PoseGraph3DOptions), ip(vp)]
@@ -949,6 +950,22 @@ class Context:
                                                      fz.ctypes.data if fz is not None else None, C.cast(cs, C.c_void_p),
                                                      len(constraints), C.byref(s), C.byref(info)))
         return poses[:S].copy(), poses[S:].copy(), s.as_dict(), info
+
+    def pose_graph_evaluate(self, submap_poses, node_poses, constraints, fix_z=False, frozen=None):
+        """The solve's factors at given poses (dl_pose_graph_evaluate); arguments as pose_graph_solve_sparse.
+        -> (residuals [m, 6], local Jacobians [m, 6, 12]: submap slots 0..5, node slots 6..11)."""
+        S, N, m = len(submap_poses), len(node_poses), len(constraints)
+        poses = np.ascontiguousarray(np.concatenate([np.asarray(submap_poses, np.float64).reshape(S, 7),
+                                                     np.asarray(node_poses, np.float64).reshape(N, 7)]))
+        cs = spa_constraints(constraints)
+        fz = None if frozen is None else np.ascontiguousarray(np.asarray(frozen, bool).astype(np.uint8).reshape(-1))
+        if fz is not None and len(fz) != S + N:
+            raise ValueError(f"frozen has {len(fz)} flags, the graph {S + N} poses")
+        r, J = np.zeros((m, 6)), np.zeros((m, 6, 12))
+        self.check(self.L.dl_pose_graph_evaluate(self.h, C.byref(PoseGraphOptions(50, int(bool(fix_z)))), S, N, poses,
+                                                 fz.ctypes.data if fz is not None else None, C.cast(cs, C.c_void_p), m,
+                                                 r.reshape(-1), J.reshape(-1)))
+        return r, J
 
     @staticmethod
     def _pairs(clouds, grids):

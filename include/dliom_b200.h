@@ -330,13 +330,17 @@ int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_const
  *      frozen: num_submaps + num_nodes flags (NULL = none); a frozen pose is constant (OptimizationProblem3D::Solve's
  *      frozen_trajectories, optimization_problem_3d.cc:283-329): it has no parameters, and if it is the first submap its rotation
  *      is constant too. Constraints between two frozen poses only add a fixed cost: initial_cost / final_cost include it (as
- *      Ceres 1.13 reports them) while the tolerances see the rest. With every pose frozen the poses come back unchanged,
+ *      Ceres 1.13 reports them) while the tolerances see the rest. A pose that no constraint refers to (on any rank) is left out
+ *      of the minimised program like a frozen one (Ceres removes unused parameter blocks): it comes back unchanged and does not
+ *      enter ||x||, so it does not widen the parameter tolerance. The ranks learn which poses are referenced from the pair lists
+ *      they exchange anyway (a pose that is not frozen and is referenced sits in a live constraint). With no parameters left the poses come back unchanged,
  *      termination CONVERGENCE, no iterations.
  *      Deterministic: no floating-point atomics; two calls on the same input return bit-identical poses, and with a communicator
  *      every rank does identical work after the all-reduce.
  *      Errors (DL_ERR_ARG, all detected before the first collective except the last, which every rank detects together after the
- *      set-up all-gather): an index outside the graph; more than DL_POSE_GRAPH_MAX_REDUCED submap parameters; a graph whose
- *      submap / node counts, frozen poses, reduced size, fix_z or iteration limit differ between the ranks. A device-memory
+ *      set-up all-gather): an index outside the graph; more than DL_POSE_GRAPH_MAX_REDUCED parameters over the submaps that are
+ *      not frozen (referenced or not: which submaps the constraints refer to is only known after the exchange); a graph whose
+ *      submap / node counts, frozen poses, fix_z or iteration limit differ between the ranks. A device-memory
  *      reservation made after the first collective is agreed on by all ranks (a one-int all-gather), so every rank returns the
  *      same failure instead of one leaving its peers waiting. ------------------------------------------------------------- */
 typedef struct dl_spa_constraint { /* PoseGraphInterface::Constraint: node j observed from submap i */
@@ -350,12 +354,12 @@ typedef struct dl_pose_graph_options {
 } dl_pose_graph_options;
 #define DL_POSE_GRAPH_MAX_REDUCED 3072
 typedef struct dl_pose_graph_sparse_info {
-  int32_t num_local_parameters;   /* live parameters of all poses */
+  int32_t num_local_parameters;   /* live parameters of all poses (neither frozen nor unreferenced) */
   int32_t all_reduce_count;       /* one per evaluation */
   int64_t all_reduce_bytes;       /* per all-reduce: 8 * (2 + 42 * (num_submaps + num_nodes) + 36 * num_pairs) */
   float all_reduce_ms;            /* summed device time of the all-reduces (CUDA events) */
   float all_reduce_min_ms;        /* fastest single all-reduce */
-  int32_t num_reduced_parameters; /* size of the factored system: the live parameters of the submaps */
+  int32_t num_reduced_parameters; /* size of the factored system: the live parameters of the submaps (unreferenced ones have none) */
   int32_t num_pairs;              /* distinct (submap, node) pairs with a constraint not between two frozen poses, all ranks */
   int64_t setup_exchange_bytes;   /* received by this rank in the set-up all-gathers (0 without a communicator):
                                      world * (32 + 4), plus world * (4 + 8 * largest per-rank pair count) if any rank has pairs */
@@ -363,6 +367,13 @@ typedef struct dl_pose_graph_sparse_info {
 int dl_pose_graph_solve_sparse(dl_context* ctx, dl_comm* comm, const dl_pose_graph_options* options, int32_t num_submaps,
                                int32_t num_nodes, double* poses, const uint8_t* frozen, const dl_spa_constraint* constraints,
                                int32_t num_constraints, dl_solve_summary* summary, dl_pose_graph_sparse_info* info);
+/* The factors of dl_pose_graph_solve_sparse alone, at the given poses (same layout, frozen flags and fix_z; options'
+ * max_num_iterations is not read): for each constraint its residual (6, into residuals[6 k ..]) and its Jacobian in the local
+ * parameters (6 x 12 row-major into jacobians[72 k ..]: columns 0..5 the submap's, 6..11 the node's slots, the first dim of
+ * each live and the rest zero; dim = 0 frozen, 2 the first submap (ConstantYawQuaternionPlus), else 3 + (fix_z ? 2 : 3)). */
+int dl_pose_graph_evaluate(dl_context* ctx, const dl_pose_graph_options* options, int32_t num_submaps, int32_t num_nodes,
+                           const double* poses, const uint8_t* frozen, const dl_spa_constraint* constraints, int32_t num_constraints,
+                           double* residuals, double* jacobians);
 
 /* ---- mapping::PoseGraph3D (C/mapping/internal/3d/pose_graph_3d.cc) on the fork's live loop-closure path: the object between the
  *      local trajectory builder and the optimizer. dl_pose_graph_3d_add_node restates, synchronously and in this order:

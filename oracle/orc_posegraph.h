@@ -114,25 +114,38 @@ inline void spa_residual(const SpaConstraint& c, const T* qi, const T* ti, const
   for (int k = 0; k < 3; ++k) e[3 + k] = aa[k] * c.rotation_weight;
 }
 
-// The problem orc_nls.h's solve_trust_region drives. Ambient layout: submap 0 rotation (4) [its translation is constant and
-// lives outside], then for submaps 1.. and all nodes: rotation (4), translation (3).
+// The problem orc_nls.h's solve_trust_region drives. Only the poses some constraint refers to are in it: Ceres 1.13's
+// Program::RemoveFixedBlocks drops parameter blocks no residual uses, so an unreferenced pose has no parameters, keeps its start
+// value and does not enter ||x||. Ambient layout over the referenced poses in order: submap 0 rotation (4) [its translation is
+// constant and lives outside], every other pose rotation (4), translation (3).
 class PoseGraphProblem {
  public:
   PoseGraphProblem(int num_submaps, int num_nodes, const V3d& first_submap_translation, std::vector<SpaConstraint> constraints,
                    bool fix_z)
-      : S_(num_submaps), N_(num_nodes), t0_(first_submap_translation), constraints_(std::move(constraints)), fix_z_(fix_z) {}
+      : S_(num_submaps), N_(num_nodes), t0_(first_submap_translation), constraints_(std::move(constraints)), fix_z_(fix_z) {
+    used_.assign(S_ + N_, false);
+    for (const SpaConstraint& c : constraints_) used_[c.submap] = used_[pose_of_node(c.node)] = true;
+    amb_.assign(S_ + N_ + 1, 0);
+    loc_.assign(S_ + N_ + 1, 0);
+    for (int p = 0; p < S_ + N_; ++p) {
+      amb_[p + 1] = amb_[p] + (!used_[p] ? 0 : p == 0 ? 4 : 7);
+      loc_[p + 1] = loc_[p] + (!used_[p] ? 0 : p == 0 ? 2 : 3 + translation_dof());
+    }
+  }
 
   int num_residuals() const { return 6 * (int)constraints_.size(); }
-  int num_ambient() const { return 4 + 7 * (S_ + N_ - 1); }
+  int num_ambient() const { return amb_[S_ + N_]; }
   int translation_dof() const { return fix_z_ ? 2 : 3; }
-  int num_local() const { return 2 + (3 + translation_dof()) * (S_ + N_ - 1); }
-  int rotation_offset(int pose) const { return pose == 0 ? 0 : 4 + 7 * (pose - 1); }             // ambient
-  int translation_offset(int pose) const { return 4 + 7 * (pose - 1) + 4; }                        // ambient, pose > 0
-  int local_offset(int pose) const { return pose == 0 ? 0 : 2 + (3 + translation_dof()) * (pose - 1); }
+  int num_local() const { return loc_[S_ + N_]; }
+  bool used(int pose) const { return used_[pose]; }
+  int rotation_offset(int pose) const { return amb_[pose]; }                                      // ambient
+  int translation_offset(int pose) const { return amb_[pose] + 4; }                               // ambient, pose > 0
+  int local_offset(int pose) const { return loc_[pose]; }
   int pose_of_node(int node) const { return S_ + node; }
 
   void Plus(const double* x, const double* delta, double* out) const {
     for (int p = 0; p < S_ + N_; ++p) {
+      if (!used_[p]) continue;
       const double* q = x + rotation_offset(p);
       const double* d = delta + local_offset(p);
       double* o = out + rotation_offset(p);
@@ -209,6 +222,8 @@ class PoseGraphProblem {
   V3d t0_;
   std::vector<SpaConstraint> constraints_;
   bool fix_z_;
+  std::vector<bool> used_;
+  std::vector<int> amb_, loc_;  // per pose: ambient / local offsets (prefix sums over the referenced poses)
 };
 
 // OptimizationProblem3D::Solve for the SPA-only problem. poses: S submaps then N nodes, 7 doubles each (t xyz, q wxyz), in-out.
@@ -218,6 +233,7 @@ inline void solve_pose_graph(int num_submaps, int num_nodes, double* poses7, con
   PoseGraphProblem problem(num_submaps, num_nodes, V3d{poses7[0], poses7[1], poses7[2]}, constraints, fix_z);
   std::vector<double> x(problem.num_ambient());
   for (int p = 0; p < num_submaps + num_nodes; ++p) {
+    if (!problem.used(p)) continue;
     const double* s = poses7 + 7 * p;
     double* q = x.data() + problem.rotation_offset(p);
     q[0] = s[3]; q[1] = s[4]; q[2] = s[5]; q[3] = s[6];
@@ -228,6 +244,7 @@ inline void solve_pose_graph(int num_submaps, int num_nodes, double* poses7, con
   }
   solve_trust_region(problem, /*use_nonmonotonic_steps=*/false, max_num_iterations, x.data(), summary, linear_solver);
   for (int p = 0; p < num_submaps + num_nodes; ++p) {
+    if (!problem.used(p)) continue;  // not in the program: unchanged
     double* s = poses7 + 7 * p;
     const double* q = x.data() + problem.rotation_offset(p);
     s[3] = q[0]; s[4] = q[1]; s[5] = q[2]; s[6] = q[3];

@@ -8,7 +8,9 @@ of the number of poses, so it checks the device's sparse solve at sizes the dens
 
 Also the frozen poses of OptimizationProblem3D::Solve's frozen_trajectories (optimization_problem_3d.cc:283-329), restating
 Ceres 1.13 from memory, as orc_nls.h does: constant parameter blocks are removed from the minimised program (a frozen first submap
-loses its rotation parameters too); residual blocks whose parameters are all constant leave it and only add a fixed cost;
+loses its rotation parameters too), and so are the blocks of a pose no constraint refers to (Program::RemoveFixedBlocks drops
+unused blocks: such a pose keeps its value and stays out of ||x||); residual blocks whose parameters are all constant leave it
+and only add a fixed cost;
 Summary::initial_cost / final_cost are reported as x_cost + fixed_cost, while the function tolerance sees x_cost; with no
 parameters left the solve returns at once with CONVERGENCE.
 
@@ -36,7 +38,10 @@ class SchurPoseGraph:
         self.P = len(poses7)
         tdof = 2 if fix_z else 3
         fr = np.zeros(self.P, bool) if frozen is None else np.asarray(frozen, bool)
-        self.dim = np.array([0 if fr[p] else (2 if p == 0 else 3 + tdof) for p in range(self.P)])
+        used = np.zeros(self.P, bool)
+        for c in constraints:
+            used[c[0]] = used[num_submaps + c[1]] = True
+        self.dim = np.array([0 if fr[p] or not used[p] else (2 if p == 0 else 3 + tdof) for p in range(self.P)])
         self.roff = np.concatenate([[0], np.cumsum(self.dim[:self.S])])
         self.n_red = int(self.roff[-1])
         live = [c for c in constraints if self.dim[c[0]] + self.dim[self.S + c[1]] > 0]

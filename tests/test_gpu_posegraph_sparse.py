@@ -142,7 +142,9 @@ def test_bit_identical_runs_and_world_of_one(ctx):
         assert np.array_equal(a[0], r[0]) and np.array_equal(a[1], r[1]) and a[2] == r[2]
 
 
-def test_argument_errors_before_any_collective(ctx):
+def test_argument_errors_and_what_the_reduced_size_counts(ctx):
+    """Errors before any collective; the reduced system's limit counts every submap that is not frozen, while the factored size
+    (num_reduced_parameters) counts only the submaps some constraint refers to."""
     import dliom
     with pytest.raises(dliom.DlError) as e:
         ctx.pose_graph_solve_sparse([IDENT], [IDENT], [(0, 3, IDENT, 1.0, 1.0)])                # node outside the graph
@@ -154,8 +156,16 @@ def test_argument_errors_before_any_collective(ctx):
     with pytest.raises(dliom.DlError) as e:
         ctx.pose_graph_solve_sparse([IDENT] * 600, [IDENT], [], comm=comm)                     # 2 + 6 * 599 > 3072
     assert e.value.status == -2 and "3072" in str(e.value)
-    assert ctx.pose_graph_solve_sparse([IDENT] * 600, [IDENT], [], comm=comm,                  # frozen submaps do not count
+    with pytest.raises(dliom.DlError) as e:
+        ctx.pose_graph_solve_sparse([IDENT] * 600, [IDENT], [])                                # also without a communicator
+    assert e.value.status == -2 and "3072" in str(e.value)
+    every = [(k, 0, IDENT, 1.0, 1.0) for k in range(600)]                                   # every submap referenced
+    assert ctx.pose_graph_solve_sparse([IDENT] * 600, [IDENT], every, comm=comm,               # frozen submaps do not count
                                        frozen=[False] * 100 + [True] * 501)[3].num_reduced_parameters == 2 + 6 * 99
+    assert ctx.pose_graph_solve_sparse([IDENT] * 600, [IDENT], every[:100], comm=comm,         # nor unreferenced ones in the
+                                       frozen=[False] * 100 + [True] * 501)[3].num_reduced_parameters == 2 + 6 * 99
+    assert ctx.pose_graph_solve_sparse([IDENT] * 600, [IDENT], every[:50], comm=comm,          # factored system
+                                       frozen=[False] * 100 + [True] * 501)[3].num_reduced_parameters == 2 + 6 * 49
     comm.close()
 
 
