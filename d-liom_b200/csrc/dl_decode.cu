@@ -7,6 +7,8 @@
 // HBM-bound byte work: reads point_step bytes per point (22-48 for the drivers the reference knows) twice, writes 16 per
 // kept point. Fields may sit at any byte offset (the velodyne driver packs its point into 22 bytes), so they are assembled
 // from bytes unless the layout is 4-byte aligned.
+#include <cstdint>
+
 #include "dl_internal.cuh"
 
 namespace dl {
@@ -140,3 +142,77 @@ int launch_decode_point_cloud2(dl_context* ctx, const DecodeArgs& a) {
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ decode
+using namespace dl;
+
+namespace {
+int decode_common(dl_context* ctx, const dl_point_cloud2_layout* l, const void* data_host, const void* data_dev, int64_t n,
+                  const double* sensor_to_tracking, float* rows_host, float* rows_dev, int64_t* num_rows_out,
+                  double* stamp_offset_seconds) {
+  if (!ctx || !l || !sensor_to_tracking || !num_rows_out || !stamp_offset_seconds || n < 0 || n >= (1ll << 31)) return DL_ERR_ARG;
+  const int time_bytes = l->time_type == DL_TIME_FLOAT64_SECONDS ? 8 : (l->time_type == DL_TIME_NONE ? 0 : 4);
+  if (l->time_type < DL_TIME_NONE || l->time_type > DL_TIME_FLOAT64_SECONDS) return ctx->fail(DL_ERR_ARG, "unknown time_type");
+  if (l->point_step < 12 || l->offset_x < 0 || l->offset_y < 0 || l->offset_z < 0 || l->offset_x + 4 > l->point_step ||
+      l->offset_y + 4 > l->point_step || l->offset_z + 4 > l->point_step ||
+      (time_bytes && (l->offset_time < 0 || l->offset_time + time_bytes > l->point_step)))
+    return ctx->fail(DL_ERR_ARG, "field offsets do not fit point_step");
+  *num_rows_out = 0;
+  *stamp_offset_seconds = 0.;
+  if (n == 0) return DL_OK;
+  if ((!data_host && !data_dev) || (!rows_host && !rows_dev)) return DL_ERR_ARG;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t bytes = (size_t)n * l->point_step;
+  const size_t tiles = (size_t)((n + 255) / 256);
+  DecodeArgs d{};
+  uint8_t* up = nullptr;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    if (data_host) up = a.take<uint8_t>(bytes);
+    d.rows_out = rows_host ? a.take<float>((size_t)n * 4) : rows_dev;
+    d.tile_counts = a.take<int32_t>(tiles);
+    d.num_out = a.take<int32_t>(1);
+    d.stamp_offset = a.take<double>(1);
+  }));
+  if (data_host) {
+    DL_TRY(h2d(ctx, up, (const uint8_t*)data_host, bytes));
+    d.data = up;
+  } else {
+    d.data = (const uint8_t*)data_dev;
+  }
+  if (((uintptr_t)d.rows_out & 15) != 0) return ctx->fail(DL_ERR_ARG, "rows_out must be 16-byte aligned");
+  d.n = n;
+  d.point_step = l->point_step; d.offset_x = l->offset_x; d.offset_y = l->offset_y; d.offset_z = l->offset_z;
+  d.offset_time = l->offset_time; d.time_type = l->time_type;
+  const bool base4 = ((uintptr_t)d.data & 3) == 0 && l->point_step % 4 == 0;
+  d.xyz_aligned = base4 && l->offset_x % 4 == 0 && l->offset_y % 4 == 0 && l->offset_z % 4 == 0;
+  d.time_aligned = time_bytes == 8 ? (((uintptr_t)d.data & 7) == 0 && l->point_step % 8 == 0 && l->offset_time % 8 == 0)
+                                   : (base4 && l->offset_time % 4 == 0);
+  d.sensor_to_tracking = to_float(pose_from7(sensor_to_tracking));  // sensor_to_tracking->cast<float>()
+  DL_TRY(launch_decode_point_cloud2(ctx, d));
+  int32_t kept = 0;
+  DL_TRY(d2h(ctx, &kept, d.num_out, 1));
+  DL_TRY(d2h(ctx, stamp_offset_seconds, d.stamp_offset, 1));
+  DL_TRY(sync(ctx));
+  *num_rows_out = kept;
+  if (rows_host && kept > 0) {
+    DL_TRY(d2h(ctx, rows_host, d.rows_out, (size_t)kept * 4));
+    DL_TRY(sync(ctx));
+  }
+  return DL_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int dl_decode_point_cloud2(dl_context* ctx, const dl_point_cloud2_layout* layout, const void* data, int64_t num_points,
+                           const double* sensor_to_tracking, float* rows_out, int64_t* num_rows_out, double* stamp_offset_seconds) {
+  return decode_common(ctx, layout, data, nullptr, num_points, sensor_to_tracking, rows_out, nullptr, num_rows_out, stamp_offset_seconds);
+}
+int dl_decode_point_cloud2_dev(dl_context* ctx, const dl_point_cloud2_layout* layout, const void* data_dev, int64_t num_points,
+                               const double* sensor_to_tracking, float* rows_out_dev, int64_t* num_rows_out,
+                               double* stamp_offset_seconds) {
+  return decode_common(ctx, layout, nullptr, data_dev, num_points, sensor_to_tracking, nullptr, rows_out_dev, num_rows_out,
+                       stamp_offset_seconds);
+}
+
+}  // extern "C"

@@ -21,6 +21,14 @@
 // block whose bound still reaches the best leaf found (>=, so equal-score leaves with a lower index are not lost) — and
 // everything else is provably below the answer. On street scenes ~3-5 % of the blocks are opened
 // (tools/fcsm_pruning_study.py); results are identical to the exhaustive kernel, which stays as the fallback.
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+#include <mutex>
+#include <vector>
+
 #include "dl_internal.cuh"
 
 namespace dl {
@@ -564,3 +572,513 @@ int launch_fcsm(dl_context* ctx, const FcsmPair* pairs_dev, int count, int max_p
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ loop closure
+using namespace dl;
+
+namespace {
+struct CoarseSearch {  // device state of one chunk of (node, submap) pairs
+  bool pruned;     // pruned search (plan_coarse); otherwise exhaustive
+  int max_blocks;  // most pruning blocks of any pair of the chunk (pruned search)
+  float *d_hi, *d_lo;  // uploaded clouds (null when device-resident)
+  int* d_cells;
+  float* d_rot;
+  FcsmPair* d_pairs;
+  FcsmPick* d_picks;
+  unsigned long long* d_best;
+  int *d_bounds, *d_max_bound;  // pruned search only
+  std::vector<const float*> hi, lo;  // per pair of the chunk: its clouds on the device (uploaded or resident)
+};
+int check_fcsm_options(dl_context* ctx, const dl_fcsm_options& o) {
+  if (o.branch_and_bound_depth < 1 || o.full_resolution_depth < 1)
+    return ctx->fail(DL_ERR_ARG, "branch_and_bound_depth and full_resolution_depth must be >= 1 (CHECK_GE)");
+  if (o.linear_xy_search_window < 0 || o.linear_z_search_window < 0) return ctx->fail(DL_ERR_ARG, "negative search window");
+  return DL_OK;
+}
+// Loop-closure search index of a grid (dense sliding 8^3 maximum over the bounding box of its bricks), cached in the grid
+// and rebuilt when the grid changed. Returns false (no error) when the grid is empty or the volume would be unreasonably
+// large: the caller then searches exhaustively.
+int ensure_search_index(dl_context* ctx, dl_grid* g, bool* have) {
+  std::lock_guard<std::mutex> lock(g->index_mutex);  // grids are shared read-only between contexts: build once
+  *have = false;
+  if (g->m8_version == g->version && g->d_m8.get()) {
+    *have = true;
+    return DL_OK;
+  }
+  if (g->mirror_stale) DL_TRY(grid_download(g));
+  const int side = 1 << g->bits;
+  int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+  for (int tz = 0; tz < side; ++tz)
+    for (int ty = 0; ty < side; ++ty)
+      for (int tx = 0; tx < side; ++tx) {
+        const int node = g->top[top_flat(tx, ty, tz, g->bits)];
+        if (node < 0) continue;
+        for (int k = 0; k < 512; ++k) {
+          if (g->nodes[(size_t)node * 512 + k] < 0) continue;
+          const int b[3] = {(tx << 3) | (k & 7), (ty << 3) | ((k >> 3) & 7), (tz << 3) | (k >> 6)};  // brick coordinates
+          for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], b[a]); hi[a] = std::max(hi[a], b[a]); }
+        }
+      }
+  if (hi[0] < lo[0]) return DL_OK;  // empty grid
+  const int half = (64 << g->bits) >> 1;
+  int org[3], dim[3];
+  for (int a = 0; a < 3; ++a) {
+    org[a] = lo[a] * 8 - half - 8;                 // one brick of margin below: M8 is non-zero from 7 cells before the data
+    dim[a] = (hi[a] - lo[a] + 1) * 8 + 8;           // (org + half) % 8 == 0 and dim % 8 == 0 by construction
+  }
+  const size_t bytes = (size_t)dim[0] * dim[1] * dim[2];
+  if (bytes > ((size_t)3 << 30)) return DL_OK;    // > 3 GiB per submap: stay exhaustive
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (g->d_m8.cap < bytes) DL_TRY(grow(ctx, g->d_m8, bytes));
+  DeviceBuffer<uint8_t> tmp;
+  DL_TRY(alloc(ctx, tmp, bytes));
+  const int st = launch_fcsm_index(ctx, g->view(), org[0], org[1], org[2], dim[0], dim[1], dim[2], tmp.get(), g->d_m8.get());
+  ctx->wait_stream();  // tmp is freed on return
+  DL_TRY(st);
+  for (int a = 0; a < 3; ++a) { g->m8_org[a] = org[a]; g->m8_dim[a] = dim[a]; }
+  g->m8_version = g->version;
+  *have = true;
+  return DL_OK;
+}
+
+// Window half-widths in cells of a search in `hi` (double / float -> double, common::RoundToInt, cc:174-176).
+void search_window(const dl_fcsm_options& o, const dl_grid* hi, int* wxy, int* wz) {
+  *wxy = (int)std::lround(o.linear_xy_search_window / hi->resolution);
+  *wz = (int)std::lround(o.linear_z_search_window / hi->resolution);
+}
+// Decides, before the scratch is carved, whether pairs [first, first + n) get the pruned search and how many pruning blocks
+// its bounds table needs per pair. The pruned search needs the index of every high-resolution grid of the chunk
+// (DLIOM_FCSM_EXHAUSTIVE=1 or allow_pruned = false forces the fallback, and then no index is built) and at most 60 000 blocks
+// per pair (one CTA per block and pair in grid.x).
+int plan_coarse(dl_context* ctx, const dl_fcsm_options& o, int first, int n, const dl_grid* const* hi_grids, CoarseSearch* cs,
+                bool allow_pruned = true) {
+  cs->pruned = allow_pruned && std::getenv("DLIOM_FCSM_EXHAUSTIVE") == nullptr;
+  cs->max_blocks = 1;
+  for (int k = 0; k < n && cs->pruned; ++k) {
+    bool have = false;
+    DL_TRY(ensure_search_index(ctx, const_cast<dl_grid*>(hi_grids[first + k]), &have));
+    cs->pruned = have;
+  }
+  for (int k = 0; k < n; ++k) {
+    int wxy, wz;
+    search_window(o, hi_grids[first + k], &wxy, &wz);
+    const long long side = 2ll * wxy + 1, K = side * side * (2ll * wz + 1);
+    if (K >= 0xFFFFFFFFll) return ctx->fail(DL_ERR_ARG, "more than 2^32-1 translation candidates");
+    if (cs->pruned) {
+      const long long bxy = (side + 7) / 8, bz = (2ll * wz + 1 + 7) / 8;
+      if (bxy * bxy * bz > 60000) cs->pruned = false;
+      cs->max_blocks = (int)std::max<long long>(cs->max_blocks, bxy * bxy * bz);
+    }
+  }
+  return DL_OK;
+}
+// The device buffers of the coarse search of pairs [first, first + n), as plan_coarse decided it.
+void carve_coarse(Arena& a, const PairClouds& pc, int first, int n, CoarseSearch* cs) {
+  const int64_t n_hi = pc.hi_off[first + n] - pc.hi_off[first], n_lo = pc.lo_off[first + n] - pc.lo_off[first];
+  const bool resident = pc.hi_store != nullptr;
+  cs->d_hi = resident ? nullptr : a.take<float>(3 * n_hi);
+  cs->d_lo = resident ? nullptr : a.take<float>(3 * n_lo);
+  cs->d_cells = a.take<int>(3 * n_hi);
+  cs->d_rot = a.take<float>(3 * n_lo);
+  cs->d_pairs = a.take<FcsmPair>(n);
+  cs->d_picks = a.take<FcsmPick>(n);
+  cs->d_best = a.take<unsigned long long>(n);
+  cs->d_bounds = cs->pruned ? a.take<int>((size_t)n * cs->max_blocks) : nullptr;
+  cs->d_max_bound = cs->pruned ? a.take<int>(n) : nullptr;
+}
+
+// Runs the coarse search for pairs [first, first + n) in the buffers carve_coarse took, uploading their clouds first unless they
+// are device-resident; leaves the picks on the device. all_scores_dev (exhaustive search of one pair only): every leaf score.
+int coarse_search(dl_context* ctx, const dl_fcsm_options& o, float min_score, int first, int n, const double* guesses,
+                  const PairClouds& pc, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, CoarseSearch* out,
+                  float* all_scores_dev = nullptr) {
+  const int64_t* hi_off = pc.hi_off;
+  const int64_t* lo_off = pc.lo_off;
+  const int64_t hi0 = hi_off[first], lo0 = lo_off[first];
+  const int64_t n_hi = hi_off[first + n] - hi0, n_lo = lo_off[first + n] - lo0;
+  const bool resident = pc.hi_store != nullptr;
+  out->hi.resize(n);
+  out->lo.resize(n);
+  for (int k = 0; k < n; ++k) {
+    const int g = first + k;
+    out->hi[k] = resident ? pc.hi_store + 3 * pc.hi_begin[g] : out->d_hi + 3 * (hi_off[g] - hi0);
+    out->lo[k] = resident ? pc.lo_store + 3 * pc.lo_begin[g] : out->d_lo + 3 * (lo_off[g] - lo0);
+  }
+  if (!resident) {
+    DL_TRY(h2d(ctx, out->d_hi, pc.hi_pts + 3 * hi0, 3 * n_hi));
+    DL_TRY(h2d(ctx, out->d_lo, pc.lo_pts + 3 * lo0, 3 * n_lo));
+  }
+  std::vector<FcsmPair> pairs(n);
+  int max_points = 1;
+  long long max_candidates = 1;
+  for (int k = 0; k < n; ++k) {
+    const int g = first + k;
+    FcsmPair& p = pairs[k];
+    std::memset(&p, 0, sizeof(p));
+    p.hi = hi_grids[g]->view();
+    p.lo = lo_grids[g]->view();
+    p.hi_pts = out->hi[k];
+    p.lo_pts = out->lo[k];
+    p.cells = out->d_cells + 3 * (hi_off[g] - hi0);
+    p.lo_rot = out->d_rot + 3 * (lo_off[g] - lo0);
+    p.n_hi = (int)(hi_off[g + 1] - hi_off[g]);
+    p.n_lo = (int)(lo_off[g + 1] - lo_off[g]);
+    p.pose = to_float(pose_from7(guesses + 7 * g));
+    search_window(o, hi_grids[g], &p.wxy, &p.wz);
+    p.min_score = min_score;
+    p.min_low = o.min_low_resolution_score;
+    if (out->pruned) {
+      p.m8 = hi_grids[g]->d_m8.get();
+      for (int a3 = 0; a3 < 3; ++a3) { p.m8_org[a3] = hi_grids[g]->m8_org[a3]; p.m8_dim[a3] = hi_grids[g]->m8_dim[a3]; }
+    }
+    const long long side = 2ll * p.wxy + 1;
+    max_candidates = std::max(max_candidates, side * (2ll * p.wz + 1) * ((side + kFcsmRun - 1) / kFcsmRun));  // search threads
+    max_points = std::max(max_points, std::max(p.n_hi, p.n_lo));
+  }
+  DL_TRY(h2d(ctx, out->d_pairs, pairs.data(), n));
+  DL_TRY(sync(ctx));  // `pairs` is pageable host memory
+  StageScope st(ctx, "loop_closure_search");
+  if (out->pruned)
+    return launch_fcsm_pruned(ctx, out->d_pairs, n, max_points, out->max_blocks, out->d_bounds, out->d_max_bound, out->d_best,
+                              out->d_picks);
+  return launch_fcsm(ctx, out->d_pairs, n, max_points, max_candidates, out->d_best, out->d_picks, all_scores_dev);
+}
+int check_pairs(dl_context* ctx, int count, const double* guesses, const float* hi_pts, const int64_t* hi_off, const float* lo_pts,
+                const int64_t* lo_off, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids) {
+  if (!guesses || !hi_off || !lo_off || !hi_grids || !lo_grids || !hi_pts || !lo_pts) return DL_ERR_ARG;
+  for (int k = 0; k < count; ++k) {
+    if (!hi_grids[k] || !lo_grids[k]) return DL_ERR_ARG;
+    if (hi_off[k + 1] < hi_off[k] || lo_off[k + 1] < lo_off[k]) return ctx->fail(DL_ERR_ARG, "offsets must be non-decreasing");
+    if (hi_off[k + 1] == hi_off[k] || lo_off[k + 1] == lo_off[k]) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
+    if (hi_grids[k]->structure_dirty || lo_grids[k]->structure_dirty)
+      return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+  }
+  return DL_OK;
+}
+// RotateHistogram / MatchHistograms (rotational_scan_matcher.cc:123-155), float arithmetic in the reference's order
+std::vector<float> rotate_histogram(const float* h, int n, float angle) {
+  const float rotate_by_buckets = (float)(-angle * n / M_PI);
+  int full_buckets = (int)std::lround(rotate_by_buckets - 0.5f);
+  const float fraction = rotate_by_buckets - full_buckets;
+  while (full_buckets < 0) full_buckets += n;
+  std::vector<float> out(n);
+  for (int i = 0; i < n; ++i) out[i] = fraction * h[(i + 1 + full_buckets) % n] + (1.f - fraction) * h[(i + full_buckets) % n];
+  return out;
+}
+float match_histograms(const float* submap, const float* scan, int n) {
+  float ss = 0.f, sm = 0.f, dot = 0.f;
+  for (int i = 0; i < n; ++i) ss += scan[i] * scan[i];
+  for (int i = 0; i < n; ++i) sm += submap[i] * submap[i];
+  const float normalization = std::sqrt(ss) * std::sqrt(sm);
+  if (normalization < 1e-3f) return 1.f;
+  for (int i = 0; i < n; ++i) dot += submap[i] * scan[i];
+  return dot / normalization;
+}
+Quatf eigen_quaternion_inverse_f(const Quatf& q) {  // Eigen::Quaternion::inverse(): conjugate / squared norm
+  const float n2 = (q.x * q.x + q.y * q.y) + (q.z * q.z + q.w * q.w);
+  return {q.w / n2, -q.x / n2, -q.y / n2, -q.z / n2};
+}
+Quatd eigen_quaternion_inverse_d(const Quatd& q) {
+  const double n2 = (q.x * q.x + q.y * q.y) + (q.z * q.z + q.w * q.w);
+  return {q.w / n2, -q.x / n2, -q.y / n2, -q.z / n2};
+}
+}  // namespace
+
+namespace dl {
+int check_constraint_options(dl_context* ctx, const dl_constraint_options& o) {
+  DL_TRY(check_fcsm_options(ctx, o.fast_correlative_scan_matcher_3d));
+  return check_ceres_options(ctx, &o.ceres_scan_matcher_3d, 2);
+}
+int constraint_search(dl_context* ctx, const dl_constraint_options& o, int count, const double* guesses, const PairClouds& pc,
+                      const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, dl_constraint* constraints) {
+  const dl_constraint_options* options = &o;
+  const int64_t* hi_off = pc.hi_off;
+  const int64_t* lo_off = pc.lo_off;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const NlsOptions nls = to_nls_options(options->ceres_scan_matcher_3d, 2);
+  constexpr int kChunk = 1024;  // pairs per launch set: bounds the scratch, keeps every grid dimension legal
+  for (int first = 0; first < count; first += kChunk) {
+    const int n = std::min(kChunk, count - first);
+    CoarseSearch cs;
+    NlsProblem* d_problems;
+    NlsOutput* d_out;
+    DL_TRY(plan_coarse(ctx, options->fast_correlative_scan_matcher_3d, first, n, hi_grids, &cs));
+    DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+      carve_coarse(a, pc, first, n, &cs);
+      d_problems = a.take<NlsProblem>(n);
+      d_out = a.take<NlsOutput>(n);
+    }));
+    DL_TRY(coarse_search(ctx, options->fast_correlative_scan_matcher_3d, (float)options->min_score, first, n, guesses, pc,
+                         hi_grids, lo_grids, &cs));
+    // refinement: initial pose = translation target = the coarse pose, read from the pick record on the device
+    std::vector<NlsProblem> problems(n);
+    for (int k = 0; k < n; ++k) {
+      const int g = first + k;
+      NlsProblem& p = problems[k];
+      std::memset(&p, 0, sizeof(p));
+      p.cloud[0] = cs.hi[k];
+      p.cloud[1] = cs.lo[k];
+      p.count[0] = (int32_t)(hi_off[g + 1] - hi_off[g]);
+      p.count[1] = (int32_t)(lo_off[g + 1] - lo_off[g]);
+      p.grid[0] = hi_grids[g]->view();
+      p.grid[1] = lo_grids[g]->view();
+      p.initial_dev = cs.d_picks[k].pose;  // address arithmetic only
+      p.enabled_dev = &cs.d_picks[k].found;
+    }
+    DL_TRY(h2d(ctx, d_problems, problems.data(), n));
+    DL_CUDA(ctx, cudaMemsetAsync(d_out, 0, sizeof(NlsOutput) * n, ctx->stream));
+    {
+      StageScope st(ctx, "loop_closure_refine");
+      DL_TRY(launch_nls(ctx, nls, d_problems, n, d_out));
+    }
+    std::vector<FcsmPick> picks(n);
+    std::vector<NlsOutput> out(n);
+    DL_TRY(d2h(ctx, picks.data(), cs.d_picks, n));
+    DL_TRY(d2h(ctx, out.data(), d_out, n));
+    DL_TRY(sync(ctx));
+    for (int k = 0; k < n; ++k) {
+      dl_constraint& c = constraints[first + k];
+      std::memset(&c, 0, sizeof(c));
+      std::memcpy(c.coarse_pose, picks[k].pose, sizeof(c.coarse_pose));
+      if (!picks[k].found) continue;
+      c.found = 1;
+      c.score = picks[k].score;
+      c.rotational_score = (float)(options->fast_correlative_scan_matcher_3d.min_rotational_score + 0.01);
+      c.low_resolution_score = picks[k].low_resolution_score;
+      std::memcpy(c.pose, out[k].pose, sizeof(c.pose));
+      c.translation_weight = options->loop_closure_translation_weight;
+      c.rotation_weight = options->loop_closure_rotation_weight;
+      c.summary = out[k].summary;
+    }
+  }
+  return DL_OK;
+}
+}  // namespace dl
+
+extern "C" {
+
+int dl_fcsm_match_3dof(dl_context* ctx, const dl_fcsm_options* o, const double* guess, const float* hi_pts, int64_t n_hi,
+                       const float* lo_pts, int64_t n_lo, const dl_grid* hi, const dl_grid* lo, float min_score,
+                       dl_fcsm_result* result, float* all_scores, int64_t all_scores_capacity) {
+  if (!ctx || !o || !result || n_hi < 0 || n_lo < 0) return DL_ERR_ARG;
+  const int64_t hi_off[2] = {0, n_hi}, lo_off[2] = {0, n_lo};
+  if (guess && hi && lo && (n_hi == 0 || n_lo == 0)) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
+  DL_TRY(check_pairs(ctx, 1, guess, hi_pts, hi_off, lo_pts, lo_off, &hi, &lo));
+  DL_TRY(check_fcsm_options(ctx, *o));
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  CoarseSearch cs;
+  PairClouds pc;
+  pc.hi_pts = hi_pts;
+  pc.lo_pts = lo_pts;
+  pc.hi_off = hi_off;
+  pc.lo_off = lo_off;
+  int wxy, wz;
+  search_window(*o, hi, &wxy, &wz);
+  const int64_t K = (2ll * wxy + 1) * (2ll * wxy + 1) * (2ll * wz + 1);
+  if (all_scores && all_scores_capacity < K) return ctx->fail(DL_ERR_ARG, "all_scores has room for fewer than num_candidates floats");
+  DL_TRY(plan_coarse(ctx, *o, 0, 1, &hi, &cs, all_scores == nullptr));  // only the exhaustive kernel scores every leaf
+  float* d_scores = nullptr;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    carve_coarse(a, pc, 0, 1, &cs);
+    d_scores = all_scores ? a.take<float>(K) : nullptr;
+  }));
+  DL_TRY(coarse_search(ctx, *o, min_score, 0, 1, guess, pc, &hi, &lo, &cs, d_scores));
+  FcsmPick pick;
+  DL_TRY(d2h(ctx, &pick, cs.d_picks, 1));
+  if (all_scores) DL_TRY(d2h(ctx, all_scores, d_scores, K));
+  DL_TRY(sync(ctx));
+  std::memset(result, 0, sizeof(*result));
+  result->num_candidates = pick.num_candidates;
+  if (!pick.found) return DL_OK;  // nothing above min_score passes the low-resolution gate: the reference returns nullptr
+  result->found = 1;
+  result->score = pick.score;
+  std::memcpy(result->pose_estimate, pick.pose, sizeof(pick.pose));
+  result->rotational_score = (float)(o->min_rotational_score + 0.01);  // what MatchWith3DofInitial reports (cc:179-181)
+  result->low_resolution_score = pick.low_resolution_score;
+  std::memcpy(result->offset, pick.offset, sizeof(pick.offset));
+  return DL_OK;
+}
+
+int dl_fcsm_match(dl_context* ctx, const dl_fcsm_options* o, const float* submap_histogram, const float* scan_histogram,
+                  int32_t histogram_size, const double* global_node_pose, const double* global_submap_pose,
+                  const double* gravity_alignment, const float* hi_pts, int64_t n_hi, const float* lo_pts, int64_t n_lo,
+                  const dl_grid* hi, const dl_grid* lo, float min_score, dl_fcsm_result* result) {
+  if (!ctx || !o || !result || !submap_histogram || !scan_histogram || histogram_size < 1 || !global_node_pose ||
+      !global_submap_pose || !gravity_alignment || !hi || !lo || n_hi < 0 || n_lo < 0 || (n_hi > 0 && !hi_pts) || (n_lo > 0 && !lo_pts))
+    return DL_ERR_ARG;
+  if (n_hi == 0 || n_lo == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
+  DL_TRY(check_fcsm_options(ctx, *o));
+  std::memset(result, 0, sizeof(*result));
+  const float res = hi->resolution;
+  const Rigidf node = to_float(pose_from7(global_node_pose)), submap = to_float(pose_from7(global_submap_pose));
+  // GenerateDiscreteScans (cc:296-350)
+  float max_scan_range = 3.f * res;
+  for (int64_t i = 0; i < n_hi; ++i) max_scan_range = std::max(norm3(Vec3f{hi_pts[3 * i], hi_pts[3 * i + 1], hi_pts[3 * i + 2]}), max_scan_range);
+  const float angular_step_size = (1.f - 1e-2f) * std::acos(1.f - (res * res) / (2.f * (max_scan_range * max_scan_range)));
+  const int angular_window_size = (int)std::lround(o->angular_search_window / angular_step_size);
+  if (angular_window_size < 0 || angular_window_size > 100000) return ctx->fail(DL_ERR_ARG, "angular window out of range");
+  const Rigidf node_to_submap = compose(inverse(submap), node);
+  const Quatd ga_inv_d = eigen_quaternion_inverse_d(Quatd{gravity_alignment[0], gravity_alignment[1], gravity_alignment[2], gravity_alignment[3]});
+  const Quatf ga_inv{(float)ga_inv_d.w, (float)ga_inv_d.x, (float)ga_inv_d.y, (float)ga_inv_d.z};
+  const Vec3f dir = rotate(qmul(node_to_submap.q, ga_inv), Vec3f{1.f, 0.f, 0.f});
+  const float initial_angle = std::atan2(dir.y, dir.x);  // transform::GetYaw
+  std::vector<double> guesses;
+  std::vector<float> scores;
+  for (int rz = -angular_window_size; rz <= angular_window_size; ++rz) {
+    const float angle = rz * angular_step_size;
+    const std::vector<float> rotated = rotate_histogram(scan_histogram, histogram_size, initial_angle + angle);
+    const float score = match_histograms(submap_histogram, rotated.data(), histogram_size);
+    if (score < o->min_rotational_score) continue;
+    const Quatf q = qmul(qmul(eigen_quaternion_inverse_f(submap.q), angle_axis_to_quat(Vec3f{0.f, 0.f, angle})), node.q);
+    const double g[7] = {node_to_submap.t.x, node_to_submap.t.y, node_to_submap.t.z, q.w, q.x, q.y, q.z};  // floats widen exactly
+    guesses.insert(guesses.end(), g, g + 7);
+    scores.push_back(score);
+  }
+  const int n = (int)scores.size();
+  if (n == 0) return DL_OK;  // no yaw step passes the rotational score: the reference returns nullptr
+  std::vector<float> hi_all((size_t)n * n_hi * 3), lo_all((size_t)n * n_lo * 3);
+  std::vector<int64_t> hi_off(n + 1), lo_off(n + 1);
+  std::vector<const dl_grid*> his(n, hi), los(n, lo);
+  for (int k = 0; k < n; ++k) {
+    std::memcpy(hi_all.data() + (size_t)k * n_hi * 3, hi_pts, (size_t)n_hi * 12);
+    std::memcpy(lo_all.data() + (size_t)k * n_lo * 3, lo_pts, (size_t)n_lo * 12);
+    hi_off[k] = k * n_hi; lo_off[k] = k * n_lo;
+  }
+  hi_off[n] = n * n_hi; lo_off[n] = n * n_lo;
+  DL_TRY(check_pairs(ctx, n, guesses.data(), hi_all.data(), hi_off.data(), lo_all.data(), lo_off.data(), his.data(), los.data()));
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  FcsmPick best{};
+  int best_scan = -1;
+  constexpr int kChunk = 1024;
+  for (int first = 0; first < n; first += kChunk) {
+    const int m = std::min(kChunk, n - first);
+    CoarseSearch cs;
+    PairClouds pc;
+    pc.hi_pts = hi_all.data();
+    pc.lo_pts = lo_all.data();
+    pc.hi_off = hi_off.data();
+    pc.lo_off = lo_off.data();
+    DL_TRY(plan_coarse(ctx, *o, first, m, his.data(), &cs));
+    DL_TRY(carve_scratch(ctx, [&](Arena& a) { carve_coarse(a, pc, first, m, &cs); }));
+    DL_TRY(coarse_search(ctx, *o, min_score, first, m, guesses.data(), pc, his.data(), los.data(), &cs));
+    std::vector<FcsmPick> picks(m);
+    DL_TRY(d2h(ctx, picks.data(), cs.d_picks, m));
+    DL_TRY(sync(ctx));
+    for (int k = 0; k < m; ++k) {
+      result->num_candidates += picks[k].num_candidates;
+      if (picks[k].found && (best_scan < 0 || picks[k].score > best.score)) {  // first of equal scores: lowest yaw step
+        best = picks[k];
+        best_scan = first + k;
+      }
+    }
+  }
+  if (best_scan < 0) return DL_OK;
+  result->found = 1;
+  result->score = best.score;
+  std::memcpy(result->pose_estimate, best.pose, sizeof(best.pose));
+  result->rotational_score = scores[best_scan];
+  result->low_resolution_score = best.low_resolution_score;
+  std::memcpy(result->offset, best.offset, sizeof(best.offset));
+  result->scan_index = best_scan;
+  return DL_OK;
+}
+
+int dl_constraint_search_batch(dl_context* ctx, const dl_constraint_options* options, int32_t count, const double* guesses,
+                               const float* hi_pts, const int64_t* hi_off, const float* lo_pts, const int64_t* lo_off,
+                               const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, dl_constraint* constraints) {
+  if (!ctx || !options || count < 0) return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  if (!constraints) return DL_ERR_ARG;
+  DL_TRY(check_pairs(ctx, count, guesses, hi_pts, hi_off, lo_pts, lo_off, hi_grids, lo_grids));
+  DL_TRY(check_constraint_options(ctx, *options));
+  PairClouds pc;
+  pc.hi_pts = hi_pts;
+  pc.lo_pts = lo_pts;
+  pc.hi_off = hi_off;
+  pc.lo_off = lo_off;
+  return constraint_search(ctx, *options, count, guesses, pc, hi_grids, lo_grids, constraints);
+}
+
+int dl_constraint_search_exchange(dl_context* ctx, dl_comm* comm, const dl_constraint_options* options, int32_t count,
+                                  int32_t capacity, const int32_t* submap_ids, const int32_t* node_ids, const double* guesses,
+                                  const float* hi_pts, const int64_t* hi_off, const float* lo_pts, const int64_t* lo_off,
+                                  const dl_grid* const* hi_grids, const dl_grid* const* lo_grids, dl_constraint_row* table,
+                                  dl_exchange_info* info) {
+  if (!ctx || !comm || !options || count < 0 || capacity < 1 || count > capacity || !table) return DL_ERR_ARG;
+  if (capacity > 1024) return ctx->fail(DL_ERR_ARG, "capacity > 1024 pairs per rank and exchange: split the call");
+  if (count > 0 && (!submap_ids || !node_ids)) return DL_ERR_ARG;
+  if (count > 0) DL_TRY(check_pairs(ctx, count, guesses, hi_pts, hi_off, lo_pts, lo_off, hi_grids, lo_grids));
+  DL_TRY(check_constraint_options(ctx, *options));
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int world = dl_comm_world_size(comm), rank = dl_comm_rank(comm);
+  const size_t row_bytes = sizeof(dl_constraint_row), block = (size_t)capacity * row_bytes;
+  DL_TRY(comm_reserve(comm, block));
+  dl_constraint_row* d_send = (dl_constraint_row*)comm_send_buffer(comm);
+  dl_constraint_row* d_recv = (dl_constraint_row*)comm_recv_buffer(comm);
+  // padding rows: found = -1 (every int32 of the row is -1; the doubles are NaN and never read)
+  DL_CUDA(ctx, cudaMemsetAsync(d_send, 0xFF, block, ctx->stream));
+  if (count > 0) {
+    const NlsOptions nls = to_nls_options(options->ceres_scan_matcher_3d, 2);
+    const int n = count;
+    CoarseSearch cs;
+    PairClouds pc;
+    pc.hi_pts = hi_pts;
+    pc.lo_pts = lo_pts;
+    pc.hi_off = hi_off;
+    pc.lo_off = lo_off;
+    NlsProblem* d_problems;
+    NlsOutput* d_out;
+    int32_t* d_ids;
+    DL_TRY(plan_coarse(ctx, options->fast_correlative_scan_matcher_3d, 0, n, hi_grids, &cs));
+    DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+      carve_coarse(a, pc, 0, n, &cs);
+      d_problems = a.take<NlsProblem>(n);
+      d_out = a.take<NlsOutput>(n);
+      d_ids = a.take<int32_t>(2 * (size_t)n);
+    }));
+    DL_TRY(coarse_search(ctx, options->fast_correlative_scan_matcher_3d, (float)options->min_score, 0, n, guesses, pc,
+                         hi_grids, lo_grids, &cs));
+    std::vector<NlsProblem> problems(n);
+    for (int k = 0; k < n; ++k) {
+      NlsProblem& p = problems[k];
+      std::memset(&p, 0, sizeof(p));
+      p.cloud[0] = cs.hi[k];
+      p.cloud[1] = cs.lo[k];
+      p.count[0] = (int32_t)(hi_off[k + 1] - hi_off[k]);
+      p.count[1] = (int32_t)(lo_off[k + 1] - lo_off[k]);
+      p.grid[0] = hi_grids[k]->view();
+      p.grid[1] = lo_grids[k]->view();
+      p.initial_dev = cs.d_picks[k].pose;  // address arithmetic only
+      p.enabled_dev = &cs.d_picks[k].found;
+    }
+    DL_TRY(h2d(ctx, d_problems, problems.data(), n));
+    DL_TRY(h2d(ctx, d_ids, submap_ids, n));
+    DL_TRY(h2d(ctx, d_ids + n, node_ids, n));
+    DL_CUDA(ctx, cudaMemsetAsync(d_out, 0, sizeof(NlsOutput) * n, ctx->stream));
+    {
+      StageScope st(ctx, "loop_closure_refine");
+      DL_TRY(launch_nls(ctx, nls, d_problems, n, d_out));
+    }
+    DL_TRY(launch_pack_constraint_rows(ctx, n, cs.d_picks, d_out, d_ids, d_ids + n, options->loop_closure_translation_weight,
+                                       options->loop_closure_rotation_weight, rank, d_send));
+    DL_TRY(sync(ctx));  // `problems` is pageable host memory; also keeps the search out of the collective's timing
+  }
+  float ms = 0.f;
+  {
+    StageScope st(ctx, "constraint_all_gather");
+    DL_TRY(comm_all_gather(comm, d_send, d_recv, block, &ms));
+  }
+  DL_TRY(d2h(ctx, table, d_recv, (size_t)world * capacity));
+  DL_TRY(sync(ctx));
+  if (info) {
+    info->bytes_sent = (int64_t)block;
+    info->bytes_received = (int64_t)block * world;
+    info->collective_ms = ms;
+    int found = 0;
+    for (int i = 0; i < world * capacity; ++i) found += table[i].found == 1;
+    info->found_total = found;
+  }
+  return DL_OK;
+}
+
+}  // extern "C"

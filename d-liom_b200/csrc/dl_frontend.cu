@@ -32,6 +32,12 @@
 // 1 bit (+12/16 B row + 4 B time, writes 16 B record for survivors, 8 B entry per tile winner, read back by B2) and writes
 // 2 bits; C reads 16 B and writes 12 B per output point.
 #include <type_traits>
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+#include <functional>
+#include <vector>
 
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
@@ -851,3 +857,753 @@ int launch_finalize_results(dl_context* ctx, const ResultArgs& a) {
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ batched front end
+using namespace dl;
+
+namespace {
+
+// Device scratch of one front-end run.
+void carve(Arena& a, int batch, int64_t cap, int num_origins, FrontendBuffers* f) {
+  const size_t B = (size_t)batch, C = (size_t)cap;
+  f->batch = batch;
+  f->cap = cap;
+  f->tcap = next_pow2(2 * cap);
+  f->counts0 = a.take<int32_t>(B); f->n1 = a.take<int32_t>(B); f->n_ret = a.take<int32_t>(B);
+  f->n2 = a.take<int32_t>(B); f->n3 = a.take<int32_t>(B); f->countsA = a.take<int32_t>(2 * B); f->npassesA = a.take<int32_t>(2 * B);
+  f->croppedA = a.take<int32_t>(2 * B);
+  f->tableA = a.take<uint32_t>(B * 2 * f->tcap); f->scratchA = a.take<uint32_t>(B * 4 * C);
+  f->keepA = a.take<int32_t>(B * 2 * C);
+  f->returns_tracking = a.take<float>(B * C * 3); f->misses_tracking = a.take<float>(B * C * 3);
+  f->clouds = a.take<float>(B * 2 * C * 3); f->current_pose = a.take<float>(B * 7); f->origins = a.take<float>((size_t)num_origins * 3);
+  f->passesA = a.take<float>(B * 2 * 32); f->rtcsm_scores = a.take<float>(B);
+  f->scans = a.take<ScanConstants>(B); f->filters = a.take<AdaptiveParams>(2);
+  f->submap = a.take<Rigidd>(B); f->submap_inverse = a.take<Rigidd>(B); f->origin_base = a.take<int32_t>(B);
+  f->initial_pose = a.take<double>(B * 7); f->target = a.take<double>(B * 3);
+  f->problems = a.take<NlsProblem>(B); f->nls_out = a.take<NlsOutput>(B);
+  f->bit_words = (int64_t)((C + 31) / 32);
+  f->bits = a.take<uint32_t>(B * 2 * f->bit_words);
+  f->first_bits = a.take<uint32_t>(B * f->bit_words);
+  const size_t tiles = (C + kFrontendTile - 1) / kFrontendTile;
+  f->stage = a.take<int4>(B * tiles * kFrontendTile);
+  f->part_ends = a.take<int32_t>(B * tiles * kFrontendParts);
+  f->spill = a.take<uint32_t>(B * 2 * tiles * kFrontendTile);
+  f->spill_used = a.take<int32_t>(2 * B);
+  f->last_index = a.take<int32_t>(B); f->error_flag = a.take<int32_t>(B);
+  f->local4 = a.take<float>(B * C * 4);
+}
+
+// Device copies of the time_run_* arrays of 12-byte rows (validated by check_frontend) and, with many runs per scan, the table
+// of per-run deskew poses: one pose per run (fe_run_poses) instead of one per survivor.
+void carve_time_runs(Arena& a, const dl_frontend_options& o, int num_scans, FrontendBuffers* f) {
+  if (o.range_row_floats != 3) return;
+  const size_t runs = (size_t)o.time_run_offsets[num_scans];
+  f->run_offsets = a.take<int32_t>((size_t)num_scans + 1);
+  f->run_first_row = a.take<int32_t>(runs);
+  f->run_value = a.take<float>(runs);
+  if (runs > (size_t)8 * num_scans) f->run_pose = a.take<float>(runs * 8);
+}
+
+// The pre-match's per-scan flags, carved last so that every other buffer sits where it does without the pre-match.
+void carve_prematch(Arena& a, const dl_frontend_options& o, int num_scans, FrontendBuffers* f) {
+  if (o.use_online_correlative_scan_matching) f->rtcsm_nonpositive = a.take<int32_t>((size_t)num_scans);
+}
+
+FrontendArgs make_frontend_args(const dl_frontend_options& o, const FrontendBuffers& f, const float* d_ranges,
+                                int64_t in_cap, int row_floats) {
+  FrontendArgs fa{};
+  fa.ranges = d_ranges; fa.in_cap = in_cap; fa.row_floats = row_floats; fa.counts = f.counts0; fa.scans = f.scans;
+  fa.origins = f.origins; fa.origin_base = f.origin_base; fa.cap = f.cap;
+  fa.first_resolution = 0.5f * o.voxel_filter_size;  // LTB:394
+  fa.second_resolution = o.voxel_filter_size;        // LTB:479-484
+  fa.min_range = o.min_range; fa.max_range = o.max_range; fa.scan_period = o.scan_period;
+  fa.first_bits = f.first_bits; fa.bits = f.bits; fa.bit_words = f.bit_words;
+  fa.stage = f.stage; fa.part_ends = f.part_ends; fa.spill = f.spill; fa.spill_used = f.spill_used;
+  fa.idx_bits = 1;
+  while (((int64_t)1 << fa.idx_bits) < f.cap) ++fa.idx_bits;      // point indices are < cap
+  fa.axis_bits = std::min(21, (63 - fa.idx_bits) / 3);             // 15 bits per axis up to 256 k points per scan
+  fa.local = f.local4;
+  fa.returns_tracking = f.returns_tracking; fa.misses_tracking = f.misses_tracking;
+  fa.n_first = f.n1; fa.n_returns_local = f.n_ret; fa.n_returns = f.n2; fa.n_misses = f.n3; fa.last_index = f.last_index;
+  fa.current_pose = f.current_pose; fa.error_flag = f.error_flag;
+  return fa;
+}
+
+int row_floats_of(const dl_frontend_options& o) { return o.range_row_floats == 4 ? 4 : (o.range_row_floats == 3 ? 3 : 8); }
+
+ScanConstants make_scan_constants(const double* prev7, const double* cur7) {  // dl_pipeline.cuh has the arithmetic
+  return dl::make_scan_constants(pose_from7(prev7), pose_from7(cur7));
+}
+
+// The pinned staging block of a front-end batch: the small per-call tables, then the results and estimated IMU states that a
+// submitted batch downloads (dl_frontend_submit*, collected by dl_frontend_collect*).
+struct Staging {
+  int32_t* counts;
+  ScanConstants* scans;
+  float* origins;
+  AdaptiveParams* filters;
+  NlsProblem* problems;
+  dl_scan_result* results;
+  dl_nav_state* states;
+  Rigidd* submaps;      // per scan: pose, inverse
+  int32_t* origin_base;
+};
+void carve_staging(Arena& h, int batch, int num_origins, Staging* s) {
+  const size_t B = (size_t)batch;
+  s->counts = h.take<int32_t>(B);
+  s->submaps = h.take<Rigidd>(2 * B);
+  s->origin_base = h.take<int32_t>(B);
+  s->scans = h.take<ScanConstants>(B);
+  s->origins = h.take<float>((size_t)num_origins * 3);
+  s->filters = h.take<AdaptiveParams>(2);
+  s->problems = h.take<NlsProblem>(B);
+  s->results = h.take<dl_scan_result>(B);
+  s->states = h.take<dl_nav_state>(B);
+}
+
+// Uploads the small per-call tables (counts, deskew constants, origins, filter options, NLS problem records, matching
+// submaps) through the pinned staging block. No host synchronisation: the block is reused only after `staging_done`.
+// origin_base (optional, per scan): where each scan's origins start in `origins`; without it every scan uses them all.
+int frontend_upload_small(dl_context* ctx, const dl_frontend_options& o, const FrontendBuffers& f, const int64_t* sizes,
+                          const float* origins, int num_origins, const double* prev_poses, const double* cur_poses,
+                          const SubmapSet* submaps, const int32_t* origin_base = nullptr, const int32_t* enabled_dev = nullptr) {
+  const size_t B = (size_t)f.batch;
+  Staging s;
+  Arena count(nullptr);
+  carve_staging(count, f.batch, num_origins, &s);
+  DL_TRY(ctx->reserve_pinned(count.off));
+  DL_CUDA(ctx, cudaEventSynchronize(ctx->staging_done));
+  Arena h(ctx->h_pinned.get());
+  carve_staging(h, f.batch, num_origins, &s);
+  for (int b = 0; b < f.batch; ++b) {
+    s.counts[b] = (int32_t)sizes[b];
+    s.origin_base[b] = origin_base ? origin_base[b] : 0;
+    if (prev_poses) s.scans[b] = make_scan_constants(prev_poses + 7 * b, cur_poses + 7 * b);
+    NlsProblem& p = s.problems[b];
+    std::memset(&p, 0, sizeof(p));
+    if (submaps) {
+      const Rigidd pose = pose_from7(submaps->pose(b));
+      s.submaps[2 * b] = pose;
+      s.submaps[2 * b + 1] = inverse(pose);
+      for (int k = 0; k < 2; ++k) {
+        p.cloud[k] = f.clouds + (size_t)(2 * b + k) * f.cap * 3;
+        p.count_dev[k] = f.countsA + 2 * b + k;
+        p.grid[k] = k == 0 ? submaps->high(b)->view() : submaps->low(b)->view();
+      }
+      p.initial_dev = f.initial_pose + 7 * b;
+      p.target_dev = f.target + 3 * b;
+      if (enabled_dev) p.enabled_dev = enabled_dev + b;  // scans whose IMU factor could not be formed are not solved
+    }
+  }
+  std::memcpy(s.origins, origins, (size_t)num_origins * 12);
+  s.filters[0] = {o.high_resolution_adaptive_voxel_filter.max_length, o.high_resolution_adaptive_voxel_filter.min_num_points,
+                  o.high_resolution_adaptive_voxel_filter.max_range};
+  s.filters[1] = {o.low_resolution_adaptive_voxel_filter.max_length, o.low_resolution_adaptive_voxel_filter.min_num_points,
+                  o.low_resolution_adaptive_voxel_filter.max_range};
+  DL_TRY(h2d(ctx, f.counts0, s.counts, B));
+  if (prev_poses) DL_TRY(h2d(ctx, f.scans, s.scans, B));  // otherwise imu_prepare_kernel writes them on the device
+  DL_TRY(h2d(ctx, f.origins, s.origins, (size_t)num_origins * 3));
+  DL_TRY(h2d(ctx, f.filters, s.filters, 2));
+  DL_TRY(h2d(ctx, f.problems, s.problems, B));
+  DL_TRY(h2d(ctx, f.origin_base, s.origin_base, B));
+  if (submaps) {
+    DL_CUDA(ctx, cudaMemcpy2DAsync(f.submap, sizeof(Rigidd), s.submaps, 2 * sizeof(Rigidd), sizeof(Rigidd), B, cudaMemcpyHostToDevice,
+                                   ctx->stream));
+    DL_CUDA(ctx, cudaMemcpy2DAsync(f.submap_inverse, sizeof(Rigidd), s.submaps + 1, 2 * sizeof(Rigidd), sizeof(Rigidd), B,
+                                   cudaMemcpyHostToDevice, ctx->stream));
+  }
+  DL_CUDA(ctx, cudaEventRecord(ctx->staging_done, ctx->stream));
+  return DL_OK;
+}
+
+void carve_imu(Arena& a, int num_scans, ImuRun* r) {
+  r->d_terms = a.take<ImuTerm>(num_scans);
+  r->d_init16 = a.take<double>((size_t)num_scans * 16);
+  r->d_fused = a.take<FusedOutput>(num_scans);
+  r->d_states = r->d_states_out ? r->d_states_out : a.take<dl_nav_state>(num_scans);
+  if (!r->samples) return;
+  const size_t ns = (size_t)r->samples->offsets[num_scans];
+  r->d_off = a.take<int32_t>(num_scans + 1);
+  r->d_dt = a.take<double>(ns);
+  r->d_acc = a.take<double>(3 * ns);
+  r->d_gyr = a.take<double>(3 * ns);
+  r->d_si = a.take<dl_nav_state>(num_scans);
+  r->d_pre = a.take<dl_preintegration>(num_scans);
+  r->d_predicted = a.take<dl_nav_state>(num_scans);
+  r->d_ok = a.take<int32_t>(num_scans);
+}
+
+// CTAs per least-squares problem. The pipeline's adaptive filters hand the matcher a few hundred points: one CTA. With the filters
+// opened up (min_num_points in the thousands: SURVEY 8d's full-cloud mode F, tens of thousands of points per solve) one 256-thread
+// CTA per problem is latency-bound and leaves half the SMs idle, so the problem is spread over a thread-block cluster — as many
+// CTAs as keep the launch within one wave of the SMs (on an H100's 132 SMs: 2 for sub-batches of up to 66 problems, 1 for the
+// bench's 74), at most the portable 8.
+// DLIOM_NLS_CLUSTER=n forces n (1 = never).
+int solve_cluster_size(dl_context* ctx, const dl_frontend_options& o, int problems) {
+  if (const char* env = std::getenv("DLIOM_NLS_CLUSTER")) return std::max(1, std::min(8, std::atoi(env)));
+  const float few = 4096.f;
+  if (o.high_resolution_adaptive_voxel_filter.min_num_points < few && o.low_resolution_adaptive_voxel_filter.min_num_points < few) return 1;
+  int sms = kNumSMs;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
+  int cs = 1;
+  while (cs < 8 && problems * cs * 2 <= sms) cs *= 2;
+  return cs;
+}
+
+// The batch is processed as `chunks` sub-batches that alternate between two streams, so that
+//   - with host scans (host_ranges != nullptr) the upload of sub-batch k+1 (copy stream) overlaps the kernels of k;
+//   - the latency-bound tail of sub-batch k (adaptive filter: 2 CTAs per scan, LM solve: 1 CTA per scan) overlaps the
+//     bandwidth-bound front half of sub-batch k+1.
+// Every kernel launcher enqueues on ctx->stream, which is pointed at the sub-batch's stream while it is enqueued.
+int frontend_run(dl_context* ctx, const dl_frontend_options& o, int num_scans, float* d_ranges, int64_t in_cap,
+                 const void* const* host_ranges, const int64_t* sizes, const float* origins, int num_origins,
+                 const int32_t* origin_base, const double* prev_poses, const double* cur_poses, const SubmapSet& submaps,
+                 const FrontendBuffers& f, Arena& a, dl_scan_result* d_results, ImuRun* imu_run = nullptr) {
+  // optional IMU coupling: one pre-integration factor per scan, the 15-parameter solve instead of the 6-parameter one
+  const ImuRun no_imu;
+  const ImuRun& m = imu_run ? *imu_run : no_imu;
+  const dl_frontend_imu* imu = m.host;
+  const dl_frontend_imu_samples* raw = m.samples;
+  if (imu) {
+    std::vector<ImuTerm> terms(num_scans);
+    std::vector<double> init16((size_t)num_scans * 16);
+    for (int b = 0; b < num_scans; ++b)
+      if (!build_imu_term(inverse(pose_from7(submaps.pose(b))), imu->states_i[b], imu->predicted_states[b], imu->preintegrations[b], imu->gravity,
+                          imu->imu_weight, &terms[b], init16.data() + 16 * b))
+        return ctx->fail(DL_ERR_ARG, "pre-integration covariance is not positive definite");
+    DL_TRY(h2d(ctx, m.d_terms, terms.data(), num_scans));
+    DL_TRY(h2d(ctx, m.d_init16, init16.data(), (size_t)num_scans * 16));
+    DL_TRY(sync(ctx));  // the staging vectors are pageable and local
+  }
+  if (imu || raw) DL_CUDA(ctx, cudaMemsetAsync(m.d_fused, 0, sizeof(FusedOutput) * num_scans, ctx->stream));
+  const int rf = row_floats_of(o);
+  DL_TRY(frontend_upload_small(ctx, o, f, sizes, origins, num_origins, raw ? nullptr : prev_poses, cur_poses, &submaps, origin_base,
+                               m.d_ok));
+  FrontendArgs fa = make_frontend_args(o, f, d_ranges, in_cap, rf);
+  if (rf == 3) {  // per-point times as runs: validated by check_frontend, uploaded next to the scans
+    const size_t runs = (size_t)o.time_run_offsets[num_scans];
+    DL_TRY(h2d(ctx, f.run_offsets, o.time_run_offsets, (size_t)num_scans + 1));
+    DL_TRY(h2d(ctx, f.run_first_row, o.time_run_first_row, runs));
+    DL_TRY(h2d(ctx, f.run_value, o.time_run_value, runs));
+    fa.run_offsets = f.run_offsets; fa.run_first_row = f.run_first_row; fa.run_value = f.run_value;
+    if (f.run_pose) {
+      int max_runs = 0;
+      for (int b = 0; b < num_scans; ++b) max_runs = std::max(max_runs, (int)(o.time_run_offsets[b + 1] - o.time_run_offsets[b]));
+      fa.run_pose = f.run_pose;  // filled per sub-batch by fe_run_poses once the scans' deskew constants exist
+      fa.max_runs = max_runs;
+    }
+  }
+  DL_TRY(launch_fe_prepare(ctx, fa, f.batch));
+  const float hi_resolution = submaps.high(0)->resolution;  // one for the batch (check_frontend)
+  const bool rtcsm = o.use_online_correlative_scan_matching != 0;
+  int chunks = rtcsm ? 1 : (host_ranges ? 5 : 2);
+  if (f.batch < 8 * chunks) chunks = std::max(1, f.batch / 8);
+  // Sub-batches alternate between two equal-priority streams. Every back half (latency-bound, one or two CTAs per scan) on one
+  // high-priority stream behind its front half would serialise the back halves, which costs more than the priority gains.
+  // DLIOM_SERIAL=1: every sub-batch on the main stream, nothing overlaps (bench.py's per-stage roofline pass: the stage events then
+  // bracket the kernels' own durations at the sub-batch size the step really uses)
+  const bool serial = std::getenv("DLIOM_SERIAL") != nullptr;
+  cudaStream_t main_stream = ctx->stream;
+  cudaEvent_t prepared = ctx->take_event();
+  DL_CUDA(ctx, cudaEventRecord(prepared, main_stream));
+  DL_CUDA(ctx, cudaStreamWaitEvent(ctx->aux_stream, prepared, 0));
+  DL_CUDA(ctx, cudaStreamWaitEvent(ctx->tail_stream, prepared, 0));
+  if (host_ranges) DL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, prepared, 0));  // the upload target may be in use
+  ctx->event_pool.push_back(prepared);
+  cudaEvent_t imu_ready = nullptr;
+  if (raw) {
+    // Raw samples: pre-integration, prediction, deskew constants, factor and information matrix all on the device; the
+    // only host work is the upload of the samples and of the states at the previous scans. The chain runs on its own
+    // stream next to the first voxel filter (which needs none of it); the ingest kernels wait for `imu_ready`.
+    ctx->stream = ctx->tail_stream;
+    auto chain = [&]() -> int {
+      StageScope st(ctx, "imu_preintegrate_predict");
+      const size_t ns = (size_t)raw->offsets[num_scans];
+      DL_TRY(h2d(ctx, m.d_off, raw->offsets, (size_t)num_scans + 1));
+      DL_TRY(h2d(ctx, m.d_dt, raw->dt, ns));
+      DL_TRY(h2d(ctx, m.d_acc, raw->acc, 3 * ns));
+      DL_TRY(h2d(ctx, m.d_gyr, raw->gyr, 3 * ns));
+      DL_TRY(h2d(ctx, m.d_si, raw->states_i, (size_t)num_scans));
+      DL_TRY(launch_imu_preintegrate(ctx, num_scans, m.d_off, m.d_dt, m.d_acc, m.d_gyr, (const double*)m.d_si + 10, 16, raw->noise,
+                                     m.d_pre));
+      ImuPrepareArgs pa{};
+      pa.count = num_scans; pa.preint = m.d_pre; pa.states_i = m.d_si; pa.to_submap = f.submap_inverse;
+      for (int k = 0; k < 3; ++k) pa.gravity[k] = raw->gravity[k];
+      pa.imu_weight = raw->imu_weight; pa.scans = f.scans; pa.terms = m.d_terms; pa.init16 = m.d_init16; pa.predicted = m.d_predicted;
+      pa.ok = m.d_ok;
+      return launch_imu_prepare(ctx, pa);
+    };
+    const int st_imu = chain();
+    ctx->stream = main_stream;
+    DL_TRY(st_imu);
+    imu_ready = ctx->take_event();
+    DL_CUDA(ctx, cudaEventRecord(imu_ready, ctx->tail_stream));  // recycled once every sub-batch's wait is enqueued
+  }
+  std::vector<float> rtcsm_scores;
+  bool have_scores = false;
+  int status = DL_OK;
+  // Sub-batch boundaries. Device-resident scans: equal parts. Host scans: the upload is the long pole and the kernels of
+  // the LAST sub-batch are exposed after its copy ends, so the last parts shrink (shares 1 : ... : 1 : 1/2 : 1/4) — their
+  // back halves are latency-bound (~0.6 ms however few scans), so only the front-half time shrinks with them.
+  std::vector<int> bounds(chunks + 1, 0);
+  {
+    std::vector<double> share(chunks, 1.0);
+    if (host_ranges && chunks >= 3) {
+      share[chunks - 2] = 0.5;
+      share[chunks - 1] = 0.25;
+    }
+    double total = 0, acc = 0;
+    for (double v : share) total += v;
+    for (int k = 0; k < chunks; ++k) {
+      acc += share[k];
+      bounds[k + 1] = k + 1 == chunks ? f.batch : (int)std::lround(f.batch * acc / total);
+    }
+  }
+  for (int k = 0; k < chunks && status == DL_OK; ++k) {
+    const int b0 = bounds[k], b1 = bounds[k + 1], nb = b1 - b0;
+    if (nb <= 0) continue;
+    ctx->stream = (!serial && (k & 1)) ? ctx->aux_stream : main_stream;
+    auto run = [&]() -> int {
+      {
+        StageScope st(ctx, "voxel_filter_first");
+        if (host_ranges && o.host_scan_stride_rows > 0) {
+          int64_t widest = 0;
+          for (int b = b0; b < b1; ++b) widest = std::max(widest, sizes[b]);
+          if (widest > 0)
+            DL_CUDA(ctx, cudaMemcpy2DAsync(d_ranges + (size_t)b0 * in_cap * rf, (size_t)in_cap * rf * 4, host_ranges[b0],
+                                           (size_t)o.host_scan_stride_rows * rf * 4, (size_t)widest * rf * 4, (size_t)nb,
+                                           cudaMemcpyHostToDevice, ctx->copy_stream));
+        } else if (host_ranges) {
+          for (int b = b0; b < b1; ++b)
+            if (sizes[b] > 0)
+              DL_CUDA(ctx, cudaMemcpyAsync(d_ranges + (size_t)b * in_cap * rf, host_ranges[b], (size_t)sizes[b] * rf * 4,
+                                           cudaMemcpyHostToDevice, ctx->copy_stream));
+        }
+        if (host_ranges) {
+          cudaEvent_t ev = ctx->take_event();
+          DL_CUDA(ctx, cudaEventRecord(ev, ctx->copy_stream));
+          DL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev, 0));
+          ctx->event_pool.push_back(ev);  // safe to recycle: the wait has been enqueued
+        }
+        DL_TRY(launch_fe_first_filter(ctx, fa, b0, nb));
+      }
+      if (imu_ready) DL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, imu_ready, 0));
+      {
+        StageScope st(ctx, "ingest_second_filter");
+        DL_TRY(launch_fe_rest(ctx, fa, b0, nb));
+      }
+      {
+        // adaptive voxel filters (high, low resolution) on the tracking-frame returns: one CTA per (scan, filter)
+        StageScope st(ctx, "adaptive_voxel_filter");
+        DL_TRY(launch_adaptive_voxel_filter(ctx, f.returns_tracking + (size_t)b0 * f.cap * 3, 3, f.cap, f.n2 + b0, nb, f.filters, 2,
+                                            f.tableA + (size_t)2 * b0 * f.tcap, f.tcap, f.scratchA + (size_t)4 * b0 * f.cap,
+                                            f.keepA + (size_t)2 * b0 * f.cap, f.countsA + 2 * b0, f.passesA + 64 * b0,
+                                            f.npassesA + 2 * b0, f.croppedA + 2 * b0));
+      }
+      DL_TRY(launch_gather_rows(ctx, f.returns_tracking + (size_t)b0 * f.cap * 3, f.cap, 2, f.keepA + (size_t)2 * b0 * f.cap,
+                                f.countsA + 2 * b0, f.cap, f.clouds + (size_t)2 * b0 * f.cap * 3, 2 * nb));
+      DL_TRY(launch_initial_pose(ctx, nb, f.current_pose + 7 * b0, f.submap_inverse + b0, f.initial_pose + 7 * b0, f.target + 3 * b0));
+      if (rtcsm) {
+        // The angular window depends on the farthest point of each cloud through acosf, which must be the host's to stay
+        // bit-exact: ONE synchronisation per batch brings back the clouds' sizes, farthest points and initial poses; the
+        // candidate tables of all scans then go up in one copy and one launch scores every (scan, rotation, translation),
+        // each scan against its own matching submap's high-resolution grid. The best poses are written into f.initial_pose on
+        // the device, where the solve reads them (the fused solve takes them as the pose part of state j's initial value);
+        // f.target keeps the prediction's translation (LTB:536).
+        std::vector<int32_t> countsA(2 * f.batch);
+        std::vector<double> init(7 * f.batch);
+        std::vector<float> far(f.batch);
+        float* d_far = a.take<float>(f.batch);
+        DL_TRY(launch_max_range_batch(ctx, f.clouds, (int64_t)2 * f.cap * 3, f.countsA, 2, f.batch, 3.f * hi_resolution, d_far));
+        DL_TRY(d2h(ctx, countsA.data(), f.countsA, 2 * f.batch));
+        DL_TRY(d2h(ctx, init.data(), f.initial_pose, 7 * f.batch));
+        DL_TRY(d2h(ctx, far.data(), d_far, f.batch));
+        DL_TRY(sync(ctx));
+        StageScope st(ctx, "rtcsm");
+        std::vector<RtcsmBatchItem> items;
+        std::vector<int32_t> slots;
+        for (int b = 0; b < f.batch; ++b) {
+          if (countsA[2 * b] <= 0) continue;
+          items.push_back(RtcsmBatchItem{submaps.high(b), f.clouds + (size_t)(2 * b) * f.cap * 3, countsA[2 * b],
+                                         pose_from7(init.data() + 7 * b), far[b], nullptr, f.rtcsm_nonpositive + b});
+          slots.push_back(b);
+        }
+        DL_CUDA(ctx, cudaMemsetAsync(f.rtcsm_scores, 0, sizeof(float) * f.batch, ctx->stream));
+        DL_CUDA(ctx, cudaMemsetAsync(f.rtcsm_nonpositive, 0, sizeof(int32_t) * f.batch, ctx->stream));
+        if (!items.empty()) {
+          RtcsmBatchPlan plan;
+          DL_TRY(plan_rtcsm_batch(ctx, o.real_time_correlative_scan_matcher, hi_resolution, items, &plan));
+          plan.take(a);
+          if (a.off > ctx->d_scratch.cap) return ctx->fail(DL_ERR_ARG, "internal: RT-CSM scratch underestimated");
+          DL_TRY(run_rtcsm_batch(ctx, items, plan));
+          int32_t* d_slots = a.take<int32_t>(items.size());
+          DL_TRY(h2d(ctx, d_slots, slots.data(), slots.size()));
+          DL_TRY(launch_rtcsm_pick(ctx, plan.d_scans, (int)items.size(), f.initial_pose, d_slots, f.rtcsm_scores, d_slots));
+          DL_TRY(sync(ctx));  // `slots` is pageable and local
+        }
+        have_scores = true;
+      }
+      {
+        StageScope st(ctx, "nls_solve");
+        NlsOptions no = to_nls_options(o.ceres_scan_matcher, 2);
+        no.cluster = solve_cluster_size(ctx, o, nb);
+        if (imu || raw)  // pose part of the initial state comes from problems[].initial_dev like the plain solve's
+          DL_TRY(launch_nls_fused(ctx, no, f.problems + b0, m.d_terms + b0, m.d_init16 + 16 * b0, nb, m.d_fused + b0));
+        else
+          DL_TRY(launch_nls(ctx, no, f.problems + b0, nb, f.nls_out + b0));
+      }
+      ResultArgs ra{};
+      ra.batch = nb; ra.first_counts = f.n1 + b0; ra.return_counts = f.n2 + b0; ra.miss_counts = f.n3 + b0;
+      ra.adaptive_counts = f.countsA + 2 * b0; ra.adaptive_cropped = f.croppedA + 2 * b0; ra.adaptive_passes = f.npassesA + 2 * b0;
+      ra.rtcsm_scores = have_scores ? f.rtcsm_scores + b0 : nullptr; ra.nls = f.nls_out + b0; ra.fused = (imu || raw) ? m.d_fused + b0 : nullptr; ra.submap = f.submap + b0;
+      ra.results = d_results + b0; ra.error_flag = f.error_flag + b0;
+      ra.imu_ok = m.d_ok ? m.d_ok + b0 : nullptr; ra.states_out = m.d_states ? m.d_states + b0 : nullptr;
+      DL_TRY(launch_finalize_results(ctx, ra));
+      return DL_OK;
+    };
+    status = run();
+  }
+  ctx->stream = main_stream;
+  if (imu_ready) ctx->event_pool.push_back(imu_ready);
+  if (chunks > 1) {  // later work on the main stream (result copies, the next call) waits for the other stream
+    cudaEvent_t joined = ctx->take_event();
+    DL_CUDA(ctx, cudaEventRecord(joined, ctx->aux_stream));
+    DL_CUDA(ctx, cudaStreamWaitEvent(main_stream, joined, 0));
+    ctx->event_pool.push_back(joined);
+  }
+  return status;
+}
+
+int check_frontend(dl_context* ctx, const dl_frontend_options* o, int num_scans, const int64_t* sizes,
+                   const SubmapSet& submaps, int64_t* max_size) {
+  if (!o || num_scans < 0 || !submaps.hi || !submaps.lo || (num_scans > 0 && !sizes)) return DL_ERR_ARG;
+  for (int b = 0; b < (submaps.per_scan ? num_scans : 1); ++b) {
+    if (!submaps.high(b) || !submaps.low(b)) return DL_ERR_ARG;
+    if (submaps.high(b)->structure_dirty || submaps.low(b)->structure_dirty)
+      return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+    // the pre-match's candidate tables and the 3 * resolution floor of the farthest point take one resolution per batch
+    if (o->use_online_correlative_scan_matching && submaps.high(b)->resolution != submaps.high(0)->resolution)
+      return ctx->fail(DL_ERR_ARG, "the correlative pre-match takes one high-resolution grid resolution per batch");
+  }
+  DL_TRY(check_ceres_options(ctx, &o->ceres_scan_matcher, 2));
+  int64_t m = 0;
+  for (int b = 0; b < num_scans; ++b) {
+    if (sizes[b] < 0 || sizes[b] > 0x3fffffff) return ctx->fail(DL_ERR_ARG, "scan size out of range");
+    m = std::max(m, sizes[b]);
+  }
+  *max_size = m;
+  if (o->range_row_floats == 3 && num_scans > 0) {
+    if (!o->time_run_offsets || !o->time_run_first_row || !o->time_run_value)
+      return ctx->fail(DL_ERR_ARG, "range_row_floats = 3 needs the time_run_* arrays");
+    if (o->time_run_offsets[0] != 0) return ctx->fail(DL_ERR_ARG, "time_run_offsets[0] must be 0");
+    for (int b = 0; b < num_scans; ++b) {
+      const int32_t r0 = o->time_run_offsets[b], r1 = o->time_run_offsets[b + 1];
+      if (r1 < r0 || (sizes[b] > 0 && r1 == r0)) return ctx->fail(DL_ERR_ARG, "every non-empty scan needs at least one time run");
+      // O(scans) checks only (this runs on the issue path of every batch): first run at row 0, last run inside the scan. The
+      // kernels clamp every run to its scan, so a table that does not ascend gives wrong times, never a wild access.
+      if (r1 > r0 && (o->time_run_first_row[r0] != 0 || o->time_run_first_row[r1 - 1] >= std::max<int64_t>(sizes[b], 1) ||
+                      o->time_run_first_row[r1 - 1] < 0))
+        return ctx->fail(DL_ERR_ARG, "time_run_first_row must start at 0 and stay inside the scan");
+    }
+  }
+  return DL_OK;
+}
+
+}  // namespace
+
+namespace dl {
+
+int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int num_scans, const FrontendScans& in,
+                     const int64_t* sizes, const float* origins, int num_origins, const double* prev_poses,
+                     const double* predicted_poses, const SubmapSet& submaps, dl_scan_result** d_results_out, ImuRun* imu,
+                     FrontendBuffers* buffers_out, const int32_t* origin_base, const std::function<void(Arena&)>* more) {
+  int64_t max_size = 0;
+  DL_TRY(check_frontend(ctx, options, num_scans, sizes, submaps, &max_size));
+  if (num_scans == 0) return DL_OK;
+  const bool raw = imu && imu->samples;
+  if (!origins || num_origins < 1 || (!raw && (!prev_poses || !predicted_poses)) || !submaps.poses) return DL_ERR_ARG;
+  if (in.on_device) {
+    if (!in.dev || !in.results_dev || (imu && !imu->d_states_out) || in.cap_rows < max_size || in.cap_rows < 1) return DL_ERR_ARG;
+  } else {
+    if (!in.host) return DL_ERR_ARG;
+    for (int b = 0; b < num_scans; ++b)
+      if (sizes[b] > 0 && !in.host[b]) return DL_ERR_ARG;
+    if (options->host_scan_stride_rows != 0) {
+      const int64_t stride = options->host_scan_stride_rows;
+      const size_t row_bytes = (size_t)row_floats_of(*options) * 4;
+      if (stride < max_size) return ctx->fail(DL_ERR_ARG, "host_scan_stride_rows is smaller than a scan");
+      for (int b = 0; b < num_scans; ++b)
+        if ((const char*)in.host[b] != (const char*)in.host[0] + (size_t)b * stride * row_bytes)
+          return ctx->fail(DL_ERR_ARG, "host_scan_stride_rows does not describe the ranges pointers");
+    }
+  }
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int64_t cap = in.on_device ? in.cap_rows : std::max<int64_t>(max_size, 1);
+  // The correlative pre-match takes its candidate tables after the carve (see rtcsm_scratch_bound).
+  const size_t rtcsm_extra = options->use_online_correlative_scan_matching
+      ? (size_t)num_scans * rtcsm_scratch_bound(options->real_time_correlative_scan_matcher, submaps.high(0)->resolution,
+                                                options->high_resolution_adaptive_voxel_filter.max_range)
+      : 0;
+  float* d_ranges;
+  dl_scan_result* d_results;
+  FrontendBuffers f;
+  Arena rest(nullptr);
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_ranges = in.on_device ? (float*)in.dev : a.take<float>((size_t)num_scans * cap * 8);
+    d_results = in.on_device ? in.results_dev : a.take<dl_scan_result>(num_scans);
+    carve(a, num_scans, cap, num_origins, &f);
+    if (imu) carve_imu(a, num_scans, imu);
+    carve_time_runs(a, *options, num_scans, &f);
+    if (more) (*more)(a);
+    carve_prematch(a, *options, num_scans, &f);
+  }, rtcsm_extra, &rest));
+  if (d_results_out) *d_results_out = d_results;
+  if (buffers_out) *buffers_out = f;
+  return frontend_run(ctx, *options, num_scans, d_ranges, cap, in.host, sizes, origins, num_origins, origin_base, prev_poses,
+                      predicted_poses, submaps, f, rest, d_results, imu);
+}
+
+int check_imu_options(dl_context* ctx, const dl_frontend_options* options) {
+  if (options && options->ceres_scan_matcher.only_optimize_yaw)
+    return ctx->fail(DL_ERR_ARG, "only_optimize_yaw is not supported by the fused solve");
+  return DL_OK;
+}
+
+int check_imu_samples(dl_context* ctx, const dl_frontend_options* options, const dl_frontend_imu_samples* imu, int num_scans) {
+  if (!imu || num_scans < 0) return DL_ERR_ARG;
+  if (num_scans == 0) return DL_OK;
+  if (!imu->states_i || !imu->offsets || !(imu->imu_weight >= 0.)) return DL_ERR_ARG;
+  if (imu->offsets[0] != 0) return ctx->fail(DL_ERR_ARG, "offsets[0] must be 0");
+  for (int k = 0; k < num_scans; ++k)
+    if (imu->offsets[k + 1] < imu->offsets[k]) return ctx->fail(DL_ERR_ARG, "offsets must be non-decreasing");
+  if (imu->offsets[num_scans] > 0 && (!imu->dt || !imu->acc || !imu->gyr)) return DL_ERR_ARG;
+  return check_imu_options(ctx, options);
+}
+
+}  // namespace dl
+
+extern "C" {
+
+int dl_frontend_match_batch_dev(dl_context* ctx, const dl_frontend_options* options, int32_t num_scans,
+                                const void* ranges_dev, int64_t cap_rows, const int64_t* sizes, const float* origins,
+                                int32_t num_origins, const double* prev_poses, const double* predicted_poses,
+                                const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo,
+                                dl_scan_result* results_dev) {
+  if (!ctx) return DL_ERR_ARG;
+  FrontendScans in;
+  in.on_device = true;
+  in.dev = ranges_dev;
+  in.cap_rows = cap_rows;
+  in.results_dev = results_dev;
+  return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, prev_poses, predicted_poses,
+                          OneSubmap(submap_local_pose, hi, lo), nullptr);
+}
+
+int dl_frontend_fetch_results(dl_context* ctx, const dl_scan_result* results_dev, int32_t num_scans,
+                              dl_scan_result* results) {
+  if (!ctx || num_scans < 0 || (num_scans > 0 && (!results_dev || !results))) return DL_ERR_ARG;
+  DL_TRY(d2h(ctx, results, results_dev, num_scans));
+  return sync(ctx);
+}
+
+int dl_frontend_match_batch(dl_context* ctx, const dl_frontend_options* options, int32_t num_scans,
+                            const void* const* ranges, const int64_t* sizes, const float* origins, int32_t num_origins,
+                            const double* prev_poses, const double* predicted_poses, const double* submap_local_pose,
+                            const dl_grid* hi, const dl_grid* lo, dl_scan_result* results) {
+  if (!ctx) return DL_ERR_ARG;
+  if (num_scans == 0) {
+    int64_t m = 0;
+    return check_frontend(ctx, options, num_scans, sizes, OneSubmap(submap_local_pose, hi, lo), &m);
+  }
+  if (!results) return DL_ERR_ARG;
+  dl_scan_result* d_results = nullptr;
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev_poses, predicted_poses,
+                          OneSubmap(submap_local_pose, hi, lo), &d_results));
+  DL_TRY(d2h(ctx, results, d_results, num_scans));
+  return sync(ctx);
+}
+
+int dl_frontend_match_batch_imu(dl_context* ctx, const dl_frontend_options* options, const dl_frontend_imu* imu,
+                                int32_t num_scans, const void* const* ranges, const int64_t* sizes, const float* origins,
+                                int32_t num_origins, const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo,
+                                dl_scan_result* results) {
+  if (!ctx || !imu) return DL_ERR_ARG;
+  if (num_scans == 0) return DL_OK;
+  if (num_scans < 0 || !results || !imu->states_i || !imu->predicted_states || !imu->preintegrations || !imu->states_out ||
+      !(imu->imu_weight >= 0.))
+    return DL_ERR_ARG;
+  DL_TRY(check_imu_options(ctx, options));
+  std::vector<double> prev((size_t)num_scans * 7), pred((size_t)num_scans * 7);
+  for (int b = 0; b < num_scans; ++b) {
+    const dl_nav_state& si = imu->states_i[b];
+    const dl_nav_state& sj = imu->predicted_states[b];
+    for (int k = 0; k < 3; ++k) { prev[7 * b + k] = si.p[k]; pred[7 * b + k] = sj.p[k]; }
+    for (int k = 0; k < 4; ++k) { prev[7 * b + 3 + k] = si.q[k]; pred[7 * b + 3 + k] = sj.q[k]; }
+  }
+  dl_scan_result* d_results = nullptr;
+  ImuRun run;
+  run.host = imu;
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev.data(), pred.data(),
+                          OneSubmap(submap_local_pose, hi, lo), &d_results, &run));
+  DL_TRY(d2h(ctx, results, d_results, num_scans));
+  DL_TRY(d2h(ctx, imu->states_out, run.d_states, num_scans));
+  return sync(ctx);
+}
+
+int dl_frontend_match_batch_imu_samples(dl_context* ctx, const dl_frontend_options* options, const dl_frontend_imu_samples* imu,
+                                        int32_t num_scans, const void* const* ranges, const int64_t* sizes, const float* origins,
+                                        int32_t num_origins, const double* submap_local_pose, const dl_grid* hi,
+                                        const dl_grid* lo, dl_scan_result* results, dl_nav_state* states_out,
+                                        dl_nav_state* predicted_states_out) {
+  if (!ctx) return DL_ERR_ARG;
+  DL_TRY(check_imu_samples(ctx, options, imu, num_scans));
+  if (num_scans == 0) return DL_OK;
+  if (!results || !states_out) return DL_ERR_ARG;
+  dl_scan_result* d_results = nullptr;
+  ImuRun run;
+  run.samples = imu;
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, nullptr, nullptr,
+                          OneSubmap(submap_local_pose, hi, lo), &d_results, &run));
+  DL_TRY(d2h(ctx, results, d_results, num_scans));
+  DL_TRY(d2h(ctx, states_out, run.d_states, num_scans));
+  if (predicted_states_out) DL_TRY(d2h(ctx, predicted_states_out, run.d_predicted, num_scans));
+  return sync(ctx);
+}
+
+int dl_frontend_match_batch_imu_samples_dev(dl_context* ctx, const dl_frontend_options* options,
+                                            const dl_frontend_imu_samples* imu, int32_t num_scans, const void* ranges_dev,
+                                            int64_t cap_rows, const int64_t* sizes, const float* origins, int32_t num_origins,
+                                            const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo,
+                                            dl_scan_result* results_dev, dl_nav_state* states_out_dev) {
+  if (!ctx) return DL_ERR_ARG;
+  DL_TRY(check_imu_samples(ctx, options, imu, num_scans));
+  FrontendScans in;
+  in.on_device = true;
+  in.dev = ranges_dev;
+  in.cap_rows = cap_rows;
+  in.results_dev = results_dev;
+  ImuRun run;
+  run.samples = imu;
+  run.d_states_out = states_out_dev;
+  return frontend_enqueue(ctx, options, num_scans, in, sizes, origins, num_origins, nullptr, nullptr, OneSubmap(submap_local_pose, hi, lo),
+                          nullptr, &run);
+}
+
+// Tail of a submit: the results (and, with the IMU, the estimated states) go to pinned staging behind the batch.
+static int submit_finish(dl_context* ctx, int num_scans, int num_origins, const dl_scan_result* d_results,
+                         const dl_nav_state* d_states) {
+  Staging s;
+  Arena h(ctx->h_pinned.get());  // the block frontend_upload_small reserved for this batch
+  carve_staging(h, num_scans, num_origins, &s);
+  DL_CUDA(ctx, cudaMemcpyAsync(s.results, d_results, (size_t)num_scans * sizeof(dl_scan_result), cudaMemcpyDeviceToHost,
+                               ctx->stream));
+  if (d_states)
+    DL_CUDA(ctx, cudaMemcpyAsync(s.states, d_states, (size_t)num_scans * sizeof(dl_nav_state), cudaMemcpyDeviceToHost, ctx->stream));
+  DL_CUDA(ctx, cudaEventRecord(ctx->batch_done, ctx->stream));
+  ctx->in_flight = num_scans;
+  ctx->in_flight_states = d_states != nullptr;
+  ctx->staged_results = s.results;
+  ctx->staged_states = s.states;
+  return DL_OK;
+}
+
+int dl_frontend_submit(dl_context* ctx, const dl_frontend_options* options, int32_t num_scans, const void* const* ranges,
+                       const int64_t* sizes, const float* origins, int32_t num_origins, const double* prev_poses,
+                       const double* predicted_poses, const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo) {
+  if (!ctx || num_scans < 1) return DL_ERR_ARG;
+  if (ctx->in_flight) return ctx->fail(DL_ERR_ARG, "a submitted batch is already in flight on this context");
+  dl_scan_result* d_results = nullptr;
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, prev_poses, predicted_poses,
+                          OneSubmap(submap_local_pose, hi, lo), &d_results));
+  return submit_finish(ctx, num_scans, num_origins, d_results, nullptr);
+}
+
+int dl_frontend_submit_imu_samples(dl_context* ctx, const dl_frontend_options* options, const dl_frontend_imu_samples* imu,
+                                   int32_t num_scans, const void* const* ranges, const int64_t* sizes, const float* origins,
+                                   int32_t num_origins, const double* submap_local_pose, const dl_grid* hi, const dl_grid* lo) {
+  if (!ctx || num_scans < 1) return DL_ERR_ARG;
+  if (ctx->in_flight) return ctx->fail(DL_ERR_ARG, "a submitted batch is already in flight on this context");
+  DL_TRY(check_imu_samples(ctx, options, imu, num_scans));
+  dl_scan_result* d_results = nullptr;
+  ImuRun run;
+  run.samples = imu;
+  DL_TRY(frontend_enqueue(ctx, options, num_scans, FrontendScans{ranges}, sizes, origins, num_origins, nullptr, nullptr, OneSubmap(submap_local_pose, hi, lo), &d_results, &run));
+  return submit_finish(ctx, num_scans, num_origins, d_results, run.d_states);
+}
+
+static int collect_common(dl_context* ctx, int32_t num_scans, dl_scan_result* results, dl_nav_state* states_out) {
+  if (!ctx || !results) return DL_ERR_ARG;
+  if (!ctx->in_flight) return ctx->fail(DL_ERR_ARG, "no submitted batch on this context");
+  if (num_scans != ctx->in_flight) return ctx->fail(DL_ERR_ARG, "num_scans differs from the submitted batch");
+  if (states_out && !ctx->in_flight_states) return ctx->fail(DL_ERR_ARG, "the submitted batch carries no IMU states");
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaError_t e = cudaEventSynchronize(ctx->batch_done);
+  ctx->in_flight = 0;
+  if (e != cudaSuccess) return ctx->cuda_fail(e, "dl_frontend_collect");
+  std::memcpy(results, ctx->staged_results, (size_t)num_scans * sizeof(dl_scan_result));
+  if (states_out) std::memcpy(states_out, ctx->staged_states, (size_t)num_scans * sizeof(dl_nav_state));
+  return DL_OK;
+}
+int dl_frontend_collect(dl_context* ctx, int32_t num_scans, dl_scan_result* results) {
+  return collect_common(ctx, num_scans, results, nullptr);
+}
+int dl_frontend_collect_imu(dl_context* ctx, int32_t num_scans, dl_scan_result* results, dl_nav_state* states_out) {
+  if (!states_out) return DL_ERR_ARG;
+  return collect_common(ctx, num_scans, results, states_out);
+}
+
+int dl_ingest_scan(dl_context* ctx, const dl_frontend_options* options, const void* ranges, int64_t n,
+                   const float* origins, int32_t num_origins, const double* prev_pose, const double* predicted_pose,
+                   int64_t* first_keep_out, float* returns_local_out, float* returns_tracking_out,
+                   float* misses_tracking_out, float* current_pose7f_out, int64_t* counts_out) {
+  if (!ctx || !options || !ranges || n < 1 || n > 0x3fffffff || !origins || num_origins < 1 || !prev_pose || !predicted_pose ||
+      !counts_out)
+    return DL_ERR_ARG;
+  if (row_floats_of(*options) != 8) return ctx->fail(DL_ERR_ARG, "dl_ingest_scan takes RangeMeasurement rows (range_row_floats = 8)");
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  float* d_ranges;
+  FrontendBuffers f;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_ranges = a.take<float>((size_t)n * 8);
+    carve(a, 1, n, num_origins, &f);
+  }));
+  DL_TRY(h2d(ctx, d_ranges, (const float*)ranges, (size_t)n * 8));
+  DL_TRY(frontend_upload_small(ctx, *options, f, &n, origins, num_origins, prev_pose, predicted_pose, nullptr, nullptr));
+  // fe_ingest_tile writes the local record of a return or a miss only: zeroed records read as class 0 for every other row
+  DL_CUDA(ctx, cudaMemsetAsync(f.local4, 0, (size_t)n * 4 * sizeof(float), ctx->stream));
+  const FrontendArgs fa = make_frontend_args(*options, f, d_ranges, n, 8);
+  DL_TRY(launch_fe_prepare(ctx, fa, 1));
+  DL_TRY(launch_fe_first_filter(ctx, fa, 0, 1));
+  DL_TRY(launch_fe_rest(ctx, fa, 0, 1));
+  int32_t c[4], error_flag;
+  DL_TRY(d2h(ctx, &c[0], f.n1, 1));
+  DL_TRY(d2h(ctx, &c[1], f.n_ret, 1));
+  DL_TRY(d2h(ctx, &c[2], f.n2, 1));
+  DL_TRY(d2h(ctx, &c[3], f.n3, 1));
+  DL_TRY(d2h(ctx, &error_flag, f.error_flag, 1));
+  std::vector<uint32_t> first_bits(f.bit_words);
+  DL_TRY(d2h(ctx, first_bits.data(), f.first_bits, first_bits.size()));
+  std::vector<float> local(returns_local_out ? (size_t)n * 4 : 0);  // float4 per row: local-frame point, class in .w
+  DL_TRY(d2h(ctx, local.data(), f.local4, local.size()));
+  DL_TRY(sync(ctx));
+  for (int i = 0; i < 4; ++i) counts_out[i] = c[i];
+  if (error_flag)
+    return ctx->fail(DL_ERR_ARG, "a point lies outside the voxel-key span of the second voxel filter (dl_scan_result.ok = -1)");
+  if (returns_tracking_out) DL_TRY(d2h(ctx, returns_tracking_out, f.returns_tracking, (size_t)c[2] * 3));
+  if (misses_tracking_out) DL_TRY(d2h(ctx, misses_tracking_out, f.misses_tracking, (size_t)c[3] * 3));
+  if (current_pose7f_out) DL_TRY(d2h(ctx, current_pose7f_out, f.current_pose, 7));
+  DL_TRY(sync(ctx));
+  // first_keep: the rows of the first filter's bitmap in index order; returns_local: those of them in class 1 (a return)
+  int64_t kept = 0, returns = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    if (!(first_bits[i >> 5] >> (i & 31) & 1u)) continue;
+    if (first_keep_out) first_keep_out[kept++] = i;
+    if (!returns_local_out) continue;
+    int32_t cls;
+    std::memcpy(&cls, &local[4 * i + 3], sizeof(cls));
+    if (cls == 1) std::memcpy(returns_local_out + 3 * returns++, &local[4 * i], 3 * sizeof(float));
+  }
+  return DL_OK;
+}
+
+}  // extern "C"

@@ -20,6 +20,7 @@
 // order libstdc++'s insertion sort gives slices of at most 16 points; std::sort leaves it unspecified beyond), with -0 and +0
 // equal as std::sort's operator< sees them. tests/test_gpu_rotational_histogram.py checks bit equality on clouds cleared of
 // such points and, on scene clouds, that any difference comes from one.
+#include <algorithm>
 #include <vector>
 
 #include "dl_internal.cuh"
@@ -329,3 +330,27 @@ int launch_rotational_histograms(dl_context* ctx, const HistogramScratch* s, con
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ rotational histogram
+using namespace dl;
+
+extern "C" int dl_rotational_histogram(dl_context* ctx, const float* points, int64_t n, int32_t size, float* histogram_out) {
+  if (!ctx || n < 0 || (n > 0 && !points) || !histogram_out) return DL_ERR_ARG;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  float *d_pts, *d_hist;
+  HistogramScratch hs;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(3 * (size_t)std::max<int64_t>(n, 1));
+    d_hist = a.take<float>(std::max(size, 1));
+    carve_rotational_histogram(a, n, &hs);
+  }));
+  DL_TRY(h2d(ctx, d_pts, points, 3 * (size_t)n));
+  int32_t* d_err = nullptr;
+  DL_TRY(launch_rotational_histogram(ctx, hs, d_pts, n, size, d_hist, &d_err));
+  int32_t err = 0;
+  DL_TRY(d2h(ctx, histogram_out, d_hist, (size_t)size));
+  DL_TRY(d2h(ctx, &err, d_err, 1));
+  DL_TRY(sync(ctx));
+  if (err) return ctx->fail(DL_ERR_ARG, "a point lies outside +-2^19 slices of 0.2 m");
+  return DL_OK;
+}

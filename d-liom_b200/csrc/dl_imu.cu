@@ -6,6 +6,11 @@
 // one interval are inherently sequential (~20 at 200 Hz), so the parallelism is (a) across scans: one warp each, and
 // (b) inside a step: the three 15x15 products F*J, F*P*F^T, V*N*V^T are spread over the 32 lanes. The state lives in
 // shared memory (4 warps per CTA, 9.6 KB each). Row/column order: delta_p, delta_theta, delta_v, b_a, b_g.
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
 #include "dl_internal.cuh"
 #include "dl_pipeline.cuh"
 
@@ -179,7 +184,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) imu_preintegrate_kernel(
 // IMU samples needs no host round trip: state prediction (dl_imu_predict's arithmetic = the front end's
 // pose prediction, LTB:188-199), the deskew constants of LTB:426-428, the pre-integration factor moved into the submap
 // frame, and its information matrix W = weight^2 * Sigma^-1 (Sigma = L L^T, W = L^-T L^-1; the same operation order as the
-// host path in dl_api.cu, so both produce the same bits). One warp per scan; lane i owns row / column i of the 15x15 work.
+// host path, information_matrix below, so both produce the same bits). One warp per scan; lane i owns row / column i of
+// the 15x15 work.
 struct PrepareShared {
   double L[15][15], Li[15][15];
 };
@@ -282,3 +288,250 @@ int launch_imu_preintegrate(dl_context* ctx, int count, const int32_t* offsets, 
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ IMU
+using namespace dl;
+
+namespace {
+// W = weight^2 * Sigma^-1 by Cholesky (Sigma = L L^T, W = L^-T L^-1). False if Sigma is not positive definite.
+bool information_matrix(const double* sigma, double weight, double* W) {
+  double L[15][15] = {};
+  for (int i = 0; i < 15; ++i)
+    for (int j = 0; j <= i; ++j) {
+      double s = sigma[i * 15 + j];
+      for (int k = 0; k < j; ++k) s -= L[i][k] * L[j][k];
+      if (i == j) {
+        if (!(s > 0)) return false;
+        L[i][i] = std::sqrt(s);
+      } else {
+        L[i][j] = s / L[j][j];
+      }
+    }
+  double Li[15][15] = {};  // L^-1 (lower)
+  for (int c = 0; c < 15; ++c) {
+    for (int i = c; i < 15; ++i) {
+      double s = i == c ? 1.0 : 0.0;
+      for (int k = c; k < i; ++k) s -= L[i][k] * Li[k][c];
+      Li[i][c] = s / L[i][i];
+    }
+  }
+  for (int a = 0; a < 15; ++a)
+    for (int b = 0; b < 15; ++b) {
+      double s = 0;
+      for (int k = std::max(a, b); k < 15; ++k) s += Li[k][a] * Li[k][b];
+      W[a * 15 + b] = weight * weight * s;
+    }
+  return true;
+}
+// Solver state (submap frame) -> dl_nav_state in the local frame.
+void state_to_local(const Rigidd& submap, const double* x, dl_nav_state* o) {
+  const Rigidd pose = compose(submap, pose_from7(x));
+  const Vec3d v = rotate(submap.q, Vec3d{x[7], x[8], x[9]});
+  o->p[0] = pose.t.x; o->p[1] = pose.t.y; o->p[2] = pose.t.z;
+  o->q[0] = pose.q.w; o->q[1] = pose.q.x; o->q[2] = pose.q.y; o->q[3] = pose.q.z;
+  o->v[0] = v.x; o->v[1] = v.y; o->v[2] = v.z;
+  for (int k = 0; k < 3; ++k) { o->ba[k] = x[10 + k]; o->bg[k] = x[13 + k]; }
+}
+}  // namespace
+
+namespace dl {
+// One pre-integration factor in the submap frame (the grids live there and the solve is frame-invariant) + the initial
+// 16-vector of state j. False if the covariance is not positive definite.
+bool build_imu_term(const Rigidd& to_submap, const dl_nav_state& si, const dl_nav_state& sj, const dl_preintegration& m,
+                    const double* gravity, double imu_weight, ImuTerm* t, double* x16) {
+  const Rigidd pose_i = compose(to_submap, Rigidd{{si.p[0], si.p[1], si.p[2]}, {si.q[0], si.q[1], si.q[2], si.q[3]}});
+  const Rigidd pose_j = compose(to_submap, Rigidd{{sj.p[0], sj.p[1], sj.p[2]}, {sj.q[0], sj.q[1], sj.q[2], sj.q[3]}});
+  const Vec3d vi = rotate(to_submap.q, Vec3d{si.v[0], si.v[1], si.v[2]});
+  const Vec3d vj = rotate(to_submap.q, Vec3d{sj.v[0], sj.v[1], sj.v[2]});
+  const Vec3d G = rotate(to_submap.q, Vec3d{gravity[0], gravity[1], gravity[2]});
+  t->pi[0] = pose_i.t.x; t->pi[1] = pose_i.t.y; t->pi[2] = pose_i.t.z;
+  t->qi[0] = pose_i.q.w; t->qi[1] = pose_i.q.x; t->qi[2] = pose_i.q.y; t->qi[3] = pose_i.q.z;
+  t->vi[0] = vi.x; t->vi[1] = vi.y; t->vi[2] = vi.z;
+  imu_term_deltas(m, si.ba, si.bg, t);
+  t->G[0] = G.x; t->G[1] = G.y; t->G[2] = G.z;
+  t->sum_dt = m.sum_dt;
+  if (!information_matrix(m.covariance, imu_weight, t->W)) return false;
+  pose_to7(pose_j, x16);
+  x16[7] = vj.x; x16[8] = vj.y; x16[9] = vj.z;
+  for (int k = 0; k < 3; ++k) { x16[10 + k] = sj.ba[k]; x16[13 + k] = sj.bg[k]; }
+  return true;
+}
+}  // namespace dl
+
+extern "C" {
+
+int dl_imu_preintegrate(dl_context* ctx, const dl_imu_noise* noise, int32_t count, const int32_t* offsets,
+                        const double* dt, const double* acc, const double* gyr, const double* biases,
+                        dl_preintegration* out) {
+  if (!ctx || !noise || count < 0 || (count > 0 && (!offsets || !dt || !acc || !gyr || !biases || !out))) return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t n = (size_t)offsets[count];
+  for (int k = 0; k < count; ++k)
+    if (offsets[k + 1] < offsets[k]) return ctx->fail(DL_ERR_ARG, "offsets must be non-decreasing");
+  int32_t* d_off;
+  double *d_dt, *d_acc, *d_gyr, *d_bias;
+  dl_preintegration* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_off = a.take<int32_t>(count + 1);
+    d_dt = a.take<double>(n);
+    d_acc = a.take<double>(3 * n);
+    d_gyr = a.take<double>(3 * n);
+    d_bias = a.take<double>(6 * (size_t)count);
+    d_out = a.take<dl_preintegration>(count);
+  }));
+  DL_TRY(h2d(ctx, d_off, offsets, count + 1));
+  DL_TRY(h2d(ctx, d_dt, dt, n));
+  DL_TRY(h2d(ctx, d_acc, acc, 3 * n));
+  DL_TRY(h2d(ctx, d_gyr, gyr, 3 * n));
+  DL_TRY(h2d(ctx, d_bias, biases, 6 * (size_t)count));
+  DL_TRY(launch_imu_preintegrate(ctx, count, d_off, d_dt, d_acc, d_gyr, d_bias, 6, *noise, d_out));
+  DL_TRY(d2h(ctx, out, d_out, count));
+  return sync(ctx);
+}
+
+int dl_imu_predict(const dl_nav_state* si, const dl_preintegration* m, const double* gravity, dl_nav_state* sj) {
+  if (!si || !m || !gravity || !sj) return DL_ERR_ARG;
+  const double T = m->sum_dt;
+  const Quatd qi{si->q[0], si->q[1], si->q[2], si->q[3]};
+  const Vec3d G{gravity[0], gravity[1], gravity[2]};
+  const Vec3d p = add(sub(add(Vec3d{si->p[0], si->p[1], si->p[2]}, mul(T, Vec3d{si->v[0], si->v[1], si->v[2]})), mul(0.5 * T * T, G)),
+                      rotate(qi, Vec3d{m->delta_p[0], m->delta_p[1], m->delta_p[2]}));
+  const Vec3d v = add(sub(Vec3d{si->v[0], si->v[1], si->v[2]}, mul(T, G)), rotate(qi, Vec3d{m->delta_v[0], m->delta_v[1], m->delta_v[2]}));
+  const Quatd q = qnormalized(qmul(qi, Quatd{m->delta_q[0], m->delta_q[1], m->delta_q[2], m->delta_q[3]}));
+  *sj = *si;
+  sj->p[0] = p.x; sj->p[1] = p.y; sj->p[2] = p.z;
+  sj->v[0] = v.x; sj->v[1] = v.y; sj->v[2] = v.z;
+  sj->q[0] = q.w; sj->q[1] = q.x; sj->q[2] = q.y; sj->q[3] = q.z;
+  return DL_OK;
+}
+
+int dl_imu_factor_evaluate(dl_context* ctx, int32_t count, const dl_nav_state* states_i, const dl_preintegration* preintegrations,
+                           const double* submap_local_poses, const double* gravity, double imu_weight, const double* x16,
+                           int32_t* ok, dl_nav_state* predicted, double* information, double* residual, double* hessian,
+                           double* gradient, double* cost2) {
+  if (!ctx || count < 0 || !gravity || !(imu_weight >= 0.) ||
+      (count > 0 && (!states_i || !preintegrations || !submap_local_poses || !ok || !predicted || !information || !residual ||
+                     !hessian || !gradient || !cost2)))
+    return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  dl_preintegration* d_pre;
+  dl_nav_state *d_si, *d_pred;
+  Rigidd* d_to_submap;
+  ScanConstants* d_scans;
+  ImuTerm* d_terms;
+  double *d_init, *d_x, *d_out;
+  int32_t* d_ok;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pre = a.take<dl_preintegration>(count);
+    d_si = a.take<dl_nav_state>(count);
+    d_pred = a.take<dl_nav_state>(count);
+    d_to_submap = a.take<Rigidd>(count);
+    d_scans = a.take<ScanConstants>(count);
+    d_terms = a.take<ImuTerm>(count);
+    d_init = a.take<double>((size_t)count * 16);
+    d_x = x16 ? a.take<double>((size_t)count * 16) : nullptr;
+    d_out = a.take<double>((size_t)count * kImuFactorOutDoubles);
+    d_ok = a.take<int32_t>(count);
+  }));
+  std::vector<Rigidd> to_submap(count);
+  for (int c = 0; c < count; ++c) to_submap[c] = inverse(pose_from7(submap_local_poses + 7 * c));
+  DL_TRY(h2d(ctx, d_pre, preintegrations, count));
+  DL_TRY(h2d(ctx, d_si, states_i, count));
+  DL_TRY(h2d(ctx, d_to_submap, to_submap.data(), count));
+  if (x16) DL_TRY(h2d(ctx, d_x, x16, (size_t)count * 16));
+  ImuPrepareArgs pa{};
+  pa.count = count; pa.preint = d_pre; pa.states_i = d_si; pa.to_submap = d_to_submap;
+  for (int k = 0; k < 3; ++k) pa.gravity[k] = gravity[k];
+  pa.imu_weight = imu_weight; pa.scans = d_scans; pa.terms = d_terms; pa.init16 = d_init; pa.predicted = d_pred; pa.ok = d_ok;
+  DL_TRY(launch_imu_prepare(ctx, pa));
+  DL_TRY(launch_imu_factor_evaluate(ctx, count, d_terms, d_ok, x16 ? d_x : d_init, d_out));
+  std::vector<ImuTerm> terms(count);
+  std::vector<double> out((size_t)count * kImuFactorOutDoubles);
+  DL_TRY(d2h(ctx, ok, d_ok, count));
+  DL_TRY(d2h(ctx, predicted, d_pred, count));
+  DL_TRY(d2h(ctx, terms.data(), d_terms, count));
+  DL_TRY(d2h(ctx, out.data(), d_out, out.size()));
+  DL_TRY(sync(ctx));
+  for (int c = 0; c < count; ++c) {
+    const double* o = out.data() + (size_t)c * kImuFactorOutDoubles;
+    const bool good = ok[c] != 0;
+    for (int e = 0; e < 225; ++e) {
+      information[225 * (size_t)c + e] = good ? terms[c].W[e] : 0.0;
+      hessian[225 * (size_t)c + e] = good ? o[15 + e] : 0.0;
+    }
+    for (int e = 0; e < 15; ++e) {
+      residual[15 * (size_t)c + e] = good ? o[e] : 0.0;
+      gradient[15 * (size_t)c + e] = good ? o[240 + e] : 0.0;
+    }
+    cost2[c] = good ? o[255] : 0.0;
+  }
+  return DL_OK;
+}
+
+int dl_fused_match_batch(dl_context* ctx, const dl_ceres_options* options, double imu_weight, const double* gravity,
+                         int32_t count, int32_t num_pairs, const double* submap_local_poses,
+                         const dl_nav_state* states_i, const dl_nav_state* initial_states_j,
+                         const dl_preintegration* preints, const float* const* clouds, const int64_t* sizes,
+                         const dl_grid* const* grids, dl_nav_state* states_j_out, dl_solve_summary* summaries) {
+  if (!ctx) return DL_ERR_ARG;
+  DL_TRY(check_ceres_options(ctx, options, num_pairs));
+  if (options->only_optimize_yaw) return ctx->fail(DL_ERR_ARG, "only_optimize_yaw is not supported by the fused solve");
+  if (count < 0 || !gravity || !(imu_weight >= 0.) ||
+      (count > 0 && (!submap_local_poses || !states_i || !initial_states_j || !preints || !clouds || !sizes || !grids || !states_j_out)))
+    return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < count * num_pairs; ++i) {
+    if (sizes[i] < 0 || !grids[i] || (sizes[i] > 0 && !clouds[i])) return DL_ERR_ARG;
+    if (sizes[i] == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
+    if (grids[i]->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+  }
+  std::vector<float*> d_clouds(count * num_pairs);
+  NlsProblem* d_problems;
+  ImuTerm* d_terms;
+  double* d_init;
+  FusedOutput* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    for (int i = 0; i < count * num_pairs; ++i) d_clouds[i] = a.take<float>(3 * sizes[i]);
+    d_problems = a.take<NlsProblem>(count);
+    d_terms = a.take<ImuTerm>(count);
+    d_init = a.take<double>((size_t)count * 16);
+    d_out = a.take<FusedOutput>(count);
+  }));
+  std::vector<NlsProblem> problems(count);
+  std::vector<ImuTerm> terms(count);
+  std::vector<double> init16((size_t)count * 16);
+  for (int c = 0; c < count; ++c) {
+    const Rigidd to_submap = inverse(pose_from7(submap_local_poses + 7 * c));
+    double* x = init16.data() + 16 * c;
+    if (!build_imu_term(to_submap, states_i[c], initial_states_j[c], preints[c], gravity, imu_weight, &terms[c], x))
+      return ctx->fail(DL_ERR_ARG, "pre-integration covariance is not positive definite");
+    NlsProblem& p = problems[c];
+    std::memset(&p, 0, sizeof(p));
+    for (int k = 0; k < num_pairs; ++k) {
+      const int i = c * num_pairs + k;
+      DL_TRY(h2d(ctx, d_clouds[i], clouds[i], 3 * sizes[i]));
+      p.cloud[k] = d_clouds[i];
+      p.count[k] = (int32_t)sizes[i];
+      p.grid[k] = grids[i]->view();
+    }
+    for (int k = 0; k < 7; ++k) p.initial[k] = x[k];
+    for (int k = 0; k < 3; ++k) p.target_t[k] = x[k];  // the translation prior (if weighted) pulls to the IMU prediction
+  }
+  DL_TRY(h2d(ctx, d_problems, problems.data(), count));
+  DL_TRY(h2d(ctx, d_terms, terms.data(), count));
+  DL_TRY(h2d(ctx, d_init, init16.data(), (size_t)count * 16));
+  DL_TRY(launch_nls_fused(ctx, to_nls_options(*options, num_pairs), d_problems, d_terms, d_init, count, d_out));
+  std::vector<FusedOutput> out(count);
+  DL_TRY(d2h(ctx, out.data(), d_out, count));
+  DL_TRY(sync(ctx));
+  for (int c = 0; c < count; ++c) {
+    state_to_local(pose_from7(submap_local_poses + 7 * c), out[c].state, &states_j_out[c]);
+    if (summaries) summaries[c] = out[c].summary;
+  }
+  return DL_OK;
+}
+
+}  // extern "C"

@@ -496,3 +496,113 @@ int launch_local_frame(dl_context* ctx, const LocalFrameJob* jobs, int count, vo
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ grid write side
+using namespace dl;
+
+namespace {
+uint32_t* take_update_list(Arena& a, const dl_range_data_inserter_options& o, int64_t n) {
+  return a.take<uint32_t>((size_t)n * (size_t)(1 + std::max(o.num_free_space_voxels, 0)));
+}
+}  // namespace
+
+namespace dl {
+// The scratch every insert_range_data_device call of `jobs` jobs shares; each job's update list is carved by take_update_list.
+void carve_insert(Arena& a, int jobs, InsertScratch* s) {
+  s->hit_table = a.take<uint16_t>(32768);
+  s->miss_table = a.take<uint16_t>(32768);
+  s->bbox = a.take<int32_t>(8 * (size_t)std::max(jobs, 1));
+  s->args = a.take<char>(insert_args_bytes(std::max(jobs, 1)));
+}
+void carve_submap_insert(Arena& a, const dl_range_data_inserter_options& o, int64_t n, SubmapInsertScratch* s) {
+  s->all = a.take<float>(3 * (size_t)n);
+  s->near = a.take<float>(3 * (size_t)n);
+  s->near_count = a.take<int32_t>(1);
+  s->tiles = a.take<int32_t>((size_t)(n + 255) / 256 + 1);
+  s->update_hi = take_update_list(a, o, n);
+  s->update_lo = take_update_list(a, o, n);
+}
+// Submap3D::InsertRangeData of `returns` (n points, local frame, device) into the submap at `submap_local_pose`: the transform
+// job that moves them into the submap frame and the two Insert jobs that read its output.
+void submap_insert_jobs(dl_grid* hi, dl_grid* lo, const double* submap_local_pose, int32_t high_resolution_max_range,
+                        const float* origin, const float* d_returns, int n, const SubmapInsertScratch& s, TransformJob* transform,
+                        InsertJob* inserts) {
+  // TransformRangeData(range_data, local_pose().inverse().cast<float>())
+  const Rigidf to_submap = to_float(inverse(pose_from7(submap_local_pose)));
+  const Vec3f origin_submap = apply(to_submap, Vec3f{origin[0], origin[1], origin[2]});
+  *transform = TransformJob{d_returns, n, to_submap, origin_submap, (float)high_resolution_max_range, s.all, s.near, s.near_count, s.tiles};
+  inserts[0] = InsertJob{hi, origin_submap, s.near, n, s.near_count, s.update_hi};
+  inserts[1] = InsertJob{lo, origin_submap, s.all, n, nullptr, s.update_lo};
+}
+int upload_odds_tables(dl_context* ctx, const dl_range_data_inserter_options& o, const InsertScratch& s) {
+  static thread_local std::vector<uint16_t> tables(65536);
+  static thread_local double cached_hit = -1, cached_miss = -1;
+  if (cached_hit != o.hit_probability || cached_miss != o.miss_probability) {
+    compute_odds_table((float)o.hit_probability, tables.data());           // Odds(options.hit_probability()) takes a float
+    compute_odds_table((float)o.miss_probability, tables.data() + 32768);
+    cached_hit = o.hit_probability;
+    cached_miss = o.miss_probability;
+  }
+  DL_TRY(h2d(ctx, s.hit_table, tables.data(), 32768));
+  DL_TRY(h2d(ctx, s.miss_table, tables.data() + 32768, 32768));
+  return DL_OK;
+}
+int check_inserter(dl_context* ctx, const dl_range_data_inserter_options* o) {
+  if (!o) return DL_ERR_ARG;
+  if (!(o->hit_probability > 0.5) || !(o->miss_probability < 0.5) || o->num_free_space_voxels < 0)
+    return ctx->fail(DL_ERR_ARG, "hit_probability must be > 0.5 and miss_probability < 0.5 (CHECK_GT / CHECK_LT)");
+  return DL_OK;
+}
+}  // namespace dl
+
+extern "C" {
+
+int dl_grid_insert_range_data(dl_context* ctx, dl_grid* grid, const dl_range_data_inserter_options* options,
+                              const float* origin, const float* returns, int64_t n) {
+  if (!ctx || !grid || !origin || n < 0 || n > 0x3fffffff || (n > 0 && !returns)) return DL_ERR_ARG;  // CHECK_NOTNULL(hybrid_grid)
+  DL_TRY(check_inserter(ctx, options));
+  if (n == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  float* d_returns;
+  uint32_t* update_list;
+  InsertScratch s;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_returns = a.take<float>(3 * n);
+    carve_insert(a, 1, &s);
+    update_list = take_update_list(a, *options, n);
+  }));
+  DL_TRY(h2d(ctx, d_returns, returns, 3 * n));
+  DL_TRY(upload_odds_tables(ctx, *options, s));
+  const InsertJob job{grid, Vec3f{origin[0], origin[1], origin[2]}, d_returns, (int)n, nullptr, update_list};
+  DL_TRY(insert_range_data_device(ctx, &job, 1, options->num_free_space_voxels, s.hit_table, s.miss_table, s.bbox, s.args));
+  return sync(ctx);
+}
+
+int dl_submap_insert_range_data(dl_context* ctx, dl_grid* hi, dl_grid* lo, const dl_range_data_inserter_options* options,
+                                const double* submap_local_pose, int32_t high_resolution_max_range, const float* origin,
+                                const float* returns, int64_t n) {
+  if (!ctx || !hi || !lo || !submap_local_pose || !origin || n < 0 || n > 0x3fffffff || (n > 0 && !returns)) return DL_ERR_ARG;
+  DL_TRY(check_inserter(ctx, options));
+  if (n == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  float* d_in;
+  void* d_transform;
+  SubmapInsertScratch t;
+  InsertScratch s;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_in = a.take<float>(3 * n);
+    d_transform = a.take<char>(transform_jobs_bytes(1));
+    carve_submap_insert(a, *options, n, &t);
+    carve_insert(a, 2, &s);
+  }));
+  DL_TRY(h2d(ctx, d_in, returns, 3 * n));
+  TransformJob transform;
+  InsertJob jobs[2];
+  submap_insert_jobs(hi, lo, submap_local_pose, high_resolution_max_range, origin, d_in, (int)n, t, &transform, jobs);
+  DL_TRY(launch_transform_filter(ctx, &transform, 1, d_transform));
+  DL_TRY(upload_odds_tables(ctx, *options, s));
+  DL_TRY(insert_range_data_device(ctx, jobs, 2, options->num_free_space_voxels, s.hit_table, s.miss_table, s.bbox, s.args));
+  return sync(ctx);
+}
+
+}  // extern "C"

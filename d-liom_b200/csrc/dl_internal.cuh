@@ -162,6 +162,10 @@ struct dl_grid {
     if (st__ != DL_OK) return st__; \
   } while (0)
 
+// Host helpers and types that several units of the library share. Hidden, so that like file-local code they bind inside the
+// library and stay out of its exported symbols.
+#define DL_SHARED __attribute__((visibility("hidden")))
+
 #define DL_LAUNCH_CHECK(ctx, name)                          \
   do {                                                      \
     (ctx)->launches++;                                      \
@@ -269,13 +273,8 @@ int carve_scratch(dl_context* ctx, Carve&& carve, size_t extra = 0, Arena* rest 
 
 // ---- kernel launchers (each defined in its own .cu), all asynchronous on `stream`, device pointers only.
 
-// Voxel filter over `batch` clouds. Cloud b = rows [b * cap, b * cap + counts[b]) of `points` (stride floats per row).
-// keep[b * cap ...] receives the surviving row indices (relative to the cloud) in input order, keep_counts[b] their number.
-// table: batch * table_cap uint32 (table_cap a power of two >= 2 * max count); slot: batch * cap uint32.
-int launch_voxel_filter(dl_context* ctx, const float* points, int stride, int64_t cap, const int32_t* counts, int batch,
-                        float resolution, uint32_t* table, int64_t table_cap, uint32_t* slot, int32_t* keep,
-                        int32_t* keep_counts, int32_t* block_counts);
-int launch_voxel_indices(dl_context* ctx, const float* points, int stride, int64_t n, float resolution, int32_t* out);
+// dl_voxel.cu: the smallest power of two >= v, at least 64 (the capacity of a voxel filter's hash table)
+DL_SHARED int64_t next_pow2(int64_t v);
 
 struct AdaptiveParams {
   float max_length, min_num_points, max_range;
@@ -301,8 +300,49 @@ struct RtcsmScan {  // one scan of a batched correlative search (dl_rtcsm.cu), d
   unsigned long long* best;          // (score bits << 32) | ~index, zeroed before the launch
   int32_t* nonpositive;              // optional, zeroed before the launch: set to 1 when a candidate's score is not > 0
 };
-int rtcsm_ctas_for(int64_t R, int64_t L);
-int launch_rtcsm_batch(dl_context* ctx, const RtcsmScan* scans_dev, const int32_t* cta_prefix_dev, int num_scans, int total_ctas);
+// dl_rtcsm.cu: the host part of the batched correlative search, shared by dl_rtcsm_match and the front end's pre-match
+DL_SHARED Quatf angle_axis_to_quat(const Vec3f& aa);
+struct DL_SHARED RtcsmTables {
+  int linear = 0, angular = 0;
+  float step = 0.f;
+  std::vector<Quatf> cand_q;
+  std::vector<Vec3f> cand_t;
+  std::vector<double> pen_r, pen_t;
+};
+// One batched correlative search. Clouds are on the device: cloud k = points[k] with counts[k] rows (host-known). The tables
+// of every scan (R rotations, L translations, their penalties) are built on the host with the reference's float operations
+// — the angular window depends on each cloud's farthest point through acosf, which must be the host's to stay bit-exact —
+// and go up in ONE copy; one launch scores all (scan, rotation, translation) candidates.
+struct DL_SHARED RtcsmBatchItem {
+  const dl_grid* grid;  // the grid this scan is scored against; every grid of a batch has the plan's resolution
+  const float* d_points;
+  int64_t n;
+  Rigidd initial;
+  float max_scan_range;
+  float* d_scores;          // optional
+  int32_t* d_nonpositive;   // optional: set to 1 when a candidate's score is not > 0
+};
+// plan_rtcsm_batch builds the tables and lays out the one upload (every scan's tables, the descriptors, the CTA prefix); take()
+// carves that upload and the argmax words, so a caller can count the scratch before it reserves it; run_rtcsm_batch uploads
+// and launches.
+struct DL_SHARED RtcsmBatchPlan {
+  std::vector<RtcsmTables> tables;
+  std::vector<size_t> off_q, off_t, off_pr, off_pt;
+  std::vector<int32_t> prefix;
+  size_t off_scans = 0, off_prefix = 0, blob = 0;
+  unsigned char* d_blob = nullptr;
+  RtcsmScan* d_scans = nullptr;
+  unsigned long long* d_best = nullptr;
+  void take(Arena& a) {
+    d_blob = a.take<unsigned char>(blob);
+    d_best = a.take<unsigned long long>(tables.size());
+    d_scans = (RtcsmScan*)(d_blob + off_scans);
+  }
+};
+DL_SHARED int plan_rtcsm_batch(dl_context* ctx, const dl_rtcsm_options& opt, float resolution,
+                               const std::vector<RtcsmBatchItem>& items, RtcsmBatchPlan* plan);
+DL_SHARED int run_rtcsm_batch(dl_context* ctx, const std::vector<RtcsmBatchItem>& items, const RtcsmBatchPlan& plan);
+DL_SHARED size_t rtcsm_scratch_bound(const dl_rtcsm_options& opt, float resolution, float max_range);
 int launch_rtcsm_pick(dl_context* ctx, const RtcsmScan* scans_dev, int num_scans, double* pose_out, const int32_t* pose_slot,
                       float* score_out, const int32_t* score_slot);
 int launch_max_range_batch(dl_context* ctx, const float* points, int64_t stride_floats, const int32_t* counts, int count_stride,
@@ -333,11 +373,14 @@ struct NlsOutput {
   dl_solve_summary summary;
 };
 int launch_nls(dl_context* ctx, const NlsOptions& opt, const NlsProblem* problems_dev, int count, NlsOutput* out_dev);
+// dl_nls.cu: the checks of a dl_ceres_options block for `num_pairs` (cloud, grid) pairs, and the kernels' form of it
+DL_SHARED int check_ceres_options(dl_context* ctx, const dl_ceres_options* o, int num_pairs);
+DL_SHARED NlsOptions to_nls_options(const dl_ceres_options& o, int num_pairs);
 struct FusedOutput {
   double state[16];  // p(3) q(4 wxyz) v(3) ba(3) bg(3)
   dl_solve_summary summary;
 };
-// IMU term of the fused solve in the SUBMAP frame (built by dl_api.cu on the host or by imu_prepare_kernel on the device):
+// IMU term of the fused solve in the SUBMAP frame (built on the host by build_imu_term or on the device by imu_prepare_kernel):
 // state i (fixed), the pre-integrated deltas, gravity, and W = weight^2 * Sigma^-1 (row-major 15x15, order p, theta, v, ba, bg).
 // dp, dq, dv carry the bias correction of imu_term_deltas: the residual reads conj(dq) as the inverse of the corrected delta_q.
 struct ImuTerm {
@@ -382,10 +425,12 @@ DL_HD void imu_term_deltas(const dl_preintegration& m, const double* ba_i, const
   const double n2 = (c.x * c.x + c.y * c.y) + (c.z * c.z + c.w * c.w);
   t->dq[0] = c.w / n2; t->dq[1] = c.x / n2; t->dq[2] = c.y / n2; t->dq[3] = c.z / n2;
 }
+// dl_imu.cu: one pre-integration factor in the submap frame and the initial 16-vector of state j. False if the covariance is
+// not positive definite.
+DL_SHARED bool build_imu_term(const Rigidd& to_submap, const dl_nav_state& si, const dl_nav_state& sj, const dl_preintegration& m,
+                              const double* gravity, double imu_weight, ImuTerm* t, double* x16);
 int launch_nls_fused(dl_context* ctx, const NlsOptions& opt, const NlsProblem* problems_dev, const ImuTerm* imu_terms_dev,
                      const double* initial16_dev, int count, FusedOutput* out_dev);
-int launch_nls_normal_equations(dl_context* ctx, const NlsOptions& opt, const NlsProblem* problems_dev,
-                                const double* at_pose_dev, double* out28_dev);
 // The fused solve's IMU normal equations of each prepared factor at x16_dev (16 doubles per factor, submap frame), into
 // kImuFactorOutDoubles doubles per factor: residual (15), H (225, row-major), g (15), r^T W r. Factors with ok == 0 are skipped.
 constexpr int kImuFactorOutDoubles = 15 + 225 + 15 + 1;
@@ -405,7 +450,6 @@ struct DecodeArgs {  // one sensor_msgs/PointCloud2 message (dl_decode.cu)
   int32_t* num_out;
   double* stamp_offset;
 };
-int launch_decode_point_cloud2(dl_context* ctx, const DecodeArgs& a);
 struct FcsmPair {  // one (node, submap) loop-closure search, device pointers
   GridView hi, lo;
   const float* hi_pts;
@@ -429,12 +473,6 @@ struct FcsmPick {
   double pose[7];  // coarse pose (the guess itself when nothing was found)
 };
 constexpr int kFcsmRun = 8;  // x offsets per search thread (dl_fcsm.cu)
-int launch_fcsm_index(dl_context* ctx, const GridView& g, int ox, int oy, int oz, int nx, int ny, int nz, uint8_t* tmp, uint8_t* out);
-int launch_fcsm_pruned(dl_context* ctx, const FcsmPair* pairs_dev, int count, int max_points, int max_blocks, int* bounds_dev,
-                       int* max_bound_dev, unsigned long long* best_dev, FcsmPick* picks_dev);
-int launch_fcsm(dl_context* ctx, const FcsmPair* pairs_dev, int count, int max_points, long long max_threads,
-                unsigned long long* best_dev, FcsmPick* picks_dev, float* all_scores_dev);
-void compute_odds_table(float probability, uint16_t* table32768);
 // One RangeDataInserter3D::Insert per job (dl_inserter.cu). Device pointers; the grid's frame.
 struct InsertJob {
   dl_grid* grid;
@@ -450,6 +488,14 @@ struct InsertJob {
 size_t insert_args_bytes(int jobs);
 int insert_range_data_device(dl_context* ctx, const InsertJob* jobs, int count, int num_free, const uint16_t* d_hit_table,
                              const uint16_t* d_miss_table, int32_t* d_bbox, void* d_args);
+struct DL_SHARED InsertScratch {
+  uint16_t *hit_table, *miss_table;
+  int32_t* bbox;
+  void* args;
+};
+DL_SHARED void carve_insert(Arena& a, int jobs, InsertScratch* s);
+DL_SHARED int upload_odds_tables(dl_context* ctx, const dl_range_data_inserter_options& o, const InsertScratch& s);
+DL_SHARED int check_inserter(dl_context* ctx, const dl_range_data_inserter_options* o);
 // TransformRangeData into the submap frame + FilterRangeDataByMaxRange (submap_3d.cc:42-51, :264-279) of one cloud per job:
 // `all` receives every point, `near` (count in *near_count) those within max_range of the origin, in input order.
 struct TransformJob {
@@ -464,6 +510,16 @@ struct TransformJob {
 };
 size_t transform_jobs_bytes(int jobs);
 int launch_transform_filter(dl_context* ctx, const TransformJob* jobs, int count, void* d_jobs);
+// The submap-frame transform and range filter of Submap3D::InsertRangeData for one cloud (carve_transform) and its two Inserts.
+struct DL_SHARED SubmapInsertScratch {
+  float *all, *near;
+  int32_t *near_count, *tiles;
+  uint32_t *update_hi, *update_lo;
+};
+DL_SHARED void carve_submap_insert(Arena& a, const dl_range_data_inserter_options& o, int64_t n, SubmapInsertScratch* s);
+DL_SHARED void submap_insert_jobs(dl_grid* hi, dl_grid* lo, const double* submap_local_pose, int32_t high_resolution_max_range,
+                                  const float* origin, const float* d_returns, int n, const SubmapInsertScratch& s,
+                                  TransformJob* transform, InsertJob* inserts);
 // range_data_in_local and the histogram's gravity-aligned returns of one scan per job.
 struct LocalFrameJob {
   const float *returns, *misses;   // tracking frame
@@ -475,14 +531,20 @@ struct LocalFrameJob {
 size_t local_frame_jobs_bytes(int jobs);
 int launch_local_frame(dl_context* ctx, const LocalFrameJob* jobs, int count, void* d_jobs);
 // dl_window.cu
-int launch_window_optimize(dl_context* ctx, int count, const dl_nav_state* states_i, const double* prior_information,
-                           const dl_preintegration* preint, const double* matched_pose, const dl_nav_state* initial_j,
-                           const dl_window_options& opt, dl_nav_state* states_i_out, dl_nav_state* states_j_out,
-                           double* information_out, dl_solve_summary* summaries);
 constexpr int kWindowEvalDoubles = 38 + 38 * 30 + 38 * 38;  // per problem: residual, Jacobian, weight
-int launch_window_evaluate(dl_context* ctx, int count, const dl_nav_state* states_i, const double* prior_information,
-                           const dl_preintegration* preint, const double* matched_pose, const dl_window_options& opt, const double* x,
-                           int32_t* ok, double* out);
+// Device buffers of `count` window updates (carve_window) and the upload / launch / read-back of dl_window_optimize_batch on them,
+// shared with the trajectory builders' batch, which carves them next to its front end's buffers.
+struct DL_SHARED WindowBuffers {
+  dl_nav_state *si, *init, *si_out, *sj_out;
+  double *prior, *z, *info;
+  dl_preintegration* pre;
+  dl_solve_summary* sum;
+};
+DL_SHARED void carve_window(Arena& a, int count, WindowBuffers* w);
+DL_SHARED int window_optimize(dl_context* ctx, const dl_window_options& options, int count, const WindowBuffers& w,
+                              const dl_nav_state* states_i, const double* prior_information, const dl_preintegration* preintegrations,
+                              const double* matched_poses, const dl_nav_state* initial_states_j, dl_nav_state* states_i_out,
+                              dl_nav_state* states_j_out, double* information_out, dl_solve_summary* summaries);
 // dl_histogram.cu
 struct HistogramScratch {  // device scratch of one rotational histogram of n points
   unsigned long long* keys;
@@ -493,8 +555,6 @@ struct HistogramScratch {  // device scratch of one rotational histogram of n po
   int* counters;
 };
 void carve_rotational_histogram(Arena& a, int64_t n, HistogramScratch* s);
-int launch_rotational_histogram(dl_context* ctx, const HistogramScratch& s, const float* d_points, int64_t n, int size,
-                                float* d_histogram, int32_t** d_error_out);
 // `count` clouds in one launch, one CTA each: cloud k = n[k] (>= 1) points at d_points[k], scratch s[k] carved for at least n[k],
 // histogram k (`size` floats) at d_histograms[k]. d_args: rotational_histograms_args_bytes(count) bytes of device memory. The error
 // flag of cloud k is s[k].counters[1].
@@ -506,10 +566,6 @@ int comm_reserve(dl_comm* c, size_t bytes_per_rank);
 void* comm_send_buffer(dl_comm* c);
 void* comm_recv_buffer(dl_comm* c);
 int comm_all_gather(dl_comm* c, const void* send_dev, void* recv_dev, size_t bytes, float* ms);
-// dl_fcsm.cu: one dl_constraint_row per searched pair from the coarse picks and the refinement's output
-int launch_pack_constraint_rows(dl_context* ctx, int n, const FcsmPick* picks, const NlsOutput* refined, const int32_t* submap_ids,
-                                const int32_t* node_ids, double translation_weight, double rotation_weight, int rank,
-                                dl_constraint_row* rows);
 // The clouds of a batch of (node, submap) loop-closure searches. Pair k has hi_off[k+1] - hi_off[k] high-resolution points
 // (likewise low). Host batch (hi_store == nullptr): they are rows [off[k], off[k+1]) of the host arrays hi_pts / lo_pts and the
 // search uploads them. Device-resident (hi_store / lo_store set, dl_posegraph3d.cu's node store): they already sit on the
@@ -524,15 +580,18 @@ struct PairClouds {
   const int64_t* hi_begin = nullptr;
   const int64_t* lo_begin = nullptr;
 };
-// dl_api.cu: the option checks of dl_constraint_search_batch (fast correlative matcher, and the refine's two-weight Ceres
+// dl_fcsm.cu: the option checks of dl_constraint_search_batch (fast correlative matcher, and the refine's two-weight Ceres
 // options), shared by every entry point that searches.
 int check_constraint_options(dl_context* ctx, const dl_constraint_options& options);
-// dl_api.cu: dl_constraint_search_batch's body (coarse search, min_score prune, refine) for `count` pairs in chunks of 1024.
+// dl_fcsm.cu: dl_constraint_search_batch's body (coarse search, min_score prune, refine) for `count` pairs in chunks of 1024.
 int constraint_search(dl_context* ctx, const dl_constraint_options& options, int count, const double* guesses,
                       const PairClouds& clouds, const dl_grid* const* hi_grids, const dl_grid* const* lo_grids,
                       dl_constraint* constraints);
-// dl_api.cu: uploads a grid's host mirror where the device copy is behind; grows its node pool (level 0) or brick pool (level 1)
-// from `used` entries in use by `add` more, keeping those in use
+// dl_api.cu: the flat index of top cell (x, y, z) in a grid's top level of 2^bits cells per axis; downloads a grid's host mirror
+// where the device copy is ahead; uploads it where the device copy is behind; grows its node pool (level 0) or brick pool
+// (level 1) from `used` entries in use by `add` more, keeping those in use
+DL_SHARED inline size_t top_flat(int x, int y, int z, int bits) { return ((((size_t)z << bits) + y) << bits) + x; }
+DL_SHARED int grid_download(dl_grid* g);
 int grid_ensure_device_state(dl_grid* g);
 int grid_grow_pool(dl_grid* g, int level, size_t used, size_t add);
 int launch_interpolate(dl_context* ctx, const GridView& grid, int64_t n, const double* xyz, double* out);

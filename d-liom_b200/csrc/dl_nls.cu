@@ -21,7 +21,9 @@
 // mix exactly, so the piecewise-polynomial pieces are the same ones the CPU path picks.
 //
 // Algorithmic bytes: 12 B point + 8 corners * 2 B = 28 B per point per evaluation (SURVEY 8d).
+#include <cstring>
 #include <type_traits>
+#include <vector>
 
 #include <cooperative_groups.h>
 
@@ -963,3 +965,132 @@ int launch_grid_lookup(dl_context* ctx, const GridView& grid, int64_t n, const i
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ Ceres-equivalent matcher
+namespace dl {
+int check_ceres_options(dl_context* ctx, const dl_ceres_options* o, int num_pairs) {
+  if (!o) return DL_ERR_ARG;
+  if (num_pairs < 1 || num_pairs > DL_MAX_PAIRS) return ctx->fail(DL_ERR_ARG, "num_pairs out of range");
+  if (o->num_occupied_space_weights != num_pairs)
+    return ctx->fail(DL_ERR_ARG, "occupied_space_weight count != number of (cloud, grid) pairs (CHECK_EQ)");
+  for (int i = 0; i < num_pairs; ++i)
+    if (!(o->occupied_space_weight[i] > 0.)) return ctx->fail(DL_ERR_ARG, "occupied_space_weight must be > 0 (CHECK_GT)");
+  if (o->max_num_iterations <= 0) return ctx->fail(DL_ERR_ARG, "max_num_iterations must be > 0 (CHECK_GT)");
+  return DL_OK;
+}
+NlsOptions to_nls_options(const dl_ceres_options& o, int num_pairs) {
+  NlsOptions n{};
+  n.num_pairs = num_pairs;
+  for (int i = 0; i < num_pairs; ++i) n.occ_weight[i] = o.occupied_space_weight[i];
+  n.trans_weight = o.translation_weight;
+  n.rot_weight = o.rotation_weight;
+  n.only_yaw = o.only_optimize_yaw;
+  n.nonmono = o.use_nonmonotonic_steps;
+  n.max_iter = o.max_num_iterations;
+  return n;
+}
+}  // namespace dl
+
+using namespace dl;
+
+extern "C" {
+
+int dl_ceres_match_batch(dl_context* ctx, const dl_ceres_options* options, int32_t count, int32_t num_pairs,
+                         const double* target_translations, const double* initial_poses, const float* const* clouds,
+                         const int64_t* sizes, const dl_grid* const* grids, double* poses_out,
+                         dl_solve_summary* summaries) {
+  if (!ctx) return DL_ERR_ARG;
+  DL_TRY(check_ceres_options(ctx, options, num_pairs));
+  if (count < 0 || (count > 0 && (!target_translations || !initial_poses || !clouds || !sizes || !grids || !poses_out)))
+    return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < count * num_pairs; ++i) {
+    if (sizes[i] < 0 || !grids[i] || (sizes[i] > 0 && !clouds[i])) return DL_ERR_ARG;
+    if (sizes[i] == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
+    if (grids[i]->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+  }
+  std::vector<float*> d_clouds(count * num_pairs);
+  NlsProblem* d_problems;
+  NlsOutput* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    for (int i = 0; i < count * num_pairs; ++i) d_clouds[i] = a.take<float>(3 * sizes[i]);
+    d_problems = a.take<NlsProblem>(count);
+    d_out = a.take<NlsOutput>(count);
+  }));
+  std::vector<NlsProblem> problems(count);
+  for (int c = 0; c < count; ++c) {
+    NlsProblem& p = problems[c];
+    std::memset(&p, 0, sizeof(p));
+    for (int k = 0; k < num_pairs; ++k) {
+      const int i = c * num_pairs + k;
+      DL_TRY(h2d(ctx, d_clouds[i], clouds[i], 3 * sizes[i]));
+      p.cloud[k] = d_clouds[i];
+      p.count[k] = (int32_t)sizes[i];
+      p.grid[k] = grids[i]->view();
+    }
+    for (int j = 0; j < 3; ++j) p.target_t[j] = target_translations[3 * c + j];
+    for (int j = 0; j < 7; ++j) p.initial[j] = initial_poses[7 * c + j];
+  }
+  DL_TRY(h2d(ctx, d_problems, problems.data(), count));
+  DL_TRY(launch_nls(ctx, to_nls_options(*options, num_pairs), d_problems, count, d_out));
+  std::vector<NlsOutput> out(count);
+  DL_TRY(d2h(ctx, out.data(), d_out, count));
+  DL_TRY(sync(ctx));
+  for (int c = 0; c < count; ++c) {
+    std::memcpy(poses_out + 7 * c, out[c].pose, 7 * sizeof(double));
+    if (summaries) summaries[c] = out[c].summary;
+  }
+  return DL_OK;
+}
+
+int dl_ceres_match(dl_context* ctx, const dl_ceres_options* options, const double* target_translation,
+                   const double* initial_pose, int32_t num_pairs, const float* const* clouds, const int64_t* sizes,
+                   const dl_grid* const* grids, double* pose_out, dl_solve_summary* summary) {
+  return dl_ceres_match_batch(ctx, options, 1, num_pairs, target_translation, initial_pose, clouds, sizes, grids,
+                              pose_out, summary);
+}
+
+int dl_ceres_normal_equations(dl_context* ctx, const dl_ceres_options* options, const double* target_translation,
+                              const double* reference_pose, const double* at_pose, int32_t num_pairs,
+                              const float* const* clouds, const int64_t* sizes, const dl_grid* const* grids,
+                              double* cost, double* gradient6, double* hessian36) {
+  if (!ctx) return DL_ERR_ARG;
+  DL_TRY(check_ceres_options(ctx, options, num_pairs));
+  if (!target_translation || !reference_pose || !at_pose || !clouds || !sizes || !grids || !cost || !gradient6 || !hessian36)
+    return DL_ERR_ARG;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  float* d_clouds[DL_MAX_PAIRS];
+  NlsProblem* d_p;
+  double *d_at, *d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    for (int k = 0; k < num_pairs; ++k) d_clouds[k] = a.take<float>(3 * sizes[k]);
+    d_p = a.take<NlsProblem>(1);
+    d_at = a.take<double>(7);
+    d_out = a.take<double>(28);
+  }));
+  NlsProblem p;
+  std::memset(&p, 0, sizeof(p));
+  for (int k = 0; k < num_pairs; ++k) {
+    DL_TRY(h2d(ctx, d_clouds[k], clouds[k], 3 * sizes[k]));
+    p.cloud[k] = d_clouds[k];
+    p.count[k] = (int32_t)sizes[k];
+    p.grid[k] = grids[k]->view();
+  }
+  for (int j = 0; j < 3; ++j) p.target_t[j] = target_translation[j];
+  for (int j = 0; j < 7; ++j) p.initial[j] = reference_pose[j];
+  DL_TRY(h2d(ctx, d_p, &p, 1));
+  DL_TRY(h2d(ctx, d_at, at_pose, 7));
+  DL_TRY(launch_nls_normal_equations(ctx, to_nls_options(*options, num_pairs), d_p, d_at, d_out));
+  double out[28];
+  DL_TRY(d2h(ctx, out, d_out, 28));
+  DL_TRY(sync(ctx));
+  *cost = out[0];
+  for (int i = 0; i < 6; ++i) gradient6[i] = out[1 + i];
+  int t = 7;
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) hessian36[r * 6 + c] = hessian36[c * 6 + r] = out[t++];
+  return DL_OK;
+}
+
+}  // extern "C"

@@ -1,5 +1,7 @@
 // Argument blocks of the batched front-end kernels (dl_frontend.cu, dl_imu.cu) and their launchers.
 #pragma once
+#include <functional>
+
 #include "dl_internal.cuh"
 
 namespace dl {
@@ -132,5 +134,103 @@ int launch_gather_rows(dl_context* ctx, const float* in, int64_t cap_in, int pai
 int launch_initial_pose(dl_context* ctx, int batch, const float* current_pose, const Rigidd* submap_inverse,
                         double* initial_pose, double* target_translation);
 int launch_finalize_results(dl_context* ctx, const ResultArgs& a);
+
+// ---- the batched front end's host side (dl_frontend.cu), shared with the trajectory builders' batch (dl_ltb.cu)
+// The submaps a front-end batch matches against: one for every scan (the public front-end entry points) or one per scan
+// (dl_ltb_add_range_data_batch, whose scans come from different trajectories).
+struct DL_SHARED SubmapSet {
+  const double* poses = nullptr;             // 7 doubles: the local pose, once or per scan
+  const dl_grid* const* hi = nullptr;        // one grid, or one per scan
+  const dl_grid* const* lo = nullptr;
+  bool per_scan = false;
+  const double* pose(int b) const { return poses + (per_scan ? 7 * b : 0); }
+  const dl_grid* high(int b) const { return hi[per_scan ? b : 0]; }
+  const dl_grid* low(int b) const { return lo[per_scan ? b : 0]; }
+};
+// The single-submap form; the grid pointers must outlive the call.
+struct DL_SHARED OneSubmap : SubmapSet {
+  const dl_grid* h;
+  const dl_grid* l;
+  OneSubmap(const double* pose7, const dl_grid* hi_grid, const dl_grid* lo_grid) : h(hi_grid), l(lo_grid) {
+    poses = pose7;
+    hi = &h;
+    lo = &l;
+  }
+  OneSubmap(const OneSubmap&) = delete;
+};
+
+struct DL_SHARED FrontendBuffers {
+  int batch = 0;
+  int64_t cap = 0, tcap = 0;
+  int32_t *counts0, *n1, *n_ret, *n2, *n3, *countsA, *npassesA, *croppedA;
+  uint32_t *tableA, *scratchA;
+  int32_t* keepA;
+  float *returns_tracking, *misses_tracking, *clouds, *current_pose, *origins, *passesA, *rtcsm_scores;
+  int32_t* rtcsm_nonpositive = nullptr;  // pre-match only (carve_prematch): per scan, a candidate scored <= 0 (CHECK_GT)
+  // fused front half
+  int64_t bit_words = 0;
+  uint32_t* bits;              // two survivor bitmaps per scan
+  uint32_t* first_bits;        // the first filter's survivor bitmap per scan
+  int4* stage;                 // tile winners by hash partition, and their ends per tile (dl_frontend.cu)
+  int32_t *part_ends, *spill_used;
+  uint32_t* spill;
+  int32_t *last_index, *error_flag;
+  float* local4;
+  ScanConstants* scans;
+  AdaptiveParams* filters;
+  Rigidd *submap, *submap_inverse;  // per scan: its matching submap's local pose and the inverse (host arithmetic)
+  int32_t* origin_base;             // per scan: its first origin in `origins`
+  double *initial_pose, *target;
+  NlsProblem* problems;
+  NlsOutput* nls_out;
+  // 12-byte rows only (carve_time_runs)
+  int32_t *run_offsets = nullptr, *run_first_row = nullptr;
+  float *run_value = nullptr, *run_pose = nullptr;
+};
+
+// IMU coupling of one front-end run: either finished pre-integrations (`host`, factors built on the host) or raw samples
+// (`samples`, everything on the device), and its device buffers (carve_imu).
+struct DL_SHARED ImuRun {
+  const dl_frontend_imu* host = nullptr;
+  const dl_frontend_imu_samples* samples = nullptr;
+  dl_nav_state* d_states_out = nullptr;  // in: optional caller-provided device buffer for the estimated states
+  ImuTerm* d_terms = nullptr;
+  double* d_init16 = nullptr;
+  FusedOutput* d_fused = nullptr;
+  dl_nav_state* d_states = nullptr;      // estimated states, local frame
+  // raw samples only
+  int32_t* d_off = nullptr;
+  double *d_dt = nullptr, *d_acc = nullptr, *d_gyr = nullptr;
+  dl_nav_state* d_si = nullptr;
+  dl_preintegration* d_pre = nullptr;
+  dl_nav_state* d_predicted = nullptr;   // predicted states, local frame
+  int32_t* d_ok = nullptr;               // per scan: its IMU factor could be formed
+};
+
+// Where the scans of a batch are: host rows, one pointer per scan, which the batch uploads into its scratch; or device rows
+// (scan b at row b * cap_rows) with a caller-provided device buffer for the results (and, with raw IMU samples, one for the
+// estimated states in ImuRun::d_states_out).
+struct DL_SHARED FrontendScans {
+  const void* const* host = nullptr;
+  bool on_device = false;
+  const void* dev = nullptr;
+  int64_t cap_rows = 0;
+  dl_scan_result* results_dev = nullptr;
+};
+
+// Validates, reserves, carves and enqueues one front-end batch: the one place that sizes a batch's scratch. On return
+// *d_results_out holds the device results (not yet synchronised).
+// `more` (optional) carves the caller's own buffers into the same reservation, after the batch's: they stay valid as long as the
+// batch's (the trajectory builders' batch keeps the tracking-frame clouds on the device until insertion has read them).
+// origin_base (optional): per scan, where its origins start in `origins`.
+DL_SHARED int frontend_enqueue(dl_context* ctx, const dl_frontend_options* options, int num_scans, const FrontendScans& in,
+                               const int64_t* sizes, const float* origins, int num_origins, const double* prev_poses,
+                               const double* predicted_poses, const SubmapSet& submaps, dl_scan_result** d_results_out,
+                               ImuRun* imu = nullptr, FrontendBuffers* buffers_out = nullptr, const int32_t* origin_base = nullptr,
+                               const std::function<void(Arena&)>* more = nullptr);
+// The fused solve refuses only_optimize_yaw; the raw IMU samples of `num_scans` scans.
+DL_SHARED int check_imu_options(dl_context* ctx, const dl_frontend_options* options);
+DL_SHARED int check_imu_samples(dl_context* ctx, const dl_frontend_options* options, const dl_frontend_imu_samples* imu,
+                                int num_scans);
 
 }  // namespace dl

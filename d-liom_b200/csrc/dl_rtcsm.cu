@@ -24,6 +24,10 @@
 // Algorithmic traffic (SURVEY 8d): per rotation the cloud is read once and every (point, translation) reads one 2-byte
 // voxel: R * (12 N + 2 N L) bytes per scan. The voxel reads are L1/L2 hits (a translation window touches <= 8 bricks).
 #include <cstdint>
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <vector>
 
 #include "dl_internal.cuh"
 
@@ -232,3 +236,191 @@ int launch_max_range_batch(dl_context* ctx, const float* points, int64_t stride_
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ RT-CSM (host part)
+using namespace dl;
+
+namespace {
+
+float rotation_angle(const Quatf& q) {  // transform.h:33-37
+  return 2.f * std::atan2(norm3(Vec3f{q.x, q.y, q.z}), std::fabs(q.w));
+}
+
+// GenerateExhaustiveSearchTransforms (SM/real_time_correlative_scan_matcher_3d.cc:55-95), factored into the
+// R rotations and L translations it is the outer product of, each composed with the initial pose.
+void build_rtcsm_tables(const dl_rtcsm_options& opt, float resolution, float max_scan_range, const Rigidf& initial,
+                        RtcsmTables* t) {
+  t->linear = (int)std::lround(opt.linear_search_window / resolution);  // double / float -> double
+  const float kSafetyMargin = 1.f - 1e-3f;
+  t->step = kSafetyMargin * std::acos(1.f - (resolution * resolution) / (2.f * (max_scan_range * max_scan_range)));
+  t->angular = (int)std::lround(opt.angular_search_window / t->step);
+  const int L = t->linear, A = t->angular;
+  for (int rz = -A; rz <= A; ++rz)
+    for (int ry = -A; ry <= A; ++ry)
+      for (int rx = -A; rx <= A; ++rx) {
+        const Quatf q = angle_axis_to_quat(Vec3f{rx * t->step, ry * t->step, rz * t->step});
+        t->cand_q.push_back(qnormalized(qmul(initial.q, q)));
+        t->pen_r.push_back(rotation_angle(q) * opt.rotation_delta_cost_weight);
+      }
+  for (int z = -L; z <= L; ++z)
+    for (int y = -L; y <= L; ++y)
+      for (int x = -L; x <= L; ++x) {
+        const Vec3f off{x * resolution, y * resolution, z * resolution};
+        t->cand_t.push_back(add(rotate(initial.q, off), initial.t));
+        t->pen_t.push_back(norm3(off) * opt.translation_delta_cost_weight);
+      }
+}
+
+// The farthest point of a host cloud, floored at 3 * resolution (cc:63-71), with the norm the device reduction uses.
+float max_scan_range_host(const float* points, int64_t n, float resolution) {
+  float m = 3.f * resolution;
+  for (int64_t i = 0; i < n; ++i) m = std::max(m, norm3(Vec3f{points[3 * i], points[3 * i + 1], points[3 * i + 2]}));
+  return m;
+}
+
+}  // namespace
+
+namespace dl {
+
+// AngleAxisVectorToRotationQuaternion<float> (C/transform/transform.h:85-99): the cutoff compare and sin/cos run
+// in double, results narrow to float.
+Quatf angle_axis_to_quat(const Vec3f& aa) {
+  float s = 0.5f, w = 1.f;
+  if ((double)dot3(aa, aa) > 1e-8) {
+    const float n = norm3(aa);
+    s = (float)(std::sin((double)n / 2.) / (double)n);
+    w = (float)std::cos((double)n / 2.);
+  }
+  return {w, s * aa.x, s * aa.y, s * aa.z};
+}
+int plan_rtcsm_batch(dl_context* ctx, const dl_rtcsm_options& opt, float resolution, const std::vector<RtcsmBatchItem>& items,
+                     RtcsmBatchPlan* plan) {
+  const int B = (int)items.size();
+  plan->tables.assign(B, RtcsmTables{});
+  plan->off_q.resize(B); plan->off_t.resize(B); plan->off_pr.resize(B); plan->off_pt.resize(B);
+  plan->prefix.assign(B + 1, 0);
+  auto align16 = [](size_t v) { return (v + 15) & ~size_t(15); };
+  size_t blob = 0;
+  for (int k = 0; k < B; ++k) {
+    build_rtcsm_tables(opt, resolution, items[k].max_scan_range, to_float(items[k].initial), &plan->tables[k]);
+    const RtcsmTables& t = plan->tables[k];
+    const int64_t R = (int64_t)t.cand_q.size(), L = (int64_t)t.cand_t.size();
+    if (R * L >= 0xFFFFFFFFll) return ctx->fail(DL_ERR_ARG, "more than 2^32-1 correlative candidates");
+    plan->off_q[k] = blob; blob = align16(blob + R * sizeof(Quatf));
+    plan->off_t[k] = blob; blob = align16(blob + L * sizeof(Vec3f));
+    plan->off_pr[k] = blob; blob = align16(blob + R * sizeof(double));
+    plan->off_pt[k] = blob; blob = align16(blob + L * sizeof(double));
+    plan->prefix[k + 1] = plan->prefix[k] + rtcsm_ctas_for(R, L);
+  }
+  plan->off_scans = blob; blob = align16(blob + (size_t)B * sizeof(RtcsmScan));
+  plan->off_prefix = blob; blob = align16(blob + (size_t)(B + 1) * sizeof(int32_t));
+  plan->blob = blob;
+  return DL_OK;
+}
+// `plan` has taken its scratch; items[k].d_points / d_scores / d_nonpositive are read here.
+int run_rtcsm_batch(dl_context* ctx, const std::vector<RtcsmBatchItem>& items, const RtcsmBatchPlan& plan) {
+  const int B = (int)items.size();
+  if (B == 0) return DL_OK;
+  std::vector<unsigned char> host(plan.blob);
+  for (int k = 0; k < B; ++k) {
+    const RtcsmTables& t = plan.tables[k];
+    std::memcpy(host.data() + plan.off_q[k], t.cand_q.data(), t.cand_q.size() * sizeof(Quatf));
+    std::memcpy(host.data() + plan.off_t[k], t.cand_t.data(), t.cand_t.size() * sizeof(Vec3f));
+    std::memcpy(host.data() + plan.off_pr[k], t.pen_r.data(), t.pen_r.size() * sizeof(double));
+    std::memcpy(host.data() + plan.off_pt[k], t.pen_t.data(), t.pen_t.size() * sizeof(double));
+    RtcsmScan sc{};
+    sc.grid = items[k].grid->view();
+    sc.points = items[k].d_points;
+    sc.n = (int32_t)items[k].n;
+    sc.cand_q = (const Quatf*)(plan.d_blob + plan.off_q[k]);
+    sc.cand_t = (const Vec3f*)(plan.d_blob + plan.off_t[k]);
+    sc.pen_r = (const double*)(plan.d_blob + plan.off_pr[k]);
+    sc.pen_t = (const double*)(plan.d_blob + plan.off_pt[k]);
+    sc.R = (int32_t)t.cand_q.size();
+    sc.L = (int32_t)t.cand_t.size();
+    sc.scores = items[k].d_scores;
+    sc.best = plan.d_best + k;
+    sc.nonpositive = items[k].d_nonpositive;
+    std::memcpy(host.data() + plan.off_scans + (size_t)k * sizeof(RtcsmScan), &sc, sizeof(sc));
+  }
+  std::memcpy(host.data() + plan.off_prefix, plan.prefix.data(), (size_t)(B + 1) * sizeof(int32_t));
+  DL_TRY(h2d(ctx, plan.d_blob, host.data(), plan.blob));
+  DL_CUDA(ctx, cudaMemsetAsync(plan.d_best, 0, sizeof(unsigned long long) * B, ctx->stream));
+  DL_TRY(sync(ctx));  // `host` is pageable and local
+  return launch_rtcsm_batch(ctx, plan.d_scans, (const int32_t*)(plan.d_blob + plan.off_prefix), B, plan.prefix[B]);
+}
+
+// Upper bound of the scratch one scan of the front end's correlative pre-match takes (tables, descriptor, prefix, argmax word).
+// The tables' size follows from the cloud's farthest point, which a device reduction finds after the front end has carved its
+// scratch, so it is bounded from the options. Every point the pre-match sees has passed the high-resolution filter's
+// norm3(p) <= max_range, so max_scan_range <= max(3 * resolution, max_range). The float step does not grow with the range, so
+// A is largest at that range, until the argument of acosf rounds to 1 (about 4096 resolutions): there the step is 0 and A is 0,
+// and below it the step is never smaller than 0.999f * acosf(1 - 2^-24). So A is bounded by its value at max_range, or by the
+// smallest positive step when max_range is past that cliff.
+size_t rtcsm_scratch_bound(const dl_rtcsm_options& opt, float resolution, float max_range) {
+  const int L1 = 2 * (int)std::lround(opt.linear_search_window / resolution) + 1;
+  const float r = max_range > 3.f * resolution ? max_range : 3.f * resolution;
+  const float kSafetyMargin = 1.f - 1e-3f;
+  float step = kSafetyMargin * std::acos(1.f - (resolution * resolution) / (2.f * (r * r)));
+  if (!(step > 0.f)) step = kSafetyMargin * std::acos(std::nextafter(1.f, 0.f));
+  const int A1 = 2 * (int)std::lround(opt.angular_search_window / step) + 1;
+  const size_t R = (size_t)A1 * A1 * A1, L = (size_t)L1 * L1 * L1;
+  Arena bound(nullptr);  // the plan's takes at the largest tables, with room for the blob's 16-byte alignment
+  bound.take<unsigned char>(R * 16 + L * 12 + R * 8 + L * 8 + 256 + sizeof(RtcsmScan) + 64);
+  bound.take<unsigned long long>(1);
+  return bound.off + 4096;
+}
+
+}  // namespace dl
+
+extern "C" {
+
+int dl_rtcsm_match(dl_context* ctx, const dl_rtcsm_options* options, const double* initial_pose, const float* points,
+                   int64_t n, const dl_grid* grid, double* pose_out, float* score_out, dl_rtcsm_info* info,
+                   float* all_scores) {
+  if (!ctx || !options || !initial_pose || !grid || !pose_out || n < 0 || (n > 0 && !points)) return DL_ERR_ARG;  // CHECK_NOTNULL(pose_estimate)
+  if (n == 0) return ctx->fail(DL_ERR_EMPTY, "empty point cloud");
+  if (grid->structure_dirty) return ctx->fail(DL_ERR_ARG, "dl_grid_sync not called after dl_grid_set_cells");
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  // The cloud is on the host: its farthest point, hence the tables and the exact scratch, are known before the carve.
+  const float max_scan_range = max_scan_range_host(points, n, grid->resolution);
+  std::vector<RtcsmBatchItem> items{RtcsmBatchItem{grid, nullptr, n, pose_from7(initial_pose), max_scan_range, nullptr, nullptr}};
+  RtcsmBatchPlan plan;
+  DL_TRY(plan_rtcsm_batch(ctx, *options, grid->resolution, items, &plan));
+  const RtcsmTables& t = plan.tables[0];
+  const int64_t R = (int64_t)t.cand_q.size(), K = R * (int64_t)t.cand_t.size();
+  float* d_pts;
+  float* d_scores = nullptr;
+  DL_TRY(carve_scratch(ctx, [&](Arena& c) {
+    d_pts = c.take<float>(3 * n);
+    if (all_scores) d_scores = c.take<float>(K);
+    plan.take(c);
+  }));
+  DL_TRY(h2d(ctx, d_pts, points, 3 * n));
+  items[0].d_points = d_pts;
+  items[0].d_scores = d_scores;
+  DL_TRY(run_rtcsm_batch(ctx, items, plan));
+  unsigned long long best = 0;
+  DL_TRY(d2h(ctx, &best, plan.d_best, 1));
+  if (all_scores) DL_TRY(d2h(ctx, all_scores, d_scores, K));
+  DL_TRY(sync(ctx));
+  if (best == 0) return ctx->fail(DL_ERR_SCORE, "no candidate with a positive score (CHECK_GT(score, 0))");
+  const uint32_t score_bits = (uint32_t)(best >> 32);
+  const int64_t index = (int64_t)(0xFFFFFFFFull - (best & 0xFFFFFFFFull));
+  float score;
+  std::memcpy(&score, &score_bits, 4);
+  const int64_t l = index / R, r = index - l * R;
+  pose_to7(to_double(Rigidf{t.cand_t[l], t.cand_q[r]}), pose_out);
+  if (score_out) *score_out = score;
+  if (info) {
+    info->best_index = index;
+    info->num_candidates = K;
+    info->linear_window = t.linear;
+    info->angular_window = t.angular;
+    info->angular_step = t.step;
+    info->max_scan_range = max_scan_range;
+  }
+  return DL_OK;
+}
+
+}  // extern "C"

@@ -13,6 +13,8 @@
 // point) lives in L2. Compile with -fmad=false: index = lroundf(x / resolution) must match the CPU bit for bit.
 #include <algorithm>
 #include <cstdlib>
+#include <cstring>
+#include <vector>
 
 #include "dl_internal.cuh"
 
@@ -677,6 +679,9 @@ __global__ void __launch_bounds__(kSearchBlock, 2) adaptive_voxel_kernel(
 
 }  // namespace
 
+// Voxel filter over `batch` clouds. Cloud b = rows [b * cap, b * cap + counts[b]) of `points` (stride floats per row).
+// keep[b * cap ...] receives the surviving row indices (relative to the cloud) in input order, keep_counts[b] their number.
+// table: batch * table_cap uint32 (table_cap a power of two >= 2 * max count); slot: batch * cap uint32.
 int launch_voxel_filter(dl_context* ctx, const float* points, int stride, int64_t cap, const int32_t* counts, int batch,
                         float resolution, uint32_t* table, int64_t table_cap, uint32_t* slot, int32_t* keep,
                         int32_t* keep_counts, int32_t* block_counts) {
@@ -714,3 +719,115 @@ int launch_adaptive_voxel_filter(dl_context* ctx, const float* points, int strid
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ voxel filters
+namespace dl {
+int64_t next_pow2(int64_t v) {
+  int64_t p = 64;
+  while (p < v) p <<= 1;
+  return p;
+}
+}  // namespace dl
+
+using namespace dl;
+
+extern "C" {
+
+int dl_voxel_indices(dl_context* ctx, const float* points, int64_t n, int stride, float resolution, int32_t* out) {
+  if (!ctx || n < 0 || stride < 3 || !(resolution > 0.f) || (n > 0 && (!points || !out))) return DL_ERR_ARG;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  float* d_pts;
+  int32_t* d_out;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(n * stride);
+    d_out = a.take<int32_t>(3 * n);
+  }));
+  DL_TRY(h2d(ctx, d_pts, points, n * stride));
+  DL_TRY(launch_voxel_indices(ctx, d_pts, stride, n, resolution, d_out));
+  DL_TRY(d2h(ctx, out, d_out, 3 * n));
+  return sync(ctx);
+}
+
+int dl_voxel_filter(dl_context* ctx, const float* points, int64_t n, int stride, float resolution, int64_t* keep_out,
+                    int64_t* n_keep) {
+  if (!ctx || n < 0 || stride < 3 || !(resolution > 0.f) || !n_keep || (n > 0 && (!points || !keep_out)))
+    return DL_ERR_ARG;
+  *n_keep = 0;
+  if (n == 0) return DL_OK;
+  if (n > 0x7fffffff) return ctx->fail(DL_ERR_ARG, "more than 2^31-1 points");
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int64_t tcap = next_pow2(2 * n);
+  const int tiles = (int)((n + 255) / 256);
+  float* d_pts;
+  uint32_t *d_table, *d_slot;
+  int32_t *d_keep, *d_blocks, *d_counts;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(n * stride);
+    d_table = a.take<uint32_t>(tcap);
+    d_slot = a.take<uint32_t>(n);
+    d_keep = a.take<int32_t>(n);
+    d_blocks = a.take<int32_t>(tiles);
+    d_counts = a.take<int32_t>(2);  // [0] = n, [1] = survivors
+  }));
+  const int32_t n32 = (int32_t)n;
+  DL_TRY(h2d(ctx, d_pts, points, n * stride));
+  DL_TRY(h2d(ctx, d_counts, &n32, 1));
+  DL_TRY(launch_voxel_filter(ctx, d_pts, stride, n, d_counts, 1, resolution, d_table, tcap, d_slot, d_keep, d_counts + 1,
+                             d_blocks));
+  int32_t kept = 0;
+  DL_TRY(d2h(ctx, &kept, d_counts + 1, 1));
+  DL_TRY(sync(ctx));
+  std::vector<int32_t> keep32(kept);
+  DL_TRY(d2h(ctx, keep32.data(), d_keep, kept));
+  DL_TRY(sync(ctx));
+  for (int32_t i = 0; i < kept; ++i) keep_out[i] = keep32[i];
+  *n_keep = kept;
+  return DL_OK;
+}
+
+int dl_adaptive_voxel_filter(dl_context* ctx, const dl_adaptive_voxel_filter_options* options, const float* points,
+                             int64_t n, int stride, int64_t* keep_out, int64_t* n_keep, float* passes_out,
+                             int* n_passes) {
+  if (!ctx || !options || n < 0 || stride < 3 || !n_keep || (n > 0 && (!points || !keep_out))) return DL_ERR_ARG;
+  *n_keep = 0;
+  if (n_passes) *n_passes = 0;
+  if (n == 0) return DL_OK;
+  if (n > 0x7fffffff) return ctx->fail(DL_ERR_ARG, "more than 2^31-1 points");
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int64_t tcap = next_pow2(2 * n);
+  float *d_pts, *d_passes;
+  uint32_t *d_table, *d_scratch;
+  int32_t *d_keep, *d_counts;
+  AdaptiveParams* d_params;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_pts = a.take<float>(n * stride);
+    d_table = a.take<uint32_t>(tcap);
+    d_scratch = a.take<uint32_t>(2 * n);
+    d_keep = a.take<int32_t>(n);
+    d_counts = a.take<int32_t>(3);  // n, survivors, passes
+    d_params = a.take<AdaptiveParams>(1);
+    d_passes = a.take<float>(32);
+  }));
+  const int32_t n32 = (int32_t)n;
+  const AdaptiveParams params{options->max_length, options->min_num_points, options->max_range};
+  DL_TRY(h2d(ctx, d_pts, points, n * stride));
+  DL_TRY(h2d(ctx, d_counts, &n32, 1));
+  DL_TRY(h2d(ctx, d_params, &params, 1));
+  DL_TRY(launch_adaptive_voxel_filter(ctx, d_pts, stride, n, d_counts, 1, d_params, 1, d_table, tcap, d_scratch, d_keep,
+                                      d_counts + 1, d_passes, d_counts + 2, nullptr));
+  int32_t res[2] = {0, 0};
+  float passes[32];
+  DL_TRY(d2h(ctx, res, d_counts + 1, 2));
+  DL_TRY(d2h(ctx, passes, d_passes, 32));
+  DL_TRY(sync(ctx));
+  std::vector<int32_t> keep32(res[0]);
+  DL_TRY(d2h(ctx, keep32.data(), d_keep, res[0]));
+  DL_TRY(sync(ctx));
+  for (int32_t i = 0; i < res[0]; ++i) keep_out[i] = keep32[i];
+  *n_keep = res[0];
+  if (n_passes) *n_passes = res[1];
+  if (passes_out) std::memcpy(passes_out, passes, sizeof(float) * std::min(res[1], 32));
+  return DL_OK;
+}
+
+}  // extern "C"

@@ -25,6 +25,10 @@
 //              R_j and the residual has no offset.
 // dl_window_evaluate runs window_weights and window_residuals alone at given (x_i, x_j), so the factors can be checked on their own.
 // One warp per trajectory: lane 0 forms the residuals and their duals, the 32 lanes share the 30 x 30 linear algebra.
+#include <cmath>
+#include <cstring>
+#include <vector>
+
 #include "dl_internal.cuh"
 
 namespace dl {
@@ -474,3 +478,133 @@ int launch_window_optimize(dl_context* ctx, int count, const dl_nav_state* state
 }
 
 }  // namespace dl
+
+// ------------------------------------------------------------------------------------------------ two-stage window
+using namespace dl;
+
+namespace {
+// The options of dl_window_optimize_batch and dl_window_evaluate as the kernels take them: sigmas and the IMU weight positive and,
+// with the gravity factor on, both directions finite and non-zero. Only their orientation enters the factor (Unit3 normalises
+// too), so both are normalised here, the one place that does it.
+int window_options_checked(dl_context* ctx, const dl_window_options& in, dl_window_options* out) {
+  if (!(in.pose_sigma_translation > 0.) || !(in.pose_sigma_rotation > 0.) || !(in.imu_weight > 0.) ||
+      (in.use_gravity_factor && !(in.gravity_sigma > 0.)))
+    return ctx->fail(DL_ERR_ARG, "dl_window_options: sigmas and the IMU weight must be positive");
+  *out = in;
+  if (!in.use_gravity_factor) return DL_OK;
+  for (double* d : {out->gravity_direction, out->body_reference_direction}) {
+    const double n = std::sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    if (!std::isfinite(n) || !(n > 0.))
+      return ctx->fail(DL_ERR_ARG, "dl_window_options: the gravity and body reference directions must be finite and non-zero");
+    for (int k = 0; k < 3; ++k) d[k] /= n;
+  }
+  return DL_OK;
+}
+}  // namespace
+
+namespace dl {
+void carve_window(Arena& a, int count, WindowBuffers* w) {
+  const size_t n = (size_t)count;
+  w->si = a.take<dl_nav_state>(n);
+  w->prior = a.take<double>(n * 225);
+  w->pre = a.take<dl_preintegration>(n);
+  w->z = a.take<double>(n * 7);
+  w->init = a.take<dl_nav_state>(n);
+  w->si_out = a.take<dl_nav_state>(n);
+  w->sj_out = a.take<dl_nav_state>(n);
+  w->info = a.take<double>(n * 225);
+  w->sum = a.take<dl_solve_summary>(n);
+}
+int window_optimize(dl_context* ctx, const dl_window_options& options, int count, const WindowBuffers& w, const dl_nav_state* states_i,
+                    const double* prior_information, const dl_preintegration* preintegrations, const double* matched_poses,
+                    const dl_nav_state* initial_states_j, dl_nav_state* states_i_out, dl_nav_state* states_j_out,
+                    double* information_out, dl_solve_summary* summaries) {
+  const size_t n = (size_t)count;
+  DL_TRY(h2d(ctx, w.si, states_i, n));
+  DL_TRY(h2d(ctx, w.prior, prior_information, n * 225));
+  DL_TRY(h2d(ctx, w.pre, preintegrations, n));
+  DL_TRY(h2d(ctx, w.z, matched_poses, n * 7));
+  if (initial_states_j) DL_TRY(h2d(ctx, w.init, initial_states_j, n));
+  DL_CUDA(ctx, cudaMemsetAsync(w.sj_out, 0, n * sizeof(dl_nav_state), ctx->stream));
+  DL_CUDA(ctx, cudaMemsetAsync(w.info, 0, n * 225 * 8, ctx->stream));
+  DL_TRY(launch_window_optimize(ctx, count, w.si, w.prior, w.pre, w.z, initial_states_j ? w.init : nullptr, options, w.si_out, w.sj_out,
+                                w.info, w.sum));
+  DL_TRY(d2h(ctx, states_j_out, w.sj_out, n));
+  if (states_i_out) DL_TRY(d2h(ctx, states_i_out, w.si_out, n));
+  DL_TRY(d2h(ctx, information_out, w.info, n * 225));
+  std::vector<dl_solve_summary> sums(n);
+  DL_TRY(d2h(ctx, sums.data(), w.sum, n));
+  DL_TRY(sync(ctx));
+  if (summaries) std::memcpy(summaries, sums.data(), n * sizeof(dl_solve_summary));
+  return DL_OK;
+}
+}  // namespace dl
+
+extern "C" int dl_window_optimize_batch(dl_context* ctx, const dl_window_options* options, int32_t count, const dl_nav_state* states_i,
+                                        const double* prior_information, const dl_preintegration* preintegrations,
+                                        const double* matched_poses, const dl_nav_state* initial_states_j, dl_nav_state* states_i_out,
+                                        dl_nav_state* states_j_out, double* information_out, dl_solve_summary* summaries) {
+  if (!ctx || !options || count < 0) return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  if (!states_i || !prior_information || !preintegrations || !matched_poses || !states_j_out || !information_out) return DL_ERR_ARG;
+  dl_window_options o;
+  DL_TRY(window_options_checked(ctx, *options, &o));
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  WindowBuffers w;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) { carve_window(a, count, &w); }));
+  return window_optimize(ctx, o, count, w, states_i, prior_information, preintegrations, matched_poses, initial_states_j,
+                         states_i_out, states_j_out, information_out, summaries);
+}
+
+extern "C" int dl_window_evaluate(dl_context* ctx, const dl_window_options* options, int32_t count, const dl_nav_state* states_i,
+                                  const double* prior_information, const dl_preintegration* preintegrations, const double* matched_poses,
+                                  const dl_nav_state* x_i, const dl_nav_state* x_j, int32_t* ok, double* residuals, double* jacobians,
+                                  double* weights) {
+  if (!ctx || !options || count < 0) return DL_ERR_ARG;
+  if (count == 0) return DL_OK;
+  if (!states_i || !prior_information || !preintegrations || !matched_poses || !x_i || !x_j || !ok || !residuals || !jacobians ||
+      !weights)
+    return DL_ERR_ARG;
+  dl_window_options o;
+  DL_TRY(window_options_checked(ctx, *options, &o));
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t n = (size_t)count;
+  dl_nav_state* d_si;
+  dl_preintegration* d_pre;
+  double *d_prior, *d_z, *d_x, *d_out;
+  int32_t* d_ok;
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_si = a.take<dl_nav_state>(n);
+    d_prior = a.take<double>(n * 225);
+    d_pre = a.take<dl_preintegration>(n);
+    d_z = a.take<double>(n * 7);
+    d_x = a.take<double>(n * 32);
+    d_out = a.take<double>(n * kWindowEvalDoubles);
+    d_ok = a.take<int32_t>(n);
+  }));
+  std::vector<double> x(n * 32);
+  for (size_t k = 0; k < n; ++k)
+    for (int s = 0; s < 2; ++s) {
+      const dl_nav_state& v = (s == 0 ? x_i : x_j)[k];
+      double* d = x.data() + 32 * k + 16 * s;
+      for (int c = 0; c < 3; ++c) { d[c] = v.p[c]; d[7 + c] = v.v[c]; d[10 + c] = v.ba[c]; d[13 + c] = v.bg[c]; }
+      for (int c = 0; c < 4; ++c) d[3 + c] = v.q[c];
+    }
+  DL_TRY(h2d(ctx, d_si, states_i, n));
+  DL_TRY(h2d(ctx, d_prior, prior_information, n * 225));
+  DL_TRY(h2d(ctx, d_pre, preintegrations, n));
+  DL_TRY(h2d(ctx, d_z, matched_poses, n * 7));
+  DL_TRY(h2d(ctx, d_x, x.data(), n * 32));
+  DL_TRY(launch_window_evaluate(ctx, count, d_si, d_prior, d_pre, d_z, o, d_x, d_ok, d_out));
+  std::vector<double> out(n * kWindowEvalDoubles);
+  DL_TRY(d2h(ctx, ok, d_ok, n));
+  DL_TRY(d2h(ctx, out.data(), d_out, out.size()));
+  DL_TRY(sync(ctx));
+  for (size_t k = 0; k < n; ++k) {
+    const double* s = out.data() + k * kWindowEvalDoubles;
+    std::memcpy(residuals + 38 * k, s, 38 * sizeof(double));
+    std::memcpy(jacobians + 38 * 30 * k, s + 38, 38 * 30 * sizeof(double));
+    std::memcpy(weights + 38 * 38 * k, s + 38 + 38 * 30, 38 * 38 * sizeof(double));
+  }
+  return DL_OK;
+}

@@ -1,5 +1,5 @@
-"""Inputs for the real-time correlative scan matcher, one generator per edge of the device search (dl_rtcsm.cu, the tables of
-dl_api.cu) and of the reference's Match.
+"""Inputs for the real-time correlative scan matcher, one generator per edge of the device search (dl_rtcsm.cu, its kernels and the
+tables of its host part) and of the reference's Match.
 
 Every generator builds a Case and checks, with the numpy reference (rtcsm_reference), that its input sits on the side of the
 edge it is named for; the assertion at its end names the edge. Every case but the penalty-underflow ones also checks that no
