@@ -8,8 +8,9 @@
 // it moves are 56 bytes per submap or node, so there is no second copy of its set-up here. Pure localization adds trimming
 // (TrimmingHandle::MarkSubmapAsTrimmed, :1002-1058, and PureLocalizationTrimmer, C/mapping/pose_graph_trimmer.cc:24-45),
 // FinishTrajectory (:535-547) and SetInitialTrajectoryPose (:849-876); a trimmed node's clouds become dead ranges of the
-// node store, and pg3d_store_compact copies the live ones into a fresh store once the dead outweigh them. See
-// include/dliom_b200.h.
+// node store, and pg3d_store_compact copies the live ones into a fresh store once the dead outweigh them. The range-data map
+// (dl_range_data_map_set_node, dl_range_data_map) keeps a node's range_data_in_local returns in the same store and
+// emits them at the optimized node poses with one launch of pg3d_range_data_map. See include/dliom_b200.h.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -42,6 +43,8 @@ struct Node {
   Rigidd global;          // trajectory_nodes_' global_pose
   Rigidd problem_global;  // optimization_problem_->node_data()
   int64_t hi_begin = 0, n_hi = 0, lo_begin = 0, n_lo = 0;  // points in the node store
+  bool has_range_data = false;    // dl_range_data_map_set_node was called: n_rd returns at rd_begin in the node store
+  int64_t rd_begin = 0, n_rd = 0;
 };
 struct Trajectory {
   // MapById (C/mapping/id.h): indices in order; a trimmed index is a hole
@@ -58,8 +61,14 @@ struct InitialTrajectoryPose {  // PoseGraph3D::InitialTrajectoryPose
   Rigidd relative_pose;
   double time;
 };
-struct StoreSegment {  // one live node's clouds (high- then low-resolution xyz floats) in the old and the fresh store
+struct StoreSegment {  // one live node's clouds (high- then low-resolution xyz floats), or its returns, in the old and the fresh store
   int64_t src, dst, floats;
+};
+// One node of a range-data map: its returns in the store, its rows of the output and the two transforms of
+// pb_range_data_to_ros_cloud_main.cc:155-176, local_pose.cast<float>().inverse() and global_pose.cast<float>().
+struct RangeDataMapNode {
+  int64_t src, dst, count;  // store point, first output point, points (> 0)
+  Rigidf local_inverse, global;
 };
 constexpr int64_t kMinDeadFloats = (int64_t)1 << 20;  // compaction waits for at least this many dead floats (4 MiB)
 constexpr int kCompactBlock = 256;
@@ -69,6 +78,53 @@ __global__ void __launch_bounds__(kCompactBlock) pg3d_store_compact(const float*
                                                                     const StoreSegment* __restrict__ segments) {
   const StoreSegment s = segments[blockIdx.x];
   for (int64_t i = threadIdx.x; i < s.floats; i += kCompactBlock) dst[s.dst + i] = src[s.src + i];
+}
+
+constexpr int kMapBlock = 256;
+constexpr int kMapTile = 1024;  // output points per CTA: 12 KiB of xyz, staged in shared memory
+
+// The last node in [lo, hi] whose first output point is <= p (every node of the table has points, so `dst` increases).
+__device__ __forceinline__ int map_node_of(const RangeDataMapNode* __restrict__ nodes, int lo, int hi, int64_t p) {
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (nodes[mid].dst <= p) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// One CTA per kMapTile output points. Each point is read from the store (consecutive threads, consecutive points) and moved
+// by two separate Rigid3f * Vector3f products, tp = L^-1 * p and then G * tp, as the tool does; folding them into one composed
+// transform would change the bits. The tile's xyz rows are staged in shared memory and written out as float4 when the output
+// is 16-byte aligned.
+__global__ void __launch_bounds__(kMapBlock) pg3d_range_data_map(const float* __restrict__ store,
+                                                                 const RangeDataMapNode* __restrict__ nodes, int num_nodes,
+                                                                 int64_t total, float* __restrict__ out) {
+  __shared__ __align__(16) float tile[3 * kMapTile];
+  __shared__ int range[2];
+  const int64_t first = (int64_t)blockIdx.x * kMapTile;
+  const int n = (int)min((int64_t)kMapTile, total - first);
+  if (threadIdx.x < 2) range[threadIdx.x] = map_node_of(nodes, 0, num_nodes - 1, first + (threadIdx.x ? n - 1 : 0));
+  __syncthreads();
+  for (int k = threadIdx.x; k < n; k += kMapBlock) {
+    const int64_t p = first + k;
+    const RangeDataMapNode& node = nodes[map_node_of(nodes, range[0], range[1], p)];
+    const float* s = store + 3 * (node.src + (p - node.dst));
+    const Vec3f tp = apply(node.local_inverse, Vec3f{s[0], s[1], s[2]});
+    const Vec3f gp = apply(node.global, tp);
+    tile[3 * k] = gp.x;
+    tile[3 * k + 1] = gp.y;
+    tile[3 * k + 2] = gp.z;
+  }
+  __syncthreads();
+  float* o = out + 3 * first;
+  if (n == kMapTile && ((uintptr_t)out & 15) == 0) {  // 3 * kMapTile floats from a multiple of 4 floats: whole float4s
+    const float4* t4 = reinterpret_cast<const float4*>(tile);
+    float4* o4 = reinterpret_cast<float4*>(o);
+    for (int j = threadIdx.x; j < 3 * kMapTile / 4; j += kMapBlock) o4[j] = t4[j];
+  } else {
+    for (int j = threadIdx.x; j < 3 * n; j += kMapBlock) o[j] = tile[j];
+  }
 }
 
 double ms_since(std::chrono::steady_clock::time_point t0) {
@@ -172,6 +228,8 @@ struct dl_pose_graph_3d {
   int check_trimmable(int32_t trajectory_id, int32_t submap_index) const;
   int mark_submap_as_trimmed(const Id& submap_id);
   int compact_store();
+  int range_data_map(int32_t num_trajectories, const int32_t* trajectory_ids, int32_t node_capacity, dl_range_data_map_node* nodes,
+                     int32_t* num_nodes, int64_t capacity_points, float* points, int64_t* num_points, bool device_points);
 };
 
 namespace {
@@ -329,7 +387,7 @@ int dl_pose_graph_3d::mark_submap_as_trimmed(const Id& submap_id) {
     Trajectory& nt = trajectories.at(node_id.first);
     const auto n = nt.nodes.find(node_id.second);
     if (std::next(n) == nt.nodes.end()) nt.nodes_can_append = false;
-    store_live -= 3 * (n->second.n_hi + n->second.n_lo);
+    store_live -= 3 * (n->second.n_hi + n->second.n_lo + n->second.n_rd);
     nt.nodes.erase(n);
     for (auto& kv : computed) kv.second.erase(node_id);
   }
@@ -348,6 +406,10 @@ int dl_pose_graph_3d::compact_store() {
     for (const auto& [i, n] : t.nodes) {
       segments.push_back(StoreSegment{3 * n.hi_begin, live, 3 * (n.n_hi + n.n_lo)});
       live += 3 * (n.n_hi + n.n_lo);
+      if (n.n_rd > 0) {  // returns attached later: one more segment
+        segments.push_back(StoreSegment{3 * n.rd_begin, live, 3 * n.n_rd});
+        live += 3 * n.n_rd;
+      }
     }
   if (live == 0) {  // nothing left to copy: the store is freed, and the next add_node grows a new one
     DL_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -377,8 +439,78 @@ int dl_pose_graph_3d::compact_store() {
     for (auto& [i, n] : t.nodes) {
       n.hi_begin = segments[k++].dst / 3;
       n.lo_begin = n.hi_begin + n.n_hi;
+      if (n.n_rd > 0) n.rd_begin = segments[k++].dst / 3;
     }
   return DL_OK;
+}
+
+// The body of dl_range_data_map and its _dev variant: the selection and the counts on the host, then, when there are
+// points to write, one upload of the table of nodes with points, one launch and one host wait (after the download into
+// `points` for the host variant).
+int dl_pose_graph_3d::range_data_map(int32_t num_trajectories, const int32_t* trajectory_ids, int32_t node_capacity,
+                                     dl_range_data_map_node* nodes, int32_t* num_nodes, int64_t capacity_points, float* points,
+                                     int64_t* num_points, bool device_points) {
+  if (!num_nodes || !num_points || node_capacity < 0 || capacity_points < 0) return DL_ERR_ARG;
+  if (num_trajectories < 0) return ctx->fail(DL_ERR_ARG, "num_trajectories must be >= 0");
+  std::vector<const std::pair<const int32_t, Trajectory>*> selected;
+  if (!trajectory_ids) {
+    for (const auto& kv : trajectories) selected.push_back(&kv);
+  } else {
+    std::set<int32_t> ids;
+    for (int32_t k = 0; k < num_trajectories; ++k)
+      if (!ids.insert(trajectory_ids[k]).second) return ctx->fail(DL_ERR_ARG, "a trajectory id is listed twice");
+    for (const int32_t id : ids) {
+      const auto it = trajectories.find(id);
+      if (it == trajectories.end()) return ctx->fail(DL_ERR_ARG, "unknown trajectory id");
+      selected.push_back(&*it);
+    }
+  }
+  int64_t count = 0, total = 0;
+  for (const auto* t : selected)
+    for (const auto& [i, n] : t->second.nodes)
+      if (n.has_range_data) {
+        ++count;
+        total += n.n_rd;
+      }
+  if (count > INT32_MAX) return ctx->fail(DL_ERR_ARG, "more than INT32_MAX nodes with range data");
+  *num_nodes = (int32_t)count;
+  *num_points = total;
+  if (!nodes || !points) return DL_OK;
+  if (node_capacity < count) return ctx->fail(DL_ERR_ARG, "node_capacity smaller than the map's nodes");
+  if (capacity_points < total) return ctx->fail(DL_ERR_ARG, "capacity_points smaller than the map's points");
+  std::vector<RangeDataMapNode> table;  // the nodes with points: the kernel's binary search needs increasing first points
+  int32_t k = 0;
+  int64_t offset = 0;
+  for (const auto* t : selected)
+    for (const auto& [i, n] : t->second.nodes) {
+      if (!n.has_range_data) continue;
+      dl_range_data_map_node& out = nodes[k++];
+      out.trajectory_id = t->first;
+      out.node_index = i;
+      out.first_point = offset;
+      out.num_points = n.n_rd;
+      pose_to7(n.global, out.global_pose);
+      if (n.n_rd > 0) table.push_back(RangeDataMapNode{n.rd_begin, offset, n.n_rd, inverse(to_float(n.local)), to_float(n.global)});
+      offset += n.n_rd;
+    }
+  if (total == 0) return DL_OK;
+  RangeDataMapNode* d_table = nullptr;
+  float* d_points = points;
+  DL_CUDA(ctx, cudaSetDevice(ctx->device));
+  DL_TRY(carve_scratch(ctx, [&](Arena& a) {
+    d_table = a.take<RangeDataMapNode>(table.size());
+    if (!device_points) d_points = a.take<float>(3 * (size_t)total);
+  }));
+  DL_TRY(h2d(ctx, d_table, table.data(), table.size()));
+  const int64_t blocks = (total + kMapTile - 1) / kMapTile;
+  if (blocks > INT32_MAX) return ctx->fail(DL_ERR_ARG, "map too large for one launch");
+  {
+    StageScope stage(ctx, "pg3d_range_data_map");
+    pg3d_range_data_map<<<(unsigned)blocks, kMapBlock, 0, ctx->stream>>>(d_store.get(), d_table, (int)table.size(), total, d_points);
+    DL_LAUNCH_CHECK(ctx, "pg3d_range_data_map");
+  }
+  if (!device_points) DL_TRY(d2h(ctx, points, d_points, 3 * (size_t)total));
+  return sync(ctx);
 }
 
 extern "C" {
@@ -800,6 +932,49 @@ int dl_pg3d_store_usage(const dl_pose_graph_3d* g, int64_t* live_bytes, int64_t*
   if (used_bytes) *used_bytes = g->store_used * (int64_t)sizeof(float);
   if (capacity_bytes) *capacity_bytes = (int64_t)g->d_store.cap * (int64_t)sizeof(float);
   return DL_OK;
+}
+
+int dl_range_data_map_set_node(dl_pose_graph_3d* g, int32_t trajectory_id, int32_t node_index, const float* returns,
+                               int64_t num_returns) {
+  if (!g) return DL_ERR_ARG;
+  dl_context* ctx = g->ctx;
+  if (num_returns < 0) return ctx->fail(DL_ERR_ARG, "num_returns must be >= 0");
+  if (!returns && num_returns > 0) return ctx->fail(DL_ERR_ARG, "returns is NULL");
+  const auto t = g->trajectories.find(trajectory_id);
+  if (t == g->trajectories.end() || !t->second.nodes.count(node_index))
+    return ctx->fail(DL_ERR_ARG, "range data for an unknown or trimmed node");
+  Node& n = t->second.nodes.at(node_index);
+  if (n.has_range_data) return ctx->fail(DL_ERR_ARG, "the node already has range data");
+  // the returns into the node store (store_used moves on only at the commit below)
+  DL_TRY(g->reserve_store(3 * num_returns));
+  const int64_t begin = g->store_used / 3;
+  if (num_returns > 0) {
+    DL_CUDA(ctx, cudaSetDevice(ctx->device));
+    DL_TRY(h2d(ctx, g->d_store.get() + 3 * begin, returns, 3 * (size_t)num_returns));
+    DL_TRY(sync(ctx));  // pageable host memory
+  }
+  g->store_used += 3 * num_returns;
+  g->store_live += 3 * num_returns;
+  g->bytes_uploaded += 12 * num_returns;
+  n.has_range_data = true;
+  n.rd_begin = begin;
+  n.n_rd = num_returns;
+  return DL_OK;
+}
+
+int dl_range_data_map(dl_pose_graph_3d* g, int32_t num_trajectories, const int32_t* trajectory_ids, int32_t node_capacity,
+                      dl_range_data_map_node* nodes, int32_t* num_nodes, int64_t capacity_points, float* points, int64_t* num_points) {
+  if (!g) return DL_ERR_ARG;
+  return g->range_data_map(num_trajectories, trajectory_ids, node_capacity, nodes, num_nodes, capacity_points, points, num_points,
+                           false);
+}
+
+int dl_range_data_map_dev(dl_pose_graph_3d* g, int32_t num_trajectories, const int32_t* trajectory_ids, int32_t node_capacity,
+                          dl_range_data_map_node* nodes, int32_t* num_nodes, int64_t capacity_points, float* points_dev,
+                          int64_t* num_points) {
+  if (!g) return DL_ERR_ARG;
+  return g->range_data_map(num_trajectories, trajectory_ids, node_capacity, nodes, num_nodes, capacity_points, points_dev,
+                           num_points, true);
 }
 
 }  // extern "C"

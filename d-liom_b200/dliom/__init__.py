@@ -42,6 +42,7 @@ EXPORTS = [
     "dl_pose_graph_3d_constraints", "dl_pose_graph_3d_last_searches", "dl_pose_graph_3d_store_bytes",
     "dl_pg3d_trim_submap", "dl_pg3d_add_pure_localization_trimmer", "dl_pg3d_finish_trajectory", "dl_pg3d_is_trajectory_finished",
     "dl_pg3d_set_initial_trajectory_pose", "dl_pg3d_ids", "dl_pg3d_last_trimmed", "dl_pg3d_store_usage",
+    "dl_range_data_map_set_node", "dl_range_data_map", "dl_range_data_map_dev",
     "dl_map_writer_create", "dl_map_writer_destroy", "dl_map_writer_add_trajectory", "dl_map_writer_process",
     "dl_map_writer_process_dev", "dl_map_writer_flush", "dl_map_writer_voxels", "dl_map_writer_add_color",
     "dl_map_writer_add_xray", "dl_map_writer_xray_image", "dl_map_writer_add_probability_grid", "dl_map_writer_probability_grid",
@@ -383,6 +384,11 @@ class Pg3dSubmapId(C.Structure):   # dl_pg3d_submap_id
     _fields_ = [("trajectory_id", C.c_int32), ("submap_index", C.c_int32)]
 
 
+class RangeDataMapNode(C.Structure):   # dl_range_data_map_node
+    _fields_ = [("trajectory_id", C.c_int32), ("node_index", C.c_int32), ("first_point", C.c_int64), ("num_points", C.c_int64),
+                ("global_pose", C.c_double * 7)]
+
+
 class MapWriterOptions(C.Structure):   # dl_map_writer_options
     _fields_ = [("range_filter", C.c_int32), ("reserved", C.c_int32), ("min_range", C.c_double), ("max_range", C.c_double),
                 ("outlier_voxel_size", C.c_double)]
@@ -569,6 +575,9 @@ def lib():
     L.dl_pg3d_ids.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, ip(C.c_int32)]
     L.dl_pg3d_last_trimmed.argtypes = [vp, C.c_int32, vp, ip(C.c_int32)]
     L.dl_pg3d_store_usage.argtypes = [vp, ip(C.c_int64), ip(C.c_int64), ip(C.c_int64)]
+    L.dl_range_data_map_set_node.argtypes = [vp, C.c_int32, C.c_int32, vp, C.c_int64]
+    for name in ("dl_range_data_map", "dl_range_data_map_dev"):
+        getattr(L, name).argtypes = [vp, C.c_int32, vp, C.c_int32, vp, ip(C.c_int32), C.c_int64, vp, ip(C.c_int64)]
     L.dl_map_writer_create.argtypes = [vp, ip(MapWriterOptions), ip(vp)]
     L.dl_map_writer_destroy.argtypes = [vp]
     L.dl_map_writer_destroy.restype = None
@@ -667,6 +676,7 @@ class Context:
         if st != 0:
             raise DlError(st, self.L.dl_last_error(None).decode())
         self.h = h
+        self.device = device
 
     def close(self):
         if getattr(self, "h", None):
@@ -1377,17 +1387,51 @@ class PoseGraph3D:
                                                                               C.cast(m, C.c_void_p), C.byref(info)))
         return info
 
-    def add_node_from_builder(self, trajectory_id, builder, result, matches=()):
+    def add_node_from_builder(self, trajectory_id, builder, result, matches=(), range_data=False):
         """GlobalTrajectoryBuilder's AddNode call site: the node of a dl_ltb MatchingResult with insertion submaps, its clouds
-        and the submaps' grids, local poses and finished flags from the builder."""
+        and the submaps' grids, local poses and finished flags from the builder. range_data=True also attaches the builder's
+        range_data_in_local returns (cloud 0) to the new node (set_node_range_data), for range_data_map."""
         subs = []
         for i in range(result.num_insertion_submaps):
             index = result.insertion_submap_index[i]
             hg, lg, pose, _, finished = builder.submap(index)
             subs.append((index, finished, hg, lg, pose))
             self._feeders[(int(trajectory_id), int(index))] = builder
-        return self.add_node(trajectory_id, result.time, np.array(result.local_pose[:]), builder.cloud(2), builder.cloud(3),
+        info = self.add_node(trajectory_id, result.time, np.array(result.local_pose[:]), builder.cloud(2), builder.cloud(3),
                              subs, matches)
+        if range_data:
+            self.set_node_range_data(trajectory_id, info.node_index, builder.cloud(0))
+        return info
+
+    def set_node_range_data(self, trajectory_id, node_index, returns):
+        """Attach a node's range_data_in_local returns (n x 3, the builder's local frame) to the node store
+        (dl_range_data_map_set_node): once per node."""
+        r = np.ascontiguousarray(returns, np.float32).reshape(-1, 3)
+        self.ctx.check(self.ctx.L.dl_range_data_map_set_node(self.h, int(trajectory_id), int(node_index), r.ctypes.data, len(r)))
+
+    def range_data_map(self, trajectory_ids=None, device=False):
+        """The range-data map (dl_range_data_map): every live node with range data of the listed trajectories (None: all)
+        in (trajectory, node index) order, its returns at the node's optimized pose -> (points n x 3 float32, nodes: [(trajectory
+        id, node index, first point, num points, global pose7)]). device=True: points is a torch CUDA tensor on the context's
+        device, filled by dl_range_data_map_dev."""
+        ids = None if trajectory_ids is None else np.ascontiguousarray(trajectory_ids, np.int32).reshape(-1)
+        args = (0 if ids is None else len(ids), None if ids is None else ids.ctypes.data)
+        nn, npts = C.c_int32(0), C.c_int64(0)
+        self.ctx.check(self.ctx.L.dl_range_data_map(self.h, *args, 0, None, C.byref(nn), 0, None, C.byref(npts)))
+        nodes = (RangeDataMapNode * max(nn.value, 1))()
+        if device:
+            import torch
+            dev = torch.device("cuda", self.ctx.device)
+            points = torch.empty((max(npts.value, 1), 3), dtype=torch.float32, device=dev)
+            torch.cuda.current_stream(dev).synchronize()   # the allocation is ordered on torch's stream, the fill on the context's
+            self.ctx.check(self.ctx.L.dl_range_data_map_dev(self.h, *args, nn.value, C.cast(nodes, C.c_void_p), C.byref(nn),
+                                                                 npts.value, points.data_ptr(), C.byref(npts)))
+        else:
+            points = np.zeros((max(npts.value, 1), 3), np.float32)
+            self.ctx.check(self.ctx.L.dl_range_data_map(self.h, *args, nn.value, C.cast(nodes, C.c_void_p), C.byref(nn),
+                                                             npts.value, points.ctypes.data, C.byref(npts)))
+        return points[:npts.value], [(n.trajectory_id, n.node_index, n.first_point, n.num_points, np.array(n.global_pose[:]))
+                                     for n in list(nodes)[:nn.value]]
 
     def _checked_forgetting_trimmed(self, status):
         """After a call that may have trimmed, whatever its status (the call empties the trimmed list when it starts, so a

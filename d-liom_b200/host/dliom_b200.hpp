@@ -955,11 +955,29 @@ class PoseGraph3D {
     const int st = dl_pose_graph_3d_add_node(graph_, &node, (int32_t)m.size(), m.data(), &local);
     if (st == DL_OK)
       for (int i = 0; i < node.num_insertion_submaps; ++i) feeders_[{trajectory_id, node.insertion_submaps[i].submap_index}] = &builder;
+    if (st == DL_OK && range_data_cache_) {  // the builder's range_data_in_local.returns of this node
+      int64_t n = 0;
+      ctx_->check(dl_ltb_get_cloud(builder.get(), 0, nullptr, 0, &n));
+      PointCloud returns((size_t)n);
+      if (n) ctx_->check(dl_ltb_get_cloud(builder.get(), 0, returns[0].data(), n, &n));
+      ctx_->check(dl_range_data_map_set_node(graph_, trajectory_id, local.node_index, n ? returns[0].data() : nullptr, n));
+    }
     AfterCall(st, st == DL_OK && local.optimized);
     if (info) *info = local;
     return {trajectory_id, local.node_index};
   }
   void FreezeTrajectory(int trajectory_id) { ctx_->check(dl_pose_graph_3d_freeze_trajectory(graph_, trajectory_id)); }
+  // MapBuilderBridge::EnableFullCloudCache (map_builder_bridge.cc:591-607), the cache behind --save_range_data: after it, AddNode
+  // also keeps the node's range_data_in_local.returns in the graph's node store (dl_range_data_map_set_node).
+  void EnableRangeDataCache() { range_data_cache_ = true; }
+  // pb_range_data_to_ros_cloud's map (dl_range_data_map): every node with cached range data, in (trajectory, node index)
+  // order, its returns at the node's optimized pose; `nodes` gives each node's rows of `points` and the pose used.
+  struct RangeDataMapResult {
+    std::vector<dl_range_data_map_node> nodes;
+    PointCloud points;
+  };
+  RangeDataMapResult RangeDataMap() const { return RangeDataMap(nullptr); }
+  RangeDataMapResult RangeDataMap(const std::vector<int32_t>& trajectory_ids) const { return RangeDataMap(&trajectory_ids); }
   dl_solve_summary RunFinalOptimization() {
     dl_solve_summary s{};
     const int st = dl_pose_graph_3d_run_final_optimization(graph_, &s);
@@ -1038,6 +1056,21 @@ class PoseGraph3D {
     if (n) ctx_->check(dl_pg3d_ids(graph_, trajectory_id, which, n, ids.data(), &n));
     return ids;
   }
+  RangeDataMapResult RangeDataMap(const std::vector<int32_t>* ids) const {
+    const int32_t num_ids = ids ? (int32_t)ids->size() : 0;
+    const int32_t* id_ptr = ids ? ids->data() : nullptr;
+    int32_t num_nodes = 0;
+    int64_t num_points = 0;
+    ctx_->check(dl_range_data_map(graph_, num_ids, id_ptr, 0, nullptr, &num_nodes, 0, nullptr, &num_points));
+    RangeDataMapResult out;
+    out.nodes.resize((size_t)num_nodes + 1);  // never empty: data() is then non-null and the call fills, not sizes
+    out.points.resize((size_t)num_points + 1);
+    ctx_->check(dl_range_data_map(graph_, num_ids, id_ptr, num_nodes, out.nodes.data(), &num_nodes, num_points,
+                                  out.points[0].data(), &num_points));
+    out.nodes.resize((size_t)num_nodes);
+    out.points.resize((size_t)num_points);
+    return out;
+  }
   std::vector<Rigid3d> Poses(int trajectory_id, int which) const {
     int32_t n = 0;
     ctx_->check(dl_pose_graph_3d_poses(graph_, trajectory_id, which, 0, nullptr, &n));
@@ -1051,6 +1084,7 @@ class PoseGraph3D {
   dl_pose_graph_3d* graph_ = nullptr;
   std::map<optimization::SubmapId, const LocalTrajectoryBuilder3D*> feeders_;  // where AddNode got each submap's grids
   std::vector<std::unique_ptr<PoseGraphTrimmer>> trimmers_;                     // host trimmers, in the order added
+  bool range_data_cache_ = false;                                               // EnableRangeDataCache
 };
 
 }  // namespace mapping

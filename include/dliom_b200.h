@@ -556,6 +556,49 @@ int dl_pg3d_last_trimmed(const dl_pose_graph_3d* graph, int32_t capacity, dl_pg3
 /* The node store in bytes: live (the clouds of the nodes still in the graph), used (written, dead ranges included), capacity. */
 int dl_pg3d_store_usage(const dl_pose_graph_3d* graph, int64_t* live_bytes, int64_t* used_bytes, int64_t* capacity_bytes);
 
+/* ---- Range-data map (dl_range_data_map_*, the block's prefix; it works on a dl_pose_graph_3d): the point-cloud map of the
+ *      fork's --save_range_data (MapBuilderBridge::OnLocalSlamResult caching every
+ *      range_data_in_local once EnableFullCloudCache is on, map_builder_bridge.cc:170-200, :591-607) followed by its tool
+ *      pb_range_data_to_ros_cloud (pb_range_data_to_ros_cloud_main.cc:105-182), with the cache kept in the graph's node store.
+ *      dl_range_data_map_set_node is the opt-in: it uploads one node's range_data_in_local.returns (xyz floats in the builder's
+ *      local frame, e.g. dl_ltb_get_cloud(..., 0, ...)) ONCE into the node store, through the growth path of the node clouds.
+ *      They follow the clouds' trim and compaction rules: a trimmed node's returns become dead floats, pg3d_store_compact
+ *      copies the live ones, and the rule "after every trim used <= 2 * live or used - live < 4 MiB" counts them. They count
+ *      in dl_pg3d_store_usage and dl_pose_graph_3d_store_bytes; dl_pg3d_add_node_info::cloud_bytes_uploaded does not. A graph
+ *      on which it is never called behaves exactly as without it. Rejected with DL_ERR_ARG, the graph unchanged: an unknown or
+ *      trimmed node, a node that already has range data, num_returns < 0, returns == NULL with num_returns > 0; a failed
+ *      reservation also leaves the graph unchanged. num_returns == 0 is allowed: the node is in the map with no points.
+ *      dl_range_data_map writes every live node with range data of the listed trajectories (trajectory_ids == NULL: all
+ *      of them), in ascending (trajectory, node index) order, each node's points in the order attached, with the tool's
+ *      arithmetic bit for bit: L = local_pose.cast<float>(), G = global_pose.cast<float>() (per coefficient, no
+ *      renormalisation; the global pose is DL_PG3D_NODE_POSES), then per point tp = L.inverse() * p and gp = G * tp, two
+ *      separate Rigid3f * Vector3f products (L.inverse() is formed once per node; it is deterministic). nodes[k] gives node
+ *      k's rows of `points` and the pose used. With points == NULL or nodes == NULL only *num_nodes and *num_points are
+ *      written (host bookkeeping, no device work); a capacity below them gives DL_ERR_ARG with only the counts written. An
+ *      unknown or repeated trajectory id, or num_trajectories < 0: DL_ERR_ARG. Device work: when the map has points, one
+ *      upload of a table of the nodes with points, ONE launch of pg3d_range_data_map over all points and ONE host wait,
+ *      whatever the node count; the host variant also downloads the points (through the context's device scratch, which
+ *      stays reserved) before that wait. The _dev variant writes device memory on the graph's device and waits before it
+ *      returns, so the buffer is ready on any stream. Both fail with DL_ERR_ARG while a dl_frontend_submit batch is in flight.
+ *      Deliberate differences from the fork: nodes are found by id (the tool keys nodes by timestamp, first one wins across
+ *      trajectories, and reads the pose graph by position, which breaks with trimmed holes and trajectory ids other than
+ *      0..n-1); only nodes in the graph carry range data (the fork caches results the motion filter dropped and the tool skips
+ *      them: the output is the same); only the returns are kept (the tool never reads the misses) and the output is xyz
+ *      (without the tool's constant fourth component 1.0); trajectories come in ascending id order (the fork's cache is an
+ *      unordered_map); no ROS publishing, rate or pbstream: the caller gets arrays. ---- */
+typedef struct dl_range_data_map_node {
+  int32_t trajectory_id, node_index;
+  int64_t first_point, num_points;   /* rows of this node in the output */
+  double global_pose[7];             /* the node pose used: DL_PG3D_NODE_POSES */
+} dl_range_data_map_node;
+int dl_range_data_map_set_node(dl_pose_graph_3d* graph, int32_t trajectory_id, int32_t node_index, const float* returns,
+                               int64_t num_returns);
+int dl_range_data_map(dl_pose_graph_3d* graph, int32_t num_trajectories, const int32_t* trajectory_ids, int32_t node_capacity,
+                      dl_range_data_map_node* nodes, int32_t* num_nodes, int64_t capacity_points, float* points, int64_t* num_points);
+int dl_range_data_map_dev(dl_pose_graph_3d* graph, int32_t num_trajectories, const int32_t* trajectory_ids, int32_t node_capacity,
+                          dl_range_data_map_node* nodes, int32_t* num_nodes, int64_t capacity_points, float* points_dev,
+                          int64_t* num_points);
+
 /* ---- IMU: pre-integration (LocalTrajectoryBuilder3D::AddImuData, LTB:164-201, with the in-repo mid-point integrator
  *      C/mapping/internal/3d/initialization/integration_base.h:109-265 instead of the un-vendored GTSAM one) and the
  *      scan match with the pre-integration residual (integration_base.h:267-301) fused into the same solve.
